@@ -86,30 +86,19 @@ __global__ void __launch_bounds__(256) bruteforce_kernel(AuxParams p) {
   }
 }
 
+template <class Op, int CH, int U>
+static cudaError_t launch_aux_kernel(const AuxParams& p, bool brute, int grid, size_t smem, cudaStream_t st) {
+  return launch_kernel(brute ? bruteforce_kernel<Op, CH, U> : dist_batch_kernel<Op, CH, U>, p, grid, 256, smem, st, nullptr);
+}
+
 template <class Op>
 static cudaError_t launch_aux_for_op(const AuxParams& p, bool brute, int grid, size_t smem, cudaStream_t st) {
   const int ch = p.g.d4 / 8;
-#define HB_LAUNCH(CHV, UV)                                                                                \
-  do {                                                                                                    \
-    if (brute) {                                                                                          \
-      auto kern = bruteforce_kernel<Op, CHV, UV>;                                                         \
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-      if (e != cudaSuccess) return e;                                                                     \
-      kern<<<grid, 256, smem, st>>>(p);                                                                   \
-    } else {                                                                                              \
-      auto kern = dist_batch_kernel<Op, CHV, UV>;                                                         \
-      cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-      if (e != cudaSuccess) return e;                                                                     \
-      kern<<<grid, 256, smem, st>>>(p);                                                                   \
-    }                                                                                                     \
-    return cudaGetLastError();                                                                            \
-  } while (0)
   if constexpr (Specialise<Op>::value) {
-    if (ch == 1) HB_LAUNCH(1, 4);
-    if (ch == 4) HB_LAUNCH(4, 2);
+    if (ch == 1) return launch_aux_kernel<Op, 1, 4>(p, brute, grid, smem, st);
+    if (ch == 4) return launch_aux_kernel<Op, 4, 2>(p, brute, grid, smem, st);
   }
-  HB_LAUNCH(0, 2);
-#undef HB_LAUNCH
+  return launch_aux_kernel<Op, 0, 2>(p, brute, grid, smem, st);
 }
 
 static cudaError_t launch_aux(const AuxParams& p, int metric, int dtype, bool brute, int grid, size_t smem, cudaStream_t st) {

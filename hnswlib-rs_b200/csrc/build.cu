@@ -71,9 +71,7 @@ __global__ void __launch_bounds__(BUILD_THREADS) insert_search_kernel(InsertPara
   const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
 
   for (;;) {
-    uint32_t wi = 0;
-    if (lane == 0) wi = atomicAdd(p.work_counter, 1u);
-    wi = __shfl_sync(FULL, wi, 0);
+    const uint32_t wi = next_item(p.work_counter);
     if (wi >= p.count) break;
     const uint32_t x = p.first + wi;
     const int lv = g.level[x];
@@ -207,11 +205,7 @@ __global__ void __launch_bounds__(BUILD_THREADS) insert_search_kernel(InsertPara
     if (overflow && lane == 0) atomicExch(p.status, 1);
   }
   vis.save(p.vis, slot);
-  if (p.stats && lane == 0) {
-    atomicAdd(p.stats + 0, (unsigned long long)st.evals);
-    atomicAdd(p.stats + 1, (unsigned long long)st.expansions);
-    atomicAdd(p.stats + 2, (unsigned long long)st.adj);
-  }
+  flush_stats(p.stats, st);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -333,39 +327,25 @@ __global__ void __launch_bounds__(BUILD_THREADS) insert_link_kernel(InsertParams
 }
 
 template <class Op, int NS>
-static cudaError_t launch_insert_for_op(const InsertParams& p, int grid, size_t smem, cudaStream_t st, bool query_only,
-                                        int* blocks_per_sm) {
+static cudaError_t launch_insert_for_op(const InsertParams& p, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm) {
   const int ch = p.g.d4 / 8;
-#define HB_LAUNCH(CHV, UV)                                                                              \
-  do {                                                                                                  \
-    auto kern = insert_search_kernel<Op, CHV, UV, NS>;                                                  \
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-    if (e != cudaSuccess) return e;                                                                     \
-    if (blocks_per_sm) {                                                                                \
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, kern, p.threads, smem);      \
-      if (e != cudaSuccess) return e;                                                                   \
-    }                                                                                                   \
-    if (!query_only) kern<<<grid, p.threads, smem, st>>>(p);                                        \
-    return cudaGetLastError();                                                                          \
-  } while (0)
   if constexpr (Specialise<Op>::value) {
-    if (ch == 1) HB_LAUNCH(1, 4);
-    if (ch == 2) HB_LAUNCH(2, 4);
-    if (ch == 4) HB_LAUNCH(4, 2);
+    if (ch == 1) return launch_kernel(insert_search_kernel<Op, 1, 4, NS>, p, grid, p.threads, smem, st, blocks_per_sm);
+    if (ch == 2) return launch_kernel(insert_search_kernel<Op, 2, 4, NS>, p, grid, p.threads, smem, st, blocks_per_sm);
+    if (ch == 4) return launch_kernel(insert_search_kernel<Op, 4, 2, NS>, p, grid, p.threads, smem, st, blocks_per_sm);
   }
-  HB_LAUNCH(0, 2);
-#undef HB_LAUNCH
+  return launch_kernel(insert_search_kernel<Op, 0, 2, NS>, p, grid, p.threads, smem, st, blocks_per_sm);
 }
 
 cudaError_t launch_insert_search(const InsertParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st,
-                                 bool query_only, int* blocks_per_sm) {
+                                 int* blocks_per_sm) {
   return dispatch_op(metric, dtype, [&](auto tag) -> cudaError_t {
     using Op = typename decltype(tag)::type;
     if constexpr (Specialise<Op>::value) {
-      if (p.q_kind == 108) return launch_insert_for_op<Op, 108>(p, grid, smem, st, query_only, blocks_per_sm);
-      if (p.q_kind == 104) return launch_insert_for_op<Op, 104>(p, grid, smem, st, query_only, blocks_per_sm);
+      if (p.q_kind == 108) return launch_insert_for_op<Op, 108>(p, grid, smem, st, blocks_per_sm);
+      if (p.q_kind == 104) return launch_insert_for_op<Op, 104>(p, grid, smem, st, blocks_per_sm);
     }
-    return launch_insert_for_op<Op, 0>(p, grid, smem, st, query_only, blocks_per_sm);
+    return launch_insert_for_op<Op, 0>(p, grid, smem, st, blocks_per_sm);
   });
 }
 

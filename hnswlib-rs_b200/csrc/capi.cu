@@ -494,6 +494,24 @@ int hnsw_b200_insert_flat(void* h, const void* vecs, uint64_t n, uint64_t dim, c
   return pass(ix, ix->insert_batch(vecs, n, dim, nullptr, ids, levels));
 }
 
+// answers of nq queries (k slots each, as the kernels left them) into the caller's arrays; internal ids and PointIds are
+// optional.  The kernels fill the slots beyond a query's count with (~0, +inf, INVALID_ID): plain field copies.
+static void unpack_answers(const Index* rx, const NeighbourOut* a, const int32_t* cnts, uint64_t nq, uint64_t k, uint64_t* ids,
+                           float* dist, uint32_t* internal, int32_t* pid, int32_t* counts) {
+  memcpy(counts, cnts, nq * sizeof(int32_t));
+  const uint64_t tot = nq * k;
+  for (uint64_t s = 0; s < tot; ++s) ids[s] = a[s].origin;
+  for (uint64_t s = 0; s < tot; ++s) dist[s] = a[s].dist;
+  if (internal)
+    for (uint64_t s = 0; s < tot; ++s) internal[s] = a[s].internal;
+  if (pid)  // PointId(level, rank), hnsw.rs:46
+    for (uint64_t s = 0; s < tot; ++s) {
+      const uint32_t it = a[s].internal;
+      pid[2 * s] = it != hb::INVALID_ID ? (int32_t)rx->h_level[it] : -1;
+      pid[2 * s + 1] = it != hb::INVALID_ID ? rx->h_rank[it] : -1;
+    }
+}
+
 int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
                           uint64_t ef_search, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,
                           hnsw_b200_filter_fn fn, void* ctx, uint64_t* out_ids, float* out_dist,
@@ -516,19 +534,9 @@ int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint6
     Index::CtxLease lease(rx);  // the answers stay in the context's pinned buffer until they are unpacked below
     int r = rx->search_host_staged(lease.c, (const char*)queries + first * qrow, nullptr, count, (int)dim, knbn, ef_search, fb, &tmp, &cnts);
     if (r) return r;
-    memcpy(out_counts + first, cnts, count * sizeof(int32_t));
-    // the kernel fills the slots beyond a query's count with (~0, +inf, INVALID_ID): plain field copies
-    const uint64_t tot = count * knbn, o0 = first * knbn;
-    for (uint64_t s = 0; s < tot; ++s) out_ids[o0 + s] = tmp[s].origin;
-    for (uint64_t s = 0; s < tot; ++s) out_dist[o0 + s] = tmp[s].dist;
-    if (out_internal)
-      for (uint64_t s = 0; s < tot; ++s) out_internal[o0 + s] = tmp[s].internal;
-    if (out_pid)  // PointId(level, rank), hnsw.rs:46
-      for (uint64_t s = 0; s < tot; ++s) {
-        const uint32_t it = tmp[s].internal;
-        out_pid[2 * (o0 + s)] = it != hb::INVALID_ID ? (int32_t)rx->h_level[it] : -1;
-        out_pid[2 * (o0 + s) + 1] = it != hb::INVALID_ID ? rx->h_rank[it] : -1;
-      }
+    const uint64_t o0 = first * knbn;
+    unpack_answers(rx, tmp, cnts, count, knbn, out_ids + o0, out_dist + o0, out_internal ? out_internal + o0 : nullptr,
+                   out_pid ? out_pid + 2 * o0 : nullptr, out_counts + first);
     return 0;
   };
   return pass(ix, use_shards(ix, nq) ? ix->for_each_shard(nq, run) : run(ix, 0, nq));
@@ -560,18 +568,7 @@ static int wait_on(Index* rx, int ci) {
   int r = rx->search_host_finish(ci, &tmp, &cnts);
   if (!r) {
     const Index::SearchCtx::Pending& p = rx->ctx(ci).pend;
-    memcpy(p.u_counts, cnts, p.nq * sizeof(int32_t));
-    const uint64_t tot = p.nq * p.k;
-    for (uint64_t s = 0; s < tot; ++s) p.u_ids[s] = tmp[s].origin;
-    for (uint64_t s = 0; s < tot; ++s) p.u_dist[s] = tmp[s].dist;
-    if (p.u_internal)
-      for (uint64_t s = 0; s < tot; ++s) p.u_internal[s] = tmp[s].internal;
-    if (p.u_pid)
-      for (uint64_t s = 0; s < tot; ++s) {
-        const uint32_t it = tmp[s].internal;
-        p.u_pid[2 * s] = it != hb::INVALID_ID ? (int32_t)rx->h_level[it] : -1;
-        p.u_pid[2 * s + 1] = it != hb::INVALID_ID ? rx->h_rank[it] : -1;
-      }
+    unpack_answers(rx, tmp, cnts, p.nq, p.k, p.u_ids, p.u_dist, p.u_internal, p.u_pid, p.u_counts);
   }
   rx->release_ctx(ci);
   return r;

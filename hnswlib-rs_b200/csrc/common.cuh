@@ -675,7 +675,6 @@ struct SortedQueue {
     n = 1;
     __syncwarp();
   }
-  __device__ __forceinline__ void clear() { n = 0; }
   // index of the nearest unexpanded entry, or -1
   __device__ __forceinline__ int first_unexpanded() const {
     const int lane = lane_id();
@@ -752,7 +751,6 @@ struct SmemQueueN {
     for (int c = 0; c < NCH; ++c) w[32 * c + lane] = ~0ull;
     __syncwarp();
   }
-  __device__ __forceinline__ void clear() { reset(w, cap); }
   __device__ __forceinline__ uint64_t get(int i) const { return w[i]; }
   __device__ __forceinline__ uint64_t local(int i) const { return w[i]; }
   __device__ __forceinline__ void mark_expanded(int i) {

@@ -19,6 +19,27 @@ __device__ __forceinline__ bool filter_pass(const uint32_t* bits, uint32_t id) {
   return (__ldg(bits + (id >> 5)) >> (id & 31)) & 1u;
 }
 
+// keeps the keys w[0, n) whose points pass the filter, in order, at the front of w; returns how many there are
+__device__ __forceinline__ int keep_passing(uint64_t* w, int n, const uint32_t* fbits) {
+  const int lane = lane_id();
+  int out = 0;
+  for (int b = 0; b < n; b += 32) {
+    const int i = b + lane;
+    uint64_t v = 0;
+    bool keep = false;
+    if (i < n) {
+      v = w[i];
+      keep = filter_pass(fbits, key_id(v));
+    }
+    const unsigned m = __ballot_sync(FULL, keep);
+    __syncwarp();
+    if (keep) w[out + __popc(m & ((1u << lane) - 1u))] = v;
+    out += __popc(m);
+    __syncwarp();
+  }
+  return out;
+}
+
 template <class Op, int CH, int U>
 __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const WarpSmem& s, Visited& vis, SortedQueue& W,
                                                       uint64_t* cbuf, uint32_t ccap, const uint32_t* fbits, uint32_t ep,
@@ -74,24 +95,7 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
     const uint64_t fkey = W.w[W.n - 1] & ~1ull;
     // 981: the reference compares DISTANCES here (-(c.dist) > f.dist); with equal distances a larger id must not
     // trigger the retain pass (Hamming / Jaccard / integer L1 tie often)
-    if ((best >> 32) > (fkey >> 32) && W.n >= ef) {  // 994-1000: retain only the points passing the filter
-      int out = 0;
-      for (int b = 0; b < W.n; b += 32) {
-        const int i = b + lane;
-        uint64_t v = 0;
-        bool keep = false;
-        if (i < W.n) {
-          v = W.w[i];
-          keep = filter_pass(fbits, key_id(v));
-        }
-        const unsigned m = __ballot_sync(FULL, keep);
-        __syncwarp();
-        if (keep) W.w[out + __popc(m & ((1u << lane) - 1u))] = v;
-        out += __popc(m);
-        __syncwarp();
-      }
-      W.n = out;
-    }
+    if ((best >> 32) > (fkey >> 32) && W.n >= ef) W.n = keep_passing(W.w, W.n, fbits);  // 994-1000
     const uint32_t c = key_id(best);
     int cap;
     const uint32_t* ids = list_ids(g, c, layer, cap);  // 1006
@@ -166,58 +170,17 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
   uint64_t* cbuf = p.cbuf + (size_t)slot * p.ccap;
   SortedQueue W;
   Stats st{0, 0, 0};
-  const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
 
   for (;;) {
-    uint32_t qi = 0;
-    if (lane == 0) qi = atomicAdd(p.work_counter, 1u);
-    qi = __shfl_sync(FULL, qi, 0);
+    const uint32_t qi = next_item(p.work_counter);
     if (qi >= p.nq) break;
     stage_row_bytes(s.q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes, p.q_bytes, g.d4 * 16);
     int count = 0;
     bool overflow = false;
     W.reset(s.wbuf, p.ef);
     if (g.entry != INVALID_ID) {
-      // descent identical to the unfiltered kernel (hnsw.rs:1511-1529: the filter plays no role here)
-      uint32_t pivot = g.entry;
-      if (lane == 0) s.cand_id[0] = pivot;
-      __syncwarp();
-      warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, 1, s.cand_d);
-      __syncwarp();
-      st.evals += 1;
-      float best = Op::post(s.cand_d[0]);
-      for (int layer = g.entry_level; layer >= 1; --layer) {
-        int cap;
-        const uint32_t* ids = list_ids(g, pivot, layer, cap);
-        uint32_t new_pivot = pivot;
-        for (int b = 0; b < cap; b += 32) {
-          const uint32_t nid = (b + lane < cap) ? ids[b + lane] : INVALID_ID;
-          const unsigned valid = __ballot_sync(FULL, nid != INVALID_ID);
-          const int cnt = __popc(valid);
-          if (cnt) {
-            __syncwarp();
-            if (lane < cnt) s.cand_id[lane] = nid;
-            __syncwarp();
-            warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, cnt, s.cand_d);
-            __syncwarp();
-            st.evals += cnt;
-            st.adj += cnt;
-            uint64_t key = lane < cnt ? (((uint64_t)__float_as_uint(Op::post(s.cand_d[lane])) << 32) | (uint32_t)lane) : ~0ull;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-              uint64_t other = __shfl_xor_sync(FULL, key, o);
-              key = other < key ? other : key;
-            }
-            const float dmin = __uint_as_float((uint32_t)(key >> 32));
-            if (dmin < best) {
-              best = dmin;
-              new_pivot = s.cand_id[(uint32_t)key & 31u];
-            }
-          }
-          if (valid != FULL) break;
-        }
-        pivot = new_pivot;
-      }
+      const Entry e = descend<Op, CH, U>(g, s, st);  // the filter plays no role in the descent (hnsw.rs:1511-1529)
+      const uint32_t pivot = e.pivot;
       search_layer_filtered<Op, CH, U>(g, s, vis, W, cbuf, p.ccap, p.filter_bits, pivot, p.ef, p.layer0, st, overflow);
       count = min(p.k, min(p.ef, W.n));  // hnsw.rs:1547
     }
@@ -248,41 +211,22 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
     __syncwarp();
   }
   vis.save(p.vis, slot);
-  if (p.stats && lane == 0) {
-    atomicAdd(p.stats + 0, (unsigned long long)st.evals);
-    atomicAdd(p.stats + 1, (unsigned long long)st.expansions);
-    atomicAdd(p.stats + 2, (unsigned long long)st.adj);
-  }
+  flush_stats(p.stats, st);
 }
 
 template <class Op>
-static cudaError_t launch_filter_for_op(const SearchParams& p, int grid, size_t smem, cudaStream_t st, bool query_only,
-                                        int* blocks_per_sm) {
-  const int ch = p.g.d4 / 8;
-#define HB_LAUNCH(CHV, UV)                                                                              \
-  do {                                                                                                  \
-    auto kern = search_filter_kernel<Op, CHV, UV>;                                                      \
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-    if (e != cudaSuccess) return e;                                                                     \
-    if (blocks_per_sm) {                                                                                \
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, kern, p.threads, smem);     \
-      if (e != cudaSuccess) return e;                                                                   \
-    }                                                                                                   \
-    if (!query_only) kern<<<grid, p.threads, smem, st>>>(p);                                       \
-    return cudaGetLastError();                                                                          \
-  } while (0)
+static cudaError_t launch_filter_for_op(const SearchParams& p, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm) {
   if constexpr (Specialise<Op>::value) {
-    if (ch == 4) HB_LAUNCH(4, 2);
+    if (p.g.d4 / 8 == 4) return launch_kernel(search_filter_kernel<Op, 4, 2>, p, grid, p.threads, smem, st, blocks_per_sm);
   }
-  HB_LAUNCH(0, 2);
-#undef HB_LAUNCH
+  return launch_kernel(search_filter_kernel<Op, 0, 2>, p, grid, p.threads, smem, st, blocks_per_sm);
 }
 
 cudaError_t launch_search_filtered(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st,
-                                   bool query_only, int* blocks_per_sm) {
+                                   int* blocks_per_sm) {
   return dispatch_op(metric, dtype, [&](auto tag) -> cudaError_t {
     using Op = typename decltype(tag)::type;
-    return launch_filter_for_op<Op>(p, grid, smem, st, query_only, blocks_per_sm);
+    return launch_filter_for_op<Op>(p, grid, smem, st, blocks_per_sm);
   });
 }
 

@@ -81,8 +81,6 @@ Index::Index(int M_, size_t max_elements_, int max_layer_, int ef_c_, int metric
   }
   own_stream_ = stream_;
   sm_count_ = prop.multiProcessorCount;
-  if (const char* k = getenv("HNSW_B200_KERNEL")) kernel_pref_ = strcmp(k, "warp") == 0 ? 1 : 0;
-  if (const char* k = getenv("HNSW_B200_ZERO_COPY")) zero_copy_ = atoi(k) != 0;
   if ((e = cudaMalloc(&d_counter_, sizeof(unsigned int))) != cudaSuccess || (e = cudaMalloc(&d_status_, sizeof(int))) != cudaSuccess ||
       (e = cudaMalloc(&d_stats_, 4 * sizeof(unsigned long long))) != cudaSuccess) {
     err_ = std::string("cudaMalloc: ") + cudaGetErrorString(e);
@@ -106,7 +104,7 @@ Index::~Index() {
   for (SearchCtx& c : ctx_) {
     if (c.stream) cudaStreamSynchronize(c.stream);
     cudaFree(c.vis.tab); cudaFree(c.vis.epoch); cudaFree(c.fvis.tab); cudaFree(c.fvis.epoch); cudaFree(c.d_counter); cudaFree(c.d_status);
-    cudaFree(c.d_q); cudaFree(c.d_out); cudaFree(c.d_cnt); cudaFree(c.d_fbits); cudaFree(c.d_cbuf);
+    cudaFree(c.d_fbits); cudaFree(c.d_cbuf);
     if (c.h_pin) cudaFreeHost(c.h_pin);
     if (c.h_res) cudaFreeHost(c.h_res);
     if (c.fork) cudaEventDestroy(c.fork);
@@ -302,8 +300,7 @@ void Index::rollback_points(size_t keep) {
   }
 }
 
-int Index::run_insert_range(size_t first, size_t count, const std::vector<uint16_t>& masks, size_t mask_off) {
-  (void)masks;
+int Index::run_insert_range(size_t first, size_t count, size_t mask_off) {
   InsertParams p;
   p.g = view();
   p.first = (uint32_t)first;
@@ -327,7 +324,7 @@ int Index::run_insert_range(size_t first, size_t count, const std::vector<uint16
   if (smem > 220 * 1024) return fail("ef_construction / dimension too large for the insert kernel's shared memory");
   p.threads = wpb * 32;
   int bps = 0;
-  HB_CUDA(launch_insert_search(p, metric, dtype, 0, smem, stream_, true, &bps));
+  HB_CUDA(launch_insert_search(p, metric, dtype, 0, smem, stream_, &bps));
   if (bps < 1) return fail("insert kernel does not fit on an SM");
   int grid = (int)std::min<size_t>((size_t)sm_count_ * bps, (count + wpb - 1) / wpb);
   size_t vcap = next_pow2(std::max<size_t>(1024, (size_t)2 * (ef_c + 16) * p.g.deg0));
@@ -336,7 +333,7 @@ int Index::run_insert_range(size_t first, size_t count, const std::vector<uint16
     if ((r = ensure_visited(vis_, (size_t)grid * wpb, vcap, stream_))) return r;
     if ((r = fill_visited_cfg(vis_, p.vis, stream_))) return r;
     HB_CUDA(cudaMemsetAsync(d_counter_, 0, sizeof(unsigned int), stream_));
-    HB_CUDA(launch_insert_search(p, metric, dtype, grid, smem, stream_, false, nullptr));
+    HB_CUDA(launch_insert_search(p, metric, dtype, grid, smem, stream_, nullptr));
     int status = 0;
     HB_CUDA(cudaMemcpyAsync(&status, d_status_, sizeof(int), cudaMemcpyDeviceToHost, stream_));
     HB_CUDA(cudaStreamSynchronize(stream_));
@@ -453,7 +450,7 @@ int Index::insert_batch(const void* vecs, size_t n_new, size_t stride, const voi
       }
     }
     r = promo ? grow_plevel(entry, lv[done]) : 0;  // old entry point gains lists up to the new top
-    if (!r) r = run_insert_range(id, nb, masks, done);
+    if (!r) r = run_insert_range(id, nb, done);
     if (r) {
       // the batches before this one are fully linked and stay; the rest of the call is forgotten.  A CUDA failure can
       // leave half-written links behind: the handle then refuses further work instead of serving a broken graph.
@@ -669,18 +666,17 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.stats = stats_on_ ? d_stats_ : nullptr;
   p.status = c.d_status;
   const bool filtered = d_filter_bits != nullptr;
-  // kernel choice: lean (search_lean.cuh) whenever it applies, else the generic warp kernel (search.cu / filter.cu)
-  // tie mode "std" (search_std.cu): the reference's heaps replayed literally, unfiltered searches only
-  const bool stdtie = tie_std_ && !filtered;
-  const bool lean = !stdtie && !filtered && kernel_pref_ == 0 && entry != INVALID_ID && lean_eligible(p.g.d4, p.ef) && lean_op_supported(metric, dtype);
-  p.q_kind = (filtered || lean || stdtie) ? 0 : queue_kind(p.ef, metric, dtype);
-  p.q_smem = stdtie ? p.ef + 2 : (lean ? lean_queue_slots(p.ef) : queue_slots(p.q_kind, p.ef));
-  size_t spw = stdtie ? (((size_t)p.g.d4 * 16 + (size_t)p.q_smem * 8 + 256 + 127) & ~(size_t)127)
-                      : (lean ? lean_smem_per_warp(p.q_smem) : search_smem_per_warp(p.g.d4, p.q_smem));
+  QueryKernel kind = QueryKernel::Generic;
+  if (filtered) kind = QueryKernel::Filtered;
+  else if (tie_std_) kind = QueryKernel::StdTie;  // unfiltered searches only
+  else if (entry != INVALID_ID && lean_eligible(p.g.d4, p.ef) && lean_op_supported(metric, dtype)) kind = QueryKernel::Lean;
+  p.q_kind = kind == QueryKernel::Generic ? queue_kind(p.ef, metric, dtype) : 0;
+  p.q_smem = query_queue_slots(kind, p.q_kind, p.ef);
+  const size_t spw = query_smem_per_warp(kind, p.g.d4, p.q_smem);
   p.smem_per_warp = (int)spw;
   // warps per CTA: as many as the kernel is built for, fewer when one warp's share of shared memory is large (wide rows,
   // big ef); a single warp must fit
-  int wpb = (lean ? LEAN_THREADS : SEARCH_THREADS) / 32;
+  int wpb = query_threads(kind) / 32;
   while (wpb > 1 && spw * wpb > 220 * 1024) wpb >>= 1;
   const size_t smem = spw * wpb;
   if (smem > 220 * 1024)
@@ -691,15 +687,12 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   int bps = 0;
   {
     std::lock_guard<std::mutex> lk(occ_mu_);
-    const auto key = std::make_tuple(stdtie ? 4 : (lean ? 3 : (int)filtered), (lean ? p.q_smem : p.q_kind) * 64 + wpb, p.g.d4, smem);
+    const auto key = std::make_tuple(kind, p.q_kind, p.q_smem, wpb, p.g.d4, smem);
     auto it = occ_cache_.find(key);
     if (it != occ_cache_.end()) {
       bps = it->second;
     } else {
-      if (stdtie) HB_CUDA(launch_search_std(p, metric, dtype, 0, smem, st, true, &bps));
-      else if (lean) HB_CUDA(launch_search_lean(p, metric, dtype, 0, smem, st, true, &bps));
-      else if (filtered) HB_CUDA(launch_search_filtered(p, metric, dtype, 0, smem, st, true, &bps));
-      else HB_CUDA(launch_search(p, metric, dtype, 0, smem, st, true, &bps));
+      HB_CUDA(launch_query(kind, p, metric, dtype, 0, smem, st, &bps));
       occ_cache_[key] = bps;
     }
   }
@@ -723,17 +716,14 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
     }
     if ((r = ensure_visited(pool, (size_t)grid * per_cta, vcap, st))) return r;
     if ((r = fill_visited_cfg(pool, p.vis, st))) return r;
-    if (filtered || stdtie) {  // candidate queue C: one region per warp slot
+    if (kind == QueryKernel::Filtered || kind == QueryKernel::StdTie) {  // candidate queue C: one region per warp slot
       if ((r = ensure_scratch(&c.d_cbuf, &c.d_cbuf_bytes, (size_t)grid * wpb * pool.cap * 8, st))) return r;
       p.cbuf = (uint64_t*)c.d_cbuf;
       p.ccap = (uint32_t)pool.cap;
     }
     HB_CUDA(cudaMemsetAsync(c.d_counter, 0, sizeof(unsigned int), st));
     HB_CUDA(cudaEventRecord(c.ev0, st));
-    if (stdtie) HB_CUDA(launch_search_std(p, metric, dtype, grid, smem, st, false, nullptr));
-    else if (lean) HB_CUDA(launch_search_lean(p, metric, dtype, grid, smem, st, false, nullptr));
-    else if (filtered) HB_CUDA(launch_search_filtered(p, metric, dtype, grid, smem, st, false, nullptr));
-    else HB_CUDA(launch_search(p, metric, dtype, grid, smem, st, false, nullptr));
+    HB_CUDA(launch_query(kind, p, metric, dtype, grid, smem, st, nullptr));
     HB_CUDA(cudaEventRecord(c.ev1, st));
     if (!sync) break;
     int status = 0;
@@ -763,12 +753,11 @@ static const void* device_view_of_host(const void* p) {
   return nullptr;
 }
 
-// Host queries in, host answers out.  ZERO-COPY when the memory allows it: a pinned query buffer is read by the
-// kernel itself (each query crosses the bus once, 512 bytes when its warp picks it up, while thousands of other
-// queries are being searched), and the answers are written by the kernel straight into the index's pinned result
-// buffer: no cudaMemcpy before or after the launch, one synchronisation.  Pageable queries and row pointers are
-// gathered into the index's own pinned staging buffer first (the only host-side copy), which the kernel then reads
-// the same way.  zero_copy_ = false (env HNSW_B200_ZERO_COPY=0) restores explicit H2D / D2H copies.
+// Host queries in, host answers out, with no cudaMemcpy before or after the launch.  A pinned query buffer is read by the
+// kernel itself (each query crosses the bus once, 512 bytes when its warp picks it up, while thousands of other queries
+// are being searched), and the answers are written by the kernel straight into the context's pinned result buffer: one
+// synchronisation.  Pageable queries and row pointers are gathered into the context's own pinned staging buffer first
+// (the only host-side copy), which the kernel then reads the same way.
 int Index::search_host_begin(int ci, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
                              const uint32_t* filter_bits_host) {
   SearchCtx& c = ctx_[ci];
@@ -795,52 +784,34 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
   c.pend.nq = nq;
   c.pend.k = k;
   c.pend.ef = ef;
-  c.pend.out_bytes = out_bytes;
-  c.pend.cnt_bytes = cnt_bytes;
   if (dim == 0) {  // empty index: every answer is empty (hnsw.rs:1498-1500)
     for (size_t i = 0; i < nq; ++i) hcnt[i] = 0;
     for (size_t i = 0; i < nq * k; ++i) hout[i] = NeighbourOut{~0ull, __builtin_inff(), INVALID_ID};
     return 0;
   }
   const size_t qbytes = nq * (size_t)dim * es;
-  const void* d_queries = nullptr;  // what the kernel reads
-  const void* host_src = queries;
-  if (rows || !(zero_copy_ && device_view_of_host(queries))) {
-    // gather into pinned staging (rows: one pointer per query, libext.rs parallel_search_neighbours_<ty>)
-    if (rows || !device_view_of_host(queries)) {
-      if (c.h_pin_bytes < qbytes) {
-        if (c.h_pin) cudaFreeHost(c.h_pin);
-        c.h_pin = nullptr;
-        c.h_pin_bytes = 0;
-        HB_CUDA(cudaHostAlloc(&c.h_pin, qbytes, cudaHostAllocMapped | cudaHostAllocPortable));
-        c.h_pin_bytes = qbytes;
-      }
-      unsigned char* st = (unsigned char*)c.h_pin;
-      if (rows)
-        for (size_t i = 0; i < nq; ++i) memcpy(st + i * (size_t)dim * es, rows[i], (size_t)dim * es);
-      else
-        memcpy(st, queries, qbytes);
-      host_src = st;
-    }
-  }
-  if (zero_copy_) d_queries = device_view_of_host(host_src);
+  const void* d_queries = rows ? nullptr : device_view_of_host(queries);  // what the kernel reads
   if (!d_queries) {
-    if ((r = ensure_scratch(&c.d_q, &c.d_q_bytes, qbytes, st))) return r;
-    HB_CUDA(cudaMemcpyAsync(c.d_q, host_src, qbytes, cudaMemcpyHostToDevice, st));
-    d_queries = c.d_q;
+    // gather into pinned staging (rows: one pointer per query, libext.rs parallel_search_neighbours_<ty>)
+    if (c.h_pin_bytes < qbytes) {
+      if (c.h_pin) cudaFreeHost(c.h_pin);
+      c.h_pin = nullptr;
+      c.h_pin_bytes = 0;
+      HB_CUDA(cudaHostAlloc(&c.h_pin, qbytes, cudaHostAllocMapped | cudaHostAllocPortable));
+      c.h_pin_bytes = qbytes;
+    }
+    unsigned char* stage = (unsigned char*)c.h_pin;
+    if (rows)
+      for (size_t i = 0; i < nq; ++i) memcpy(stage + i * (size_t)dim * es, rows[i], (size_t)dim * es);
+    else
+      memcpy(stage, queries, qbytes);
+    d_queries = device_view_of_host(stage);
+    if (!d_queries) return fail("the pinned query staging buffer has no device address");
   }
-  NeighbourOut* k_out = nullptr;  // where the kernel writes
-  int32_t* k_cnt = nullptr;
-  const void* dv = zero_copy_ ? device_view_of_host(c.h_res) : nullptr;
-  if (dv) {
-    k_out = (NeighbourOut*)dv;
-    k_cnt = (int32_t*)((char*)dv + out_bytes);
-  } else {
-    if ((r = ensure_scratch(&c.d_out, &c.d_out_bytes, out_bytes, st))) return r;
-    if ((r = ensure_scratch(&c.d_cnt, &c.d_cnt_bytes, cnt_bytes, st))) return r;
-    k_out = (NeighbourOut*)c.d_out;
-    k_cnt = (int32_t*)c.d_cnt;
-  }
+  char* dv = (char*)device_view_of_host(c.h_res);  // where the kernel writes
+  if (!dv) return fail("the pinned result buffer has no device address");
+  NeighbourOut* k_out = (NeighbourOut*)dv;
+  int32_t* k_cnt = (int32_t*)(dv + out_bytes);
   const uint32_t* dfb = nullptr;
   if (filter_bits_host) {
     const size_t fb = ((n + 31) / 32) * 4;
@@ -848,19 +819,14 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
     HB_CUDA(cudaMemcpyAsync(c.d_fbits, filter_bits_host, fb, cudaMemcpyHostToDevice, st));
     dfb = (const uint32_t*)c.d_fbits;
   }
-  // one enqueue (copies if any, kernel, status); search_host_finish synchronises once and takes the slow path (a visited
-  // table overflowed: grow and re-run) only when the status says so
+  // one enqueue (filter bits if any, kernel, status); search_host_finish synchronises once and takes the slow path (a
+  // visited table overflowed: grow and re-run) only when the status says so
   c.pend.d_queries = d_queries;
   c.pend.dfb = dfb;
   c.pend.k_out = k_out;
   c.pend.k_cnt = k_cnt;
-  c.pend.direct = dv != nullptr;
   c.pend.enqueued = true;
   if ((r = search_on_ctx(c, d_queries, nq, k, ef, dfb, k_out, k_cnt, false, nullptr))) return r;
-  if (!c.pend.direct) {
-    HB_CUDA(cudaMemcpyAsync(hout, c.d_out, out_bytes, cudaMemcpyDeviceToHost, st));
-    HB_CUDA(cudaMemcpyAsync(hcnt, c.d_cnt, cnt_bytes, cudaMemcpyDeviceToHost, st));
-  }
   HB_CUDA(cudaMemcpyAsync(hstatus, c.d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   return 0;
 }
@@ -876,14 +842,7 @@ int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** 
   HB_CUDA(cudaStreamSynchronize(st));
   if (*p.hstatus == 0) return 0;
   HB_CUDA(cudaMemsetAsync(c.d_status, 0, sizeof(int), st));
-  int r;
-  if ((r = search_on_ctx(c, p.d_queries, p.nq, p.k, p.ef, p.dfb, p.k_out, p.k_cnt, true, nullptr))) return r;  // grows the tables
-  if (!p.direct) {
-    HB_CUDA(cudaMemcpyAsync(p.hout, c.d_out, p.out_bytes, cudaMemcpyDeviceToHost, st));
-    HB_CUDA(cudaMemcpyAsync(p.hcnt, c.d_cnt, p.cnt_bytes, cudaMemcpyDeviceToHost, st));
-    HB_CUDA(cudaStreamSynchronize(st));
-  }
-  return 0;
+  return search_on_ctx(c, p.d_queries, p.nq, p.k, p.ef, p.dfb, p.k_out, p.k_cnt, true, nullptr);  // grows the tables
 }
 
 int Index::search_host_staged(int ci, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,

@@ -174,8 +174,8 @@ class Index {
     unsigned int* d_counter = nullptr;
     int* d_status = nullptr;
     VisitedPool vis, fvis;  // unfiltered / filtered searches
-    void *d_q = nullptr, *d_out = nullptr, *d_cnt = nullptr, *d_fbits = nullptr, *d_cbuf = nullptr;
-    size_t d_q_bytes = 0, d_out_bytes = 0, d_cnt_bytes = 0, d_fbits_bytes = 0, d_cbuf_bytes = 0;
+    void *d_fbits = nullptr, *d_cbuf = nullptr;
+    size_t d_fbits_bytes = 0, d_cbuf_bytes = 0;
     void *h_pin = nullptr, *h_res = nullptr;  // pinned, mapped: query staging / answers
     size_t h_pin_bytes = 0, h_res_bytes = 0;
     bool busy = false;
@@ -184,8 +184,8 @@ class Index {
       const uint32_t* dfb = nullptr;
       NeighbourOut *k_out = nullptr, *hout = nullptr;
       int32_t *k_cnt = nullptr, *hcnt = nullptr, *hstatus = nullptr;
-      size_t nq = 0, k = 0, ef = 0, out_bytes = 0, cnt_bytes = 0;
-      bool direct = false, enqueued = false;
+      size_t nq = 0, k = 0, ef = 0;
+      bool enqueued = false;
       // where hnsw_b200_search_flat_wait unpacks to
       uint64_t* u_ids = nullptr;
       float* u_dist = nullptr;
@@ -230,7 +230,7 @@ class Index {
   int fill_visited_cfg(VisitedPool& v, VisitedCfg& c, cudaStream_t st);
   int ensure_scratch(void** p, size_t* cur, size_t need, cudaStream_t st);
   int grow_plevel(uint32_t id, int new_plevel);
-  int run_insert_range(size_t first, size_t count, const std::vector<uint16_t>& masks, size_t mask_off);
+  int run_insert_range(size_t first, size_t count, size_t mask_off);
   int check_insert_fit();
   void rollback_points(size_t keep);
   template <class T>
@@ -277,8 +277,6 @@ class Index {
   int last_async_ = -1;
   unsigned ctx_rr_ = 0;        // round robin of the asynchronous device-resident launches
   std::mutex occ_mu_;
-  int kernel_pref_ = 0;        // env HNSW_B200_KERNEL=warp (A/B measurements): 1 = always the generic warp kernel
-  bool zero_copy_ = true;      // env HNSW_B200_ZERO_COPY=0: explicit H2D / D2H copies instead of kernel access to pinned host memory
 
   // small device scratch (insert path; searches: SearchCtx)
   unsigned int* d_counter_ = nullptr;
@@ -290,7 +288,8 @@ class Index {
   // staging of the insert path
   void* h_pin_ = nullptr;
   size_t h_pin_bytes_ = 0;
-  std::map<std::tuple<int, int, int, size_t>, int> occ_cache_;  // (filtered, queue kind, d4, smem) -> CTAs/SM
+  // (kernel, queue kind, queue slots, warps per CTA, d4, shared memory per CTA) -> CTAs per SM
+  std::map<std::tuple<QueryKernel, int, int, int, int, size_t>, int> occ_cache_;
   void* d_mask_ = nullptr;
   size_t d_mask_bytes_ = 0;
 };

@@ -69,16 +69,32 @@ inline int queue_kind(int ef, int metric, int dtype) {
   return 108;
 }
 inline int queue_slots(int kind, int ef) { return kind >= 100 ? 32 * (kind - 100) : ef; }
-inline size_t search_smem_per_warp(int d4, int q_smem) {
-  size_t b = stage_bytes(d4) + (size_t)d4 * 16 + (size_t)q_smem * 8 + 64 * 8 + 16;
-  return (b + 127) & ~(size_t)127;
-}
 
-// ---- lean kernel (search_lean.cuh): eligibility and shared-memory footprint
-// rows of 128 / 256 / 512 bytes (compile-time chunk count), ef <= 128, no filter
+// ---- lean kernel (search_lean.cuh): rows of 128 / 256 / 512 bytes (compile-time chunk count), ef <= 128, no filter
 inline int lean_queue_slots(int ef) { return ef <= 64 ? 64 : (ef <= 128 ? 128 : 0); }
 inline bool lean_eligible(int d4, int ef) { return (d4 == 8 || d4 == 16 || d4 == 32) && lean_queue_slots(ef) != 0; }
-inline size_t lean_smem_per_warp(int qc) { return (size_t)qc * 8 + 256; }
+
+// ---- the query kernels.  Lean (search_lean.cuh) whenever it applies, else the generic warp kernel (search.cu), the
+// filtered kernel (filter.cu), or with tie mode "std" the reference's heaps replayed literally (search_std.cu).
+enum class QueryKernel { Lean, Generic, Filtered, StdTie };
+// queue slots in shared memory (q_kind: QueueSel kind, used by the generic kernel only)
+inline int query_queue_slots(QueryKernel kind, int q_kind, int ef) {
+  switch (kind) {
+    case QueryKernel::Lean: return lean_queue_slots(ef);
+    case QueryKernel::StdTie: return ef + 2;
+    default: return queue_slots(q_kind, ef);
+  }
+}
+inline size_t query_smem_per_warp(QueryKernel kind, int d4, int q_smem) {
+  size_t b;
+  switch (kind) {
+    case QueryKernel::Lean: return (size_t)q_smem * 8 + 256;  // [queue keys / query staging][row ids][distances]
+    case QueryKernel::StdTie: b = (size_t)d4 * 16 + (size_t)q_smem * 8 + 256; break;  // [query][W heap][row ids][distances]
+    default: b = stage_bytes(d4) + (size_t)d4 * 16 + (size_t)q_smem * 8 + 64 * 8 + 16;  // search.cu's layout
+  }
+  return (b + 127) & ~(size_t)127;
+}
+inline int query_threads(QueryKernel kind) { return kind == QueryKernel::Lean ? LEAN_THREADS : SEARCH_THREADS; }
 
 struct InsertParams {
   GraphView g;
@@ -104,22 +120,41 @@ inline size_t insert_smem_per_warp(int d4, int ef_c, int deg0, int q_smem) {
   return (b + 127) & ~(size_t)127;
 }
 
+// Every launcher below sets the kernel's dynamic shared-memory limit to `smem`, then either launches it (blocks_per_sm ==
+// nullptr) or only reports how many CTAs of `threads` threads fit on one SM.
+template <class P>
+cudaError_t launch_kernel(void (*kern)(P), const P& p, int grid, int threads, size_t smem, cudaStream_t st, int* blocks_per_sm) {
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  if (e != cudaSuccess) return e;
+  if (blocks_per_sm) return cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, kern, threads, smem);
+  kern<<<grid, threads, smem, st>>>(p);
+  return cudaGetLastError();
+}
+
 cudaError_t launch_insert_search(const InsertParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st,
-                                 bool query_only, int* blocks_per_sm);
+                                 int* blocks_per_sm);
 cudaError_t launch_insert_link(const InsertParams& p, int grid, cudaStream_t st);
 
 cudaError_t launch_search_filtered(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st,
-                                   bool query_only, int* blocks_per_sm);
-cudaError_t launch_search(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st, bool query_only,
-                          int* blocks_per_sm);
-cudaError_t launch_search_std(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st, bool query_only,
+                                   int* blocks_per_sm);
+cudaError_t launch_search(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm);
+cudaError_t launch_search_std(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st,
                               int* blocks_per_sm);
 cudaError_t launch_search_lean(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st,
-                               bool query_only, int* blocks_per_sm);
-cudaError_t launch_search_lean_u8(const SearchParams& p, int metric, int grid, size_t smem, cudaStream_t st, bool query_only,
-                                  int* blocks_per_sm);
-cudaError_t launch_search_lean_u16(const SearchParams& p, int metric, int grid, size_t smem, cudaStream_t st, bool query_only,
-                                   int* blocks_per_sm);
+                               int* blocks_per_sm);
+cudaError_t launch_search_lean_u8(const SearchParams& p, int metric, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm);
+cudaError_t launch_search_lean_u16(const SearchParams& p, int metric, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm);
+
+inline cudaError_t launch_query(QueryKernel kind, const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st,
+                                int* blocks_per_sm) {
+  switch (kind) {
+    case QueryKernel::Lean: return launch_search_lean(p, metric, dtype, grid, smem, st, blocks_per_sm);
+    case QueryKernel::Generic: return launch_search(p, metric, dtype, grid, smem, st, blocks_per_sm);
+    case QueryKernel::Filtered: return launch_search_filtered(p, metric, dtype, grid, smem, st, blocks_per_sm);
+    case QueryKernel::StdTie: return launch_search_std(p, metric, dtype, grid, smem, st, blocks_per_sm);
+  }
+  return cudaErrorInvalidValue;
+}
 
 // ---- (metric, element type) -> distance functor.  f is called as f(OpTag<Op>{}) and returns cudaError_t.
 template <class Op>

@@ -24,23 +24,15 @@ __device__ __forceinline__ MinMax64 rshfl(const MinMax64& a, int off) {
 // ---- the "still unexpanded" mask over queue positions: bit p set <=> W[p] has not been expanded yet
 struct Mask64 {
   uint64_t m;
-  __device__ __forceinline__ void clear() { m = 0; }
   __device__ __forceinline__ bool none() const { return m == 0; }
   __device__ __forceinline__ int first() const { return __ffsll((long long)m) - 1; }  // -1 when none
   __device__ __forceinline__ void drop_first() { m &= m - 1; }
   __device__ __forceinline__ void set_only(int p) { m = 1ull << p; }
   __device__ __forceinline__ bool test(int p) const { return (m >> p) & 1ull; }
   __device__ __forceinline__ void set_words(const uint32_t (&w)[2]) { m = (uint64_t)w[0] | ((uint64_t)w[1] << 32); }
-  // a key enters the queue at position p: entries at >= p move up by one, the bit beyond `cap` entries falls off
-  __device__ __forceinline__ void insert_at(int p, int cap) {
-    const uint64_t low = (1ull << p) - 1ull;
-    m = (m & low) | (1ull << p) | ((m & ~low) << 1);
-    if (cap < 64) m &= (1ull << cap) - 1ull;
-  }
 };
 struct Mask128 {
   uint64_t lo, hi;
-  __device__ __forceinline__ void clear() { lo = hi = 0; }
   __device__ __forceinline__ bool none() const { return (lo | hi) == 0; }
   __device__ __forceinline__ int first() const {
     return lo ? __ffsll((long long)lo) - 1 : (hi ? 63 + __ffsll((long long)hi) : -1);
@@ -57,26 +49,6 @@ struct Mask128 {
   __device__ __forceinline__ void set_words(const uint32_t (&w)[4]) {
     lo = (uint64_t)w[0] | ((uint64_t)w[1] << 32);
     hi = (uint64_t)w[2] | ((uint64_t)w[3] << 32);
-  }
-  __device__ __forceinline__ void insert_at(int p, int cap) {
-    const uint64_t carry = lo >> 63;
-    if (p < 64) {
-      const uint64_t low = (1ull << p) - 1ull;
-      lo = (lo & low) | (1ull << p) | ((lo & ~low) << 1);
-      hi = (hi << 1) | carry;
-    } else {
-      const int q = p - 64;
-      const uint64_t low = (1ull << q) - 1ull;
-      hi = (hi & low) | (1ull << q) | ((hi & ~low) << 1);
-    }
-    if (cap < 128) {
-      if (cap <= 64) {
-        hi = 0;
-        if (cap < 64) lo &= (1ull << cap) - 1ull;
-      } else {
-        hi &= (1ull << (cap - 64)) - 1ull;
-      }
-    }
   }
 };
 template <int QC>

@@ -34,128 +34,50 @@ __global__ void __launch_bounds__(SEARCH_THREADS, 4) search_kernel(SearchParams 
   Queue Q;
   Q.reset(s.wbuf, p.ef);
   Stats st{0, 0, 0};
-  const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
 
   for (;;) {
-    uint32_t qi = 0;
-    if (lane == 0) qi = atomicAdd(p.work_counter, 1u);
-    qi = __shfl_sync(FULL, qi, 0);
+    const uint32_t qi = next_item(p.work_counter);
     if (qi >= p.nq) break;
     // stage the query (zero padded to d_pad)
     stage_row_bytes(s.q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes, p.q_bytes, g.d4 * 16);
-
     int count = 0;
     bool overflow = false;
     if (g.entry != INVALID_ID) {  // hnsw.rs:1498-1503
-      // ---- descent: ONE pass over pivot.neighbours[layer] per layer (hnsw.rs:1511-1529)
-      uint32_t pivot = g.entry;
-      if (lane == 0) s.cand_id[0] = pivot;
-      __syncwarp();
-      warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, 1, s.cand_d);  // hnsw.rs:1506
-      __syncwarp();
-      st.evals += 1;
-      float best = Op::post(s.cand_d[0]);
-      for (int layer = g.entry_level; layer >= 1; --layer) {
-        int cap;
-        const uint32_t* ids = list_ids(g, pivot, layer, cap);
-        uint32_t new_pivot = pivot;
-        for (int b = 0; b < cap; b += 32) {
-          const uint32_t nid = (b + lane < cap) ? ids[b + lane] : INVALID_ID;
-          const unsigned valid = __ballot_sync(FULL, nid != INVALID_ID);
-          const int cnt = __popc(valid);  // dense prefix
-          if (cnt) {
-            __syncwarp();
-            if (lane < cnt) s.cand_id[lane] = nid;
-            __syncwarp();
-            warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, cnt, s.cand_d);  // hnsw.rs:1518
-            __syncwarp();
-            st.evals += cnt;
-            st.adj += cnt;
-            // strict `<` scanned in list order == first minimum of the list, if below `best`
-            uint64_t key = lane < cnt ? (((uint64_t)__float_as_uint(Op::post(s.cand_d[lane])) << 32) | (uint32_t)lane) : ~0ull;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-              uint64_t other = __shfl_xor_sync(FULL, key, o);
-              key = other < key ? other : key;
-            }
-            const float dmin = __uint_as_float((uint32_t)(key >> 32));
-            if (dmin < best) {
-              best = dmin;
-              new_pivot = s.cand_id[(uint32_t)key & 31u];
-            }
-          }
-          if (valid != FULL) break;
-        }
-        pivot = new_pivot;  // hnsw.rs:1526-1528
-      }
+      const Entry e = descend<Op, CH, U>(g, s, st);
       // ---- layer-0 (lowest populated layer) search, hnsw.rs:1531-1542
-      search_layer<Op, CH, U, Queue>(g, s, stg, vis, Q, pivot, p.ef, p.layer0, st, overflow);
+      search_layer<Op, CH, U, Queue>(g, s, stg, vis, Q, e.pivot, p.ef, p.layer0, st, overflow);
       count = min(p.k, min(p.ef, Q.n));  // hnsw.rs:1547
     }
-    if (overflow) {
-      if (lane == 0) atomicExch(p.status, 1);
-      count = 0;
-    }
-    // ---- ascending top-k (hnsw.rs:1544-1579); the queue is already sorted
-    const size_t ob = (size_t)qi * p.k;
-    for (int j = lane; j < p.k; j += 32) {
-      if (j < count) {
-        const uint64_t key = Q.local(j);
-        const uint32_t id = key_id(key);
-        p.out_nb[ob + j] = NeighbourOut{g.origin[id], key_dist(key), id};
-      } else {
-        p.out_nb[ob + j] = NeighbourOut{~0ull, __int_as_float(0x7f800000), INVALID_ID};
-      }
-    }
-    if (lane == 0) p.out_count[qi] = count;
-    __syncwarp();
+    write_answers(p, qi, overflow, count, [&](int j) { return Q.local(j); });  // the queue is already sorted
   }
   vis.save(p.vis, slot);
-  if (p.stats) {
-    if (lane == 0) {  // the counters are warp-uniform
-      atomicAdd(p.stats + 0, (unsigned long long)st.evals);
-      atomicAdd(p.stats + 1, (unsigned long long)st.expansions);
-      atomicAdd(p.stats + 2, (unsigned long long)st.adj);
-    }
-  }
+  flush_stats(p.stats, st);
 }
 
+// Compile-time row length (CH chunks of 128 bytes) only where the lean kernel cannot take the search: a 256-slot queue
+// (ef 129-256) or the generic one (ef > 256).  With a 32 / 64 / 128-slot queue the generic kernel runs only on an index
+// without an entry point, whose answers are empty.
 template <class Op, int NS>
-static cudaError_t launch_for_op(const SearchParams& p, int grid, size_t smem, cudaStream_t st, bool query_only,
-                                 int* blocks_per_sm) {
+static cudaError_t launch_for_op(const SearchParams& p, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm) {
   const int ch = p.g.d4 / 8;
-#define HB_LAUNCH(CHV, UV)                                                                                      \
-  do {                                                                                                          \
-    auto kern = search_kernel<Op, CHV, UV, NS>;                                                                 \
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);         \
-    if (e != cudaSuccess) return e;                                                                             \
-    if (blocks_per_sm) {                                                                                        \
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, kern, p.threads, smem);             \
-      if (e != cudaSuccess) return e;                                                                           \
-    }                                                                                                           \
-    if (!query_only) kern<<<grid, p.threads, smem, st>>>(p);                                               \
-    return cudaGetLastError();                                                                                  \
-  } while (0)
-  if constexpr (Specialise<Op>::value) {
-    if (ch == 1) HB_LAUNCH(1, 4);
-    if (ch == 2) HB_LAUNCH(2, 4);
-    if (ch == 4) HB_LAUNCH(4, 2);
+  if constexpr (Specialise<Op>::value && (NS == 0 || NS == 108)) {
+    if (ch == 1) return launch_kernel(search_kernel<Op, 1, 4, NS>, p, grid, p.threads, smem, st, blocks_per_sm);
+    if (ch == 2) return launch_kernel(search_kernel<Op, 2, 4, NS>, p, grid, p.threads, smem, st, blocks_per_sm);
+    if (ch == 4) return launch_kernel(search_kernel<Op, 4, 2, NS>, p, grid, p.threads, smem, st, blocks_per_sm);
   }
-  HB_LAUNCH(0, 2);
-#undef HB_LAUNCH
+  return launch_kernel(search_kernel<Op, 0, 2, NS>, p, grid, p.threads, smem, st, blocks_per_sm);
 }
 
-cudaError_t launch_search(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st,
-                          bool query_only, int* blocks_per_sm) {
+cudaError_t launch_search(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm) {
   return dispatch_op(metric, dtype, [&](auto tag) -> cudaError_t {
     using Op = typename decltype(tag)::type;
     if constexpr (Specialise<Op>::value) {
-      if (p.q_kind == 101) return launch_for_op<Op, 101>(p, grid, smem, st, query_only, blocks_per_sm);
-      if (p.q_kind == 102) return launch_for_op<Op, 102>(p, grid, smem, st, query_only, blocks_per_sm);
-      if (p.q_kind == 104) return launch_for_op<Op, 104>(p, grid, smem, st, query_only, blocks_per_sm);
-      if (p.q_kind == 108) return launch_for_op<Op, 108>(p, grid, smem, st, query_only, blocks_per_sm);
+      if (p.q_kind == 101) return launch_for_op<Op, 101>(p, grid, smem, st, blocks_per_sm);
+      if (p.q_kind == 102) return launch_for_op<Op, 102>(p, grid, smem, st, blocks_per_sm);
+      if (p.q_kind == 104) return launch_for_op<Op, 104>(p, grid, smem, st, blocks_per_sm);
+      if (p.q_kind == 108) return launch_for_op<Op, 108>(p, grid, smem, st, blocks_per_sm);
     }
-    return launch_for_op<Op, 0>(p, grid, smem, st, query_only, blocks_per_sm);
+    return launch_for_op<Op, 0>(p, grid, smem, st, blocks_per_sm);
   });
 }
 

@@ -1,8 +1,10 @@
 // search_layer on a warp: the ef-bounded best-first expansion of one layer.
 // Restates /root/reference/src/hnsw.rs:922-1064 (search_layer) for one warp that owns the whole
 // queue state of one query; used by the query kernel (search.cu) and the insert kernel (build.cu).
+// Also the per-query scaffold the warp query kernels (search.cu, filter.cu, search_std.cu) share: work counter,
+// upper-layer descent, answer write-out, counter flush.
 #pragma once
-#include "common.cuh"
+#include "kernels.h"
 
 namespace hb {
 
@@ -89,6 +91,99 @@ __device__ __forceinline__ void search_layer(const GraphView& g, const WarpSmem&
       overflow = true;
       break;
     }
+  }
+}
+
+// the next work item of this warp from a launch's work counter (warp-uniform)
+__device__ __forceinline__ uint32_t next_item(unsigned int* work_counter) {
+  uint32_t i = 0;
+  if (lane_id() == 0) i = atomicAdd(work_counter, 1u);
+  return __shfl_sync(FULL, i, 0);
+}
+
+struct Entry {
+  uint32_t pivot;  // entry point of the lowest layer
+  float best;      // its distance
+};
+
+// Upper-layer descent (hnsw.rs:1498-1529): from the graph's entry point, ONE pass over pivot.neighbours[layer] per
+// layer, moving to the first minimum of the list when it is strictly below the best distance so far.
+template <class Op, int CH, int U>
+__device__ __forceinline__ Entry descend(const GraphView& g, const WarpSmem& s, Stats& st) {
+  const int lane = lane_id();
+  const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
+  uint32_t pivot = g.entry;
+  if (lane == 0) s.cand_id[0] = pivot;
+  __syncwarp();
+  warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, 1, s.cand_d);  // hnsw.rs:1506
+  __syncwarp();
+  st.evals += 1;
+  float best = Op::post(s.cand_d[0]);
+  for (int layer = g.entry_level; layer >= 1; --layer) {
+    int cap;
+    const uint32_t* ids = list_ids(g, pivot, layer, cap);
+    uint32_t new_pivot = pivot;
+    for (int b = 0; b < cap; b += 32) {
+      const uint32_t nid = (b + lane < cap) ? ids[b + lane] : INVALID_ID;
+      const unsigned valid = __ballot_sync(FULL, nid != INVALID_ID);
+      const int cnt = __popc(valid);  // dense prefix
+      if (cnt) {
+        __syncwarp();
+        if (lane < cnt) s.cand_id[lane] = nid;
+        __syncwarp();
+        warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, cnt, s.cand_d);  // hnsw.rs:1518
+        __syncwarp();
+        st.evals += cnt;
+        st.adj += cnt;
+        // strict `<` scanned in list order == first minimum of the list, if below `best`
+        uint64_t key = lane < cnt ? (((uint64_t)__float_as_uint(Op::post(s.cand_d[lane])) << 32) | (uint32_t)lane) : ~0ull;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+          const uint64_t other = __shfl_xor_sync(FULL, key, o);
+          key = other < key ? other : key;
+        }
+        const float dmin = __uint_as_float((uint32_t)(key >> 32));
+        if (dmin < best) {
+          best = dmin;
+          new_pivot = s.cand_id[(uint32_t)key & 31u];
+        }
+      }
+      if (valid != FULL) break;
+    }
+    pivot = new_pivot;  // hnsw.rs:1526-1528
+  }
+  return Entry{pivot, best};
+}
+
+// The answers of query qi (hnsw.rs:1544-1579): key_at(j) for j < count, ascending, then (~0, +inf, INVALID_ID) up to k.
+// A query whose visited table overflowed answers nothing and raises the launch's status flag (the host re-runs it).
+template <class KeyAt>
+__device__ __forceinline__ void write_answers(const SearchParams& p, uint32_t qi, bool overflow, int count, KeyAt&& key_at) {
+  const int lane = lane_id();
+  if (overflow) {
+    if (lane == 0) atomicExch(p.status, 1);
+    count = 0;
+  }
+  const size_t ob = (size_t)qi * p.k;
+  for (int j = lane; j < p.k; j += 32) {
+    if (j < count) {
+      const uint64_t key = key_at(j);
+      const uint32_t id = key_id(key);
+      p.out_nb[ob + j] = NeighbourOut{p.g.origin[id], key_dist(key), id};
+    } else {
+      p.out_nb[ob + j] = NeighbourOut{~0ull, __int_as_float(0x7f800000), INVALID_ID};
+    }
+  }
+  if (lane == 0) p.out_count[qi] = count;
+  __syncwarp();
+}
+
+// the traversal counters of one warp into the launch's totals (the counters are warp-uniform)
+__device__ __forceinline__ void flush_stats(unsigned long long* stats, const Stats& st) {
+  if (stats && lane_id() == 0) {
+    atomicAdd(stats + 0, (unsigned long long)st.evals);
+    atomicAdd(stats + 1, (unsigned long long)st.expansions);
+    atomicAdd(stats + 2, (unsigned long long)st.adj);
   }
 }
 

@@ -403,47 +403,33 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
   }
 }
 
+template <class Op, int CH, int QC>
+static cudaError_t launch_lean_kernel(const SearchParams& p, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm) {
+  if (p.stats) return launch_kernel(search_lean_kernel<Op, CH, QC, true>, p, grid, LEAN_THREADS, smem, st, blocks_per_sm);
+  return launch_kernel(search_lean_kernel<Op, CH, QC, false>, p, grid, LEAN_THREADS, smem, st, blocks_per_sm);
+}
+
 template <class Op, int QC>
-static cudaError_t launch_lean_for_op(const SearchParams& p, int grid, size_t smem, cudaStream_t st, bool query_only,
-                                      int* blocks_per_sm) {
+static cudaError_t launch_lean_for_op(const SearchParams& p, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm) {
   const int ch = p.g.d4 / 8;
-#define HB_LAUNCH_LEAN2(CHV, STV)                                                                            \
-  do {                                                                                                       \
-    auto kern = search_lean_kernel<Op, CHV, QC, STV>;                                                        \
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);      \
-    if (e != cudaSuccess) return e;                                                                          \
-    if (blocks_per_sm) {                                                                                     \
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, kern, LEAN_THREADS, smem);            \
-      if (e != cudaSuccess) return e;                                                                        \
-    }                                                                                                        \
-    if (!query_only) kern<<<grid, LEAN_THREADS, smem, st>>>(p);                                              \
-    return cudaGetLastError();                                                                               \
-  } while (0)
-#define HB_LAUNCH_LEAN(CHV)                  \
-  do {                                       \
-    if (p.stats) HB_LAUNCH_LEAN2(CHV, true); \
-    HB_LAUNCH_LEAN2(CHV, false);             \
-  } while (0)
 #ifndef HB_FAST_BUILD
-  if (ch == 1) HB_LAUNCH_LEAN(1);
-  if (ch == 2) HB_LAUNCH_LEAN(2);
+  if (ch == 1) return launch_lean_kernel<Op, 1, QC>(p, grid, smem, st, blocks_per_sm);
+  if (ch == 2) return launch_lean_kernel<Op, 2, QC>(p, grid, smem, st, blocks_per_sm);
 #endif
-  if (ch == 4) HB_LAUNCH_LEAN(4);
-#undef HB_LAUNCH_LEAN
-#undef HB_LAUNCH_LEAN2
+  if (ch == 4) return launch_lean_kernel<Op, 4, QC>(p, grid, smem, st, blocks_per_sm);
   return cudaErrorInvalidValue;
 }
 
 // one translation unit per element type instantiates the kernels (search_lean_f32.cu, search_lean_u8.cu, search_lean_u16.cu)
 template <class Op>
-static cudaError_t launch_lean_op(const SearchParams& p, int grid, size_t smem, cudaStream_t st, bool query_only, int* blocks_per_sm) {
+static cudaError_t launch_lean_op(const SearchParams& p, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm) {
 #ifdef HB_FAST_BUILD  // scripts/variants.sh: one instantiation, for A/B builds
   if constexpr (std::is_same<Op, OpL2>::value) {
-    if (p.q_smem == 64) return launch_lean_for_op<Op, 64>(p, grid, smem, st, query_only, blocks_per_sm);
+    if (p.q_smem == 64) return launch_lean_for_op<Op, 64>(p, grid, smem, st, blocks_per_sm);
   }
 #else
-  if (p.q_smem == 64) return launch_lean_for_op<Op, 64>(p, grid, smem, st, query_only, blocks_per_sm);
-  if (p.q_smem == 128) return launch_lean_for_op<Op, 128>(p, grid, smem, st, query_only, blocks_per_sm);
+  if (p.q_smem == 64) return launch_lean_for_op<Op, 64>(p, grid, smem, st, blocks_per_sm);
+  if (p.q_smem == 128) return launch_lean_for_op<Op, 128>(p, grid, smem, st, blocks_per_sm);
 #endif
   return cudaErrorInvalidValue;
 }

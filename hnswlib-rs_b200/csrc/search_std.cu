@@ -140,55 +140,19 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_std_kernel(SearchParams
     StdHeap W{wv, 0}, C{cv, 0};
     if (g.entry != INVALID_ID) {
       // ---- descent (hnsw.rs:1498-1529): strict '<' in list order, distances only: as in every kernel
-      uint32_t pivot = g.entry;
-      if (lane == 0) cand_id[0] = pivot;
-      __syncwarp();
-      warp_dists<Op, 0, 2>(vec4, g.d4, g.dim, q4, cand_id, 1, cand_d);
-      __syncwarp();
-      st.evals += 1;
-      float best = Op::post(cand_d[0]);
-      for (int layer = g.entry_level; layer >= 1; --layer) {
-        int cap;
-        const uint32_t* ids = list_ids(g, pivot, layer, cap);
-        uint32_t new_pivot = pivot;
-        for (int b = 0; b < cap; b += 32) {
-          const uint32_t nid = (b + lane < cap) ? ids[b + lane] : INVALID_ID;
-          const unsigned valid = __ballot_sync(FULL, nid != INVALID_ID);
-          const int cnt = __popc(valid);
-          if (cnt) {
-            __syncwarp();
-            if (lane < cnt) cand_id[lane] = nid;
-            __syncwarp();
-            warp_dists<Op, 0, 2>(vec4, g.d4, g.dim, q4, cand_id, cnt, cand_d);
-            __syncwarp();
-            st.evals += cnt;
-            st.adj += cnt;
-            uint64_t key = lane < cnt ? (((uint64_t)__float_as_uint(Op::post(cand_d[lane])) << 32) | (uint32_t)lane) : ~0ull;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-              const uint64_t other = __shfl_xor_sync(FULL, key, o);
-              key = other < key ? other : key;
-            }
-            const float dmin = __uint_as_float((uint32_t)(key >> 32));
-            if (dmin < best) {
-              best = dmin;
-              new_pivot = cand_id[(uint32_t)key & 31u];
-            }
-          }
-          if (valid != FULL) break;
-        }
-        pivot = new_pivot;
-      }
+      const WarpSmem s{q4, nullptr, cand_id, cand_d};
+      const Entry e = descend<Op, 0, 2>(g, s, st);
+      const uint32_t pivot = e.pivot;
+      const float best = e.best;
       // ---- search_layer, literally (hnsw.rs:940-1063)
       vis.begin();
       vis.test_and_set(pivot, lane == 0);  // 955-956
       st.evals += 1;                       // 952: dist(q, ep), the value is `best`
-      int wn = 0, cn = 0;
+      int wn = 0;
       if (lane == 0) {
         C.push(SItem{-best, pivot});  // 960-963
         W.push(SItem{best, pivot});   // 964-967
         wn = W.n;
-        cn = C.n;
       }
       for (;;) {
         uint32_t c = INVALID_ID;
@@ -243,7 +207,6 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_std_kernel(SearchParams
         wn = W.n;
       }
       wn = __shfl_sync(FULL, wn, 0);
-      (void)cn;
       __syncwarp();
       count = min(p.k, min(ef, wn));  // 1547
     }
@@ -272,18 +235,10 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_std_kernel(SearchParams
 }
 
 cudaError_t launch_search_std(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st,
-                              bool query_only, int* blocks_per_sm) {
+                              int* blocks_per_sm) {
   return dispatch_op(metric, dtype, [&](auto tag) -> cudaError_t {
     using Op = typename decltype(tag)::type;
-    auto kern = search_std_kernel<Op>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    if (blocks_per_sm) {
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, kern, p.threads, smem);
-      if (e != cudaSuccess) return e;
-    }
-    if (!query_only) kern<<<grid, p.threads, smem, st>>>(p);
-    return cudaGetLastError();
+    return launch_kernel(search_std_kernel<Op>, p, grid, p.threads, smem, st, blocks_per_sm);
   });
 }
 

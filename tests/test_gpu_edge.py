@@ -168,6 +168,13 @@ def test_failed_insert_leaves_a_consistent_index(pkg):
     assert bad.get_nb_point() == 0                       # nothing of the refused call is counted
     o, d, it, _, c = bad.search_flat(X[:4], 2, 8)
     assert np.all(c == 0)
+    # 128-byte rows and a small ef, but no entry point: the generic kernel with a row length read at run time answers
+    bad32 = pkg.Hnsw(16, 1000, 16, 200000, "DistL2")
+    X32 = pkg.datagen.uniform(50, 32, 1)
+    with pytest.raises(pkg.HnswError):
+        bad32.insert_flat(X32)
+    o, d, it, _, c = bad32.search_flat(X32[:4], 2, 8)
+    assert np.all(c == 0)
     # the healthy handle is unaffected, and a refused dimension mismatch changes nothing either
     with pytest.raises(pkg.HnswError):
         h.insert_flat(pkg.datagen.uniform(5, 17, 2))

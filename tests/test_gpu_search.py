@@ -33,6 +33,7 @@ CASES = [
     (1500, 784, 32, 100, "DistL2", "uniform", 10, 200),    # MNIST shape: wide rows, generic-d kernel
     (2000, 10, 32, 128, "DistL1", "uniform", 16, 1024),    # tests/equality.rs shape: k=16, ef=1024
     (2000, 70, 8, 60, "DistL2", "uniform", 5, 5),          # d_pad=96 (generic path), ef == k
+    (3000, 32, 16, 100, "DistL2", "clustered", 10, 200),   # 128-byte rows, ef 129-256: generic kernel, 256-slot queue
 ]
 
 
