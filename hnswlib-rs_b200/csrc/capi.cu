@@ -405,6 +405,21 @@ void init_rust_log(void) {}
 // ------------------------------------------------------------------ extensions
 const char* hnsw_b200_last_error(void) { return g_err.c_str(); }
 
+int hnsw_b200_last_kernel(char* buf, size_t cap) {
+  if (buf && cap) buf[0] = '\0';
+  if (!hb::last_launched_kernel) return 0;
+  const char* name = nullptr;
+  cudaError_t e = cudaFuncGetName(&name, hb::last_launched_kernel);
+  if (e != cudaSuccess || !name) return set_err(std::string("cudaFuncGetName: ") + cudaGetErrorString(e));
+  const size_t len = strlen(name);
+  if (buf && cap) {
+    const size_t m = len < cap - 1 ? len : cap - 1;
+    memcpy(buf, name, m);
+    buf[m] = '\0';
+  }
+  return (int)len;
+}
+
 int hnsw_b200_device_count(void) {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;

@@ -120,6 +120,10 @@ inline size_t insert_smem_per_warp(int d4, int ef_c, int deg0, int q_smem) {
   return (b + 127) & ~(size_t)127;
 }
 
+// The kernel this host thread last launched through launch_kernel (hnsw_b200_last_kernel reports its name), so that a
+// test can tell which template instantiation served a call.
+inline thread_local const void* last_launched_kernel = nullptr;
+
 // Every launcher below sets the kernel's dynamic shared-memory limit to `smem`, then either launches it (blocks_per_sm ==
 // nullptr) or only reports how many CTAs of `threads` threads fit on one SM.
 template <class P>
@@ -128,6 +132,7 @@ cudaError_t launch_kernel(void (*kern)(P), const P& p, int grid, int threads, si
   if (e != cudaSuccess) return e;
   if (blocks_per_sm) return cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, kern, threads, smem);
   kern<<<grid, threads, smem, st>>>(p);
+  last_launched_kernel = reinterpret_cast<const void*>(kern);
   return cudaGetLastError();
 }
 
@@ -179,14 +184,16 @@ inline bool lean_op_supported(int metric, int dtype) {
   return false;
 }
 
-template <class T, class F>
-cudaError_t dispatch_int(int metric, bool with_jaccard, F&& f) {
+// WITH_JACCARD is a template parameter so that the Jaccard kernels of an element type without DistJaccard (i32) are
+// not compiled at all
+template <class T, bool WITH_JACCARD, class F>
+cudaError_t dispatch_int(int metric, F&& f) {
   switch (metric) {
     case METRIC_L1: return f(OpTag<OpCast<T, OpL1>>{});
     case METRIC_L2: return f(OpTag<OpCast<T, OpL2>>{});
     case METRIC_HAMMING: return f(OpTag<OpHamming<T>>{});
     case METRIC_JACCARD:
-      if (with_jaccard) return f(OpTag<OpJaccard<T>>{});
+      if constexpr (WITH_JACCARD) return f(OpTag<OpJaccard<T>>{});
       break;
   }
   return cudaErrorInvalidValue;
@@ -206,10 +213,10 @@ cudaError_t dispatch_op(int metric, int dtype, F&& f) {
         case METRIC_JENSENSHANNON: return f(OpTag<OpJS>{});
       }
       break;
-    case DT_U8: return dispatch_int<uint8_t>(metric, true, f);
-    case DT_U16: return dispatch_int<uint16_t>(metric, true, f);
-    case DT_U32: return dispatch_int<uint32_t>(metric, true, f);
-    case DT_I32: return dispatch_int<int32_t>(metric, false, f);
+    case DT_U8: return dispatch_int<uint8_t, true>(metric, f);
+    case DT_U16: return dispatch_int<uint16_t, true>(metric, f);
+    case DT_U32: return dispatch_int<uint32_t, true>(metric, f);
+    case DT_I32: return dispatch_int<int32_t, false>(metric, f);
   }
   return cudaErrorInvalidValue;
 }

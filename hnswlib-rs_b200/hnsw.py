@@ -69,6 +69,7 @@ def load_library():
     L.hnsw_b200_new.argtypes = [i32, sz, sz, sz, C.c_char_p, sz, sz]
     L.hnsw_b200_drop.argtypes = [vp]
     L.hnsw_b200_last_error.restype = C.c_char_p
+    L.hnsw_b200_last_kernel.argtypes = [C.c_char_p, sz]
     L.hnsw_b200_device_count.restype = i32
     L.hnsw_b200_set_device.argtypes = [i32]
     L.hnsw_b200_free_neighbourhood.argtypes = [vp]
@@ -123,6 +124,17 @@ def load_library():
 
 def last_error():
     return load_library().hnsw_b200_last_error().decode("utf-8", "replace")
+
+
+def last_kernel():
+    """mangled name of the last kernel this thread launched through the library ("" before the first launch)"""
+    L = load_library()
+    n = L.hnsw_b200_last_kernel(None, 0)
+    if n < 0:
+        raise HnswError(last_error())
+    buf = C.create_string_buffer(n + 1)
+    L.hnsw_b200_last_kernel(buf, n + 1)
+    return buf.value.decode()
 
 
 def _p(a):

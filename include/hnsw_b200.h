@@ -196,6 +196,10 @@ void hnsw_b200_drop(const void* h);
 
 
 const char* hnsw_b200_last_error(void);
+/* Diagnostics: the mangled name of the last kernel the calling thread launched through the library (the query, insert
+ * search, dist_batch and bruteforce kernels; occupancy queries do not count), written NUL-terminated and truncated to
+ * cap bytes.  Returns the full length of the name, 0 when this thread has launched none, -1 on a CUDA error. */
+int hnsw_b200_last_kernel(char* buf, size_t cap);
 int hnsw_b200_device_count(void);
 /* Limits: max_nb_connection <= 256; fewer than 2^31 points; one query (or insert) must fit 220 KB of shared memory:
  * 16 * ceil(dim * sizeof(T) / 128) * 8 bytes for the query (twice that for an insert) plus 8 bytes per ef (ef_construction)
