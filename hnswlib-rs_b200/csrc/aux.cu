@@ -108,81 +108,60 @@ static cudaError_t launch_aux(const AuxParams& p, int metric, int dtype, bool br
   });
 }
 
-#define HB_CUDA(call)                                     \
-  do {                                                    \
-    cudaError_t e__ = (call);                             \
-    if (e__ != cudaSuccess) return cuda_fail(e__, #call); \
-  } while (0)
-
 int Index::dist_batch(const void* queries, size_t nq, int d, const uint32_t* cand, size_t m, float* out) {
   if (nq == 0 || m == 0) return 0;
   if (d != dim) return fail("query length differs from the index dimension");
   for (size_t i = 0; i < nq * m; ++i)
     if (cand[i] >= n) return fail("candidate id out of range");
   HB_CUDA(cudaSetDevice(device));
-  void* dq = nullptr;
-  uint32_t* dc = nullptr;
-  float* dout = nullptr;
-  HB_CUDA(cudaMalloc(&dq, nq * d * es));
-  HB_CUDA(cudaMalloc(&dc, nq * m * 4));
-  HB_CUDA(cudaMalloc(&dout, nq * m * 4));
-  cudaMemcpyAsync(dq, queries, nq * d * es, cudaMemcpyHostToDevice, stream_);
-  cudaMemcpyAsync(dc, cand, nq * m * 4, cudaMemcpyHostToDevice, stream_);
+  DevBuf dq, dc, dout;
+  HB_CUDA(cudaMalloc(&dq.p, nq * d * es));
+  HB_CUDA(cudaMalloc(&dc.p, nq * m * 4));
+  HB_CUDA(cudaMalloc(&dout.p, nq * m * 4));
+  HB_CUDA(cudaMemcpyAsync(dq.p, queries, nq * d * es, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(dc.p, cand, nq * m * 4, cudaMemcpyHostToDevice, stream_));
   AuxParams p{};
   p.g = view();
-  p.queries = dq;
+  p.queries = dq.p;
   p.q_bytes = d * es;
   p.nq = (uint32_t)nq;
-  p.cand = dc;
+  p.cand = (const uint32_t*)dc.p;
   p.m = (uint32_t)m;
-  p.out = dout;
+  p.out = (float*)dout.p;
   p.smem_per_warp = p.g.d4 * 16 + 256;
   const size_t smem = (size_t)p.smem_per_warp * 8;
   const int grid = (int)std::min<size_t>((size_t)sm_count_ * 8, (nq + 7) / 8);
-  cudaError_t e = launch_aux(p, metric, dtype, false, grid, smem, stream_);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out, dout, nq * m * 4, cudaMemcpyDeviceToHost, stream_);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(stream_);
-  cudaFree(dq);
-  cudaFree(dc);
-  cudaFree(dout);
-  if (e != cudaSuccess) return cuda_fail(e, "dist_batch");
+  HB_CUDA(launch_aux(p, metric, dtype, false, grid, smem, stream_));
+  HB_CUDA(cudaMemcpyAsync(out, dout.p, nq * m * 4, cudaMemcpyDeviceToHost, stream_));
+  HB_CUDA(cudaStreamSynchronize(stream_));
   return 0;
 }
 
 int Index::bruteforce(const void* queries, size_t nq, int d, size_t k, uint32_t* out_ids, float* out_dist) {
   if (nq == 0 || k == 0) return 0;
   if (d != dim) return fail("query length differs from the index dimension");
-  HB_CUDA(cudaSetDevice(device));
-  void* dq = nullptr;
-  uint32_t* dids = nullptr;
-  float* dd = nullptr;
-  HB_CUDA(cudaMalloc(&dq, nq * d * es));
-  HB_CUDA(cudaMalloc(&dids, nq * k * 4));
-  HB_CUDA(cudaMalloc(&dd, nq * k * 4));
-  cudaMemcpyAsync(dq, queries, nq * d * es, cudaMemcpyHostToDevice, stream_);
   AuxParams p{};
   p.g = view();
-  p.queries = dq;
   p.q_bytes = d * es;
   p.nq = (uint32_t)nq;
   p.k = (int)k;
-  p.out_ids = dids;
-  p.out_dist = dd;
   p.smem_per_warp = (int)(((size_t)p.g.d4 * 16 + 256 + k * 8 + 15) & ~(size_t)15);
-  const size_t smem = (size_t)p.smem_per_warp * 8;
-  if (smem > 220 * 1024) {
-    cudaFree(dq); cudaFree(dids); cudaFree(dd);
-    return fail("k / dimension too large for the brute-force kernel");
-  }
+  const size_t smem = (size_t)p.smem_per_warp * 8;  // the kernel indexes its 8 warps itself
+  if (smem > SMEM_BUDGET) return fail("k / dimension too large for the brute-force kernel");
+  HB_CUDA(cudaSetDevice(device));
+  DevBuf dq, dids, dd;
+  HB_CUDA(cudaMalloc(&dq.p, nq * d * es));
+  HB_CUDA(cudaMalloc(&dids.p, nq * k * 4));
+  HB_CUDA(cudaMalloc(&dd.p, nq * k * 4));
+  HB_CUDA(cudaMemcpyAsync(dq.p, queries, nq * d * es, cudaMemcpyHostToDevice, stream_));
+  p.queries = dq.p;
+  p.out_ids = (uint32_t*)dids.p;
+  p.out_dist = (float*)dd.p;
   const int grid = (int)std::min<size_t>((size_t)sm_count_ * 4, (nq + 7) / 8);
-  cudaError_t e = launch_aux(p, metric, dtype, true, grid, smem, stream_);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out_ids, dids, nq * k * 4, cudaMemcpyDeviceToHost, stream_);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out_dist, dd, nq * k * 4, cudaMemcpyDeviceToHost, stream_);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(stream_);
-  cudaFree(dq);
-  cudaFree(dids);
-  cudaFree(dd);
-  if (e != cudaSuccess) return cuda_fail(e, "bruteforce");
+  HB_CUDA(launch_aux(p, metric, dtype, true, grid, smem, stream_));
+  HB_CUDA(cudaMemcpyAsync(out_ids, dids.p, nq * k * 4, cudaMemcpyDeviceToHost, stream_));
+  HB_CUDA(cudaMemcpyAsync(out_dist, dd.p, nq * k * 4, cudaMemcpyDeviceToHost, stream_));
+  HB_CUDA(cudaStreamSynchronize(stream_));
   return 0;
 }
 

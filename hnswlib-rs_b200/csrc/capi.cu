@@ -50,17 +50,7 @@ static int pass(Index* ix, int r) {
   std::shared_lock<std::shared_mutex> g__(ix->mu)
 
 static int metric_from_name(const uint8_t* name, size_t len) {
-  std::string s((const char*)name, len);
-  if (s == "DistL1") return hb::METRIC_L1;
-  if (s == "DistL2") return hb::METRIC_L2;
-  if (s == "DistDot") return hb::METRIC_DOT;
-  if (s == "DistCosine") return hb::METRIC_COSINE;
-  if (s == "DistHellinger") return hb::METRIC_HELLINGER;
-  if (s == "DistJeffreys") return hb::METRIC_JEFFREYS;
-  if (s == "DistJensenShannon") return hb::METRIC_JENSENSHANNON;
-  if (s == "DistHamming") return hb::METRIC_HAMMING;
-  if (s == "DistJaccard") return hb::METRIC_JACCARD;
-  return -1;
+  return hb::metric_from_name(std::string((const char*)name, len));
 }
 
 static void* make_index(int dtype, size_t max_nb_conn, size_t ef_const, size_t namelen, const uint8_t* cdistname,

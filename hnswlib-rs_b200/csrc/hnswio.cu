@@ -25,19 +25,14 @@ static const uint32_t MAGICDESCR_4 = 0x002a6779;  // :60
 static const uint32_t MAGICLAYER = 0x000a676f;    // :63
 static const uint32_t MAGICDATAP = 0xa67f0000;    // :65
 
-static const char* metric_type_name(int metric) {
-  switch (metric) {  // std::any::type_name::<D>() of the anndists types; matched on the last `::` segment at load
-    case METRIC_L1: return "anndists::dist::distances::DistL1";
-    case METRIC_L2: return "anndists::dist::distances::DistL2";
-    case METRIC_DOT: return "anndists::dist::distances::DistDot";
-    case METRIC_COSINE: return "anndists::dist::distances::DistCosine";
-    case METRIC_HAMMING: return "anndists::dist::distances::DistHamming";
-    case METRIC_JACCARD: return "anndists::dist::distances::DistJaccard";
-    case METRIC_HELLINGER: return "anndists::dist::distances::DistHellinger";
-    case METRIC_JEFFREYS: return "anndists::dist::distances::DistJeffreys";
-    case METRIC_JENSENSHANNON: return "anndists::dist::distances::DistJensenShannon";
-  }
-  return "?";
+// the anndists distance types, by metric id: the C ABI names them bare, a dump by their full type path
+static const char* const METRIC_NAMES[] = {"DistL1",      "DistL2",        "DistDot",      "DistCosine",       "DistHamming",
+                                           "DistJaccard", "DistHellinger", "DistJeffreys", "DistJensenShannon"};
+static_assert(sizeof(METRIC_NAMES) / sizeof(METRIC_NAMES[0]) == METRIC_JENSENSHANNON + 1, "one name per metric id");
+
+static std::string metric_type_name(int metric) {  // std::any::type_name::<D>()
+  if (metric < 0 || metric > METRIC_JENSENSHANNON) return "?";
+  return std::string("anndists::dist::distances::") + METRIC_NAMES[metric];
 }
 static const char* dtype_type_name(int dt) {
   switch (dt) {
@@ -49,19 +44,14 @@ static const char* dtype_type_name(int dt) {
   }
   return "?";
 }
+int metric_from_name(const std::string& name) {
+  for (int m = 0; m <= METRIC_JENSENSHANNON; ++m)
+    if (name == METRIC_NAMES[m]) return m;
+  return -1;
+}
 int metric_from_type_name(const std::string& full) {
   const size_t p = full.rfind("::");
-  const std::string s = p == std::string::npos ? full : full.substr(p + 2);
-  if (s == "DistL1") return METRIC_L1;
-  if (s == "DistL2") return METRIC_L2;
-  if (s == "DistDot") return METRIC_DOT;
-  if (s == "DistCosine") return METRIC_COSINE;
-  if (s == "DistHamming") return METRIC_HAMMING;
-  if (s == "DistJaccard") return METRIC_JACCARD;
-  if (s == "DistHellinger") return METRIC_HELLINGER;
-  if (s == "DistJeffreys") return METRIC_JEFFREYS;
-  if (s == "DistJensenShannon") return METRIC_JENSENSHANNON;
-  return -1;
+  return metric_from_name(p == std::string::npos ? full : full.substr(p + 2));
 }
 int dtype_from_type_name(const std::string& s) {
   if (s == "f32") return DT_F32;
@@ -117,25 +107,11 @@ int Index::file_dump(const std::string& dir, const std::string& basename_default
     }
   }
   // ---- gather the graph on the host
-  std::vector<std::vector<uint64_t>> off(MAX_LAYERS);
-  std::vector<std::vector<uint32_t>> ids(MAX_LAYERS);
-  std::vector<std::vector<float>> ds(MAX_LAYERS);
-  int top = 0;
-  for (size_t p = 0; p < n; ++p) top = std::max<int>(top, h_plevel[p]);
-  for (int l = 0; l <= top && l < MAX_LAYERS; ++l) {
-    int64_t total = 0;
-    int r;
-    if ((r = export_layer(l, nullptr, nullptr, nullptr, &total))) return r;
-    off[l].resize(n + 1);
-    ids[l].resize((size_t)total);
-    ds[l].resize((size_t)total);
-    if ((r = export_layer(l, off[l].data(), ids[l].data(), ds[l].data(), nullptr))) return r;
-  }
+  std::vector<LayerCsr> layers;
+  int r;
+  if ((r = export_layers(0, top_layer(), layers))) return r;
   std::vector<unsigned char> vecs(n * (size_t)dim * es);
-  {
-    int r;
-    if ((r = export_vectors(vecs.data()))) return r;
-  }
+  if ((r = export_vectors(vecs.data()))) return r;
   std::vector<std::vector<uint32_t>> by_level(MAX_LAYERS);  // points_by_layer: rank order == insertion order
   for (size_t p = 0; p < n; ++p) by_level[h_level[p]].push_back((uint32_t)p);
 
@@ -176,17 +152,17 @@ int Index::file_dump(const std::string& dir, const std::string& basename_default
       g.put<int32_t>(h_rank[p]);
       for (int l = 0; l < MAX_LAYERS; ++l) {
         uint64_t b = 0, e = 0;
-        if (l <= top && (l == 0 || l <= h_plevel[p])) {
-          b = off[l][p];
-          e = off[l][p + 1];
+        if (l < (int)layers.size()) {  // above the top layer every list is empty
+          b = layers[l].off[p];
+          e = layers[l].off[p + 1];
         }
         g.put<uint64_t>(e - b);
         for (uint64_t j = b; j < e; ++j) {
-          const uint32_t q = ids[l][j];
+          const uint32_t q = layers[l].ids[j];
           g.put<uint64_t>(h_origin[q]);
           g.put<uint8_t>(h_level[q]);
           g.put<int32_t>(h_rank[q]);
-          g.put<float>(ds[l][j]);
+          g.put<float>(layers[l].dists[j]);
         }
       }
       d.put<uint32_t>(MAGICDATAP);

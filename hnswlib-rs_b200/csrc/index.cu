@@ -10,11 +10,7 @@
 
 namespace hb {
 
-#define HB_CUDA(call)                                   \
-  do {                                                  \
-    cudaError_t e__ = (call);                           \
-    if (e__ != cudaSuccess) return cuda_fail(e__, #call); \
-  } while (0)
+using GS = GraphStore;
 
 static size_t next_pow2(size_t x) {
   size_t p = 1;
@@ -97,8 +93,7 @@ Index::~Index() {
   nccl_destroy();
   cudaSetDevice(device);
   if (stream_) cudaStreamSynchronize(stream_);
-  cudaFree(d_vec_.p); cudaFree(d_adj0_.p); cudaFree(d_adjU_.p); cudaFree(d_upoff_.p); cudaFree(d_adj0d_.p);
-  cudaFree(d_adjUd_.p); cudaFree(d_level_.p); cudaFree(d_plevel_.p); cudaFree(d_origin_.p); cudaFree(d_locks_.p);
+  for (void* a : graph_.p) cudaFree(a);
   cudaFree(vis_.tab); cudaFree(vis_.epoch); cudaFree(d_counter_); cudaFree(d_status_); cudaFree(d_stats_); cudaFree(d_mask_);
   if (h_pin_) cudaFreeHost(h_pin_);
   for (SearchCtx& c : ctx_) {
@@ -116,17 +111,23 @@ Index::~Index() {
   if (own_stream_) cudaStreamDestroy(own_stream_);
 }
 
-template <class T>
-int Index::grow(DevArray<T>& a, size_t need, size_t keep, int fill) {
-  if (need <= a.cap) return 0;
-  T* np = nullptr;
-  HB_CUDA(cudaMalloc(&np, need * sizeof(T)));
-  HB_CUDA(cudaMemsetAsync(np, fill, need * sizeof(T), stream_));
-  if (keep && a.p) HB_CUDA(cudaMemcpyAsync(np, a.p, keep * sizeof(T), cudaMemcpyDeviceToDevice, stream_));
-  HB_CUDA(cudaStreamSynchronize(stream_));
-  cudaFree(a.p);
-  a.p = np;
-  a.cap = need;
+size_t Index::row_size(int a) const {
+  const size_t elems[] = {(size_t)row_bytes, (size_t)2 * M, 1, (size_t)M};  // by GraphStore::Row
+  return elems[GS::DESC[a].row] * GS::DESC[a].elem;
+}
+
+// reallocates every array that grows per upper-layer list (per_list) or per point to `cap` rows, keeping the first `keep`
+int Index::grow_store(bool per_list, size_t cap, size_t keep) {
+  for (int a = 0; a < GS::COUNT; ++a) {
+    if ((GS::DESC[a].row == GS::LISTU) != per_list) continue;
+    const size_t row = row_size(a);
+    DevBuf grown;
+    HB_CUDA(cudaMalloc(&grown.p, cap * row));
+    HB_CUDA(cudaMemsetAsync(grown.p, GS::DESC[a].fill, cap * row, stream_));
+    if (keep && graph_.p[a]) HB_CUDA(cudaMemcpyAsync(grown.p, graph_.p[a], keep * row, cudaMemcpyDeviceToDevice, stream_));
+    HB_CUDA(cudaStreamSynchronize(stream_));
+    std::swap(graph_.p[a], grown.p);  // the old array is freed with `grown`
+  }
   return 0;
 }
 
@@ -142,31 +143,22 @@ int Index::set_dim(int d) {
 }
 
 int Index::ensure_points(size_t need) {
-  if (need <= cap_) return 0;
+  if (need <= graph_.cap) return 0;
   if (need >= (size_t)1 << 31) return fail("more than 2^31 points are not supported");
-  size_t nc = std::max(need, cap_ * 2);
-  if (cap_ == 0) nc = std::max(nc, std::max<size_t>(max_elements, 1024));
-  const size_t deg0 = (size_t)2 * M;
+  size_t nc = std::max(need, graph_.cap * 2);
+  if (graph_.cap == 0) nc = std::max(nc, std::max<size_t>(max_elements, 1024));
   int r;
-  if ((r = grow(d_vec_, nc * (size_t)row_bytes, n * (size_t)row_bytes, 0))) return r;
-  if ((r = grow(d_adj0_, nc * deg0, n * deg0, 0xFF))) return r;
-  if ((r = grow(d_adj0d_, nc * deg0, n * deg0, 0))) return r;
-  if ((r = grow(d_upoff_, nc, n, 0xFF))) return r;
-  if ((r = grow(d_level_, nc, n, 0))) return r;
-  if ((r = grow(d_plevel_, nc, n, 0))) return r;
-  if ((r = grow(d_origin_, nc, n, 0))) return r;
-  if ((r = grow(d_locks_, nc, n, 0))) return r;
-  cap_ = nc;
+  if ((r = grow_store(false, nc, n))) return r;
+  graph_.cap = nc;
   return 0;
 }
 
 int Index::ensure_upper(size_t need) {
-  if (need <= cap_ul_) return 0;
-  size_t nc = std::max(need, std::max<size_t>(cap_ul_ * 2, 1024));
+  if (need <= graph_.cap_ul) return 0;
+  size_t nc = std::max(need, std::max<size_t>(graph_.cap_ul * 2, 1024));
   int r;
-  if ((r = grow(d_adjU_, nc * M, n_ul * M, 0xFF))) return r;
-  if ((r = grow(d_adjUd_, nc * M, n_ul * M, 0))) return r;
-  cap_ul_ = nc;
+  if ((r = grow_store(true, nc, n_ul))) return r;
+  graph_.cap_ul = nc;
   return 0;
 }
 
@@ -196,7 +188,7 @@ int Index::ensure_visited(VisitedPool& v, size_t slots, size_t cap_entries, cuda
 }
 
 int Index::fill_visited_cfg(VisitedPool& v, VisitedCfg& c, cudaStream_t st) {
-  const int id_bits = std::max(1, ilog2(std::max<size_t>(cap_, 2)));
+  const int id_bits = std::max(1, ilog2(std::max<size_t>(graph_.cap, 2)));
   if (id_bits != v.id_bits) {  // entries are (epoch << id_bits) | id: a new split invalidates every table
     HB_CUDA(cudaMemsetAsync(v.epoch, 0xFF, v.slots * sizeof(uint32_t), st));
     v.id_bits = id_bits;
@@ -221,21 +213,32 @@ int Index::ensure_scratch(void** p, size_t* cur, size_t need, cudaStream_t st) {
   return 0;
 }
 
+// the same for a pinned host buffer, allocated with cudaHostAlloc `flags`
+int Index::ensure_pinned(void** p, size_t* cur, size_t need, unsigned int flags) {
+  if (need <= *cur) return 0;
+  if (*p) cudaFreeHost(*p);
+  *p = nullptr;
+  *cur = 0;
+  HB_CUDA(cudaHostAlloc(p, need, flags));
+  *cur = need;
+  return 0;
+}
+
 GraphView Index::view() const {
   GraphView g;
-  g.vec = d_vec_.p;
+  g.vec = graph_.p[GS::VEC];
   g.d4 = row_bytes / 16;
   g.dim = dim;
-  g.adj0 = d_adj0_.p;
-  g.adj0_d = d_adj0d_.p;
+  g.adj0 = graph_.at<uint32_t>(GS::ADJ0);
+  g.adj0_d = graph_.at<float>(GS::ADJ0_D);
   g.deg0 = 2 * M;
-  g.adjU = d_adjU_.p;
-  g.adjU_d = d_adjUd_.p;
+  g.adjU = graph_.at<uint32_t>(GS::ADJU);
+  g.adjU_d = graph_.at<float>(GS::ADJU_D);
   g.M = M;
-  g.up_off = d_upoff_.p;
-  g.plevel = d_plevel_.p;
-  g.level = d_level_.p;
-  g.origin = d_origin_.p;
+  g.up_off = graph_.at<uint32_t>(GS::UP_OFF);
+  g.plevel = graph_.at<uint8_t>(GS::PLEVEL);
+  g.level = graph_.at<uint8_t>(GS::LEVEL);
+  g.origin = graph_.at<uint64_t>(GS::ORIGIN);
   g.n = (uint32_t)n;
   g.entry = entry;
   g.entry_level = entry_level;
@@ -261,25 +264,47 @@ int Index::grow_plevel(uint32_t id, int new_pl) {
   if ((r = ensure_upper(n_ul + new_pl))) return r;
   if (old > 0) {
     const size_t src = (size_t)h_upoff[id] * M, dst = n_ul * M, cnt = (size_t)old * M;
-    HB_CUDA(cudaMemcpyAsync(d_adjU_.p + dst, d_adjU_.p + src, cnt * 4, cudaMemcpyDeviceToDevice, stream_));
-    HB_CUDA(cudaMemcpyAsync(d_adjUd_.p + dst, d_adjUd_.p + src, cnt * 4, cudaMemcpyDeviceToDevice, stream_));
+    uint32_t* adjU = graph_.at<uint32_t>(GS::ADJU);
+    float* adjU_d = graph_.at<float>(GS::ADJU_D);
+    HB_CUDA(cudaMemcpyAsync(adjU + dst, adjU + src, cnt * 4, cudaMemcpyDeviceToDevice, stream_));
+    HB_CUDA(cudaMemcpyAsync(adjU_d + dst, adjU_d + src, cnt * 4, cudaMemcpyDeviceToDevice, stream_));
   }
   h_upoff[id] = (uint32_t)n_ul;
   h_plevel[id] = (uint8_t)new_pl;
   n_ul += new_pl;
-  HB_CUDA(cudaMemcpyAsync(d_upoff_.p + id, &h_upoff[id], 4, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(d_plevel_.p + id, &h_plevel[id], 1, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.at<uint32_t>(GS::UP_OFF) + id, &h_upoff[id], 4, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.at<uint8_t>(GS::PLEVEL) + id, &h_plevel[id], 1, cudaMemcpyHostToDevice, stream_));
   HB_CUDA(cudaStreamSynchronize(stream_));
   return 0;
 }
 
-// shared-memory footprint of the insert kernel for this (dimension, ef_construction, M): checked before an insert
-// changes any state
+// Launch shape for a kernel built for up to `max_warps` warps per CTA: fewer warps when one warp's share of shared
+// memory is large (wide rows, big ef).  warps == 0: a single warp does not fit.
+struct CtaShape {
+  int warps;
+  size_t smem;
+};
+static CtaShape cta_shape(size_t smem_per_warp, int max_warps) {
+  int w = max_warps;
+  while (w > 1 && smem_per_warp * w > SMEM_BUDGET) w >>= 1;
+  if (smem_per_warp * w > SMEM_BUDGET) return {0, 0};
+  return {w, smem_per_warp * w};
+}
+
+// the insert kernel's queue (it is built for the 128 / 256-slot queues and the generic one only) and shared memory
+Index::InsertShape Index::insert_shape() const {
+  InsertShape s;
+  s.q_kind = queue_kind(ef_c, metric, dtype);
+  if (s.q_kind != 0 && s.q_kind < 104) s.q_kind = 104;
+  s.q_smem = queue_slots(s.q_kind, ef_c);
+  s.smem_per_warp = insert_smem_per_warp(row_bytes / 16, ef_c, 2 * M, s.q_smem);
+  return s;
+}
+
+// checked before an insert changes any state
 int Index::check_insert_fit() {
-  int qk = queue_kind(ef_c, metric, dtype);
-  if (qk != 0 && qk < 104) qk = 104;
-  const size_t spw = insert_smem_per_warp(row_bytes / 16, ef_c, 2 * M, queue_slots(qk, ef_c));
-  if (spw > 220 * 1024)
+  const size_t spw = insert_shape().smem_per_warp;
+  if (spw > SMEM_BUDGET)
     return fail("ef_construction / dimension too large: one insert needs " + std::to_string(spw) + " bytes of shared memory (limit 220 KB)");
   return 0;
 }
@@ -287,17 +312,33 @@ int Index::check_insert_fit() {
 // forget the points [keep, n): they were stored but never linked (a failed insert call)
 void Index::rollback_points(size_t keep) {
   n = keep;
-  h_level.resize(keep);
-  h_plevel.resize(keep);
-  h_rank.resize(keep);
-  h_origin.resize(keep);
-  h_upoff.resize(keep);
-  for (int l = 0; l < MAX_LAYERS; ++l) layer_count[l] = 0;
+  resize_points(keep);
+  rank_points();
   n_ul = 0;
-  for (size_t p = 0; p < keep; ++p) {
-    layer_count[h_level[p]]++;
+  for (size_t p = 0; p < keep; ++p)
     if (h_plevel[p] > 0) n_ul = std::max<size_t>(n_ul, (size_t)h_upoff[p] + h_plevel[p]);
-  }
+}
+
+void Index::resize_points(size_t count) {
+  h_level.resize(count);
+  h_plevel.resize(count);
+  h_rank.resize(count);
+  h_origin.resize(count);
+  h_upoff.resize(count);
+}
+
+// a point's rank is its position among the points of its level (PointId), in internal-id order
+void Index::rank_points() {
+  for (int l = 0; l < MAX_LAYERS; ++l) layer_count[l] = 0;
+  for (size_t p = 0; p < h_level.size(); ++p) h_rank[p] = (int32_t)layer_count[h_level[p]]++;
+}
+
+int Index::upload_points(size_t first, size_t count) {
+  HB_CUDA(cudaMemcpyAsync(graph_.at<uint8_t>(GS::LEVEL) + first, h_level.data() + first, count, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.at<uint8_t>(GS::PLEVEL) + first, h_plevel.data() + first, count, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.at<uint64_t>(GS::ORIGIN) + first, h_origin.data() + first, count * 8, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.at<uint32_t>(GS::UP_OFF) + first, h_upoff.data() + first, count * 4, cudaMemcpyHostToDevice, stream_));
+  return 0;
 }
 
 int Index::run_insert_range(size_t first, size_t count, size_t mask_off) {
@@ -310,18 +351,17 @@ int Index::run_insert_range(size_t first, size_t count, size_t mask_off) {
   p.keep_pruned = keep_pruned ? 1 : 0;
   p.extend = extend_candidates ? 1 : 0;
   p.work_counter = d_counter_;
-  p.locks = d_locks_.p;
+  p.locks = graph_.at<int>(GS::LOCKS);
   p.stats = stats_on_ ? d_stats_ : nullptr;  // insert-path distance evaluations / expansions / adjacency ids read
   p.status = d_status_;
-  p.q_kind = queue_kind(ef_c, metric, dtype);
-  if (p.q_kind != 0 && p.q_kind < 104) p.q_kind = 104;  // the insert kernel is built for 128 / 256-slot queues only
-  p.q_smem = queue_slots(p.q_kind, ef_c);
-  const size_t spw = insert_smem_per_warp(p.g.d4, ef_c, p.g.deg0, p.q_smem);
-  p.smem_per_warp = (int)spw;
-  int wpb = BUILD_THREADS / 32;
-  while (wpb > 1 && spw * wpb > 220 * 1024) wpb >>= 1;  // fewer inserts per CTA when one warp's share is large
-  const size_t smem = spw * wpb;
-  if (smem > 220 * 1024) return fail("ef_construction / dimension too large for the insert kernel's shared memory");
+  const InsertShape s = insert_shape();
+  p.q_kind = s.q_kind;
+  p.q_smem = s.q_smem;
+  p.smem_per_warp = (int)s.smem_per_warp;
+  const CtaShape cta = cta_shape(s.smem_per_warp, BUILD_THREADS / 32);
+  if (!cta.warps) return fail("ef_construction / dimension too large for the insert kernel's shared memory");
+  const int wpb = cta.warps;
+  const size_t smem = cta.smem;
   p.threads = wpb * 32;
   int bps = 0;
   HB_CUDA(launch_insert_search(p, metric, dtype, 0, smem, stream_, &bps));
@@ -370,11 +410,7 @@ int Index::insert_batch(const void* vecs, size_t n_new, size_t stride, const voi
   if ((r = ensure_points(n + n_new))) return r;
   if ((r = ensure_upper(n_ul + need_ul + 2 * MAX_LAYERS))) return r;
   const size_t first = n;
-  h_level.resize(first + n_new);
-  h_plevel.resize(first + n_new);
-  h_rank.resize(first + n_new);
-  h_origin.resize(first + n_new);
-  h_upoff.resize(first + n_new);
+  resize_points(first + n_new);
   std::vector<uint16_t> masks(n_new);
   for (size_t i = 0; i < n_new; ++i) {
     const size_t id = first + i;
@@ -398,29 +434,20 @@ int Index::insert_batch(const void* vecs, size_t n_new, size_t stride, const voi
   if (rows) {
     const size_t rb = (size_t)dim * es;  // bytes of one user row
     const size_t chunk = std::max<size_t>(1, (size_t)(8u << 20) / rb);
-    if (h_pin_bytes_ < chunk * rb) {
-      if (h_pin_) cudaFreeHost(h_pin_);
-      h_pin_ = nullptr;
-      h_pin_bytes_ = 0;
-      HB_CUDA(cudaMallocHost(&h_pin_, chunk * rb));
-      h_pin_bytes_ = chunk * rb;
-    }
+    if ((r = ensure_pinned(&h_pin_, &h_pin_bytes_, chunk * rb, cudaHostAllocDefault))) return r;
     for (size_t b = 0; b < n_new; b += chunk) {
       const size_t c = std::min(chunk, n_new - b);
       unsigned char* st = (unsigned char*)h_pin_;
       for (size_t i = 0; i < c; ++i) memcpy(st + i * rb, rows[b + i], rb);
-      HB_CUDA(cudaMemcpy2DAsync(d_vec_.p + (first + b) * (size_t)row_bytes, (size_t)row_bytes, st, rb, rb, c,
+      HB_CUDA(cudaMemcpy2DAsync(graph_.at<unsigned char>(GS::VEC) + (first + b) * (size_t)row_bytes, (size_t)row_bytes, st, rb, rb, c,
                                 cudaMemcpyHostToDevice, stream_));
       HB_CUDA(cudaStreamSynchronize(stream_));
     }
   } else {
-    HB_CUDA(cudaMemcpy2DAsync(d_vec_.p + first * (size_t)row_bytes, (size_t)row_bytes, vecs, stride * es, (size_t)dim * es, n_new,
-                              cudaMemcpyHostToDevice, stream_));
+    HB_CUDA(cudaMemcpy2DAsync(graph_.at<unsigned char>(GS::VEC) + first * (size_t)row_bytes, (size_t)row_bytes, vecs, stride * es,
+                              (size_t)dim * es, n_new, cudaMemcpyHostToDevice, stream_));
   }
-  HB_CUDA(cudaMemcpyAsync(d_level_.p + first, h_level.data() + first, n_new, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(d_plevel_.p + first, h_plevel.data() + first, n_new, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(d_origin_.p + first, h_origin.data() + first, n_new * 8, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(d_upoff_.p + first, h_upoff.data() + first, n_new * 4, cudaMemcpyHostToDevice, stream_));
+  if ((r = upload_points(first, n_new))) return r;
   if ((r = ensure_scratch(&d_mask_, &d_mask_bytes_, n_new * 2, stream_))) return r;
   HB_CUDA(cudaMemcpyAsync(d_mask_, masks.data(), n_new * 2, cudaMemcpyHostToDevice, stream_));
   n = first + n_new;  // stored; points become reachable as their batch links them
@@ -512,16 +539,13 @@ int Index::import_graph(const void* vecs, size_t n_new, int d, const uint64_t* o
   for (size_t p = 0; p < n_new; ++p) need_ul += pl[p];
   if ((r = ensure_points(n_new))) return r;
   if ((r = ensure_upper(need_ul + 2 * MAX_LAYERS))) return r;
-  const size_t deg0 = (size_t)2 * M;
-  h_level.assign(levels, levels + n_new);
+  resize_points(n_new);
+  std::copy(levels, levels + n_new, h_level.begin());
   h_plevel = pl;
-  h_rank.resize(n_new);
-  h_origin.assign(origin, origin + n_new);
-  h_upoff.resize(n_new);
-  for (int l = 0; l < MAX_LAYERS; ++l) layer_count[l] = 0;
+  std::copy(origin, origin + n_new, h_origin.begin());
+  rank_points();
   n_ul = 0;
   for (size_t p = 0; p < n_new; ++p) {
-    h_rank[p] = (int32_t)layer_count[levels[p]]++;
     if (pl[p] > 0) {
       h_upoff[p] = (uint32_t)n_ul;
       n_ul += pl[p];
@@ -529,38 +553,32 @@ int Index::import_graph(const void* vecs, size_t n_new, int d, const uint64_t* o
       h_upoff[p] = INVALID_ID;
     }
   }
+  const size_t deg0 = (size_t)2 * M;
   std::vector<uint32_t> a0(n_new * deg0, INVALID_ID), aU(std::max<size_t>(n_ul, 1) * M, INVALID_ID);
   std::vector<float> a0d(n_new * deg0, 0.f), aUd(std::max<size_t>(n_ul, 1) * M, 0.f);
-  for (size_t p = 0; p < n_new; ++p) {
-    if (nlayers > 0) {
-      uint64_t b = offsets[0][p], e = offsets[0][p + 1];
-      if (e - b > deg0) return fail("layer-0 list longer than 2*max_nb_connection");
+  for (size_t p = 0; p < n_new; ++p)
+    for (int l = 0; l < nlayers; ++l) {
+      const ListRef li = list_of(p, l);
+      if (li.cap == 0) continue;  // p is not present at layer l
+      const uint64_t b = offsets[l][p], e = offsets[l][p + 1];
+      if (e - b > li.cap)
+        return fail(l == 0 ? "layer-0 list longer than 2*max_nb_connection" : "upper-layer list longer than max_nb_connection");
+      uint32_t* a = (l == 0 ? a0 : aU).data() + li.at;
+      float* ad = (l == 0 ? a0d : aUd).data() + li.at;
       for (uint64_t j = b; j < e; ++j) {
-        a0[p * deg0 + (j - b)] = ids[0][j];
-        if (dists && dists[0]) a0d[p * deg0 + (j - b)] = dists[0][j];
+        a[j - b] = ids[l][j];
+        if (dists && dists[l]) ad[j - b] = dists[l][j];
       }
     }
-    for (int l = 1; l <= pl[p] && l < nlayers; ++l) {
-      uint64_t b = offsets[l][p], e = offsets[l][p + 1];
-      if (e - b > (uint64_t)M) return fail("upper-layer list longer than max_nb_connection");
-      const size_t li = (size_t)h_upoff[p] + (l - 1);
-      for (uint64_t j = b; j < e; ++j) {
-        aU[li * M + (j - b)] = ids[l][j];
-        if (dists && dists[l]) aUd[li * M + (j - b)] = dists[l][j];
-      }
-    }
-  }
-  HB_CUDA(cudaMemcpy2DAsync(d_vec_.p, (size_t)row_bytes, vecs, (size_t)dim * es, (size_t)dim * es, n_new, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(d_adj0_.p, a0.data(), a0.size() * 4, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(d_adj0d_.p, a0d.data(), a0d.size() * 4, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpy2DAsync(graph_.p[GS::VEC], (size_t)row_bytes, vecs, (size_t)dim * es, (size_t)dim * es, n_new,
+                            cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.p[GS::ADJ0], a0.data(), a0.size() * 4, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.p[GS::ADJ0_D], a0d.data(), a0d.size() * 4, cudaMemcpyHostToDevice, stream_));
   if (n_ul) {
-    HB_CUDA(cudaMemcpyAsync(d_adjU_.p, aU.data(), n_ul * M * 4, cudaMemcpyHostToDevice, stream_));
-    HB_CUDA(cudaMemcpyAsync(d_adjUd_.p, aUd.data(), n_ul * M * 4, cudaMemcpyHostToDevice, stream_));
+    HB_CUDA(cudaMemcpyAsync(graph_.p[GS::ADJU], aU.data(), n_ul * M * 4, cudaMemcpyHostToDevice, stream_));
+    HB_CUDA(cudaMemcpyAsync(graph_.p[GS::ADJU_D], aUd.data(), n_ul * M * 4, cudaMemcpyHostToDevice, stream_));
   }
-  HB_CUDA(cudaMemcpyAsync(d_level_.p, h_level.data(), n_new, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(d_plevel_.p, h_plevel.data(), n_new, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(d_origin_.p, h_origin.data(), n_new * 8, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(d_upoff_.p, h_upoff.data(), n_new * 4, cudaMemcpyHostToDevice, stream_));
+  if ((r = upload_points(0, n_new))) return r;
   HB_CUDA(cudaStreamSynchronize(stream_));
   n = n_new;
   if (entry_id >= 0 && (size_t)entry_id < n_new) {
@@ -674,13 +692,11 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.q_smem = query_queue_slots(kind, p.q_kind, p.ef);
   const size_t spw = query_smem_per_warp(kind, p.g.d4, p.q_smem);
   p.smem_per_warp = (int)spw;
-  // warps per CTA: as many as the kernel is built for, fewer when one warp's share of shared memory is large (wide rows,
-  // big ef); a single warp must fit
-  int wpb = query_threads(kind) / 32;
-  while (wpb > 1 && spw * wpb > 220 * 1024) wpb >>= 1;
-  const size_t smem = spw * wpb;
-  if (smem > 220 * 1024)
+  const CtaShape cta = cta_shape(spw, query_threads(kind) / 32);
+  if (!cta.warps)
     return fail("ef / dimension too large: one query needs " + std::to_string(spw) + " bytes of shared memory (limit 220 KB)");
+  const int wpb = cta.warps;
+  const size_t smem = cta.smem;
   p.threads = wpb * 32;
   p.cbuf = nullptr;
   p.ccap = 0;
@@ -768,13 +784,7 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
   if (dim != 0 && d != dim) return fail("query length differs from the index dimension");
   int r;
   const size_t out_bytes = nq * k * sizeof(NeighbourOut), cnt_bytes = nq * sizeof(int32_t);
-  if (c.h_res_bytes < out_bytes + cnt_bytes + 16) {
-    if (c.h_res) cudaFreeHost(c.h_res);
-    c.h_res = nullptr;
-    c.h_res_bytes = 0;
-    HB_CUDA(cudaHostAlloc(&c.h_res, out_bytes + cnt_bytes + 16, cudaHostAllocMapped | cudaHostAllocPortable));
-    c.h_res_bytes = out_bytes + cnt_bytes + 16;
-  }
+  if ((r = ensure_pinned(&c.h_res, &c.h_res_bytes, out_bytes + cnt_bytes + 16, cudaHostAllocMapped | cudaHostAllocPortable))) return r;
   NeighbourOut* hout = (NeighbourOut*)c.h_res;
   int32_t* hcnt = (int32_t*)((char*)c.h_res + out_bytes);
   int32_t* hstatus = hcnt + nq;
@@ -793,13 +803,7 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
   const void* d_queries = rows ? nullptr : device_view_of_host(queries);  // what the kernel reads
   if (!d_queries) {
     // gather into pinned staging (rows: one pointer per query, libext.rs parallel_search_neighbours_<ty>)
-    if (c.h_pin_bytes < qbytes) {
-      if (c.h_pin) cudaFreeHost(c.h_pin);
-      c.h_pin = nullptr;
-      c.h_pin_bytes = 0;
-      HB_CUDA(cudaHostAlloc(&c.h_pin, qbytes, cudaHostAllocMapped | cudaHostAllocPortable));
-      c.h_pin_bytes = qbytes;
-    }
+    if ((r = ensure_pinned(&c.h_pin, &c.h_pin_bytes, qbytes, cudaHostAllocMapped | cudaHostAllocPortable))) return r;
     unsigned char* stage = (unsigned char*)c.h_pin;
     if (rows)
       for (size_t i = 0; i < nq; ++i) memcpy(stage + i * (size_t)dim * es, rows[i], (size_t)dim * es);
@@ -884,69 +888,76 @@ int Index::make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, i
 
 // ------------------------------------------------------------------------------------------------
 // export
+Index::ListRef Index::list_of(size_t p, int layer) const {
+  if (layer == 0) return {p * 2 * M, (size_t)2 * M};
+  if (layer > h_plevel[p]) return {0, 0};
+  return {((size_t)h_upoff[p] + (layer - 1)) * M, (size_t)M};
+}
+
+int Index::top_layer() const {
+  int top = 0;
+  for (size_t p = 0; p < n; ++p) top = std::max<int>(top, h_plevel[p]);
+  return std::min(top, MAX_LAYERS - 1);
+}
+
+// One copy of the adjacency (adj0 if layer 0 is asked for, adjU if a layer above it is) from the device, then the
+// lists of every point at each layer lo..hi, up to the first empty slot.
+int Index::export_layers(int lo, int hi, std::vector<LayerCsr>& out) const {
+  cudaSetDevice(device);
+  std::vector<uint32_t> a0, aU;
+  std::vector<float> a0d, aUd;
+  if (lo == 0 && n) {
+    a0.resize(n * 2 * M);
+    a0d.resize(a0.size());
+    HB_CUDA(cudaMemcpy(a0.data(), graph_.p[GS::ADJ0], a0.size() * 4, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(a0d.data(), graph_.p[GS::ADJ0_D], a0d.size() * 4, cudaMemcpyDeviceToHost));
+  }
+  if (hi > 0 && n_ul) {
+    aU.resize(n_ul * M);
+    aUd.resize(aU.size());
+    HB_CUDA(cudaMemcpy(aU.data(), graph_.p[GS::ADJU], aU.size() * 4, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(aUd.data(), graph_.p[GS::ADJU_D], aUd.size() * 4, cudaMemcpyDeviceToHost));
+  }
+  out.assign(hi - lo + 1, LayerCsr());
+  for (int l = lo; l <= hi; ++l) {
+    LayerCsr& c = out[l - lo];
+    const uint32_t* a = (l == 0 ? a0 : aU).data();
+    const float* ad = (l == 0 ? a0d : aUd).data();
+    c.off.resize(n + 1);
+    for (size_t p = 0; p < n; ++p) {
+      c.off[p] = c.ids.size();
+      const ListRef li = list_of(p, l);
+      for (size_t j = li.at; j < li.at + li.cap && a[j] != INVALID_ID; ++j) {
+        c.ids.push_back(a[j]);
+        c.dists.push_back(ad[j]);
+      }
+    }
+    c.off[n] = c.ids.size();
+  }
+  return 0;
+}
+
 int Index::export_layer(int layer, uint64_t* offsets, uint32_t* ids, float* dists, int64_t* total) const {
   if (layer < 0 || layer >= MAX_LAYERS) return fail("bad layer");
-  cudaSetDevice(device);
-  const size_t deg0 = (size_t)2 * M;
-  std::vector<uint32_t> a;
-  std::vector<float> ad;
-  if (layer == 0) {
-    a.resize(n * deg0);
-    ad.resize(n * deg0);
-    if (n) {
-      HB_CUDA(cudaMemcpy(a.data(), d_adj0_.p, a.size() * 4, cudaMemcpyDeviceToHost));
-      HB_CUDA(cudaMemcpy(ad.data(), d_adj0d_.p, ad.size() * 4, cudaMemcpyDeviceToHost));
-    }
-  } else {
-    a.resize(n_ul * M);
-    ad.resize(n_ul * M);
-    if (n_ul) {
-      HB_CUDA(cudaMemcpy(a.data(), d_adjU_.p, a.size() * 4, cudaMemcpyDeviceToHost));
-      HB_CUDA(cudaMemcpy(ad.data(), d_adjUd_.p, ad.size() * 4, cudaMemcpyDeviceToHost));
-    }
-  }
-  uint64_t o = 0;
-  for (size_t p = 0; p < n; ++p) {
-    if (offsets) offsets[p] = o;
-    const uint32_t* l = nullptr;
-    const float* ld = nullptr;
-    size_t cap = 0;
-    if (layer == 0) {
-      l = a.data() + p * deg0;
-      ld = ad.data() + p * deg0;
-      cap = deg0;
-    } else if (layer <= h_plevel[p]) {
-      const size_t li = (size_t)h_upoff[p] + (layer - 1);
-      l = a.data() + li * M;
-      ld = ad.data() + li * M;
-      cap = M;
-    }
-    for (size_t j = 0; j < cap && l[j] != INVALID_ID; ++j) {
-      if (ids) ids[o] = l[j];
-      if (dists) dists[o] = ld[j];
-      ++o;
-    }
-  }
-  if (offsets) offsets[n] = o;
-  if (total) *total = (int64_t)o;
+  std::vector<LayerCsr> g;
+  int r;
+  if ((r = export_layers(layer, layer, g))) return r;
+  const LayerCsr& c = g[0];
+  if (offsets) memcpy(offsets, c.off.data(), c.off.size() * 8);
+  if (ids) memcpy(ids, c.ids.data(), c.ids.size() * 4);
+  if (dists) memcpy(dists, c.dists.data(), c.dists.size() * 4);
+  if (total) *total = (int64_t)c.ids.size();
   return 0;
 }
 
 int Index::flatten(std::vector<uint64_t>& offsets, std::vector<uint64_t>& nb_origin, std::vector<float>& nb_dist) const {
   std::vector<std::vector<std::pair<float, uint32_t>>> per(n);
-  int top = 0;
-  for (size_t p = 0; p < n; ++p) top = std::max<int>(top, h_plevel[p]);
-  for (int l = 0; l <= top && l < MAX_LAYERS; ++l) {
-    int64_t total = 0;
-    int r;
-    if ((r = export_layer(l, nullptr, nullptr, nullptr, &total))) return r;
-    std::vector<uint64_t> off(n + 1);
-    std::vector<uint32_t> ids((size_t)total);
-    std::vector<float> ds((size_t)total);
-    if ((r = export_layer(l, off.data(), ids.data(), ds.data(), nullptr))) return r;
+  std::vector<LayerCsr> g;
+  int r;
+  if ((r = export_layers(0, top_layer(), g))) return r;
+  for (const LayerCsr& c : g)
     for (size_t p = 0; p < n; ++p)
-      for (uint64_t j = off[p]; j < off[p + 1]; ++j) per[p].emplace_back(ds[j], ids[j]);
-  }
+      for (uint64_t j = c.off[p]; j < c.off[p + 1]; ++j) per[p].emplace_back(c.dists[j], c.ids[j]);
   offsets.assign(n + 1, 0);
   nb_origin.clear();
   nb_dist.clear();
@@ -965,7 +976,7 @@ int Index::flatten(std::vector<uint64_t>& offsets, std::vector<uint64_t>& nb_ori
 int Index::export_vectors(void* out) const {
   if (n == 0) return 0;
   cudaSetDevice(device);
-  HB_CUDA(cudaMemcpy2D(out, (size_t)dim * es, d_vec_.p, (size_t)row_bytes, (size_t)dim * es, n, cudaMemcpyDeviceToHost));
+  HB_CUDA(cudaMemcpy2D(out, (size_t)dim * es, graph_.p[GS::VEC], (size_t)row_bytes, (size_t)dim * es, n, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -1013,7 +1024,7 @@ int Index::get_stats(uint64_t* out4, bool reset) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// replication blobs: 0 vec, 1 adj0, 2 adjU, 3 up_off, 4 plevel, 5 level, 6 origin, 7 adj0_d, 8 adjU_d
+// replication blobs: the arrays of the graph store, in GraphStore::Array order, without the locks
 static const uint64_t BLOB_MAGIC = 0x68623230306e7377ull;
 
 int Index::blob_header(uint64_t* h) const {
@@ -1053,36 +1064,22 @@ int Index::blob_alloc(const uint64_t* h) {
 }
 
 int Index::blob_info(int i, void** p, uint64_t* bytes) const {
-  const size_t deg0 = (size_t)2 * M;
-  switch (i) {
-    case 0: *p = d_vec_.p; *bytes = n * (size_t)row_bytes; return 0;
-    case 1: *p = d_adj0_.p; *bytes = n * deg0 * 4; return 0;
-    case 2: *p = d_adjU_.p; *bytes = n_ul * M * 4; return 0;
-    case 3: *p = d_upoff_.p; *bytes = n * 4; return 0;
-    case 4: *p = d_plevel_.p; *bytes = n; return 0;
-    case 5: *p = d_level_.p; *bytes = n; return 0;
-    case 6: *p = d_origin_.p; *bytes = n * 8; return 0;
-    case 7: *p = d_adj0d_.p; *bytes = n * deg0 * 4; return 0;
-    case 8: *p = d_adjUd_.p; *bytes = n_ul * M * 4; return 0;
-  }
-  return fail("bad blob index");
+  if (i < 0 || i >= GS::BLOBS) return fail("bad blob index");
+  *p = graph_.p[i];
+  *bytes = (GS::DESC[i].row == GS::LISTU ? n_ul : n) * row_size(i);
+  return 0;
 }
 
 int Index::blob_commit() {
   cudaSetDevice(device);
-  h_level.resize(n);
-  h_plevel.resize(n);
-  h_origin.resize(n);
-  h_upoff.resize(n);
-  h_rank.resize(n);
+  resize_points(n);
   if (n) {
-    HB_CUDA(cudaMemcpy(h_level.data(), d_level_.p, n, cudaMemcpyDeviceToHost));
-    HB_CUDA(cudaMemcpy(h_plevel.data(), d_plevel_.p, n, cudaMemcpyDeviceToHost));
-    HB_CUDA(cudaMemcpy(h_origin.data(), d_origin_.p, n * 8, cudaMemcpyDeviceToHost));
-    HB_CUDA(cudaMemcpy(h_upoff.data(), d_upoff_.p, n * 4, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(h_level.data(), graph_.p[GS::LEVEL], n, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(h_plevel.data(), graph_.p[GS::PLEVEL], n, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(h_origin.data(), graph_.p[GS::ORIGIN], n * 8, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(h_upoff.data(), graph_.p[GS::UP_OFF], n * 4, cudaMemcpyDeviceToHost));
   }
-  for (int l = 0; l < MAX_LAYERS; ++l) layer_count[l] = 0;
-  for (size_t p = 0; p < n; ++p) h_rank[p] = (int32_t)layer_count[h_level[p]]++;
+  rank_points();
   return 0;
 }
 

@@ -44,10 +44,49 @@ struct DeviceRestore {
   }
 };
 
-template <class T>
-struct DevArray {  // growable device array, contents preserved on growth
-  T* p = nullptr;
-  size_t cap = 0;
+// in an Index member: a failed CUDA call returns its status (-2) with the message set
+#define HB_CUDA(call)                                     \
+  do {                                                    \
+    cudaError_t e__ = (call);                             \
+    if (e__ != cudaSuccess) return cuda_fail(e__, #call); \
+  } while (0)
+
+struct DevBuf {  // device memory freed on scope exit, so that no early return leaks it
+  void* p = nullptr;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { cudaFree(p); }
+};
+
+// The device arrays that hold the graph.  Replication blob i is array i, in this order (the order is part of the blob
+// protocol between processes); the per-point insert locks come last and are not replicated.
+struct GraphStore {
+  enum Array { VEC, ADJ0, ADJU, UP_OFF, PLEVEL, LEVEL, ORIGIN, ADJ0_D, ADJU_D, LOCKS, COUNT };
+  static constexpr int BLOBS = LOCKS;
+  // elements per point: a vector row (row_bytes), a layer-0 list (2M), one; or per upper-layer list: a list (M)
+  enum Row { VEC_ROW, LIST0, ONE, LISTU };
+  struct Desc {
+    int elem;  // bytes per element
+    Row row;
+    int fill;  // byte new space is filled with
+  };
+  static constexpr Desc DESC[COUNT] = {
+      {1, VEC_ROW, 0},   // VEC: zero padded to whole 128-byte lines
+      {4, LIST0, 0xFF},  // ADJ0: neighbour ids, INVALID_ID = empty slot
+      {4, LISTU, 0xFF},  // ADJU
+      {4, ONE, 0xFF},    // UP_OFF: the point's first upper-layer list, INVALID_ID = none
+      {1, ONE, 0},       // PLEVEL
+      {1, ONE, 0},       // LEVEL
+      {8, ONE, 0},       // ORIGIN
+      {4, LIST0, 0},     // ADJ0_D: neighbour distances
+      {4, LISTU, 0},     // ADJU_D
+      {4, ONE, 0},       // LOCKS
+  };
+  void* p[COUNT] = {};
+  size_t cap = 0, cap_ul = 0;  // points / upper-layer lists allocated
+  template <class T>
+  T* at(Array a) const { return static_cast<T*>(p[a]); }
 };
 
 struct DumpDescription {  // Description, /root/reference/src/hnswio.rs:846-870
@@ -59,7 +98,8 @@ struct DumpDescription {  // Description, /root/reference/src/hnswio.rs:846-870
   long header_bytes = 0;
 };
 int read_description(const std::string& graph_path, DumpDescription& out, std::string& err);
-int metric_from_type_name(const std::string& full);
+int metric_from_name(const std::string& name);       // "DistL2" -> METRIC_L2; -1 if unknown
+int metric_from_type_name(const std::string& full);  // the same on the last `::` segment of a type path
 int dtype_from_type_name(const std::string& s);
 
 class Index {
@@ -131,7 +171,7 @@ class Index {
   // replication blobs
   int blob_header(uint64_t* h16) const;
   int blob_alloc(const uint64_t* h16);
-  int blob_count() const { return 9; }
+  int blob_count() const { return GraphStore::BLOBS; }
   int blob_info(int i, void** p, uint64_t* bytes) const;
   int blob_commit();
 
@@ -224,17 +264,41 @@ class Index {
  private:
   int fail(const std::string& m) const;
   int cuda_fail(cudaError_t e, const char* what) const;
+  // ---- graph store
+  size_t row_size(int a) const;  // bytes of array a per point (per upper-layer list for ADJU, ADJU_D)
+  int grow_store(bool per_list, size_t cap, size_t keep);
   int ensure_points(size_t need);
   int ensure_upper(size_t need_lists);
+  // ---- point ledger: the host mirrors (h_level ... h_upoff) and the per-layer counts
+  void resize_points(size_t count);
+  void rank_points();  // layer_count and h_rank from h_level, in internal-id order
+  int upload_points(size_t first, size_t count);  // level, plevel, origin, up_off of [first, first + count)
+  // ---- graph export
+  struct ListRef {  // a point's list at one layer: adj0 (layer 0) or adjU from element `at`, `cap` slots (0: none)
+    size_t at, cap;
+  };
+  ListRef list_of(size_t p, int layer) const;
+  struct LayerCsr {  // one layer over internal ids: point p's neighbours are ids / dists [off[p], off[p + 1])
+    std::vector<uint64_t> off;
+    std::vector<uint32_t> ids;
+    std::vector<float> dists;
+  };
+  int export_layers(int lo, int hi, std::vector<LayerCsr>& out) const;  // out[l - lo] for layers lo..hi
+  int top_layer() const;  // highest layer any point is present at
+  // ---- insert launch
+  struct InsertShape {
+    int q_kind, q_smem;
+    size_t smem_per_warp;
+  };
+  InsertShape insert_shape() const;
   int ensure_visited(VisitedPool& v, size_t slots, size_t cap_entries, cudaStream_t st);
   int fill_visited_cfg(VisitedPool& v, VisitedCfg& c, cudaStream_t st);
   int ensure_scratch(void** p, size_t* cur, size_t need, cudaStream_t st);
+  int ensure_pinned(void** p, size_t* cur, size_t need, unsigned int flags);
   int grow_plevel(uint32_t id, int new_plevel);
   int run_insert_range(size_t first, size_t count, size_t mask_off);
   int check_insert_fit();
   void rollback_points(size_t keep);
-  template <class T>
-  int grow(DevArray<T>& a, size_t need_elems, size_t keep_elems, int fill_byte);
 
   struct Worker;
   struct WorkerDeleter {
@@ -257,13 +321,7 @@ class Index {
   cudaStream_t stream_ = nullptr, own_stream_ = nullptr;
   int sm_count_ = 0;
 
-  size_t cap_ = 0, cap_ul_ = 0;
-  DevArray<unsigned char> d_vec_;
-  DevArray<uint32_t> d_adj0_, d_adjU_, d_upoff_;
-  DevArray<float> d_adj0d_, d_adjUd_;
-  DevArray<uint8_t> d_level_, d_plevel_;
-  DevArray<uint64_t> d_origin_;
-  DevArray<int> d_locks_;
+  GraphStore graph_;
 
   VisitedPool vis_;  // visited tables of the insert kernel (searches: SearchCtx)
   SearchCtx ctx_[NCTX + NASYNC];

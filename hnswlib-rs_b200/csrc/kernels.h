@@ -14,6 +14,7 @@ inline int dtype_size(int dt) { return dt == DT_U8 ? 1 : dt == DT_U16 ? 2 : 4; }
 constexpr int SEARCH_THREADS = 256;  // 8 warps = 8 queries in flight per CTA
 constexpr int BUILD_THREADS = 128;   // 4 warps = 4 inserts in flight per CTA
 constexpr int LEAN_THREADS = 32;      // lean kernel (search_lean.cuh): one warp per CTA, so that a finished query frees its slot at once
+constexpr size_t SMEM_BUDGET = 220 * 1024;  // dynamic shared memory one CTA may ask for (an H100 SM offers 227 KB)
 #ifndef HB_LEAN_BLOCKS
 #define HB_LEAN_BLOCKS 20
 #endif

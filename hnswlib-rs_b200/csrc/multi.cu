@@ -77,11 +77,6 @@ static NcclApi& nccl() {
     ncclResult_t r__ = (call);                                                                              \
     if (r__ != ncclSuccess) return fail(std::string("NCCL error: ") + nccl().GetErrorString(r__) + " at " #call); \
   } while (0)
-#define HB_CUDA(call)                                     \
-  do {                                                    \
-    cudaError_t e__ = (call);                             \
-    if (e__ != cudaSuccess) return cuda_fail(e__, #call); \
-  } while (0)
 
 // ------------------------------------------------------------------------------------------------ worker threads
 // One per replica: runs the closures the owner hands it, on the replica's device.
@@ -141,7 +136,7 @@ void Index::drop_replicas() {
   replica_devices_.clear();
 }
 
-// broadcast the nine blobs of `this` (communicator rank 0) to the replicas (ranks 1..), then rebuild their host mirrors
+// broadcast the blobs of `this` (communicator rank 0) to the replicas (ranks 1..), then rebuild their host mirrors
 int Index::broadcast_to_replicas() {
   DeviceRestore keep;
   NcclApi& nc = nccl();
@@ -362,12 +357,9 @@ int Index::nccl_broadcast_index(int root) {
   if (!comm_) return fail("nccl_broadcast_index: call hnsw_b200_nccl_init first");
   if (root < 0 || root >= nranks_) return fail("nccl_broadcast_index: bad root");
   HB_CUDA(cudaSetDevice(device));
-  struct DevBuf {  // freed on every return path
-    uint64_t* p = nullptr;
-    ~DevBuf() { cudaFree(p); }
-  } hdr;
+  DevBuf hdr;
   HB_CUDA(cudaMalloc(&hdr.p, 16 * sizeof(uint64_t)));
-  uint64_t* d_hdr = hdr.p;
+  uint64_t* d_hdr = (uint64_t*)hdr.p;
   uint64_t header[16];
   if (rank_ == root) {
     blob_header(header);
