@@ -10,9 +10,11 @@
 
 #include "../../include/hnsw_b200.h"
 #include "index.h"
+#include "partition.h"
 
 using hb::Index;
 using hb::NeighbourOut;
+using hb::AnswerArrays;
 
 // every typed handle of libext.rs (HnswApif32, HnswApii32, HnswApiu32, HnswApiu16, HnswApiu8) has this layout
 struct HnswApif32 { Index* ix; };
@@ -48,6 +50,25 @@ static int pass(Index* ix, int r) {
   if (!(h)) return set_err("NULL handle"); \
   Index* ix = ((const AnyApi*)(h))->ix;    \
   std::shared_lock<std::shared_mutex> g__(ix->mu)
+
+// Partitioned handles (partition.h) and their views.  A view serves read-only calls only; a call the partitioned handle
+// cannot serve is refused before it changes anything.  A partitioned call holds the handle's lock, then every
+// partition's in partition order (HB_PARTS_SHARED for searches, HB_PARTS_EXCLUSIVE for inserts and settings).
+#define HB_NOT_VIEW(ix) \
+  if ((ix)->owner) return set_err("a partition view is read-only")
+#define HB_NOT_PARTITIONED(ix, what) \
+  if ((ix)->parts) return set_err(std::string(what) + " is not available on a partitioned handle")
+#define HB_PARTS_SHARED(ix) const auto pl__ = (ix)->parts->lock_shared()
+#define HB_PARTS_EXCLUSIVE(ix) const auto pl__ = (ix)->parts->lock_exclusive()
+
+// a setting: on a partitioned handle it is applied to the handle and to every partition
+static void apply(Index* ix, const std::function<void(Index*)>& set) {
+  set(ix);
+  if (!ix->parts) return;
+  HB_PARTS_EXCLUSIVE(ix);
+  for (int p = 0; p < ix->parts->count(); ++p) set(ix->parts->part(p));
+}
+static uint64_t nb_point(const Index* ix) { return ix->parts ? ix->parts->nb_point() : ix->n; }
 
 static int metric_from_name(const uint8_t* name, size_t len) {
   return hb::metric_from_name(std::string((const char*)name, len));
@@ -88,10 +109,19 @@ static void insert_any(void* hv, size_t len, const void* data, size_t id) {
     set_err("insert: NULL argument");
     return;
   }
+  if (h->ix->owner) {
+    set_err("insert: a partition view is read-only");
+    return;
+  }
   std::unique_lock<std::shared_mutex> g(h->ix->mu);
   h->ix->drain_pending();
-  if (pass(h->ix, h->ix->set_dim((int)len))) return;
   uint64_t id64 = id;
+  if (h->ix->parts) {
+    HB_PARTS_EXCLUSIVE(h->ix);
+    pass(h->ix, h->ix->parts->insert(data, 1, len, nullptr, &id64, nullptr, (int)len));
+    return;
+  }
+  if (pass(h->ix, h->ix->set_dim((int)len))) return;
   pass(h->ix, h->ix->insert_batch(data, 1, len, nullptr, &id64, nullptr));
 }
 
@@ -101,10 +131,19 @@ static void parallel_insert_any(void* hv, size_t nb_vec, size_t vec_len, const v
     set_err("parallel_insert: NULL argument");
     return;
   }
+  if (h->ix->owner) {
+    set_err("parallel_insert: a partition view is read-only");
+    return;
+  }
   std::unique_lock<std::shared_mutex> g(h->ix->mu);
   h->ix->drain_pending();
-  if (pass(h->ix, h->ix->set_dim((int)vec_len))) return;
   std::vector<uint64_t> id64(ids, ids + nb_vec);
+  if (h->ix->parts) {
+    HB_PARTS_EXCLUSIVE(h->ix);
+    pass(h->ix, h->ix->parts->insert(nullptr, nb_vec, vec_len, datas, id64.data(), nullptr, (int)vec_len));
+    return;
+  }
+  if (pass(h->ix, h->ix->set_dim((int)vec_len))) return;
   pass(h->ix, h->ix->insert_batch(nullptr, nb_vec, vec_len, datas, id64.data(), nullptr));
 }
 
@@ -117,7 +156,17 @@ static const Neighbourhood_api* search_any(const void* hv, size_t len, const voi
   std::shared_lock<std::shared_mutex> g(h->ix->mu);
   Neighbour_api* nb = (Neighbour_api*)malloc(sizeof(Neighbour_api) * knbn);
   int32_t cnt = 0;
-  if (pass(h->ix, h->ix->search_host(data, nullptr, 1, (int)len, knbn, ef_search, nullptr, (NeighbourOut*)nb, &cnt))) {
+  int rc;
+  if (h->ix->parts) {
+    HB_PARTS_SHARED(h->ix);
+    AnswerArrays out;
+    out.nb = (NeighbourOut*)nb;
+    out.counts = &cnt;
+    rc = h->ix->parts->search(data, nullptr, 1, (int)len, knbn, ef_search, 0, nullptr, 0, nullptr, nullptr, out);
+  } else {
+    rc = h->ix->search_host(data, nullptr, 1, (int)len, knbn, ef_search, nullptr, (NeighbourOut*)nb, &cnt);
+  }
+  if (pass(h->ix, rc)) {
     free(nb);
     return nullptr;
   }
@@ -149,7 +198,13 @@ static const Vec_api_Neighbourhood_api* parallel_search_any(const void* hv, size
   box->block = (Neighbour_api*)malloc(sizeof(Neighbour_api) * (nb_vec ? nb_vec * knbn : 1));
   std::vector<int32_t> cnt(nb_vec);
   int rc;
-  if (use_shards(h->ix, nb_vec)) {  // replicas on other GPUs: every device answers its slice of the batch in place
+  if (h->ix->parts) {
+    HB_PARTS_SHARED(h->ix);
+    AnswerArrays out;
+    out.nb = (NeighbourOut*)box->block;
+    out.counts = cnt.data();
+    rc = h->ix->parts->search(nullptr, data, nb_vec, (int)vec_len, knbn, ef_search, 0, nullptr, 0, nullptr, nullptr, out);
+  } else if (use_shards(h->ix, nb_vec)) {  // replicas on other GPUs: every device answers its slice of the batch in place
     NeighbourOut* block = (NeighbourOut*)box->block;
     int32_t* cp = cnt.data();
     rc = h->ix->for_each_shard(nb_vec, [=](Index* rx, size_t first, size_t count) {
@@ -176,6 +231,10 @@ static const Vec_api_Neighbourhood_api* parallel_search_any(const void* hv, size
 static void drop_any(const void* p) {
   const AnyApi* h = (const AnyApi*)p;
   if (!h) return;
+  if (h->ix->owner) {  // a partition view is freed with its partitioned handle
+    set_err("drop: a partition view is not a handle of its own");
+    return;
+  }
   delete h->ix;
   delete h;
 }
@@ -248,6 +307,7 @@ static int64_t file_dump_any(const void* hv, size_t namelen, const uint8_t* file
     set_err("file_dump: NULL argument");
     return -1;
   }
+  HB_NOT_PARTITIONED(h->ix, "file_dump (dump each partition_view)");
   std::shared_lock<std::shared_mutex> g(h->ix->mu);
   std::string used;
   // api.rs:76-78: the reference refuses to overwrite only while a dump is memory-mapped; nothing is mapped here
@@ -345,6 +405,7 @@ void* hnsw_b200_load_dump(HnswIo* io, int dtype, size_t namelen, const uint8_t* 
 int hnsw_b200_file_dump(const void* h, const char* dir, const char* basename, int overwrite, char* used_basename,
                         size_t used_cap) {
   HB_H(h);
+  HB_NOT_PARTITIONED(ix, "file_dump (dump each partition_view)");
   if (!dir || !basename) return set_err("NULL path");
   std::string used;
   int r = pass(ix, ix->file_dump(dir, basename, overwrite != 0, &used));
@@ -440,10 +501,11 @@ void hnsw_b200_free_vec_api(const Vec_api_Neighbourhood_api* p) {
 
 int hnsw_b200_set_extend_candidates(void* h, int flag) {
   HB_H(h);
+  HB_NOT_VIEW(ix);
   if (flag && ix->ef_c <= 2 * ix->M)
     return set_err("extend_candidates needs ef_construction > 2*max_nb_connection in this engine (otherwise the "
                    "extension set of hnsw.rs:1336-1362 is not provably empty)");
-  ix->extend_candidates = flag != 0;
+  apply(ix, [=](Index* x) { x->extend_candidates = flag != 0; });
   return 0;
 }
 int hnsw_b200_get_extend_candidates(const void* h) {
@@ -452,48 +514,87 @@ int hnsw_b200_get_extend_candidates(const void* h) {
 }
 int hnsw_b200_set_keeping_pruned(void* h, int flag) {
   HB_H(h);
-  ix->keep_pruned = flag != 0;
+  HB_NOT_VIEW(ix);
+  apply(ix, [=](Index* x) { x->keep_pruned = flag != 0; });
   return 0;
 }
 int hnsw_b200_modify_level_scale(void* h, double scale) {
   HB_H(h);
-  if (ix->n > 0) return set_err("modify_level_scale: index already holds points (hnsw.rs:881-888)");
+  HB_NOT_VIEW(ix);
+  if (nb_point(ix) > 0) return set_err("modify_level_scale: index already holds points (hnsw.rs:881-888)");
   if (!(scale >= 0.2 && scale <= 1.0)) return set_err("modify_level_scale: factor must be in [0.2, 1]");  // hnsw.rs:889-900
-  ix->level_scale = scale / std::log((double)ix->M);
+  apply(ix, [=](Index* x) { x->level_scale = scale / std::log((double)x->M); });
   return 0;
 }
 int hnsw_b200_set_tie_mode(void* h, int mode) {
   HB_H(h);
+  HB_NOT_VIEW(ix);
   if (mode != 0 && mode != 1) return set_err("tie mode must be 0 (distance, id) or 1 (reference std heaps)");
-  ix->tie_std_ = mode == 1;
+  apply(ix, [=](Index* x) { x->tie_std_ = mode == 1; });
   return 0;
 }
 int hnsw_b200_set_searching_mode(void* h, int flag) {
   HB_H(h);
-  ix->searching = flag != 0;
+  HB_NOT_VIEW(ix);
+  apply(ix, [=](Index* x) { x->searching = flag != 0; });
   return 0;
 }
 int hnsw_b200_set_level_seed(void* h, uint64_t seed) {
   HB_H(h);
-  ix->rng.s = seed;
+  HB_NOT_VIEW(ix);
+  ix->rng.s = seed;  // a partitioned handle draws every level itself, in global insertion order
   return 0;
 }
-uint64_t hnsw_b200_get_nb_point(const void* h) { return h ? ((const AnyApi*)h)->ix->n : 0; }
-int hnsw_b200_get_max_level_observed(const void* h) { return h ? std::max(((const AnyApi*)h)->ix->entry_level, 0) : 0; }
+uint64_t hnsw_b200_get_nb_point(const void* h) { return h ? nb_point(((const AnyApi*)h)->ix) : 0; }
+int hnsw_b200_get_max_level_observed(const void* h) {
+  if (!h) return 0;
+  const Index* ix = ((const AnyApi*)h)->ix;
+  return ix->parts ? ix->parts->max_level() : std::max(ix->entry_level, 0);
+}
 int hnsw_b200_get_dim(const void* h) { return h ? ((const AnyApi*)h)->ix->dim : 0; }
 int hnsw_b200_set_insert_batching(void* h, uint32_t ratio, uint32_t max_batch) {
   HB_H(h);
+  HB_NOT_VIEW(ix);
   if (ratio == 0 || max_batch == 0) return set_err("ratio and max_batch must be positive");
-  ix->batch_ratio = ratio;
-  ix->batch_max = max_batch;
+  apply(ix, [=](Index* x) {
+    x->batch_ratio = ratio;
+    x->batch_max = max_batch;
+  });
   return 0;
+}
+
+int hnsw_b200_partition(void* h, int nparts, const int* devices) {
+  HB_H(h);
+  return pass(ix, hb::Partitions::create(ix, nparts, devices));
+}
+int hnsw_b200_partition_count(const void* h) {
+  if (!h) return set_err("NULL handle");
+  const Index* ix = ((const AnyApi*)h)->ix;
+  return ix->parts ? ix->parts->count() : 1;
+}
+const void* hnsw_b200_partition_view(const void* h, int p) {
+  if (!h) {
+    set_err("NULL handle");
+    return nullptr;
+  }
+  const Index* ix = ((const AnyApi*)h)->ix;
+  if (!ix->parts || p < 0 || p >= ix->parts->count()) {
+    set_err("partition_view: no such partition");
+    return nullptr;
+  }
+  return ix->parts->view_handle(p);
 }
 
 int hnsw_b200_insert_flat(void* h, const void* vecs, uint64_t n, uint64_t dim, const uint64_t* ids,
                           const int32_t* levels) {
   HB_H(h);
+  HB_NOT_VIEW(ix);
   if (n == 0) return 0;
   if (!vecs) return set_err("vecs is NULL");
+  if (ix->parts) {
+    HB_PARTS_EXCLUSIVE(ix);
+    return pass(ix, ix->parts->insert(vecs, n, dim, nullptr, ids, levels, (int)dim));
+  }
   int r;
   if ((r = pass(ix, ix->set_dim((int)dim)))) return r;
   return pass(ix, ix->insert_batch(vecs, n, dim, nullptr, ids, levels));
@@ -509,12 +610,8 @@ static void unpack_answers(const Index* rx, const NeighbourOut* a, const int32_t
   for (uint64_t s = 0; s < tot; ++s) dist[s] = a[s].dist;
   if (internal)
     for (uint64_t s = 0; s < tot; ++s) internal[s] = a[s].internal;
-  if (pid)  // PointId(level, rank), hnsw.rs:46
-    for (uint64_t s = 0; s < tot; ++s) {
-      const uint32_t it = a[s].internal;
-      pid[2 * s] = it != hb::INVALID_ID ? (int32_t)rx->h_level[it] : -1;
-      pid[2 * s + 1] = it != hb::INVALID_ID ? rx->h_rank[it] : -1;
-    }
+  if (pid)
+    for (uint64_t s = 0; s < tot; ++s) hb::point_id(rx, a[s].internal, pid + 2 * s);
 }
 
 int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
@@ -524,6 +621,17 @@ int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint6
   HB_HS(h);
   if (nq == 0) return 0;
   if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0) return set_err("bad argument");
+  if (ix->parts) {  // every query on every partition, the answers merged straight into the caller's arrays
+    HB_PARTS_SHARED(ix);
+    AnswerArrays out;
+    out.ids = out_ids;
+    out.dist = out_dist;
+    out.internal = out_internal;
+    out.pid = out_pid;
+    out.counts = out_counts;
+    return pass(ix, ix->parts->search(queries, nullptr, nq, (int)dim, knbn, ef_search, filter_mode, filter_ids, nfilter, fn,
+                                      ctx, out));
+  }
   std::vector<uint32_t> bits;
   const uint32_t* fb = nullptr;
   if (filter_mode) {
@@ -586,6 +694,7 @@ int64_t hnsw_b200_search_flat_submit(const void* h, const void* queries, uint64_
                                      uint64_t ef_search, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                      int32_t* out_pid, int32_t* out_counts) {
   HB_HS(h);
+  HB_NOT_PARTITIONED(ix, "search_flat_submit");
   if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0 || nq == 0) return set_err("bad argument");
   Index::Ticket t;
   const size_t qrow = (size_t)dim * ix->es;
@@ -635,6 +744,7 @@ int hnsw_b200_search_flat_wait(const void* h, int64_t ticket) {
 int hnsw_b200_search_device(const void* h, const void* d_queries, uint64_t nq, uint64_t knbn,
                             uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
   HB_HS(h);
+  HB_NOT_PARTITIONED(ix, "search_device");
   return pass(ix, ix->search_device(d_queries, nq, knbn, ef_search, nullptr, (NeighbourOut*)d_out, d_counts, sync != 0,
                                     kernel_ms));
 }
@@ -649,6 +759,7 @@ int hnsw_b200_stream_wait_last(void* h, void* cuda_stream) {
 }
 int hnsw_b200_set_stream(void* h, void* cuda_stream) {
   HB_H(h);
+  HB_NOT_VIEW(ix);
   return pass(ix, ix->set_stream((cudaStream_t)cuda_stream));
 }
 int hnsw_b200_check_status(void* h) {
@@ -660,15 +771,22 @@ int hnsw_b200_check_status(void* h) {
 
 int hnsw_b200_enable_stats(void* h, int enable) {
   HB_H(h);
-  return ix->enable_stats(enable != 0);
+  HB_NOT_VIEW(ix);
+  apply(ix, [=](Index* x) { x->enable_stats(enable != 0); });
+  return 0;
 }
 int hnsw_b200_get_stats(const void* h, uint64_t* out4, int reset) {
   HB_H(h);
+  if (ix->parts) {  // the sum over the partitions: out4[3] counts a query once per partition
+    HB_PARTS_EXCLUSIVE(ix);
+    return pass(ix, ix->parts->get_stats(out4, reset != 0));
+  }
   return pass(ix, ix->get_stats(out4, reset != 0));
 }
 
 int hnsw_b200_export_points(const void* h, uint8_t* levels, int32_t* ranks, uint64_t* origin, int64_t* entry) {
   HB_H(h);
+  HB_NOT_PARTITIONED(ix, "export_points (export each partition_view)");
   for (size_t i = 0; i < ix->n; ++i) {
     if (levels) levels[i] = ix->h_level[i];
     if (ranks) ranks[i] = ix->h_rank[i];
@@ -679,6 +797,7 @@ int hnsw_b200_export_points(const void* h, uint8_t* levels, int32_t* ranks, uint
 }
 int hnsw_b200_export_vectors(const void* h, void* out) {
   HB_H(h);
+  HB_NOT_PARTITIONED(ix, "export_vectors (export each partition_view)");
   return pass(ix, ix->export_vectors(out));
 }
 // FlatNeighborhood::from(&hnsw) + get_neighbours(DataId) (flatten.rs:93-126): neighbours of `origin_id` over all
@@ -686,6 +805,7 @@ int hnsw_b200_export_vectors(const void* h, void* out) {
 int64_t hnsw_b200_flat_neighbours(const void* h, uint64_t origin_id, Neighbour_api* out, uint64_t cap) {
   if (!h) return set_err("NULL handle");
   Index* ix = ((const AnyApi*)h)->ix;
+  HB_NOT_PARTITIONED(ix, "flatten (flatten each partition_view)");
   std::shared_lock<std::shared_mutex> g(ix->mu);
   std::vector<uint64_t> off, nbo;
   std::vector<float> nbd;
@@ -704,6 +824,7 @@ int64_t hnsw_b200_flat_neighbours(const void* h, uint64_t origin_id, Neighbour_a
 int64_t hnsw_b200_flatten(const void* h, uint64_t* offsets, uint64_t* nb_origin, float* nb_dist) {
   if (!h) return set_err("NULL handle");
   Index* ix = ((const AnyApi*)h)->ix;
+  HB_NOT_PARTITIONED(ix, "flatten (flatten each partition_view)");
   std::shared_lock<std::shared_mutex> g(ix->mu);
   std::vector<uint64_t> off, nbo;
   std::vector<float> nbd;
@@ -717,6 +838,7 @@ int64_t hnsw_b200_flatten(const void* h, uint64_t* offsets, uint64_t* nb_origin,
 int64_t hnsw_b200_layer_edges(const void* h, int layer) {
   if (!h) return set_err("NULL handle");
   Index* ix = ((const AnyApi*)h)->ix;
+  HB_NOT_PARTITIONED(ix, "layer_edges (export each partition_view)");
   std::shared_lock<std::shared_mutex> g(ix->mu);
   int64_t total = 0;
   if (pass(ix, ix->export_layer(layer, nullptr, nullptr, nullptr, &total))) return -1;
@@ -724,36 +846,51 @@ int64_t hnsw_b200_layer_edges(const void* h, int layer) {
 }
 int hnsw_b200_export_layer(const void* h, int layer, uint64_t* offsets, uint32_t* ids, float* dists) {
   HB_H(h);
+  HB_NOT_PARTITIONED(ix, "export_layer (export each partition_view)");
   return pass(ix, ix->export_layer(layer, offsets, ids, dists, nullptr));
 }
 int hnsw_b200_import_graph(void* h, const void* vecs, uint64_t n, uint64_t dim, const uint64_t* origin,
                            const uint8_t* levels, int64_t entry, int nlayers, const uint64_t* const* offsets,
                            const uint32_t* const* ids, const float* const* dists) {
   HB_H(h);
+  HB_NOT_VIEW(ix);
+  HB_NOT_PARTITIONED(ix, "import_graph");
   return pass(ix, ix->import_graph(vecs, n, (int)dim, origin, levels, entry, nlayers, offsets, ids, dists));
 }
 
 int hnsw_b200_blob_header(const void* h, uint64_t* header16) {
   HB_H(h);
+  HB_NOT_PARTITIONED(ix, "blob_header");
   return ix->blob_header(header16);
 }
 int hnsw_b200_blob_alloc(void* h, const uint64_t* header16) {
   HB_H(h);
+  HB_NOT_VIEW(ix);
+  HB_NOT_PARTITIONED(ix, "blob_alloc");
   return pass(ix, ix->blob_alloc(header16));
 }
-int hnsw_b200_blob_count(const void* h) { return h ? ((const AnyApi*)h)->ix->blob_count() : 0; }
+int hnsw_b200_blob_count(const void* h) {
+  if (!h) return 0;
+  HB_NOT_PARTITIONED(((const AnyApi*)h)->ix, "blob_count");
+  return ((const AnyApi*)h)->ix->blob_count();
+}
 int hnsw_b200_blob_info(const void* h, int i, void** dev_ptr, uint64_t* nbytes) {
   HB_H(h);
+  HB_NOT_PARTITIONED(ix, "blob_info");
   return pass(ix, ix->blob_info(i, dev_ptr, nbytes));
 }
 int hnsw_b200_blob_commit(void* h) {
   HB_H(h);
+  HB_NOT_VIEW(ix);
+  HB_NOT_PARTITIONED(ix, "blob_commit");
   return pass(ix, ix->blob_commit());
 }
 
 // ---- multi-GPU (multi.cu)
 int hnsw_b200_replicate(void* h, int ndev, const int* devices) {
   HB_H(h);
+  HB_NOT_VIEW(ix);
+  HB_NOT_PARTITIONED(ix, "replicate");
   return pass(ix, ix->replicate(ndev, devices));
 }
 int hnsw_b200_replica_count(const void* h) { return h ? (int)((const AnyApi*)h)->ix->replica_count() : 0; }
@@ -763,26 +900,36 @@ int hnsw_b200_nccl_unique_id(uint8_t* id128) {
 }
 int hnsw_b200_nccl_init(void* h, int nranks, int rank, const uint8_t* id128) {
   HB_H(h);
+  HB_NOT_VIEW(ix);
+  HB_NOT_PARTITIONED(ix, "nccl_init");
   if (!id128) return set_err("NULL argument");
   return pass(ix, ix->nccl_init(nranks, rank, id128));
 }
 int hnsw_b200_nccl_broadcast_index(void* h, int root) {
   HB_H(h);
+  HB_NOT_VIEW(ix);
+  HB_NOT_PARTITIONED(ix, "nccl_broadcast_index");
   return pass(ix, ix->nccl_broadcast_index(root));
 }
 int hnsw_b200_nccl_allgather(void* h, const void* d_send, void* d_recv, uint64_t bytes_per_rank, void* cuda_stream) {
   HB_H(h);
+  HB_NOT_PARTITIONED(ix, "nccl_allgather");
   return pass(ix, ix->nccl_allgather(d_send, d_recv, bytes_per_rank, (cudaStream_t)cuda_stream));
 }
 
 int hnsw_b200_dist_batch(const void* h, const void* queries, uint64_t nq, uint64_t dim, const uint32_t* cand,
                          uint64_t m, float* out) {
   HB_H(h);
+  HB_NOT_PARTITIONED(ix, "dist_batch");
   return pass(ix, ix->dist_batch(queries, nq, (int)dim, cand, m, out));
 }
 int hnsw_b200_bruteforce(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t k,
                          uint32_t* out_ids, float* out_dist) {
   HB_H(h);
+  if (ix->parts) {  // every partition's exact answers, merged like a search; ids are global insertion ranks
+    HB_PARTS_EXCLUSIVE(ix);
+    return pass(ix, ix->parts->bruteforce(queries, nq, (int)dim, k, out_ids, out_dist));
+  }
   return pass(ix, ix->bruteforce(queries, nq, (int)dim, k, out_ids, out_dist));
 }
 

@@ -102,6 +102,11 @@ int metric_from_name(const std::string& name);       // "DistL2" -> METRIC_L2; -
 int metric_from_type_name(const std::string& full);  // the same on the last `::` segment of a type path
 int dtype_from_type_name(const std::string& s);
 
+class Partitions;  // partition.cu: the points of one handle split over several Index objects
+struct PartitionsDeleter {
+  void operator()(Partitions* p) const;
+};
+
 class Index {
  public:
   Index(int M, size_t max_elements, int max_layer, int ef_c, int metric, int dtype, int device);
@@ -188,6 +193,18 @@ class Index {
     std::vector<std::pair<Index*, int>> parts;
   };
   int finish_parts(const std::vector<std::pair<Index*, int>>& parts, const std::function<int(Index*, int)>& fn);
+  // One thread that runs the closures its owner hands it, one at a time (replicas here, partitions in partition.cu).
+  struct Worker {
+    std::thread th;
+    std::mutex m;
+    std::condition_variable cv;
+    std::function<void()> job;
+    bool has_job = false, done = true, quit = false;
+    Worker();
+    ~Worker();
+    void submit(std::function<void()> j);
+    void wait();
+  };
   int64_t park_ticket(Ticket&& t);
   bool take_ticket(int64_t id, Ticket& out);
   void drop_replicas();
@@ -261,7 +278,13 @@ class Index {
   // (insert, import, load, replicate) holds it exclusively
   mutable std::shared_mutex mu;
 
+  // ---- partitions (partition.cu).  A partitioned handle keeps its settings and level RNG here and its points in `parts`;
+  // each partition is an Index of its own whose `owner` is that handle (the C ABI serves it read-only, as a view).
+  std::unique_ptr<Partitions, PartitionsDeleter> parts;
+  const Index* owner = nullptr;
+
  private:
+  friend class Partitions;
   int fail(const std::string& m) const;
   int cuda_fail(cudaError_t e, const char* what) const;
   // ---- graph store
@@ -300,7 +323,6 @@ class Index {
   int check_insert_fit();
   void rollback_points(size_t keep);
 
-  struct Worker;
   struct WorkerDeleter {
     void operator()(Worker* w) const;
   };

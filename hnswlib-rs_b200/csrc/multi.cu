@@ -80,48 +80,41 @@ static NcclApi& nccl() {
 
 // ------------------------------------------------------------------------------------------------ worker threads
 // One per replica: runs the closures the owner hands it, on the replica's device.
-struct Index::Worker {
-  std::thread th;
-  std::mutex m;
-  std::condition_variable cv;
-  std::function<void()> job;
-  bool has_job = false, done = true, quit = false;
-  Worker() {
-    th = std::thread([this] {
-      std::unique_lock<std::mutex> lk(m);
-      for (;;) {
-        cv.wait(lk, [this] { return has_job || quit; });
-        if (quit) return;
-        auto j = std::move(job);
-        has_job = false;
-        lk.unlock();
-        j();
-        lk.lock();
-        done = true;
-        cv.notify_all();
-      }
-    });
-  }
-  void submit(std::function<void()> j) {
+Index::Worker::Worker() {
+  th = std::thread([this] {
     std::unique_lock<std::mutex> lk(m);
-    job = std::move(j);
-    has_job = true;
-    done = false;
-    cv.notify_all();
-  }
-  void wait() {
-    std::unique_lock<std::mutex> lk(m);
-    cv.wait(lk, [this] { return done; });
-  }
-  ~Worker() {
-    {
-      std::unique_lock<std::mutex> lk(m);
-      quit = true;
+    for (;;) {
+      cv.wait(lk, [this] { return has_job || quit; });
+      if (quit) return;
+      auto j = std::move(job);
+      has_job = false;
+      lk.unlock();
+      j();
+      lk.lock();
+      done = true;
       cv.notify_all();
     }
-    th.join();
+  });
+}
+void Index::Worker::submit(std::function<void()> j) {
+  std::unique_lock<std::mutex> lk(m);
+  job = std::move(j);
+  has_job = true;
+  done = false;
+  cv.notify_all();
+}
+void Index::Worker::wait() {
+  std::unique_lock<std::mutex> lk(m);
+  cv.wait(lk, [this] { return done; });
+}
+Index::Worker::~Worker() {
+  {
+    std::unique_lock<std::mutex> lk(m);
+    quit = true;
+    cv.notify_all();
   }
-};
+  th.join();
+}
 
 void Index::WorkerDeleter::operator()(Worker* w) const { delete w; }
 

@@ -116,6 +116,10 @@ def load_library():
     L.hnsw_b200_nccl_init.argtypes = [vp, i32, i32, vp]
     L.hnsw_b200_nccl_broadcast_index.argtypes = [vp, i32]
     L.hnsw_b200_nccl_allgather.argtypes = [vp, vp, vp, u64, vp]
+    L.hnsw_b200_partition.argtypes = [vp, i32, vp]
+    L.hnsw_b200_partition_count.argtypes = [vp]
+    L.hnsw_b200_partition_view.restype = vp
+    L.hnsw_b200_partition_view.argtypes = [vp, i32]
     L.hnsw_b200_dist_batch.argtypes = [vp, vp, u64, u64, vp, u64, vp]
     L.hnsw_b200_bruteforce.argtypes = [vp, vp, u64, u64, u64, vp, vp]
     _LIB = L
@@ -194,6 +198,8 @@ class Hnsw:
 
     # ---- lifetime
     def close(self):
+        if getattr(self, "_parent", None) is not None:  # a partition view: freed with its partitioned handle
+            self._h = self._parent = None
         if getattr(self, "_h", None):
             self._L.hnsw_b200_drop(self._h)
             self._h = None
@@ -440,6 +446,27 @@ class Hnsw:
 
     def replica_count(self):
         return int(self._L.hnsw_b200_replica_count(self._h))
+
+    # ---- partitioned index (include/hnsw_b200.h "Partitioned index")
+    def partition(self, devices):
+        """split this EMPTY index into len(devices) partitions, partition p on devices[p] (devices[0] = this index's
+        device; a device may repeat).  Point g goes to partition g % P; searches run on every partition and merge."""
+        d = np.ascontiguousarray(devices, np.int32)
+        self._chk(self._L.hnsw_b200_partition(self._h, len(d), _p(d)))
+
+    def partition_count(self):
+        return int(self._L.hnsw_b200_partition_count(self._h))
+
+    def partition_view(self, p):
+        """read-only Hnsw on partition p (its own local ids); it keeps this index alive and is never dropped itself"""
+        v = self._L.hnsw_b200_partition_view(self._h, int(p))
+        if not v:
+            raise HnswError(last_error())
+        view = type(self).__new__(type(self))
+        view.__dict__.update({k: getattr(self, k) for k in ("_L", "dtype", "_suf", "dist_name", "max_nb_connection",
+                                                              "ef_construction")})
+        view._h, view._parent = v, self
+        return view
 
     @staticmethod
     def nccl_unique_id():

@@ -51,6 +51,9 @@ extern "C" {
     // multi-GPU (include/hnsw_b200.h "Multi-GPU search"): one process drives several devices
     fn hnsw_b200_replicate(h: *mut HnswApif32, ndev: c_int, devices: *const c_int) -> c_int;
     fn hnsw_b200_replica_count(h: *const HnswApif32) -> c_int;
+    // partitioned index (include/hnsw_b200.h "Partitioned index"): the points split over several devices
+    fn hnsw_b200_partition(h: *mut HnswApif32, nparts: c_int, devices: *const c_int) -> c_int;
+    fn hnsw_b200_partition_count(h: *const HnswApif32) -> c_int;
 }
 
 /// hnsw.rs:46
@@ -119,6 +122,14 @@ impl<D: DistName> Hnsw<D> {
         if r == 0 { Ok(()) } else { Err(r) }
     }
     pub fn replica_count(&self) -> usize { unsafe { hnsw_b200_replica_count(self.h) as usize } }
+    /// Extension (uncompiled, like the rest of this shim): split this EMPTY index into `devs.len()` partitions, partition p
+    /// on `devs[p]` (devs[0] = the device it lives on; a device may repeat).  Point g goes to partition g % P; every
+    /// search runs on all partitions and merges their answers, so the index may exceed one device's memory.
+    pub fn partition(&mut self, devs: &[i32]) -> Result<(), i32> {
+        let r = unsafe { hnsw_b200_partition(self.h, devs.len() as c_int, devs.as_ptr()) };
+        if r == 0 { Ok(()) } else { Err(r) }
+    }
+    pub fn partition_count(&self) -> usize { unsafe { hnsw_b200_partition_count(self.h) as usize } }
 
     /// hnsw.rs:1069-1071
     pub fn insert(&self, datav_with_id: (&[f32], usize)) {

@@ -343,6 +343,41 @@ int hnsw_b200_nccl_init(void* h, int nranks, int rank, const uint8_t* id128);
 int hnsw_b200_nccl_broadcast_index(void* h, int root);
 int hnsw_b200_nccl_allgather(void* h, const void* d_send, void* d_recv, uint64_t bytes_per_rank, void* cuda_stream);
 
+/* ---- Partitioned index: one index larger than one device.  hnsw_b200_replicate copies a whole index to every GPU (more
+ * throughput, no more capacity); a partitioned handle splits its points over P partitions, each an HNSW graph of its own
+ * on its own GPU (several partitions may share one), searches every query on every partition and merges the answers.
+ *
+ * Split an EMPTY handle into nparts partitions, partition p on devices[p] (devices[0] = the handle's device).
+ * A device may be named more than once: several partitions then share one GPU.  Refused on a non-empty, replicated or
+ * NCCL-initialised handle.  Settings made before the call are copied to the partitions.
+ *   Placement: the g-th point inserted into the handle, counted over all insert calls, goes to partition g % P as that
+ *     partition's local id g / P.  Levels are drawn once, in global insertion order, from the handle's RNG (explicit
+ *     levels are passed through), so a partitioned build draws the levels an unpartitioned build of the same sequence
+ *     draws.  Default origin ids (ids == NULL) are the global rank g.
+ *   Inserts (insert_<ty>, parallel_insert_<ty>, hnsw_b200_insert_flat) split the batch by placement; the partitions insert
+ *     their shares at once.  Dimension, shared-memory fit and every partition's capacity are checked first: a failure
+ *     there leaves every partition unchanged.  A failure after that can leave the partitions at counts the placement rule
+ *     does not give: the handle then refuses further inserts, with a message that names the partition; searches go on.
+ *   Searches (search_neighbours_<ty>, parallel_search_neighbours_<ty>, hnsw_b200_search_flat with filter modes 0, 1, 2)
+ *     run every query on every partition with the caller's k and ef.  The answer is the first min(k, sum of counts)
+ *     entries of the P ascending lists, ordered by (distance, partition index, position in that partition's list), in
+ *     both tie modes; slots past the count are (~0, +inf, INVALID_ID).  out_internal = local * P + p, the global
+ *     insertion rank; out_pid is the PointId (level, rank) in the answering partition's own graph.  A filter callback
+ *     (mode 2) is called on the calling thread only, once per stored origin id over all partitions.
+ *   hnsw_b200_bruteforce merges every partition's exact answers by the same rule and returns global insertion ranks.
+ *   Setters apply to every partition.  get_nb_point is the sum over the partitions, get_max_level_observed the max,
+ *     get_stats the sum (out[3] counts each query once per partition).
+ *   Refused with an error and no change: hnsw_b200_replicate, hnsw_b200_nccl_*, search_flat_submit / _wait,
+ *     search_device, dist_batch, file_dump*, export_*, layer_edges, flatten, flat_neighbours, import_graph, blob_*.
+ *   Calls take the handle's lock, then every partition's in partition order: shared for searches, exclusive otherwise.
+ *   hnsw_b200_drop / drop_hnsw_<ty> on the handle frees every partition. */
+int hnsw_b200_partition(void* h, int nparts, const int* devices);
+int hnsw_b200_partition_count(const void* h); /* 1 for an ordinary handle */
+/* Borrowed, read-only handle on partition p (valid until h is dropped; never pass it to a drop function).  Read-only
+ * calls work on it (export_*, flatten, file_dump, get_*, search_flat ...), so each partition can be dumped; calls that
+ * change the graph or its settings are refused.  Its internal ids are the partition's local ids. */
+const void* hnsw_b200_partition_view(const void* h, int p);
+
 /* Stand-alone kernels.  dist_batch: out[nq][m] = dist(queries[i], base[cand[i][j]]) on the index's
  * point store (host pointers).  bruteforce: exact k nearest (ascending) of each query over the
  * index's point store: out_ids are INTERNAL ids. */
