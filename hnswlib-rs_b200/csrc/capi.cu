@@ -162,7 +162,7 @@ static const Neighbourhood_api* search_any(const void* hv, size_t len, const voi
     AnswerArrays out;
     out.nb = (NeighbourOut*)nb;
     out.counts = &cnt;
-    rc = h->ix->parts->search(data, nullptr, 1, (int)len, knbn, ef_search, 0, nullptr, 0, nullptr, nullptr, out);
+    rc = h->ix->parts->search(data, nullptr, 1, (int)len, knbn, ef_search, 0, nullptr, 0, nullptr, nullptr, nullptr, out);
   } else {
     rc = h->ix->search_host(data, nullptr, 1, (int)len, knbn, ef_search, nullptr, (NeighbourOut*)nb, &cnt);
   }
@@ -203,7 +203,8 @@ static const Vec_api_Neighbourhood_api* parallel_search_any(const void* hv, size
     AnswerArrays out;
     out.nb = (NeighbourOut*)box->block;
     out.counts = cnt.data();
-    rc = h->ix->parts->search(nullptr, data, nb_vec, (int)vec_len, knbn, ef_search, 0, nullptr, 0, nullptr, nullptr, out);
+    rc = h->ix->parts->search(nullptr, data, nb_vec, (int)vec_len, knbn, ef_search, 0, nullptr, 0, nullptr, nullptr, nullptr,
+                                 out);
   } else if (use_shards(h->ix, nb_vec)) {  // replicas on other GPUs: every device answers its slice of the batch in place
     NeighbourOut* block = (NeighbourOut*)box->block;
     int32_t* cp = cnt.data();
@@ -614,10 +615,12 @@ static void unpack_answers(const Index* rx, const NeighbourOut* a, const int32_t
     for (uint64_t s = 0; s < tot; ++s) hb::point_id(rx, a[s].internal, pid + 2 * s);
 }
 
-int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
-                          uint64_t ef_search, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,
-                          hnsw_b200_filter_fn fn, void* ctx, uint64_t* out_ids, float* out_dist,
-                          uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+// hnsw_b200_search_flat and _search_flat_filtered: the filter is the FilterT arguments (filter_mode 1, 2) or, when
+// `resident` is set, one of the handle's resident filters (filter_mode 0).  The kernels and the answers are the same.
+static int search_flat_any(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
+                           int filter_mode, const uint64_t* filter_ids, uint64_t nfilter, hnsw_b200_filter_fn fn, void* ctx,
+                           const int64_t* resident, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                           int32_t* out_pid, int32_t* out_counts) {
   HB_HS(h);
   if (nq == 0) return 0;
   if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0) return set_err("bad argument");
@@ -630,7 +633,7 @@ int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint6
     out.pid = out_pid;
     out.counts = out_counts;
     return pass(ix, ix->parts->search(queries, nullptr, nq, (int)dim, knbn, ef_search, filter_mode, filter_ids, nfilter, fn,
-                                      ctx, out));
+                                      ctx, resident, out));
   }
   std::vector<uint32_t> bits;
   const uint32_t* fb = nullptr;
@@ -644,8 +647,11 @@ int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint6
   auto run = [=](Index* rx, size_t first, size_t count) -> int {
     const NeighbourOut* tmp = nullptr;
     const int32_t* cnts = nullptr;
+    const uint32_t* dfb = nullptr;  // a resident filter's copy on rx's device
+    if (resident && ix->filters.use(*resident, 0, 1, rx, &dfb)) return -1;
     Index::CtxLease lease(rx);  // the answers stay in the context's pinned buffer until they are unpacked below
-    int r = rx->search_host_staged(lease.c, (const char*)queries + first * qrow, nullptr, count, (int)dim, knbn, ef_search, fb, &tmp, &cnts);
+    int r = rx->search_host_staged(lease.c, (const char*)queries + first * qrow, nullptr, count, (int)dim, knbn, ef_search, fb,
+                                   dfb, &tmp, &cnts);
     if (r) return r;
     const uint64_t o0 = first * knbn;
     unpack_answers(rx, tmp, cnts, count, knbn, out_ids + o0, out_dist + o0, out_internal ? out_internal + o0 : nullptr,
@@ -655,13 +661,26 @@ int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint6
   return pass(ix, use_shards(ix, nq) ? ix->for_each_shard(nq, run) : run(ix, 0, nq));
 }
 
-// Submit / wait: the same search with the call split in two, so that one host thread keeps several batches in flight
-// (batch i+1 is enqueued before batch i's answers are collected).  Unfiltered, one device.
+int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
+                          uint64_t ef_search, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,
+                          hnsw_b200_filter_fn fn, void* ctx, uint64_t* out_ids, float* out_dist,
+                          uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+  return search_flat_any(h, queries, nq, dim, knbn, ef_search, filter_mode, filter_ids, nfilter, fn, ctx, nullptr, out_ids,
+                         out_dist, out_internal, out_pid, out_counts);
+}
+int hnsw_b200_search_flat_filtered(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim,
+                                   uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
+                                   uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+  return search_flat_any(h, queries, nq, dim, knbn, ef_search, 0, nullptr, 0, nullptr, nullptr, &filter, out_ids, out_dist,
+                         out_internal, out_pid, out_counts);
+}
+
 // one device's share of a submitted batch: enqueue on a leased context of `rx`, remember where to unpack to
 static int submit_on(Index* rx, int* ctx_out, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
-                     uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+                     const uint32_t* d_filter_bits, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                     int32_t* out_pid, int32_t* out_counts) {
   const int ci = rx->acquire_ctx();
-  int r = rx->search_host_begin(ci, queries, nullptr, nq, (int)dim, knbn, ef_search, nullptr);
+  int r = rx->search_host_begin(ci, queries, nullptr, nq, (int)dim, knbn, ef_search, nullptr, d_filter_bits);
   if (r) {
     rx->release_ctx(ci);
     return r;
@@ -688,37 +707,45 @@ static int wait_on(Index* rx, int ci) {
 }
 
 // Submit / wait: the same search with the call split in two, so that one host thread keeps several batches in flight
-// (batch i+1 is enqueued before batch i's answers are collected).  Unfiltered.  With replicas (hnsw_b200_replicate) the
-// batch is sharded like a search_flat call: every device gets its contiguous share enqueued at submit time.
-int64_t hnsw_b200_search_flat_submit(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
-                                     uint64_t ef_search, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
-                                     int32_t* out_pid, int32_t* out_counts) {
+// (batch i+1 is enqueued before batch i's answers are collected).  Unfiltered, or with a resident filter.  With replicas
+// (hnsw_b200_replicate) the batch is sharded like a search_flat call: every device gets its contiguous share enqueued at
+// submit time.
+static int64_t submit_any(const void* h, const int64_t* resident, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
+                          uint64_t ef_search, uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
+                          int32_t* out_counts) {
   HB_HS(h);
-  HB_NOT_PARTITIONED(ix, "search_flat_submit");
+  HB_NOT_PARTITIONED(ix, resident ? "search_flat_submit_filtered" : "search_flat_submit");
   if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0 || nq == 0) return set_err("bad argument");
   Index::Ticket t;
   const size_t qrow = (size_t)dim * ix->es;
-  int r = 0;
-  if (use_shards(ix, nq)) {
-    r = ix->for_each_shard_inline(nq, [&](Index* rx, size_t first, size_t count) {
-      int ci = -1;
-      int rr = submit_on(rx, &ci, (const char*)queries + first * qrow, count, dim, knbn, ef_search, out_ids + first * knbn,
-                         out_dist + first * knbn, out_internal ? out_internal + first * knbn : nullptr,
-                         out_pid ? out_pid + 2 * first * knbn : nullptr, out_counts + first);
-      if (!rr) t.parts.push_back({rx, ci});
-      return rr;
-    });
-  } else {
+  auto run = [&](Index* rx, size_t first, size_t count) -> int {
+    const uint32_t* dfb = nullptr;
+    if (resident && ix->filters.use(*resident, 0, 1, rx, &dfb)) return -1;
     int ci = -1;
-    r = submit_on(ix, &ci, queries, nq, dim, knbn, ef_search, out_ids, out_dist, out_internal, out_pid, out_counts);
-    if (!r) t.parts.push_back({ix, ci});
-  }
+    int r = submit_on(rx, &ci, (const char*)queries + first * qrow, count, dim, knbn, ef_search, dfb, out_ids + first * knbn,
+                      out_dist + first * knbn, out_internal ? out_internal + first * knbn : nullptr,
+                      out_pid ? out_pid + 2 * first * knbn : nullptr, out_counts + first);
+    if (!r) t.parts.push_back({rx, ci});
+    return r;
+  };
+  const int r = use_shards(ix, nq) ? ix->for_each_shard_inline(nq, run) : run(ix, 0, nq);
   if (r) {
     for (auto& pr : t.parts) wait_on(pr.first, pr.second);  // collect what was enqueued before the failure
     return pass(ix, r);
   }
   ix->pending_.fetch_add(1);
   return ix->park_ticket(std::move(t));
+}
+
+int64_t hnsw_b200_search_flat_submit(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
+                                     uint64_t ef_search, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                                     int32_t* out_pid, int32_t* out_counts) {
+  return submit_any(h, nullptr, queries, nq, dim, knbn, ef_search, out_ids, out_dist, out_internal, out_pid, out_counts);
+}
+int64_t hnsw_b200_search_flat_submit_filtered(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim,
+                                              uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
+                                              uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+  return submit_any(h, &filter, queries, nq, dim, knbn, ef_search, out_ids, out_dist, out_internal, out_pid, out_counts);
 }
 
 int hnsw_b200_search_flat_wait(const void* h, int64_t ticket) {
@@ -741,12 +768,40 @@ int hnsw_b200_search_flat_wait(const void* h, int64_t ticket) {
   return r;
 }
 
+static int search_device_any(const void* h, const int64_t* resident, const void* d_queries, uint64_t nq, uint64_t knbn,
+                             uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
+  HB_HS(h);
+  HB_NOT_PARTITIONED(ix, resident ? "search_device_filtered" : "search_device");
+  const uint32_t* dfb = nullptr;
+  if (resident && ix->filters.use(*resident, 0, 1, ix, &dfb)) return pass(ix, -1);
+  return pass(ix, ix->search_device(d_queries, nq, knbn, ef_search, dfb, (NeighbourOut*)d_out, d_counts, sync != 0, kernel_ms));
+}
 int hnsw_b200_search_device(const void* h, const void* d_queries, uint64_t nq, uint64_t knbn,
                             uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
-  HB_HS(h);
-  HB_NOT_PARTITIONED(ix, "search_device");
-  return pass(ix, ix->search_device(d_queries, nq, knbn, ef_search, nullptr, (NeighbourOut*)d_out, d_counts, sync != 0,
-                                    kernel_ms));
+  return search_device_any(h, nullptr, d_queries, nq, knbn, ef_search, d_out, d_counts, sync, kernel_ms);
+}
+int hnsw_b200_search_device_filtered(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
+                                     uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
+  return search_device_any(h, &filter, d_queries, nq, knbn, ef_search, d_out, d_counts, sync, kernel_ms);
+}
+
+int64_t hnsw_b200_filter_new(const void* h, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,
+                             hnsw_b200_filter_fn fn, void* ctx) {
+  HB_HS(h);  // shared: the points cannot change while the bitmap is made
+  HB_NOT_VIEW(ix);
+  if (ix->parts) {
+    HB_PARTS_SHARED(ix);
+    const int64_t id = ix->new_filter(filter_mode, filter_ids, nfilter, fn, ctx);
+    if (id < 0) g_err = ix->err();
+    return id;
+  }
+  const int64_t id = ix->new_filter(filter_mode, filter_ids, nfilter, fn, ctx);
+  if (id < 0) g_err = ix->err();
+  return id;
+}
+int hnsw_b200_filter_free(const void* h, int64_t filter) {
+  HB_H(h);  // exclusive: waits for every search under the shared lock and every outstanding ticket
+  return pass(ix, ix->free_filter(filter));
 }
 
 int hnsw_b200_join(void* h) {

@@ -775,7 +775,7 @@ static const void* device_view_of_host(const void* p) {
 // synchronisation.  Pageable queries and row pointers are gathered into the context's own pinned staging buffer first
 // (the only host-side copy), which the kernel then reads the same way.
 int Index::search_host_begin(int ci, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                             const uint32_t* filter_bits_host) {
+                             const uint32_t* filter_bits_host, const uint32_t* d_filter_bits) {
   SearchCtx& c = ctx_[ci];
   cudaStream_t st = c.stream;
   c.pend = SearchCtx::Pending();
@@ -816,7 +816,7 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
   if (!dv) return fail("the pinned result buffer has no device address");
   NeighbourOut* k_out = (NeighbourOut*)dv;
   int32_t* k_cnt = (int32_t*)(dv + out_bytes);
-  const uint32_t* dfb = nullptr;
+  const uint32_t* dfb = d_filter_bits;  // a resident filter: already on this device
   if (filter_bits_host) {
     const size_t fb = ((n + 31) / 32) * 4;
     if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, fb, st))) return r;
@@ -850,10 +850,11 @@ int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** 
 }
 
 int Index::search_host_staged(int ci, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                              const uint32_t* filter_bits_host, const NeighbourOut** out, const int32_t** counts) {
+                              const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const NeighbourOut** out,
+                              const int32_t** counts) {
   *out = nullptr;
   *counts = nullptr;
-  int r = search_host_begin(ci, queries, rows, nq, d, k, ef, filter_bits_host);
+  int r = search_host_begin(ci, queries, rows, nq, d, k, ef, filter_bits_host, d_filter_bits);
   if (r) return r;
   return search_host_finish(ci, out, counts);
 }
@@ -863,7 +864,7 @@ int Index::search_host(const void* queries, const void* const* rows, size_t nq, 
   CtxLease lease(this);
   const NeighbourOut* so;
   const int32_t* sc;
-  int r = search_host_staged(lease.c, queries, rows, nq, d, k, ef, filter_bits_host, &so, &sc);
+  int r = search_host_staged(lease.c, queries, rows, nq, d, k, ef, filter_bits_host, nullptr, &so, &sc);
   if (r || nq == 0) return r;
   memcpy(counts, sc, nq * sizeof(int32_t));
   memcpy(out, so, nq * k * sizeof(NeighbourOut));

@@ -102,6 +102,36 @@ int metric_from_name(const std::string& name);       // "DistL2" -> METRIC_L2; -
 int metric_from_type_name(const std::string& full);  // the same on the last `::` segment of a type path
 int dtype_from_type_name(const std::string& s);
 
+class Index;
+
+// Resident filters (hnsw_b200_filter_new, filter_store.cu): a FilterT materialised once per handle, as one bitmap per
+// partition (one for an ordinary handle) over the points stored when it was made.  The host copy stays; each device a
+// search uses it on gets one device copy, made at its first use there.  Ids are unique over all handles, so an id that
+// belongs to another handle is unknown here.  A search takes the handle's lock shared and uses a filter under it; free
+// takes it exclusively, so a filter is never freed while a search holds it.
+class FilterStore {
+ public:
+  struct Filter {
+    std::vector<std::vector<uint32_t>> bits;  // [partition] bit per internal id (make_filter_bits)
+    std::vector<size_t> counts;               // [partition] points stored when the filter was made
+    std::map<std::pair<int, int>, void*> dev;  // (partition, device) -> device copy of bits[partition]
+  };
+  FilterStore() = default;
+  FilterStore(const FilterStore&) = delete;
+  FilterStore& operator=(const FilterStore&) = delete;
+  ~FilterStore();  // frees every device copy (the owner has synchronised its streams)
+  int64_t add(Filter&& f);
+  bool has(int64_t id);
+  // the device copy of partition p's bitmap on rx's device (copied there on first use), after checking that the filter
+  // exists and that rx, partition p of `nparts`, still holds the points the filter was made over; if not, rx's error
+  int use(int64_t id, int p, int nparts, const Index* rx, const uint32_t** d_bits);
+  void erase(int64_t id);  // frees its device copies; the caller waited for every search that may read them
+
+ private:
+  std::mutex mu_;
+  std::map<int64_t, Filter> f_;
+};
+
 class Partitions;  // partition.cu: the points of one handle split over several Index objects
 struct PartitionsDeleter {
   void operator()(Partitions* p) const;
@@ -145,9 +175,11 @@ class Index {
   // host queries (flat or row pointers); results to host NeighbourOut[nq][k] + counts
   int search_host(const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
                   const uint32_t* filter_bits_host, NeighbourOut* out, int32_t* counts);
-  // same on context c (a CtxLease), answers left in the context's pinned buffer (valid until the lease ends)
+  // same on context c (a CtxLease), answers left in the context's pinned buffer (valid until the lease ends).  The filter
+  // is either host bits, uploaded into the context for this call, or d_filter_bits already on this device (a resident
+  // filter); at most one of the two is non-null.
   int search_host_begin(int c, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                        const uint32_t* filter_bits_host);
+                        const uint32_t* filter_bits_host, const uint32_t* d_filter_bits);
   int search_host_finish(int c, const NeighbourOut** out, const int32_t** counts);
   // submitted-but-not-waited host searches: anything that changes the graph waits for them (drain_pending)
   std::atomic<int> pending_{0};
@@ -155,12 +187,19 @@ class Index {
     while (pending_.load() != 0) std::this_thread::yield();
   }
   int search_host_staged(int c, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                         const uint32_t* filter_bits_host, const NeighbourOut** out, const int32_t** counts);
+                         const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const NeighbourOut** out,
+                         const int32_t** counts);
   int search_device(const void* d_queries, size_t nq, size_t k, size_t ef, const uint32_t* d_filter_bits,
                     NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms);
   // filter materialisation: bit per internal id from a sorted origin-id list or a callback
   int make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx,
                        std::vector<uint32_t>& bits) const;
+  // resident filters of this handle; free_filter waits for the asynchronous device-resident launches that may still read
+  // the filter (the caller holds the handle exclusively, so no other search and no submitted batch is left)
+  FilterStore filters;
+  // a resident filter over every stored point (every partition's, on a partitioned handle): its id (>= 0), or < 0
+  int64_t new_filter(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx);
+  int free_filter(int64_t id);
 
   int export_layer(int layer, uint64_t* offsets, uint32_t* ids, float* dists, int64_t* total) const;
   int export_vectors(void* out) const;
@@ -285,6 +324,7 @@ class Index {
 
  private:
   friend class Partitions;
+  friend class FilterStore;
   int fail(const std::string& m) const;
   int cuda_fail(cudaError_t e, const char* what) const;
   // ---- graph store

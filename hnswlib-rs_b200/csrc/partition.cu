@@ -172,16 +172,19 @@ static size_t merge_lists(int P, size_t k, const int32_t* cnt, const Dist& dist,
 
 int Partitions::search(const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef, int filter_mode,
                        const uint64_t* filter_ids, size_t nfilter, int (*fn)(uint64_t, void*), void* ctx,
-                       const AnswerArrays& out) {
+                       const int64_t* resident, const AnswerArrays& out) {
   if (nq == 0) return 0;
   if (k == 0) return parent_->fail("knbn must be positive");
   if (parent_->dim != 0 && d != parent_->dim) return parent_->fail("query length differs from the index dimension");
   const int P = count();
-  // every partition's filter bitmap, on the calling thread: a FilterT callback need not be thread-safe
+  // every partition's filter bitmap: a resident filter's device copy, or host bits made here, on the calling thread (a
+  // FilterT callback need not be thread-safe) and uploaded with the search
   std::vector<std::vector<uint32_t>> bits(P);
-  if (filter_mode)
-    for (int p = 0; p < P; ++p)
-      if (ix_[p]->make_filter_bits(filter_mode, filter_ids, nfilter, fn, ctx, bits[p])) return fail(p, ix_[p]->err());
+  std::vector<const uint32_t*> dbits(P, nullptr);
+  for (int p = 0; p < P; ++p) {
+    if (resident && parent_->filters.use(*resident, p, P, ix_[p].get(), &dbits[p])) return fail(p, ix_[p]->err());
+    if (filter_mode && ix_[p]->make_filter_bits(filter_mode, filter_ids, nfilter, fn, ctx, bits[p])) return fail(p, ix_[p]->err());
+  }
   // one leased context per partition, taken in partition order; the answers stay in them until the merge is done
   std::vector<int> ci(P, -1);
   struct Leases {
@@ -197,7 +200,8 @@ int Partitions::search(const void* queries, const void* const* rows, size_t nq, 
   DeviceRestore keep;
   int failed = -1, begun = 0;
   for (; begun < P; ++begun)
-    if (ix_[begun]->search_host_begin(ci[begun], queries, rows, nq, d, k, ef, filter_mode ? bits[begun].data() : nullptr)) {
+    if (ix_[begun]->search_host_begin(ci[begun], queries, rows, nq, d, k, ef, filter_mode ? bits[begun].data() : nullptr,
+                                      dbits[begun])) {
       failed = begun;
       break;
     }

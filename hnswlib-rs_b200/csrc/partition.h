@@ -57,9 +57,11 @@ class Partitions {
   // a batch in the engine's insert form (flat `vecs` with `stride` elements per row, or `rows`), split by placement
   int insert(const void* vecs, size_t n_new, size_t stride, const void* const* rows, const uint64_t* ids,
              const int32_t* levels, int d);
-  // every query on every partition with the caller's k and ef, merged into `out`
+  // every query on every partition with the caller's k and ef, merged into `out`.  The filter is the FilterT arguments
+  // (filter_mode 1, 2) or `resident`, the id of one of the handle's resident filters (filter_mode 0).
   int search(const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef, int filter_mode,
-             const uint64_t* filter_ids, size_t nfilter, int (*fn)(uint64_t, void*), void* ctx, const AnswerArrays& out);
+             const uint64_t* filter_ids, size_t nfilter, int (*fn)(uint64_t, void*), void* ctx, const int64_t* resident,
+             const AnswerArrays& out);
   // exact k nearest over all partitions, merged like search; out_ids are global insertion ranks
   int bruteforce(const void* queries, size_t nq, int d, size_t k, uint32_t* out_ids, float* out_dist);
   int get_stats(uint64_t* out4, bool reset);

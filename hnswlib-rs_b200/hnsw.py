@@ -90,6 +90,13 @@ def load_library():
     L.hnsw_b200_search_flat_submit.restype = i64
     L.hnsw_b200_search_flat_submit.argtypes = [vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_flat_wait.argtypes = [vp, i64]
+    L.hnsw_b200_filter_new.restype = i64
+    L.hnsw_b200_filter_new.argtypes = [vp, i32, vp, u64, FILTER_FN, vp]
+    L.hnsw_b200_filter_free.argtypes = [vp, i64]
+    L.hnsw_b200_search_flat_filtered.argtypes = [vp, i64, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_flat_submit_filtered.restype = i64
+    L.hnsw_b200_search_flat_submit_filtered.argtypes = [vp, i64, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_device_filtered.argtypes = [vp, i64, vp, u64, u64, u64, vp, vp, i32, vp]
     L.hnsw_b200_get_stats.argtypes = [vp, vp, i32]
     L.hnsw_b200_set_stream.argtypes = [vp, vp]
     L.hnsw_b200_join.argtypes = [vp]
@@ -168,6 +175,36 @@ class Neighbour:
 
 _DT = {np.dtype(np.float32): (0, "f32"), np.dtype(np.uint8): (1, "u8"), np.dtype(np.uint16): (2, "u16"),
        np.dtype(np.uint32): (3, "u32"), np.dtype(np.int32): (4, "i32")}
+
+
+def _filter_args(filter):
+    """(mode, sorted ids | None, count, callback) of a FilterT given as a sorted id sequence or a callable(id)->bool"""
+    if callable(filter):
+        return 2, None, 0, FILTER_FN(lambda i, _c: 1 if filter(int(i)) else 0)
+    fids = np.ascontiguousarray(np.sort(np.asarray(filter, np.uint64)))
+    return 1, fids, len(fids), FILTER_FN(0)
+
+
+class ResidentFilter:
+    """A FilterT materialised once on the device (hnsw_b200_filter_new), made by Hnsw.make_filter and passed as
+    `filter=` to search_flat, search_filter, submit_flat and search_device.  It covers the points stored when it was
+    made: after an insert, searches with it are refused.  free() (or leaving a `with` block) releases it; the handle
+    frees the filters still alive when it is closed.  Not freed by garbage collection: free() waits for the handle's
+    submitted batches, so a thread must collect its own tickets first."""
+
+    def __init__(self, index, fid):
+        self.index, self.id = index, int(fid)
+
+    def free(self):
+        if self.index is not None and self.index._h:
+            self.index._chk(self.index._L.hnsw_b200_filter_free(self.index._h, self.id))
+        self.index = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.free()
 
 
 class Hnsw:
@@ -293,7 +330,7 @@ class Hnsw:
         return self.search_filter(data, knbn, ef_arg, filter)
 
     def search_filter(self, data, knbn, ef_arg, filter=None):
-        """filter: None | sorted sequence of ids (FilterT for Vec<usize>) | callable(id)->bool."""
+        """filter: None | sorted sequence of ids (FilterT for Vec<usize>) | callable(id)->bool | ResidentFilter."""
         if filter is None:
             v = np.ascontiguousarray(data, self.dtype)
             res = getattr(self._L, "search_neighbours_" + self._suf)(self._h, v.size, _p(v), int(knbn), int(ef_arg))
@@ -328,7 +365,7 @@ class Hnsw:
 
     def search_flat(self, queries, knbn, ef, filter=None, with_internal=True, with_pid=True):
         """Extension: flat batch.  Returns (origin u64[nq,k], dist f32[nq,k], internal u32[nq,k] | None,
-        pid i32[nq,k,2] | None, counts)."""
+        pid i32[nq,k,2] | None, counts).  filter: as search_filter takes it."""
         q = np.ascontiguousarray(queries, self.dtype)
         nq, d = q.shape
         o = np.empty((nq, knbn), np.uint64)
@@ -336,21 +373,29 @@ class Hnsw:
         it = np.empty((nq, knbn), np.uint32) if with_internal else None
         pid = np.empty((nq, knbn, 2), np.int32) if with_pid else None
         cnt = np.empty(nq, np.int32)
+        if isinstance(filter, ResidentFilter):
+            self._chk(self._L.hnsw_b200_search_flat_filtered(self._h, filter.id, _p(q), nq, d, int(knbn), int(ef), _p(o),
+                                                             _p(ds), _p(it), _p(pid), _p(cnt)))
+            return o, ds, it, pid, cnt
         mode, fids, nf, cb = 0, None, 0, FILTER_FN(0)
         if filter is not None:
-            if callable(filter):
-                mode = 2
-                cb = FILTER_FN(lambda i, _c: 1 if filter(int(i)) else 0)
-            else:
-                mode = 1
-                fids = np.ascontiguousarray(np.sort(np.asarray(filter, np.uint64)))
-                nf = len(fids)
+            mode, fids, nf, cb = _filter_args(filter)
         self._chk(self._L.hnsw_b200_search_flat(self._h, _p(q), nq, d, int(knbn), int(ef), mode, _p(fids), nf, cb, None,
                                                 _p(o), _p(ds), _p(it), _p(pid), _p(cnt)))
         return o, ds, it, pid, cnt
 
-    def submit_flat(self, queries, knbn, ef, with_internal=True, with_pid=True):
-        """hnsw_b200_search_flat_submit: enqueue a batch, return a ticket for wait_flat (up to 4 outstanding)"""
+    def make_filter(self, filter):
+        """hnsw_b200_filter_new: materialise a FilterT (sorted id sequence or callable(id)->bool, as search_flat takes)
+        once, over the points stored now; a callable is called once per stored point, here.  Returns a ResidentFilter."""
+        mode, fids, nf, cb = _filter_args(filter)
+        fid = self._L.hnsw_b200_filter_new(self._h, mode, _p(fids), nf, cb, None)
+        if fid < 0:
+            raise HnswError(last_error())
+        return ResidentFilter(self, fid)
+
+    def submit_flat(self, queries, knbn, ef, with_internal=True, with_pid=True, filter=None):
+        """hnsw_b200_search_flat_submit: enqueue a batch, return a ticket for wait_flat (up to 4 outstanding).
+        filter: None or a ResidentFilter (hnsw_b200_search_flat_submit_filtered)."""
         q = np.ascontiguousarray(queries, self.dtype)
         nq, d = q.shape
         o = np.empty((nq, knbn), np.uint64)
@@ -358,7 +403,14 @@ class Hnsw:
         it = np.empty((nq, knbn), np.uint32) if with_internal else None
         pid = np.empty((nq, knbn, 2), np.int32) if with_pid else None
         cnt = np.empty(nq, np.int32)
-        t = self._L.hnsw_b200_search_flat_submit(self._h, _p(q), nq, d, int(knbn), int(ef), _p(o), _p(ds), _p(it), _p(pid), _p(cnt))
+        if filter is None:
+            t = self._L.hnsw_b200_search_flat_submit(self._h, _p(q), nq, d, int(knbn), int(ef), _p(o), _p(ds), _p(it), _p(pid),
+                                                     _p(cnt))
+        elif isinstance(filter, ResidentFilter):
+            t = self._L.hnsw_b200_search_flat_submit_filtered(self._h, filter.id, _p(q), nq, d, int(knbn), int(ef), _p(o),
+                                                              _p(ds), _p(it), _p(pid), _p(cnt))
+        else:
+            raise TypeError("submit_flat takes a ResidentFilter (Hnsw.make_filter) as its filter")
         if t < 0:
             raise HnswError(last_error())
         return (int(t), q, o, ds, it, pid, cnt)
@@ -429,13 +481,19 @@ class Hnsw:
             raise HnswError(last_error())
         return r
 
-    def search_device(self, d_queries_ptr, nq, knbn, ef, d_out_ptr, d_counts_ptr, sync=True):
+    def search_device(self, d_queries_ptr, nq, knbn, ef, d_out_ptr, d_counts_ptr, sync=True, filter=None):
         """Device-resident search: raw device pointers in, Neighbour_api[nq][knbn] + int32 counts out.
-        Returns the kernel's CUDA-event time in ms when sync is true."""
+        Returns the kernel's CUDA-event time in ms when sync is true.  filter: None or a ResidentFilter
+        (hnsw_b200_search_device_filtered)."""
         ms = C.c_float(0.0)
-        self._chk(self._L.hnsw_b200_search_device(self._h, C.c_void_p(d_queries_ptr), nq, int(knbn), int(ef),
-                                                  C.c_void_p(d_out_ptr), C.c_void_p(d_counts_ptr), int(bool(sync)),
-                                                  C.byref(ms) if sync else None))
+        args = (C.c_void_p(d_queries_ptr), nq, int(knbn), int(ef), C.c_void_p(d_out_ptr), C.c_void_p(d_counts_ptr),
+                int(bool(sync)), C.byref(ms) if sync else None)
+        if filter is None:
+            self._chk(self._L.hnsw_b200_search_device(self._h, *args))
+        elif isinstance(filter, ResidentFilter):
+            self._chk(self._L.hnsw_b200_search_device_filtered(self._h, filter.id, *args))
+        else:
+            raise TypeError("search_device takes a ResidentFilter (Hnsw.make_filter) as its filter")
         return float(ms.value)
 
     # ---- multi-GPU (include/hnsw_b200.h "Multi-GPU search")

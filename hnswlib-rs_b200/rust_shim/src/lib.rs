@@ -54,6 +54,19 @@ extern "C" {
     // partitioned index (include/hnsw_b200.h "Partitioned index"): the points split over several devices
     fn hnsw_b200_partition(h: *mut HnswApif32, nparts: c_int, devices: *const c_int) -> c_int;
     fn hnsw_b200_partition_count(h: *const HnswApif32) -> c_int;
+    // resident filters (include/hnsw_b200.h "Resident filters"): a FilterT materialised once, passed by id
+    fn hnsw_b200_filter_new(h: *const HnswApif32, filter_mode: c_int, filter_ids: *const u64, nfilter: u64,
+                            f: Option<extern "C" fn(u64, *mut c_void) -> c_int>, ctx: *mut c_void) -> i64;
+    fn hnsw_b200_filter_free(h: *const HnswApif32, filter: i64) -> c_int;
+    fn hnsw_b200_search_flat_filtered(h: *const HnswApif32, filter: i64, queries: *const f32, nq: u64, dim: u64, knbn: u64,
+                                      ef: u64, out_ids: *mut u64, out_dist: *mut f32, out_internal: *mut u32,
+                                      out_pid: *mut i32, out_counts: *mut i32) -> c_int;
+    fn hnsw_b200_search_flat_submit_filtered(h: *const HnswApif32, filter: i64, queries: *const f32, nq: u64, dim: u64,
+                                             knbn: u64, ef: u64, out_ids: *mut u64, out_dist: *mut f32,
+                                             out_internal: *mut u32, out_pid: *mut i32, out_counts: *mut i32) -> i64;
+    fn hnsw_b200_search_device_filtered(h: *const HnswApif32, filter: i64, d_queries: *const c_void, nq: u64, knbn: u64,
+                                        ef: u64, d_out: *mut c_void, d_counts: *mut i32, sync: c_int,
+                                        kernel_ms: *mut f32) -> c_int;
 }
 
 /// hnsw.rs:46
@@ -164,6 +177,27 @@ impl<D: DistName> Hnsw<D> {
         assert_eq!(r, 0, "hnsw_b200_search_flat failed");
         (0..cnt as usize).map(|j| Neighbour { d_id: ids[j] as usize, distance: ds[j], p_id: PointId(pid[2 * j] as u8, pid[2 * j + 1]) }).collect()
     }
+    /// Extension: materialise `filter` once, over the points stored now (the closure runs once per stored origin id,
+    /// here).  Searches with the returned filter answer exactly as `search_filter` with `filter` does, without
+    /// re-evaluating it; after an insert they are refused.
+    pub fn make_filter(&self, filter: &dyn FilterT) -> Result<ResidentFilter<'_, D>, i64> {
+        let ctx = &filter as *const &dyn FilterT as *mut c_void;
+        let id = unsafe { hnsw_b200_filter_new(self.h, 2, std::ptr::null(), 0, Some(filter_trampoline), ctx) };
+        if id >= 0 { Ok(ResidentFilter { index: self, id }) } else { Err(id) }
+    }
+    /// search_filter with a resident filter
+    pub fn search_resident(&self, data: &[f32], knbn: usize, ef_arg: usize, filter: &ResidentFilter<'_, D>) -> Vec<Neighbour> {
+        let mut ids = vec![0u64; knbn];
+        let mut ds = vec![0f32; knbn];
+        let mut pid = vec![0i32; 2 * knbn];
+        let mut cnt = 0i32;
+        let r = unsafe {
+            hnsw_b200_search_flat_filtered(self.h, filter.id, data.as_ptr(), 1, data.len() as u64, knbn as u64, ef_arg as u64,
+                                           ids.as_mut_ptr(), ds.as_mut_ptr(), std::ptr::null_mut(), pid.as_mut_ptr(), &mut cnt)
+        };
+        assert_eq!(r, 0, "hnsw_b200_search_flat_filtered failed");
+        (0..cnt as usize).map(|j| Neighbour { d_id: ids[j] as usize, distance: ds[j], p_id: PointId(pid[2 * j] as u8, pid[2 * j + 1]) }).collect()
+    }
     /// hnsw.rs:1612-1635: one answer per request, in input order
     pub fn parallel_search(&self, datas: &[Vec<f32>], knbn: usize, ef: usize) -> Vec<Vec<Neighbour>> {
         if datas.is_empty() { return Vec::new(); }
@@ -183,6 +217,19 @@ impl<D: DistName> Hnsw<D> {
 
 impl<D: DistName> Drop for Hnsw<D> {
     fn drop(&mut self) { unsafe { drop_hnsw_f32(self.h) } }
+}
+
+/// A filter made by `Hnsw::make_filter`; it borrows its index and is freed when dropped (the drop waits for searches that
+/// may still read it, so collect this thread's own submitted batches first).
+pub struct ResidentFilter<'a, D: DistName> {
+    index: &'a Hnsw<D>,
+    id: i64,
+}
+impl<'a, D: DistName> ResidentFilter<'a, D> {
+    pub fn id(&self) -> i64 { self.id }
+}
+impl<'a, D: DistName> Drop for ResidentFilter<'a, D> {
+    fn drop(&mut self) { unsafe { hnsw_b200_filter_free(self.index.h, self.id); } }
 }
 
 /// api.rs:13-38

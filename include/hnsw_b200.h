@@ -273,6 +273,41 @@ int hnsw_b200_search_flat_wait(const void* h, int64_t ticket);
 int hnsw_b200_search_device(const void* h, const void* d_queries, uint64_t nq, uint64_t knbn,
                             uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms);
 
+/* ---- Resident filters: a FilterT materialised once, kept on the device, and passed by id to every search path.
+ * hnsw_b200_search_flat rebuilds its filter bitmap on the calling thread (one binary search or one callback call per
+ * stored point) and uploads it on every call; a resident filter does that work once.
+ *
+ * hnsw_b200_filter_new: filter_mode 1 = sorted origin-id list (filter_ids / nfilter), 2 = predicate, called once per
+ * stored point, on the calling thread, during this call only.  Returns a filter id >= 0, valid for this handle only,
+ * or < 0 on error.  The bitmap is copied to the handle's device (every partition's) now; a replica's device gets its
+ * copy at the first sharded search there, also when hnsw_b200_replicate is called after the filter was made.  No
+ * search uploads it again.
+ *   Answers: a search with filter F returns, bit for bit, what hnsw_b200_search_flat returns for the filter arguments F
+ *     was made from (ids, distances, internal ids, PointIds, counts, statistics): the same filtered kernel, the same
+ *     post-filter.  Like every filtered search it ignores the tie mode.
+ *   Snapshot: F covers the points stored when it was made (on a partitioned handle, each partition's).  Once an insert
+ *     or import has changed that count, every search with F is refused with a message saying so; make a new filter.
+ *   Ids: a freed id, an unknown id or another handle's id is refused and nothing is read.
+ *   Freeing: hnsw_b200_filter_free waits for every search that may still read F (searches of other threads, submitted
+ *     batches, asynchronous search_device launches), then frees it.  As before an insert, a thread must collect its own
+ *     tickets before it frees a filter.  hnsw_b200_drop frees every filter of the handle.
+ *   Partitioned handles: filter_new makes one bitmap per partition (a callback still runs once per stored point in
+ *     all); search_flat_filtered merges like an unfiltered search.  submit_filtered and search_device_filtered are
+ *     refused there, as their unfiltered twins are.  filter_new on a partition view is refused.
+ * Every other argument and output of the _filtered calls is that of its unfiltered twin; a submit_filtered ticket is
+ * collected by hnsw_b200_search_flat_wait. */
+int64_t hnsw_b200_filter_new(const void* h, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,
+                             hnsw_b200_filter_fn fn, void* ctx);
+int hnsw_b200_filter_free(const void* h, int64_t filter);
+int hnsw_b200_search_flat_filtered(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim,
+                                   uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
+                                   uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
+int64_t hnsw_b200_search_flat_submit_filtered(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim,
+                                              uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
+                                              uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
+int hnsw_b200_search_device_filtered(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
+                                     uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms);
+
 /* Run this handle's kernels and copies on a caller-owned CUDA stream (cudaStream_t passed as void*; NULL
  * restores the handle's own stream), e.g. so that torch.cuda.Event on torch's current stream brackets them. */
 int hnsw_b200_join(void* h);
