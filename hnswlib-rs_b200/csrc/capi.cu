@@ -15,6 +15,8 @@
 using hb::Index;
 using hb::NeighbourOut;
 using hb::AnswerArrays;
+using hb::FilterArg;
+using hb::HostBatch;
 
 // every typed handle of libext.rs (HnswApif32, HnswApii32, HnswApiu32, HnswApiu16, HnswApiu8) has this layout
 struct HnswApif32 { Index* ix; };
@@ -59,6 +61,8 @@ static int pass(Index* ix, int r) {
 #define HB_NOT_PARTITIONED(ix, what) \
   if ((ix)->parts) return set_err(std::string(what) + " is not available on a partitioned handle")
 #define HB_PARTS_SHARED(ix) const auto pl__ = (ix)->parts->lock_shared()
+#define HB_PARTS_SHARED_IF(ix) \
+  const auto pl__ = (ix)->parts ? (ix)->parts->lock_shared() : std::vector<std::shared_lock<std::shared_mutex>>()
 #define HB_PARTS_EXCLUSIVE(ix) const auto pl__ = (ix)->parts->lock_exclusive()
 
 // a setting: on a partitioned handle it is applied to the handle and to every partition
@@ -154,19 +158,11 @@ static const Neighbourhood_api* search_any(const void* hv, size_t len, const voi
     return nullptr;
   }
   std::shared_lock<std::shared_mutex> g(h->ix->mu);
+  HB_PARTS_SHARED_IF(h->ix);
   Neighbour_api* nb = (Neighbour_api*)malloc(sizeof(Neighbour_api) * knbn);
   int32_t cnt = 0;
-  int rc;
-  if (h->ix->parts) {
-    HB_PARTS_SHARED(h->ix);
-    AnswerArrays out;
-    out.nb = (NeighbourOut*)nb;
-    out.counts = &cnt;
-    rc = h->ix->parts->search(data, nullptr, 1, (int)len, knbn, ef_search, 0, nullptr, 0, nullptr, nullptr, nullptr, out);
-  } else {
-    rc = h->ix->search_host(data, nullptr, 1, (int)len, knbn, ef_search, nullptr, (NeighbourOut*)nb, &cnt);
-  }
-  if (pass(h->ix, rc)) {
+  const AnswerArrays ans{(NeighbourOut*)nb, nullptr, nullptr, nullptr, nullptr, &cnt};
+  if (pass(h->ix, h->ix->search_batch(HostBatch{data, nullptr, 1, (int)len, knbn, ef_search, FilterArg(), ans}))) {
     free(nb);
     return nullptr;
   }
@@ -175,9 +171,6 @@ static const Neighbourhood_api* search_any(const void* hv, size_t len, const voi
   out->neighbours = nb;
   return out;
 }
-
-// a batch is split over the replicas when there are any and every device gets a worthwhile share
-static bool use_shards(const Index* ix, size_t nq) { return ix->replica_count() > 0 && nq >= 64 * (ix->replica_count() + 1); }
 
 struct VecApiBox {
   Vec_api_Neighbourhood_api v;  // first member: the pointer handed to the caller
@@ -193,28 +186,14 @@ static const Vec_api_Neighbourhood_api* parallel_search_any(const void* hv, size
     return nullptr;
   }
   std::shared_lock<std::shared_mutex> g(h->ix->mu);
+  HB_PARTS_SHARED_IF(h->ix);
   VecApiBox* box = (VecApiBox*)malloc(sizeof(VecApiBox));
   box->hoods = (Neighbourhood_api*)malloc(sizeof(Neighbourhood_api) * (nb_vec ? nb_vec : 1));
   box->block = (Neighbour_api*)malloc(sizeof(Neighbour_api) * (nb_vec ? nb_vec * knbn : 1));
   std::vector<int32_t> cnt(nb_vec);
-  int rc;
-  if (h->ix->parts) {
-    HB_PARTS_SHARED(h->ix);
-    AnswerArrays out;
-    out.nb = (NeighbourOut*)box->block;
-    out.counts = cnt.data();
-    rc = h->ix->parts->search(nullptr, data, nb_vec, (int)vec_len, knbn, ef_search, 0, nullptr, 0, nullptr, nullptr, nullptr,
-                                 out);
-  } else if (use_shards(h->ix, nb_vec)) {  // replicas on other GPUs: every device answers its slice of the batch in place
-    NeighbourOut* block = (NeighbourOut*)box->block;
-    int32_t* cp = cnt.data();
-    rc = h->ix->for_each_shard(nb_vec, [=](Index* rx, size_t first, size_t count) {
-      return rx->search_host(nullptr, data + first, count, (int)vec_len, knbn, ef_search, nullptr, block + first * knbn, cp + first);
-    });
-  } else {
-    rc = h->ix->search_host(nullptr, data, nb_vec, (int)vec_len, knbn, ef_search, nullptr, (NeighbourOut*)box->block, cnt.data());
-  }
-  if (pass(h->ix, rc)) {
+  const AnswerArrays out{(NeighbourOut*)box->block, nullptr, nullptr, nullptr, nullptr, cnt.data()};
+  // with replicas, every device answers its slice of the batch in place
+  if (pass(h->ix, h->ix->search_batch(HostBatch{nullptr, data, nb_vec, (int)vec_len, knbn, ef_search, FilterArg(), out}))) {
     free(box->hoods);
     free(box->block);
     free(box);
@@ -601,20 +580,6 @@ int hnsw_b200_insert_flat(void* h, const void* vecs, uint64_t n, uint64_t dim, c
   return pass(ix, ix->insert_batch(vecs, n, dim, nullptr, ids, levels));
 }
 
-// answers of nq queries (k slots each, as the kernels left them) into the caller's arrays; internal ids and PointIds are
-// optional.  The kernels fill the slots beyond a query's count with (~0, +inf, INVALID_ID): plain field copies.
-static void unpack_answers(const Index* rx, const NeighbourOut* a, const int32_t* cnts, uint64_t nq, uint64_t k, uint64_t* ids,
-                           float* dist, uint32_t* internal, int32_t* pid, int32_t* counts) {
-  memcpy(counts, cnts, nq * sizeof(int32_t));
-  const uint64_t tot = nq * k;
-  for (uint64_t s = 0; s < tot; ++s) ids[s] = a[s].origin;
-  for (uint64_t s = 0; s < tot; ++s) dist[s] = a[s].dist;
-  if (internal)
-    for (uint64_t s = 0; s < tot; ++s) internal[s] = a[s].internal;
-  if (pid)
-    for (uint64_t s = 0; s < tot; ++s) hb::point_id(rx, a[s].internal, pid + 2 * s);
-}
-
 // hnsw_b200_search_flat and _search_flat_filtered: the filter is the FilterT arguments (filter_mode 1, 2) or, when
 // `resident` is set, one of the handle's resident filters (filter_mode 0).  The kernels and the answers are the same.
 static int search_flat_any(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
@@ -624,41 +589,10 @@ static int search_flat_any(const void* h, const void* queries, uint64_t nq, uint
   HB_HS(h);
   if (nq == 0) return 0;
   if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0) return set_err("bad argument");
-  if (ix->parts) {  // every query on every partition, the answers merged straight into the caller's arrays
-    HB_PARTS_SHARED(ix);
-    AnswerArrays out;
-    out.ids = out_ids;
-    out.dist = out_dist;
-    out.internal = out_internal;
-    out.pid = out_pid;
-    out.counts = out_counts;
-    return pass(ix, ix->parts->search(queries, nullptr, nq, (int)dim, knbn, ef_search, filter_mode, filter_ids, nfilter, fn,
-                                      ctx, resident, out));
-  }
-  std::vector<uint32_t> bits;
-  const uint32_t* fb = nullptr;
-  if (filter_mode) {
-    int r = pass(ix, ix->make_filter_bits(filter_mode, filter_ids, nfilter, fn, ctx, bits));
-    if (r) return r;
-    fb = bits.data();
-  }
-  // one device, or one contiguous shard per device: search, then unpack the shard's answers into the caller's arrays
-  const size_t qrow = (size_t)dim * ix->es;
-  auto run = [=](Index* rx, size_t first, size_t count) -> int {
-    const NeighbourOut* tmp = nullptr;
-    const int32_t* cnts = nullptr;
-    const uint32_t* dfb = nullptr;  // a resident filter's copy on rx's device
-    if (resident && ix->filters.use(*resident, 0, 1, rx, &dfb)) return -1;
-    Index::CtxLease lease(rx);  // the answers stay in the context's pinned buffer until they are unpacked below
-    int r = rx->search_host_staged(lease.c, (const char*)queries + first * qrow, nullptr, count, (int)dim, knbn, ef_search, fb,
-                                   dfb, &tmp, &cnts);
-    if (r) return r;
-    const uint64_t o0 = first * knbn;
-    unpack_answers(rx, tmp, cnts, count, knbn, out_ids + o0, out_dist + o0, out_internal ? out_internal + o0 : nullptr,
-                   out_pid ? out_pid + 2 * o0 : nullptr, out_counts + first);
-    return 0;
-  };
-  return pass(ix, use_shards(ix, nq) ? ix->for_each_shard(nq, run) : run(ix, 0, nq));
+  HB_PARTS_SHARED_IF(ix);
+  const FilterArg f{filter_mode, filter_ids, nfilter, fn, ctx, resident};
+  const AnswerArrays out{nullptr, out_ids, out_dist, out_internal, out_pid, out_counts};
+  return pass(ix, ix->search_batch(HostBatch{queries, nullptr, nq, (int)dim, knbn, ef_search, f, out}));
 }
 
 int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
@@ -675,37 +609,6 @@ int hnsw_b200_search_flat_filtered(const void* h, int64_t filter, const void* qu
                          out_internal, out_pid, out_counts);
 }
 
-// one device's share of a submitted batch: enqueue on a leased context of `rx`, remember where to unpack to
-static int submit_on(Index* rx, int* ctx_out, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
-                     const uint32_t* d_filter_bits, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
-                     int32_t* out_pid, int32_t* out_counts) {
-  const int ci = rx->acquire_ctx();
-  int r = rx->search_host_begin(ci, queries, nullptr, nq, (int)dim, knbn, ef_search, nullptr, d_filter_bits);
-  if (r) {
-    rx->release_ctx(ci);
-    return r;
-  }
-  Index::SearchCtx::Pending& p = rx->ctx(ci).pend;
-  p.u_ids = out_ids;
-  p.u_dist = out_dist;
-  p.u_internal = out_internal;
-  p.u_pid = out_pid;
-  p.u_counts = out_counts;
-  *ctx_out = ci;
-  return 0;
-}
-static int wait_on(Index* rx, int ci) {
-  const NeighbourOut* tmp = nullptr;
-  const int32_t* cnts = nullptr;
-  int r = rx->search_host_finish(ci, &tmp, &cnts);
-  if (!r) {
-    const Index::SearchCtx::Pending& p = rx->ctx(ci).pend;
-    unpack_answers(rx, tmp, cnts, p.nq, p.k, p.u_ids, p.u_dist, p.u_internal, p.u_pid, p.u_counts);
-  }
-  rx->release_ctx(ci);
-  return r;
-}
-
 // Submit / wait: the same search with the call split in two, so that one host thread keeps several batches in flight
 // (batch i+1 is enqueued before batch i's answers are collected).  Unfiltered, or with a resident filter.  With replicas
 // (hnsw_b200_replicate) the batch is sharded like a search_flat call: every device gets its contiguous share enqueued at
@@ -716,25 +619,11 @@ static int64_t submit_any(const void* h, const int64_t* resident, const void* qu
   HB_HS(h);
   HB_NOT_PARTITIONED(ix, resident ? "search_flat_submit_filtered" : "search_flat_submit");
   if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0 || nq == 0) return set_err("bad argument");
-  Index::Ticket t;
-  const size_t qrow = (size_t)dim * ix->es;
-  auto run = [&](Index* rx, size_t first, size_t count) -> int {
-    const uint32_t* dfb = nullptr;
-    if (resident && ix->filters.use(*resident, 0, 1, rx, &dfb)) return -1;
-    int ci = -1;
-    int r = submit_on(rx, &ci, (const char*)queries + first * qrow, count, dim, knbn, ef_search, dfb, out_ids + first * knbn,
-                      out_dist + first * knbn, out_internal ? out_internal + first * knbn : nullptr,
-                      out_pid ? out_pid + 2 * first * knbn : nullptr, out_counts + first);
-    if (!r) t.parts.push_back({rx, ci});
-    return r;
-  };
-  const int r = use_shards(ix, nq) ? ix->for_each_shard_inline(nq, run) : run(ix, 0, nq);
-  if (r) {
-    for (auto& pr : t.parts) wait_on(pr.first, pr.second);  // collect what was enqueued before the failure
-    return pass(ix, r);
-  }
-  ix->pending_.fetch_add(1);
-  return ix->park_ticket(std::move(t));
+  const FilterArg f{0, nullptr, 0, nullptr, nullptr, resident};
+  const AnswerArrays out{nullptr, out_ids, out_dist, out_internal, out_pid, out_counts};
+  const int64_t t = ix->submit_batch(HostBatch{queries, nullptr, nq, (int)dim, knbn, ef_search, f, out});
+  if (t < 0) g_err = ix->err();
+  return t;
 }
 
 int64_t hnsw_b200_search_flat_submit(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
@@ -754,16 +643,7 @@ int hnsw_b200_search_flat_wait(const void* h, int64_t ticket) {
   hb::DeviceRestore keep;
   Index::Ticket t;
   if (!ix->take_ticket(ticket, t)) return set_err("bad ticket");
-  int r = 0;
-  if (t.parts.size() > 1) {  // sharded batch: every device's part is collected and unpacked by that device's worker thread
-    r = ix->finish_parts(t.parts, [](Index* rx, int ci) { return wait_on(rx, ci); });
-    if (r) g_err = ix->err();
-  } else {
-    for (auto& pr : t.parts) {
-      r = wait_on(pr.first, pr.second);
-      if (r) g_err = pr.first->err();
-    }
-  }
+  const int r = pass(ix, ix->finish_batch(t));  // sharded: every replica's leg is collected by that replica's worker
   ix->pending_.fetch_sub(1);
   return r;
 }
@@ -772,9 +652,8 @@ static int search_device_any(const void* h, const int64_t* resident, const void*
                              uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
   HB_HS(h);
   HB_NOT_PARTITIONED(ix, resident ? "search_device_filtered" : "search_device");
-  const uint32_t* dfb = nullptr;
-  if (resident && ix->filters.use(*resident, 0, 1, ix, &dfb)) return pass(ix, -1);
-  return pass(ix, ix->search_device(d_queries, nq, knbn, ef_search, dfb, (NeighbourOut*)d_out, d_counts, sync != 0, kernel_ms));
+  const FilterArg f{0, nullptr, 0, nullptr, nullptr, resident};
+  return pass(ix, ix->search_device(f, d_queries, nq, knbn, ef_search, (NeighbourOut*)d_out, d_counts, sync != 0, kernel_ms));
 }
 int hnsw_b200_search_device(const void* h, const void* d_queries, uint64_t nq, uint64_t knbn,
                             uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {

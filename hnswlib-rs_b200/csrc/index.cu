@@ -614,8 +614,13 @@ void Index::release_ctx(int c) {
 // context streams, so that two consecutive launches overlap.  The handle's stream does NOT wait for it: join() (or
 // check_status, set_stream, any synchronous call's own synchronisation) makes it do so; stream_wait_last() makes any
 // stream wait for the most recent launch alone.
-int Index::search_device(const void* d_queries, size_t nq, size_t k, size_t ef_arg, const uint32_t* d_filter_bits,
-                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms) {
+int Index::search_device(const FilterArg& f, const void* d_queries, size_t nq, size_t k, size_t ef_arg, NeighbourOut* d_out,
+                         int32_t* d_counts, bool sync, float* kernel_ms) {
+  Leg leg{this};
+  std::vector<std::vector<uint32_t>> bits;
+  int r;
+  if (resolve_filter(f, &leg, 1, bits)) return legs_fail(&leg, 1, false);
+  const uint32_t* d_filter_bits = leg.dev_bits;
   if (nq == 0) return 0;
   HB_CUDA(cudaSetDevice(device));
   if (sync) {
@@ -633,7 +638,7 @@ int Index::search_device(const void* d_queries, size_t nq, size_t k, size_t ef_a
   SearchCtx& c = ctx_[ci];
   HB_CUDA(cudaEventRecord(c.fork, stream_));
   HB_CUDA(cudaStreamWaitEvent(c.stream, c.fork, 0));
-  int r = search_on_ctx(c, d_queries, nq, k, ef_arg, d_filter_bits, d_out, d_counts, false, nullptr);
+  r = search_on_ctx(c, d_queries, nq, k, ef_arg, d_filter_bits, d_out, d_counts, false, nullptr);
   if (r) return r;
   HB_CUDA(cudaEventRecord(c.join, c.stream));
   last_async_ = ci;
@@ -847,28 +852,6 @@ int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** 
   if (*p.hstatus == 0) return 0;
   HB_CUDA(cudaMemsetAsync(c.d_status, 0, sizeof(int), st));
   return search_on_ctx(c, p.d_queries, p.nq, p.k, p.ef, p.dfb, p.k_out, p.k_cnt, true, nullptr);  // grows the tables
-}
-
-int Index::search_host_staged(int ci, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                              const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const NeighbourOut** out,
-                              const int32_t** counts) {
-  *out = nullptr;
-  *counts = nullptr;
-  int r = search_host_begin(ci, queries, rows, nq, d, k, ef, filter_bits_host, d_filter_bits);
-  if (r) return r;
-  return search_host_finish(ci, out, counts);
-}
-
-int Index::search_host(const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                       const uint32_t* filter_bits_host, NeighbourOut* out, int32_t* counts) {
-  CtxLease lease(this);
-  const NeighbourOut* so;
-  const int32_t* sc;
-  int r = search_host_staged(lease.c, queries, rows, nq, d, k, ef, filter_bits_host, nullptr, &so, &sc);
-  if (r || nq == 0) return r;
-  memcpy(counts, sc, nq * sizeof(int32_t));
-  memcpy(out, so, nq * k * sizeof(NeighbourOut));
-  return 0;
 }
 
 int Index::make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx,

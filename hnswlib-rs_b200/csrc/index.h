@@ -137,6 +137,80 @@ struct PartitionsDeleter {
   void operator()(Partitions* p) const;
 };
 
+// One thread that runs the closures its owner hands it, one at a time.
+struct Worker {
+  std::thread th;
+  std::mutex m;
+  std::condition_variable cv;
+  std::function<void()> job;
+  bool has_job = false, done = true, quit = false;
+  Worker();
+  ~Worker();
+  void submit(std::function<void()> j);
+  void wait();
+};
+
+// The worker threads of a fan-out over devices (replicas) or partitions: run(n, job) runs job(0) on the calling thread
+// and job(i) on worker i - 1, all at once, waits for every one and returns the first i whose job failed (-1: none).
+// One run at a time (a worker holds one job); `mu` is the lock run takes.
+class WorkerGroup {
+ public:
+  void resize(size_t n);  // n workers
+  int run(int n, const std::function<int(int)>& job);
+  std::mutex mu;
+
+ private:
+  std::vector<std::unique_ptr<Worker>> w_;
+};
+
+// ---- host searches (host_search.cu)
+// Where a host search writes its [nq][k] answer slots and counts[nq]: either the reference entry points' answer blocks
+// (`nb`: Neighbour_api with the internal id in its tail padding) or hnsw_b200_search_flat's arrays (internal and pid
+// optional).
+struct AnswerArrays {
+  NeighbourOut* nb = nullptr;
+  uint64_t* ids = nullptr;
+  float* dist = nullptr;
+  uint32_t* internal = nullptr;
+  int32_t* pid = nullptr;
+  int32_t* counts = nullptr;
+};
+
+// The filter of a search: none, a FilterT (mode != 0, as make_filter_bits reads it: 1 sorted origin-id list, 2 callback),
+// or one of the handle's resident filters (the id *resident).
+struct FilterArg {
+  int mode = 0;
+  const uint64_t* ids = nullptr;
+  size_t nids = 0;
+  int (*fn)(uint64_t, void*) = nullptr;
+  void* ctx = nullptr;
+  const int64_t* resident = nullptr;
+};
+
+// One host search batch: flat queries or one pointer per query (rows), k answers each into `out`
+struct HostBatch {
+  const void* queries = nullptr;
+  const void* const* rows = nullptr;
+  size_t nq = 0;
+  int d = 0;
+  size_t k = 0, ef = 0;
+  FilterArg filter;
+  AnswerArrays out;
+};
+
+// One Index's part of a batch: queries [first, first + count) searched on rx (the handle, a replica, or partition `part`)
+// on its leased context ctx, with the filter bits resolve_filter gave it
+struct Leg {
+  Index* rx = nullptr;
+  int part = 0;
+  size_t first = 0, count = 0;
+  int ctx = -1;  // -1: not leased
+  const uint32_t* host_bits = nullptr;
+  const uint32_t* dev_bits = nullptr;
+  bool begun = false;  // enqueued
+  int rc = 0;
+};
+
 class Index {
  public:
   Index(int M, size_t max_elements, int max_layer, int ef_c, int metric, int dtype, int device);
@@ -172,25 +246,33 @@ class Index {
   int import_graph(const void* vecs, size_t n_new, int d, const uint64_t* origin, const uint8_t* levels,
                    int64_t entry_id, int nlayers, const uint64_t* const* offsets, const uint32_t* const* ids,
                    const float* const* dists);
-  // host queries (flat or row pointers); results to host NeighbourOut[nq][k] + counts
-  int search_host(const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                  const uint32_t* filter_bits_host, NeighbourOut* out, int32_t* counts);
-  // same on context c (a CtxLease), answers left in the context's pinned buffer (valid until the lease ends).  The filter
-  // is either host bits, uploaded into the context for this call, or d_filter_bits already on this device (a resident
-  // filter); at most one of the two is non-null.
+  // host queries (flat or row pointers) on leased context c, answers left in the context's pinned buffer (valid until
+  // it is released).  The filter is either host bits, uploaded into the context for this call, or d_filter_bits already
+  // on this device (a resident filter); at most one of the two is non-null.
   int search_host_begin(int c, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
                         const uint32_t* filter_bits_host, const uint32_t* d_filter_bits);
   int search_host_finish(int c, const NeighbourOut** out, const int32_t** counts);
+  // host search batches (host_search.cu): synchronous, or submitted now and collected by finish_batch
+  struct Ticket {
+    std::vector<Leg> legs;
+    size_t k = 0;
+    AnswerArrays out;
+  };
+  int search_batch(const HostBatch& b);
+  int64_t submit_batch(const HostBatch& b);  // a ticket id, or < 0
+  int finish_batch(Ticket& t);
   // submitted-but-not-waited host searches: anything that changes the graph waits for them (drain_pending)
   std::atomic<int> pending_{0};
   void drain_pending() const {
     while (pending_.load() != 0) std::this_thread::yield();
   }
-  int search_host_staged(int c, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                         const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const NeighbourOut** out,
-                         const int32_t** counts);
-  int search_device(const void* d_queries, size_t nq, size_t k, size_t ef, const uint32_t* d_filter_bits,
-                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms);
+  // the filter bits of legs[0, n): a FilterT's host bits, made on the calling thread once per partition (a replica
+  // shares the handle's internal ids, and so its bits) into `bits`, or a resident filter's copy on each leg's device.
+  // Nonzero when a leg could not have them; that leg's rc is set (legs_fail reports it).
+  int resolve_filter(const FilterArg& f, Leg* legs, size_t n, std::vector<std::vector<uint32_t>>& bits);
+  // device queries in, device answers out; the filter is none or a resident filter
+  int search_device(const FilterArg& f, const void* d_queries, size_t nq, size_t k, size_t ef, NeighbourOut* d_out,
+                    int32_t* d_counts, bool sync, float* kernel_ms);
   // filter materialisation: bit per internal id from a sorted origin-id list or a callback
   int make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx,
                        std::vector<uint32_t>& bits) const;
@@ -220,30 +302,10 @@ class Index {
   int blob_commit();
 
   // ---- multi-GPU (multi.cu).  One process, N devices: replicate() builds a copy of the frozen index on every listed
-  // device (NCCL broadcast) and for_each_shard() runs a batch split into contiguous shards, one worker thread per
-  // device.  One process per GPU: nccl_init() + nccl_broadcast_index() + nccl_allgather().
+  // device (NCCL broadcast), and a host search batch is split into contiguous shards over them, one worker thread per
+  // device (host_search.cu).  One process per GPU: nccl_init() + nccl_broadcast_index() + nccl_allgather().
   int replicate(int ndev, const int* devices);
   size_t replica_count() const { return replicas_.size(); }
-  int for_each_shard(size_t nq, const std::function<int(Index*, size_t, size_t)>& run);
-  // same shards, visited one after the other on the calling thread (asynchronous enqueues: submit)
-  int for_each_shard_inline(size_t nq, const std::function<int(Index*, size_t, size_t)>& run);
-  // outstanding submit tickets: (index, context) per device
-  struct Ticket {
-    std::vector<std::pair<Index*, int>> parts;
-  };
-  int finish_parts(const std::vector<std::pair<Index*, int>>& parts, const std::function<int(Index*, int)>& fn);
-  // One thread that runs the closures its owner hands it, one at a time (replicas here, partitions in partition.cu).
-  struct Worker {
-    std::thread th;
-    std::mutex m;
-    std::condition_variable cv;
-    std::function<void()> job;
-    bool has_job = false, done = true, quit = false;
-    Worker();
-    ~Worker();
-    void submit(std::function<void()> j);
-    void wait();
-  };
   int64_t park_ticket(Ticket&& t);
   bool take_ticket(int64_t id, Ticket& out);
   void drop_replicas();
@@ -282,11 +344,6 @@ class Index {
       int32_t *k_cnt = nullptr, *hcnt = nullptr, *hstatus = nullptr;
       size_t nq = 0, k = 0, ef = 0;
       bool enqueued = false;
-      // where hnsw_b200_search_flat_wait unpacks to
-      uint64_t* u_ids = nullptr;
-      float* u_dist = nullptr;
-      uint32_t* u_internal = nullptr;
-      int32_t *u_pid = nullptr, *u_counts = nullptr;
     } pend;
   };
   static constexpr int NCTX = 4;    // leased by synchronous calls (host threads)
@@ -294,7 +351,7 @@ class Index {
   int acquire_ctx();            // blocks until a context is free
   void release_ctx(int c);
   SearchCtx& ctx(int c) { return ctx_[c]; }
-  struct CtxLease {             // RAII: answers returned by search_host_staged live in the context until release
+  struct CtxLease {             // RAII: a context leased for the scope
     Index* ix;
     int c;
     explicit CtxLease(Index* i) : ix(i), c(i->acquire_ctx()) {}
@@ -363,12 +420,16 @@ class Index {
   int check_insert_fit();
   void rollback_points(size_t keep);
 
-  struct WorkerDeleter {
-    void operator()(Worker* w) const;
-  };
+  // ---- host search batches (host_search.cu)
+  int plan(size_t nq, std::vector<Leg>& legs);
+  void begin_leg(const HostBatch& b, Leg& l);
+  void release_leg(Leg& l);
+  int end_leg(Leg& l, size_t k, const AnswerArrays& out);
+  int legs_fail(const Leg* legs, size_t n, bool replicas_first);
+
   int broadcast_to_replicas();
   std::vector<std::unique_ptr<Index>> replicas_;  // replicas_[i] lives on replica_devices_[i + 1]
-  std::vector<std::unique_ptr<Worker, WorkerDeleter>> workers_;
+  WorkerGroup workers_;                           // worker i serves replicas_[i]
   std::vector<void*> comms_;                      // ncclComm_t per device, rank 0 = this index
   std::vector<int> replica_devices_;
   bool replicas_stale_ = false;                   // the index changed after the last broadcast
@@ -391,7 +452,7 @@ class Index {
                     NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms);
   std::mutex ctx_mu_;
   std::condition_variable ctx_cv_;
-  std::mutex ticket_mu_, shard_mu_;
+  std::mutex ticket_mu_;
   std::map<int64_t, Ticket> tickets_;
   int64_t next_ticket_ = 0;
   int last_async_ = -1;

@@ -4,9 +4,9 @@
 // host's cores; here the same call fans it out over the GPUs of the box.  Two ways to get the replicas:
 //   * one process, N devices (hnsw_b200_replicate): the library creates a replica Index per extra device, one
 //     ncclCommInitAll communicator, and broadcasts every blob of the frozen index with grouped ncclBroadcast calls
-//     over NVLink.  Afterwards search_flat / parallel_search_neighbours_<ty> split the batch into contiguous shards,
-//     one worker thread per device runs its shard (H2D, kernel, D2H) and writes its slice of the caller's output:
-//     no result gather at all for host results;
+//     over NVLink.  Afterwards search_flat / parallel_search_neighbours_<ty> split the batch into contiguous shards
+//     (host_search.cu): one worker thread per device runs its shard (H2D, kernel, D2H) and writes its slice of the
+//     caller's output, so there is no result gather at all for host results;
 //   * one process per GPU (hnsw_b200_nccl_*): the host exchanges an ncclUniqueId by its own means (MPI, a TCP store,
 //     torch.distributed ...), every rank opens the communicator on its handle's device, the building rank broadcasts
 //     header + blobs, and device-resident answers can be all-gathered on a caller-chosen stream.
@@ -14,10 +14,6 @@
 // already loaded an NCCL (torch) shares it.
 #include <dlfcn.h>
 #include <nccl.h>
-
-#include <condition_variable>
-#include <functional>
-#include <thread>
 
 #include "index.h"
 
@@ -78,49 +74,9 @@ static NcclApi& nccl() {
     if (r__ != ncclSuccess) return fail(std::string("NCCL error: ") + nccl().GetErrorString(r__) + " at " #call); \
   } while (0)
 
-// ------------------------------------------------------------------------------------------------ worker threads
-// One per replica: runs the closures the owner hands it, on the replica's device.
-Index::Worker::Worker() {
-  th = std::thread([this] {
-    std::unique_lock<std::mutex> lk(m);
-    for (;;) {
-      cv.wait(lk, [this] { return has_job || quit; });
-      if (quit) return;
-      auto j = std::move(job);
-      has_job = false;
-      lk.unlock();
-      j();
-      lk.lock();
-      done = true;
-      cv.notify_all();
-    }
-  });
-}
-void Index::Worker::submit(std::function<void()> j) {
-  std::unique_lock<std::mutex> lk(m);
-  job = std::move(j);
-  has_job = true;
-  done = false;
-  cv.notify_all();
-}
-void Index::Worker::wait() {
-  std::unique_lock<std::mutex> lk(m);
-  cv.wait(lk, [this] { return done; });
-}
-Index::Worker::~Worker() {
-  {
-    std::unique_lock<std::mutex> lk(m);
-    quit = true;
-    cv.notify_all();
-  }
-  th.join();
-}
-
-void Index::WorkerDeleter::operator()(Worker* w) const { delete w; }
-
 void Index::drop_replicas() {
   DeviceRestore keep;
-  workers_.clear();
+  workers_.resize(0);
   if (nccl().ok)
     for (void* c : comms_)
       if (c) nccl().CommDestroy((ncclComm_t)c);
@@ -208,7 +164,7 @@ int Index::replicate(int ndev, const int* devices) {
     return fail(std::string("replicate: ncclCommInitAll: ") + nc.GetErrorString(ir));
   }
   comms_.assign(cs.begin(), cs.end());
-  for (int i = 1; i < ndev; ++i) workers_.emplace_back(new Worker());  // NOLINT: owned by workers_
+  workers_.resize(ndev - 1);
   int r = broadcast_to_replicas();
   if (r) drop_replicas();
   HB_CUDA(cudaSetDevice(device));
@@ -229,79 +185,6 @@ bool Index::take_ticket(int64_t id, Ticket& out) {
   out = std::move(it->second);
   tickets_.erase(it);
   return true;
-}
-
-// the parts of a submitted batch finished in parallel: part (replica i, ctx) on replica i's worker thread, the root's part on
-// the calling thread
-int Index::finish_parts(const std::vector<std::pair<Index*, int>>& parts, const std::function<int(Index*, int)>& fn) {
-  DeviceRestore keep;
-  std::lock_guard<std::mutex> one(shard_mu_);
-  std::vector<int> rc(parts.size(), 0);
-  std::vector<Worker*> used;
-  int own = -1;
-  for (size_t k = 0; k < parts.size(); ++k) {
-    Worker* w = nullptr;
-    for (size_t i = 0; i < replicas_.size(); ++i)
-      if (replicas_[i].get() == parts[k].first) w = workers_[i].get();
-    if (!w) {
-      own = (int)k;
-      continue;
-    }
-    int* out = &rc[k];
-    Index* rx = parts[k].first;
-    const int ci = parts[k].second;
-    w->submit([=, &fn] { *out = fn(rx, ci); });
-    used.push_back(w);
-  }
-  if (own >= 0) rc[own] = fn(parts[own].first, parts[own].second);
-  for (Worker* w : used) w->wait();
-  for (size_t k = 0; k < parts.size(); ++k)
-    if (rc[k]) return parts[k].first == this ? rc[k] : fail("device " + std::to_string(parts[k].first->device) + ": " + parts[k].first->err());
-  return 0;
-}
-
-int Index::for_each_shard_inline(size_t nq, const std::function<int(Index*, size_t, size_t)>& run) {
-  DeviceRestore keep;
-  std::lock_guard<std::mutex> one(shard_mu_);
-  if (replicas_stale_) {
-    int r = broadcast_to_replicas();
-    if (r) return r;
-  }
-  const size_t ndev = replicas_.size() + 1;
-  const size_t per = (nq + ndev - 1) / ndev;
-  for (size_t i = 0; i < ndev; ++i) {
-    const size_t first = std::min(nq, i * per), count = std::min(nq, (i + 1) * per) - first;
-    if (!count) continue;
-    Index* rx = i == 0 ? this : replicas_[i - 1].get();
-    int r = run(rx, first, count);
-    if (r) return i == 0 ? r : fail("device " + std::to_string(rx->device) + ": " + rx->err());
-  }
-  return 0;
-}
-
-// Contiguous shards, one per device; shard 0 runs on the calling thread.  `run` is called as run(index, first, count).
-int Index::for_each_shard(size_t nq, const std::function<int(Index*, size_t, size_t)>& run) {
-  DeviceRestore keep;
-  std::lock_guard<std::mutex> one(shard_mu_);  // one sharded call at a time: the workers hold one job each
-  if (replicas_stale_) {
-    int r = broadcast_to_replicas();
-    if (r) return r;
-  }
-  const size_t ndev = replicas_.size() + 1;
-  const size_t per = (nq + ndev - 1) / ndev;
-  std::vector<int> rc(ndev, 0);
-  for (size_t i = 1; i < ndev; ++i) {
-    const size_t first = std::min(nq, i * per), count = std::min(nq, (i + 1) * per) - first;
-    Index* rep = replicas_[i - 1].get();
-    int* out = &rc[i];
-    workers_[i - 1]->submit([=, &run] { *out = count ? run(rep, first, count) : 0; });
-  }
-  rc[0] = run(this, 0, std::min(nq, per));
-  for (auto& w : workers_) w->wait();
-  cudaSetDevice(device);
-  for (size_t i = 1; i < ndev; ++i)
-    if (rc[i]) return fail("device " + std::to_string(replicas_[i - 1]->device) + ": " + replicas_[i - 1]->err());
-  return rc[0];
 }
 
 // ------------------------------------------------------------------------------------------------ one process per GPU

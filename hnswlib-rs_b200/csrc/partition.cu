@@ -1,6 +1,6 @@
-// Partitioned index (partition.h): placement, the fan-out of inserts and searches over the partitions, and the merge of
-// their answers.  No kernel of its own: every partition runs the ordinary insert and query kernels on its own stream,
-// and the merge reads the answers the kernels wrote to each partition's pinned result buffer.
+// Partitioned index (partition.h): placement, the fan-out of inserts and brute-force searches over the partitions.  No
+// kernel of its own: every partition runs the ordinary insert kernels on its own stream.  Searches run through the host
+// search driver (host_search.cu), which merges the partitions' answers.
 #include "partition.h"
 
 #include <algorithm>
@@ -44,7 +44,7 @@ int Partitions::create(Index* parent, int nparts, const int* devices) {
     ix->owner = parent;
     ps->ix_.push_back(std::move(ix));
   }
-  for (int p = 1; p < nparts; ++p) ps->workers_.emplace_back(new Index::Worker());
+  ps->workers_.resize(nparts - 1);
   for (auto& ix : ps->ix_) ps->views_.push_back(ix.get());
   parent->parts = std::move(ps);
   return 0;
@@ -73,21 +73,6 @@ int Partitions::max_level() const {
   int m = 0;
   for (auto& ix : ix_) m = std::max(m, ix->entry_level);
   return m;
-}
-
-int Partitions::fan_out(const std::function<int(int)>& job) {
-  DeviceRestore keep;
-  std::lock_guard<std::mutex> one(fan_mu_);
-  std::vector<int> rc(count(), 0);
-  for (int p = 1; p < count(); ++p) {
-    int* out = &rc[p];
-    workers_[p - 1]->submit([=, &job] { *out = job(p); });
-  }
-  rc[0] = job(0);
-  for (auto& w : workers_) w->wait();
-  for (int p = 0; p < count(); ++p)
-    if (rc[p]) return fail(p, ix_[p]->err());
-  return 0;
 }
 
 int Partitions::insert(const void* vecs, size_t n_new, size_t stride, const void* const* rows, const uint64_t* ids,
@@ -131,10 +116,11 @@ int Partitions::insert(const void* vecs, size_t n_new, size_t stride, const void
   cudaSetDevice(parent_->device);
   // ---- every partition inserts its share at once
   const size_t row = stride * parent_->es;
-  r = fan_out([&](int p) {
+  const int bad = workers_.run(P, [&](int p) {
     const void* v = rows ? nullptr : (const void*)((const char*)vecs + first[p] * row);
     return ix_[p]->insert_batch(v, share[p], stride * P, rows ? pr[p].data() : nullptr, og[p].data(), pl[p].data());
   });
+  r = bad < 0 ? 0 : fail(bad, ix_[bad]->err());
   if (r) {
     bool unchanged = true;
     for (int p = 0; p < P; ++p) unchanged = unchanged && ix_[p]->n == expected_count(p, before);
@@ -146,107 +132,19 @@ int Partitions::insert(const void* vecs, size_t n_new, size_t stride, const void
   return r;
 }
 
-// Merge rule: the first min(k, sum of counts) entries of the P ascending lists of one query, ordered by (distance,
-// partition, position in that partition's list).  dist(p, i) is entry i of list p; emit(j, p, i) writes output slot j.
-template <class Dist, class Emit>
-static size_t merge_lists(int P, size_t k, const int32_t* cnt, const Dist& dist, const Emit& emit) {
-  int pos[Partitions::MAX_PARTS] = {};
-  size_t total = 0;
-  for (int p = 0; p < P; ++p) total += (size_t)cnt[p];
-  total = std::min(total, k);
-  for (size_t j = 0; j < total; ++j) {
-    int best = -1;
-    float bd = 0.f;
-    for (int p = 0; p < P; ++p) {
-      if (pos[p] >= cnt[p]) continue;
-      const float dp = dist(p, pos[p]);
-      if (best < 0 || dp < bd) {
-        best = p;
-        bd = dp;
-      }
-    }
-    emit(j, best, pos[best]++);
-  }
-  return total;
-}
-
-int Partitions::search(const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef, int filter_mode,
-                       const uint64_t* filter_ids, size_t nfilter, int (*fn)(uint64_t, void*), void* ctx,
-                       const int64_t* resident, const AnswerArrays& out) {
-  if (nq == 0) return 0;
-  if (k == 0) return parent_->fail("knbn must be positive");
-  if (parent_->dim != 0 && d != parent_->dim) return parent_->fail("query length differs from the index dimension");
-  const int P = count();
-  // every partition's filter bitmap: a resident filter's device copy, or host bits made here, on the calling thread (a
-  // FilterT callback need not be thread-safe) and uploaded with the search
-  std::vector<std::vector<uint32_t>> bits(P);
-  std::vector<const uint32_t*> dbits(P, nullptr);
-  for (int p = 0; p < P; ++p) {
-    if (resident && parent_->filters.use(*resident, p, P, ix_[p].get(), &dbits[p])) return fail(p, ix_[p]->err());
-    if (filter_mode && ix_[p]->make_filter_bits(filter_mode, filter_ids, nfilter, fn, ctx, bits[p])) return fail(p, ix_[p]->err());
-  }
-  // one leased context per partition, taken in partition order; the answers stay in them until the merge is done
-  std::vector<int> ci(P, -1);
-  struct Leases {
-    const std::vector<std::unique_ptr<Index>>& ix;
-    std::vector<int>& ci;
-    ~Leases() {
-      for (size_t p = 0; p < ci.size(); ++p)
-        if (ci[p] >= 0) ix[p]->release_ctx(ci[p]);
-    }
-  } leases{ix_, ci};
-  for (int p = 0; p < P; ++p) ci[p] = ix_[p]->acquire_ctx();
-  // enqueue every partition's search, then collect them: the P searches run at once, on one device or several
-  DeviceRestore keep;
-  int failed = -1, begun = 0;
-  for (; begun < P; ++begun)
-    if (ix_[begun]->search_host_begin(ci[begun], queries, rows, nq, d, k, ef, filter_mode ? bits[begun].data() : nullptr,
-                                      dbits[begun])) {
-      failed = begun;
-      break;
-    }
-  std::vector<const NeighbourOut*> a(P);
-  std::vector<const int32_t*> c(P);
-  for (int p = 0; p < begun; ++p) {  // every enqueued search is collected, also after a failure
-    const int rp = ix_[p]->search_host_finish(ci[p], &a[p], &c[p]);
-    if (rp && failed < 0) failed = p;
-  }
-  if (begun < P) {  // the partition whose enqueue failed: nothing of it may still run once its context is released
-    cudaSetDevice(ix_[begun]->device);
-    cudaStreamSynchronize(ix_[begun]->ctx(ci[begun]).stream);
-  }
-  if (failed >= 0) return fail(failed, ix_[failed]->err());
-  // merge on the calling thread, straight into the caller's arrays
-  const NeighbourOut pad{~0ull, __builtin_inff(), INVALID_ID};
-  int32_t cnt[MAX_PARTS];
-  for (size_t q = 0; q < nq; ++q) {
-    for (int p = 0; p < P; ++p) cnt[p] = c[p][q];
-    const size_t o = q * k;
-    const size_t total = merge_lists(
-        P, k, cnt, [&](int p, int i) { return a[p][o + i].dist; },
-        [&](size_t j, int p, int i) {
-          const NeighbourOut& e = a[p][o + i];
-          put_answer(out, o + j, ix_[p].get(), e, e.internal * (uint32_t)P + (uint32_t)p);
-        });
-    for (size_t j = total; j < k; ++j) put_answer(out, o + j, nullptr, pad, INVALID_ID);
-    out.counts[q] = (int32_t)total;
-  }
-  return 0;
-}
-
 int Partitions::bruteforce(const void* queries, size_t nq, int d, size_t k, uint32_t* out_ids, float* out_dist) {
   if (nq == 0 || k == 0) return 0;
   if (d != parent_->dim) return parent_->fail("query length differs from the index dimension");
   const int P = count();
   std::vector<std::vector<uint32_t>> ids(P);
   std::vector<std::vector<float>> ds(P);
-  int r = fan_out([&](int p) {
+  const int bad = workers_.run(P, [&](int p) {
     if (ix_[p]->n == 0) return 0;  // an empty partition answers nothing
     ids[p].resize(nq * k);
     ds[p].resize(nq * k);
     return ix_[p]->bruteforce(queries, nq, d, k, ids[p].data(), ds[p].data());
   });
-  if (r) return r;
+  if (bad >= 0) return fail(bad, ix_[bad]->err());
   int32_t cnt[MAX_PARTS];
   for (size_t q = 0; q < nq; ++q) {
     const size_t o = q * k;

@@ -3,39 +3,11 @@
 // partition and the P answer lists are merged.  This adds capacity (P devices' HBM for one index), where replication
 // (multi.cu) adds throughput.  DESIGN.md §6 "Partitioned index" states the rules.
 #pragma once
+#include <algorithm>
+
 #include "index.h"
 
 namespace hb {
-
-// Where a host search writes its [nq][k] answer slots and counts[nq]: either the reference entry points' answer blocks
-// (`nb`: Neighbour_api with the internal id in its tail padding) or hnsw_b200_search_flat's arrays (internal and pid
-// optional).
-struct AnswerArrays {
-  NeighbourOut* nb = nullptr;
-  uint64_t* ids = nullptr;
-  float* dist = nullptr;
-  uint32_t* internal = nullptr;
-  int32_t* pid = nullptr;
-  int32_t* counts = nullptr;
-};
-
-// PointId (level, rank) of internal id `it` of `rx`, hnsw.rs:46; (-1, -1) for an empty slot
-inline void point_id(const Index* rx, uint32_t it, int32_t* pid2) {
-  pid2[0] = it != INVALID_ID ? (int32_t)rx->h_level[it] : -1;
-  pid2[1] = it != INVALID_ID ? rx->h_rank[it] : -1;
-}
-
-// slot s of `out` from answer e of index rx, reported with internal id `internal` (a partitioned handle's global rank)
-inline void put_answer(const AnswerArrays& out, size_t s, const Index* rx, const NeighbourOut& e, uint32_t internal) {
-  if (out.nb) {
-    out.nb[s] = NeighbourOut{e.origin, e.dist, internal};
-    return;
-  }
-  out.ids[s] = e.origin;
-  out.dist[s] = e.dist;
-  if (out.internal) out.internal[s] = internal;
-  if (out.pid) point_id(rx, e.internal, out.pid + 2 * s);
-}
 
 class Partitions {
  public:
@@ -57,28 +29,45 @@ class Partitions {
   // a batch in the engine's insert form (flat `vecs` with `stride` elements per row, or `rows`), split by placement
   int insert(const void* vecs, size_t n_new, size_t stride, const void* const* rows, const uint64_t* ids,
              const int32_t* levels, int d);
-  // every query on every partition with the caller's k and ef, merged into `out`.  The filter is the FilterT arguments
-  // (filter_mode 1, 2) or `resident`, the id of one of the handle's resident filters (filter_mode 0).
-  int search(const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef, int filter_mode,
-             const uint64_t* filter_ids, size_t nfilter, int (*fn)(uint64_t, void*), void* ctx, const int64_t* resident,
-             const AnswerArrays& out);
-  // exact k nearest over all partitions, merged like search; out_ids are global insertion ranks
+  // exact k nearest over all partitions, merged like a search (host_search.cu); out_ids are global insertion ranks
   int bruteforce(const void* queries, size_t nq, int d, size_t k, uint32_t* out_ids, float* out_dist);
   int get_stats(uint64_t* out4, bool reset);
+  // the handle's error "partition p (device D): why"
+  int fail(int p, const std::string& why) const;
 
  private:
   explicit Partitions(Index* parent) : parent_(parent) {}
-  int fail(int p, const std::string& why) const;
-  // job(p) for every partition at once: partition 0 on the calling thread, partition p > 0 on worker p - 1
-  int fan_out(const std::function<int(int)>& job);
   size_t expected_count(int p, size_t total) const { return (total + count() - 1 - p) / count(); }
 
   Index* parent_;
   std::vector<std::unique_ptr<Index>> ix_;
-  std::vector<std::unique_ptr<Index::Worker>> workers_;
+  WorkerGroup workers_;  // worker p - 1 serves partition p
   std::vector<Index*> views_;
   std::string broken_;  // set when a failed insert left the partitions at counts the placement rule does not give
-  std::mutex fan_mu_;   // one fan-out at a time: a worker holds one job
 };
+
+// Merge rule: the first min(k, sum of counts) entries of the P ascending lists of one query, ordered by (distance,
+// partition, position in that partition's list).  dist(p, i) is entry i of list p; emit(j, p, i) writes output slot j.
+template <class Dist, class Emit>
+size_t merge_lists(int P, size_t k, const int32_t* cnt, const Dist& dist, const Emit& emit) {
+  int pos[Partitions::MAX_PARTS] = {};
+  size_t total = 0;
+  for (int p = 0; p < P; ++p) total += (size_t)cnt[p];
+  total = std::min(total, k);
+  for (size_t j = 0; j < total; ++j) {
+    int best = -1;
+    float bd = 0.f;
+    for (int p = 0; p < P; ++p) {
+      if (pos[p] >= cnt[p]) continue;
+      const float dp = dist(p, pos[p]);
+      if (best < 0 || dp < bd) {
+        best = p;
+        bd = dp;
+      }
+    }
+    emit(j, best, pos[best]++);
+  }
+  return total;
+}
 
 }  // namespace hb

@@ -115,7 +115,8 @@ def test_replicated_search_equals_one_gpu(pkg, po):
 
 
 def test_calls_leave_the_current_device_alone(pkg, po):
-    """a host that tracks the current device itself (torch) must find it unchanged after replicate / search / drop"""
+    """a host that tracks the current device itself (torch) must find it unchanged after replicate, search, submit, wait
+    and drop"""
     import torch
     L = pkg.load_library()
     if L.hnsw_b200_device_count() < 2:
@@ -133,6 +134,10 @@ def test_calls_leave_the_current_device_alone(pkg, po):
     h.replicate([0, 1])
     assert current() == 0
     h.search_flat(Q, 5, 32)
+    assert current() == 0
+    t = h.submit_flat(Q, 5, 32)   # sharded: every device's share is enqueued from this thread
+    assert current() == 0
+    h.wait_flat(t)
     assert current() == 0
     h.replicate([0])
     assert current() == 0
