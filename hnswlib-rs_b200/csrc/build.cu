@@ -33,34 +33,20 @@ __global__ void __launch_bounds__(BUILD_THREADS) insert_search_kernel(InsertPara
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const GraphView& g = p.g;
   unsigned char* base = smem_raw + (size_t)warp * p.smem_per_warp;
-  // layout: q4 | qe4 | wbuf[ef_c] | cand_id[32] cand_d[32] | sel_id[nbmax] sel_d[nbmax] tmp[nbmax] | disc[ef_c] (u16)
-  WarpSmem s;
-  size_t off = stage_bytes(g.d4);
+  const InsertLayout L = insert_layout(g.d4, p.ef_c, g.deg0, p.q_smem);
+  const WarpSmem s{reinterpret_cast<uint4*>(base + L.query), reinterpret_cast<uint64_t*>(base + L.queue),
+                   reinterpret_cast<uint32_t*>(base + L.cand_id), reinterpret_cast<float*>(base + L.cand_d)};
   Stage stg;
-  stg.buf = off ? reinterpret_cast<uint4*>(base) : nullptr;
-  s.q4 = reinterpret_cast<uint4*>(base + off);
-  off += (size_t)g.d4 * 16;
-  uint4* qe4 = reinterpret_cast<uint4*>(base + off);
-  off += (size_t)g.d4 * 16;
-  s.wbuf = reinterpret_cast<uint64_t*>(base + off);
-  off += (size_t)p.q_smem * 8;
-  s.cand_id = reinterpret_cast<uint32_t*>(base + off);
-  off += 256;
-  s.cand_d = reinterpret_cast<float*>(base + off);
-  off += 256;
-  stg.bar = reinterpret_cast<uint64_t*>(base + off);
-  off += 16;
+  stg.buf = stage_bytes(g.d4) ? reinterpret_cast<uint4*>(base + L.stage) : nullptr;
+  stg.bar = reinterpret_cast<uint64_t*>(base + L.bar);
   stg.phase = 0;
   if (lane == 0) mbar_init(stg.bar, 1);
   __syncwarp();
-  const int nbmax = g.deg0;
-  uint32_t* sel_id = reinterpret_cast<uint32_t*>(base + off);
-  off += (size_t)nbmax * 4;
-  float* sel_d = reinterpret_cast<float*>(base + off);
-  off += (size_t)nbmax * 4;
-  float* tmp = reinterpret_cast<float*>(base + off);
-  off += (size_t)nbmax * 4;
-  uint16_t* disc = reinterpret_cast<uint16_t*>(base + off);
+  uint4* qe4 = reinterpret_cast<uint4*>(base + L.point);
+  uint32_t* sel_id = reinterpret_cast<uint32_t*>(base + L.sel_id);
+  float* sel_d = reinterpret_cast<float*>(base + L.sel_d);
+  float* tmp = reinterpret_cast<float*>(base + L.tmp);
+  uint16_t* disc = reinterpret_cast<uint16_t*>(base + L.disc);
 
   const uint32_t slot = blockIdx.x * (blockDim.x >> 5) + warp;
   Visited vis;
@@ -71,7 +57,7 @@ __global__ void __launch_bounds__(BUILD_THREADS) insert_search_kernel(InsertPara
   const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
 
   for (;;) {
-    const uint32_t wi = next_item(p.work_counter);
+    const uint32_t wi = next_item(p.work_counter, lane);
     if (wi >= p.count) break;
     const uint32_t x = p.first + wi;
     const int lv = g.level[x];
@@ -81,18 +67,14 @@ __global__ void __launch_bounds__(BUILD_THREADS) insert_search_kernel(InsertPara
 
     bool overflow = false;
     uint32_t cur = g.entry;
-    // dist_to_entry, hnsw.rs:1110-1112
-    if (lane == 0) s.cand_id[0] = cur;
-    __syncwarp();
-    warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, 1, s.cand_d);
-    __syncwarp();
+    WarpChunk<Op, CH, U>{g, s, lane}.score(cur, 1);  // dist_to_entry, hnsw.rs:1110-1112
     float dist_to_entry = Op::post(s.cand_d[0]);
     // ---- layers above the new point's level: ef = 1 (hnsw.rs:1114-1155).  The reference also pushes
     // the result into new_point.neighbours[l] for l above its level (1140-1144); that list can never
     // be traversed (DESIGN.md "lists above a point's level") and is not materialised.
     for (int l = g.entry_level; l > lv; --l) {
       if (!((mask >> l) & 1u)) continue;  // points_by_layer[l].is_empty() => empty result (942-946)
-      search_layer<Op, CH, U, Queue>(g, s, stg, vis, Q, cur, 1, l, st, overflow);
+      search_layer<Op, CH, U, Queue>(g, s, stg, p.vis, vis, Q, cur, 1, l, st, overflow);
       if (overflow) break;
       const uint64_t k0 = Q.get(0);
       const float t = key_dist(k0);  // == dist(data, ep) recomputed at 1146
@@ -104,7 +86,7 @@ __global__ void __launch_bounds__(BUILD_THREADS) insert_search_kernel(InsertPara
     // ---- layers level..0: ef_construction search + selection (hnsw.rs:1158-1205)
     for (int l = lv; l >= 0 && !overflow; --l) {
       if (!((mask >> l) & 1u)) continue;
-      search_layer<Op, CH, U, Queue>(g, s, stg, vis, Q, cur, p.ef_c, l, st, overflow);
+      search_layer<Op, CH, U, Queue>(g, s, stg, p.vis, vis, Q, cur, p.ef_c, l, st, overflow);
       if (overflow) break;
       const int n = Q.n;
       const int nb = (l == 0) ? g.deg0 : g.M;  // 1177-1183
@@ -180,32 +162,18 @@ __global__ void __launch_bounds__(BUILD_THREADS) insert_search_kernel(InsertPara
         }
       }
       // own list of layer l (hnsw.rs:1197), ascending, INVALID padded
-      {
-        uint32_t* ids;
-        float* ds;
-        int cap;
-        if (l == 0) {
-          ids = g.adj0 + (size_t)x * g.deg0;
-          ds = g.adj0_d + (size_t)x * g.deg0;
-          cap = g.deg0;
-        } else {
-          const size_t li = (size_t)g.up_off[x] + (l - 1);
-          ids = g.adjU + li * g.M;
-          ds = g.adjU_d + li * g.M;
-          cap = g.M;
-        }
-        for (int i = lane; i < cap; i += 32) {
-          ids[i] = i < cnt ? sel_id[i] : INVALID_ID;
-          ds[i] = i < cnt ? sel_d[i] : 0.f;
-        }
+      const List own = list_at(g, x, l);
+      for (int i = lane; i < own.cap; i += 32) {
+        own.ids[i] = i < cnt ? sel_id[i] : INVALID_ID;
+        own.dists[i] = i < cnt ? sel_d[i] : 0.f;
       }
       if (cnt > 0) cur = sel_id[0];  // 1201-1203
       __syncwarp();
     }
     if (overflow && lane == 0) atomicExch(p.status, 1);
   }
-  vis.save(p.vis, slot);
-  flush_stats(p.stats, st);
+  vis.save(p.vis, slot, lane);
+  flush_stats(p.stats, st, lane);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -284,41 +252,18 @@ __global__ void __launch_bounds__(BUILD_THREADS) insert_link_kernel(InsertParams
     const uint32_t x = p.first + wi;
     const int L = g.level[x];
     for (int l = L; l >= 0; --l) {  // hnsw.rs:1248
-      const uint32_t* ids;
-      const float* ds;
-      int cap;
-      if (l == 0) {
-        ids = g.adj0 + (size_t)x * g.deg0;
-        ds = g.adj0_d + (size_t)x * g.deg0;
-        cap = g.deg0;
-      } else {
-        const size_t li = (size_t)g.up_off[x] + (l - 1);
-        ids = g.adjU + li * g.M;
-        ds = g.adjU_d + li * g.M;
-        cap = g.M;
-      }
-      for (int j = 0; j < cap; ++j) {  // hnsw.rs:1249
-        const uint32_t q = ids[j];
+      const List own = list_at(g, x, l);
+      for (int j = 0; j < own.cap; ++j) {  // hnsw.rs:1249
+        const uint32_t q = own.ids[j];
         if (q == INVALID_ID) break;
         if (q == x) continue;  // 1250
-        const float d = ds[j];
-        // target list: q.neighbours[L] with L = the NEW point's level (1257)
-        uint32_t* tids;
-        float* tds;
-        int tcap;
-        if (L == 0) {
-          tids = g.adj0 + (size_t)q * g.deg0;
-          tds = g.adj0_d + (size_t)q * g.deg0;
-          tcap = g.deg0;  // 1272-1276: 2*max_nb_connection at layer 0
-        } else {
-          if (L > (int)g.plevel[q]) continue;  // a list no search can ever read; not materialised
-          const size_t li = (size_t)g.up_off[q] + (L - 1);
-          tids = g.adjU + li * g.M;
-          tds = g.adjU_d + li * g.M;
-          tcap = g.M;
-        }
+        const float d = own.dists[j];
+        // target list: q.neighbours[L] with L = the NEW point's level (1257); 2*max_nb_connection slots at layer 0
+        // (1272-1276).  Above plevel[q] it is a list no search can ever read, and is not materialised.
+        const List t = list_at(g, q, L);
+        if (!t.ids) continue;
         lock_point(p.locks, q);
-        list_add_sorted(tids, tds, tcap, x, d);
+        list_add_sorted(t.ids, t.dists, t.cap, x, d);
         unlock_point(p.locks, q);
       }
     }

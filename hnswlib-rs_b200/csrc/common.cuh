@@ -94,7 +94,8 @@ __device__ __forceinline__ void st_keep(uint32_t* p, uint32_t v, uint64_t pol) {
   asm volatile("st.global.cg.L2::cache_hint.u32 [%0], %1, %2;" ::"l"(p), "r"(v), "l"(pol) : "memory");
 }
 
-// list of (p, layer): returns pointer to ids (or nullptr when the point owns no list there) and capacity
+// The list of (p, layer): pointer to its ids and its capacity, or nullptr / 0 above plevel[p], where the point owns no list.
+// The one place a list's address is worked out; list_at adds the distances, which sit at the same offset.
 __device__ __forceinline__ const uint32_t* list_ids(const GraphView& g, uint32_t p, int layer, int& cap) {
   if (layer == 0) {
     cap = g.deg0;
@@ -106,6 +107,17 @@ __device__ __forceinline__ const uint32_t* list_ids(const GraphView& g, uint32_t
   }
   cap = g.M;
   return g.adjU + ((size_t)g.up_off[p] + (layer - 1)) * g.M;
+}
+struct List {
+  uint32_t* ids;  // nullptr above plevel[p]
+  float* dists;   // distance of each link to p
+  int cap;
+};
+__device__ __forceinline__ List list_at(const GraphView& g, uint32_t p, int layer) {
+  List l;
+  l.ids = const_cast<uint32_t*>(list_ids(g, p, layer, l.cap));
+  l.dists = !l.ids ? nullptr : layer == 0 ? g.adj0_d + (l.ids - g.adj0) : g.adjU_d + (l.ids - g.adjU);
+  return l;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -560,61 +572,60 @@ struct VisitedCfg {
   int id_bits;        // bits needed for ids
 };
 
+// The state of one warp's set is what changes during a search: table pointer, epoch, insert count.  Capacity, hash shift
+// and the epoch / id split are read from the launch's VisitedCfg (kernel parameters) where they are used.  Every
+// function is warp-collective and takes the caller's lane (the lean kernel pins it, see lean_common.cuh pin()).
 struct Visited {
   uint32_t* tab;
-  uint32_t mask;
-  int shift;
-  int id_bits;
   uint32_t epoch;
-  uint32_t epoch_max;
-  uint32_t tag;
   uint32_t used;  // insertions of the current search (warp-uniform)
-  uint32_t limit;
 
   __device__ __forceinline__ void init(const VisitedCfg& c, uint32_t slot) {
     tab = c.tables + (size_t)slot * c.cap;
-    mask = c.cap - 1;
-    shift = c.shift;
-    id_bits = c.id_bits;
-    epoch_max = (id_bits >= 32) ? 0u : ((1u << (32 - id_bits)) - 1u);
     epoch = c.epochs[slot];
-    limit = c.cap - (c.cap >> 2);
     used = 0;
   }
-  __device__ __forceinline__ void save(const VisitedCfg& c, uint32_t slot) {
-    if (lane_id() == 0) c.epochs[slot] = epoch;
+  __device__ __forceinline__ void save(const VisitedCfg& c, uint32_t slot, int lane) const {
+    if (lane == 0) c.epochs[slot] = epoch;
   }
-  // start a new search: all lanes call
-  __device__ __forceinline__ void begin() {
+  static __device__ __forceinline__ uint32_t home(const VisitedCfg& c, uint32_t id) { return (id * 2654435761u) >> c.shift; }
+  // Start a new search from `entry` (hnsw.rs:955-956): bump the epoch instead of clearing the table (cleared only when the
+  // epoch wraps), then record the entry.  The table holds nothing of the new epoch yet, so the entry's home slot is free.
+  __device__ __forceinline__ void begin(const VisitedCfg& c, uint32_t entry, int lane) {
+    const uint32_t epoch_max = (c.id_bits >= 32) ? 0u : ((1u << (32 - c.id_bits)) - 1u);
     if (epoch >= epoch_max) {
-      for (uint32_t i = lane_id(); i <= mask; i += 32) tab[i] = 0u;
-      __syncwarp();
+      for (uint32_t i = lane; i < c.cap; i += 32) tab[i] = 0u;
       epoch = 0;
     }
     epoch += 1;
-    tag = epoch << id_bits;
-    used = 0;
+    used = 1;
+    __syncwarp();
+    if (lane == 0) st_keep(tab + home(c, entry), (epoch << c.id_bits) | entry, l2_policy_evict_last());
+    __syncwarp();
   }
-  // Warp-collective test-and-set of up to 32 ids (one per lane, `valid` lanes only).  Returns true in the
-  // lanes whose id was not yet in the set (it is afterwards).  The table is private to this warp, so no
-  // atomics are needed: lanes that find the same free slot in the same round elect the lowest lane
-  // (match_any); the others probe on.  One L2 round trip per round, and almost always one round.
-  __device__ __forceinline__ bool test_and_set(uint32_t id, bool valid) {
-    const uint32_t want = tag | id;
+  // Test-and-set of up to 32 ids (one per lane, `valid` lanes only).  Returns true in the lanes whose id was not yet in
+  // the set (it is afterwards).  The table is private to this warp, so no atomics are needed: lanes that find the same
+  // free slot in the same round elect the lowest lane (match_any); the others probe on.  One L2 round trip per round,
+  // and almost always one round.  The first probe may have been done ahead of time (`pre`: slot pre_h was read as
+  // pre_cv after the last store to the table).
+  __device__ __forceinline__ bool test_and_set(const VisitedCfg& c, int lane, uint32_t id, bool valid, bool pre = false,
+                                               uint32_t pre_h = 0, uint32_t pre_cv = 0) {
+    const uint32_t want = (epoch << c.id_bits) | id;
     const uint64_t pol_keep = l2_policy_evict_last();
-    uint32_t h = (id * 2654435761u) >> shift;
-    bool pending = valid, fresh = false;
+    uint32_t h = pre ? pre_h : home(c, id);
+    bool pending = valid, fresh = false, first = pre;
     while (__any_sync(FULL, pending)) {
       uint32_t cur = 0;
-      if (pending) cur = ld_keep(tab + h, pol_keep);
+      if (pending) cur = first ? pre_cv : ld_keep(tab + h, pol_keep);
+      first = false;
       bool claim = false;
       if (pending) {
         if (cur == want) {
           pending = false;  // already visited
-        } else if ((cur >> id_bits) != epoch) {
+        } else if ((cur >> c.id_bits) != epoch) {
           claim = true;  // stale or empty slot
         } else {
-          h = (h + 1) & mask;
+          h = (h + 1) & (c.cap - 1);
         }
       }
       const unsigned claimers = __ballot_sync(FULL, claim);
@@ -622,14 +633,14 @@ struct Visited {
         const unsigned same = __match_any_sync(claimers, h);
         const int leader = __ffs(same) - 1;
         const uint32_t lead_id = __shfl_sync(claimers, id, leader);
-        if (lane_id() == leader) {
+        if (lane == leader) {
           st_keep(tab + h, want, pol_keep);
           fresh = true;
           pending = false;
         } else if (lead_id == id) {
           pending = false;  // the same id twice in one chunk: the leader records it
         } else {
-          h = (h + 1) & mask;
+          h = (h + 1) & (c.cap - 1);
         }
       }
       __syncwarp();  // orders this round's stores before the next round's loads
@@ -637,7 +648,7 @@ struct Visited {
     used += __popc(__ballot_sync(FULL, fresh));  // warp-uniform count
     return fresh;
   }
-  __device__ __forceinline__ bool overflowing() const { return used >= limit; }
+  __device__ __forceinline__ bool overflowing(const VisitedCfg& c) const { return used >= c.cap - (c.cap >> 2); }
 };
 
 // ------------------------------------------------------------------------------------------------

@@ -41,20 +41,15 @@ __device__ __forceinline__ int keep_passing(uint64_t* w, int n, const uint32_t* 
 }
 
 template <class Op, int CH, int U>
-__device__ __forceinline__ void search_layer_filtered(const GraphView& g, const WarpSmem& s, Visited& vis, SortedQueue& W,
-                                                      uint64_t* cbuf, uint32_t ccap, const uint32_t* fbits, uint32_t ep,
-                                                      int ef, int layer, Stats& st, bool& overflow) {
+__device__ __forceinline__ void search_layer_filtered(const GraphView& g, const WarpSmem& s, const VisitedCfg& vc, Visited& vis,
+                                                      SortedQueue& W, uint64_t* cbuf, uint32_t ccap, const uint32_t* fbits,
+                                                      uint32_t ep, int ef, int layer, Stats& st, bool& overflow) {
   const int lane = lane_id();
   const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
-  vis.begin();
-  __syncwarp();  // the descent's reads of cand_id happen-before the write below
-  if (lane == 0) s.cand_id[0] = ep;
-  __syncwarp();
-  warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, 1, s.cand_d);  // hnsw.rs:952
-  __syncwarp();
+  vis.begin(vc, ep, lane);  // hnsw.rs:955-956
+  WarpChunk<Op, CH, U>{g, s, lane}.score(ep, 1);  // hnsw.rs:952
   st.evals += 1;
   const float d0 = Op::post(s.cand_d[0]);
-  vis.test_and_set(ep, lane == 0);
   W.reset(s.wbuf, ef);
   if (lane == 0) {
     s.wbuf[0] = make_key(d0, ep);  // ep enters W unfiltered (hnsw.rs:964-967)
@@ -105,7 +100,7 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
       const uint32_t nid = (base + lane < cap) ? ids[base + lane] : INVALID_ID;
       const unsigned valid = __ballot_sync(FULL, nid != INVALID_ID);
       st.adj += __popc(valid);
-      const bool fresh = vis.test_and_set(nid, nid != INVALID_ID);  // 1016-1017
+      const bool fresh = vis.test_and_set(vc, lane, nid, nid != INVALID_ID);  // 1016-1017
       const unsigned m = __ballot_sync(FULL, fresh);
       const int cnt = __popc(m);
       if (cnt) {
@@ -145,7 +140,7 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
       if (valid != FULL) break;
     }
     if (done && W.n == 0) break;
-    if (overflow || vis.overflowing()) {
+    if (overflow || vis.overflowing(vc)) {
       overflow = true;
       break;
     }
@@ -158,12 +153,9 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const GraphView& g = p.g;
   unsigned char* base = smem_raw + (size_t)warp * p.smem_per_warp;
-  const size_t stb = stage_bytes(g.d4);  // same per-warp layout as search.cu (the stage is unused here)
-  WarpSmem s;
-  s.q4 = reinterpret_cast<uint4*>(base + stb);
-  s.wbuf = reinterpret_cast<uint64_t*>(base + stb + (size_t)g.d4 * 16);
-  s.cand_id = reinterpret_cast<uint32_t*>(base + stb + (size_t)g.d4 * 16 + (size_t)p.q_smem * 8);
-  s.cand_d = reinterpret_cast<float*>(s.cand_id + 32);
+  const QueryLayout L = query_layout(g.d4, p.q_smem);  // search.cu's layout; the stage and its mbarrier are unused here
+  const WarpSmem s{reinterpret_cast<uint4*>(base + L.query), reinterpret_cast<uint64_t*>(base + L.queue),
+                   reinterpret_cast<uint32_t*>(base + L.cand_id), reinterpret_cast<float*>(base + L.cand_d)};
   const uint32_t slot = blockIdx.x * (blockDim.x >> 5) + warp;  // the host launches fewer warps per CTA when shared memory is short
   Visited vis;
   vis.init(p.vis, slot);
@@ -172,16 +164,16 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
   Stats st{0, 0, 0};
 
   for (;;) {
-    const uint32_t qi = next_item(p.work_counter);
+    const uint32_t qi = next_item(p.work_counter, lane);
     if (qi >= p.nq) break;
     stage_row_bytes(s.q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes, p.q_bytes, g.d4 * 16);
     int count = 0;
     bool overflow = false;
     W.reset(s.wbuf, p.ef);
     if (g.entry != INVALID_ID) {
-      const Entry e = descend<Op, CH, U>(g, s, st);  // the filter plays no role in the descent (hnsw.rs:1511-1529)
-      const uint32_t pivot = e.pivot;
-      search_layer_filtered<Op, CH, U>(g, s, vis, W, cbuf, p.ccap, p.filter_bits, pivot, p.ef, p.layer0, st, overflow);
+      // the filter plays no role in the descent (hnsw.rs:1511-1529)
+      const Entry e = descend<Op>(g, lane, st, WarpChunk<Op, CH, U>{g, s, lane});
+      search_layer_filtered<Op, CH, U>(g, s, p.vis, vis, W, cbuf, p.ccap, p.filter_bits, e.pivot, p.ef, p.layer0, st, overflow);
       count = min(p.k, min(p.ef, W.n));  // hnsw.rs:1547
     }
     if (overflow) {
@@ -210,8 +202,8 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
     if (lane == 0) p.out_count[qi] = outn;
     __syncwarp();
   }
-  vis.save(p.vis, slot);
-  flush_stats(p.stats, st);
+  vis.save(p.vis, slot, lane);
+  flush_stats(p.stats, st, lane);
 }
 
 template <class Op>

@@ -297,7 +297,7 @@ Index::InsertShape Index::insert_shape() const {
   s.q_kind = queue_kind(ef_c, metric, dtype);
   if (s.q_kind != 0 && s.q_kind < 104) s.q_kind = 104;
   s.q_smem = queue_slots(s.q_kind, ef_c);
-  s.smem_per_warp = insert_smem_per_warp(row_bytes / 16, ef_c, 2 * M, s.q_smem);
+  s.smem_per_warp = insert_layout(row_bytes / 16, ef_c, 2 * M, s.q_smem).bytes;
   return s;
 }
 

@@ -15,13 +15,10 @@ constexpr int SEARCH_THREADS = 256;  // 8 warps = 8 queries in flight per CTA
 constexpr int BUILD_THREADS = 128;   // 4 warps = 4 inserts in flight per CTA
 constexpr int LEAN_THREADS = 32;      // lean kernel (search_lean.cuh): one warp per CTA, so that a finished query frees its slot at once
 constexpr size_t SMEM_BUDGET = 220 * 1024;  // dynamic shared memory one CTA may ask for (an H100 SM offers 227 KB)
-#ifndef HB_LEAN_BLOCKS
-#define HB_LEAN_BLOCKS 20
-#endif
 // 20 one-warp CTAs per SM, <= 96 registers per thread, no spills.  H100 SXM 80 GB at a 400 W power limit, c2 workload, one
 // launch of 100 000 queries: 25.8 ms at 20, 26.7 at 24, 28.3 at 28 (72 registers, spills), 32.4 at 32 (64 registers); 16
 // (100 registers) took 26.5 ms against 25.8 at 20 in a separate run.
-constexpr int LEAN_MIN_BLOCKS = HB_LEAN_BLOCKS;
+constexpr int LEAN_MIN_BLOCKS = 20;
 
 // One answer slot.  Same 16-byte layout as the reference's #[repr(C)] Neighbour_api {id: usize, d: f32}
 // (/root/reference/src/libext.rs:64-71); the internal id rides in what is tail padding there.
@@ -57,7 +54,72 @@ struct SearchParams {
 
 // rows of up to 512 bytes are (partly) staged by TMA: STAGE_ROWS rows + an mbarrier per warp
 __host__ __device__ inline size_t stage_bytes(int d4) { return d4 <= 32 ? (size_t)STAGE_ROWS * d4 * 16 : 0; }
-// register-queue stripes for a given ef (0 = queue in shared memory)
+
+// ---- per-warp shared-memory layouts: the byte offset of each region and the total, rounded to 128 bytes.  The host sizes
+// a launch from `bytes` (query_smem_per_warp, Index::insert_shape), the kernel takes its regions from the offsets.
+__host__ __device__ constexpr size_t round128(size_t b) { return (b + 127) & ~(size_t)127; }
+
+// generic and filtered kernels (search.cu, filter.cu): [TMA stage][query][queue keys][chunk ids][chunk distances][mbarrier]
+struct QueryLayout {
+  size_t stage, query, queue, cand_id, cand_d, bar, bytes;
+};
+__host__ __device__ inline QueryLayout query_layout(int d4, int q_smem) {
+  QueryLayout l;
+  l.stage = 0;
+  l.query = stage_bytes(d4);
+  l.queue = l.query + (size_t)d4 * 16;
+  l.cand_id = l.queue + (size_t)q_smem * 8;
+  l.cand_d = l.cand_id + 64 * 4;  // 64 slots reserved, 32 used (one chunk of neighbours)
+  l.bar = l.cand_d + 64 * 4;
+  l.bytes = round128(l.bar + 16);
+  return l;
+}
+
+// std-tie kernel (search_std.cu): [query][W heap, q_smem 8-byte items][chunk ids][chunk distances]
+struct StdLayout {
+  size_t query, heap, cand_id, cand_d, bytes;
+};
+__host__ __device__ inline StdLayout std_layout(int d4, int q_smem) {
+  StdLayout l;
+  l.query = 0;
+  l.heap = (size_t)d4 * 16;
+  l.cand_id = l.heap + (size_t)q_smem * 8;
+  l.cand_d = l.cand_id + 32 * 4;
+  l.bytes = round128(l.cand_d + 32 * 4);
+  return l;
+}
+
+// lean kernel (search_lean.cuh): [queue keys, also the query's staging buffer][chunk ids][chunk distances]
+struct LeanLayout {
+  uint32_t queue, cand_id, cand_d, bytes;
+};
+__host__ __device__ constexpr LeanLayout lean_layout(int q_smem) {
+  const uint32_t cand_id = (uint32_t)q_smem * 8, cand_d = cand_id + 32 * 4;
+  return LeanLayout{0, cand_id, cand_d, (uint32_t)round128(cand_d + 32 * 4)};
+}
+
+// insert kernel (build.cu): [TMA stage][new point][point of a selection step][queue keys][chunk ids][chunk distances]
+// [mbarrier][selected ids][selected distances][distances of a selection step][discarded positions, u16]
+struct InsertLayout {
+  size_t stage, query, point, queue, cand_id, cand_d, bar, sel_id, sel_d, tmp, disc, bytes;
+};
+__host__ __device__ inline InsertLayout insert_layout(int d4, int ef_c, int deg0, int q_smem) {
+  InsertLayout l;
+  l.stage = 0;
+  l.query = stage_bytes(d4);
+  l.point = l.query + (size_t)d4 * 16;
+  l.queue = l.point + (size_t)d4 * 16;
+  l.cand_id = l.queue + (size_t)q_smem * 8;
+  l.cand_d = l.cand_id + 64 * 4;
+  l.bar = l.cand_d + 64 * 4;
+  l.sel_id = l.bar + 16;
+  l.sel_d = l.sel_id + (size_t)deg0 * 4;
+  l.tmp = l.sel_d + (size_t)deg0 * 4;
+  l.disc = l.tmp + (size_t)deg0 * 4;
+  l.bytes = round128(l.disc + (size_t)ef_c * 2);
+  return l;
+}
+
 // Queue kind for a given ef (see QueueSel): compile-time chunked shared-memory queue up to ef = 256, generic beyond.
 // (A register-resident variant spilled at 64 registers/thread, and a speculative two-candidates-per-iteration loop was
 // exact but slower; both were removed.)
@@ -82,18 +144,16 @@ enum class QueryKernel { Lean, Generic, Filtered, StdTie };
 inline int query_queue_slots(QueryKernel kind, int q_kind, int ef) {
   switch (kind) {
     case QueryKernel::Lean: return lean_queue_slots(ef);
-    case QueryKernel::StdTie: return ef + 2;
+    case QueryKernel::StdTie: return ef + 2;  // the W heap holds at most ef + 1 items (push, then pop when over ef)
     default: return queue_slots(q_kind, ef);
   }
 }
 inline size_t query_smem_per_warp(QueryKernel kind, int d4, int q_smem) {
-  size_t b;
   switch (kind) {
-    case QueryKernel::Lean: return (size_t)q_smem * 8 + 256;  // [queue keys / query staging][row ids][distances]
-    case QueryKernel::StdTie: b = (size_t)d4 * 16 + (size_t)q_smem * 8 + 256; break;  // [query][W heap][row ids][distances]
-    default: b = stage_bytes(d4) + (size_t)d4 * 16 + (size_t)q_smem * 8 + 64 * 8 + 16;  // search.cu's layout
+    case QueryKernel::Lean: return lean_layout(q_smem).bytes;
+    case QueryKernel::StdTie: return std_layout(d4, q_smem).bytes;
+    default: return query_layout(d4, q_smem).bytes;
   }
-  return (b + 127) & ~(size_t)127;
 }
 inline int query_threads(QueryKernel kind) { return kind == QueryKernel::Lean ? LEAN_THREADS : SEARCH_THREADS; }
 
@@ -115,11 +175,6 @@ struct InsertParams {
   int q_smem;
   int q_kind;
 };
-
-inline size_t insert_smem_per_warp(int d4, int ef_c, int deg0, int q_smem) {
-  size_t b = stage_bytes(d4) + (size_t)d4 * 32 + (size_t)q_smem * 8 + 512 + 16 + (size_t)deg0 * 12 + (size_t)ef_c * 2;
-  return (b + 127) & ~(size_t)127;
-}
 
 // The kernel this host thread last launched through launch_kernel (hnsw_b200_last_kernel reports its name), so that a
 // test can tell which template instantiation served a call.

@@ -14,16 +14,12 @@ __global__ void __launch_bounds__(SEARCH_THREADS, 4) search_kernel(SearchParams 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const GraphView& g = p.g;
   unsigned char* base = smem_raw + (size_t)warp * p.smem_per_warp;
-  // per-warp layout: [TMA stage][query][queue keys][cand ids][cand dists][mbarrier]
-  const size_t stb = stage_bytes(g.d4);
-  WarpSmem s;
-  s.q4 = reinterpret_cast<uint4*>(base + stb);
-  s.wbuf = reinterpret_cast<uint64_t*>(base + stb + (size_t)g.d4 * 16);
-  s.cand_id = reinterpret_cast<uint32_t*>(base + stb + (size_t)g.d4 * 16 + (size_t)p.q_smem * 8);
-  s.cand_d = reinterpret_cast<float*>(s.cand_id + 64);
+  const QueryLayout L = query_layout(g.d4, p.q_smem);
+  const WarpSmem s{reinterpret_cast<uint4*>(base + L.query), reinterpret_cast<uint64_t*>(base + L.queue),
+                   reinterpret_cast<uint32_t*>(base + L.cand_id), reinterpret_cast<float*>(base + L.cand_d)};
   Stage stg;
-  stg.buf = stb ? reinterpret_cast<uint4*>(base) : nullptr;
-  stg.bar = reinterpret_cast<uint64_t*>(s.cand_d + 64);
+  stg.buf = stage_bytes(g.d4) ? reinterpret_cast<uint4*>(base + L.stage) : nullptr;
+  stg.bar = reinterpret_cast<uint64_t*>(base + L.bar);
   stg.phase = 0;
   if (lane == 0) mbar_init(stg.bar, 1);
   __syncwarp();
@@ -36,22 +32,22 @@ __global__ void __launch_bounds__(SEARCH_THREADS, 4) search_kernel(SearchParams 
   Stats st{0, 0, 0};
 
   for (;;) {
-    const uint32_t qi = next_item(p.work_counter);
+    const uint32_t qi = next_item(p.work_counter, lane);
     if (qi >= p.nq) break;
     // stage the query (zero padded to d_pad)
     stage_row_bytes(s.q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes, p.q_bytes, g.d4 * 16);
     int count = 0;
     bool overflow = false;
     if (g.entry != INVALID_ID) {  // hnsw.rs:1498-1503
-      const Entry e = descend<Op, CH, U>(g, s, st);
+      const Entry e = descend<Op>(g, lane, st, WarpChunk<Op, CH, U>{g, s, lane});
       // ---- layer-0 (lowest populated layer) search, hnsw.rs:1531-1542
-      search_layer<Op, CH, U, Queue>(g, s, stg, vis, Q, e.pivot, p.ef, p.layer0, st, overflow);
+      search_layer<Op, CH, U, Queue>(g, s, stg, p.vis, vis, Q, e.pivot, p.ef, p.layer0, st, overflow);
       count = min(p.k, min(p.ef, Q.n));  // hnsw.rs:1547
     }
-    write_answers(p, qi, overflow, count, [&](int j) { return Q.local(j); });  // the queue is already sorted
+    write_answers(p, lane, qi, overflow, count, [&](int j) { return Q.local(j); });  // the queue is already sorted
   }
-  vis.save(p.vis, slot);
-  flush_stats(p.stats, st);
+  vis.save(p.vis, slot, lane);
+  flush_stats(p.stats, st, lane);
 }
 
 // Compile-time row length (CH chunks of 128 bytes) only where the lean kernel cannot take the search: a 256-slot queue

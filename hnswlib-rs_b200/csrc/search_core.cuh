@@ -1,8 +1,11 @@
 // search_layer on a warp: the ef-bounded best-first expansion of one layer.
 // Restates /root/reference/src/hnsw.rs:922-1064 (search_layer) for one warp that owns the whole
 // queue state of one query; used by the query kernel (search.cu) and the insert kernel (build.cu).
-// Also the per-query scaffold the warp query kernels (search.cu, filter.cu, search_std.cu) share: work counter,
-// upper-layer descent, answer write-out, counter flush.
+// Also the per-query scaffold the query kernels share: the work counter (all four), the upper-layer descent and the counter
+// flush (the warp kernels search.cu, filter.cu, search_std.cu), the answer write-out (all but the filtered kernel, which
+// compacts its answers).  The scaffold functions (and Visited) take the caller's lane, because the lean kernel
+// (search_lean.cuh) pins its lane; a layer search (search_layer here, search_layer_filtered in filter.cu) is a warp kernel's
+// own loop, not scaffold, and takes the lane once at its top.
 #pragma once
 #include "kernels.h"
 
@@ -11,8 +14,25 @@ namespace hb {
 struct WarpSmem {
   uint4* q4;          // query row, d4 16-byte chunks (zero padded)
   uint64_t* wbuf;     // queue keys, capacity >= ef
-  uint32_t* cand_id;  // 64 slots reserved, 32 used (one chunk of neighbours)
-  float* cand_d;      // 64
+  uint32_t* cand_id;  // one chunk of neighbours: 32 ids
+  float* cand_d;      // and their distances
+};
+
+// One chunk of up to 32 candidates of a warp kernel, scored by warp_dists into WarpSmem (see descend()).
+template <class Op, int CH, int U>
+struct WarpChunk {
+  const GraphView& g;
+  const WarpSmem& s;
+  int lane;
+  __device__ __forceinline__ void score(uint32_t id, int cnt) const {
+    __syncwarp();  // earlier reads of the chunk happen-before the writes below
+    if (lane < cnt) s.cand_id[lane] = id;
+    __syncwarp();
+    warp_dists<Op, CH, U>(reinterpret_cast<const uint4*>(g.vec), g.d4, g.dim, s.q4, s.cand_id, cnt, s.cand_d);
+    __syncwarp();
+  }
+  __device__ __forceinline__ float dist(int j) const { return s.cand_d[j]; }
+  __device__ __forceinline__ uint32_t id(int j) const { return s.cand_id[j]; }
 };
 
 struct Stats {
@@ -27,19 +47,14 @@ struct Stats {
 //     so it would trip the stop rule the moment it is popped.
 // Ties on distance are ordered by id (oracle MODE_DET).
 template <class Op, int CH, int U, class Queue>
-__device__ __forceinline__ void search_layer(const GraphView& g, const WarpSmem& s, Stage& stg, Visited& vis,
-                                             Queue& Q, uint32_t ep, int ef, int layer, Stats& st, bool& overflow) {
+__device__ __forceinline__ void search_layer(const GraphView& g, const WarpSmem& s, Stage& stg, const VisitedCfg& vc,
+                                             Visited& vis, Queue& Q, uint32_t ep, int ef, int layer, Stats& st, bool& overflow) {
   const int lane = lane_id();
   const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
-  vis.begin();
-  __syncwarp();  // earlier reads of cand_id (descent, previous layer) happen-before the write below
-  if (lane == 0) s.cand_id[0] = ep;
-  __syncwarp();
-  warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, 1, s.cand_d);  // hnsw.rs:952
-  __syncwarp();
+  vis.begin(vc, ep, lane);  // hnsw.rs:955-956
+  WarpChunk<Op, CH, U>{g, s, lane}.score(ep, 1);  // hnsw.rs:952
   st.evals += 1;
   const float d0 = Op::post(s.cand_d[0]);
-  vis.test_and_set(ep, lane == 0);  // hnsw.rs:955-956
   Q.reset(s.wbuf, ef);
   Q.push_first(make_key(d0, ep));  // hnsw.rs:958-967 (ep enters W and C)
   for (;;) {
@@ -66,7 +81,7 @@ __device__ __forceinline__ void search_layer(const GraphView& g, const WarpSmem&
       const uint32_t nid = (base + lane < cap) ? ids[base + lane] : INVALID_ID;
       const unsigned valid = __ballot_sync(FULL, nid != INVALID_ID);
       st.adj += __popc(valid);
-      const bool fresh = vis.test_and_set(nid, nid != INVALID_ID);  // hnsw.rs:1016-1017
+      const bool fresh = vis.test_and_set(vc, lane, nid, nid != INVALID_ID);  // hnsw.rs:1016-1017
       const unsigned m = __ballot_sync(FULL, fresh);
       const int cnt = __popc(m);
       if (cnt) {
@@ -87,7 +102,7 @@ __device__ __forceinline__ void search_layer(const GraphView& g, const WarpSmem&
       }
       if (valid != FULL) break;  // lists are dense prefixes terminated by INVALID_ID
     }
-    if (vis.overflowing()) {
+    if (vis.overflowing(vc)) {
       overflow = true;
       break;
     }
@@ -95,9 +110,9 @@ __device__ __forceinline__ void search_layer(const GraphView& g, const WarpSmem&
 }
 
 // the next work item of this warp from a launch's work counter (warp-uniform)
-__device__ __forceinline__ uint32_t next_item(unsigned int* work_counter) {
+__device__ __forceinline__ uint32_t next_item(unsigned int* work_counter, int lane) {
   uint32_t i = 0;
-  if (lane_id() == 0) i = atomicAdd(work_counter, 1u);
+  if (lane == 0) i = atomicAdd(work_counter, 1u);
   return __shfl_sync(FULL, i, 0);
 }
 
@@ -108,17 +123,14 @@ struct Entry {
 
 // Upper-layer descent (hnsw.rs:1498-1529): from the graph's entry point, ONE pass over pivot.neighbours[layer] per
 // layer, moving to the first minimum of the list when it is strictly below the best distance so far.
-template <class Op, int CH, int U>
-__device__ __forceinline__ Entry descend(const GraphView& g, const WarpSmem& s, Stats& st) {
-  const int lane = lane_id();
-  const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
+// How one chunk is scored is the parameter: ch.score(id, cnt) puts the ids of lanes i < cnt in slots 0..cnt-1 and scores
+// them, ch.dist(j) / ch.id(j) read slot j back (distance before Op::post).
+template <class Op, class Chunk>
+__device__ __forceinline__ Entry descend(const GraphView& g, int lane, Stats& st, const Chunk& ch) {
   uint32_t pivot = g.entry;
-  if (lane == 0) s.cand_id[0] = pivot;
-  __syncwarp();
-  warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, 1, s.cand_d);  // hnsw.rs:1506
-  __syncwarp();
+  ch.score(pivot, 1);  // hnsw.rs:1506
   st.evals += 1;
-  float best = Op::post(s.cand_d[0]);
+  float best = Op::post(ch.dist(0));
   for (int layer = g.entry_level; layer >= 1; --layer) {
     int cap;
     const uint32_t* ids = list_ids(g, pivot, layer, cap);
@@ -128,15 +140,11 @@ __device__ __forceinline__ Entry descend(const GraphView& g, const WarpSmem& s, 
       const unsigned valid = __ballot_sync(FULL, nid != INVALID_ID);
       const int cnt = __popc(valid);  // dense prefix
       if (cnt) {
-        __syncwarp();
-        if (lane < cnt) s.cand_id[lane] = nid;
-        __syncwarp();
-        warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, cnt, s.cand_d);  // hnsw.rs:1518
-        __syncwarp();
+        ch.score(nid, cnt);  // hnsw.rs:1518
         st.evals += cnt;
         st.adj += cnt;
         // strict `<` scanned in list order == first minimum of the list, if below `best`
-        uint64_t key = lane < cnt ? (((uint64_t)__float_as_uint(Op::post(s.cand_d[lane])) << 32) | (uint32_t)lane) : ~0ull;
+        uint64_t key = lane < cnt ? (((uint64_t)__float_as_uint(Op::post(ch.dist(lane))) << 32) | (uint32_t)lane) : ~0ull;
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) {
           const uint64_t other = __shfl_xor_sync(FULL, key, o);
@@ -145,7 +153,7 @@ __device__ __forceinline__ Entry descend(const GraphView& g, const WarpSmem& s, 
         const float dmin = __uint_as_float((uint32_t)(key >> 32));
         if (dmin < best) {
           best = dmin;
-          new_pivot = s.cand_id[(uint32_t)key & 31u];
+          new_pivot = ch.id((uint32_t)key & 31u);
         }
       }
       if (valid != FULL) break;
@@ -158,8 +166,7 @@ __device__ __forceinline__ Entry descend(const GraphView& g, const WarpSmem& s, 
 // The answers of query qi (hnsw.rs:1544-1579): key_at(j) for j < count, ascending, then (~0, +inf, INVALID_ID) up to k.
 // A query whose visited table overflowed answers nothing and raises the launch's status flag (the host re-runs it).
 template <class KeyAt>
-__device__ __forceinline__ void write_answers(const SearchParams& p, uint32_t qi, bool overflow, int count, KeyAt&& key_at) {
-  const int lane = lane_id();
+__device__ __forceinline__ void write_answers(const SearchParams& p, int lane, uint32_t qi, bool overflow, int count, KeyAt&& key_at) {
   if (overflow) {
     if (lane == 0) atomicExch(p.status, 1);
     count = 0;
@@ -179,8 +186,8 @@ __device__ __forceinline__ void write_answers(const SearchParams& p, uint32_t qi
 }
 
 // the traversal counters of one warp into the launch's totals (the counters are warp-uniform)
-__device__ __forceinline__ void flush_stats(unsigned long long* stats, const Stats& st) {
-  if (stats && lane_id() == 0) {
+__device__ __forceinline__ void flush_stats(unsigned long long* stats, const Stats& st, int lane) {
+  if (stats && lane == 0) {
     atomicAdd(stats + 0, (unsigned long long)st.evals);
     atomicAdd(stats + 1, (unsigned long long)st.expansions);
     atomicAdd(stats + 2, (unsigned long long)st.adj);

@@ -19,10 +19,9 @@
 //   * two rows per lane group are reduced with one transposed reduction (3 shuffles for 2 rows, same sums);
 //   * the traversal counters are a template parameter: the production instantiation does not carry them.
 #pragma once
-#include <type_traits>
-
 #include "kernels.h"
 #include "lean_common.cuh"
+#include "search_core.cuh"
 
 namespace hb {
 
@@ -130,83 +129,30 @@ __device__ __forceinline__ void lean_merge(uint32_t wa, int lane, uint64_t key, 
   thr = lds64(wa + 8 * (cap - 1));
 }
 
-// The visited set of common.cuh (Visited) with its state cut down to what changes: table pointer, epoch, insert count;
-// capacity, hash shift and the epoch/id split are read from the kernel parameters (constant bank) where they are used.
-// test_and_set: the first probe may have been done ahead of time (`pre`: slot pre_h was read as pre_cv after the last
-// store to the table).
-struct LeanVisited {
-  uint32_t* tab;
-  uint32_t epoch, used;
-};
-__device__ __forceinline__ bool lean_test_and_set(const VisitedCfg& c, LeanVisited& vis, int lane, uint32_t id, bool valid, bool pre,
-                                                  uint32_t pre_h, uint32_t pre_cv) {
-  const uint32_t want = (vis.epoch << c.id_bits) | id;
-  const uint64_t pol_keep = l2_policy_evict_last();
-  uint32_t h = pre ? pre_h : (id * 2654435761u) >> c.shift;
-  bool pending = valid, fresh = false, first = pre;
-  while (__any_sync(FULL, pending)) {
-    uint32_t cur = 0;
-    if (pending) cur = first ? pre_cv : ld_keep(vis.tab + h, pol_keep);
-    first = false;
-    bool claim = false;
-    if (pending) {
-      if (cur == want) {
-        pending = false;  // already visited
-      } else if ((cur >> c.id_bits) != vis.epoch) {
-        claim = true;  // stale or empty slot
-      } else {
-        h = (h + 1) & (c.cap - 1);
-      }
-    }
-    const unsigned claimers = __ballot_sync(FULL, claim);
-    if (claim) {
-      const unsigned same = __match_any_sync(claimers, h);
-      const int leader = __ffs(same) - 1;
-      const uint32_t lead_id = __shfl_sync(claimers, id, leader);
-      if (lane == leader) {
-        st_keep(vis.tab + h, want, pol_keep);
-        fresh = true;
-        pending = false;
-      } else if (lead_id == id) {
-        pending = false;  // the same id twice in one chunk: the leader records it
-      } else {
-        h = (h + 1) & (c.cap - 1);
-      }
-    }
-    __syncwarp();  // orders this round's stores before the next round's loads
-  }
-  vis.used += __popc(__ballot_sync(FULL, fresh));  // warp-uniform count
-  return fresh;
-}
-
 template <class Op, int CH, int QC, bool STATS>
 __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_kernel(SearchParams p) {
   typedef typename MaskSel<QC>::type MaskT;
   constexpr int NCH = QC / 32;
-  constexpr int WARP_SMEM = QC * 8 + 256;  // queue keys (also the query staging buffer), row ids, distances
+  constexpr LeanLayout L = lean_layout(QC);
   static_assert(CH * 128 <= QC * 8, "the query is staged in the queue buffer");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const GraphView& G = p.g;
   const int lane = (int)pin(threadIdx.x & 31);
   const int g = lane & 7, r = lane >> 3;
-  const uint32_t wa = pin(smem_u32(smem_raw) + (uint32_t)(threadIdx.x >> 5) * WARP_SMEM);
-  const uint32_t ca = wa + QC * 8, da = ca + 128;
+  const uint32_t wa = pin(smem_u32(smem_raw) + (uint32_t)(threadIdx.x >> 5) * L.bytes + L.queue);
+  const uint32_t ca = wa + L.cand_id, da = wa + L.cand_d;
   const char* const vecb = reinterpret_cast<const char*>(G.vec);
   constexpr uint32_t row_bytes = (uint32_t)CH * 128u;
   const uint64_t pol_rows = l2_policy_evict_first();
 
   const uint32_t slot = blockIdx.x * (LEAN_THREADS / 32) + (threadIdx.x >> 5);
-  LeanVisited vis;
-  vis.tab = p.vis.tables + (size_t)slot * p.vis.cap;
-  vis.epoch = p.vis.epochs[slot];
-  vis.used = 0;
+  Visited vis;
+  vis.init(p.vis, slot);
   unsigned evals = 0, expans = 0, adjr = 0;
   const int cap = p.ef;
 
   for (;;) {
-    uint32_t qi = 0;
-    if (lane == 0) qi = atomicAdd(p.work_counter, 1u);
-    qi = __shfl_sync(FULL, qi, 0);
+    const uint32_t qi = next_item(p.work_counter, lane);
     if (qi >= p.nq) break;
     // ---- the lane's chunks of the query (zero padded) -> registers, through the queue buffer
     {
@@ -236,7 +182,9 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
     for (int i = 0; i < CH; ++i) qv[i] = lds128(wa + 16 * (g + 8 * i));
     __syncwarp();
 
-    // ---- descent: ONE pass over pivot.neighbours[layer] per layer (hnsw.rs:1498-1529)
+    // ---- descent: ONE pass over pivot.neighbours[layer] per layer (hnsw.rs:1498-1529).  descend() (search_core.cuh) with
+    // lean_score as its chunk scorer computes the same, but the compiler then schedules and allocates this kernel differently
+    // (more registers in most instantiations, spills in the Jaccard ones with 512-byte rows); this copy keeps its code as tuned.
     uint32_t pivot = G.entry;
     if (lane == 0) sts32(ca, pivot);
     __syncwarp();
@@ -281,19 +229,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
     }
 
     // ---- search_layer on the lowest populated layer (hnsw.rs:1531-1542, 940-1057)
-    {  // a new search bumps the epoch instead of clearing the table (Visited::begin)
-      const uint32_t epoch_max = (p.vis.id_bits >= 32) ? 0u : ((1u << (32 - p.vis.id_bits)) - 1u);
-      if (vis.epoch >= epoch_max) {
-        for (uint32_t i = lane; i < p.vis.cap; i += 32) vis.tab[i] = 0u;
-        vis.epoch = 0;
-      }
-      vis.epoch += 1;
-      vis.used = 1;
-      __syncwarp();
-      // hnsw.rs:955-956: the table holds nothing of this epoch yet, the entry's home slot is free
-      if (lane == 0) st_keep(vis.tab + ((pivot * 2654435761u) >> p.vis.shift), (vis.epoch << p.vis.id_bits) | pivot, l2_policy_evict_last());
-    }
-    __syncwarp();
+    vis.begin(p.vis, pivot, lane);  // hnsw.rs:955-956
 #pragma unroll
     for (int c = 0; c < NCH; ++c) sts64(wa + 8 * (32 * c + lane), ~0ull);
     __syncwarp();
@@ -336,7 +272,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
         if (!use_pre) nid = (b + lane < lcap) ? ids[b + lane] : INVALID_ID;
         const unsigned valid = __ballot_sync(FULL, nid != INVALID_ID);
         if (STATS) adjr += __popc(valid);
-        const bool fresh = lean_test_and_set(p.vis, vis, lane, nid, nid != INVALID_ID, use_pre, pre_h, pre_cv);  // hnsw.rs:1016-1017
+        const bool fresh = vis.test_and_set(p.vis, lane, nid, nid != INVALID_ID, use_pre, pre_h, pre_cv);  // hnsw.rs:1016-1017
         const unsigned m = __ballot_sync(FULL, fresh);
         const int cnt = __popc(m);
         const bool last = valid != FULL || b + 32 >= lcap;
@@ -346,7 +282,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
             int pcap;
             const uint32_t* pids = list_ids(G, pre_c, p.layer0, pcap);
             pre_nid = (lane < pcap) ? pids[lane] : INVALID_ID;
-            pre_h = (pre_nid * 2654435761u) >> p.vis.shift;
+            pre_h = Visited::home(p.vis, pre_nid);
             pre_cv = 0;
             if (pre_nid != INVALID_ID) pre_cv = ld_keep(vis.tab + pre_h, l2_policy_evict_last());
             pre_ok = true;
@@ -371,31 +307,15 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
         }
         if (last) break;  // lists are dense prefixes terminated by INVALID_ID
       }
-      if (vis.used >= p.vis.cap - (p.vis.cap >> 2)) {
+      if (vis.overflowing(p.vis)) {
         overflow = true;
         break;
       }
     }
     // ---- ascending top-k (hnsw.rs:1544-1579); the queue is already sorted
-    int count = n < p.k ? n : p.k;  // hnsw.rs:1547 (n <= ef)
-    if (overflow) {
-      if (lane == 0) atomicExch(p.status, 1);
-      count = 0;
-    }
-    const size_t ob = (size_t)qi * p.k;
-    for (int j = lane; j < p.k; j += 32) {
-      if (j < count) {
-        const uint64_t key = lds64(wa + 8 * j);
-        const uint32_t id = key_id(key);
-        p.out_nb[ob + j] = NeighbourOut{G.origin[id], key_dist(key), id};
-      } else {
-        p.out_nb[ob + j] = NeighbourOut{~0ull, __int_as_float(0x7f800000), INVALID_ID};
-      }
-    }
-    if (lane == 0) p.out_count[qi] = count;
-    __syncwarp();
+    write_answers(p, lane, qi, overflow, n < p.k ? n : p.k, [&](int j) { return lds64(wa + 8 * j); });  // hnsw.rs:1547 (n <= ef)
   }
-  if (lane == 0) p.vis.epochs[slot] = vis.epoch;
+  vis.save(p.vis, slot, lane);
   if (STATS && p.stats && lane == 0) {
     atomicAdd(p.stats + 0, (unsigned long long)evals);
     atomicAdd(p.stats + 1, (unsigned long long)expans);
@@ -412,10 +332,8 @@ static cudaError_t launch_lean_kernel(const SearchParams& p, int grid, size_t sm
 template <class Op, int QC>
 static cudaError_t launch_lean_for_op(const SearchParams& p, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm) {
   const int ch = p.g.d4 / 8;
-#ifndef HB_FAST_BUILD
   if (ch == 1) return launch_lean_kernel<Op, 1, QC>(p, grid, smem, st, blocks_per_sm);
   if (ch == 2) return launch_lean_kernel<Op, 2, QC>(p, grid, smem, st, blocks_per_sm);
-#endif
   if (ch == 4) return launch_lean_kernel<Op, 4, QC>(p, grid, smem, st, blocks_per_sm);
   return cudaErrorInvalidValue;
 }
@@ -423,14 +341,8 @@ static cudaError_t launch_lean_for_op(const SearchParams& p, int grid, size_t sm
 // one translation unit per element type instantiates the kernels (search_lean_f32.cu, search_lean_u8.cu, search_lean_u16.cu)
 template <class Op>
 static cudaError_t launch_lean_op(const SearchParams& p, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm) {
-#ifdef HB_FAST_BUILD  // scripts/variants.sh: one instantiation, for A/B builds
-  if constexpr (std::is_same<Op, OpL2>::value) {
-    if (p.q_smem == 64) return launch_lean_for_op<Op, 64>(p, grid, smem, st, blocks_per_sm);
-  }
-#else
   if (p.q_smem == 64) return launch_lean_for_op<Op, 64>(p, grid, smem, st, blocks_per_sm);
   if (p.q_smem == 128) return launch_lean_for_op<Op, 128>(p, grid, smem, st, blocks_per_sm);
-#endif
   return cudaErrorInvalidValue;
 }
 

@@ -7,11 +7,9 @@ cudaError_t launch_search_lean_f32(const SearchParams& p, int metric, int grid, 
                                    int* blocks_per_sm) {
   switch (metric) {
     case METRIC_L2: return launch_lean_op<OpL2>(p, grid, smem, st, blocks_per_sm);
-#ifndef HB_FAST_BUILD
     case METRIC_L1: return launch_lean_op<OpL1>(p, grid, smem, st, blocks_per_sm);
     case METRIC_DOT: return launch_lean_op<OpDot>(p, grid, smem, st, blocks_per_sm);
     case METRIC_COSINE: return launch_lean_op<OpCosine>(p, grid, smem, st, blocks_per_sm);
-#endif
   }
   return cudaErrorInvalidValue;
 }
@@ -20,10 +18,8 @@ cudaError_t launch_search_lean_f32(const SearchParams& p, int metric, int grid, 
 cudaError_t launch_search_lean(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st,
                                int* blocks_per_sm) {
   if (dtype == DT_F32) return launch_search_lean_f32(p, metric, grid, smem, st, blocks_per_sm);
-#ifndef HB_FAST_BUILD
   if (dtype == DT_U8) return launch_search_lean_u8(p, metric, grid, smem, st, blocks_per_sm);
   if (dtype == DT_U16) return launch_search_lean_u16(p, metric, grid, smem, st, blocks_per_sm);
-#endif
   return cudaErrorInvalidValue;
 }
 

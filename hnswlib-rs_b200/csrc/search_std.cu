@@ -116,11 +116,10 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_std_kernel(SearchParams
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const GraphView& g = p.g;
   unsigned char* base = smem_raw + (size_t)warp * p.smem_per_warp;
-  // per-warp layout: [query][W heap: (ef + 1) items][row ids][distances]
-  uint4* q4 = reinterpret_cast<uint4*>(base);
-  SItem* wv = reinterpret_cast<SItem*>(base + (size_t)g.d4 * 16);
-  uint32_t* cand_id = reinterpret_cast<uint32_t*>(base + (size_t)g.d4 * 16 + (size_t)p.q_smem * 8);
-  float* cand_d = reinterpret_cast<float*>(cand_id + 32);
+  const StdLayout L = std_layout(g.d4, p.q_smem);
+  const WarpSmem s{reinterpret_cast<uint4*>(base + L.query), nullptr, reinterpret_cast<uint32_t*>(base + L.cand_id),
+                   reinterpret_cast<float*>(base + L.cand_d)};
+  SItem* wv = reinterpret_cast<SItem*>(base + L.heap);
   const uint32_t slot = blockIdx.x * (blockDim.x >> 5) + warp;  // the host launches fewer warps per CTA when shared memory is short
   Visited vis;
   vis.init(p.vis, slot);
@@ -130,24 +129,20 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_std_kernel(SearchParams
   const int ef = p.ef;
 
   for (;;) {
-    uint32_t qi = 0;
-    if (lane == 0) qi = atomicAdd(p.work_counter, 1u);
-    qi = __shfl_sync(FULL, qi, 0);
+    const uint32_t qi = next_item(p.work_counter, lane);
     if (qi >= p.nq) break;
-    stage_row_bytes(q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes, p.q_bytes, g.d4 * 16);
+    stage_row_bytes(s.q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes, p.q_bytes, g.d4 * 16);
     int count = 0;
     bool overflow = false;
     StdHeap W{wv, 0}, C{cv, 0};
     if (g.entry != INVALID_ID) {
       // ---- descent (hnsw.rs:1498-1529): strict '<' in list order, distances only: as in every kernel
-      const WarpSmem s{q4, nullptr, cand_id, cand_d};
-      const Entry e = descend<Op, 0, 2>(g, s, st);
+      const Entry e = descend<Op>(g, lane, st, WarpChunk<Op, 0, 2>{g, s, lane});
       const uint32_t pivot = e.pivot;
       const float best = e.best;
       // ---- search_layer, literally (hnsw.rs:940-1063)
-      vis.begin();
-      vis.test_and_set(pivot, lane == 0);  // 955-956
-      st.evals += 1;                       // 952: dist(q, ep), the value is `best`
+      vis.begin(p.vis, pivot, lane);  // 955-956
+      st.evals += 1;                  // 952: dist(q, ep), the value is `best`
       int wn = 0;
       if (lane == 0) {
         C.push(SItem{-best, pivot});  // 960-963
@@ -170,27 +165,27 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_std_kernel(SearchParams
           const uint32_t nid = (b + lane < cap) ? ids[b + lane] : INVALID_ID;
           const unsigned valid = __ballot_sync(FULL, nid != INVALID_ID);
           st.adj += __popc(valid);
-          const bool fresh = vis.test_and_set(nid, nid != INVALID_ID);  // 1016-1017
+          const bool fresh = vis.test_and_set(p.vis, lane, nid, nid != INVALID_ID);  // 1016-1017
           const unsigned m = __ballot_sync(FULL, fresh);
           const int cnt = __popc(m);
           if (cnt) {
             const int pos = __popc(m & ((1u << lane) - 1u));  // lane order == list order
-            if (fresh) cand_id[pos] = nid;
+            if (fresh) s.cand_id[pos] = nid;
             __syncwarp();
-            warp_dists<Op, 0, 2>(vec4, g.d4, g.dim, q4, cand_id, cnt, cand_d);  // 1026
+            warp_dists<Op, 0, 2>(vec4, g.d4, g.dim, s.q4, s.cand_id, cnt, s.cand_d);  // 1026
             __syncwarp();
             st.evals += cnt;
             if (lane == 0) {
               for (int i = 0; i < cnt; ++i) {
-                const float de = Op::post(cand_d[i]);
+                const float de = Op::post(s.cand_d[i]);
                 const SItem f2 = W.v[0];  // 1019-1024
                 if (de < f2.kd || W.n < ef) {  // 1028
                   if (C.n >= (int)p.ccap) {
                     overflow = true;
                     break;
                   }
-                  C.push(SItem{-de, cand_id[i]});  // 1035-1036
-                  W.push(SItem{de, cand_id[i]});   // 1038
+                  C.push(SItem{-de, s.cand_id[i]});  // 1035-1036
+                  W.push(SItem{de, s.cand_id[i]});   // 1038
                   if (W.n > ef) W.pop();           // 1051-1053
                 }
               }
@@ -199,7 +194,7 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_std_kernel(SearchParams
           }
           if (valid != FULL) break;
         }
-        overflow = __shfl_sync(FULL, (int)overflow, 0) != 0 || vis.overflowing();
+        overflow = __shfl_sync(FULL, (int)overflow, 0) != 0 || vis.overflowing(p.vis);
         if (overflow) break;
       }
       if (lane == 0) {
@@ -210,28 +205,10 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_std_kernel(SearchParams
       __syncwarp();
       count = min(p.k, min(ef, wn));  // 1547
     }
-    if (overflow) {
-      if (lane == 0) atomicExch(p.status, 1);
-      count = 0;
-    }
-    const size_t ob = (size_t)qi * p.k;
-    for (int j = lane; j < p.k; j += 32) {
-      if (j < count) {
-        const SItem it = wv[j];
-        p.out_nb[ob + j] = NeighbourOut{g.origin[it.id], it.kd, it.id};
-      } else {
-        p.out_nb[ob + j] = NeighbourOut{~0ull, __int_as_float(0x7f800000), INVALID_ID};
-      }
-    }
-    if (lane == 0) p.out_count[qi] = count;
-    __syncwarp();
+    write_answers(p, lane, qi, overflow, count, [&](int j) { return make_key(wv[j].kd, wv[j].id); });
   }
-  vis.save(p.vis, slot);
-  if (p.stats && lane == 0) {
-    atomicAdd(p.stats + 0, (unsigned long long)st.evals);
-    atomicAdd(p.stats + 1, (unsigned long long)st.expansions);
-    atomicAdd(p.stats + 2, (unsigned long long)st.adj);
-  }
+  vis.save(p.vis, slot, lane);
+  flush_stats(p.stats, st, lane);
 }
 
 cudaError_t launch_search_std(const SearchParams& p, int metric, int dtype, int grid, size_t smem, cudaStream_t st,
