@@ -653,7 +653,8 @@ static int search_device_any(const void* h, const int64_t* resident, const void*
   HB_HS(h);
   HB_NOT_PARTITIONED(ix, resident ? "search_device_filtered" : "search_device");
   const FilterArg f{0, nullptr, 0, nullptr, nullptr, resident};
-  return pass(ix, ix->search_device(f, d_queries, nq, knbn, ef_search, (NeighbourOut*)d_out, d_counts, sync != 0, kernel_ms));
+  return pass(ix, ix->search_device(f, false, d_queries, nq, knbn, ef_search, (NeighbourOut*)d_out, d_counts, sync != 0,
+                                    kernel_ms));
 }
 int hnsw_b200_search_device(const void* h, const void* d_queries, uint64_t nq, uint64_t knbn,
                             uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
@@ -662,6 +663,29 @@ int hnsw_b200_search_device(const void* h, const void* d_queries, uint64_t nq, u
 int hnsw_b200_search_device_filtered(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                      uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
   return search_device_any(h, &filter, d_queries, nq, knbn, ef_search, d_out, d_counts, sync, kernel_ms);
+}
+
+// Exact search: the exact scan of the points a resident filter admits (filter >= 0) or of every point (-1), through the
+// same batch driver and device-resident path as the graph searches
+int hnsw_b200_search_exact(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
+                           uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+  HB_HS(h);
+  if (nq == 0) return 0;
+  if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0) return set_err("bad argument");
+  HB_PARTS_SHARED_IF(ix);
+  FilterArg f;
+  if (filter != -1) f.resident = &filter;
+  HostBatch b{queries, nullptr, nq, (int)dim, knbn, 0, f, AnswerArrays{nullptr, out_ids, out_dist, out_internal, out_pid, out_counts}};
+  b.exact = true;
+  return pass(ix, ix->search_batch(b));
+}
+int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
+                                  void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
+  HB_HS(h);
+  HB_NOT_PARTITIONED(ix, "search_exact_device");
+  FilterArg f;
+  if (filter != -1) f.resident = &filter;
+  return pass(ix, ix->search_device(f, true, d_queries, nq, knbn, 0, (NeighbourOut*)d_out, d_counts, sync != 0, kernel_ms));
 }
 
 int64_t hnsw_b200_filter_new(const void* h, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,

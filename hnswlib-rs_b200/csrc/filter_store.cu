@@ -1,6 +1,7 @@
 // Resident filters (index.h FilterStore): a FilterT materialised once and kept on every device that searches with it.
 // No kernel of its own: a search with a resident filter runs the same filtered query kernel a per-call filter runs, on
-// a bitmap that is already on the device instead of one uploaded for the call.
+// a bitmap that is already on the device instead of one uploaded for the call.  An exact search with it runs the exact
+// scan over the filter's sorted id list, made from the bitmap at the first exact search on a device.
 #include "index.h"
 #include "partition.h"
 
@@ -12,13 +13,20 @@ static std::string unknown_filter(int64_t id) {
   return "filter " + std::to_string(id) + " is not a live filter of this handle (freed, or made on another handle)";
 }
 
+static void free_device_copies(FilterStore::Filter& f) {
+  for (auto& d : f.dev) {
+    cudaSetDevice(d.first.second);
+    cudaFree(d.second);
+  }
+  for (auto& d : f.ids) {
+    cudaSetDevice(d.first.second);
+    cudaFree(d.second.first);
+  }
+}
+
 FilterStore::~FilterStore() {
   DeviceRestore keep;
-  for (auto& kv : f_)
-    for (auto& d : kv.second.dev) {
-      cudaSetDevice(d.first.second);
-      cudaFree(d.second);
-    }
+  for (auto& kv : f_) free_device_copies(kv.second);
 }
 
 int64_t FilterStore::add(Filter&& f) {
@@ -33,7 +41,7 @@ bool FilterStore::has(int64_t id) {
   return f_.count(id) != 0;
 }
 
-int FilterStore::use(int64_t id, int p, int nparts, const Index* rx, const uint32_t** d_bits) {
+int FilterStore::use(int64_t id, int p, int nparts, const Index* rx, const uint32_t** d_bits, ExactScan* list) {
   std::lock_guard<std::mutex> lk(mu_);
   auto it = f_.find(id);
   if (it == f_.end()) return rx->fail(unknown_filter(id));
@@ -45,6 +53,27 @@ int FilterStore::use(int64_t id, int p, int nparts, const Index* rx, const uint3
     return rx->fail("filter " + std::to_string(id) + " is stale: it covers " + std::to_string(f.counts[p]) + " points and the " +
                     (nparts > 1 ? "partition" : "index") + " now holds " + std::to_string(rx->n) + ": make a new filter");
   const std::pair<int, int> key(p, rx->device);
+  if (list) {
+    auto l = f.ids.find(key);
+    if (l == f.ids.end()) {  // first exact search on this device: the admitted ids in order, kept until the filter is freed
+      const std::vector<uint32_t>& b = f.bits[p];
+      std::vector<uint32_t> ids;
+      for (size_t i = 0; i < f.counts[p]; ++i)
+        if ((b[i >> 5] >> (i & 31)) & 1u) ids.push_back((uint32_t)i);
+      DeviceRestore keep;
+      void* ptr = nullptr;
+      cudaError_t e;
+      if ((e = cudaSetDevice(rx->device)) != cudaSuccess || (e = cudaMalloc(&ptr, std::max<size_t>(1, ids.size()) * 4)) != cudaSuccess ||
+          (e = cudaMemcpy(ptr, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice)) != cudaSuccess) {
+        cudaFree(ptr);
+        return rx->cuda_fail(e, "filter id list upload");
+      }
+      l = f.ids.emplace(key, std::make_pair(ptr, ids.size())).first;
+    }
+    list->ids = (const uint32_t*)l->second.first;
+    list->n = l->second.second;
+    return 0;
+  }
   auto d = f.dev.find(key);
   if (d == f.dev.end()) {  // first use on this device: one copy, kept until the filter is freed
     DeviceRestore keep;
@@ -67,10 +96,7 @@ void FilterStore::erase(int64_t id) {
   auto it = f_.find(id);
   if (it == f_.end()) return;
   DeviceRestore keep;
-  for (auto& d : it->second.dev) {
-    cudaSetDevice(d.first.second);
-    cudaFree(d.second);
-  }
+  free_device_copies(it->second);
   f_.erase(it);
 }
 
@@ -103,7 +129,7 @@ int64_t Index::new_filter(int mode, const uint64_t* sorted_ids, size_t nids, int
 
 int Index::free_filter(int64_t id) {
   if (!filters.has(id)) return fail(unknown_filter(id));
-  // an asynchronous search_device launch may still read the bitmap: wait for the contexts those launches run on
+  // an asynchronous search_device / search_exact_device launch may still read the bitmap or the id list: wait for the contexts those launches run on
   DeviceRestore keep;
   HB_CUDA(cudaSetDevice(device));
   for (int i = NCTX; i < NCTX + NASYNC; ++i) HB_CUDA(cudaStreamSynchronize(ctx_[i].stream));

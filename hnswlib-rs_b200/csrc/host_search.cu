@@ -1,6 +1,6 @@
 // Host search batches (index.h "host searches"): every host entry point's batch is planned into legs, each leg is begun
 // and finished on its Index, and the answers are written into the caller's AnswerArrays.  No kernel of its own: a leg
-// runs the ordinary query kernels through search_host_begin / search_host_finish.
+// runs the ordinary query kernels, or for an exact batch the exact scan (aux.cu), through search_host_begin / finish.
 //
 // A leg is leased, begun, finished and written, and its context released.  Every begun leg is collected, also after
 // another leg failed, and a leg whose enqueue failed has its stream synchronised before its context is released.  Who
@@ -93,9 +93,11 @@ static void put_slice(const AnswerArrays& out, const Index* rx, size_t first, si
     memcpy(out.nb + o, a, tot * sizeof(NeighbourOut));
     return;
   }
-  uint64_t* ids = out.ids + o;
+  if (out.ids) {
+    uint64_t* ids = out.ids + o;
+    for (size_t s = 0; s < tot; ++s) ids[s] = a[s].origin;
+  }
   float* dist = out.dist + o;
-  for (size_t s = 0; s < tot; ++s) ids[s] = a[s].origin;
   for (size_t s = 0; s < tot; ++s) dist[s] = a[s].dist;
   if (out.internal) {
     uint32_t* internal = out.internal + o;
@@ -113,7 +115,7 @@ static inline void put_answer(const AnswerArrays& out, size_t s, const Index* rx
     out.nb[s] = NeighbourOut{e.origin, e.dist, internal};
     return;
   }
-  out.ids[s] = e.origin;
+  if (out.ids) out.ids[s] = e.origin;
   out.dist[s] = e.dist;
   if (out.internal) out.internal[s] = internal;
   if (out.pid) point_id(rx, e.internal, out.pid + 2 * s);
@@ -170,7 +172,7 @@ int Index::plan(size_t nq, std::vector<Leg>& legs) {
   return 0;
 }
 
-int Index::resolve_filter(const FilterArg& f, Leg* legs, size_t n, std::vector<std::vector<uint32_t>>& bits) {
+int Index::resolve_filter(const FilterArg& f, bool exact, Leg* legs, size_t n, std::vector<std::vector<uint32_t>>& bits) {
   const int P = parts ? parts->count() : 1;
   int r = 0;
   if (f.mode) {
@@ -186,7 +188,7 @@ int Index::resolve_filter(const FilterArg& f, Leg* legs, size_t n, std::vector<s
     for (size_t i = 0; i < n; ++i) legs[i].host_bits = bits[legs[i].part].data();
   }
   for (Leg* l = legs; f.resident && l < legs + n; ++l)  // every leg, so that the caller reports the failure it chooses
-    if (filters.use(*f.resident, l->part, P, l->rx, &l->dev_bits)) r = l->rc = -1;
+    if (filters.use(*f.resident, l->part, P, l->rx, &l->dev_bits, exact ? &l->scan : nullptr)) r = l->rc = -1;
   return r;
 }
 
@@ -207,7 +209,7 @@ void Index::begin_leg(const HostBatch& b, Leg& l) {
   if (l.ctx < 0) l.ctx = l.rx->acquire_ctx();
   const void* q = b.rows ? nullptr : (const char*)b.queries + l.first * (size_t)b.d * es;
   l.rc = l.rx->search_host_begin(l.ctx, q, b.rows ? b.rows + l.first : nullptr, l.count, b.d, b.k, b.ef, l.host_bits,
-                                 l.dev_bits);
+                                 l.dev_bits, b.exact ? &l.scan : nullptr);
   l.begun = l.rc == 0;
 }
 
@@ -243,7 +245,7 @@ int Index::search_batch(const HostBatch& b) {
   if ((r = plan(b.nq, legs))) return r;
   const int n = (int)legs.size();
   const bool sharded = n > 1 && !parts;
-  if (resolve_filter(b.filter, legs.data(), n, bits)) return legs_fail(legs.data(), n, sharded);
+  if (resolve_filter(b.filter, b.exact, legs.data(), n, bits)) return legs_fail(legs.data(), n, sharded);
   if (n == 1 && !parts) {
     begin_leg(b, legs[0]);
     return end_leg(legs[0], b.k, b.out);
@@ -283,7 +285,7 @@ int64_t Index::submit_batch(const HostBatch& b) {
   std::vector<std::vector<uint32_t>> bits;
   int r;
   if ((r = plan(b.nq, t.legs))) return r;
-  if (resolve_filter(b.filter, t.legs.data(), t.legs.size(), bits)) return legs_fail(t.legs.data(), t.legs.size(), false);
+  if (resolve_filter(b.filter, b.exact, t.legs.data(), t.legs.size(), bits)) return legs_fail(t.legs.data(), t.legs.size(), false);
   int bad = -1;
   for (size_t i = 0; i < t.legs.size() && bad < 0; ++i) {  // one after the other, on the calling thread
     begin_leg(b, t.legs[i]);

@@ -99,7 +99,7 @@ Index::~Index() {
   for (SearchCtx& c : ctx_) {
     if (c.stream) cudaStreamSynchronize(c.stream);
     cudaFree(c.vis.tab); cudaFree(c.vis.epoch); cudaFree(c.fvis.tab); cudaFree(c.fvis.epoch); cudaFree(c.d_counter); cudaFree(c.d_status);
-    cudaFree(c.d_fbits); cudaFree(c.d_cbuf);
+    cudaFree(c.d_fbits); cudaFree(c.d_cbuf); cudaFree(c.d_xq); cudaFree(c.d_xpart);
     if (c.h_pin) cudaFreeHost(c.h_pin);
     if (c.h_res) cudaFreeHost(c.h_res);
     if (c.fork) cudaEventDestroy(c.fork);
@@ -613,22 +613,26 @@ void Index::release_ctx(int c) {
 // is forked from the handle's stream (it waits for everything enqueued there so far) onto the next of two alternating
 // context streams, so that two consecutive launches overlap.  The handle's stream does NOT wait for it: join() (or
 // check_status, set_stream, any synchronous call's own synchronisation) makes it do so; stream_wait_last() makes any
-// stream wait for the most recent launch alone.
-int Index::search_device(const FilterArg& f, const void* d_queries, size_t nq, size_t k, size_t ef_arg, NeighbourOut* d_out,
-                         int32_t* d_counts, bool sync, float* kernel_ms) {
+// stream wait for the most recent launch alone.  The same for the exact scan (`exact`).
+int Index::search_device(const FilterArg& f, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef_arg,
+                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms) {
   Leg leg{this};
   std::vector<std::vector<uint32_t>> bits;
   int r;
-  if (resolve_filter(f, &leg, 1, bits)) return legs_fail(&leg, 1, false);
+  if (resolve_filter(f, exact, &leg, 1, bits)) return legs_fail(&leg, 1, false);
   const uint32_t* d_filter_bits = leg.dev_bits;
   if (nq == 0) return 0;
   HB_CUDA(cudaSetDevice(device));
+  auto run = [&](SearchCtx& c, bool s, float* ms) {
+    return exact ? exact_on_ctx(c, d_queries, nq, k, leg.scan, d_out, d_counts, s, ms)
+                 : search_on_ctx(c, d_queries, nq, k, ef_arg, d_filter_bits, d_out, d_counts, s, ms);
+  };
   if (sync) {
     CtxLease lease(this);
     SearchCtx& c = ctx_[lease.c];
     HB_CUDA(cudaEventRecord(c.fork, stream_));
     HB_CUDA(cudaStreamWaitEvent(c.stream, c.fork, 0));
-    return search_on_ctx(c, d_queries, nq, k, ef_arg, d_filter_bits, d_out, d_counts, true, kernel_ms);
+    return run(c, true, kernel_ms);
   }
   int ci;
   {
@@ -638,7 +642,7 @@ int Index::search_device(const FilterArg& f, const void* d_queries, size_t nq, s
   SearchCtx& c = ctx_[ci];
   HB_CUDA(cudaEventRecord(c.fork, stream_));
   HB_CUDA(cudaStreamWaitEvent(c.stream, c.fork, 0));
-  r = search_on_ctx(c, d_queries, nq, k, ef_arg, d_filter_bits, d_out, d_counts, false, nullptr);
+  r = run(c, false, nullptr);
   if (r) return r;
   HB_CUDA(cudaEventRecord(c.join, c.stream));
   last_async_ = ci;
@@ -780,7 +784,7 @@ static const void* device_view_of_host(const void* p) {
 // synchronisation.  Pageable queries and row pointers are gathered into the context's own pinned staging buffer first
 // (the only host-side copy), which the kernel then reads the same way.
 int Index::search_host_begin(int ci, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                             const uint32_t* filter_bits_host, const uint32_t* d_filter_bits) {
+                             const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const ExactScan* scan) {
   SearchCtx& c = ctx_[ci];
   cudaStream_t st = c.stream;
   c.pend = SearchCtx::Pending();
@@ -821,6 +825,15 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
   if (!dv) return fail("the pinned result buffer has no device address");
   NeighbourOut* k_out = (NeighbourOut*)dv;
   int32_t* k_cnt = (int32_t*)(dv + out_bytes);
+  if (scan) {
+    // an exact launch may run many CTAs per query (row slices): the queries cross the bus once, into device memory
+    if ((r = ensure_scratch(&c.d_xq, &c.d_xq_bytes, qbytes, st))) return r;
+    HB_CUDA(cudaMemcpyAsync(c.d_xq, d_queries, qbytes, cudaMemcpyDefault, st));
+    *hstatus = 0;
+    c.pend.exact = true;
+    c.pend.enqueued = true;
+    return exact_on_ctx(c, c.d_xq, nq, k, *scan, k_out, k_cnt, false, nullptr);
+  }
   const uint32_t* dfb = d_filter_bits;  // a resident filter: already on this device
   if (filter_bits_host) {
     const size_t fb = ((n + 31) / 32) * 4;
@@ -849,7 +862,7 @@ int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** 
   if (!p.enqueued) return 0;  // empty batch or empty index: the answers (if any) were filled by search_host_begin
   HB_CUDA(cudaSetDevice(device));
   HB_CUDA(cudaStreamSynchronize(st));
-  if (*p.hstatus == 0) return 0;
+  if (p.exact || *p.hstatus == 0) return 0;
   HB_CUDA(cudaMemsetAsync(c.d_status, 0, sizeof(int), st));
   return search_on_ctx(c, p.d_queries, p.nq, p.k, p.ef, p.dfb, p.k_out, p.k_cnt, true, nullptr);  // grows the tables
 }

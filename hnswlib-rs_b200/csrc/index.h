@@ -104,6 +104,13 @@ int dtype_from_type_name(const std::string& s);
 
 class Index;
 
+// The points an exact scan (exact_knn_kernel, aux.cu) covers: `ids`, n sorted internal ids on the scanning device, or
+// every stored point (ids == nullptr)
+struct ExactScan {
+  const uint32_t* ids = nullptr;
+  size_t n = 0;
+};
+
 // Resident filters (hnsw_b200_filter_new, filter_store.cu): a FilterT materialised once per handle, as one bitmap per
 // partition (one for an ordinary handle) over the points stored when it was made.  The host copy stays; each device a
 // search uses it on gets one device copy, made at its first use there.  Ids are unique over all handles, so an id that
@@ -115,6 +122,9 @@ class FilterStore {
     std::vector<std::vector<uint32_t>> bits;  // [partition] bit per internal id (make_filter_bits)
     std::vector<size_t> counts;               // [partition] points stored when the filter was made
     std::map<std::pair<int, int>, void*> dev;  // (partition, device) -> device copy of bits[partition]
+    // (partition, device) -> the admitted internal ids of bits[partition], sorted, on the device, and their count; made
+    // at the first exact search with the filter there
+    std::map<std::pair<int, int>, std::pair<void*, size_t>> ids;
   };
   FilterStore() = default;
   FilterStore(const FilterStore&) = delete;
@@ -123,8 +133,9 @@ class FilterStore {
   int64_t add(Filter&& f);
   bool has(int64_t id);
   // the device copy of partition p's bitmap on rx's device (copied there on first use), after checking that the filter
-  // exists and that rx, partition p of `nparts`, still holds the points the filter was made over; if not, rx's error
-  int use(int64_t id, int p, int nparts, const Index* rx, const uint32_t** d_bits);
+  // exists and that rx, partition p of `nparts`, still holds the points the filter was made over; if not, rx's error.
+  // With `list`, the sorted id list of the admitted points instead (made and copied there on first use).
+  int use(int64_t id, int p, int nparts, const Index* rx, const uint32_t** d_bits, ExactScan* list = nullptr);
   void erase(int64_t id);  // frees its device copies; the caller waited for every search that may read them
 
  private:
@@ -187,7 +198,8 @@ struct FilterArg {
   const int64_t* resident = nullptr;
 };
 
-// One host search batch: flat queries or one pointer per query (rows), k answers each into `out`
+// One host search batch: flat queries or one pointer per query (rows), k answers each into `out`.  `exact`: the exact
+// scan of the points the filter admits (ef unused) instead of the graph search.
 struct HostBatch {
   const void* queries = nullptr;
   const void* const* rows = nullptr;
@@ -196,10 +208,11 @@ struct HostBatch {
   size_t k = 0, ef = 0;
   FilterArg filter;
   AnswerArrays out;
+  bool exact = false;
 };
 
 // One Index's part of a batch: queries [first, first + count) searched on rx (the handle, a replica, or partition `part`)
-// on its leased context ctx, with the filter bits resolve_filter gave it
+// on its leased context ctx, with the filter bits resolve_filter gave it, or for an exact batch the points to scan
 struct Leg {
   Index* rx = nullptr;
   int part = 0;
@@ -207,6 +220,7 @@ struct Leg {
   int ctx = -1;  // -1: not leased
   const uint32_t* host_bits = nullptr;
   const uint32_t* dev_bits = nullptr;
+  ExactScan scan;
   bool begun = false;  // enqueued
   int rc = 0;
 };
@@ -248,9 +262,10 @@ class Index {
                    const float* const* dists);
   // host queries (flat or row pointers) on leased context c, answers left in the context's pinned buffer (valid until
   // it is released).  The filter is either host bits, uploaded into the context for this call, or d_filter_bits already
-  // on this device (a resident filter); at most one of the two is non-null.
+  // on this device (a resident filter); at most one of the two is non-null.  With `scan`, the exact scan of those points
+  // instead of the graph search (no filter bits, ef unused).
   int search_host_begin(int c, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                        const uint32_t* filter_bits_host, const uint32_t* d_filter_bits);
+                        const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const ExactScan* scan = nullptr);
   int search_host_finish(int c, const NeighbourOut** out, const int32_t** counts);
   // host search batches (host_search.cu): synchronous, or submitted now and collected by finish_batch
   struct Ticket {
@@ -268,10 +283,11 @@ class Index {
   }
   // the filter bits of legs[0, n): a FilterT's host bits, made on the calling thread once per partition (a replica
   // shares the handle's internal ids, and so its bits) into `bits`, or a resident filter's copy on each leg's device.
-  // Nonzero when a leg could not have them; that leg's rc is set (legs_fail reports it).
-  int resolve_filter(const FilterArg& f, Leg* legs, size_t n, std::vector<std::vector<uint32_t>>& bits);
-  // device queries in, device answers out; the filter is none or a resident filter
-  int search_device(const FilterArg& f, const void* d_queries, size_t nq, size_t k, size_t ef, NeighbourOut* d_out,
+  // Nonzero when a leg could not have them; that leg's rc is set (legs_fail reports it).  `exact`: each leg's ExactScan
+  // instead (the resident filter's id list on the leg's device, or every point).
+  int resolve_filter(const FilterArg& f, bool exact, Leg* legs, size_t n, std::vector<std::vector<uint32_t>>& bits);
+  // device queries in, device answers out; the filter is none or a resident filter.  `exact`: the exact scan (ef unused).
+  int search_device(const FilterArg& f, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef, NeighbourOut* d_out,
                     int32_t* d_counts, bool sync, float* kernel_ms);
   // filter materialisation: bit per internal id from a sorted origin-id list or a callback
   int make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx,
@@ -334,12 +350,15 @@ class Index {
     VisitedPool vis, fvis;  // unfiltered / filtered searches
     void *d_fbits = nullptr, *d_cbuf = nullptr;
     size_t d_fbits_bytes = 0, d_cbuf_bytes = 0;
+    void *d_xq = nullptr, *d_xpart = nullptr;  // exact scan: the host batch's queries on the device / tickets and slice lists
+    size_t d_xq_bytes = 0, d_xpart_bytes = 0;
     void *h_pin = nullptr, *h_res = nullptr;  // pinned, mapped: query staging / answers
     size_t h_pin_bytes = 0, h_res_bytes = 0;
     bool busy = false;
     struct Pending {  // a host search enqueued by search_host_begin, completed by search_host_finish
       const void* d_queries = nullptr;
       const uint32_t* dfb = nullptr;
+      bool exact = false;  // an exact scan: no status, nothing to re-run
       NeighbourOut *k_out = nullptr, *hout = nullptr;
       int32_t *k_cnt = nullptr, *hcnt = nullptr, *hstatus = nullptr;
       size_t nq = 0, k = 0, ef = 0;
@@ -450,6 +469,9 @@ class Index {
   SearchCtx ctx_[NCTX + NASYNC];
   int search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const uint32_t* d_filter_bits,
                     NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms);
+  // the exact k nearest of device queries among scan's points (aux.cu); the slices' scratch is sized before the launch
+  int exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const ExactScan& scan, NeighbourOut* d_out,
+                   int32_t* d_counts, bool sync, float* kernel_ms);
   std::mutex ctx_mu_;
   std::condition_variable ctx_cv_;
   std::mutex ticket_mu_;

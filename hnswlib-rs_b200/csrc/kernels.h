@@ -120,6 +120,25 @@ __host__ __device__ inline InsertLayout insert_layout(int d4, int ef_c, int deg0
   return l;
 }
 
+// exact k-NN kernel (aux.cu), per CTA: [query tile, tq rows][row ring, stages x rows][tq queues of k keys]
+// [candidates, tq x rows keys][tq queue thresholds][tq candidate counts][tq queue lengths][stages mbarriers]
+struct ExactLayout {
+  size_t query, ring, queue, cand, thr, ccount, qn, bar, bytes;
+};
+__host__ __device__ inline ExactLayout exact_layout(int d4, int k, int tq, int rows, int stages) {
+  ExactLayout l;
+  l.query = 0;
+  l.ring = (size_t)tq * d4 * 16;
+  l.queue = l.ring + (size_t)stages * rows * d4 * 16;
+  l.cand = l.queue + (size_t)tq * k * 8;
+  l.thr = l.cand + (size_t)tq * rows * 8;
+  l.ccount = l.thr + (size_t)tq * 8;
+  l.qn = l.ccount + (size_t)tq * 4;
+  l.bar = (l.qn + (size_t)tq * 4 + 15) & ~(size_t)15;
+  l.bytes = round128(l.bar + (size_t)stages * 8);
+  return l;
+}
+
 // Queue kind for a given ef (see QueueSel): compile-time chunked shared-memory queue up to ef = 256, generic beyond.
 // (A register-resident variant spilled at 64 registers/thread, and a speculative two-candidates-per-iteration loop was
 // exact but slower; both were removed.)

@@ -97,6 +97,8 @@ def load_library():
     L.hnsw_b200_search_flat_submit_filtered.restype = i64
     L.hnsw_b200_search_flat_submit_filtered.argtypes = [vp, i64, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_device_filtered.argtypes = [vp, i64, vp, u64, u64, u64, vp, vp, i32, vp]
+    L.hnsw_b200_search_exact.argtypes = [vp, i64, vp, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_exact_device.argtypes = [vp, i64, vp, u64, u64, vp, vp, i32, vp]
     L.hnsw_b200_get_stats.argtypes = [vp, vp, i32]
     L.hnsw_b200_set_stream.argtypes = [vp, vp]
     L.hnsw_b200_join.argtypes = [vp]
@@ -187,8 +189,8 @@ def _filter_args(filter):
 
 class ResidentFilter:
     """A FilterT materialised once on the device (hnsw_b200_filter_new), made by Hnsw.make_filter and passed as
-    `filter=` to search_flat, search_filter, submit_flat and search_device.  It covers the points stored when it was
-    made: after an insert, searches with it are refused.  free() (or leaving a `with` block) releases it; the handle
+    `filter=` to search_flat, search_filter, submit_flat, search_device, search_exact and search_exact_device.  It
+    covers the points stored when it was made: after an insert, searches with it are refused.  free() (or leaving a `with` block) releases it; the handle
     frees the filters still alive when it is closed.  Not freed by garbage collection: free() waits for the handle's
     submitted batches, so a thread must collect its own tickets first."""
 
@@ -205,6 +207,15 @@ class ResidentFilter:
 
     def __exit__(self, *exc):
         self.free()
+
+
+def _filter_id(filter):
+    """the filter argument of the exact searches: a ResidentFilter's id, or -1 (every point) for None"""
+    if filter is None:
+        return -1
+    if not isinstance(filter, ResidentFilter):
+        raise TypeError("the exact searches take a ResidentFilter (Hnsw.make_filter) or None as their filter")
+    return filter.id
 
 
 class Hnsw:
@@ -384,6 +395,20 @@ class Hnsw:
                                                 _p(o), _p(ds), _p(it), _p(pid), _p(cnt)))
         return o, ds, it, pid, cnt
 
+    def search_exact(self, queries, knbn, filter=None, with_internal=True, with_pid=True):
+        """hnsw_b200_search_exact: the exact knbn nearest among the points a ResidentFilter admits (None: every point).
+        Returns search_flat's (origin, dist, internal | None, pid | None, counts)."""
+        q = np.ascontiguousarray(queries, self.dtype)
+        nq, d = q.shape
+        o = np.empty((nq, knbn), np.uint64)
+        ds = np.empty((nq, knbn), np.float32)
+        it = np.empty((nq, knbn), np.uint32) if with_internal else None
+        pid = np.empty((nq, knbn, 2), np.int32) if with_pid else None
+        cnt = np.empty(nq, np.int32)
+        self._chk(self._L.hnsw_b200_search_exact(self._h, _filter_id(filter), _p(q), nq, d, int(knbn), _p(o), _p(ds), _p(it),
+                                                 _p(pid), _p(cnt)))
+        return o, ds, it, pid, cnt
+
     def make_filter(self, filter):
         """hnsw_b200_filter_new: materialise a FilterT (sorted id sequence or callable(id)->bool, as search_flat takes)
         once, over the points stored now; a callable is called once per stored point, here.  Returns a ResidentFilter."""
@@ -494,6 +519,15 @@ class Hnsw:
             self._chk(self._L.hnsw_b200_search_device_filtered(self._h, filter.id, *args))
         else:
             raise TypeError("search_device takes a ResidentFilter (Hnsw.make_filter) as its filter")
+        return float(ms.value)
+
+    def search_exact_device(self, d_queries_ptr, nq, knbn, d_out_ptr, d_counts_ptr, sync=True, filter=None):
+        """hnsw_b200_search_exact_device: search_exact on device buffers, with search_device's outputs and rules.
+        Returns the kernel's CUDA-event time in ms when sync is true."""
+        ms = C.c_float(0.0)
+        self._chk(self._L.hnsw_b200_search_exact_device(self._h, _filter_id(filter), C.c_void_p(d_queries_ptr), nq, int(knbn),
+                                                        C.c_void_p(d_out_ptr), C.c_void_p(d_counts_ptr), int(bool(sync)),
+                                                        C.byref(ms) if sync else None))
         return float(ms.value)
 
     # ---- multi-GPU (include/hnsw_b200.h "Multi-GPU search")

@@ -67,6 +67,12 @@ extern "C" {
     fn hnsw_b200_search_device_filtered(h: *const HnswApif32, filter: i64, d_queries: *const c_void, nq: u64, knbn: u64,
                                         ef: u64, d_out: *mut c_void, d_counts: *mut i32, sync: c_int,
                                         kernel_ms: *mut f32) -> c_int;
+    // exact search (include/hnsw_b200.h "Exact search"): filter = a resident filter's id, or -1 for every point
+    fn hnsw_b200_search_exact(h: *const HnswApif32, filter: i64, queries: *const f32, nq: u64, dim: u64, knbn: u64,
+                              out_ids: *mut u64, out_dist: *mut f32, out_internal: *mut u32, out_pid: *mut i32,
+                              out_counts: *mut i32) -> c_int;
+    fn hnsw_b200_search_exact_device(h: *const HnswApif32, filter: i64, d_queries: *const c_void, nq: u64, knbn: u64,
+                                     d_out: *mut c_void, d_counts: *mut i32, sync: c_int, kernel_ms: *mut f32) -> c_int;
 }
 
 /// hnsw.rs:46
@@ -196,6 +202,19 @@ impl<D: DistName> Hnsw<D> {
                                            ids.as_mut_ptr(), ds.as_mut_ptr(), std::ptr::null_mut(), pid.as_mut_ptr(), &mut cnt)
         };
         assert_eq!(r, 0, "hnsw_b200_search_flat_filtered failed");
+        (0..cnt as usize).map(|j| Neighbour { d_id: ids[j] as usize, distance: ds[j], p_id: PointId(pid[2 * j] as u8, pid[2 * j + 1]) }).collect()
+    }
+    /// Extension: the exact `knbn` nearest among the points `filter` admits (None: every stored point)
+    pub fn search_exact(&self, data: &[f32], knbn: usize, filter: Option<&ResidentFilter<'_, D>>) -> Vec<Neighbour> {
+        let mut ids = vec![0u64; knbn];
+        let mut ds = vec![0f32; knbn];
+        let mut pid = vec![0i32; 2 * knbn];
+        let mut cnt = 0i32;
+        let r = unsafe {
+            hnsw_b200_search_exact(self.h, filter.map_or(-1, |f| f.id), data.as_ptr(), 1, data.len() as u64, knbn as u64,
+                                   ids.as_mut_ptr(), ds.as_mut_ptr(), std::ptr::null_mut(), pid.as_mut_ptr(), &mut cnt)
+        };
+        assert_eq!(r, 0, "hnsw_b200_search_exact failed");
         (0..cnt as usize).map(|j| Neighbour { d_id: ids[j] as usize, distance: ds[j], p_id: PointId(pid[2 * j] as u8, pid[2 * j + 1]) }).collect()
     }
     /// hnsw.rs:1612-1635: one answer per request, in input order

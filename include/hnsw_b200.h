@@ -308,6 +308,28 @@ int64_t hnsw_b200_search_flat_submit_filtered(const void* h, int64_t filter, con
 int hnsw_b200_search_device_filtered(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                      uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms);
 
+/* ---- Exact search: the exact k nearest neighbours among the points a resident filter admits (filter >= 0, a filter of
+ * h) or among every stored point (filter = -1), by a linear scan on the GPU.  Below a few per cent admitted, this is
+ * faster than a filtered graph search and has recall 1.
+ *   Answers: the first min(knbn, admitted) admitted points by (distance, internal id).  Each distance is bit-equal to
+ *     hnsw_b200_dist_batch's for that (query, point).
+ *   Ignored: there is no ef; the tie mode is ignored and hnsw_b200_get_stats is not touched.
+ *   Outputs: the columns and padding of hnsw_b200_search_flat (host variant) and hnsw_b200_search_device (device
+ *     variant), with that call's rules for sync, join, stream_wait_last and check_status.  An empty index gives every
+ *     count 0.
+ *   Filters: the stale, unknown and foreign filter rules of the _filtered calls apply.  The filter's sorted id list is
+ *     made from its bitmap at its first exact search on a device and freed with the filter; hnsw_b200_filter_free waits
+ *     for asynchronous exact launches too.
+ *   Partitioned handles: the host variant merges the partitions' answers by the rule of partitioned search (distance,
+ *     then partition, then position) and reports internal ids as global insertion ranks; the device variant is refused,
+ *     as search_device is.  A replicated handle shards the host variant like search_flat.  A partition view accepts -1
+ *     and reports its local ids.
+ *   Locks: the handle is taken shared, as for any search. */
+int hnsw_b200_search_exact(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
+                           uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
+int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
+                                  void* d_out, int32_t* d_counts, int sync, float* kernel_ms);
+
 /* Run this handle's kernels and copies on a caller-owned CUDA stream (cudaStream_t passed as void*; NULL
  * restores the handle's own stream), e.g. so that torch.cuda.Event on torch's current stream brackets them. */
 int hnsw_b200_join(void* h);
