@@ -4,7 +4,8 @@
 //            == /root/reference/src/hnsw.rs:1110-1205 (insert_slice) + 1299-1421 (select_neighbours)
 //   phase B (insert_link_kernel): reverse links under a per-point lock
 //            == /root/reference/src/hnsw.rs:1241-1289 (reverse_update_neighborhood_simple),
-//            including its quirk that every back-link is filed under the NEW point's level (1257).
+//            including its quirk that every back-link is filed under the NEW point's level (1257); with
+//            link mode 1 (hnsw_b200_set_link_mode) each back-link is filed in the layer it was made in instead.
 // The reference races inserts under parking_lot locks on a rayon pool (hnsw.rs:1224-1238); here a
 // batch of inserts searches the graph as it stood at the start of the batch (phase A is read-only
 // on other points' lists) and links afterwards; see DESIGN.md "batched insert".
@@ -258,9 +259,10 @@ __global__ void __launch_bounds__(BUILD_THREADS) insert_link_kernel(InsertParams
         if (q == INVALID_ID) break;
         if (q == x) continue;  // 1250
         const float d = own.dists[j];
-        // target list: q.neighbours[L] with L = the NEW point's level (1257); 2*max_nb_connection slots at layer 0
-        // (1272-1276).  Above plevel[q] it is a list no search can ever read, and is not materialised.
-        const List t = list_at(g, q, L);
+        // target list: q.neighbours[L] with L = the NEW point's level (1257), or in link mode 1 q.neighbours[l];
+        // 2*max_nb_connection slots at layer 0 (1272-1276).  Above plevel[q] it is a list no search can ever read, and
+        // is not materialised.  In mode 1 q was visited at layer l, so plevel[q] >= l and the list always exists.
+        const List t = list_at(g, q, p.link_mode ? l : L);
         if (!t.ids) continue;
         lock_point(p.locks, q);
         list_add_sorted(t.ids, t.dists, t.cap, x, d);

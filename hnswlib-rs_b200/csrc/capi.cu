@@ -513,6 +513,17 @@ int hnsw_b200_set_tie_mode(void* h, int mode) {
   apply(ix, [=](Index* x) { x->tie_std_ = mode == 1; });
   return 0;
 }
+int hnsw_b200_set_link_mode(void* h, int mode) {
+  HB_H(h);
+  HB_NOT_VIEW(ix);
+  if (mode != 0 && mode != 1) return set_err("link mode must be 0 (reference: new point's level) or 1 (per layer)");
+  apply(ix, [=](Index* x) { x->link_mode = mode; });
+  return 0;
+}
+int hnsw_b200_get_link_mode(const void* h) {
+  if (!h) return set_err("NULL handle");
+  return ((const AnyApi*)h)->ix->link_mode;
+}
 int hnsw_b200_set_searching_mode(void* h, int flag) {
   HB_H(h);
   HB_NOT_VIEW(ix);

@@ -350,6 +350,7 @@ int Index::run_insert_range(size_t first, size_t count, size_t mask_off) {
   p.ef_c = ef_c;
   p.keep_pruned = keep_pruned ? 1 : 0;
   p.extend = extend_candidates ? 1 : 0;
+  p.link_mode = link_mode;
   p.work_counter = d_counter_;
   p.locks = graph_.at<int>(GS::LOCKS);
   p.stats = stats_on_ ? d_stats_ : nullptr;  // insert-path distance evaluations / expansions / adjacency ids read

@@ -235,6 +235,7 @@ class Index {
   int M, max_layer, ef_c, metric, dtype, es, device;  // es = bytes per element
   size_t max_elements;
   bool extend_candidates = false, keep_pruned = false, searching = false;
+  int link_mode = 0;      // hnsw_b200_set_link_mode: 0 back-links under the new point's level (hnsw.rs:1257), 1 per layer
   bool tie_std_ = false;  // hnsw_b200_set_tie_mode: equal-distance ties resolved like the reference's std BinaryHeaps (search_std.cu)
   double level_scale;  // 1/ln(M) * factor
   SplitMix64 rng{397};

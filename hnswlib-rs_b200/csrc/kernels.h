@@ -184,6 +184,7 @@ struct InsertParams {
   int ef_c;
   int keep_pruned;
   int extend;  // extend_candidates flag (hnsw.rs:858), only with ef_c > 2M
+  int link_mode;  // phase B target layer: 0 the new point's level (hnsw.rs:1257), 1 the layer being linked
   VisitedCfg vis;
   unsigned int* work_counter;
   int* locks;  // [capacity] per-point spin locks (phase B)

@@ -34,6 +34,7 @@ int Partitions::create(Index* parent, int nparts, const int* devices) {
     // the settings made on the handle so far; the level RNG stays with the handle (levels are drawn in global order)
     ix->extend_candidates = parent->extend_candidates;
     ix->keep_pruned = parent->keep_pruned;
+    ix->link_mode = parent->link_mode;
     ix->searching = parent->searching;
     ix->tie_std_ = parent->tie_std_;
     ix->level_scale = parent->level_scale;

@@ -74,9 +74,11 @@ def load_library():
     L.hnsw_b200_set_device.argtypes = [i32]
     L.hnsw_b200_free_neighbourhood.argtypes = [vp]
     L.hnsw_b200_free_vec_api.argtypes = [vp]
-    for name in ("set_extend_candidates", "set_keeping_pruned", "set_searching_mode", "enable_stats", "set_tie_mode"):
+    for name in ("set_extend_candidates", "set_keeping_pruned", "set_searching_mode", "enable_stats", "set_tie_mode",
+                 "set_link_mode"):
         getattr(L, "hnsw_b200_" + name).argtypes = [vp, i32]
     L.hnsw_b200_get_extend_candidates.argtypes = [vp]
+    L.hnsw_b200_get_link_mode.argtypes = [vp]
     L.hnsw_b200_modify_level_scale.argtypes = [vp, C.c_double]
     L.hnsw_b200_set_level_seed.argtypes = [vp, u64]
     L.hnsw_b200_get_nb_point.restype = u64
@@ -483,6 +485,17 @@ class Hnsw:
     def set_tie_mode(self, mode):
         """0: ties by (distance, id); 1: the reference's std-BinaryHeap tie behaviour (hnsw_b200_set_tie_mode)"""
         self._chk(self._L.hnsw_b200_set_tie_mode(self._h, int(mode)))
+
+    def set_link_mode(self, mode):
+        """0: back-links filed under the new point's level, like the reference; 1: under the layer they were found in
+        (hnsw_b200_set_link_mode).  Applies to inserts made afterwards."""
+        self._chk(self._L.hnsw_b200_set_link_mode(self._h, int(mode)))
+
+    def get_link_mode(self):
+        m = int(self._L.hnsw_b200_get_link_mode(self._h))
+        if m < 0:
+            raise HnswError(last_error())
+        return m
 
     def get_stats(self, reset=True):
         out = np.zeros(4, np.uint64)

@@ -47,6 +47,9 @@ extern "C" {
     fn hnsw_b200_set_keeping_pruned(h: *mut HnswApif32, flag: c_int) -> c_int;
     fn hnsw_b200_modify_level_scale(h: *mut HnswApif32, scale: f64) -> c_int;
     fn hnsw_b200_set_searching_mode(h: *mut HnswApif32, flag: c_int) -> c_int;
+    // reverse-link layer of later inserts (include/hnsw_b200.h): 0 the reference's rule, 1 per layer
+    fn hnsw_b200_set_link_mode(h: *mut HnswApif32, mode: c_int) -> c_int;
+    fn hnsw_b200_get_link_mode(h: *const HnswApif32) -> c_int;
     fn hnsw_b200_get_nb_point(h: *const HnswApif32) -> u64;
     // multi-GPU (include/hnsw_b200.h "Multi-GPU search"): one process drives several devices
     fn hnsw_b200_replicate(h: *mut HnswApif32, ndev: c_int, devices: *const c_int) -> c_int;
@@ -134,6 +137,13 @@ impl<D: DistName> Hnsw<D> {
     pub fn set_keeping_pruned(&mut self, flag: bool) { unsafe { hnsw_b200_set_keeping_pruned(self.h, flag as c_int); } }
     pub fn modify_level_scale(&mut self, s: f64) { unsafe { hnsw_b200_modify_level_scale(self.h, s); } }
     pub fn set_searching_mode(&mut self, flag: bool) { unsafe { hnsw_b200_set_searching_mode(self.h, flag as c_int); } }
+    /// Extension: 0 files every back-link of a later insert under the new point's level, as hnsw.rs:1257 does; 1 files
+    /// it in the layer where the link was made.  Err on any other mode.
+    pub fn set_link_mode(&mut self, mode: i32) -> Result<(), i32> {
+        let r = unsafe { hnsw_b200_set_link_mode(self.h, mode as c_int) };
+        if r == 0 { Ok(()) } else { Err(r) }
+    }
+    pub fn get_link_mode(&self) -> i32 { unsafe { hnsw_b200_get_link_mode(self.h) as i32 } }
     /// Extension: copy the index to `devices[1..]` (devices[0] = the device it lives on); `parallel_search` then shards its
     /// batch over all of them, one call as on the CPU (hnsw.rs:1612-1635).
     pub fn replicate(&mut self, devices: &[i32]) -> Result<(), i32> {

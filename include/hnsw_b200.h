@@ -226,6 +226,17 @@ int hnsw_b200_set_searching_mode(void* h, int flag);     /* hnsw.rs:834 */
  * (Ord = distance only, /root/reference/src/hnsw.rs:273-297, 940-1053, 1544) replayed literally: same neighbour ids as the
  * reference on tie-heavy metrics (Hamming, Jaccard, integer L1), several times slower (one lane drives the heaps). */
 int hnsw_b200_set_tie_mode(void* h, int mode);
+/* Which layer an insert files its back-links in.  0 (default): the reference's rule, every back-link of a new point x goes
+ * to the neighbour's list of x's OWN level (the reference's src/hnsw.rs:1257), so a point of level >= 1 gets no layer-0
+ * in-links from its own insert; bit-identical to the reference's graph.  1: the per-layer rule of Malkov & Yashunin
+ * (Algorithm 1), the link (q, d) found at layer l adds (x, d) to q's layer-l list, with the reference's duplicate check,
+ * (distance, id) order, M / 2M capacity and truncation.  Gains: upper-level points keep their layer-0 in-links; recall at a
+ * given ef rose on uniform data but, at the c2 shape, only from ef = 96 on (DESIGN.md §4.3).  Gives up: the graph is no
+ * longer the one the reference would build (it is still a valid reference dump that hnsw_rs loads and searches).
+ * Applies to inserts made after the call; a reloaded dump starts in mode 0.
+ * Any other mode is refused and changes nothing.  A partition view refuses it; a partitioned handle passes it on. */
+int hnsw_b200_set_link_mode(void* h, int mode);
+int hnsw_b200_get_link_mode(const void* h);  /* the mode, or -1 on a NULL handle */
 int hnsw_b200_set_level_seed(void* h, uint64_t seed);
 uint64_t hnsw_b200_get_nb_point(const void* h);          /* hnsw.rs:810 */
 int hnsw_b200_get_max_level_observed(const void* h);     /* hnsw.rs:474 */
