@@ -76,6 +76,7 @@ struct ExactParams {
   unsigned* tickets;     // slices > 1: [tiles], zero at launch; the merging CTA leaves them zero
   NeighbourOut* out;     // [nq][k]
   int32_t* counts;       // [nq]
+  const ExactTile* tiles;  // nullptr: tile t is queries [t * tq, t * tq + tq) over (list, npts); else tile t is tiles[t]
 };
 
 // keys[0, c) (~0 = none) into the warp's sorted queue Q, 32 at a time: those Q accepts, inserted in lane order.  The keys
@@ -112,10 +113,18 @@ __global__ void __launch_bounds__(256, 2) exact_knn_kernel(ExactParams p) {
   uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw + L.bar);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t tile = blockIdx.x / p.slices, slice = blockIdx.x % p.slices;
-  const uint32_t q0 = tile * tq;
-  const int nqt = (int)min((uint32_t)tq, p.nq - q0);
-  const uint32_t per = (p.npts + p.slices - 1) / p.slices;
-  const uint32_t lo = min(p.npts, slice * per), hi = min(p.npts, lo + per);
+  uint32_t q0 = tile * tq, npts = p.npts;
+  int nqt = (int)min((uint32_t)tq, p.nq - q0);
+  const uint32_t* list = p.list;
+  if (p.tiles) {  // a tile of its own size over its own points; its slices split those points
+    const ExactTile t = p.tiles[tile];
+    q0 = t.q0;
+    nqt = (int)t.nq;
+    list = t.list;
+    npts = t.npts;
+  }
+  const uint32_t per = (npts + p.slices - 1) / p.slices;
+  const uint32_t lo = min(npts, slice * per), hi = min(npts, lo + per);
   const uint32_t nblk = (hi - lo + B - 1) / B;
   const uint32_t row_bytes = (uint32_t)d4 * 16u;
   const uint4* vec4 = reinterpret_cast<const uint4*>(p.g.vec);
@@ -141,7 +150,7 @@ __global__ void __launch_bounds__(256, 2) exact_knn_kernel(ExactParams p) {
     if (lane == 0) mbar_expect_tx(br, row_bytes * cnt);
     __syncwarp();
     if (lane < cnt) {
-      const uint32_t id = p.list ? __ldg(p.list + first + lane) : first + lane;
+      const uint32_t id = list ? __ldg(list + first + lane) : first + lane;
       bulk_g2s(ring + ((size_t)(b % NS) * B + lane) * d4, vec4 + (size_t)id * d4, row_bytes, br, l2_policy_evict_first());
     }
   };
@@ -157,7 +166,7 @@ __global__ void __launch_bounds__(256, 2) exact_knn_kernel(ExactParams p) {
     mbar_wait(bar + slot, (b / NS) & 1u);
     const uint32_t first = lo + b * B;
     const bool row_ok = rs < (int)min((uint32_t)B, hi - first);
-    const uint32_t id = !row_ok ? 0u : p.list ? __ldg(p.list + first + rs) : first + rs;
+    const uint32_t id = !row_ok ? 0u : list ? __ldg(list + first + rs) : first + rs;
     const uint4* row = ring + ((size_t)slot * B + (row_ok ? rs : 0)) * d4 + g;
     uint4 x[CH > 0 ? CH : 1];
     if constexpr (CH > 0) {
@@ -270,7 +279,7 @@ static bool exact_shape(int d4, size_t k, size_t nq, ExactParams& p, size_t& sme
 }
 
 int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const ExactScan& scan, NeighbourOut* d_out,
-                        int32_t* d_counts, bool sync, float* kernel_ms) {
+                        int32_t* d_counts, bool sync, float* kernel_ms, const std::vector<ExactGroup>* groups) {
   if (k == 0) return fail("knbn must be positive");
   if (poisoned_) return fail(poison_msg_);
   cudaStream_t st = c.stream;
@@ -287,33 +296,72 @@ int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k
   p.list = scan.ids;
   p.npts = (uint32_t)(scan.ids ? scan.n : n);
   p.k = (int)k;
+  size_t widest_group = nq;
+  if (groups) {
+    widest_group = 0;
+    for (const ExactGroup& gr : *groups) widest_group = std::max(widest_group, gr.count);
+  }
   size_t smem = 0;
-  if (!exact_shape(p.g.d4, k, nq, p, smem)) return fail("k / dimension too large for the exact search kernel");
+  if (!exact_shape(p.g.d4, k, widest_group, p, smem)) return fail("k / dimension too large for the exact search kernel");
   auto launch = [&](int grid, int* blocks_per_sm) {
     return dispatch_op(metric, dtype, [&](auto tag) -> cudaError_t {
       return launch_exact_for_op<typename decltype(tag)::type>(p, grid, smem, st, blocks_per_sm);
     });
   };
-  // slices: the CTAs of a launch run in waves of `slots` (CTAs per SM x SMs), and a CTA's time is about its share of the
-  // points.  S minimises waves / S, the launch time in units of one unsplit CTA (few queries: S ~ slots / tiles; a
-  // tile count just above a whole number of waves: a few slices even out the last wave).  Each slice keeps >= 1024
-  // points, and the smallest S within 2 % of the best is taken, since every slice adds a list to merge.
+  // groups: tiles of up to tq rows of one group each, every tile over its group's points
+  std::vector<ExactTile> tl;
+  if (groups)
+    for (const ExactGroup& gr : *groups)
+      for (size_t q = 0; q < gr.count; q += p.tq)
+        tl.push_back(ExactTile{(uint32_t)(gr.first + q), (uint32_t)std::min<size_t>(p.tq, gr.count - q), gr.scan.ids,
+                               (uint32_t)(gr.scan.ids ? gr.scan.n : n)});
+  const size_t tiles = groups ? tl.size() : (nq + p.tq - 1) / p.tq;
+  if (tiles == 0) return 0;
+  double mean = p.npts, widest = p.npts;  // points a tile scans: on average, and at most
+  if (groups) {
+    mean = widest = 0;
+    for (const ExactTile& t : tl) {
+      mean += t.npts;
+      widest = std::max(widest, (double)t.npts);
+    }
+    mean /= (double)tiles;
+  }
+  // slices: the CTAs of a launch run in waves of `slots` (CTAs per SM x SMs), and a CTA's time is about its share of its
+  // tile's points.  S minimises the launch time in units of one unsplit CTA over the widest tile: the waves the tiles
+  // fill, each as long as a slice of the mean tile, but no less than one slice of the widest tile,
+  //   cost(S) = max(ceil(tiles * S / slots) * mean, widest) / (S * widest).
+  // With equal tiles that is waves / S (few queries: S ~ slots / tiles; a tile count just above a whole number of waves:
+  // a few slices even out the last wave); with a filter per query one wide tile among narrow ones is split while the
+  // narrow ones fill the waves.  Each slice of the widest tile keeps >= 1024 points, and the smallest S within 2 % of the
+  // best is taken, since every slice adds a list to merge.
   int bps = 0;
   HB_CUDA(launch(0, &bps));
   if (bps < 1) return fail("exact search kernel does not fit on an SM");
-  const size_t tiles = (nq + p.tq - 1) / p.tq, slots = (size_t)sm_count_ * bps;
-  const size_t smax = std::max<size_t>(1, std::min<size_t>(p.npts / 1024, 4 * slots));
-  auto cost = [&](size_t S) { return (double)((tiles * S + slots - 1) / slots) / (double)S; };
+  const size_t slots = (size_t)sm_count_ * bps;
+  const size_t smax = std::max<size_t>(1, std::min<size_t>((size_t)widest / 1024, 4 * slots));
+  auto cost = [&](size_t S) {
+    return widest <= 0 ? 1.0 / (double)S
+                       : std::max((double)((tiles * S + slots - 1) / slots) * mean, widest) / ((double)S * widest);
+  };
   double best = cost(1);
   for (size_t S = 2; S <= smax; ++S) best = std::min(best, cost(S));
   p.slices = 1;
   while (cost(p.slices) > best * 1.02) ++p.slices;
-  if (p.slices > 1) {
-    const size_t tick_bytes = round128(tiles * 4);
+  // scratch: [tile table][tickets][slice lists]
+  const size_t tile_bytes = round128(tl.size() * sizeof(ExactTile));
+  const size_t tick_bytes = p.slices > 1 ? round128(tiles * 4) : 0;
+  const size_t part_bytes = p.slices > 1 ? tiles * p.slices * p.tq * k * 8 : 0;
+  if (tile_bytes + tick_bytes + part_bytes) {
     int r;
-    if ((r = ensure_scratch(&c.d_xpart, &c.d_xpart_bytes, tick_bytes + tiles * p.slices * p.tq * k * 8, st))) return r;
-    p.tickets = (unsigned*)c.d_xpart;
-    p.part = (uint64_t*)((char*)c.d_xpart + tick_bytes);
+    if ((r = ensure_scratch(&c.d_xpart, &c.d_xpart_bytes, tile_bytes + tick_bytes + part_bytes, st))) return r;
+  }
+  if (groups) {
+    p.tiles = (const ExactTile*)c.d_xpart;
+    HB_CUDA(cudaMemcpyAsync(c.d_xpart, tl.data(), tl.size() * sizeof(ExactTile), cudaMemcpyHostToDevice, st));
+  }
+  if (p.slices > 1) {
+    p.tickets = (unsigned*)((char*)c.d_xpart + tile_bytes);
+    p.part = (uint64_t*)((char*)c.d_xpart + tile_bytes + tick_bytes);
     HB_CUDA(cudaMemsetAsync(p.tickets, 0, tiles * 4, st));
   }
   p.out = d_out;

@@ -690,6 +690,35 @@ int hnsw_b200_search_exact(const void* h, int64_t filter, const void* queries, u
   b.exact = true;
   return pass(ix, ix->search_batch(b));
 }
+
+// A filter per query: filters[i] is a resident filter of the handle or -1; the graph search (ef_search) or the exact
+// scan (exact).  One batch, every entry checked before anything runs.
+static int per_query_any(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
+                         uint64_t ef_search, bool exact, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                         int32_t* out_pid, int32_t* out_counts) {
+  HB_HS(h);
+  if (nq == 0) return 0;
+  if (!filters) return set_err("filters is NULL");
+  if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0) return set_err("bad argument");
+  HB_PARTS_SHARED_IF(ix);
+  HostBatch b{queries, nullptr, nq, (int)dim, knbn, ef_search, FilterArg(),
+              AnswerArrays{nullptr, out_ids, out_dist, out_internal, out_pid, out_counts}};
+  b.exact = exact;
+  b.per_query = filters;
+  return pass(ix, ix->search_batch(b));
+}
+int hnsw_b200_search_flat_per_query(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim,
+                                    uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
+                                    uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+  return per_query_any(h, filters, queries, nq, dim, knbn, ef_search, false, out_ids, out_dist, out_internal, out_pid,
+                       out_counts);
+}
+int hnsw_b200_search_exact_per_query(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim,
+                                     uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                                     int32_t* out_pid, int32_t* out_counts) {
+  return per_query_any(h, filters, queries, nq, dim, knbn, 0, true, out_ids, out_dist, out_internal, out_pid, out_counts);
+}
+
 int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                   void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
   HB_HS(h);

@@ -10,7 +10,10 @@
 //   * partitioned: the calling thread leases the P contexts in partition order, begins all P legs, collects them and merges;
 //   * submit / wait: the calling thread begins the legs at submit; at wait the root's leg is collected by the caller and
 //     each replica's leg by that replica's worker.
+#include <algorithm>
 #include <cstring>
+#include <numeric>
+#include <set>
 
 #include "index.h"
 #include "partition.h"
@@ -82,10 +85,10 @@ static inline void point_id(const Index* rx, uint32_t it, int32_t* pid2) {
   pid2[1] = it != INVALID_ID ? rx->h_rank[it] : -1;
 }
 
-// queries [first, first + count) of `out` from one leg's answers (k slots each, as the kernels left them: the slots
-// beyond a query's count hold (~0, +inf, INVALID_ID)): plain copies
-static void put_slice(const AnswerArrays& out, const Index* rx, size_t first, size_t count, size_t k, const NeighbourOut* a,
-                      const int32_t* cnts) {
+// rows [first, first + count) of `out` from one leg's answers (k slots each, as the kernels left them: the slots beyond a
+// query's count hold (~0, +inf, INVALID_ID)): plain copies
+static void put_rows(const AnswerArrays& out, const Index* rx, size_t first, size_t count, size_t k, const NeighbourOut* a,
+                     const int32_t* cnts) {
   if (count == 0) return;
   memcpy(out.counts + first, cnts, count * sizeof(int32_t));
   const size_t o = first * k, tot = count * k;
@@ -109,6 +112,13 @@ static void put_slice(const AnswerArrays& out, const Index* rx, size_t first, si
   }
 }
 
+// queries [first, first + count) of the batch from one leg's answers, each to its row of `out` (out.perm)
+static void put_slice(const AnswerArrays& out, const Index* rx, size_t first, size_t count, size_t k, const NeighbourOut* a,
+                      const int32_t* cnts) {
+  if (!out.perm) return put_rows(out, rx, first, count, k, a, cnts);
+  for (size_t i = 0; i < count; ++i) put_rows(out, rx, out.perm[first + i], 1, k, a + i * k, cnts + i);
+}
+
 // slot s of `out` from answer e of index rx, reported with internal id `internal` (a partitioned handle's global rank)
 static inline void put_answer(const AnswerArrays& out, size_t s, const Index* rx, const NeighbourOut& e, uint32_t internal) {
   if (out.nb) {
@@ -121,8 +131,8 @@ static inline void put_answer(const AnswerArrays& out, size_t s, const Index* rx
   if (out.pid) point_id(rx, e.internal, out.pid + 2 * s);
 }
 
-// every query of `out` from the answers of P partition legs, merged by merge_lists; the slots past a query's count are
-// padded with (~0, +inf, INVALID_ID) and PointId (-1, -1)
+// every query of the batch from the answers of P partition legs, merged by merge_lists, to its row of `out` (out.perm);
+// the slots past a query's count are padded with (~0, +inf, INVALID_ID) and PointId (-1, -1)
 static void put_merged(const AnswerArrays& out, const std::vector<Leg>& legs, size_t nq, size_t k,
                        const std::vector<const NeighbourOut*>& a, const std::vector<const int32_t*>& c) {
   const int P = (int)legs.size();
@@ -130,15 +140,15 @@ static void put_merged(const AnswerArrays& out, const std::vector<Leg>& legs, si
   int32_t cnt[Partitions::MAX_PARTS];
   for (size_t q = 0; q < nq; ++q) {
     for (int p = 0; p < P; ++p) cnt[p] = c[p][q];
-    const size_t o = q * k;
+    const size_t o = q * k, row = out.perm ? out.perm[q] : q, w = row * k;
     const size_t total = merge_lists(
         P, k, cnt, [&](int p, int i) { return a[p][o + i].dist; },
         [&](size_t j, int p, int i) {
           const NeighbourOut& e = a[p][o + i];
-          put_answer(out, o + j, legs[p].rx, e, e.internal * (uint32_t)P + (uint32_t)p);
+          put_answer(out, w + j, legs[p].rx, e, e.internal * (uint32_t)P + (uint32_t)p);
         });
-    for (size_t j = total; j < k; ++j) put_answer(out, o + j, nullptr, pad, INVALID_ID);
-    out.counts[q] = (int32_t)total;
+    for (size_t j = total; j < k; ++j) put_answer(out, w + j, nullptr, pad, INVALID_ID);
+    out.counts[row] = (int32_t)total;
   }
 }
 
@@ -192,6 +202,55 @@ int Index::resolve_filter(const FilterArg& f, bool exact, Leg* legs, size_t n, s
   return r;
 }
 
+// Every filter is checked on every partition before anything runs, so that a bad entry refuses the whole call, named by
+// its first position.  The sort is stable: rows of one filter keep their order, and -1 (no filter) sorts first.
+int Index::sort_per_query(const int64_t* fid, size_t nq, std::vector<size_t>& perm) {
+  const int P = parts ? parts->count() : 1;
+  std::set<int64_t> checked;
+  for (size_t i = 0; i < nq; ++i) {
+    if (fid[i] == -1 || checked.count(fid[i])) continue;
+    for (int p = 0; p < P; ++p) {
+      Index* rx = parts ? parts->part(p) : this;
+      const uint32_t* bits = nullptr;
+      if (filters.use(fid[i], p, P, rx, &bits))
+        return fail("filters[" + std::to_string(i) + "] = " + std::to_string(fid[i]) + ": " + rx->err());
+    }
+    checked.insert(fid[i]);
+  }
+  perm.resize(nq);
+  std::iota(perm.begin(), perm.end(), (size_t)0);
+  std::stable_sort(perm.begin(), perm.end(), [&](size_t a, size_t b) { return fid[a] < fid[b]; });
+  return 0;
+}
+
+int Index::resolve_per_query(const std::vector<int64_t>& sorted, bool exact, Leg* legs, size_t n) {
+  const int P = parts ? parts->count() : 1;
+  int r = 0;
+  for (Leg* l = legs; l < legs + n; ++l) {  // every leg, so that the caller reports the failure it chooses
+    LegFilters& q = l->pq;
+    const int64_t* f = sorted.data() + l->first;
+    q.on = true;
+    while (q.plain < l->count && f[q.plain] == -1) ++q.plain;
+    if (exact && q.plain) q.groups.push_back(ExactGroup{0, q.plain, ExactScan()});
+    for (size_t j = q.plain, e; j < l->count; j = e) {  // one run of rows per filter
+      for (e = j + 1; e < l->count && f[e] == f[j];) ++e;
+      ExactScan s;
+      const uint32_t* bits = nullptr;
+      if (filters.use(f[j], l->part, P, l->rx, &bits, exact ? &s : nullptr)) {
+        r = l->rc = -1;
+        break;
+      }
+      if (exact) {
+        q.groups.push_back(ExactGroup{j, e - j, s});
+      } else {
+        q.sel.insert(q.sel.end(), e - j, (uint32_t)q.table.size());
+        q.table.push_back(bits);
+      }
+    }
+  }
+  return r;
+}
+
 // The handle's error for the first failed leg of legs[0, n) (0 if none failed): in leg order, or the replicas' before the
 // root's (replicas_first, the synchronous sharded search's order).  A partition's and a replica's message name it.
 int Index::legs_fail(const Leg* legs, size_t n, bool replicas_first) {
@@ -209,7 +268,7 @@ void Index::begin_leg(const HostBatch& b, Leg& l) {
   if (l.ctx < 0) l.ctx = l.rx->acquire_ctx();
   const void* q = b.rows ? nullptr : (const char*)b.queries + l.first * (size_t)b.d * es;
   l.rc = l.rx->search_host_begin(l.ctx, q, b.rows ? b.rows + l.first : nullptr, l.count, b.d, b.k, b.ef, l.host_bits,
-                                 l.dev_bits, b.exact ? &l.scan : nullptr);
+                                 l.dev_bits, b.exact ? &l.scan : nullptr, l.pq.on ? &l.pq : nullptr);
   l.begun = l.rc == 0;
 }
 
@@ -236,16 +295,34 @@ int Index::end_leg(Leg& l, size_t k, const AnswerArrays& out) {
 }
 
 // ------------------------------------------------------------------------------------------------ batches
-int Index::search_batch(const HostBatch& b) {
-  if (b.nq == 0) return 0;
-  if (parts && dim != 0 && b.d != dim) return fail("query length differs from the index dimension");
+int Index::search_batch(const HostBatch& call) {
+  if (call.nq == 0) return 0;
+  if (parts && dim != 0 && call.d != dim) return fail("query length differs from the index dimension");
+  int r;
+  // a filter per query: the batch is planned over the rows sorted by filter, gathered through row pointers, and each
+  // answer goes back to its caller's row
+  HostBatch b = call;
+  std::vector<size_t> perm;
+  std::vector<const void*> rows;
+  std::vector<int64_t> sorted;
+  if (call.per_query) {
+    if ((r = sort_per_query(call.per_query, call.nq, perm))) return r;
+    rows.resize(call.nq);
+    sorted.resize(call.nq);
+    for (size_t j = 0; j < call.nq; ++j) {
+      rows[j] = call.rows ? call.rows[perm[j]] : (const char*)call.queries + perm[j] * (size_t)call.d * es;
+      sorted[j] = call.per_query[perm[j]];
+    }
+    b.rows = rows.data();
+    b.out.perm = perm.data();
+  }
   std::vector<Leg> legs;
   std::vector<std::vector<uint32_t>> bits;
-  int r;
   if ((r = plan(b.nq, legs))) return r;
   const int n = (int)legs.size();
   const bool sharded = n > 1 && !parts;
-  if (resolve_filter(b.filter, b.exact, legs.data(), n, bits)) return legs_fail(legs.data(), n, sharded);
+  if (b.per_query ? resolve_per_query(sorted, b.exact, legs.data(), n) : resolve_filter(b.filter, b.exact, legs.data(), n, bits))
+    return legs_fail(legs.data(), n, sharded);
   if (n == 1 && !parts) {
     begin_leg(b, legs[0]);
     return end_leg(legs[0], b.k, b.out);

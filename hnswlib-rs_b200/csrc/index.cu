@@ -666,7 +666,8 @@ int Index::stream_wait_last(cudaStream_t s) {
 }
 
 int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const uint32_t* d_filter_bits,
-                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms) {
+                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint32_t* const* d_ftab,
+                         const uint32_t* d_fsel) {
   if (k == 0) return fail("knbn must be positive");
   if (poisoned_) return fail(poison_msg_);
   cudaStream_t st = c.stream;
@@ -691,9 +692,11 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.out_nb = d_out;
   p.out_count = d_counts;
   p.filter_bits = d_filter_bits;
+  p.filter_table = d_ftab;
+  p.filter_sel = d_fsel;
   p.stats = stats_on_ ? d_stats_ : nullptr;
   p.status = c.d_status;
-  const bool filtered = d_filter_bits != nullptr;
+  const bool filtered = d_filter_bits != nullptr || d_fsel != nullptr;
   QueryKernel kind = QueryKernel::Generic;
   if (filtered) kind = QueryKernel::Filtered;
   else if (tie_std_) kind = QueryKernel::StdTie;  // unfiltered searches only
@@ -785,7 +788,8 @@ static const void* device_view_of_host(const void* p) {
 // synchronisation.  Pageable queries and row pointers are gathered into the context's own pinned staging buffer first
 // (the only host-side copy), which the kernel then reads the same way.
 int Index::search_host_begin(int ci, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                             const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const ExactScan* scan) {
+                             const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const ExactScan* scan,
+                             const LegFilters* pq) {
   SearchCtx& c = ctx_[ci];
   cudaStream_t st = c.stream;
   c.pend = SearchCtx::Pending();
@@ -833,7 +837,27 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
     *hstatus = 0;
     c.pend.exact = true;
     c.pend.enqueued = true;
-    return exact_on_ctx(c, c.d_xq, nq, k, *scan, k_out, k_cnt, false, nullptr);
+    return exact_on_ctx(c, c.d_xq, nq, k, *scan, k_out, k_cnt, false, nullptr, pq && pq->on ? &pq->groups : nullptr);
+  }
+  if (pq && pq->on) {
+    // a filter per query: the bitmap table and the filtered rows' entries go to the device ahead of the launches
+    const size_t tb = round128(pq->table.size() * sizeof(void*)), sb = pq->sel.size() * sizeof(uint32_t);
+    if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, tb + sb, st))) return r;
+    if (sb) {
+      HB_CUDA(cudaMemcpyAsync(c.d_fbits, pq->table.data(), pq->table.size() * sizeof(void*), cudaMemcpyHostToDevice, st));
+      HB_CUDA(cudaMemcpyAsync((char*)c.d_fbits + tb, pq->sel.data(), sb, cudaMemcpyHostToDevice, st));
+    }
+    c.pend.per_query = true;
+    c.pend.plain = pq->plain;
+    c.pend.ftab = (const uint32_t* const*)c.d_fbits;
+    c.pend.fsel = (const uint32_t*)((char*)c.d_fbits + tb);
+    c.pend.d_queries = d_queries;
+    c.pend.k_out = k_out;
+    c.pend.k_cnt = k_cnt;
+    c.pend.enqueued = true;
+    if ((r = per_query_on_ctx(c, false))) return r;
+    HB_CUDA(cudaMemcpyAsync(hstatus, c.d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    return 0;
   }
   const uint32_t* dfb = d_filter_bits;  // a resident filter: already on this device
   if (filter_bits_host) {
@@ -865,7 +889,20 @@ int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** 
   HB_CUDA(cudaStreamSynchronize(st));
   if (p.exact || *p.hstatus == 0) return 0;
   HB_CUDA(cudaMemsetAsync(c.d_status, 0, sizeof(int), st));
+  if (p.per_query) return per_query_on_ctx(c, true);
   return search_on_ctx(c, p.d_queries, p.nq, p.k, p.ef, p.dfb, p.k_out, p.k_cnt, true, nullptr);  // grows the tables
+}
+
+// the rows without a filter as an ordinary unfiltered launch, then every filtered row in one filtered launch on the
+// bitmap table; both share the context's status, so an overflow in either re-runs both (sync: growing the tables)
+int Index::per_query_on_ctx(SearchCtx& c, bool sync) {
+  const SearchCtx::Pending& p = c.pend;
+  int r;
+  if (p.plain && (r = search_on_ctx(c, p.d_queries, p.plain, p.k, p.ef, nullptr, p.k_out, p.k_cnt, sync, nullptr))) return r;
+  if (p.nq == p.plain) return 0;
+  const char* fq = (const char*)p.d_queries + p.plain * (size_t)dim * es;
+  return search_on_ctx(c, fq, p.nq - p.plain, p.k, p.ef, nullptr, p.k_out + p.plain * p.k, p.k_cnt + p.plain, sync, nullptr,
+                       p.ftab, p.fsel);
 }
 
 int Index::make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx,

@@ -111,6 +111,12 @@ struct ExactScan {
   size_t n = 0;
 };
 
+// rows [first, first + count) of an exact launch with a filter per query, all scanning the same points
+struct ExactGroup {
+  size_t first, count;
+  ExactScan scan;
+};
+
 // Resident filters (hnsw_b200_filter_new, filter_store.cu): a FilterT materialised once per handle, as one bitmap per
 // partition (one for an ordinary handle) over the points stored when it was made.  The host copy stays; each device a
 // search uses it on gets one device copy, made at its first use there.  Ids are unique over all handles, so an id that
@@ -185,6 +191,7 @@ struct AnswerArrays {
   uint32_t* internal = nullptr;
   int32_t* pid = nullptr;
   int32_t* counts = nullptr;
+  const size_t* perm = nullptr;  // row j of the batch is written to row perm[j] (nullptr: to row j)
 };
 
 // The filter of a search: none, a FilterT (mode != 0, as make_filter_bits reads it: 1 sorted origin-id list, 2 callback),
@@ -209,6 +216,18 @@ struct HostBatch {
   FilterArg filter;
   AnswerArrays out;
   bool exact = false;
+  const int64_t* per_query = nullptr;  // [nq]: each query's resident filter, or -1 for none (then `filter` is unused)
+};
+
+// A leg's share of a batch with a filter per query, whose rows the driver sorted by filter (resolve_per_query): the
+// leg's first `plain` rows have no filter.  Graph search: its row plain + i uses bitmap table[sel[i]].  Exact scan:
+// `groups`, its rows by the points they scan (every point for the plain rows).
+struct LegFilters {
+  bool on = false;
+  size_t plain = 0;
+  std::vector<const uint32_t*> table;
+  std::vector<uint32_t> sel;
+  std::vector<ExactGroup> groups;
 };
 
 // One Index's part of a batch: queries [first, first + count) searched on rx (the handle, a replica, or partition `part`)
@@ -223,6 +242,7 @@ struct Leg {
   ExactScan scan;
   bool begun = false;  // enqueued
   int rc = 0;
+  LegFilters pq;
 };
 
 class Index {
@@ -264,9 +284,11 @@ class Index {
   // host queries (flat or row pointers) on leased context c, answers left in the context's pinned buffer (valid until
   // it is released).  The filter is either host bits, uploaded into the context for this call, or d_filter_bits already
   // on this device (a resident filter); at most one of the two is non-null.  With `scan`, the exact scan of those points
-  // instead of the graph search (no filter bits, ef unused).
+  // instead of the graph search (no filter bits, ef unused).  With `pq` (pq->on; no filter bits and no scan), a filter
+  // per query.
   int search_host_begin(int c, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                        const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const ExactScan* scan = nullptr);
+                        const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const ExactScan* scan = nullptr,
+                        const LegFilters* pq = nullptr);
   int search_host_finish(int c, const NeighbourOut** out, const int32_t** counts);
   // host search batches (host_search.cu): synchronous, or submitted now and collected by finish_batch
   struct Ticket {
@@ -287,6 +309,12 @@ class Index {
   // Nonzero when a leg could not have them; that leg's rc is set (legs_fail reports it).  `exact`: each leg's ExactScan
   // instead (the resident filter's id list on the leg's device, or every point).
   int resolve_filter(const FilterArg& f, bool exact, Leg* legs, size_t n, std::vector<std::vector<uint32_t>>& bits);
+  // a batch with a filter per query: every entry of filters[0, nq) is -1 or a live, current filter of this handle (else
+  // the first bad position is refused), and `perm` orders the rows stably by filter, the unfiltered ones first
+  int sort_per_query(const int64_t* filters, size_t nq, std::vector<size_t>& perm);
+  // each leg's LegFilters for the rows sorted by filter (sorted[j]: the filter of sorted row j), on its partition and
+  // device; nonzero when a leg could not have them, with that leg's rc set
+  int resolve_per_query(const std::vector<int64_t>& sorted, bool exact, Leg* legs, size_t n);
   // device queries in, device answers out; the filter is none or a resident filter.  `exact`: the exact scan (ef unused).
   int search_device(const FilterArg& f, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef, NeighbourOut* d_out,
                     int32_t* d_counts, bool sync, float* kernel_ms);
@@ -349,7 +377,7 @@ class Index {
     unsigned int* d_counter = nullptr;
     int* d_status = nullptr;
     VisitedPool vis, fvis;  // unfiltered / filtered searches
-    void *d_fbits = nullptr, *d_cbuf = nullptr;
+    void *d_fbits = nullptr, *d_cbuf = nullptr;  // the call's filter bits (or its per-query bitmap table and selectors) / C
     size_t d_fbits_bytes = 0, d_cbuf_bytes = 0;
     void *d_xq = nullptr, *d_xpart = nullptr;  // exact scan: the host batch's queries on the device / tickets and slice lists
     size_t d_xq_bytes = 0, d_xpart_bytes = 0;
@@ -360,6 +388,11 @@ class Index {
       const void* d_queries = nullptr;
       const uint32_t* dfb = nullptr;
       bool exact = false;  // an exact scan: no status, nothing to re-run
+      // a filter per query: rows [0, plain) unfiltered, the others on the device bitmap table / selectors
+      bool per_query = false;
+      size_t plain = 0;
+      const uint32_t* const* ftab = nullptr;
+      const uint32_t* fsel = nullptr;
       NeighbourOut *k_out = nullptr, *hout = nullptr;
       int32_t *k_cnt = nullptr, *hcnt = nullptr, *hstatus = nullptr;
       size_t nq = 0, k = 0, ef = 0;
@@ -468,11 +501,16 @@ class Index {
 
   VisitedPool vis_;  // visited tables of the insert kernel (searches: SearchCtx)
   SearchCtx ctx_[NCTX + NASYNC];
+  // d_ftab / d_fsel: a filter per query, query i on bitmap d_ftab[d_fsel[i]] (then d_filter_bits is null)
   int search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const uint32_t* d_filter_bits,
-                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms);
-  // the exact k nearest of device queries among scan's points (aux.cu); the slices' scratch is sized before the launch
+                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms,
+                    const uint32_t* const* d_ftab = nullptr, const uint32_t* d_fsel = nullptr);
+  // the exact k nearest of device queries among scan's points (aux.cu); the slices' scratch is sized before the launch.
+  // With `groups` (a filter per query), each group's rows among that group's points instead of scan's.
   int exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const ExactScan& scan, NeighbourOut* d_out,
-                   int32_t* d_counts, bool sync, float* kernel_ms);
+                   int32_t* d_counts, bool sync, float* kernel_ms, const std::vector<ExactGroup>* groups = nullptr);
+  // the graph search of a per-query leg on context c: the plain rows' launch, then the filtered rows' launch
+  int per_query_on_ctx(SearchCtx& c, bool sync);
   std::mutex ctx_mu_;
   std::condition_variable ctx_cv_;
   std::mutex ticket_mu_;

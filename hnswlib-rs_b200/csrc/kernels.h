@@ -50,6 +50,10 @@ struct SearchParams {
   int q_kind;  // QueueSel kind
   uint64_t* cbuf;  // filtered search only: candidate queue C, [slots][ccap] keys
   uint32_t ccap;
+  // filtered search with a filter per query (filter_sel != nullptr): query i uses the bitmap filter_table[filter_sel[i]]
+  // instead of filter_bits.  Appended, so that every field above keeps its offset.
+  const uint32_t* const* filter_table;
+  const uint32_t* filter_sel;  // [nq]
 };
 
 // rows of up to 512 bytes are (partly) staged by TMA: STAGE_ROWS rows + an mbarrier per warp
@@ -138,6 +142,14 @@ __host__ __device__ inline ExactLayout exact_layout(int d4, int k, int tq, int r
   l.bytes = round128(l.bar + (size_t)stages * 8);
   return l;
 }
+
+// one tile of an exact launch whose tiles differ (a filter per query): queries [q0, q0 + nq) of the launch, scanned over
+// `list` (npts sorted internal ids) or, with list == nullptr, over the points 0 .. npts - 1
+struct ExactTile {
+  uint32_t q0, nq;
+  const uint32_t* list;
+  uint32_t npts;
+};
 
 // Queue kind for a given ef (see QueueSel): compile-time chunked shared-memory queue up to ef = 256, generic beyond.
 // (A register-resident variant spilled at 64 registers/thread, and a speculative two-candidates-per-iteration loop was

@@ -101,6 +101,8 @@ def load_library():
     L.hnsw_b200_search_device_filtered.argtypes = [vp, i64, vp, u64, u64, u64, vp, vp, i32, vp]
     L.hnsw_b200_search_exact.argtypes = [vp, i64, vp, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_exact_device.argtypes = [vp, i64, vp, u64, u64, vp, vp, i32, vp]
+    L.hnsw_b200_search_flat_per_query.argtypes = [vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_exact_per_query.argtypes = [vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_get_stats.argtypes = [vp, vp, i32]
     L.hnsw_b200_set_stream.argtypes = [vp, vp]
     L.hnsw_b200_join.argtypes = [vp]
@@ -218,6 +220,14 @@ def _filter_id(filter):
     if not isinstance(filter, ResidentFilter):
         raise TypeError("the exact searches take a ResidentFilter (Hnsw.make_filter) or None as their filter")
     return filter.id
+
+
+def _filter_ids(filters, nq):
+    """the filters argument of the per-query searches: one ResidentFilter or None per query, as an int64 id array (-1:
+    no filter)"""
+    if len(filters) != nq:
+        raise ValueError(f"filters has {len(filters)} entries for {nq} queries")
+    return np.ascontiguousarray([_filter_id(f) for f in filters], np.int64).reshape(nq)
 
 
 class Hnsw:
@@ -410,6 +420,31 @@ class Hnsw:
         self._chk(self._L.hnsw_b200_search_exact(self._h, _filter_id(filter), _p(q), nq, d, int(knbn), _p(o), _p(ds), _p(it),
                                                  _p(pid), _p(cnt)))
         return o, ds, it, pid, cnt
+
+    def _per_query(self, fn, queries, knbn, filters, ef_args, with_internal, with_pid):
+        q = np.ascontiguousarray(queries, self.dtype)
+        nq, d = q.shape
+        fids = _filter_ids(filters, nq)
+        o = np.empty((nq, knbn), np.uint64)
+        ds = np.empty((nq, knbn), np.float32)
+        it = np.empty((nq, knbn), np.uint32) if with_internal else None
+        pid = np.empty((nq, knbn, 2), np.int32) if with_pid else None
+        cnt = np.empty(nq, np.int32)
+        self._chk(fn(self._h, _p(fids), _p(q), nq, d, int(knbn), *ef_args, _p(o), _p(ds), _p(it), _p(pid), _p(cnt)))
+        return o, ds, it, pid, cnt
+
+    def search_flat_per_query(self, queries, knbn, ef, filters, with_internal=True, with_pid=True):
+        """hnsw_b200_search_flat_per_query: one batch, query i filtered by filters[i] (a ResidentFilter of this handle,
+        or None for no filter).  Row i equals search_flat(queries[i:i+1], knbn, ef, filter=filters[i]).  Returns
+        search_flat's (origin, dist, internal | None, pid | None, counts)."""
+        return self._per_query(self._L.hnsw_b200_search_flat_per_query, queries, knbn, filters, (int(ef),), with_internal,
+                               with_pid)
+
+    def search_exact_per_query(self, queries, knbn, filters, with_internal=True, with_pid=True):
+        """hnsw_b200_search_exact_per_query: search_exact with query i over the points filters[i] admits (a
+        ResidentFilter of this handle, or None for every point), in one batch.  Returns search_exact's tuple."""
+        return self._per_query(self._L.hnsw_b200_search_exact_per_query, queries, knbn, filters, (), with_internal,
+                               with_pid)
 
     def make_filter(self, filter):
         """hnsw_b200_filter_new: materialise a FilterT (sorted id sequence or callable(id)->bool, as search_flat takes)

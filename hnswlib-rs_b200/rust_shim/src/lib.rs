@@ -76,6 +76,13 @@ extern "C" {
                               out_counts: *mut i32) -> c_int;
     fn hnsw_b200_search_exact_device(h: *const HnswApif32, filter: i64, d_queries: *const c_void, nq: u64, knbn: u64,
                                      d_out: *mut c_void, d_counts: *mut i32, sync: c_int, kernel_ms: *mut f32) -> c_int;
+    // a filter per query (include/hnsw_b200.h "A filter per query"): filters[i] = a resident filter's id, or -1
+    fn hnsw_b200_search_flat_per_query(h: *const HnswApif32, filters: *const i64, queries: *const f32, nq: u64, dim: u64,
+                                       knbn: u64, ef: u64, out_ids: *mut u64, out_dist: *mut f32, out_internal: *mut u32,
+                                       out_pid: *mut i32, out_counts: *mut i32) -> c_int;
+    fn hnsw_b200_search_exact_per_query(h: *const HnswApif32, filters: *const i64, queries: *const f32, nq: u64, dim: u64,
+                                        knbn: u64, out_ids: *mut u64, out_dist: *mut f32, out_internal: *mut u32,
+                                        out_pid: *mut i32, out_counts: *mut i32) -> c_int;
 }
 
 /// hnsw.rs:46
@@ -226,6 +233,35 @@ impl<D: DistName> Hnsw<D> {
         };
         assert_eq!(r, 0, "hnsw_b200_search_exact failed");
         (0..cnt as usize).map(|j| Neighbour { d_id: ids[j] as usize, distance: ds[j], p_id: PointId(pid[2 * j] as u8, pid[2 * j + 1]) }).collect()
+    }
+    /// Extension: one batch, request i filtered by `filters[i]` (None: no filter); answer i is what search_resident
+    /// (or search, for None) returns for request i.  Graph search with `Some(ef)`, the exact scan with None.
+    pub fn search_per_query(&self, datas: &[Vec<f32>], knbn: usize, ef: Option<usize>,
+                            filters: &[Option<&ResidentFilter<'_, D>>]) -> Vec<Vec<Neighbour>> {
+        assert_eq!(datas.len(), filters.len(), "one filter per request");
+        if datas.is_empty() { return Vec::new(); }
+        let (nq, dim) = (datas.len(), datas[0].len());
+        let flat: Vec<f32> = datas.iter().flat_map(|d| d.iter().copied()).collect();
+        let fids: Vec<i64> = filters.iter().map(|f| f.map_or(-1, |f| f.id)).collect();
+        let mut ids = vec![0u64; nq * knbn];
+        let mut ds = vec![0f32; nq * knbn];
+        let mut pid = vec![0i32; 2 * nq * knbn];
+        let mut cnt = vec![0i32; nq];
+        let r = unsafe {
+            match ef {
+                Some(ef) => hnsw_b200_search_flat_per_query(self.h, fids.as_ptr(), flat.as_ptr(), nq as u64, dim as u64, knbn as u64,
+                                                            ef as u64, ids.as_mut_ptr(), ds.as_mut_ptr(), std::ptr::null_mut(),
+                                                            pid.as_mut_ptr(), cnt.as_mut_ptr()),
+                None => hnsw_b200_search_exact_per_query(self.h, fids.as_ptr(), flat.as_ptr(), nq as u64, dim as u64, knbn as u64,
+                                                         ids.as_mut_ptr(), ds.as_mut_ptr(), std::ptr::null_mut(), pid.as_mut_ptr(),
+                                                         cnt.as_mut_ptr()),
+            }
+        };
+        assert_eq!(r, 0, "hnsw_b200_search_flat_per_query / _exact_per_query failed");
+        (0..nq).map(|i| (0..cnt[i] as usize).map(|j| {
+            let s = i * knbn + j;
+            Neighbour { d_id: ids[s] as usize, distance: ds[s], p_id: PointId(pid[2 * s] as u8, pid[2 * s + 1]) }
+        }).collect()).collect()
     }
     /// hnsw.rs:1612-1635: one answer per request, in input order
     pub fn parallel_search(&self, datas: &[Vec<f32>], knbn: usize, ef: usize) -> Vec<Vec<Neighbour>> {

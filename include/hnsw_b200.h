@@ -341,6 +341,30 @@ int hnsw_b200_search_exact(const void* h, int64_t filter, const void* queries, u
 int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                   void* d_out, int32_t* d_counts, int sync, float* kernel_ms);
 
+/* ---- A filter per query: one batch whose query i uses resident filter filters[i] of h, or no filter (-1).  A batch
+ * that mixes tenants, users or categories runs as one call (one launch per leg for the filtered rows) instead of one
+ * call per distinct filter.
+ *   Answers: row i is, bit for bit, what the single-filter call returns for query i (ids, distance bits, internal ids,
+ *     PointIds, count).  For search_flat_per_query that is hnsw_b200_search_flat_filtered(filters[i], ...), or the
+ *     unfiltered hnsw_b200_search_flat when filters[i] == -1; for search_exact_per_query, hnsw_b200_search_exact(
+ *     filters[i], ...).  So rows with a filter ignore the tie mode, as every filtered search does, and rows with -1
+ *     follow it.  With statistics on, one call adds what the single-filter calls over the same queries add together.
+ *   Checks, before anything runs: every entry must be -1 or a live filter of h that is not stale; the first bad entry
+ *     refuses the whole call, and the message names its position and id.  filters == NULL with nq > 0 is refused;
+ *     nq == 0 returns 0.  An empty index gives every count 0.
+ *   Partitioned handles: each row is merged over the partitions by the rule of partitioned search (distance, then
+ *     partition, then position); internal ids are global ranks.  A replicated handle shards the batch like search_flat;
+ *     each replica's device gets a filter's copies at their first use there.  A partition view owns no filters, so it
+ *     accepts only -1 entries.
+ *   Locks: the handle is taken shared; hnsw_b200_filter_free waits for the call.
+ * Every other argument and output is that of hnsw_b200_search_flat_filtered / hnsw_b200_search_exact. */
+int hnsw_b200_search_flat_per_query(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim,
+                                    uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
+                                    uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
+int hnsw_b200_search_exact_per_query(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim,
+                                     uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                                     int32_t* out_pid, int32_t* out_counts);
+
 /* Run this handle's kernels and copies on a caller-owned CUDA stream (cudaStream_t passed as void*; NULL
  * restores the handle's own stream), e.g. so that torch.cuda.Event on torch's current stream brackets them. */
 int hnsw_b200_join(void* h);
