@@ -719,6 +719,88 @@ int hnsw_b200_search_exact_per_query(const void* h, const int64_t* filters, cons
   return per_query_any(h, filters, queries, nq, dim, knbn, 0, true, out_ids, out_dist, out_internal, out_pid, out_counts);
 }
 
+// Point labels.  On a partitioned handle point g (its insertion rank) is local point g / P of partition g % P.
+static int label_range(const Index* ix, uint64_t first, uint64_t n) {
+  const uint64_t have = nb_point(ix);
+  if (first > have || n > have - first)
+    return set_err("labels [" + std::to_string(first) + ", " + std::to_string(first + n) + ") are out of range: the " +
+                   (ix->owner ? "partition" : "index") + " holds " + std::to_string(have) + " points");
+  return 0;
+}
+// calls f(index, partition, local first, count, stride, at) for each Index that holds some of the points [first, first + n):
+// its points lo .. lo + count - 1 are entries at, at + stride, ... of the caller's array
+static int for_label_range(Index* ix, uint64_t first, uint64_t n,
+                           const std::function<int(Index*, int, uint64_t, uint64_t, uint64_t, uint64_t)>& f) {
+  if (!ix->parts) return f(ix, 0, first, n, 1, 0);
+  const uint64_t P = (uint64_t)ix->parts->count();
+  for (uint64_t p = 0; p < P; ++p) {
+    const uint64_t g0 = first + (p + P - first % P) % P;  // the first rank of partition p in the range
+    if (g0 >= first + n) continue;
+    int r = f(ix->parts->part((int)p), (int)p, g0 / P, (first + n - g0 + P - 1) / P, P, g0 - first);
+    if (r) return r;
+  }
+  return 0;
+}
+int hnsw_b200_set_labels(void* h, uint64_t first, uint64_t n, const uint32_t* labels) {
+  HB_H(h);
+  HB_NOT_VIEW(ix);
+  if (label_range(ix, first, n)) return -1;
+  if (n == 0) return 0;
+  if (!labels) return set_err("labels is NULL");
+  hb::DeviceRestore keep;
+  const auto pl__ = ix->parts ? ix->parts->lock_exclusive() : std::vector<std::unique_lock<std::shared_mutex>>();
+  std::vector<uint32_t> mine;
+  return for_label_range(ix, first, n, [&](Index* x, int part, uint64_t lo, uint64_t cnt, uint64_t stride, uint64_t at) {
+    const uint32_t* src = labels + at;
+    if (stride != 1) {
+      mine.resize(cnt);
+      for (uint64_t i = 0; i < cnt; ++i) mine[i] = labels[at + i * stride];
+      src = mine.data();
+    }
+    const int r = x->set_labels(lo, cnt, src);
+    return pass(ix, r && ix->parts ? ix->parts->fail(part, x->err()) : r);
+  });
+}
+int hnsw_b200_get_labels(const void* h, uint64_t first, uint64_t n, uint32_t* out) {
+  HB_HS(h);
+  if (label_range(ix, first, n)) return -1;
+  if (n == 0) return 0;
+  if (!out) return set_err("out is NULL");
+  HB_PARTS_SHARED_IF(ix);
+  return for_label_range(ix, first, n, [&](Index* x, int, uint64_t lo, uint64_t cnt, uint64_t stride, uint64_t at) {
+    for (uint64_t i = 0; i < cnt; ++i) out[at + i * stride] = x->h_label[lo + i];
+    return 0;
+  });
+}
+
+// A label per query: labels[i] is the label query i is restricted to, or LABEL_NONE for none; the graph search
+// (ef_search) or the exact scan (exact).
+static int labeled_any(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
+                       uint64_t ef_search, bool exact, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                       int32_t* out_pid, int32_t* out_counts) {
+  HB_HS(h);
+  if (nq == 0) return 0;
+  if (!qlabels) return set_err("qlabels is NULL");
+  if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0) return set_err("bad argument");
+  HB_PARTS_SHARED_IF(ix);
+  HostBatch b{queries, nullptr, nq, (int)dim, knbn, ef_search, FilterArg(),
+              AnswerArrays{nullptr, out_ids, out_dist, out_internal, out_pid, out_counts}};
+  b.exact = exact;
+  b.labels = qlabels;
+  return pass(ix, ix->search_batch(b));
+}
+int hnsw_b200_search_flat_labeled(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim,
+                                  uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
+                                  uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+  return labeled_any(h, qlabels, queries, nq, dim, knbn, ef_search, false, out_ids, out_dist, out_internal, out_pid,
+                     out_counts);
+}
+int hnsw_b200_search_exact_labeled(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim,
+                                   uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                                   int32_t* out_pid, int32_t* out_counts) {
+  return labeled_any(h, qlabels, queries, nq, dim, knbn, 0, true, out_ids, out_dist, out_internal, out_pid, out_counts);
+}
+
 int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                   void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
   HB_HS(h);

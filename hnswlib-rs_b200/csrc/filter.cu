@@ -9,18 +9,29 @@
 //     and keeps expanding, until C is empty.
 // So here C is a real queue: an unsorted array of keys per warp in global memory, pop = warp-wide min scan
 // (consumed entries are overwritten with ~0).  W is the same sorted shared-memory array as elsewhere.
-// The FilterT predicate (filter.rs:7-24) is a device bitmap over internal ids, materialised by the host.
+// The FilterT predicate (filter.rs:7-24) is a device bitmap over internal ids, materialised by the host, or a point
+// label: the predicate label(p) == L over the label array of the graph store.
 #include "kernels.h"
 #include "search_core.cuh"
 
 namespace hb {
 
-__device__ __forceinline__ bool filter_pass(const uint32_t* bits, uint32_t id) {
-  return (__ldg(bits + (id >> 5)) >> (id & 31)) & 1u;
+// A query's filter, kept in its warp's mbarrier slot (unused by this kernel) and read at each use, so that the search
+// loop holds no extra register: a bitmap (label == LABEL_NONE), or the label array and the label the query admits.
+struct FilterSlot {
+  const uint32_t* ptr;
+  uint32_t label;
+};
+
+// the one admission test: the point's label, or its bit of the bitmap
+__device__ __forceinline__ bool filter_pass(const FilterSlot* f, uint32_t id) {
+  const uint32_t want = f->label;
+  if (want != LABEL_NONE) return __ldg(f->ptr + id) == want;
+  return (__ldg(f->ptr + (id >> 5)) >> (id & 31)) & 1u;
 }
 
 // keeps the keys w[0, n) whose points pass the filter, in order, at the front of w; returns how many there are
-__device__ __forceinline__ int keep_passing(uint64_t* w, int n, const uint32_t* fbits) {
+__device__ __forceinline__ int keep_passing(uint64_t* w, int n, const FilterSlot* fslot) {
   const int lane = lane_id();
   int out = 0;
   for (int b = 0; b < n; b += 32) {
@@ -29,7 +40,7 @@ __device__ __forceinline__ int keep_passing(uint64_t* w, int n, const uint32_t* 
     bool keep = false;
     if (i < n) {
       v = w[i];
-      keep = filter_pass(fbits, key_id(v));
+      keep = filter_pass(fslot, key_id(v));
     }
     const unsigned m = __ballot_sync(FULL, keep);
     __syncwarp();
@@ -43,7 +54,7 @@ __device__ __forceinline__ int keep_passing(uint64_t* w, int n, const uint32_t* 
 template <class Op, int CH, int U>
 __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const WarpSmem& s, const VisitedCfg& vc, Visited& vis,
                                                       SortedQueue& W, uint64_t* cbuf, uint32_t ccap,
-                                                      const uint32_t* const* fslot, uint32_t ep, int ef, int layer, Stats& st, bool& overflow) {
+                                                      const FilterSlot* fslot, uint32_t ep, int ef, int layer, Stats& st, bool& overflow) {
   const int lane = lane_id();
   const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
   vis.begin(vc, ep, lane);  // hnsw.rs:955-956
@@ -90,7 +101,7 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
     const uint64_t fkey = W.w[W.n - 1] & ~1ull;
     // 981: the reference compares DISTANCES here (-(c.dist) > f.dist); with equal distances a larger id must not
     // trigger the retain pass (Hamming / Jaccard / integer L1 tie often)
-    if ((best >> 32) > (fkey >> 32) && W.n >= ef) W.n = keep_passing(W.w, W.n, *fslot);  // 994-1000
+    if ((best >> 32) > (fkey >> 32) && W.n >= ef) W.n = keep_passing(W.w, W.n, fslot);  // 994-1000
     const uint32_t c = key_id(best);
     int cap;
     const uint32_t* ids = list_ids(g, c, layer, cap);  // 1006
@@ -112,7 +123,7 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
         st.evals += cnt;
         const uint32_t my_id = lane < cnt ? s.cand_id[lane] : 0u;
         const uint64_t key = lane < cnt ? make_key(Op::post(s.cand_d[lane]), my_id) : ~0ull;
-        const bool my_pass = lane < cnt && filter_pass(*fslot, my_id);
+        const bool my_pass = lane < cnt && filter_pass(fslot, my_id);
         const unsigned passmask = __ballot_sync(FULL, my_pass);
         for (int j = 0; j < cnt; ++j) {  // strictly in list order: the accept rule sees the W of that moment
           if (W.n == 0) {                // 1019-1024
@@ -129,7 +140,7 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
             if (lane == 0) __stcg(cbuf + cn, kj);  // 1035-1036: every accepted candidate goes to C
             cn += 1;
             if ((passmask >> j) & 1u) {  // 1040-1049
-              if (W.n == 1 && !filter_pass(*fslot, key_id(W.w[0]))) W.n = 0;
+              if (W.n == 1 && !filter_pass(fslot, key_id(W.w[0]))) W.n = 0;
               __syncwarp();
               W.insert(kj);  // push, and pop the farthest when over ef (1051-1053)
             }
@@ -156,7 +167,7 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
   const QueryLayout L = query_layout(g.d4, p.q_smem);  // search.cu's layout; the stage is unused here
   const WarpSmem s{reinterpret_cast<uint4*>(base + L.query), reinterpret_cast<uint64_t*>(base + L.queue),
                    reinterpret_cast<uint32_t*>(base + L.cand_id), reinterpret_cast<float*>(base + L.cand_d)};
-  const uint32_t** fslot = reinterpret_cast<const uint32_t**>(base + L.bar);
+  FilterSlot* fslot = reinterpret_cast<FilterSlot*>(base + L.bar);
   const uint32_t slot = blockIdx.x * (blockDim.x >> 5) + warp;  // the host launches fewer warps per CTA when shared memory is short
   Visited vis;
   vis.init(p.vis, slot);
@@ -168,9 +179,16 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
     const uint32_t qi = next_item(p.work_counter, lane);
     if (qi >= p.nq) break;
     stage_row_bytes(s.q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes, p.q_bytes, g.d4 * 16);
-    // this query's bitmap: the launch's one filter, or its own entry of the filter table.  It is kept in the warp's
-    // mbarrier slot (unused by this kernel) and read at each use, so that the search loop holds no extra register.
-    if (lane == 0) *fslot = p.filter_sel ? p.filter_table[p.filter_sel[qi]] : p.filter_bits;
+    // this query's filter: the launch's one bitmap, its own entry of the bitmap table, or its own label
+    if (lane == 0) {
+      if (p.labels) {
+        fslot->ptr = p.labels;
+        fslot->label = p.filter_sel[qi];
+      } else {
+        fslot->ptr = p.filter_sel ? p.filter_table[p.filter_sel[qi]] : p.filter_bits;
+        fslot->label = LABEL_NONE;
+      }
+    }
     __syncwarp();
     int count = 0;
     bool overflow = false;
@@ -194,7 +212,7 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
       bool keep = false;
       if (j < count) {
         key = W.w[j];
-        keep = filter_pass(*fslot, key_id(key));
+        keep = filter_pass(fslot, key_id(key));
       }
       const unsigned m = __ballot_sync(FULL, keep);
       if (keep) {

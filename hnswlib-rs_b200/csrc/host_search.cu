@@ -203,11 +203,20 @@ int Index::resolve_filter(const FilterArg& f, bool exact, Leg* legs, size_t n, s
 }
 
 // Every filter is checked on every partition before anything runs, so that a bad entry refuses the whole call, named by
-// its first position.  The sort is stable: rows of one filter keep their order, and -1 (no filter) sorts first.
-int Index::sort_per_query(const int64_t* fid, size_t nq, std::vector<size_t>& perm) {
+// its first position.  The sort is stable: rows of one filter keep their order, and -1 (no filter) sorts first.  A label
+// needs no check; LABEL_NONE sorts first as -1.
+int Index::sort_per_query(const HostBatch& b, std::vector<size_t>& perm, std::vector<int64_t>& sorted) {
   const int P = parts ? parts->count() : 1;
+  const size_t nq = b.nq;
+  std::vector<int64_t> key;
+  const int64_t* fid = b.per_query;
+  if (b.labels) {
+    key.resize(nq);
+    for (size_t i = 0; i < nq; ++i) key[i] = b.labels[i] == LABEL_NONE ? -1 : (int64_t)b.labels[i];
+    fid = key.data();
+  }
   std::set<int64_t> checked;
-  for (size_t i = 0; i < nq; ++i) {
+  for (size_t i = 0; !b.labels && i < nq; ++i) {
     if (fid[i] == -1 || checked.count(fid[i])) continue;
     for (int p = 0; p < P; ++p) {
       Index* rx = parts ? parts->part(p) : this;
@@ -220,10 +229,12 @@ int Index::sort_per_query(const int64_t* fid, size_t nq, std::vector<size_t>& pe
   perm.resize(nq);
   std::iota(perm.begin(), perm.end(), (size_t)0);
   std::stable_sort(perm.begin(), perm.end(), [&](size_t a, size_t b) { return fid[a] < fid[b]; });
+  sorted.resize(nq);
+  for (size_t j = 0; j < nq; ++j) sorted[j] = fid[perm[j]];
   return 0;
 }
 
-int Index::resolve_per_query(const std::vector<int64_t>& sorted, bool exact, Leg* legs, size_t n) {
+int Index::resolve_per_query(const std::vector<int64_t>& sorted, bool labels, bool exact, Leg* legs, size_t n) {
   const int P = parts ? parts->count() : 1;
   int r = 0;
   for (Leg* l = legs; l < legs + n; ++l) {  // every leg, so that the caller reports the failure it chooses
@@ -231,12 +242,27 @@ int Index::resolve_per_query(const std::vector<int64_t>& sorted, bool exact, Leg
     const int64_t* f = sorted.data() + l->first;
     q.on = true;
     while (q.plain < l->count && f[q.plain] == -1) ++q.plain;
+    // labels: the leg's own, or on a replica its copy of the handle's, made current first.  The graph search reads the
+    // label array and each row's label; the exact scan, a slice per label of the leg's CSR.
+    if (labels && q.plain < l->count && l->rx->labels_on_device(parts ? l->rx : this, &q.labels)) {
+      r = l->rc = -1;
+      continue;
+    }
     if (exact && q.plain) q.groups.push_back(ExactGroup{0, q.plain, ExactScan()});
-    for (size_t j = q.plain, e; j < l->count; j = e) {  // one run of rows per filter
+    for (size_t j = q.plain, e; j < l->count; j = e) {  // one run of rows per filter or label
       for (e = j + 1; e < l->count && f[e] == f[j];) ++e;
       ExactScan s;
       const uint32_t* bits = nullptr;
-      if (filters.use(f[j], l->part, P, l->rx, &bits, exact ? &s : nullptr)) {
+      if (labels) {
+        if (!exact) {
+          q.sel.insert(q.sel.end(), e - j, (uint32_t)f[j]);
+          continue;
+        }
+        if (l->rx->label_scan((uint32_t)f[j], &s)) {
+          r = l->rc = -1;
+          break;
+        }
+      } else if (filters.use(f[j], l->part, P, l->rx, &bits, exact ? &s : nullptr)) {
         r = l->rc = -1;
         break;
       }
@@ -299,20 +325,18 @@ int Index::search_batch(const HostBatch& call) {
   if (call.nq == 0) return 0;
   if (parts && dim != 0 && call.d != dim) return fail("query length differs from the index dimension");
   int r;
-  // a filter per query: the batch is planned over the rows sorted by filter, gathered through row pointers, and each
-  // answer goes back to its caller's row
+  // a filter or a label per query: the batch is planned over the rows sorted by filter or label, gathered through row
+  // pointers, and each answer goes back to its caller's row
   HostBatch b = call;
   std::vector<size_t> perm;
   std::vector<const void*> rows;
   std::vector<int64_t> sorted;
-  if (call.per_query) {
-    if ((r = sort_per_query(call.per_query, call.nq, perm))) return r;
+  const bool per_row = call.per_query || call.labels;
+  if (per_row) {
+    if ((r = sort_per_query(call, perm, sorted))) return r;
     rows.resize(call.nq);
-    sorted.resize(call.nq);
-    for (size_t j = 0; j < call.nq; ++j) {
+    for (size_t j = 0; j < call.nq; ++j)
       rows[j] = call.rows ? call.rows[perm[j]] : (const char*)call.queries + perm[j] * (size_t)call.d * es;
-      sorted[j] = call.per_query[perm[j]];
-    }
     b.rows = rows.data();
     b.out.perm = perm.data();
   }
@@ -321,7 +345,8 @@ int Index::search_batch(const HostBatch& call) {
   if ((r = plan(b.nq, legs))) return r;
   const int n = (int)legs.size();
   const bool sharded = n > 1 && !parts;
-  if (b.per_query ? resolve_per_query(sorted, b.exact, legs.data(), n) : resolve_filter(b.filter, b.exact, legs.data(), n, bits))
+  if (per_row ? resolve_per_query(sorted, b.labels != nullptr, b.exact, legs.data(), n)
+              : resolve_filter(b.filter, b.exact, legs.data(), n, bits))
     return legs_fail(legs.data(), n, sharded);
   if (n == 1 && !parts) {
     begin_leg(b, legs[0]);

@@ -95,6 +95,7 @@ Index::~Index() {
   if (stream_) cudaStreamSynchronize(stream_);
   for (void* a : graph_.p) cudaFree(a);
   cudaFree(vis_.tab); cudaFree(vis_.epoch); cudaFree(d_counter_); cudaFree(d_status_); cudaFree(d_stats_); cudaFree(d_mask_);
+  cudaFree(label_csr_.d_ids);
   if (h_pin_) cudaFreeHost(h_pin_);
   for (SearchCtx& c : ctx_) {
     if (c.stream) cudaStreamSynchronize(c.stream);
@@ -324,6 +325,7 @@ void Index::resize_points(size_t count) {
   h_plevel.resize(count);
   h_rank.resize(count);
   h_origin.resize(count);
+  h_label.resize(count, LABEL_NONE);
   h_upoff.resize(count);
 }
 
@@ -338,6 +340,7 @@ int Index::upload_points(size_t first, size_t count) {
   HB_CUDA(cudaMemcpyAsync(graph_.at<uint8_t>(GS::PLEVEL) + first, h_plevel.data() + first, count, cudaMemcpyHostToDevice, stream_));
   HB_CUDA(cudaMemcpyAsync(graph_.at<uint64_t>(GS::ORIGIN) + first, h_origin.data() + first, count * 8, cudaMemcpyHostToDevice, stream_));
   HB_CUDA(cudaMemcpyAsync(graph_.at<uint32_t>(GS::UP_OFF) + first, h_upoff.data() + first, count * 4, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.at<uint32_t>(GS::LABEL) + first, h_label.data() + first, count * 4, cudaMemcpyHostToDevice, stream_));
   return 0;
 }
 
@@ -667,7 +670,7 @@ int Index::stream_wait_last(cudaStream_t s) {
 
 int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const uint32_t* d_filter_bits,
                          NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint32_t* const* d_ftab,
-                         const uint32_t* d_fsel) {
+                         const uint32_t* d_fsel, const uint32_t* d_labels) {
   if (k == 0) return fail("knbn must be positive");
   if (poisoned_) return fail(poison_msg_);
   cudaStream_t st = c.stream;
@@ -694,6 +697,7 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.filter_bits = d_filter_bits;
   p.filter_table = d_ftab;
   p.filter_sel = d_fsel;
+  p.labels = d_labels;
   p.stats = stats_on_ ? d_stats_ : nullptr;
   p.status = c.d_status;
   const bool filtered = d_filter_bits != nullptr || d_fsel != nullptr;
@@ -840,17 +844,19 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
     return exact_on_ctx(c, c.d_xq, nq, k, *scan, k_out, k_cnt, false, nullptr, pq && pq->on ? &pq->groups : nullptr);
   }
   if (pq && pq->on) {
-    // a filter per query: the bitmap table and the filtered rows' entries go to the device ahead of the launches
+    // a filter per query: the bitmap table and the filtered rows' entries go to the device ahead of the launches (a
+    // label per query: the labelled rows' labels; the label array is already there)
     const size_t tb = round128(pq->table.size() * sizeof(void*)), sb = pq->sel.size() * sizeof(uint32_t);
     if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, tb + sb, st))) return r;
     if (sb) {
-      HB_CUDA(cudaMemcpyAsync(c.d_fbits, pq->table.data(), pq->table.size() * sizeof(void*), cudaMemcpyHostToDevice, st));
+      if (tb) HB_CUDA(cudaMemcpyAsync(c.d_fbits, pq->table.data(), pq->table.size() * sizeof(void*), cudaMemcpyHostToDevice, st));
       HB_CUDA(cudaMemcpyAsync((char*)c.d_fbits + tb, pq->sel.data(), sb, cudaMemcpyHostToDevice, st));
     }
     c.pend.per_query = true;
     c.pend.plain = pq->plain;
     c.pend.ftab = (const uint32_t* const*)c.d_fbits;
     c.pend.fsel = (const uint32_t*)((char*)c.d_fbits + tb);
+    c.pend.labels = pq->labels;
     c.pend.d_queries = d_queries;
     c.pend.k_out = k_out;
     c.pend.k_cnt = k_cnt;
@@ -894,7 +900,8 @@ int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** 
 }
 
 // the rows without a filter as an ordinary unfiltered launch, then every filtered row in one filtered launch on the
-// bitmap table; both share the context's status, so an overflow in either re-runs both (sync: growing the tables)
+// bitmap table or the label array; both share the context's status, so an overflow in either re-runs both (sync:
+// growing the tables)
 int Index::per_query_on_ctx(SearchCtx& c, bool sync) {
   const SearchCtx::Pending& p = c.pend;
   int r;
@@ -902,7 +909,7 @@ int Index::per_query_on_ctx(SearchCtx& c, bool sync) {
   if (p.nq == p.plain) return 0;
   const char* fq = (const char*)p.d_queries + p.plain * (size_t)dim * es;
   return search_on_ctx(c, fq, p.nq - p.plain, p.k, p.ef, nullptr, p.k_out + p.plain * p.k, p.k_cnt + p.plain, sync, nullptr,
-                       p.ftab, p.fsel);
+                       p.labels ? nullptr : p.ftab, p.fsel, p.labels);
 }
 
 int Index::make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx,

@@ -17,6 +17,7 @@
 #include <tuple>
 #include <string>
 #include <thread>
+#include <unordered_map>
 #include <vector>
 
 #include "kernels.h"
@@ -60,9 +61,9 @@ struct DevBuf {  // device memory freed on scope exit, so that no early return l
 };
 
 // The device arrays that hold the graph.  Replication blob i is array i, in this order (the order is part of the blob
-// protocol between processes); the per-point insert locks come last and are not replicated.
+// protocol between processes); the per-point insert locks and labels come last and are not replicated.
 struct GraphStore {
-  enum Array { VEC, ADJ0, ADJU, UP_OFF, PLEVEL, LEVEL, ORIGIN, ADJ0_D, ADJU_D, LOCKS, COUNT };
+  enum Array { VEC, ADJ0, ADJU, UP_OFF, PLEVEL, LEVEL, ORIGIN, ADJ0_D, ADJU_D, LOCKS, LABEL, COUNT };
   static constexpr int BLOBS = LOCKS;
   // elements per point: a vector row (row_bytes), a layer-0 list (2M), one; or per upper-layer list: a list (M)
   enum Row { VEC_ROW, LIST0, ONE, LISTU };
@@ -82,6 +83,7 @@ struct GraphStore {
       {4, LIST0, 0},     // ADJ0_D: neighbour distances
       {4, LISTU, 0},     // ADJU_D
       {4, ONE, 0},       // LOCKS
+      {4, ONE, 0xFF},    // LABEL: the point's label, LABEL_NONE = none
   };
   void* p[COUNT] = {};
   size_t cap = 0, cap_ul = 0;  // points / upper-layer lists allocated
@@ -217,16 +219,19 @@ struct HostBatch {
   AnswerArrays out;
   bool exact = false;
   const int64_t* per_query = nullptr;  // [nq]: each query's resident filter, or -1 for none (then `filter` is unused)
+  const uint32_t* labels = nullptr;    // [nq]: each query's label, or LABEL_NONE for none (then `filter` is unused)
 };
 
-// A leg's share of a batch with a filter per query, whose rows the driver sorted by filter (resolve_per_query): the
-// leg's first `plain` rows have no filter.  Graph search: its row plain + i uses bitmap table[sel[i]].  Exact scan:
+// A leg's share of a batch with a filter or a label per query, whose rows the driver sorted by filter or label
+// (resolve_per_query): the leg's first `plain` rows have neither.  Graph search: its row plain + i uses bitmap
+// table[sel[i]], or with `labels` (the label array on the leg's device) the points labelled sel[i].  Exact scan:
 // `groups`, its rows by the points they scan (every point for the plain rows).
 struct LegFilters {
   bool on = false;
   size_t plain = 0;
   std::vector<const uint32_t*> table;
   std::vector<uint32_t> sel;
+  const uint32_t* labels = nullptr;
   std::vector<ExactGroup> groups;
 };
 
@@ -271,6 +276,7 @@ class Index {
   std::vector<uint8_t> h_level, h_plevel;
   std::vector<int32_t> h_rank;
   std::vector<uint64_t> h_origin;
+  std::vector<uint32_t> h_label;  // LABEL_NONE = none (labels.cu)
   std::vector<uint32_t> h_upoff;
 
   // ---- operations (return 0 or a negative status; message in err())
@@ -310,11 +316,23 @@ class Index {
   // instead (the resident filter's id list on the leg's device, or every point).
   int resolve_filter(const FilterArg& f, bool exact, Leg* legs, size_t n, std::vector<std::vector<uint32_t>>& bits);
   // a batch with a filter per query: every entry of filters[0, nq) is -1 or a live, current filter of this handle (else
-  // the first bad position is refused), and `perm` orders the rows stably by filter, the unfiltered ones first
-  int sort_per_query(const int64_t* filters, size_t nq, std::vector<size_t>& perm);
-  // each leg's LegFilters for the rows sorted by filter (sorted[j]: the filter of sorted row j), on its partition and
-  // device; nonzero when a leg could not have them, with that leg's rc set
-  int resolve_per_query(const std::vector<int64_t>& sorted, bool exact, Leg* legs, size_t n);
+  // the first bad position is refused), and `perm` orders the rows stably by filter, the unfiltered ones first.  A
+  // label per query (b.labels): by label, LABEL_NONE first.  sorted[j]: the filter or label of sorted row j (-1: none).
+  int sort_per_query(const HostBatch& b, std::vector<size_t>& perm, std::vector<int64_t>& sorted);
+  // each leg's LegFilters for the rows sorted by filter or label, on its partition and device; nonzero when a leg could
+  // not have them, with that leg's rc set
+  int resolve_per_query(const std::vector<int64_t>& sorted, bool labels, bool exact, Leg* legs, size_t n);
+
+  // ---- point labels (labels.cu).  One u32 per point (GraphStore LABEL and its host mirror h_label), LABEL_NONE until
+  // set_labels names one; label_version counts the calls that changed them (a replica: the handle's version it copied).
+  uint64_t label_version = 0;
+  // labels[0, count) for the points [first, first + count) of this Index (the caller checked the range)
+  int set_labels(size_t first, size_t count, const uint32_t* labels);
+  // the label array on this Index's device, as current as `src`'s (a replica's copy of the handle's labels, refreshed
+  // when src's changed; src == this: its own)
+  int labels_on_device(const Index* src, const uint32_t** d_labels);
+  // the exact scan of the points labelled `label`: a slice of this Index's label CSR, rebuilt when the labels changed
+  int label_scan(uint32_t label, ExactScan* scan);
   // device queries in, device answers out; the filter is none or a resident filter.  `exact`: the exact scan (ef unused).
   int search_device(const FilterArg& f, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef, NeighbourOut* d_out,
                     int32_t* d_counts, bool sync, float* kernel_ms);
@@ -388,11 +406,13 @@ class Index {
       const void* d_queries = nullptr;
       const uint32_t* dfb = nullptr;
       bool exact = false;  // an exact scan: no status, nothing to re-run
-      // a filter per query: rows [0, plain) unfiltered, the others on the device bitmap table / selectors
+      // a filter per query: rows [0, plain) unfiltered, the others on the device bitmap table / selectors; a label per
+      // query: on the device label array, fsel holding the rows' labels
       bool per_query = false;
       size_t plain = 0;
       const uint32_t* const* ftab = nullptr;
       const uint32_t* fsel = nullptr;
+      const uint32_t* labels = nullptr;
       NeighbourOut *k_out = nullptr, *hout = nullptr;
       int32_t *k_cnt = nullptr, *hcnt = nullptr, *hstatus = nullptr;
       size_t nq = 0, k = 0, ef = 0;
@@ -445,7 +465,7 @@ class Index {
   // ---- point ledger: the host mirrors (h_level ... h_upoff) and the per-layer counts
   void resize_points(size_t count);
   void rank_points();  // layer_count and h_rank from h_level, in internal-id order
-  int upload_points(size_t first, size_t count);  // level, plevel, origin, up_off of [first, first + count)
+  int upload_points(size_t first, size_t count);  // level, plevel, origin, up_off, label of [first, first + count)
   // ---- graph export
   struct ListRef {  // a point's list at one layer: adj0 (layer 0) or adjU from element `at`, `cap` slots (0: none)
     size_t at, cap;
@@ -480,6 +500,18 @@ class Index {
   int end_leg(Leg& l, size_t k, const AnswerArrays& out);
   int legs_fail(const Leg* legs, size_t n, bool replicas_first);
 
+  // ---- point labels (labels.cu).  The CSR of the exact path: the internal ids of every labelled point on this device,
+  // grouped by label and ascending within a group; groups[label] = (offset, count).  Made from h_label at label version
+  // `version` (~0: never), at the first exact labelled search after the labels changed.  A point added since has no
+  // label, so inserts leave it current.  label_mu_ guards it and a replica's copy of the labels.
+  struct LabelCsr {
+    void* d_ids = nullptr;
+    size_t bytes = 0;
+    uint64_t version = ~0ull;
+    std::unordered_map<uint32_t, std::pair<uint32_t, uint32_t>> groups;
+  } label_csr_;
+  std::mutex label_mu_;
+
   int broadcast_to_replicas();
   std::vector<std::unique_ptr<Index>> replicas_;  // replicas_[i] lives on replica_devices_[i + 1]
   WorkerGroup workers_;                           // worker i serves replicas_[i]
@@ -501,10 +533,12 @@ class Index {
 
   VisitedPool vis_;  // visited tables of the insert kernel (searches: SearchCtx)
   SearchCtx ctx_[NCTX + NASYNC];
-  // d_ftab / d_fsel: a filter per query, query i on bitmap d_ftab[d_fsel[i]] (then d_filter_bits is null)
+  // d_ftab / d_fsel: a filter per query, query i on bitmap d_ftab[d_fsel[i]] (then d_filter_bits is null); with
+  // d_labels instead of d_ftab, a label per query: query i on the points whose d_labels entry is d_fsel[i]
   int search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const uint32_t* d_filter_bits,
                     NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms,
-                    const uint32_t* const* d_ftab = nullptr, const uint32_t* d_fsel = nullptr);
+                    const uint32_t* const* d_ftab = nullptr, const uint32_t* d_fsel = nullptr,
+                    const uint32_t* d_labels = nullptr);
   // the exact k nearest of device queries among scan's points (aux.cu); the slices' scratch is sized before the launch.
   // With `groups` (a filter per query), each group's rows among that group's points instead of scan's.
   int exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const ExactScan& scan, NeighbourOut* d_out,

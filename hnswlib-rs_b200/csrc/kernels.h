@@ -54,7 +54,13 @@ struct SearchParams {
   // instead of filter_bits.  Appended, so that every field above keeps its offset.
   const uint32_t* const* filter_table;
   const uint32_t* filter_sel;  // [nq]
+  // filtered search with a label per query (labels != nullptr): query i admits the points p with labels[p] ==
+  // filter_sel[i] (never LABEL_NONE) instead of a bitmap.  Appended like the two above.
+  const uint32_t* labels;  // [points]
 };
+
+// the label of a point that has none (hnsw_b200_set_labels): no label admits it
+constexpr uint32_t LABEL_NONE = 0xFFFFFFFFu;
 
 // rows of up to 512 bytes are (partly) staged by TMA: STAGE_ROWS rows + an mbarrier per warp
 __host__ __device__ inline size_t stage_bytes(int d4) { return d4 <= 32 ? (size_t)STAGE_ROWS * d4 * 16 : 0; }

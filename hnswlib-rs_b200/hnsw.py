@@ -103,6 +103,10 @@ def load_library():
     L.hnsw_b200_search_exact_device.argtypes = [vp, i64, vp, u64, u64, vp, vp, i32, vp]
     L.hnsw_b200_search_flat_per_query.argtypes = [vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_exact_per_query.argtypes = [vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_set_labels.argtypes = [vp, u64, u64, vp]
+    L.hnsw_b200_get_labels.argtypes = [vp, u64, u64, vp]
+    L.hnsw_b200_search_flat_labeled.argtypes = [vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_exact_labeled.argtypes = [vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_get_stats.argtypes = [vp, vp, i32]
     L.hnsw_b200_set_stream.argtypes = [vp, vp]
     L.hnsw_b200_join.argtypes = [vp]
@@ -228,6 +232,19 @@ def _filter_ids(filters, nq):
     if len(filters) != nq:
         raise ValueError(f"filters has {len(filters)} entries for {nq} queries")
     return np.ascontiguousarray([_filter_id(f) for f in filters], np.int64).reshape(nq)
+
+
+LABEL_NONE = 0xFFFFFFFF   # hnsw_b200.h HNSW_B200_LABEL_NONE: the label of a point that has none
+
+
+def _labels(labels, n, what):
+    """one uint32 label per entry (LABEL_NONE: none), as a contiguous array"""
+    a = np.asarray(labels)
+    if a.shape != (n,):
+        raise ValueError(f"{what} has shape {a.shape}, expected ({n},)")
+    if a.size and (a.min() < 0 or a.max() > LABEL_NONE):
+        raise ValueError(f"{what}: labels are unsigned 32-bit integers")
+    return np.ascontiguousarray(a, np.uint32)
 
 
 class Hnsw:
@@ -445,6 +462,43 @@ class Hnsw:
         ResidentFilter of this handle, or None for every point), in one batch.  Returns search_exact's tuple."""
         return self._per_query(self._L.hnsw_b200_search_exact_per_query, queries, knbn, filters, (), with_internal,
                                with_pid)
+
+    def set_labels(self, first, labels):
+        """hnsw_b200_set_labels: the labels of the points with insertion ranks first .. first + len(labels) - 1
+        (LABEL_NONE clears one).  Every point starts without a label."""
+        lab = np.ascontiguousarray(labels).reshape(-1)
+        lab = _labels(lab, lab.size, "labels")
+        self._chk(self._L.hnsw_b200_set_labels(self._h, int(first), lab.size, _p(lab)))
+
+    def get_labels(self, first, n):
+        """hnsw_b200_get_labels: the labels of the points first .. first + n - 1, as uint32 (LABEL_NONE: none)"""
+        out = np.empty(int(n), np.uint32)
+        self._chk(self._L.hnsw_b200_get_labels(self._h, int(first), int(n), _p(out)))
+        return out
+
+    def _labeled(self, fn, queries, knbn, labels, ef_args, with_internal, with_pid):
+        q = np.ascontiguousarray(queries, self.dtype)
+        nq, d = q.shape
+        lab = _labels(labels, nq, "labels")
+        o = np.empty((nq, knbn), np.uint64)
+        ds = np.empty((nq, knbn), np.float32)
+        it = np.empty((nq, knbn), np.uint32) if with_internal else None
+        pid = np.empty((nq, knbn, 2), np.int32) if with_pid else None
+        cnt = np.empty(nq, np.int32)
+        self._chk(fn(self._h, _p(lab), _p(q), nq, d, int(knbn), *ef_args, _p(o), _p(ds), _p(it), _p(pid), _p(cnt)))
+        return o, ds, it, pid, cnt
+
+    def search_flat_labeled(self, queries, knbn, ef, labels, with_internal=True, with_pid=True):
+        """hnsw_b200_search_flat_labeled: one batch, query i restricted to the points labelled labels[i] (LABEL_NONE:
+        every point).  Row i equals search_flat with a resident filter admitting exactly those points.  Returns
+        search_flat's (origin, dist, internal | None, pid | None, counts)."""
+        return self._labeled(self._L.hnsw_b200_search_flat_labeled, queries, knbn, labels, (int(ef),), with_internal,
+                             with_pid)
+
+    def search_exact_labeled(self, queries, knbn, labels, with_internal=True, with_pid=True):
+        """hnsw_b200_search_exact_labeled: the exact knbn nearest of query i among the points labelled labels[i]
+        (LABEL_NONE: every point), in one batch.  Returns search_exact's tuple."""
+        return self._labeled(self._L.hnsw_b200_search_exact_labeled, queries, knbn, labels, (), with_internal, with_pid)
 
     def make_filter(self, filter):
         """hnsw_b200_filter_new: materialise a FilterT (sorted id sequence or callable(id)->bool, as search_flat takes)

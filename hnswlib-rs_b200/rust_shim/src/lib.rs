@@ -83,7 +83,19 @@ extern "C" {
     fn hnsw_b200_search_exact_per_query(h: *const HnswApif32, filters: *const i64, queries: *const f32, nq: u64, dim: u64,
                                         knbn: u64, out_ids: *mut u64, out_dist: *mut f32, out_internal: *mut u32,
                                         out_pid: *mut i32, out_counts: *mut i32) -> c_int;
+    // point labels (include/hnsw_b200.h "Point labels"): qlabels[i] = a label, or LABEL_NONE for every point
+    fn hnsw_b200_set_labels(h: *mut HnswApif32, first: u64, n: u64, labels: *const u32) -> c_int;
+    fn hnsw_b200_get_labels(h: *const HnswApif32, first: u64, n: u64, out: *mut u32) -> c_int;
+    fn hnsw_b200_search_flat_labeled(h: *const HnswApif32, qlabels: *const u32, queries: *const f32, nq: u64, dim: u64,
+                                     knbn: u64, ef: u64, out_ids: *mut u64, out_dist: *mut f32, out_internal: *mut u32,
+                                     out_pid: *mut i32, out_counts: *mut i32) -> c_int;
+    fn hnsw_b200_search_exact_labeled(h: *const HnswApif32, qlabels: *const u32, queries: *const f32, nq: u64, dim: u64,
+                                      knbn: u64, out_ids: *mut u64, out_dist: *mut f32, out_internal: *mut u32,
+                                      out_pid: *mut i32, out_counts: *mut i32) -> c_int;
 }
+
+/// The label of a point that has none (include/hnsw_b200.h HNSW_B200_LABEL_NONE): no label admits it.
+pub const LABEL_NONE: u32 = 0xFFFF_FFFF;
 
 /// hnsw.rs:46
 #[derive(Debug, Clone, Copy, Default, PartialEq, Eq)]
@@ -258,6 +270,46 @@ impl<D: DistName> Hnsw<D> {
             }
         };
         assert_eq!(r, 0, "hnsw_b200_search_flat_per_query / _exact_per_query failed");
+        (0..nq).map(|i| (0..cnt[i] as usize).map(|j| {
+            let s = i * knbn + j;
+            Neighbour { d_id: ids[s] as usize, distance: ds[s], p_id: PointId(pid[2 * s] as u8, pid[2 * s + 1]) }
+        }).collect()).collect()
+    }
+    /// Extension: label the points with insertion ranks `first .. first + labels.len()` (LABEL_NONE clears a label).
+    /// Every point starts without one; labels are not written into dumps.  Err when the range passes nb_point.
+    pub fn set_labels(&mut self, first: usize, labels: &[u32]) -> Result<(), i32> {
+        let r = unsafe { hnsw_b200_set_labels(self.h, first as u64, labels.len() as u64, labels.as_ptr()) };
+        if r == 0 { Ok(()) } else { Err(r) }
+    }
+    /// Extension: the labels of the points `first .. first + n`
+    pub fn get_labels(&self, first: usize, n: usize) -> Result<Vec<u32>, i32> {
+        let mut out = vec![LABEL_NONE; n];
+        let r = unsafe { hnsw_b200_get_labels(self.h, first as u64, n as u64, out.as_mut_ptr()) };
+        if r == 0 { Ok(out) } else { Err(r) }
+    }
+    /// Extension: one batch, request i restricted to the points labelled `labels[i]` (LABEL_NONE: every point); answer i
+    /// is what search_resident returns with a filter admitting exactly those points (search, for LABEL_NONE).  Graph
+    /// search with `Some(ef)`, the exact scan with None.
+    pub fn search_labeled(&self, datas: &[Vec<f32>], knbn: usize, ef: Option<usize>, labels: &[u32]) -> Vec<Vec<Neighbour>> {
+        assert_eq!(datas.len(), labels.len(), "one label per request");
+        if datas.is_empty() { return Vec::new(); }
+        let (nq, dim) = (datas.len(), datas[0].len());
+        let flat: Vec<f32> = datas.iter().flat_map(|d| d.iter().copied()).collect();
+        let mut ids = vec![0u64; nq * knbn];
+        let mut ds = vec![0f32; nq * knbn];
+        let mut pid = vec![0i32; 2 * nq * knbn];
+        let mut cnt = vec![0i32; nq];
+        let r = unsafe {
+            match ef {
+                Some(ef) => hnsw_b200_search_flat_labeled(self.h, labels.as_ptr(), flat.as_ptr(), nq as u64, dim as u64, knbn as u64,
+                                                          ef as u64, ids.as_mut_ptr(), ds.as_mut_ptr(), std::ptr::null_mut(),
+                                                          pid.as_mut_ptr(), cnt.as_mut_ptr()),
+                None => hnsw_b200_search_exact_labeled(self.h, labels.as_ptr(), flat.as_ptr(), nq as u64, dim as u64, knbn as u64,
+                                                       ids.as_mut_ptr(), ds.as_mut_ptr(), std::ptr::null_mut(), pid.as_mut_ptr(),
+                                                       cnt.as_mut_ptr()),
+            }
+        };
+        assert_eq!(r, 0, "hnsw_b200_search_flat_labeled / _exact_labeled failed");
         (0..nq).map(|i| (0..cnt[i] as usize).map(|j| {
             let s = i * knbn + j;
             Neighbour { d_id: ids[s] as usize, distance: ds[s], p_id: PointId(pid[2 * s] as u8, pid[2 * s + 1]) }

@@ -365,6 +365,39 @@ int hnsw_b200_search_exact_per_query(const void* h, const int64_t* filters, cons
                                      uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                      int32_t* out_pid, int32_t* out_counts);
 
+/* ---- Point labels: one u32 per point (a tenant, owner or category id), and searches in which each query is restricted
+ * to the points of one label.  A label costs 4 bytes per point on the device and on the host whatever the number of
+ * labels, and no insert makes it stale, where a resident filter per tenant costs n/8 bytes per tenant and goes stale at
+ * the next insert.
+ *   Labels: every point starts with HNSW_B200_LABEL_NONE (new inserts, imports, reloaded dumps and replication blobs);
+ *     no label admits such a point.  Labels are not written into the dump files: hnsw_b200_get_labels reads them back
+ *     so that the caller can store them.
+ *   set_labels sets the labels of the points with insertion ranks [first, first + n) (a partitioned handle: global
+ *     ranks, point g is local point g / P of partition g % P).  first + n > nb_point is refused and nothing changes;
+ *     HNSW_B200_LABEL_NONE clears a label.  It takes the handle exclusively, as an insert does; a partition view refuses
+ *     it.  get_labels reads [first, first + n) into out[n] (a view: its own partition's local points).
+ *   Searches: search_flat_labeled / search_exact_labeled take the arguments and outputs of search_flat_per_query /
+ *     search_exact_per_query with qlabels[nq] in place of filters.  Row i is, bit for bit, what search_flat_filtered /
+ *     search_exact return for query i with a resident filter that admits exactly the points labelled qlabels[i] (ids,
+ *     distance bits, internal ids, PointIds, count), and with qlabels[i] == HNSW_B200_LABEL_NONE what the unfiltered
+ *     search_flat / search_exact return; so labelled rows ignore the tie mode and the others follow it.  With
+ *     statistics on, the counters add up as the per-query call's do.  qlabels == NULL with nq > 0 is refused; nq == 0
+ *     returns 0; a label no point carries gives count 0.
+ *   Handles: a partitioned handle merges each row over the partitions as partitioned search does.  A replicated handle
+ *     shards the batch; each replica's device gets a copy of the labels at its first labelled search after they
+ *     changed.  A partition view searches with its own partition's labels and reports local ids.  In the
+ *     one-process-per-GPU mode (nccl_broadcast_index) labels are not broadcast: each rank sets its own.
+ *   Filters: no label call reads or changes resident filters, and no filter call reads or changes labels. */
+#define HNSW_B200_LABEL_NONE 0xFFFFFFFFu
+int hnsw_b200_set_labels(void* h, uint64_t first, uint64_t n, const uint32_t* labels);
+int hnsw_b200_get_labels(const void* h, uint64_t first, uint64_t n, uint32_t* out);
+int hnsw_b200_search_flat_labeled(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim,
+                                  uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
+                                  uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
+int hnsw_b200_search_exact_labeled(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim,
+                                   uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                                   int32_t* out_pid, int32_t* out_counts);
+
 /* Run this handle's kernels and copies on a caller-owned CUDA stream (cudaStream_t passed as void*; NULL
  * restores the handle's own stream), e.g. so that torch.cuda.Event on torch's current stream brackets them. */
 int hnsw_b200_join(void* h);
