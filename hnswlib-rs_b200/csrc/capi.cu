@@ -513,6 +513,13 @@ int hnsw_b200_set_tie_mode(void* h, int mode) {
   apply(ix, [=](Index* x) { x->tie_std_ = mode == 1; });
   return 0;
 }
+int hnsw_b200_set_visited_stages(void* h, int mode) {
+  HB_H(h);
+  HB_NOT_VIEW(ix);
+  if (mode < 0 || mode > 2) return set_err("visited stages must be 0 (auto), 1 (always) or 2 (never)");
+  apply(ix, [=](Index* x) { x->visited_stages_ = mode; });
+  return 0;
+}
 int hnsw_b200_set_link_mode(void* h, int mode) {
   HB_H(h);
   HB_NOT_VIEW(ix);

@@ -60,7 +60,8 @@ struct GraphView {
 __device__ __forceinline__ int lane_id() { return threadIdx.x & 31; }
 
 // L2 cache policies (createpolicy): vector rows stream through once per query (evict_first), the per-warp visited
-// tables are re-read for the whole search (evict_last), so that 6 GB of rows per launch do not push them out of L2.
+// tables are re-read for the whole search (evict_last), so that 6 GB of rows per launch do not push them out first.
+// The tables do not all fit in L2 (50 MB) at once: see Visited for what a launch keeps resident.
 __device__ __forceinline__ uint64_t l2_policy_evict_first() {
   uint64_t p;
   asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
@@ -561,46 +562,62 @@ __device__ __forceinline__ void warp_dists_staged(const uint4* __restrict__ vec,
 }
 
 // ------------------------------------------------------------------------------------------------
-// Visited set: one open-addressing table per resident warp ("warp slot") in global memory (L2
-// resident).  Entry = (epoch << id_bits) | id; an entry whose epoch differs from the current one is
-// free, so a new search only bumps the epoch instead of clearing.  Exact (no false positives).
+// Visited set: one open-addressing table per resident warp ("warp slot") in global memory.  Entry =
+// (epoch << id_bits) | id; an entry whose epoch differs from the current one is free, so a new search only bumps the
+// epoch instead of clearing.  Exact (no false positives).
+//
+// Two stages per slot: a search starts in a small first stage (`small` entries) and moves, once, to the full stage
+// (`cap` entries) when the first one is 3/4 full.  Most searches never leave the first stage, so what a launch keeps
+// hot in L2 is about (slots x small) entries, not (slots x cap).  At the SIFT1M shape (M = 16, ef = 64: cap = 8192,
+// 21 one-warp CTAs x 132 SMs = 2 772 slots) full-size tables alone were 91 MB per search context against a 50 MB L2;
+// a search touched every line of its 32 KB table, so table lines were evicted between probes and re-read from HBM, and
+// they crowded out the rows and adjacency lists the kernel prefetches for itself.
 struct VisitedCfg {
-  uint32_t* tables;   // [n_slots][cap]
+  uint32_t* tables;   // [n_slots][small + cap]: first stage, then full stage
   uint32_t* epochs;   // [n_slots] persisted across launches
-  uint32_t cap;       // power of two
+  uint32_t cap;       // full stage, power of two
   int shift;          // 32 - log2(cap)
+  uint32_t small;     // first stage, power of two, < cap
+  int small_shift;    // 32 - log2(small)
   int id_bits;        // bits needed for ids
 };
 
-// The state of one warp's set is what changes during a search: table pointer, epoch, insert count.  Capacity, hash shift
-// and the epoch / id split are read from the launch's VisitedCfg (kernel parameters) where they are used.  Every
-// function is warp-collective and takes the caller's lane (the lean kernel pins it, see lean_common.cuh pin()).
+// The state of one warp's set is what changes during a search: the current stage (table pointer and hash shift; its
+// capacity is 2^(32 - shift)), epoch and insert count.  The stage sizes and the epoch / id split are read from the
+// launch's VisitedCfg (kernel parameters) where they are used.  Every function is warp-collective and takes the caller's
+// lane (the lean kernel pins it, see lean_common.cuh pin()).
 struct Visited {
-  uint32_t* tab;
+  uint32_t* tab;  // current stage: the slot's first stage, or its full stage (= first + small)
+  int shift;
   uint32_t epoch;
   uint32_t used;  // insertions of the current search (warp-uniform)
 
   __device__ __forceinline__ void init(const VisitedCfg& c, uint32_t slot) {
-    tab = c.tables + (size_t)slot * c.cap;
+    tab = c.tables + (size_t)slot * (c.small + c.cap);
+    shift = c.small_shift;
     epoch = c.epochs[slot];
     used = 0;
   }
   __device__ __forceinline__ void save(const VisitedCfg& c, uint32_t slot, int lane) const {
     if (lane == 0) c.epochs[slot] = epoch;
   }
-  static __device__ __forceinline__ uint32_t home(const VisitedCfg& c, uint32_t id) { return (id * 2654435761u) >> c.shift; }
-  // Start a new search from `entry` (hnsw.rs:955-956): bump the epoch instead of clearing the table (cleared only when the
-  // epoch wraps), then record the entry.  The table holds nothing of the new epoch yet, so the entry's home slot is free.
+  __device__ __forceinline__ uint32_t mask() const { return 0xFFFFFFFFu >> shift; }
+  __device__ __forceinline__ uint32_t home(uint32_t id) const { return (id * 2654435761u) >> shift; }
+  // Start a new search from `entry` (hnsw.rs:955-956) in the first stage: bump the epoch instead of clearing the tables
+  // (both stages are cleared only when the epoch wraps), then record the entry.  The stage holds nothing of the new
+  // epoch yet, so the entry's home slot is free.
   __device__ __forceinline__ void begin(const VisitedCfg& c, uint32_t entry, int lane) {
+    if (shift != c.small_shift) tab -= c.small;  // the last search moved to the full stage
+    shift = c.small_shift;
     const uint32_t epoch_max = (c.id_bits >= 32) ? 0u : ((1u << (32 - c.id_bits)) - 1u);
     if (epoch >= epoch_max) {
-      for (uint32_t i = lane; i < c.cap; i += 32) tab[i] = 0u;
+      for (uint32_t i = lane; i < c.small + c.cap; i += 32) tab[i] = 0u;
       epoch = 0;
     }
     epoch += 1;
     used = 1;
     __syncwarp();
-    if (lane == 0) st_keep(tab + home(c, entry), (epoch << c.id_bits) | entry, l2_policy_evict_last());
+    if (lane == 0) st_keep(tab + home(entry), (epoch << c.id_bits) | entry, l2_policy_evict_last());
     __syncwarp();
   }
   // Test-and-set of up to 32 ids (one per lane, `valid` lanes only).  Returns true in the lanes whose id was not yet in
@@ -612,7 +629,7 @@ struct Visited {
                                                uint32_t pre_h = 0, uint32_t pre_cv = 0) {
     const uint32_t want = (epoch << c.id_bits) | id;
     const uint64_t pol_keep = l2_policy_evict_last();
-    uint32_t h = pre ? pre_h : home(c, id);
+    uint32_t h = pre ? pre_h : home(id);
     bool pending = valid, fresh = false, first = pre;
     while (__any_sync(FULL, pending)) {
       uint32_t cur = 0;
@@ -625,7 +642,7 @@ struct Visited {
         } else if ((cur >> c.id_bits) != epoch) {
           claim = true;  // stale or empty slot
         } else {
-          h = (h + 1) & (c.cap - 1);
+          h = (h + 1) & mask();
         }
       }
       const unsigned claimers = __ballot_sync(FULL, claim);
@@ -640,7 +657,7 @@ struct Visited {
         } else if (lead_id == id) {
           pending = false;  // the same id twice in one chunk: the leader records it
         } else {
-          h = (h + 1) & (c.cap - 1);
+          h = (h + 1) & mask();
         }
       }
       __syncwarp();  // orders this round's stores before the next round's loads
@@ -648,8 +665,39 @@ struct Visited {
     used += __popc(__ballot_sync(FULL, fresh));  // warp-uniform count
     return fresh;
   }
-  __device__ __forceinline__ bool overflowing(const VisitedCfg& c) const { return used >= c.cap - (c.cap >> 2); }
+  // Called once per expansion, where an expansion has added at most one adjacency list.  A first stage at 3/4 of its
+  // capacity moves the search to the full stage (returns false); a full stage at 3/4 of its capacity is an overflow
+  // (returns true): the caller stops and the host re-runs the batch with larger tables.  A caller that probed ahead of
+  // time (the lean kernel's look-ahead) passes its flag, which a move clears.
+  __device__ __forceinline__ bool grow_or_overflow(const VisitedCfg& c, int lane, bool& probed_ahead);
+  __device__ __forceinline__ bool grow_or_overflow(const VisitedCfg& c, int lane) {
+    bool none = false;
+    return grow_or_overflow(c, lane, none);
+  }
 };
+
+// Move a search to the full stage: re-insert the live entries (current epoch) of the first stage, 32 per round; the last
+// searches' stale entries are skipped.  The full stage holds nothing of the current epoch before.  Returns the full
+// stage's state.  Out of line: it is the rare path, and inlined it took registers from the search loops around it.
+static __device__ __noinline__ Visited visited_migrate(const VisitedCfg c, const Visited from, int lane) {
+  Visited v{from.tab + c.small, c.shift, from.epoch, 0};  // `used` is counted again by the re-inserts
+  const uint64_t pol_keep = l2_policy_evict_last();
+#pragma unroll 1
+  for (uint32_t i = lane; i < c.small; i += 32) {
+    const uint32_t e = ld_keep(from.tab + i, pol_keep);
+    v.test_and_set(c, lane, e & ((1u << c.id_bits) - 1u), (e >> c.id_bits) == v.epoch);
+  }
+  return v;
+}
+// `probed_ahead` is cleared when the search moves: a probe read ahead of time came from the first stage.
+__device__ __forceinline__ bool Visited::grow_or_overflow(const VisitedCfg& c, int lane, bool& probed_ahead) {
+  if (shift == c.shift) return used >= c.cap - (c.cap >> 2);
+  if (used >= c.small - (c.small >> 2)) {
+    *this = visited_migrate(c, *this, lane);
+    probed_ahead = false;
+  }
+  return false;
+}
 
 // ------------------------------------------------------------------------------------------------
 // Queue keys: (float bits of distance << 32) | (id << 1) | expanded.  Distances are >= 0 so the

@@ -151,7 +151,7 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
       if (valid != FULL) break;
     }
     if (done && W.n == 0) break;
-    if (overflow || vis.overflowing(vc)) {
+    if (overflow || vis.grow_or_overflow(vc, lane)) {
       overflow = true;
       break;
     }

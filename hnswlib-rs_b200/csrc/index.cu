@@ -77,6 +77,7 @@ Index::Index(int M_, size_t max_elements_, int max_layer_, int ef_c_, int metric
   }
   own_stream_ = stream_;
   sm_count_ = prop.multiProcessorCount;
+  l2_bytes_ = (size_t)prop.l2CacheSize;
   if ((e = cudaMalloc(&d_counter_, sizeof(unsigned int))) != cudaSuccess || (e = cudaMalloc(&d_status_, sizeof(int))) != cudaSuccess ||
       (e = cudaMalloc(&d_stats_, 4 * sizeof(unsigned long long))) != cudaSuccess) {
     err_ = std::string("cudaMalloc: ") + cudaGetErrorString(e);
@@ -163,24 +164,25 @@ int Index::ensure_upper(size_t need) {
   return 0;
 }
 
-// A pool is laid out as [slots][cap] for the (slots, cap) it was last sized for.  Insert and filtered search share one
-// pool (large tables); unfiltered searches own another, so that their small L2-resident tables are not inflated by
-// the insert path's (4x larger: ef_construction instead of ef).
+// A pool is laid out as [slots][first stage + full stage] for the (slots, cap) it was last sized for, cap being the full
+// stage (Visited, common.cuh).  Insert and filtered search share one pool (large tables); unfiltered searches own
+// another, so that their small tables are not inflated by the insert path's (4x larger: ef_construction instead of ef).
 int Index::ensure_visited(VisitedPool& v, size_t slots, size_t cap_entries, cudaStream_t st) {
   if (slots <= v.slots && cap_entries <= v.cap) return 0;
   size_t ns = std::max(slots, v.slots), nc = std::max(cap_entries, v.cap);
-  if (ns * nc * sizeof(uint32_t) > ((size_t)8 << 30)) {  // do not carry a huge shape over (filtered searches use few, big tables)
+  if (ns * visited_slot_entries(nc) * sizeof(uint32_t) > ((size_t)8 << 30)) {  // do not carry a huge shape over (filtered searches use few, big tables)
     ns = slots;
     nc = cap_entries;
   }
+  const size_t bytes = ns * visited_slot_entries(nc) * sizeof(uint32_t);
   HB_CUDA(cudaStreamSynchronize(st));
   cudaFree(v.tab);
   cudaFree(v.epoch);
   v.tab = v.epoch = nullptr;
   v.slots = v.cap = 0;
-  HB_CUDA(cudaMalloc(&v.tab, ns * nc * sizeof(uint32_t)));
+  HB_CUDA(cudaMalloc(&v.tab, bytes));
   HB_CUDA(cudaMalloc(&v.epoch, ns * sizeof(uint32_t)));
-  HB_CUDA(cudaMemsetAsync(v.tab, 0, ns * nc * sizeof(uint32_t), st));
+  HB_CUDA(cudaMemsetAsync(v.tab, 0, bytes, st));
   // epoch = max forces a table clear on first use whatever id_bits is (Visited::begin)
   HB_CUDA(cudaMemsetAsync(v.epoch, 0xFF, ns * sizeof(uint32_t), st));
   v.slots = ns;
@@ -188,18 +190,41 @@ int Index::ensure_visited(VisitedPool& v, size_t slots, size_t cap_entries, cuda
   return 0;
 }
 
-int Index::fill_visited_cfg(VisitedPool& v, VisitedCfg& c, cudaStream_t st) {
+// `staged`: slots of [first stage + full stage], else of the full stage alone (small = 0: a search starts in the full stage
+// and never moves).  A stage is worth its denser probing only when the launch's full-size tables would not fit in L2
+// (visited_staged).
+int Index::fill_visited_cfg(VisitedPool& v, VisitedCfg& c, bool staged, cudaStream_t st) {
   const int id_bits = std::max(1, ilog2(std::max<size_t>(graph_.cap, 2)));
-  if (id_bits != v.id_bits) {  // entries are (epoch << id_bits) | id: a new split invalidates every table
+  // entries are (epoch << id_bits) | id at slot offsets of one layout: a new split or a new layout invalidates every table
+  // (epoch = max clears a slot's tables at its next begin())
+  if (id_bits != v.id_bits || staged != v.staged) {
     HB_CUDA(cudaMemsetAsync(v.epoch, 0xFF, v.slots * sizeof(uint32_t), st));
     v.id_bits = id_bits;
+    v.staged = staged;
   }
   c.tables = v.tab;
   c.epochs = v.epoch;
   c.cap = (uint32_t)v.cap;
   c.shift = 32 - ilog2(v.cap);
+  c.small = staged ? (uint32_t)visited_first_stage(v.cap) : 0u;
+  c.small_shift = staged ? 32 - ilog2(c.small) : c.shift;
   c.id_bits = id_bits;
   return 0;
+}
+
+// Whether a search launch of `slots` warp slots with full stages of `cap` entries starts its searches in a first stage.
+// A first stage is filled to 3/4 before a search moves, where linear probing takes several probe rounds per 32-id chunk
+// instead of about one, and a move costs a re-insert on the search's own path.  Auto mode therefore asks for both:
+//   * the full-size tables would not fit in L2 (else the stage only adds probes: c1, 1 000 slots x 16 KB, was 44 % slower
+//     staged);
+//   * the first stage holds at least 2/5 of the sizing estimate `need` = 2 (ef + 16) degree, so that a typical search
+//     stays in it (searches insert about 1/5 of the estimate: 1 048 of 5 120 at c2).  The power-of-two rounding of cap
+//     decides it.  H100 SXM 80 GB, 700 W, bench.py, staged vs one stage: c2 (first stage 2 048 = 0.40 of 5 120, 91 MB of
+//     tables) +9 %; c3 (4 096 = 0.30 of 13 824, 181 MB) -15 %; c4 (8 192 = 0.30 of 27 648) -1 %.
+// Inserts keep one stage: their ef_construction searches mostly outgrow a first stage.
+bool Index::visited_staged(size_t slots, size_t cap, size_t need) const {
+  if (visited_stages_ != 0) return visited_stages_ == 1;
+  return slots * cap * sizeof(uint32_t) > l2_bytes_ && visited_first_stage(cap) * 5 >= need * 2;
 }
 
 int Index::ensure_scratch(void** p, size_t* cur, size_t need, cudaStream_t st) {
@@ -375,7 +400,7 @@ int Index::run_insert_range(size_t first, size_t count, size_t mask_off) {
   for (int attempt = 0;; ++attempt) {
     int r;
     if ((r = ensure_visited(vis_, (size_t)grid * wpb, vcap, stream_))) return r;
-    if ((r = fill_visited_cfg(vis_, p.vis, stream_))) return r;
+    if ((r = fill_visited_cfg(vis_, p.vis, false, stream_))) return r;  // inserts: one stage (see visited_staged)
     HB_CUDA(cudaMemsetAsync(d_counter_, 0, sizeof(unsigned int), stream_));
     HB_CUDA(launch_insert_search(p, metric, dtype, grid, smem, stream_, nullptr));
     int status = 0;
@@ -743,12 +768,13 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
     if (filtered) {
       // a filtered search keeps expanding until its candidate queue is empty (hnsw.rs:992-1001) and may visit the
       // whole graph: keep (visited table + candidate queue) under ~6 GB by running fewer warps when tables are big
-      const size_t per_slot = std::max(vcap, pool.cap) * 12;
+      const size_t per_slot = visited_slot_entries(std::max(vcap, pool.cap)) * 4 + std::max(vcap, pool.cap) * 8;
       const size_t max_slots = std::max<size_t>(wpb, ((size_t)6 << 30) / per_slot);
       grid = (int)std::max<size_t>(1, std::min<size_t>(grid, max_slots / wpb));
     }
     if ((r = ensure_visited(pool, (size_t)grid * per_cta, vcap, st))) return r;
-    if ((r = fill_visited_cfg(pool, p.vis, st))) return r;
+    const size_t need = (size_t)2 * (p.ef + 16) * deg;  // the sizing estimate vcap was rounded up from
+    if ((r = fill_visited_cfg(pool, p.vis, visited_staged((size_t)grid * per_cta, pool.cap, need), st))) return r;
     if (kind == QueryKernel::Filtered || kind == QueryKernel::StdTie) {  // candidate queue C: one region per warp slot
       if ((r = ensure_scratch(&c.d_cbuf, &c.d_cbuf_bytes, (size_t)grid * wpb * pool.cap * 8, st))) return r;
       p.cbuf = (uint64_t*)c.d_cbuf;

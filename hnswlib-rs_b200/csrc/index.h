@@ -261,6 +261,7 @@ class Index {
   size_t max_elements;
   bool extend_candidates = false, keep_pruned = false, searching = false;
   int link_mode = 0;      // hnsw_b200_set_link_mode: 0 back-links under the new point's level (hnsw.rs:1257), 1 per layer
+  int visited_stages_ = 0;  // hnsw_b200_set_visited_stages: 0 auto (first stage when the tables outgrow L2), 1 always, 2 never
   bool tie_std_ = false;  // hnsw_b200_set_tie_mode: equal-distance ties resolved like the reference's std BinaryHeaps (search_std.cu)
   double level_scale;  // 1/ln(M) * factor
   SplitMix64 rng{397};
@@ -386,8 +387,9 @@ class Index {
   struct VisitedPool {
     uint32_t* tab = nullptr;
     uint32_t* epoch = nullptr;
-    size_t slots = 0, cap = 0;
+    size_t slots = 0, cap = 0;  // cap: the full stage; a slot also holds a first stage (visited_first_stage)
     int id_bits = 0;
+    bool staged = false;  // the layout of the last launch: [first stage + full stage] per slot, or the full stage alone
   };
   struct SearchCtx {
     cudaStream_t stream = nullptr;
@@ -485,7 +487,8 @@ class Index {
   };
   InsertShape insert_shape() const;
   int ensure_visited(VisitedPool& v, size_t slots, size_t cap_entries, cudaStream_t st);
-  int fill_visited_cfg(VisitedPool& v, VisitedCfg& c, cudaStream_t st);
+  int fill_visited_cfg(VisitedPool& v, VisitedCfg& c, bool staged, cudaStream_t st);
+  bool visited_staged(size_t slots, size_t cap, size_t need) const;
   int ensure_scratch(void** p, size_t* cur, size_t need, cudaStream_t st);
   int ensure_pinned(void** p, size_t* cur, size_t need, unsigned int flags);
   int grow_plevel(uint32_t id, int new_plevel);
@@ -528,6 +531,7 @@ class Index {
   mutable std::mutex err_mu_;
   cudaStream_t stream_ = nullptr, own_stream_ = nullptr;
   int sm_count_ = 0;
+  size_t l2_bytes_ = 0;
 
   GraphStore graph_;
 

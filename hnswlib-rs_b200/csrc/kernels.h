@@ -15,10 +15,20 @@ constexpr int SEARCH_THREADS = 256;  // 8 warps = 8 queries in flight per CTA
 constexpr int BUILD_THREADS = 128;   // 4 warps = 4 inserts in flight per CTA
 constexpr int LEAN_THREADS = 32;      // lean kernel (search_lean.cuh): one warp per CTA, so that a finished query frees its slot at once
 constexpr size_t SMEM_BUDGET = 220 * 1024;  // dynamic shared memory one CTA may ask for (an H100 SM offers 227 KB)
-// 20 one-warp CTAs per SM, <= 96 registers per thread, no spills.  H100 SXM 80 GB at a 400 W power limit, c2 workload, one
-// launch of 100 000 queries: 25.8 ms at 20, 26.7 at 24, 28.3 at 28 (72 registers, spills), 32.4 at 32 (64 registers); 16
-// (100 registers) took 26.5 ms against 25.8 at 20 in a separate run.
+// 20 one-warp CTAs per SM, <= 96 registers per thread, no spills.  With two-stage visited tables, H100 SXM 80 GB at a 700 W
+// power limit, bench.py c2, one run each: 4.60 M queries/s at 20 (96 registers, 0 spill bytes; one launch of 100 000
+// queries 22.0 ms), 4.74 M at 24 (80 registers, 26 bytes spilled; 21.6 ms), 4.59 M at 28 (72 registers, 70 bytes spilled;
+// 22.8 ms).  24 is not taken: it spills in the production kernel.  (The sweep with full-size tables, 400 W: 25.8 ms at 20,
+// 26.7 at 24, 28.3 at 28, 32.4 at 32.)
 constexpr int LEAN_MIN_BLOCKS = 20;
+
+// Visited tables (Visited, common.cuh): a search starts in a first stage of cap / VISITED_FIRST_DIV entries and moves to
+// the full stage of `cap` entries when the first one is 3/4 full.  H100 SXM 80 GB, 700 W, bench.py c2 (cap = 8 192): 4.35 M
+// queries/s at cap / 8 (65-74 % of queries move), 4.60 M at cap / 4 (7-10 % move), 4.54 M at cap / 2 (none moves); 4.21 M
+// with one full-size table per slot.
+constexpr int VISITED_FIRST_DIV = 4;
+inline size_t visited_first_stage(size_t cap) { return cap / VISITED_FIRST_DIV; }
+inline size_t visited_slot_entries(size_t cap) { return cap + visited_first_stage(cap); }
 
 // One answer slot.  Same 16-byte layout as the reference's #[repr(C)] Neighbour_api {id: usize, d: f32}
 // (/root/reference/src/libext.rs:64-71); the internal id rides in what is tail padding there.

@@ -37,6 +37,7 @@ int Partitions::create(Index* parent, int nparts, const int* devices) {
     ix->link_mode = parent->link_mode;
     ix->searching = parent->searching;
     ix->tie_std_ = parent->tie_std_;
+    ix->visited_stages_ = parent->visited_stages_;
     ix->level_scale = parent->level_scale;
     ix->batch_ratio = parent->batch_ratio;
     ix->batch_max = parent->batch_max;

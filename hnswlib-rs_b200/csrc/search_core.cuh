@@ -102,7 +102,7 @@ __device__ __forceinline__ void search_layer(const GraphView& g, const WarpSmem&
       }
       if (valid != FULL) break;  // lists are dense prefixes terminated by INVALID_ID
     }
-    if (vis.overflowing(vc)) {
+    if (vis.grow_or_overflow(vc, lane)) {
       overflow = true;
       break;
     }

@@ -282,7 +282,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
             int pcap;
             const uint32_t* pids = list_ids(G, pre_c, p.layer0, pcap);
             pre_nid = (lane < pcap) ? pids[lane] : INVALID_ID;
-            pre_h = Visited::home(p.vis, pre_nid);
+            pre_h = vis.home(pre_nid);
             pre_cv = 0;
             if (pre_nid != INVALID_ID) pre_cv = ld_keep(vis.tab + pre_h, l2_policy_evict_last());
             pre_ok = true;
@@ -307,7 +307,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
         }
         if (last) break;  // lists are dense prefixes terminated by INVALID_ID
       }
-      if (vis.overflowing(p.vis)) {
+      if (vis.grow_or_overflow(p.vis, lane, pre_ok)) {
         overflow = true;
         break;
       }

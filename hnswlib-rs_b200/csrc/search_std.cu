@@ -194,7 +194,7 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_std_kernel(SearchParams
           }
           if (valid != FULL) break;
         }
-        overflow = __shfl_sync(FULL, (int)overflow, 0) != 0 || vis.overflowing(p.vis);
+        overflow = __shfl_sync(FULL, (int)overflow, 0) != 0 || vis.grow_or_overflow(p.vis, lane);
         if (overflow) break;
       }
       if (lane == 0) {

@@ -75,7 +75,7 @@ def load_library():
     L.hnsw_b200_free_neighbourhood.argtypes = [vp]
     L.hnsw_b200_free_vec_api.argtypes = [vp]
     for name in ("set_extend_candidates", "set_keeping_pruned", "set_searching_mode", "enable_stats", "set_tie_mode",
-                 "set_link_mode"):
+                 "set_link_mode", "set_visited_stages"):
         getattr(L, "hnsw_b200_" + name).argtypes = [vp, i32]
     L.hnsw_b200_get_extend_candidates.argtypes = [vp]
     L.hnsw_b200_get_link_mode.argtypes = [vp]
@@ -570,6 +570,11 @@ class Hnsw:
     # ---- statistics / graph transfer (extensions)
     def enable_stats(self, on=True):
         self._chk(self._L.hnsw_b200_enable_stats(self._h, int(on)))
+
+    def set_visited_stages(self, mode):
+        """visited tables of searches: 0 auto (a first stage when the full-size tables outgrow L2), 1 always, 2 never
+        (hnsw_b200_set_visited_stages)"""
+        self._chk(self._L.hnsw_b200_set_visited_stages(self._h, int(mode)))
 
     def set_tie_mode(self, mode):
         """0: ties by (distance, id); 1: the reference's std-BinaryHeap tie behaviour (hnsw_b200_set_tie_mode)"""

@@ -226,6 +226,11 @@ int hnsw_b200_set_searching_mode(void* h, int flag);     /* hnsw.rs:834 */
  * (Ord = distance only, /root/reference/src/hnsw.rs:273-297, 940-1053, 1544) replayed literally: same neighbour ids as the
  * reference on tie-heavy metrics (Hamming, Jaccard, integer L1), several times slower (one lane drives the heaps). */
 int hnsw_b200_set_tie_mode(void* h, int mode);
+/* Visited tables of searches.  Each search's table can start in a first stage of a quarter of the full size and move to the
+ * full table once it is 3/4 full.  0 (default): only when the launch's full-size tables would not fit in the device's L2
+ * (large batches with large ef * M) and a typical search fits in the first stage (DESIGN.md §4.2); 1: always; 2: never.  Answers and traversal
+ * counters are the same in every mode; only speed differs.  Inserts always use one stage. */
+int hnsw_b200_set_visited_stages(void* h, int mode);
 /* Which layer an insert files its back-links in.  0 (default): the reference's rule, every back-link of a new point x goes
  * to the neighbour's list of x's OWN level (the reference's src/hnsw.rs:1257), so a point of level >= 1 gets no layer-0
  * in-links from its own insert; bit-identical to the reference's graph.  1: the per-layer rule of Malkov & Yashunin
