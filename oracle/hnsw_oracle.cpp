@@ -23,6 +23,10 @@
 //   FilterT for sorted Vec<usize> / closures /root/reference/src/filter.rs:7-24
 //   parallel_insert (racy, per-point locks) /root/reference/src/hnsw.rs:1224-1238
 //
+// It also restates the engine's own insert rule where it departs from the reference (Index::insert_batched, see its
+// comment): batch-synchronous inserts, each batch searching the graph as it stood when the batch began, and link mode 1
+// (back-links filed in the layer they were made in).  Serial mode-1 builds are restated by tests/linkgraph.py instead.
+//
 // Two comparison modes:
 //   MODE_STD : items compare by distance only, queues are Rust-std BinaryHeaps (rheap.h) —
 //              the literal reference behaviour incl. its tie handling.
@@ -209,10 +213,12 @@ class Index {
     }
   };
 
+  // `mask` (batched inserts): bit l says whether layer l counts as non-empty for this search, in place of layer_count_
   Heap search_layer(const T* q, uint32_t ep, size_t ef, int layer, const Filter* filter, Scratch& sc,
-                    bool locked) {
+                    bool locked, const uint16_t* mask = nullptr) {
     Heap W(ItemCmp{mode, false});
-    if (layer_count_[layer].load(std::memory_order_acquire) == 0) return W;  // 942-946
+    const bool empty = mask ? !((*mask >> layer) & 1u) : layer_count_[layer].load(std::memory_order_acquire) == 0;
+    if (empty) return W;  // 942-946
     // (947-950: negative rank cannot happen for a stored point)
     sc.begin(size());
     float d0 = dist(q, vec(ep));  // 952
@@ -430,8 +436,9 @@ class Index {
       std::sort(v.begin(), v.end(), [](const Edge& a, const Edge& b) { return a.d < b.d || (a.d == b.d && a.id < b.id); });
   }
 
-  // reverse_update_neighborhood_simple, hnsw.rs:1241-1289
-  void reverse_update(uint32_t np, bool locked) {
+  // reverse_update_neighborhood_simple, hnsw.rs:1241-1289.  link_mode1: each back-link goes to the layer it was made in
+  // (the engine's link mode 1, csrc/build.cu insert_link_kernel) instead of the new point's level.
+  void reverse_update(uint32_t np, bool locked, bool link_mode1 = false) {
     Node& nn = node(np);
     int level = nn.level;
     for (int l = level; l >= 0; --l) {  // 1248
@@ -443,7 +450,7 @@ class Index {
         if (q.id == np) continue;   // 1250
         Node& qn = node(q.id);
         if (locked) qn.lk.lock();
-        int l_n = level;  // 1257: the NEW point's level, not l
+        int l_n = link_mode1 ? l : level;  // 1257: the NEW point's level, not l
         std::vector<Edge>& tgt = qn.nb[l_n];
         bool already = false;
         for (const Edge& o : tgt) if (o.id == np) { already = true; break; }  // 1258-1267
@@ -463,21 +470,32 @@ class Index {
   void insert(const T* v, uint64_t origin, int level, Scratch& sc, bool locked) {
     size_t point_rank;
     uint32_t np = new_point(v, origin, level, &point_rank);
-    Node& nn = node(np);
     int64_t ep64 = entry();
     if (ep64 >= 0 && point_rank == 1) return;  // 1096-1102
     if (ep64 < 0) { check_entry_point(np); return; }  // 1106-1109
-    uint32_t ep = (uint32_t)ep64;
+    insert_search(np, (uint32_t)ep64, sc, locked, nullptr, false);
+    reverse_update(np, locked);  // 1210
+    check_entry_point(np);       // 1212
+  }
+
+  // The part of insert_slice between generate_new_point and reverse_update (hnsw.rs:1103-1205): descent from `ep`, then
+  // search and selection per layer, writing the stored point np's own lists.  `mask` as in search_layer; link_mode1
+  // drops the descent's push into np's lists above its level (1140-1144), as the engine's link mode 1 does.
+  void insert_search(uint32_t np, uint32_t ep, Scratch& sc, bool locked, const uint16_t* mask, bool link_mode1) {
+    Node& nn = node(np);
+    const T* v = vec(np);
+    const int level = nn.level;
     int max_level_observed = node(ep).level;  // 1103
     float dist_to_entry = dist(v, vec(ep));   // 1110-1112
     sc.evals++;
     for (int l = max_level_observed; l >= level + 1; --l) {  // 1114
-      Heap sp = search_layer(v, ep, 1, l, nullptr, sc, locked);
+      Heap sp = search_layer(v, ep, 1, l, nullptr, sc, locked, mask);
       if (sp.size() > 1) { fprintf(stderr, "oracle: search_layer(ef=1) returned %zu\n", sp.size()); abort(); }  // 1128
       if (!sp.empty()) {
         Item r = sp.pop();
         if (locked) nn.lk.lock();
-        if (nn.nb[l].size() < (size_t)(uint8_t)M_) nn.nb[l].push_back(Edge{r.id, r.kd});  // 1140-1144 (list ABOVE level)
+        if (!link_mode1 && nn.nb[l].size() < (size_t)(uint8_t)M_)
+          nn.nb[l].push_back(Edge{r.id, r.kd});  // 1140-1144 (list ABOVE level)
         if (locked) nn.lk.unlock();
         float t = dist(v, vec(r.id));  // 1146
         sc.evals++;
@@ -486,7 +504,7 @@ class Index {
     }
     std::vector<Edge> sel;
     for (int l = level; l >= 0; --l) {  // 1158
-      Heap sp = search_layer(v, ep, (size_t)ef_c_, l, nullptr, sc, locked);  // 1161
+      Heap sp = search_layer(v, ep, (size_t)ef_c_, l, nullptr, sc, locked, mask);  // 1161
       // from_positive_binaryheap_to_negative_binary_heap, 1664-1681: iterate in heap-vector order
       Heap neg(ItemCmp{mode, true});
       for (const Item& p : sp.items()) neg.push(Item{-p.kd, p.id});
@@ -501,8 +519,80 @@ class Index {
         if (!sel.empty()) ep = sel[0].id;  // 1201-1203
       }
     }
-    reverse_update(np, locked);  // 1210
-    check_entry_point(np);       // 1212
+  }
+
+  // The engine's batched insert (csrc/index.cu Index::insert_batch, csrc/build.cu), restated: the points go in as the
+  // batches sizes[0..nbatches) that partition [0, n).  Per batch:
+  //   * store every point in order (new_point); point i's layer mask is taken right after its own new_point: layer l
+  //     counts as non-empty iff a point of level l was stored up to and including i (Index::insert_batch's masks[i]);
+  //   * phase A (insert_search) for every point against the graph as it stood when the batch began: no list names a
+  //     point of the batch yet, so the phase is read-only on other points' lists and runs on nthreads threads;
+  //   * phase B (reverse_update) for every point, in insertion order, or in a permutation drawn from order_seed != 0;
+  //   * check_entry_point for every point.
+  // The reference instead races whole inserts on a rayon pool (hnsw.rs:1224-1238).  Batches the engine never makes are
+  // refused: a first point into an empty index that is not alone, and a batch of several points with one above the
+  // entry level (the engine cuts a batch before such a point and runs it alone).  link_mode1 as in insert_search and
+  // reverse_update.
+  void insert_batched(const T* vs, const uint64_t* ids, const int* levels, size_t n, const uint64_t* sizes,
+                      size_t nbatches, int nthreads, bool link_mode1, uint64_t order_seed) {
+    size_t done = 0;
+    for (size_t b = 0; b < nbatches; ++b) {
+      const size_t cnt = (size_t)sizes[b];
+      if (cnt == 0 || done + cnt > n) {
+        fprintf(stderr, "oracle: insert_batched: batch %zu of %zu points does not fit the %zu points left\n", b, cnt, n - done);
+        abort();
+      }
+      const int64_t e = entry();
+      if (e < 0 && cnt != 1) {
+        fprintf(stderr, "oracle: insert_batched: the first point into an empty index must be alone in its batch\n");
+        abort();
+      }
+      if (e >= 0 && cnt > 1)
+        for (size_t i = done; i < done + cnt; ++i)
+          if (levels[i] > node((uint32_t)e).level) {
+            fprintf(stderr, "oracle: insert_batched: point %zu of level %d shares batch %zu above the entry level %d\n", i,
+                    levels[i], b, (int)node((uint32_t)e).level);
+            abort();
+          }
+      std::vector<uint32_t> pts(cnt);
+      std::vector<uint16_t> masks(cnt);
+      for (size_t i = 0; i < cnt; ++i) {
+        size_t r;
+        pts[i] = new_point(vs + (done + i) * (size_t)dim_, ids[done + i], levels[done + i], &r);
+        uint16_t m = 0;
+        for (int l = 0; l < NB_LAYER_MAX; ++l)
+          if (layer_count_[l].load() > 0) m |= (uint16_t)(1u << l);
+        masks[i] = m;
+      }
+      if (e >= 0) {
+        std::atomic<size_t> next{0};
+        auto work = [&]() {
+          Scratch sc;
+          for (size_t i; (i = next.fetch_add(1)) < cnt;) insert_search(pts[i], (uint32_t)e, sc, false, &masks[i], link_mode1);
+          flush(sc, 0);
+        };
+        const size_t nth = std::min<size_t>((size_t)std::max(nthreads, 1), cnt);
+        if (nth <= 1) {
+          work();
+        } else {
+          std::vector<std::thread> th;
+          for (size_t t = 0; t < nth; ++t) th.emplace_back(work);
+          for (auto& t : th) t.join();
+        }
+        std::vector<uint32_t> order(pts);
+        if (order_seed) {  // Fisher-Yates over splitmix64
+          SplitMix g{order_seed};
+          for (size_t i = cnt; i > 1; --i) std::swap(order[i - 1], order[g.next() % i]);
+        }
+        for (uint32_t p : order) reverse_update(p, false, link_mode1);
+      }
+      for (uint32_t p : pts) check_entry_point(p);
+      done += cnt;
+    }
+    if (done != n) {
+      fprintf(stderr, "oracle: insert_batched: the batches hold %zu of %zu points\n", done, n);
+      abort();
+    }
   }
 
   // parallel_insert: rayon par_iter of insert (hnsw.rs:1224-1238).  Levels are drawn up front in
@@ -694,6 +784,17 @@ void oracle_insert_batch(void* hv, const void* vs, const uint64_t* ids, const in
     typedef typename std::remove_const<CT>::type T;
     if (levels) ix->insert_batch_levels((const T*)vs, ids, (const int*)levels, n, nthreads);
     else ix->insert_batch((const T*)vs, ids, n, nthreads);
+  });
+}
+
+// the engine's batch-synchronous insert (Index::insert_batched): sizes[0..nbatches) partition the n points; link_mode
+// 0 or 1; order_seed != 0 links each batch's points in a random order (the graph must not depend on it)
+void oracle_insert_batched(void* hv, const void* vs, const uint64_t* ids, const int32_t* levels, uint64_t n,
+                           const uint64_t* sizes, uint64_t nbatches, int nthreads, int link_mode, uint64_t order_seed) {
+  OracleHandle* h = (OracleHandle*)hv;
+  DISPATCH(h, {
+    typedef typename std::remove_const<typename std::remove_pointer<decltype(ix->vec(0))>::type>::type T;
+    ix->insert_batched((const T*)vs, ids, (const int*)levels, n, sizes, nbatches, nthreads, link_mode != 0, order_seed);
   });
 }
 

@@ -49,6 +49,7 @@ def lib():
         L.oracle_entry.restype = i64
         L.oracle_entry.argtypes = [vp]
         L.oracle_insert_batch.argtypes = [vp, vp, vp, vp, u64, i32]
+        L.oracle_insert_batched.argtypes = [vp, vp, vp, vp, u64, vp, u64, i32, i32, u64]
         L.oracle_draw_levels.argtypes = [vp, vp, u64]
         L.oracle_search_batch.argtypes = [vp, vp, u64, u64, u64, i32, vp, u64, FILTER_FN, vp, i32, vp, vp, vp, vp, vp]
         L.oracle_counters.argtypes = [vp, vp, i32]
@@ -166,6 +167,22 @@ class Oracle:
         ids = np.ascontiguousarray(ids, np.uint64)
         lv = None if levels is None else np.ascontiguousarray(levels, np.int32)
         self.L.oracle_insert_batch(self.h, _p(vecs), _p(ids), _p(lv), n, int(nthreads))
+
+    def insert_batched(self, vecs, ids=None, levels=None, *, batches, nthreads=1, link_mode=0, order_seed=0):
+        """The engine's batch-synchronous insert (hnsw_oracle.cpp Index::insert_batched): `batches` are the sizes of
+        consecutive batches covering all of vecs (tests/batched.py engine_batches gives the engine's own).  The graph and
+        the counters do not depend on nthreads or order_seed."""
+        vecs = np.ascontiguousarray(vecs, dtype=self.dtype).reshape(-1, self.dim)
+        n = vecs.shape[0]
+        if ids is None:
+            ids = np.arange(len(self), len(self) + n)
+        ids = np.ascontiguousarray(ids, np.uint64)
+        lv = self.draw_levels(n) if levels is None else np.ascontiguousarray(levels, np.int32)
+        sizes = np.ascontiguousarray(batches, np.uint64)
+        if len(ids) != n or len(lv) != n or int(sizes.sum()) != n or (len(sizes) and int(sizes.min()) == 0):
+            raise ValueError("insert_batched: ids, levels and the batch sizes must cover the points exactly")
+        self.L.oracle_insert_batched(self.h, _p(vecs), _p(ids), _p(lv), n, _p(sizes), len(sizes), int(nthreads),
+                                     int(link_mode), int(order_seed))
 
     def search_batch(self, queries, k, ef, filter_ids=None, filter_fn=None, nthreads=1):
         """Returns (origin_ids[nq,k] u64, dists[nq,k] f32, internal[nq,k] u32, pid[nq,k,2] i32, counts[nq])."""

@@ -1,7 +1,8 @@
-"""Full-size checks at BASELINE.json configs[1] (1 000 000 x 128 f32 L2, M=16, ef_c=200, 10 000 queries, ef=64): the oracle
-cannot run this size in seconds, so the engine is checked through size-independent properties (sortedness, idempotence,
-self-retrieval, permutation invariance, agreement with the exact brute-force kernel) plus an oracle spot-check of a
-query sample on the SAME graph (exported from the GPU, imported into the oracle)."""
+"""Full-size checks at BASELINE.json configs[1] (1 000 000 x 128 f32 L2, M=16, ef_c=200, 10 000 queries, ef=64): the
+searches are checked through size-independent properties (sortedness, idempotence, self-retrieval, permutation
+invariance, agreement with the exact brute-force kernel) plus an oracle spot-check of a query sample on the SAME graph
+(exported from the GPU, imported into the oracle).  The graph itself is compared with the oracle's batch-synchronous
+build of the same points and levels in tests/test_gpu_batched_insert.py::test_c2_full_size_equals_batched_oracle."""
 import numpy as np
 import pytest
 
