@@ -278,8 +278,8 @@ static bool exact_shape(int d4, size_t k, size_t nq, ExactParams& p, size_t& sme
   return false;
 }
 
-int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const ExactScan& scan, NeighbourOut* d_out,
-                        int32_t* d_counts, bool sync, float* kernel_ms, const std::vector<ExactGroup>* groups) {
+int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const std::vector<ExactGroup>& groups,
+                        NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms) {
   if (k == 0) return fail("knbn must be positive");
   if (poisoned_) return fail(poison_msg_);
   cudaStream_t st = c.stream;
@@ -288,6 +288,9 @@ int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k
     if (sync) HB_CUDA(cudaStreamSynchronize(st));
     return 0;
   }
+  // one group over every row: equal tiles over its points, taken from blockIdx (no tile table); else a tile table
+  const bool tiled = !(groups.size() == 1 && groups[0].first == 0 && groups[0].count == nq);
+  const ExactScan scan = tiled ? ExactScan() : groups[0].scan;
   ExactParams p{};
   p.g = view();
   p.queries = d_queries;
@@ -296,11 +299,8 @@ int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k
   p.list = scan.ids;
   p.npts = (uint32_t)(scan.ids ? scan.n : n);
   p.k = (int)k;
-  size_t widest_group = nq;
-  if (groups) {
-    widest_group = 0;
-    for (const ExactGroup& gr : *groups) widest_group = std::max(widest_group, gr.count);
-  }
+  size_t widest_group = 0;
+  for (const ExactGroup& gr : groups) widest_group = std::max(widest_group, gr.count);
   size_t smem = 0;
   if (!exact_shape(p.g.d4, k, widest_group, p, smem)) return fail("k / dimension too large for the exact search kernel");
   auto launch = [&](int grid, int* blocks_per_sm) {
@@ -308,17 +308,17 @@ int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k
       return launch_exact_for_op<typename decltype(tag)::type>(p, grid, smem, st, blocks_per_sm);
     });
   };
-  // groups: tiles of up to tq rows of one group each, every tile over its group's points
+  // tiled: tiles of up to tq rows of one group each, every tile over its group's points
   std::vector<ExactTile> tl;
-  if (groups)
-    for (const ExactGroup& gr : *groups)
+  if (tiled)
+    for (const ExactGroup& gr : groups)
       for (size_t q = 0; q < gr.count; q += p.tq)
         tl.push_back(ExactTile{(uint32_t)(gr.first + q), (uint32_t)std::min<size_t>(p.tq, gr.count - q), gr.scan.ids,
                                (uint32_t)(gr.scan.ids ? gr.scan.n : n)});
-  const size_t tiles = groups ? tl.size() : (nq + p.tq - 1) / p.tq;
+  const size_t tiles = tiled ? tl.size() : (nq + p.tq - 1) / p.tq;
   if (tiles == 0) return 0;
   double mean = p.npts, widest = p.npts;  // points a tile scans: on average, and at most
-  if (groups) {
+  if (tiled) {
     mean = widest = 0;
     for (const ExactTile& t : tl) {
       mean += t.npts;
@@ -355,7 +355,7 @@ int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k
     int r;
     if ((r = ensure_scratch(&c.d_xpart, &c.d_xpart_bytes, tile_bytes + tick_bytes + part_bytes, st))) return r;
   }
-  if (groups) {
+  if (tiled) {
     p.tiles = (const ExactTile*)c.d_xpart;
     HB_CUDA(cudaMemcpyAsync(c.d_xpart, tl.data(), tl.size() * sizeof(ExactTile), cudaMemcpyHostToDevice, st));
   }

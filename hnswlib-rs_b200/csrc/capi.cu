@@ -15,7 +15,7 @@
 using hb::Index;
 using hb::NeighbourOut;
 using hb::AnswerArrays;
-using hb::FilterArg;
+using hb::Restriction;
 using hb::HostBatch;
 
 // every typed handle of libext.rs (HnswApif32, HnswApii32, HnswApiu32, HnswApiu16, HnswApiu8) has this layout
@@ -162,7 +162,7 @@ static const Neighbourhood_api* search_any(const void* hv, size_t len, const voi
   Neighbour_api* nb = (Neighbour_api*)malloc(sizeof(Neighbour_api) * knbn);
   int32_t cnt = 0;
   const AnswerArrays ans{(NeighbourOut*)nb, nullptr, nullptr, nullptr, nullptr, &cnt};
-  if (pass(h->ix, h->ix->search_batch(HostBatch{data, nullptr, 1, (int)len, knbn, ef_search, FilterArg(), ans}))) {
+  if (pass(h->ix, h->ix->search_batch(HostBatch{data, nullptr, 1, (int)len, knbn, ef_search, Restriction(), ans}))) {
     free(nb);
     return nullptr;
   }
@@ -193,7 +193,7 @@ static const Vec_api_Neighbourhood_api* parallel_search_any(const void* hv, size
   std::vector<int32_t> cnt(nb_vec);
   const AnswerArrays out{(NeighbourOut*)box->block, nullptr, nullptr, nullptr, nullptr, cnt.data()};
   // with replicas, every device answers its slice of the batch in place
-  if (pass(h->ix, h->ix->search_batch(HostBatch{nullptr, data, nb_vec, (int)vec_len, knbn, ef_search, FilterArg(), out}))) {
+  if (pass(h->ix, h->ix->search_batch(HostBatch{nullptr, data, nb_vec, (int)vec_len, knbn, ef_search, Restriction(), out}))) {
     free(box->hoods);
     free(box->block);
     free(box);
@@ -598,61 +598,80 @@ int hnsw_b200_insert_flat(void* h, const void* vecs, uint64_t n, uint64_t dim, c
   return pass(ix, ix->insert_batch(vecs, n, dim, nullptr, ids, levels));
 }
 
-// hnsw_b200_search_flat and _search_flat_filtered: the filter is the FilterT arguments (filter_mode 1, 2) or, when
-// `resident` is set, one of the handle's resident filters (filter_mode 0).  The kernels and the answers are the same.
-static int search_flat_any(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
-                           int filter_mode, const uint64_t* filter_ids, uint64_t nfilter, hnsw_b200_filter_fn fn, void* ctx,
-                           const int64_t* resident, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
-                           int32_t* out_pid, int32_t* out_counts) {
+// ---- searches.  Every search entry point below is one call of search_call, which takes the handle's lock shared (and
+// every partition's), checks the arguments and runs the batch:
+//   * HOST: host queries in, host answers out (`out`), through the host batch driver; a partitioned handle searches
+//     every partition;
+//   * SUBMIT: the same, split in two (hnsw_b200_search_flat_wait collects it), so that one host thread keeps several
+//     batches in flight.  With replicas (hnsw_b200_replicate) every device gets its contiguous share enqueued at submit
+//     time.  Refused on a partitioned handle;
+//   * DEVICE: device queries in, device answers out (out.nb, out.counts), `sync` and `kernel_ms` as
+//     hnsw_b200_search_device takes them.  Refused on a partitioned handle.
+// `name` is the entry point a refusal on a partitioned handle names.  `rs` is what each query may return, `exact` the
+// exact scan of those points instead of the graph search (ef unused).
+enum Via { HOST, SUBMIT, DEVICE };
+static int64_t search_call(const void* h, Via via, const char* name, const Restriction& rs, bool exact, const void* queries,
+                           uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef, const AnswerArrays& out, int sync = 1,
+                           float* kernel_ms = nullptr) {
   HB_HS(h);
-  if (nq == 0) return 0;
-  if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0) return set_err("bad argument");
+  if (via != HOST) HB_NOT_PARTITIONED(ix, name);
+  if (via == DEVICE)
+    return pass(ix, ix->search_device(rs, exact, queries, nq, knbn, ef, out.nb, out.counts, sync != 0, kernel_ms));
+  if (via == HOST && nq == 0) return 0;
+  if (rs.kind == Restriction::ROW_FILTERS && !rs.filters) return set_err("filters is NULL");
+  if (rs.kind == Restriction::ROW_LABELS && !rs.labels) return set_err("qlabels is NULL");
+  if (!queries || !out.ids || !out.dist || !out.counts || knbn == 0 || nq == 0) return set_err("bad argument");
   HB_PARTS_SHARED_IF(ix);
-  const FilterArg f{filter_mode, filter_ids, nfilter, fn, ctx, resident};
-  const AnswerArrays out{nullptr, out_ids, out_dist, out_internal, out_pid, out_counts};
-  return pass(ix, ix->search_batch(HostBatch{queries, nullptr, nq, (int)dim, knbn, ef_search, f, out}));
+  HostBatch b{queries, nullptr, nq, (int)dim, knbn, ef, rs, out};
+  b.exact = exact;
+  if (via == HOST) return pass(ix, ix->search_batch(b));
+  const int64_t t = ix->submit_batch(b);
+  if (t < 0) g_err = ix->err();
+  return t;
+}
+static AnswerArrays columns(uint64_t* ids, float* dist, uint32_t* internal, int32_t* pid, int32_t* counts) {
+  return AnswerArrays{nullptr, ids, dist, internal, pid, counts};
+}
+static AnswerArrays on_device(void* d_out, int32_t* d_counts) {
+  return AnswerArrays{(NeighbourOut*)d_out, nullptr, nullptr, nullptr, nullptr, d_counts};
+}
+static Restriction filter_t(int mode, const uint64_t* ids, uint64_t nids, hnsw_b200_filter_fn fn, void* ctx) {
+  return mode ? Restriction{Restriction::FILTER_T, mode, ids, nids, fn, ctx} : Restriction();
+}
+static Restriction resident(int64_t f) { return {Restriction::RESIDENT, 0, nullptr, 0, nullptr, nullptr, f}; }
+static Restriction resident_or_all(int64_t f) { return f == -1 ? Restriction() : resident(f); }  // -1: every point
+static Restriction row_filters(const int64_t* f) { return {Restriction::ROW_FILTERS, 0, nullptr, 0, nullptr, nullptr, -1, f}; }
+static Restriction row_labels(const uint32_t* l) {
+  return {Restriction::ROW_LABELS, 0, nullptr, 0, nullptr, nullptr, -1, nullptr, l};
 }
 
+// hnsw_b200_search_flat and _search_flat_filtered: the filter is the FilterT arguments (filter_mode 1, 2) or one of the
+// handle's resident filters.  The kernels and the answers are the same.
 int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
                           uint64_t ef_search, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,
                           hnsw_b200_filter_fn fn, void* ctx, uint64_t* out_ids, float* out_dist,
                           uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return search_flat_any(h, queries, nq, dim, knbn, ef_search, filter_mode, filter_ids, nfilter, fn, ctx, nullptr, out_ids,
-                         out_dist, out_internal, out_pid, out_counts);
+  return (int)search_call(h, HOST, "search_flat", filter_t(filter_mode, filter_ids, nfilter, fn, ctx), false, queries, nq,
+                          dim, knbn, ef_search, columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 int hnsw_b200_search_flat_filtered(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim,
                                    uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                    uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return search_flat_any(h, queries, nq, dim, knbn, ef_search, 0, nullptr, 0, nullptr, nullptr, &filter, out_ids, out_dist,
-                         out_internal, out_pid, out_counts);
-}
-
-// Submit / wait: the same search with the call split in two, so that one host thread keeps several batches in flight
-// (batch i+1 is enqueued before batch i's answers are collected).  Unfiltered, or with a resident filter.  With replicas
-// (hnsw_b200_replicate) the batch is sharded like a search_flat call: every device gets its contiguous share enqueued at
-// submit time.
-static int64_t submit_any(const void* h, const int64_t* resident, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
-                          uint64_t ef_search, uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
-                          int32_t* out_counts) {
-  HB_HS(h);
-  HB_NOT_PARTITIONED(ix, resident ? "search_flat_submit_filtered" : "search_flat_submit");
-  if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0 || nq == 0) return set_err("bad argument");
-  const FilterArg f{0, nullptr, 0, nullptr, nullptr, resident};
-  const AnswerArrays out{nullptr, out_ids, out_dist, out_internal, out_pid, out_counts};
-  const int64_t t = ix->submit_batch(HostBatch{queries, nullptr, nq, (int)dim, knbn, ef_search, f, out});
-  if (t < 0) g_err = ix->err();
-  return t;
+  return (int)search_call(h, HOST, "search_flat_filtered", resident(filter), false, queries, nq, dim, knbn, ef_search,
+                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 
 int64_t hnsw_b200_search_flat_submit(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
                                      uint64_t ef_search, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                      int32_t* out_pid, int32_t* out_counts) {
-  return submit_any(h, nullptr, queries, nq, dim, knbn, ef_search, out_ids, out_dist, out_internal, out_pid, out_counts);
+  return search_call(h, SUBMIT, "search_flat_submit", Restriction(), false, queries, nq, dim, knbn, ef_search,
+                     columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 int64_t hnsw_b200_search_flat_submit_filtered(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim,
                                               uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                               uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return submit_any(h, &filter, queries, nq, dim, knbn, ef_search, out_ids, out_dist, out_internal, out_pid, out_counts);
+  return search_call(h, SUBMIT, "search_flat_submit_filtered", resident(filter), false, queries, nq, dim, knbn, ef_search,
+                     columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 
 int hnsw_b200_search_flat_wait(const void* h, int64_t ticket) {
@@ -666,64 +685,38 @@ int hnsw_b200_search_flat_wait(const void* h, int64_t ticket) {
   return r;
 }
 
-static int search_device_any(const void* h, const int64_t* resident, const void* d_queries, uint64_t nq, uint64_t knbn,
-                             uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
-  HB_HS(h);
-  HB_NOT_PARTITIONED(ix, resident ? "search_device_filtered" : "search_device");
-  const FilterArg f{0, nullptr, 0, nullptr, nullptr, resident};
-  return pass(ix, ix->search_device(f, false, d_queries, nq, knbn, ef_search, (NeighbourOut*)d_out, d_counts, sync != 0,
-                                    kernel_ms));
-}
 int hnsw_b200_search_device(const void* h, const void* d_queries, uint64_t nq, uint64_t knbn,
                             uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
-  return search_device_any(h, nullptr, d_queries, nq, knbn, ef_search, d_out, d_counts, sync, kernel_ms);
+  return (int)search_call(h, DEVICE, "search_device", Restriction(), false, d_queries, nq, 0, knbn, ef_search,
+                          on_device(d_out, d_counts), sync, kernel_ms);
 }
 int hnsw_b200_search_device_filtered(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                      uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
-  return search_device_any(h, &filter, d_queries, nq, knbn, ef_search, d_out, d_counts, sync, kernel_ms);
+  return (int)search_call(h, DEVICE, "search_device_filtered", resident(filter), false, d_queries, nq, 0, knbn, ef_search,
+                          on_device(d_out, d_counts), sync, kernel_ms);
 }
 
 // Exact search: the exact scan of the points a resident filter admits (filter >= 0) or of every point (-1), through the
 // same batch driver and device-resident path as the graph searches
 int hnsw_b200_search_exact(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
                            uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  HB_HS(h);
-  if (nq == 0) return 0;
-  if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0) return set_err("bad argument");
-  HB_PARTS_SHARED_IF(ix);
-  FilterArg f;
-  if (filter != -1) f.resident = &filter;
-  HostBatch b{queries, nullptr, nq, (int)dim, knbn, 0, f, AnswerArrays{nullptr, out_ids, out_dist, out_internal, out_pid, out_counts}};
-  b.exact = true;
-  return pass(ix, ix->search_batch(b));
+  return (int)search_call(h, HOST, "search_exact", resident_or_all(filter), true, queries, nq, dim, knbn, 0,
+                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 
 // A filter per query: filters[i] is a resident filter of the handle or -1; the graph search (ef_search) or the exact
-// scan (exact).  One batch, every entry checked before anything runs.
-static int per_query_any(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
-                         uint64_t ef_search, bool exact, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
-                         int32_t* out_pid, int32_t* out_counts) {
-  HB_HS(h);
-  if (nq == 0) return 0;
-  if (!filters) return set_err("filters is NULL");
-  if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0) return set_err("bad argument");
-  HB_PARTS_SHARED_IF(ix);
-  HostBatch b{queries, nullptr, nq, (int)dim, knbn, ef_search, FilterArg(),
-              AnswerArrays{nullptr, out_ids, out_dist, out_internal, out_pid, out_counts}};
-  b.exact = exact;
-  b.per_query = filters;
-  return pass(ix, ix->search_batch(b));
-}
+// scan.  One batch, every entry checked before anything runs.
 int hnsw_b200_search_flat_per_query(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim,
                                     uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                     uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return per_query_any(h, filters, queries, nq, dim, knbn, ef_search, false, out_ids, out_dist, out_internal, out_pid,
-                       out_counts);
+  return (int)search_call(h, HOST, "search_flat_per_query", row_filters(filters), false, queries, nq, dim, knbn, ef_search,
+                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 int hnsw_b200_search_exact_per_query(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim,
                                      uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                      int32_t* out_pid, int32_t* out_counts) {
-  return per_query_any(h, filters, queries, nq, dim, knbn, 0, true, out_ids, out_dist, out_internal, out_pid, out_counts);
+  return (int)search_call(h, HOST, "search_exact_per_query", row_filters(filters), true, queries, nq, dim, knbn, 0,
+                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 
 // Point labels.  On a partitioned handle point g (its insertion rank) is local point g / P of partition g % P.
@@ -781,40 +774,24 @@ int hnsw_b200_get_labels(const void* h, uint64_t first, uint64_t n, uint32_t* ou
 }
 
 // A label per query: labels[i] is the label query i is restricted to, or LABEL_NONE for none; the graph search
-// (ef_search) or the exact scan (exact).
-static int labeled_any(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
-                       uint64_t ef_search, bool exact, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
-                       int32_t* out_pid, int32_t* out_counts) {
-  HB_HS(h);
-  if (nq == 0) return 0;
-  if (!qlabels) return set_err("qlabels is NULL");
-  if (!queries || !out_ids || !out_dist || !out_counts || knbn == 0) return set_err("bad argument");
-  HB_PARTS_SHARED_IF(ix);
-  HostBatch b{queries, nullptr, nq, (int)dim, knbn, ef_search, FilterArg(),
-              AnswerArrays{nullptr, out_ids, out_dist, out_internal, out_pid, out_counts}};
-  b.exact = exact;
-  b.labels = qlabels;
-  return pass(ix, ix->search_batch(b));
-}
+// (ef_search) or the exact scan.
 int hnsw_b200_search_flat_labeled(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim,
                                   uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                   uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return labeled_any(h, qlabels, queries, nq, dim, knbn, ef_search, false, out_ids, out_dist, out_internal, out_pid,
-                     out_counts);
+  return (int)search_call(h, HOST, "search_flat_labeled", row_labels(qlabels), false, queries, nq, dim, knbn, ef_search,
+                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 int hnsw_b200_search_exact_labeled(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim,
                                    uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                    int32_t* out_pid, int32_t* out_counts) {
-  return labeled_any(h, qlabels, queries, nq, dim, knbn, 0, true, out_ids, out_dist, out_internal, out_pid, out_counts);
+  return (int)search_call(h, HOST, "search_exact_labeled", row_labels(qlabels), true, queries, nq, dim, knbn, 0,
+                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 
 int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                   void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
-  HB_HS(h);
-  HB_NOT_PARTITIONED(ix, "search_exact_device");
-  FilterArg f;
-  if (filter != -1) f.resident = &filter;
-  return pass(ix, ix->search_device(f, true, d_queries, nq, knbn, 0, (NeighbourOut*)d_out, d_counts, sync != 0, kernel_ms));
+  return (int)search_call(h, DEVICE, "search_exact_device", resident_or_all(filter), true, d_queries, nq, 0, knbn, 0,
+                          on_device(d_out, d_counts), sync, kernel_ms);
 }
 
 int64_t hnsw_b200_filter_new(const void* h, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,

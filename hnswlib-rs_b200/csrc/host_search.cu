@@ -182,41 +182,80 @@ int Index::plan(size_t nq, std::vector<Leg>& legs) {
   return 0;
 }
 
-int Index::resolve_filter(const FilterArg& f, bool exact, Leg* legs, size_t n, std::vector<std::vector<uint32_t>>& bits) {
+int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>& sorted, Leg* legs, size_t n,
+                   std::vector<std::vector<uint32_t>>& bits) {
   const int P = parts ? parts->count() : 1;
-  int r = 0;
-  if (f.mode) {
+  if (rs.kind == Restriction::FILTER_T) {
     bits.resize(P);
     for (int p = 0; p < P; ++p) {
       Index* rx = parts ? parts->part(p) : this;
-      if (rx->make_filter_bits(f.mode, f.ids, f.nids, f.fn, f.ctx, bits[p])) {
+      if (rx->make_filter_bits(rs.mode, rs.ids, rs.nids, rs.fn, rs.ctx, bits[p])) {
         for (Leg* l = legs; l < legs + n; ++l)
           if (l->rx == rx) l->rc = -1;
         return -1;
       }
     }
-    for (size_t i = 0; i < n; ++i) legs[i].host_bits = bits[legs[i].part].data();
   }
-  for (Leg* l = legs; f.resident && l < legs + n; ++l)  // every leg, so that the caller reports the failure it chooses
-    if (filters.use(*f.resident, l->part, P, l->rx, &l->dev_bits, exact ? &l->scan : nullptr)) r = l->rc = -1;
+  // run u of leg l under `key`, a resident filter or a label
+  auto restrict_run = [&](const Leg& l, int64_t key, LegPlan::Run& u) {
+    if (rs.kind == Restriction::FILTER_T) {
+      u.host_bits = bits[l.part].data();
+      return 0;
+    }
+    if (rs.kind != Restriction::ROW_LABELS) return filters.use(key, l.part, P, l.rx, &u.bits, exact ? &u.scan : nullptr);
+    u.label = (uint32_t)key;
+    return exact ? l.rx->label_scan(u.label, &u.scan) : 0;
+  };
+  int r = 0;
+  for (Leg* l = legs; l < legs + n; ++l) {  // every leg, so that the caller reports the failure it chooses
+    LegPlan& pl = l->plan;
+    pl.exact = exact;
+    if (!rs.per_row()) {  // every row unrestricted, or one run over every row
+      LegPlan::Run u{0, l->count};
+      if (rs.kind == Restriction::NONE)
+        pl.plain = l->count;
+      else if (restrict_run(*l, rs.resident, u))
+        r = l->rc = -1;
+      else
+        pl.runs.push_back(u);
+      continue;
+    }
+    const int64_t* key = sorted.data() + l->first;
+    while (pl.plain < l->count && key[pl.plain] == -1) ++pl.plain;
+    // labels: the leg's own, or on a replica its copy of the handle's, made current first
+    if (rs.kind == Restriction::ROW_LABELS && pl.plain < l->count &&
+        l->rx->labels_on_device(parts ? l->rx : this, &pl.labels)) {
+      r = l->rc = -1;
+      continue;
+    }
+    for (size_t j = pl.plain, e; j < l->count; j = e) {  // one run per filter or label
+      for (e = j + 1; e < l->count && key[e] == key[j];) ++e;
+      LegPlan::Run u{j, e - j};
+      if (restrict_run(*l, key[j], u)) {
+        r = l->rc = -1;
+        break;
+      }
+      pl.runs.push_back(u);
+    }
+  }
   return r;
 }
 
 // Every filter is checked on every partition before anything runs, so that a bad entry refuses the whole call, named by
 // its first position.  The sort is stable: rows of one filter keep their order, and -1 (no filter) sorts first.  A label
 // needs no check; LABEL_NONE sorts first as -1.
-int Index::sort_per_query(const HostBatch& b, std::vector<size_t>& perm, std::vector<int64_t>& sorted) {
+int Index::sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm, std::vector<int64_t>& sorted) {
   const int P = parts ? parts->count() : 1;
-  const size_t nq = b.nq;
+  const bool labels = rs.kind == Restriction::ROW_LABELS;
   std::vector<int64_t> key;
-  const int64_t* fid = b.per_query;
-  if (b.labels) {
+  const int64_t* fid = rs.filters;
+  if (labels) {
     key.resize(nq);
-    for (size_t i = 0; i < nq; ++i) key[i] = b.labels[i] == LABEL_NONE ? -1 : (int64_t)b.labels[i];
+    for (size_t i = 0; i < nq; ++i) key[i] = rs.labels[i] == LABEL_NONE ? -1 : (int64_t)rs.labels[i];
     fid = key.data();
   }
   std::set<int64_t> checked;
-  for (size_t i = 0; !b.labels && i < nq; ++i) {
+  for (size_t i = 0; !labels && i < nq; ++i) {
     if (fid[i] == -1 || checked.count(fid[i])) continue;
     for (int p = 0; p < P; ++p) {
       Index* rx = parts ? parts->part(p) : this;
@@ -232,49 +271,6 @@ int Index::sort_per_query(const HostBatch& b, std::vector<size_t>& perm, std::ve
   sorted.resize(nq);
   for (size_t j = 0; j < nq; ++j) sorted[j] = fid[perm[j]];
   return 0;
-}
-
-int Index::resolve_per_query(const std::vector<int64_t>& sorted, bool labels, bool exact, Leg* legs, size_t n) {
-  const int P = parts ? parts->count() : 1;
-  int r = 0;
-  for (Leg* l = legs; l < legs + n; ++l) {  // every leg, so that the caller reports the failure it chooses
-    LegFilters& q = l->pq;
-    const int64_t* f = sorted.data() + l->first;
-    q.on = true;
-    while (q.plain < l->count && f[q.plain] == -1) ++q.plain;
-    // labels: the leg's own, or on a replica its copy of the handle's, made current first.  The graph search reads the
-    // label array and each row's label; the exact scan, a slice per label of the leg's CSR.
-    if (labels && q.plain < l->count && l->rx->labels_on_device(parts ? l->rx : this, &q.labels)) {
-      r = l->rc = -1;
-      continue;
-    }
-    if (exact && q.plain) q.groups.push_back(ExactGroup{0, q.plain, ExactScan()});
-    for (size_t j = q.plain, e; j < l->count; j = e) {  // one run of rows per filter or label
-      for (e = j + 1; e < l->count && f[e] == f[j];) ++e;
-      ExactScan s;
-      const uint32_t* bits = nullptr;
-      if (labels) {
-        if (!exact) {
-          q.sel.insert(q.sel.end(), e - j, (uint32_t)f[j]);
-          continue;
-        }
-        if (l->rx->label_scan((uint32_t)f[j], &s)) {
-          r = l->rc = -1;
-          break;
-        }
-      } else if (filters.use(f[j], l->part, P, l->rx, &bits, exact ? &s : nullptr)) {
-        r = l->rc = -1;
-        break;
-      }
-      if (exact) {
-        q.groups.push_back(ExactGroup{j, e - j, s});
-      } else {
-        q.sel.insert(q.sel.end(), e - j, (uint32_t)q.table.size());
-        q.table.push_back(bits);
-      }
-    }
-  }
-  return r;
 }
 
 // The handle's error for the first failed leg of legs[0, n) (0 if none failed): in leg order, or the replicas' before the
@@ -293,8 +289,7 @@ int Index::legs_fail(const Leg* legs, size_t n, bool replicas_first) {
 void Index::begin_leg(const HostBatch& b, Leg& l) {
   if (l.ctx < 0) l.ctx = l.rx->acquire_ctx();
   const void* q = b.rows ? nullptr : (const char*)b.queries + l.first * (size_t)b.d * es;
-  l.rc = l.rx->search_host_begin(l.ctx, q, b.rows ? b.rows + l.first : nullptr, l.count, b.d, b.k, b.ef, l.host_bits,
-                                 l.dev_bits, b.exact ? &l.scan : nullptr, l.pq.on ? &l.pq : nullptr);
+  l.rc = l.rx->search_host_begin(l.ctx, q, b.rows ? b.rows + l.first : nullptr, l.count, b.d, b.k, b.ef, l.plan);
   l.begun = l.rc == 0;
 }
 
@@ -321,33 +316,39 @@ int Index::end_leg(Leg& l, size_t k, const AnswerArrays& out) {
 }
 
 // ------------------------------------------------------------------------------------------------ batches
-int Index::search_batch(const HostBatch& call) {
-  if (call.nq == 0) return 0;
+// The batch `call` planned into t's legs, each with its plan; `b` is the batch as the legs run it.  A per-row restriction:
+// the batch is planned over the rows sorted by filter or label, gathered through row pointers, and each answer goes back
+// to its caller's row.  A leg that could not have its plan is reported in leg order, or the replicas' first.
+int Index::prepare_batch(const HostBatch& call, HostBatch& b, Ticket& t, bool replicas_first) {
   if (parts && dim != 0 && call.d != dim) return fail("query length differs from the index dimension");
   int r;
-  // a filter or a label per query: the batch is planned over the rows sorted by filter or label, gathered through row
-  // pointers, and each answer goes back to its caller's row
-  HostBatch b = call;
-  std::vector<size_t> perm;
-  std::vector<const void*> rows;
+  b = call;
   std::vector<int64_t> sorted;
-  const bool per_row = call.per_query || call.labels;
-  if (per_row) {
-    if ((r = sort_per_query(call, perm, sorted))) return r;
-    rows.resize(call.nq);
+  if (call.restriction.per_row()) {
+    if ((r = sort_rows(call.restriction, call.nq, t.perm, sorted))) return r;
+    t.rows.resize(call.nq);
     for (size_t j = 0; j < call.nq; ++j)
-      rows[j] = call.rows ? call.rows[perm[j]] : (const char*)call.queries + perm[j] * (size_t)call.d * es;
-    b.rows = rows.data();
-    b.out.perm = perm.data();
+      t.rows[j] = call.rows ? call.rows[t.perm[j]] : (const char*)call.queries + t.perm[j] * (size_t)call.d * es;
+    b.rows = t.rows.data();
+    b.out.perm = t.perm.data();
   }
-  std::vector<Leg> legs;
-  std::vector<std::vector<uint32_t>> bits;
-  if ((r = plan(b.nq, legs))) return r;
+  t.k = b.k;
+  t.out = b.out;
+  if ((r = plan(b.nq, t.legs))) return r;
+  if (resolve(b.restriction, b.exact, sorted, t.legs.data(), t.legs.size(), t.bits))
+    return legs_fail(t.legs.data(), t.legs.size(), replicas_first && !parts);
+  return 0;
+}
+
+int Index::search_batch(const HostBatch& call) {
+  if (call.nq == 0) return 0;
+  HostBatch b;
+  Ticket t;
+  int r;
+  if ((r = prepare_batch(call, b, t, true))) return r;
+  std::vector<Leg>& legs = t.legs;
   const int n = (int)legs.size();
   const bool sharded = n > 1 && !parts;
-  if (per_row ? resolve_per_query(sorted, b.labels != nullptr, b.exact, legs.data(), n)
-              : resolve_filter(b.filter, b.exact, legs.data(), n, bits))
-    return legs_fail(legs.data(), n, sharded);
   if (n == 1 && !parts) {
     begin_leg(b, legs[0]);
     return end_leg(legs[0], b.k, b.out);
@@ -379,15 +380,12 @@ int Index::search_batch(const HostBatch& call) {
   return bad < 0 ? 0 : legs_fail(&legs[bad], 1, false);
 }
 
-int64_t Index::submit_batch(const HostBatch& b) {
+int64_t Index::submit_batch(const HostBatch& call) {
   DeviceRestore keep;  // the legs switch to their devices on the calling thread
+  HostBatch b;
   Ticket t;
-  t.k = b.k;
-  t.out = b.out;
-  std::vector<std::vector<uint32_t>> bits;
   int r;
-  if ((r = plan(b.nq, t.legs))) return r;
-  if (resolve_filter(b.filter, b.exact, t.legs.data(), t.legs.size(), bits)) return legs_fail(t.legs.data(), t.legs.size(), false);
+  if ((r = prepare_batch(call, b, t, false))) return r;
   int bad = -1;
   for (size_t i = 0; i < t.legs.size() && bad < 0; ++i) {  // one after the other, on the calling thread
     begin_leg(b, t.legs[i]);

@@ -643,18 +643,18 @@ void Index::release_ctx(int c) {
 // context streams, so that two consecutive launches overlap.  The handle's stream does NOT wait for it: join() (or
 // check_status, set_stream, any synchronous call's own synchronisation) makes it do so; stream_wait_last() makes any
 // stream wait for the most recent launch alone.  The same for the exact scan (`exact`).
-int Index::search_device(const FilterArg& f, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef_arg,
+int Index::search_device(const Restriction& rs, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef_arg,
                          NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms) {
-  Leg leg{this};
+  Leg leg{this, 0, 0, nq};
   std::vector<std::vector<uint32_t>> bits;
   int r;
-  if (resolve_filter(f, exact, &leg, 1, bits)) return legs_fail(&leg, 1, false);
-  const uint32_t* d_filter_bits = leg.dev_bits;
+  if (resolve(rs, exact, {}, &leg, 1, bits)) return legs_fail(&leg, 1, false);
   if (nq == 0) return 0;
   HB_CUDA(cudaSetDevice(device));
   auto run = [&](SearchCtx& c, bool s, float* ms) {
-    return exact ? exact_on_ctx(c, d_queries, nq, k, leg.scan, d_out, d_counts, s, ms)
-                 : search_on_ctx(c, d_queries, nq, k, ef_arg, d_filter_bits, d_out, d_counts, s, ms);
+    SearchCtx::Launch L{d_queries, nq, k, ef_arg, d_out, d_counts, false, 0, {}, {}};
+    const int e = stage_plan(c, leg.plan, L);
+    return e ? e : run_plan(c, L, s, ms);
   };
   if (sync) {
     CtxLease lease(this);
@@ -693,9 +693,8 @@ int Index::stream_wait_last(cudaStream_t s) {
   return 0;
 }
 
-int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const uint32_t* d_filter_bits,
-                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint32_t* const* d_ftab,
-                         const uint32_t* d_fsel, const uint32_t* d_labels) {
+int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const LaunchFilter& f,
+                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms) {
   if (k == 0) return fail("knbn must be positive");
   if (poisoned_) return fail(poison_msg_);
   cudaStream_t st = c.stream;
@@ -719,13 +718,13 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.work_counter = c.d_counter;
   p.out_nb = d_out;
   p.out_count = d_counts;
-  p.filter_bits = d_filter_bits;
-  p.filter_table = d_ftab;
-  p.filter_sel = d_fsel;
-  p.labels = d_labels;
+  p.filter_bits = f.bits;
+  p.filter_table = f.table;
+  p.filter_sel = f.sel;
+  p.labels = f.labels;
   p.stats = stats_on_ ? d_stats_ : nullptr;
   p.status = c.d_status;
-  const bool filtered = d_filter_bits != nullptr || d_fsel != nullptr;
+  const bool filtered = f.bits != nullptr || f.sel != nullptr;
   QueryKernel kind = QueryKernel::Generic;
   if (filtered) kind = QueryKernel::Filtered;
   else if (tie_std_) kind = QueryKernel::StdTie;  // unfiltered searches only
@@ -818,8 +817,7 @@ static const void* device_view_of_host(const void* p) {
 // synchronisation.  Pageable queries and row pointers are gathered into the context's own pinned staging buffer first
 // (the only host-side copy), which the kernel then reads the same way.
 int Index::search_host_begin(int ci, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                             const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const ExactScan* scan,
-                             const LegFilters* pq) {
+                             const LegPlan& plan) {
   SearchCtx& c = ctx_[ci];
   cudaStream_t st = c.stream;
   c.pend = SearchCtx::Pending();
@@ -832,12 +830,13 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
   NeighbourOut* hout = (NeighbourOut*)c.h_res;
   int32_t* hcnt = (int32_t*)((char*)c.h_res + out_bytes);
   int32_t* hstatus = hcnt + nq;
+  SearchCtx::Launch& L = c.pend.run;
   c.pend.hout = hout;
   c.pend.hcnt = hcnt;
   c.pend.hstatus = hstatus;
-  c.pend.nq = nq;
-  c.pend.k = k;
-  c.pend.ef = ef;
+  L.nq = nq;
+  L.k = k;
+  L.ef = ef;
   if (dim == 0) {  // empty index: every answer is empty (hnsw.rs:1498-1500)
     for (size_t i = 0; i < nq; ++i) hcnt[i] = 0;
     for (size_t i = 0; i < nq * k; ++i) hout[i] = NeighbourOut{~0ull, __builtin_inff(), INVALID_ID};
@@ -858,55 +857,21 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
   }
   char* dv = (char*)device_view_of_host(c.h_res);  // where the kernel writes
   if (!dv) return fail("the pinned result buffer has no device address");
-  NeighbourOut* k_out = (NeighbourOut*)dv;
-  int32_t* k_cnt = (int32_t*)(dv + out_bytes);
-  if (scan) {
+  L.d_queries = d_queries;
+  L.out = (NeighbourOut*)dv;
+  L.counts = (int32_t*)(dv + out_bytes);
+  if (plan.exact) {
     // an exact launch may run many CTAs per query (row slices): the queries cross the bus once, into device memory
     if ((r = ensure_scratch(&c.d_xq, &c.d_xq_bytes, qbytes, st))) return r;
     HB_CUDA(cudaMemcpyAsync(c.d_xq, d_queries, qbytes, cudaMemcpyDefault, st));
+    L.d_queries = c.d_xq;
     *hstatus = 0;
-    c.pend.exact = true;
-    c.pend.enqueued = true;
-    return exact_on_ctx(c, c.d_xq, nq, k, *scan, k_out, k_cnt, false, nullptr, pq && pq->on ? &pq->groups : nullptr);
   }
-  if (pq && pq->on) {
-    // a filter per query: the bitmap table and the filtered rows' entries go to the device ahead of the launches (a
-    // label per query: the labelled rows' labels; the label array is already there)
-    const size_t tb = round128(pq->table.size() * sizeof(void*)), sb = pq->sel.size() * sizeof(uint32_t);
-    if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, tb + sb, st))) return r;
-    if (sb) {
-      if (tb) HB_CUDA(cudaMemcpyAsync(c.d_fbits, pq->table.data(), pq->table.size() * sizeof(void*), cudaMemcpyHostToDevice, st));
-      HB_CUDA(cudaMemcpyAsync((char*)c.d_fbits + tb, pq->sel.data(), sb, cudaMemcpyHostToDevice, st));
-    }
-    c.pend.per_query = true;
-    c.pend.plain = pq->plain;
-    c.pend.ftab = (const uint32_t* const*)c.d_fbits;
-    c.pend.fsel = (const uint32_t*)((char*)c.d_fbits + tb);
-    c.pend.labels = pq->labels;
-    c.pend.d_queries = d_queries;
-    c.pend.k_out = k_out;
-    c.pend.k_cnt = k_cnt;
-    c.pend.enqueued = true;
-    if ((r = per_query_on_ctx(c, false))) return r;
-    HB_CUDA(cudaMemcpyAsync(hstatus, c.d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-    return 0;
-  }
-  const uint32_t* dfb = d_filter_bits;  // a resident filter: already on this device
-  if (filter_bits_host) {
-    const size_t fb = ((n + 31) / 32) * 4;
-    if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, fb, st))) return r;
-    HB_CUDA(cudaMemcpyAsync(c.d_fbits, filter_bits_host, fb, cudaMemcpyHostToDevice, st));
-    dfb = (const uint32_t*)c.d_fbits;
-  }
-  // one enqueue (filter bits if any, kernel, status); search_host_finish synchronises once and takes the slow path (a
-  // visited table overflowed: grow and re-run) only when the status says so
-  c.pend.d_queries = d_queries;
-  c.pend.dfb = dfb;
-  c.pend.k_out = k_out;
-  c.pend.k_cnt = k_cnt;
+  // one enqueue (the plan's uploads, the launches, the status); search_host_finish synchronises once and takes the slow
+  // path (a visited table overflowed: grow and re-run) only when the status says so
   c.pend.enqueued = true;
-  if ((r = search_on_ctx(c, d_queries, nq, k, ef, dfb, k_out, k_cnt, false, nullptr))) return r;
-  HB_CUDA(cudaMemcpyAsync(hstatus, c.d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if ((r = stage_plan(c, plan, L)) || (r = run_plan(c, L, false, nullptr))) return r;
+  if (!plan.exact) HB_CUDA(cudaMemcpyAsync(hstatus, c.d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   return 0;
 }
 
@@ -919,23 +884,60 @@ int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** 
   if (!p.enqueued) return 0;  // empty batch or empty index: the answers (if any) were filled by search_host_begin
   HB_CUDA(cudaSetDevice(device));
   HB_CUDA(cudaStreamSynchronize(st));
-  if (p.exact || *p.hstatus == 0) return 0;
+  if (p.run.exact || *p.hstatus == 0) return 0;  // an exact scan has no status and nothing to re-run
   HB_CUDA(cudaMemsetAsync(c.d_status, 0, sizeof(int), st));
-  if (p.per_query) return per_query_on_ctx(c, true);
-  return search_on_ctx(c, p.d_queries, p.nq, p.k, p.ef, p.dfb, p.k_out, p.k_cnt, true, nullptr);  // grows the tables
+  return run_plan(c, p.run, true, nullptr);  // grows the tables
 }
 
-// the rows without a filter as an ordinary unfiltered launch, then every filtered row in one filtered launch on the
-// bitmap table or the label array; both share the context's status, so an overflow in either re-runs both (sync:
-// growing the tables)
-int Index::per_query_on_ctx(SearchCtx& c, bool sync) {
-  const SearchCtx::Pending& p = c.pend;
+// A single bitmap run goes to the launch as its filter bits (a FilterT's host bits uploaded into the context first), as
+// a batch-wide filter does; several as a table of their bitmaps and each row's entry in it, and label runs as the label
+// array and each row's label, uploaded into the context ahead of the launches.  Exact: a group of every point for the
+// unrestricted rows, and one per run.
+int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
+  cudaStream_t st = c.stream;
   int r;
-  if (p.plain && (r = search_on_ctx(c, p.d_queries, p.plain, p.k, p.ef, nullptr, p.k_out, p.k_cnt, sync, nullptr))) return r;
-  if (p.nq == p.plain) return 0;
-  const char* fq = (const char*)p.d_queries + p.plain * (size_t)dim * es;
-  return search_on_ctx(c, fq, p.nq - p.plain, p.k, p.ef, nullptr, p.k_out + p.plain * p.k, p.k_cnt + p.plain, sync, nullptr,
-                       p.labels ? nullptr : p.ftab, p.fsel, p.labels);
+  L.exact = plan.exact;
+  L.plain = plan.plain;
+  if (plan.exact) {
+    if (plan.plain) L.groups.push_back(ExactGroup{0, plan.plain, ExactScan()});
+    for (const LegPlan::Run& u : plan.runs) L.groups.push_back(ExactGroup{u.first, u.count, u.scan});
+    return 0;
+  }
+  if (plan.runs.empty()) return 0;
+  if (plan.runs.size() == 1 && !plan.labels) {
+    L.filter.bits = plan.runs[0].bits;  // a resident filter: already on this device
+    if (plan.runs[0].host_bits) {
+      const size_t fb = ((n + 31) / 32) * 4;
+      if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, fb, st))) return r;
+      HB_CUDA(cudaMemcpyAsync(c.d_fbits, plan.runs[0].host_bits, fb, cudaMemcpyHostToDevice, st));
+      L.filter.bits = (const uint32_t*)c.d_fbits;
+    }
+    return 0;
+  }
+  std::vector<const uint32_t*> table;
+  std::vector<uint32_t> sel;
+  for (const LegPlan::Run& u : plan.runs) {
+    sel.insert(sel.end(), u.count, plan.labels ? u.label : (uint32_t)table.size());
+    if (!plan.labels) table.push_back(u.bits);
+  }
+  const size_t tb = round128(table.size() * sizeof(void*)), sb = sel.size() * sizeof(uint32_t);
+  if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, tb + sb, st))) return r;
+  if (tb) HB_CUDA(cudaMemcpyAsync(c.d_fbits, table.data(), table.size() * sizeof(void*), cudaMemcpyHostToDevice, st));
+  HB_CUDA(cudaMemcpyAsync((char*)c.d_fbits + tb, sel.data(), sb, cudaMemcpyHostToDevice, st));
+  L.filter.table = plan.labels ? nullptr : (const uint32_t* const*)c.d_fbits;
+  L.filter.sel = (const uint32_t*)((char*)c.d_fbits + tb);
+  L.filter.labels = plan.labels;
+  return 0;
+}
+
+int Index::run_plan(SearchCtx& c, const SearchCtx::Launch& L, bool sync, float* kernel_ms) {
+  if (L.exact) return exact_on_ctx(c, L.d_queries, L.nq, L.k, L.groups, L.out, L.counts, sync, kernel_ms);
+  int r;
+  if (L.plain && (r = search_on_ctx(c, L.d_queries, L.plain, L.k, L.ef, LaunchFilter(), L.out, L.counts, sync, kernel_ms)))
+    return r;
+  if (L.plain == L.nq) return 0;
+  const char* q = (const char*)L.d_queries + L.plain * (size_t)dim * es;
+  return search_on_ctx(c, q, L.nq - L.plain, L.k, L.ef, L.filter, L.out + L.plain * L.k, L.counts + L.plain, sync, kernel_ms);
 }
 
 int Index::make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx,

@@ -113,10 +113,19 @@ struct ExactScan {
   size_t n = 0;
 };
 
-// rows [first, first + count) of an exact launch with a filter per query, all scanning the same points
+// rows [first, first + count) of an exact launch, all scanning the same points
 struct ExactGroup {
   size_t first, count;
   ExactScan scan;
+};
+
+// The restriction of one search launch, as SearchParams reads it: none, one bitmap for every row (bits), a bitmap per row
+// (row i on table[sel[i]]), or a label per row (row i on the points whose `labels` entry is sel[i])
+struct LaunchFilter {
+  const uint32_t* bits = nullptr;
+  const uint32_t* const* table = nullptr;
+  const uint32_t* sel = nullptr;
+  const uint32_t* labels = nullptr;
 };
 
 // Resident filters (hnsw_b200_filter_new, filter_store.cu): a FilterT materialised once per handle, as one bitmap per
@@ -196,58 +205,63 @@ struct AnswerArrays {
   const size_t* perm = nullptr;  // row j of the batch is written to row perm[j] (nullptr: to row j)
 };
 
-// The filter of a search: none, a FilterT (mode != 0, as make_filter_bits reads it: 1 sorted origin-id list, 2 callback),
-// or one of the handle's resident filters (the id *resident).
-struct FilterArg {
+// What the rows of a batch may return: every point (NONE); the points a FilterT admits (FILTER_T: `mode` 1 sorted
+// origin-id list, 2 callback, as make_filter_bits reads it); one resident filter for every row (RESIDENT); a resident
+// filter per row, -1 = none (ROW_FILTERS); or a label per row, LABEL_NONE = none (ROW_LABELS)
+struct Restriction {
+  enum Kind { NONE, FILTER_T, RESIDENT, ROW_FILTERS, ROW_LABELS } kind = NONE;
   int mode = 0;
   const uint64_t* ids = nullptr;
   size_t nids = 0;
   int (*fn)(uint64_t, void*) = nullptr;
   void* ctx = nullptr;
-  const int64_t* resident = nullptr;
+  int64_t resident = -1;
+  const int64_t* filters = nullptr;  // [nq]
+  const uint32_t* labels = nullptr;  // [nq]
+  bool per_row() const { return kind == ROW_FILTERS || kind == ROW_LABELS; }
 };
 
 // One host search batch: flat queries or one pointer per query (rows), k answers each into `out`.  `exact`: the exact
-// scan of the points the filter admits (ef unused) instead of the graph search.
+// scan of the points each row may return (ef unused) instead of the graph search.
 struct HostBatch {
   const void* queries = nullptr;
   const void* const* rows = nullptr;
   size_t nq = 0;
   int d = 0;
   size_t k = 0, ef = 0;
-  FilterArg filter;
+  Restriction restriction;
   AnswerArrays out;
   bool exact = false;
-  const int64_t* per_query = nullptr;  // [nq]: each query's resident filter, or -1 for none (then `filter` is unused)
-  const uint32_t* labels = nullptr;    // [nq]: each query's label, or LABEL_NONE for none (then `filter` is unused)
 };
 
-// A leg's share of a batch with a filter or a label per query, whose rows the driver sorted by filter or label
-// (resolve_per_query): the leg's first `plain` rows have neither.  Graph search: its row plain + i uses bitmap
-// table[sel[i]], or with `labels` (the label array on the leg's device) the points labelled sel[i].  Exact scan:
-// `groups`, its rows by the points they scan (every point for the plain rows).
-struct LegFilters {
-  bool on = false;
+// A leg's restriction (Index::resolve): its rows [0, plain) are unrestricted, and `runs` cover the rest, each a range of
+// consecutive rows under one restriction.  A run is a resident filter's bitmap on the leg's device, a FilterT's host bits
+// (uploaded into the context when the leg begins), or a label on `labels` (the label array on the leg's device); in an
+// exact batch, the points it scans.  A batch-wide filter is a plan with no prefix and one run over every row.
+struct LegPlan {
+  struct Run {
+    size_t first, count;
+    const uint32_t* bits = nullptr;
+    const uint32_t* host_bits = nullptr;
+    uint32_t label = LABEL_NONE;
+    ExactScan scan;
+  };
+  bool exact = false;
   size_t plain = 0;
-  std::vector<const uint32_t*> table;
-  std::vector<uint32_t> sel;
+  std::vector<Run> runs;
   const uint32_t* labels = nullptr;
-  std::vector<ExactGroup> groups;
 };
 
 // One Index's part of a batch: queries [first, first + count) searched on rx (the handle, a replica, or partition `part`)
-// on its leased context ctx, with the filter bits resolve_filter gave it, or for an exact batch the points to scan
+// on its leased context ctx, under its plan
 struct Leg {
   Index* rx = nullptr;
   int part = 0;
   size_t first = 0, count = 0;
   int ctx = -1;  // -1: not leased
-  const uint32_t* host_bits = nullptr;
-  const uint32_t* dev_bits = nullptr;
-  ExactScan scan;
   bool begun = false;  // enqueued
   int rc = 0;
-  LegFilters pq;
+  LegPlan plan;
 };
 
 class Index {
@@ -288,20 +302,21 @@ class Index {
   int import_graph(const void* vecs, size_t n_new, int d, const uint64_t* origin, const uint8_t* levels,
                    int64_t entry_id, int nlayers, const uint64_t* const* offsets, const uint32_t* const* ids,
                    const float* const* dists);
-  // host queries (flat or row pointers) on leased context c, answers left in the context's pinned buffer (valid until
-  // it is released).  The filter is either host bits, uploaded into the context for this call, or d_filter_bits already
-  // on this device (a resident filter); at most one of the two is non-null.  With `scan`, the exact scan of those points
-  // instead of the graph search (no filter bits, ef unused).  With `pq` (pq->on; no filter bits and no scan), a filter
-  // per query.
+  // host queries (flat or row pointers) on leased context c under the leg's plan, answers left in the context's pinned
+  // buffer (valid until it is released)
   int search_host_begin(int c, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                        const uint32_t* filter_bits_host, const uint32_t* d_filter_bits, const ExactScan* scan = nullptr,
-                        const LegFilters* pq = nullptr);
+                        const LegPlan& plan);
   int search_host_finish(int c, const NeighbourOut** out, const int32_t** counts);
-  // host search batches (host_search.cu): synchronous, or submitted now and collected by finish_batch
+  // host search batches (host_search.cu): synchronous, or submitted now and collected by finish_batch.  A ticket is a
+  // batch planned into legs, with what the legs read until they are collected: a per-row batch's caller row of each
+  // sorted row (out.perm) and its sorted rows, and a FilterT's host bits per partition.
   struct Ticket {
     std::vector<Leg> legs;
     size_t k = 0;
     AnswerArrays out;
+    std::vector<size_t> perm;
+    std::vector<const void*> rows;
+    std::vector<std::vector<uint32_t>> bits;
   };
   int search_batch(const HostBatch& b);
   int64_t submit_batch(const HostBatch& b);  // a ticket id, or < 0
@@ -311,18 +326,18 @@ class Index {
   void drain_pending() const {
     while (pending_.load() != 0) std::this_thread::yield();
   }
-  // the filter bits of legs[0, n): a FilterT's host bits, made on the calling thread once per partition (a replica
-  // shares the handle's internal ids, and so its bits) into `bits`, or a resident filter's copy on each leg's device.
-  // Nonzero when a leg could not have them; that leg's rc is set (legs_fail reports it).  `exact`: each leg's ExactScan
-  // instead (the resident filter's id list on the leg's device, or every point).
-  int resolve_filter(const FilterArg& f, bool exact, Leg* legs, size_t n, std::vector<std::vector<uint32_t>>& bits);
-  // a batch with a filter per query: every entry of filters[0, nq) is -1 or a live, current filter of this handle (else
-  // the first bad position is refused), and `perm` orders the rows stably by filter, the unfiltered ones first.  A
-  // label per query (b.labels): by label, LABEL_NONE first.  sorted[j]: the filter or label of sorted row j (-1: none).
-  int sort_per_query(const HostBatch& b, std::vector<size_t>& perm, std::vector<int64_t>& sorted);
-  // each leg's LegFilters for the rows sorted by filter or label, on its partition and device; nonzero when a leg could
-  // not have them, with that leg's rc set
-  int resolve_per_query(const std::vector<int64_t>& sorted, bool labels, bool exact, Leg* legs, size_t n);
+  // the plan of each of legs[0, n) under `rs`; `sorted` holds a per-row restriction's keys (a filter id or a label, -1:
+  // none) in the order the legs run the rows (sort_rows).  A FilterT's host bits are made on the calling thread once per
+  // partition (a replica shares the handle's internal ids, and so its bits) into `bits`; a resident filter is its copy
+  // on each leg's device; a label needs the label array on the leg's device.  `exact`: each run's ExactScan (a filter's
+  // id list or a label's CSR slice on the leg's device).  Nonzero when a leg could not have its plan; that leg's rc is
+  // set (legs_fail reports it).
+  int resolve(const Restriction& rs, bool exact, const std::vector<int64_t>& sorted, Leg* legs, size_t n,
+              std::vector<std::vector<uint32_t>>& bits);
+  // a per-row restriction: every filter of rs.filters[0, nq) is -1 or a live, current filter of this handle (else the
+  // first bad position is refused), and `perm` orders the rows stably by filter, the unfiltered ones first; labels by
+  // label, LABEL_NONE first.  sorted[j]: the filter or label of sorted row j (-1: none).
+  int sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm, std::vector<int64_t>& sorted);
 
   // ---- point labels (labels.cu).  One u32 per point (GraphStore LABEL and its host mirror h_label), LABEL_NONE until
   // set_labels names one; label_version counts the calls that changed them (a replica: the handle's version it copied).
@@ -334,9 +349,10 @@ class Index {
   int labels_on_device(const Index* src, const uint32_t** d_labels);
   // the exact scan of the points labelled `label`: a slice of this Index's label CSR, rebuilt when the labels changed
   int label_scan(uint32_t label, ExactScan* scan);
-  // device queries in, device answers out; the filter is none or a resident filter.  `exact`: the exact scan (ef unused).
-  int search_device(const FilterArg& f, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef, NeighbourOut* d_out,
-                    int32_t* d_counts, bool sync, float* kernel_ms);
+  // device queries in, device answers out; the restriction is none or a resident filter.  `exact`: the exact scan (ef
+  // unused).
+  int search_device(const Restriction& rs, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef,
+                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms);
   // filter materialisation: bit per internal id from a sorted origin-id list or a callback
   int make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx,
                        std::vector<uint32_t>& bits) const;
@@ -397,27 +413,30 @@ class Index {
     unsigned int* d_counter = nullptr;
     int* d_status = nullptr;
     VisitedPool vis, fvis;  // unfiltered / filtered searches
-    void *d_fbits = nullptr, *d_cbuf = nullptr;  // the call's filter bits (or its per-query bitmap table and selectors) / C
+    void *d_fbits = nullptr, *d_cbuf = nullptr;  // the call's filter bits (or its bitmap table and selectors) / C
     size_t d_fbits_bytes = 0, d_cbuf_bytes = 0;
     void *d_xq = nullptr, *d_xpart = nullptr;  // exact scan: the host batch's queries on the device / tickets and slice lists
     size_t d_xq_bytes = 0, d_xpart_bytes = 0;
     void *h_pin = nullptr, *h_res = nullptr;  // pinned, mapped: query staging / answers
     size_t h_pin_bytes = 0, h_res_bytes = 0;
     bool busy = false;
-    struct Pending {  // a host search enqueued by search_host_begin, completed by search_host_finish
+    // The launches of one leg on the context (run_plan): device queries and answers, and the device view of the leg's
+    // plan (stage_plan).  Graph: rows [0, plain) unrestricted, the others under `filter`.  Exact: the rows by the points
+    // they scan.
+    struct Launch {
       const void* d_queries = nullptr;
-      const uint32_t* dfb = nullptr;
-      bool exact = false;  // an exact scan: no status, nothing to re-run
-      // a filter per query: rows [0, plain) unfiltered, the others on the device bitmap table / selectors; a label per
-      // query: on the device label array, fsel holding the rows' labels
-      bool per_query = false;
-      size_t plain = 0;
-      const uint32_t* const* ftab = nullptr;
-      const uint32_t* fsel = nullptr;
-      const uint32_t* labels = nullptr;
-      NeighbourOut *k_out = nullptr, *hout = nullptr;
-      int32_t *k_cnt = nullptr, *hcnt = nullptr, *hstatus = nullptr;
       size_t nq = 0, k = 0, ef = 0;
+      NeighbourOut* out = nullptr;
+      int32_t* counts = nullptr;
+      bool exact = false;
+      size_t plain = 0;
+      LaunchFilter filter;
+      std::vector<ExactGroup> groups;
+    };
+    struct Pending {  // a host search enqueued by search_host_begin, completed by search_host_finish
+      Launch run;
+      NeighbourOut* hout = nullptr;
+      int32_t *hcnt = nullptr, *hstatus = nullptr;
       bool enqueued = false;
     } pend;
   };
@@ -498,6 +517,7 @@ class Index {
 
   // ---- host search batches (host_search.cu)
   int plan(size_t nq, std::vector<Leg>& legs);
+  int prepare_batch(const HostBatch& call, HostBatch& b, Ticket& t, bool replicas_first);
   void begin_leg(const HostBatch& b, Leg& l);
   void release_leg(Leg& l);
   int end_leg(Leg& l, size_t k, const AnswerArrays& out);
@@ -537,18 +557,19 @@ class Index {
 
   VisitedPool vis_;  // visited tables of the insert kernel (searches: SearchCtx)
   SearchCtx ctx_[NCTX + NASYNC];
-  // d_ftab / d_fsel: a filter per query, query i on bitmap d_ftab[d_fsel[i]] (then d_filter_bits is null); with
-  // d_labels instead of d_ftab, a label per query: query i on the points whose d_labels entry is d_fsel[i]
-  int search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const uint32_t* d_filter_bits,
-                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms,
-                    const uint32_t* const* d_ftab = nullptr, const uint32_t* d_fsel = nullptr,
-                    const uint32_t* d_labels = nullptr);
-  // the exact k nearest of device queries among scan's points (aux.cu); the slices' scratch is sized before the launch.
-  // With `groups` (a filter per query), each group's rows among that group's points instead of scan's.
-  int exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const ExactScan& scan, NeighbourOut* d_out,
-                   int32_t* d_counts, bool sync, float* kernel_ms, const std::vector<ExactGroup>* groups = nullptr);
-  // the graph search of a per-query leg on context c: the plain rows' launch, then the filtered rows' launch
-  int per_query_on_ctx(SearchCtx& c, bool sync);
+  // one graph search launch (the filtered kernel when `f` restricts it)
+  int search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const LaunchFilter& f,
+                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms);
+  // the exact k nearest of device queries, each group's rows among that group's points (aux.cu); the slices' scratch is
+  // sized before the launch
+  int exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const std::vector<ExactGroup>& groups,
+                   NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms);
+  // the device view of a leg's plan in `run`, with what it needs uploaded into context c
+  int stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& run);
+  // the launches of `run` on context c: the unrestricted rows as an ordinary unfiltered launch, then the restricted ones
+  // in one filtered launch (exact: one launch over the groups).  Both share the context's status, so an overflow in either
+  // re-runs both (sync: growing the tables).
+  int run_plan(SearchCtx& c, const SearchCtx::Launch& run, bool sync, float* kernel_ms);
   std::mutex ctx_mu_;
   std::condition_variable ctx_cv_;
   std::mutex ticket_mu_;

@@ -403,65 +403,64 @@ class Hnsw:
 
     parallel_search_neighbours = parallel_search  # AnnT::parallel_search_neighbours
 
+    @staticmethod
+    def _answers(nq, knbn, with_internal, with_pid):
+        """fresh answer arrays of a host search: origin u64[nq,k], dist f32[nq,k], internal u32[nq,k] | None,
+        pid i32[nq,k,2] | None, counts i32[nq]"""
+        return (np.empty((nq, knbn), np.uint64), np.empty((nq, knbn), np.float32),
+                np.empty((nq, knbn), np.uint32) if with_internal else None,
+                np.empty((nq, knbn, 2), np.int32) if with_pid else None, np.empty(nq, np.int32))
+
+    def _host_search(self, fn, lead, q, knbn, mid, with_internal, with_pid):
+        """fn(handle, *lead, q, nq, d, knbn, *mid, *answer arrays) into fresh answer arrays, which it returns"""
+        ans = self._answers(q.shape[0], knbn, with_internal, with_pid)
+        self._chk(fn(self._h, *lead, _p(q), *q.shape, int(knbn), *mid, *map(_p, ans)))
+        return ans
+
+    def _filter_call(self, filter, name, resident_only=None):
+        """the C call of a filter= argument: (function, arguments ahead of the queries, FilterT arguments after ef).
+        hnsw_b200_<name> for None, hnsw_b200_<name>_filtered with the id of a ResidentFilter.  hnsw_b200_search_flat takes
+        a FilterT (a sorted id sequence or a callable) after ef, mode 0 for None; a method that takes only a
+        ResidentFilter (resident_only: its name) refuses anything else."""
+        if isinstance(filter, ResidentFilter):
+            return getattr(self._L, f"hnsw_b200_{name}_filtered"), (filter.id,), ()
+        if resident_only:
+            if filter is not None:
+                raise TypeError(f"{resident_only} takes a ResidentFilter (Hnsw.make_filter) as its filter")
+            return getattr(self._L, "hnsw_b200_" + name), (), ()
+        mode, fids, nf, cb = (0, None, 0, FILTER_FN(0)) if filter is None else _filter_args(filter)
+        return getattr(self._L, "hnsw_b200_" + name), (), (mode, _p(fids), nf, cb, None)
+
     def search_flat(self, queries, knbn, ef, filter=None, with_internal=True, with_pid=True):
         """Extension: flat batch.  Returns (origin u64[nq,k], dist f32[nq,k], internal u32[nq,k] | None,
         pid i32[nq,k,2] | None, counts).  filter: as search_filter takes it."""
         q = np.ascontiguousarray(queries, self.dtype)
-        nq, d = q.shape
-        o = np.empty((nq, knbn), np.uint64)
-        ds = np.empty((nq, knbn), np.float32)
-        it = np.empty((nq, knbn), np.uint32) if with_internal else None
-        pid = np.empty((nq, knbn, 2), np.int32) if with_pid else None
-        cnt = np.empty(nq, np.int32)
-        if isinstance(filter, ResidentFilter):
-            self._chk(self._L.hnsw_b200_search_flat_filtered(self._h, filter.id, _p(q), nq, d, int(knbn), int(ef), _p(o),
-                                                             _p(ds), _p(it), _p(pid), _p(cnt)))
-            return o, ds, it, pid, cnt
-        mode, fids, nf, cb = 0, None, 0, FILTER_FN(0)
-        if filter is not None:
-            mode, fids, nf, cb = _filter_args(filter)
-        self._chk(self._L.hnsw_b200_search_flat(self._h, _p(q), nq, d, int(knbn), int(ef), mode, _p(fids), nf, cb, None,
-                                                _p(o), _p(ds), _p(it), _p(pid), _p(cnt)))
-        return o, ds, it, pid, cnt
+        fn, lead, tail = self._filter_call(filter, "search_flat")
+        return self._host_search(fn, lead, q, knbn, (int(ef),) + tail, with_internal, with_pid)
 
     def search_exact(self, queries, knbn, filter=None, with_internal=True, with_pid=True):
         """hnsw_b200_search_exact: the exact knbn nearest among the points a ResidentFilter admits (None: every point).
         Returns search_flat's (origin, dist, internal | None, pid | None, counts)."""
         q = np.ascontiguousarray(queries, self.dtype)
-        nq, d = q.shape
-        o = np.empty((nq, knbn), np.uint64)
-        ds = np.empty((nq, knbn), np.float32)
-        it = np.empty((nq, knbn), np.uint32) if with_internal else None
-        pid = np.empty((nq, knbn, 2), np.int32) if with_pid else None
-        cnt = np.empty(nq, np.int32)
-        self._chk(self._L.hnsw_b200_search_exact(self._h, _filter_id(filter), _p(q), nq, d, int(knbn), _p(o), _p(ds), _p(it),
-                                                 _p(pid), _p(cnt)))
-        return o, ds, it, pid, cnt
-
-    def _per_query(self, fn, queries, knbn, filters, ef_args, with_internal, with_pid):
-        q = np.ascontiguousarray(queries, self.dtype)
-        nq, d = q.shape
-        fids = _filter_ids(filters, nq)
-        o = np.empty((nq, knbn), np.uint64)
-        ds = np.empty((nq, knbn), np.float32)
-        it = np.empty((nq, knbn), np.uint32) if with_internal else None
-        pid = np.empty((nq, knbn, 2), np.int32) if with_pid else None
-        cnt = np.empty(nq, np.int32)
-        self._chk(fn(self._h, _p(fids), _p(q), nq, d, int(knbn), *ef_args, _p(o), _p(ds), _p(it), _p(pid), _p(cnt)))
-        return o, ds, it, pid, cnt
+        return self._host_search(self._L.hnsw_b200_search_exact, (_filter_id(filter),), q, knbn, (), with_internal,
+                                 with_pid)
 
     def search_flat_per_query(self, queries, knbn, ef, filters, with_internal=True, with_pid=True):
         """hnsw_b200_search_flat_per_query: one batch, query i filtered by filters[i] (a ResidentFilter of this handle,
         or None for no filter).  Row i equals search_flat(queries[i:i+1], knbn, ef, filter=filters[i]).  Returns
         search_flat's (origin, dist, internal | None, pid | None, counts)."""
-        return self._per_query(self._L.hnsw_b200_search_flat_per_query, queries, knbn, filters, (int(ef),), with_internal,
-                               with_pid)
+        q = np.ascontiguousarray(queries, self.dtype)
+        fids = _filter_ids(filters, q.shape[0])
+        return self._host_search(self._L.hnsw_b200_search_flat_per_query, (_p(fids),), q, knbn, (int(ef),), with_internal,
+                                 with_pid)
 
     def search_exact_per_query(self, queries, knbn, filters, with_internal=True, with_pid=True):
         """hnsw_b200_search_exact_per_query: search_exact with query i over the points filters[i] admits (a
         ResidentFilter of this handle, or None for every point), in one batch.  Returns search_exact's tuple."""
-        return self._per_query(self._L.hnsw_b200_search_exact_per_query, queries, knbn, filters, (), with_internal,
-                               with_pid)
+        q = np.ascontiguousarray(queries, self.dtype)
+        fids = _filter_ids(filters, q.shape[0])
+        return self._host_search(self._L.hnsw_b200_search_exact_per_query, (_p(fids),), q, knbn, (), with_internal,
+                                 with_pid)
 
     def set_labels(self, first, labels):
         """hnsw_b200_set_labels: the labels of the points with insertion ranks first .. first + len(labels) - 1
@@ -476,29 +475,21 @@ class Hnsw:
         self._chk(self._L.hnsw_b200_get_labels(self._h, int(first), int(n), _p(out)))
         return out
 
-    def _labeled(self, fn, queries, knbn, labels, ef_args, with_internal, with_pid):
-        q = np.ascontiguousarray(queries, self.dtype)
-        nq, d = q.shape
-        lab = _labels(labels, nq, "labels")
-        o = np.empty((nq, knbn), np.uint64)
-        ds = np.empty((nq, knbn), np.float32)
-        it = np.empty((nq, knbn), np.uint32) if with_internal else None
-        pid = np.empty((nq, knbn, 2), np.int32) if with_pid else None
-        cnt = np.empty(nq, np.int32)
-        self._chk(fn(self._h, _p(lab), _p(q), nq, d, int(knbn), *ef_args, _p(o), _p(ds), _p(it), _p(pid), _p(cnt)))
-        return o, ds, it, pid, cnt
-
     def search_flat_labeled(self, queries, knbn, ef, labels, with_internal=True, with_pid=True):
         """hnsw_b200_search_flat_labeled: one batch, query i restricted to the points labelled labels[i] (LABEL_NONE:
         every point).  Row i equals search_flat with a resident filter admitting exactly those points.  Returns
         search_flat's (origin, dist, internal | None, pid | None, counts)."""
-        return self._labeled(self._L.hnsw_b200_search_flat_labeled, queries, knbn, labels, (int(ef),), with_internal,
-                             with_pid)
+        q = np.ascontiguousarray(queries, self.dtype)
+        lab = _labels(labels, q.shape[0], "labels")
+        return self._host_search(self._L.hnsw_b200_search_flat_labeled, (_p(lab),), q, knbn, (int(ef),), with_internal,
+                                 with_pid)
 
     def search_exact_labeled(self, queries, knbn, labels, with_internal=True, with_pid=True):
         """hnsw_b200_search_exact_labeled: the exact knbn nearest of query i among the points labelled labels[i]
         (LABEL_NONE: every point), in one batch.  Returns search_exact's tuple."""
-        return self._labeled(self._L.hnsw_b200_search_exact_labeled, queries, knbn, labels, (), with_internal, with_pid)
+        q = np.ascontiguousarray(queries, self.dtype)
+        lab = _labels(labels, q.shape[0], "labels")
+        return self._host_search(self._L.hnsw_b200_search_exact_labeled, (_p(lab),), q, knbn, (), with_internal, with_pid)
 
     def make_filter(self, filter):
         """hnsw_b200_filter_new: materialise a FilterT (sorted id sequence or callable(id)->bool, as search_flat takes)
@@ -513,23 +504,12 @@ class Hnsw:
         """hnsw_b200_search_flat_submit: enqueue a batch, return a ticket for wait_flat (up to 4 outstanding).
         filter: None or a ResidentFilter (hnsw_b200_search_flat_submit_filtered)."""
         q = np.ascontiguousarray(queries, self.dtype)
-        nq, d = q.shape
-        o = np.empty((nq, knbn), np.uint64)
-        ds = np.empty((nq, knbn), np.float32)
-        it = np.empty((nq, knbn), np.uint32) if with_internal else None
-        pid = np.empty((nq, knbn, 2), np.int32) if with_pid else None
-        cnt = np.empty(nq, np.int32)
-        if filter is None:
-            t = self._L.hnsw_b200_search_flat_submit(self._h, _p(q), nq, d, int(knbn), int(ef), _p(o), _p(ds), _p(it), _p(pid),
-                                                     _p(cnt))
-        elif isinstance(filter, ResidentFilter):
-            t = self._L.hnsw_b200_search_flat_submit_filtered(self._h, filter.id, _p(q), nq, d, int(knbn), int(ef), _p(o),
-                                                              _p(ds), _p(it), _p(pid), _p(cnt))
-        else:
-            raise TypeError("submit_flat takes a ResidentFilter (Hnsw.make_filter) as its filter")
+        fn, lead, _ = self._filter_call(filter, "search_flat_submit", "submit_flat")
+        ans = self._answers(q.shape[0], knbn, with_internal, with_pid)
+        t = fn(self._h, *lead, _p(q), *q.shape, int(knbn), int(ef), *map(_p, ans))
         if t < 0:
             raise HnswError(last_error())
-        return (int(t), q, o, ds, it, pid, cnt)
+        return (int(t), q) + ans
 
     def wait_flat(self, ticket):
         t, _q, o, ds, it, pid, cnt = ticket
@@ -618,14 +598,9 @@ class Hnsw:
         Returns the kernel's CUDA-event time in ms when sync is true.  filter: None or a ResidentFilter
         (hnsw_b200_search_device_filtered)."""
         ms = C.c_float(0.0)
-        args = (C.c_void_p(d_queries_ptr), nq, int(knbn), int(ef), C.c_void_p(d_out_ptr), C.c_void_p(d_counts_ptr),
-                int(bool(sync)), C.byref(ms) if sync else None)
-        if filter is None:
-            self._chk(self._L.hnsw_b200_search_device(self._h, *args))
-        elif isinstance(filter, ResidentFilter):
-            self._chk(self._L.hnsw_b200_search_device_filtered(self._h, filter.id, *args))
-        else:
-            raise TypeError("search_device takes a ResidentFilter (Hnsw.make_filter) as its filter")
+        fn, lead, _ = self._filter_call(filter, "search_device", "search_device")
+        self._chk(fn(self._h, *lead, C.c_void_p(d_queries_ptr), nq, int(knbn), int(ef), C.c_void_p(d_out_ptr),
+                     C.c_void_p(d_counts_ptr), int(bool(sync)), C.byref(ms) if sync else None))
         return float(ms.value)
 
     def search_exact_device(self, d_queries_ptr, nq, knbn, d_out_ptr, d_counts_ptr, sync=True, filter=None):
