@@ -620,6 +620,8 @@ static int64_t search_call(const void* h, Via via, const char* name, const Restr
   if (via == HOST && nq == 0) return 0;
   if (rs.kind == Restriction::ROW_FILTERS && !rs.filters) return set_err("filters is NULL");
   if (rs.kind == Restriction::ROW_LABELS && !rs.labels) return set_err("qlabels is NULL");
+  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset_off) return set_err("qset_off is NULL");
+  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset) return set_err("qset is NULL");
   if (!queries || !out.ids || !out.dist || !out.counts || knbn == 0 || nq == 0) return set_err("bad argument");
   HB_PARTS_SHARED_IF(ix);
   HostBatch b{queries, nullptr, nq, (int)dim, knbn, ef, rs, out};
@@ -643,6 +645,9 @@ static Restriction resident_or_all(int64_t f) { return f == -1 ? Restriction() :
 static Restriction row_filters(const int64_t* f) { return {Restriction::ROW_FILTERS, 0, nullptr, 0, nullptr, nullptr, -1, f}; }
 static Restriction row_labels(const uint32_t* l) {
   return {Restriction::ROW_LABELS, 0, nullptr, 0, nullptr, nullptr, -1, nullptr, l};
+}
+static Restriction row_label_sets(const uint64_t* off, const uint32_t* set) {
+  return {Restriction::ROW_LABEL_SETS, 0, nullptr, 0, nullptr, nullptr, -1, nullptr, nullptr, off, set};
 }
 
 // hnsw_b200_search_flat and _search_flat_filtered: the filter is the FilterT arguments (filter_mode 1, 2) or one of the
@@ -786,6 +791,21 @@ int hnsw_b200_search_exact_labeled(const void* h, const uint32_t* qlabels, const
                                    int32_t* out_pid, int32_t* out_counts) {
   return (int)search_call(h, HOST, "search_exact_labeled", row_labels(qlabels), true, queries, nq, dim, knbn, 0,
                           columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+}
+
+// A label set per query: query i is restricted to the points whose label is one of qset[qset_off[i], qset_off[i + 1])
+// ({LABEL_NONE}: every point); the graph search (ef_search) or the exact scan.
+int hnsw_b200_search_flat_label_sets(const void* h, const uint64_t* qset_off, const uint32_t* qset, const void* queries,
+                                     uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search, uint64_t* out_ids,
+                                     float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+  return (int)search_call(h, HOST, "search_flat_label_sets", row_label_sets(qset_off, qset), false, queries, nq, dim, knbn,
+                          ef_search, columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+}
+int hnsw_b200_search_exact_label_sets(const void* h, const uint64_t* qset_off, const uint32_t* qset, const void* queries,
+                                      uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids, float* out_dist,
+                                      uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+  return (int)search_call(h, HOST, "search_exact_label_sets", row_label_sets(qset_off, qset), true, queries, nq, dim, knbn,
+                          0, columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 
 int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,

@@ -10,27 +10,75 @@
 // So here C is a real queue: an unsorted array of keys per warp in global memory, pop = warp-wide min scan
 // (consumed entries are overwritten with ~0).  W is the same sorted shared-memory array as elsewhere.
 // The FilterT predicate (filter.rs:7-24) is a device bitmap over internal ids, materialised by the host, or a point
-// label: the predicate label(p) == L over the label array of the graph store.
+// label: the predicate label(p) == L, or label(p) in a set S of labels, over the label array of the graph store.
 #include "kernels.h"
 #include "search_core.cuh"
 
 namespace hb {
 
 // A query's filter, kept in its warp's mbarrier slot (unused by this kernel) and read at each use, so that the search
-// loop holds no extra register: a bitmap (label == LABEL_NONE), or the label array and the label the query admits.
+// loop holds no extra register: a bitmap (label == LABEL_NONE), or the label array and the label the query admits, or
+// (the launch's SearchParams::label_sets set) the label array and the query's set, label_sets[label, label + nset).
 struct FilterSlot {
   const uint32_t* ptr;
   uint32_t label;
+  uint32_t nset;
 };
 
-// the one admission test: the point's label, or its bit of the bitmap
+// The launch's label_sets (nullptr: none), kept by lane 0 in the 16 bytes just below the slot: the tail of the
+// candidate-distance region, whose first 32 of 64 reserved entries are all this kernel scores into.  Read there, the
+// admission test needs neither a register nor an argument for it; as an argument it pushed the generic (CH = 0)
+// kernels of f32 L2 and cosine into spilling.
+__device__ __forceinline__ const uint32_t** set_base(FilterSlot* f) { return reinterpret_cast<const uint32_t**>(f) - 2; }
+__device__ __forceinline__ const uint32_t* set_base(const FilterSlot* f) {
+  return *(reinterpret_cast<const uint32_t* const*>(f) - 2);
+}
+
+// x is one of the sorted values v[0, n): a binary search in global memory
+__device__ __forceinline__ bool in_sorted(const uint32_t* v, uint32_t n, uint32_t x) {
+  while (n) {
+    const uint32_t h = n >> 1, m = __ldg(v + h);
+    if (m == x) return true;
+    if (m < x) {
+      v += h + 1;
+      n -= h + 1;
+    } else {
+      n = h;
+    }
+  }
+  return false;
+}
+
+__device__ __noinline__ bool in_sorted_call(const uint32_t* v, uint32_t n, uint32_t x) { return in_sorted(v, n, x); }
+
+// Kernels whose register allocation (ptxas -v) stays the one they had before label sets only when the set lookup is a
+// call: the generic u32 / i32 Hamming and L2 and u8 / u16 Jaccard ones.  Inlined, they spill more (Hamming: 76 registers
+// and no spill became 64 and 40 bytes, measurably slower); every other kernel keeps its allocation with the lookup
+// inlined, and the f32 L2 one only then.
+template <class Op> struct SetLookupCall { static constexpr bool value = false; };
+template <> struct SetLookupCall<OpHamming<int32_t>> { static constexpr bool value = true; };
+template <> struct SetLookupCall<OpHamming<uint32_t>> { static constexpr bool value = true; };
+template <> struct SetLookupCall<OpCast<int32_t, OpL2>> { static constexpr bool value = true; };
+template <> struct SetLookupCall<OpCast<uint32_t, OpL2>> { static constexpr bool value = true; };
+template <> struct SetLookupCall<OpJaccard<uint8_t>> { static constexpr bool value = true; };
+template <> struct SetLookupCall<OpJaccard<uint16_t>> { static constexpr bool value = true; };
+
+// the one admission test: the point's label against the query's label or set, or its bit of the bitmap
+template <class Op>
 __device__ __forceinline__ bool filter_pass(const FilterSlot* f, uint32_t id) {
   const uint32_t want = f->label;
-  if (want != LABEL_NONE) return __ldg(f->ptr + id) == want;
+  if (want != LABEL_NONE) {
+    const uint32_t lab = __ldg(f->ptr + id);
+    const uint32_t* sets = set_base(f);
+    if (!sets) return lab == want;
+    if constexpr (SetLookupCall<Op>::value) return in_sorted_call(sets + want, f->nset, lab);
+    return in_sorted(sets + want, f->nset, lab);
+  }
   return (__ldg(f->ptr + (id >> 5)) >> (id & 31)) & 1u;
 }
 
 // keeps the keys w[0, n) whose points pass the filter, in order, at the front of w; returns how many there are
+template <class Op>
 __device__ __forceinline__ int keep_passing(uint64_t* w, int n, const FilterSlot* fslot) {
   const int lane = lane_id();
   int out = 0;
@@ -40,7 +88,7 @@ __device__ __forceinline__ int keep_passing(uint64_t* w, int n, const FilterSlot
     bool keep = false;
     if (i < n) {
       v = w[i];
-      keep = filter_pass(fslot, key_id(v));
+      keep = filter_pass<Op>(fslot, key_id(v));
     }
     const unsigned m = __ballot_sync(FULL, keep);
     __syncwarp();
@@ -54,7 +102,8 @@ __device__ __forceinline__ int keep_passing(uint64_t* w, int n, const FilterSlot
 template <class Op, int CH, int U>
 __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const WarpSmem& s, const VisitedCfg& vc, Visited& vis,
                                                       SortedQueue& W, uint64_t* cbuf, uint32_t ccap,
-                                                      const FilterSlot* fslot, uint32_t ep, int ef, int layer, Stats& st, bool& overflow) {
+                                                      const FilterSlot* fslot, uint32_t ep, int ef, int layer,
+                                                      Stats& st, bool& overflow) {
   const int lane = lane_id();
   const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
   vis.begin(vc, ep, lane);  // hnsw.rs:955-956
@@ -101,7 +150,7 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
     const uint64_t fkey = W.w[W.n - 1] & ~1ull;
     // 981: the reference compares DISTANCES here (-(c.dist) > f.dist); with equal distances a larger id must not
     // trigger the retain pass (Hamming / Jaccard / integer L1 tie often)
-    if ((best >> 32) > (fkey >> 32) && W.n >= ef) W.n = keep_passing(W.w, W.n, fslot);  // 994-1000
+    if ((best >> 32) > (fkey >> 32) && W.n >= ef) W.n = keep_passing<Op>(W.w, W.n, fslot);  // 994-1000
     const uint32_t c = key_id(best);
     int cap;
     const uint32_t* ids = list_ids(g, c, layer, cap);  // 1006
@@ -123,7 +172,7 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
         st.evals += cnt;
         const uint32_t my_id = lane < cnt ? s.cand_id[lane] : 0u;
         const uint64_t key = lane < cnt ? make_key(Op::post(s.cand_d[lane]), my_id) : ~0ull;
-        const bool my_pass = lane < cnt && filter_pass(fslot, my_id);
+        const bool my_pass = lane < cnt && filter_pass<Op>(fslot, my_id);
         const unsigned passmask = __ballot_sync(FULL, my_pass);
         for (int j = 0; j < cnt; ++j) {  // strictly in list order: the accept rule sees the W of that moment
           if (W.n == 0) {                // 1019-1024
@@ -140,7 +189,7 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
             if (lane == 0) __stcg(cbuf + cn, kj);  // 1035-1036: every accepted candidate goes to C
             cn += 1;
             if ((passmask >> j) & 1u) {  // 1040-1049
-              if (W.n == 1 && !filter_pass(fslot, key_id(W.w[0]))) W.n = 0;
+              if (W.n == 1 && !filter_pass<Op>(fslot, key_id(W.w[0]))) W.n = 0;
               __syncwarp();
               W.insert(kj);  // push, and pop the farthest when over ef (1051-1053)
             }
@@ -179,11 +228,18 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
     const uint32_t qi = next_item(p.work_counter, lane);
     if (qi >= p.nq) break;
     stage_row_bytes(s.q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes, p.q_bytes, g.d4 * 16);
-    // this query's filter: the launch's one bitmap, its own entry of the bitmap table, or its own label
+    // this query's filter: the launch's one bitmap, its own entry of the bitmap table, its own label or label set
     if (lane == 0) {
       if (p.labels) {
         fslot->ptr = p.labels;
-        fslot->label = p.filter_sel[qi];
+        *set_base(fslot) = p.label_sets;
+        if (p.label_sets) {
+          const uint2 s2 = reinterpret_cast<const uint2*>(p.filter_sel)[qi];
+          fslot->label = s2.x;
+          fslot->nset = s2.y;
+        } else {
+          fslot->label = p.filter_sel[qi];
+        }
       } else {
         fslot->ptr = p.filter_sel ? p.filter_table[p.filter_sel[qi]] : p.filter_bits;
         fslot->label = LABEL_NONE;
@@ -196,7 +252,8 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
     if (g.entry != INVALID_ID) {
       // the filter plays no role in the descent (hnsw.rs:1511-1529)
       const Entry e = descend<Op>(g, lane, st, WarpChunk<Op, CH, U>{g, s, lane});
-      search_layer_filtered<Op, CH, U>(g, s, p.vis, vis, W, cbuf, p.ccap, fslot, e.pivot, p.ef, p.layer0, st, overflow);
+      search_layer_filtered<Op, CH, U>(g, s, p.vis, vis, W, cbuf, p.ccap, fslot, e.pivot, p.ef, p.layer0, st,
+                                       overflow);
       count = min(p.k, min(p.ef, W.n));  // hnsw.rs:1547
     }
     if (overflow) {
@@ -212,7 +269,7 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
       bool keep = false;
       if (j < count) {
         key = W.w[j];
-        keep = filter_pass(fslot, key_id(key));
+        keep = filter_pass<Op>(fslot, key_id(key));
       }
       const unsigned m = __ballot_sync(FULL, keep);
       if (keep) {

@@ -12,6 +12,7 @@
 //     each replica's leg by that replica's worker.
 #include <algorithm>
 #include <cstring>
+#include <map>
 #include <numeric>
 #include <set>
 
@@ -183,7 +184,7 @@ int Index::plan(size_t nq, std::vector<Leg>& legs) {
 }
 
 int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>& sorted, Leg* legs, size_t n,
-                   std::vector<std::vector<uint32_t>>& bits) {
+                   std::vector<std::vector<uint32_t>>& bits, const LabelSets* sets) {
   const int P = parts ? parts->count() : 1;
   if (rs.kind == Restriction::FILTER_T) {
     bits.resize(P);
@@ -196,11 +197,16 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
       }
     }
   }
-  // run u of leg l under `key`, a resident filter or a label
+  // run u of leg l under `key`, a resident filter, a label or a label set
   auto restrict_run = [&](const Leg& l, int64_t key, LegPlan::Run& u) {
     if (rs.kind == Restriction::FILTER_T) {
       u.host_bits = bits[l.part].data();
       return 0;
+    }
+    if (rs.kind == Restriction::ROW_LABEL_SETS) {
+      u.set = sets->values.data() + sets->off[key];
+      u.nset = (uint32_t)(sets->off[key + 1] - sets->off[key]);
+      return exact ? l.rx->label_set_scan(u.set, u.nset, u.slices) : 0;
     }
     if (rs.kind != Restriction::ROW_LABELS) return filters.use(key, l.part, P, l.rx, &u.bits, exact ? &u.scan : nullptr);
     u.label = (uint32_t)key;
@@ -223,12 +229,12 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
     const int64_t* key = sorted.data() + l->first;
     while (pl.plain < l->count && key[pl.plain] == -1) ++pl.plain;
     // labels: the leg's own, or on a replica its copy of the handle's, made current first
-    if (rs.kind == Restriction::ROW_LABELS && pl.plain < l->count &&
-        l->rx->labels_on_device(parts ? l->rx : this, &pl.labels)) {
+    pl.label_sets = rs.kind == Restriction::ROW_LABEL_SETS;
+    if (rs.by_label() && pl.plain < l->count && l->rx->labels_on_device(parts ? l->rx : this, &pl.labels)) {
       r = l->rc = -1;
       continue;
     }
-    for (size_t j = pl.plain, e; j < l->count; j = e) {  // one run per filter or label
+    for (size_t j = pl.plain, e; j < l->count; j = e) {  // one run per filter, label or label set
       for (e = j + 1; e < l->count && key[e] == key[j];) ++e;
       LegPlan::Run u{j, e - j};
       if (restrict_run(*l, key[j], u)) {
@@ -241,17 +247,61 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
   return r;
 }
 
+// The label sets of rows [0, nq): each row's values made ascending without repeats and checked, the distinct sets into
+// `sets` in lexicographic order, and key[i] the set of row i, or -1 for {LABEL_NONE}.  The first row whose offsets
+// decrease or whose set holds LABEL_NONE with another label refuses the call.
+static int label_set_keys(const Restriction& rs, size_t nq, std::vector<int64_t>& key, LabelSets& sets, std::string& err) {
+  std::map<std::vector<uint32_t>, int64_t> distinct;
+  std::vector<const std::vector<uint32_t>*> row_set(nq, nullptr);
+  std::vector<uint32_t> v;
+  for (size_t i = 0; i < nq; ++i) {
+    const uint64_t lo = rs.qset_off[i], hi = rs.qset_off[i + 1];
+    if (hi < lo) {
+      err = "label set " + std::to_string(i) + ": qset_off[" + std::to_string(i + 1) + "] = " + std::to_string(hi) +
+            " is below qset_off[" + std::to_string(i) + "] = " + std::to_string(lo);
+      return -1;
+    }
+    v.assign(rs.qset + lo, rs.qset + hi);
+    std::sort(v.begin(), v.end());
+    v.erase(std::unique(v.begin(), v.end()), v.end());
+    if (!v.empty() && v.back() == LABEL_NONE) {
+      if (v.size() > 1) {
+        err = "label set " + std::to_string(i) + " holds LABEL_NONE together with another label";
+        return -1;
+      }
+      continue;  // {LABEL_NONE}: every point
+    }
+    row_set[i] = &distinct.emplace(v, 0).first->first;
+  }
+  sets.values.clear();
+  sets.off.assign(1, 0);
+  for (auto& d : distinct) {
+    d.second = (int64_t)sets.off.size() - 1;
+    sets.values.insert(sets.values.end(), d.first.begin(), d.first.end());
+    sets.off.push_back(sets.values.size());
+  }
+  key.resize(nq);
+  for (size_t i = 0; i < nq; ++i) key[i] = row_set[i] ? distinct.find(*row_set[i])->second : -1;
+  return 0;
+}
+
 // Every filter is checked on every partition before anything runs, so that a bad entry refuses the whole call, named by
 // its first position.  The sort is stable: rows of one filter keep their order, and -1 (no filter) sorts first.  A label
-// needs no check; LABEL_NONE sorts first as -1.
-int Index::sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm, std::vector<int64_t>& sorted) {
+// needs no check; LABEL_NONE sorts first as -1.  A label set is checked and made canonical (label_set_keys); {LABEL_NONE}
+// sorts first as -1.
+int Index::sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm, std::vector<int64_t>& sorted,
+                     LabelSets& sets) {
   const int P = parts ? parts->count() : 1;
-  const bool labels = rs.kind == Restriction::ROW_LABELS;
+  const bool labels = rs.by_label();
   std::vector<int64_t> key;
   const int64_t* fid = rs.filters;
-  if (labels) {
+  if (rs.kind == Restriction::ROW_LABELS) {
     key.resize(nq);
     for (size_t i = 0; i < nq; ++i) key[i] = rs.labels[i] == LABEL_NONE ? -1 : (int64_t)rs.labels[i];
+    fid = key.data();
+  } else if (rs.kind == Restriction::ROW_LABEL_SETS) {
+    std::string e;
+    if (label_set_keys(rs, nq, key, sets, e)) return fail(e);
     fid = key.data();
   }
   std::set<int64_t> checked;
@@ -325,7 +375,7 @@ int Index::prepare_batch(const HostBatch& call, HostBatch& b, Ticket& t, bool re
   b = call;
   std::vector<int64_t> sorted;
   if (call.restriction.per_row()) {
-    if ((r = sort_rows(call.restriction, call.nq, t.perm, sorted))) return r;
+    if ((r = sort_rows(call.restriction, call.nq, t.perm, sorted, t.sets))) return r;
     t.rows.resize(call.nq);
     for (size_t j = 0; j < call.nq; ++j)
       t.rows[j] = call.rows ? call.rows[t.perm[j]] : (const char*)call.queries + t.perm[j] * (size_t)call.d * es;
@@ -335,7 +385,7 @@ int Index::prepare_batch(const HostBatch& call, HostBatch& b, Ticket& t, bool re
   t.k = b.k;
   t.out = b.out;
   if ((r = plan(b.nq, t.legs))) return r;
-  if (resolve(b.restriction, b.exact, sorted, t.legs.data(), t.legs.size(), t.bits))
+  if (resolve(b.restriction, b.exact, sorted, t.legs.data(), t.legs.size(), t.bits, &t.sets))
     return legs_fail(t.legs.data(), t.legs.size(), replicas_first && !parts);
   return 0;
 }

@@ -722,6 +722,7 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.filter_table = f.table;
   p.filter_sel = f.sel;
   p.labels = f.labels;
+  p.label_sets = f.sets;
   p.stats = stats_on_ ? d_stats_ : nullptr;
   p.status = c.d_status;
   const bool filtered = f.bits != nullptr || f.sel != nullptr;
@@ -890,9 +891,11 @@ int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** 
 }
 
 // A single bitmap run goes to the launch as its filter bits (a FilterT's host bits uploaded into the context first), as
-// a batch-wide filter does; several as a table of their bitmaps and each row's entry in it, and label runs as the label
-// array and each row's label, uploaded into the context ahead of the launches.  Exact: a group of every point for the
-// unrestricted rows, and one per run.
+// a batch-wide filter does; several as a table of their bitmaps and each row's entry in it, label runs as the label
+// array and each row's label, and label-set runs as the label array, the sets' values and each row's (offset, count) in
+// them, uploaded into the context ahead of the launches.  Exact: a group of every point for the unrestricted rows, and
+// one per run; a label set scans its one CSR slice, or its slices copied one after the other into the context (a point
+// has one label, so they are disjoint, and the exact scan orders by (distance, id), so their order does not matter).
 int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
   cudaStream_t st = c.stream;
   int r;
@@ -900,10 +903,47 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
   L.plain = plan.plain;
   if (plan.exact) {
     if (plan.plain) L.groups.push_back(ExactGroup{0, plan.plain, ExactScan()});
-    for (const LegPlan::Run& u : plan.runs) L.groups.push_back(ExactGroup{u.first, u.count, u.scan});
+    size_t joined = 0;  // ids copied into the context
+    if (plan.label_sets) {
+      for (const LegPlan::Run& u : plan.runs)
+        if (u.slices.size() != 1)
+          for (const ExactScan& x : u.slices) joined += x.n;
+      if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, std::max<size_t>(joined, 1) * 4, st))) return r;  // never null
+    }
+    uint32_t* at = (uint32_t*)c.d_fbits;
+    for (const LegPlan::Run& u : plan.runs) {
+      ExactScan scan = u.scan;
+      if (plan.label_sets && u.slices.size() == 1) {
+        scan = u.slices[0];
+      } else if (plan.label_sets) {
+        scan = ExactScan{at, 0};
+        for (const ExactScan& x : u.slices) {
+          HB_CUDA(cudaMemcpyAsync(at, x.ids, x.n * 4, cudaMemcpyDeviceToDevice, st));
+          at += x.n;
+          scan.n += x.n;
+        }
+      }
+      L.groups.push_back(ExactGroup{u.first, u.count, scan});
+    }
     return 0;
   }
   if (plan.runs.empty()) return 0;
+  if (plan.label_sets) {
+    std::vector<uint32_t> sel, vals;  // sel: (offset, count) per row
+    for (const LegPlan::Run& u : plan.runs) {
+      if (vals.size() >= LABEL_NONE - u.nset) return fail("label sets: too many distinct labels in one batch");
+      for (size_t j = 0; j < u.count; ++j) sel.insert(sel.end(), {(uint32_t)vals.size(), u.nset});
+      vals.insert(vals.end(), u.set, u.set + u.nset);
+    }
+    const size_t sb = round128(sel.size() * sizeof(uint32_t)), vb = vals.size() * sizeof(uint32_t);
+    if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, sb + vb, st))) return r;
+    HB_CUDA(cudaMemcpyAsync(c.d_fbits, sel.data(), sel.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+    if (vb) HB_CUDA(cudaMemcpyAsync((char*)c.d_fbits + sb, vals.data(), vb, cudaMemcpyHostToDevice, st));
+    L.filter.sel = (const uint32_t*)c.d_fbits;
+    L.filter.sets = (const uint32_t*)((char*)c.d_fbits + sb);
+    L.filter.labels = plan.labels;
+    return 0;
+  }
   if (plan.runs.size() == 1 && !plan.labels) {
     L.filter.bits = plan.runs[0].bits;  // a resident filter: already on this device
     if (plan.runs[0].host_bits) {

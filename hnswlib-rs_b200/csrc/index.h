@@ -120,12 +120,14 @@ struct ExactGroup {
 };
 
 // The restriction of one search launch, as SearchParams reads it: none, one bitmap for every row (bits), a bitmap per row
-// (row i on table[sel[i]]), or a label per row (row i on the points whose `labels` entry is sel[i])
+// (row i on table[sel[i]]), a label per row (row i on the points whose `labels` entry is sel[i]), or a label set per row
+// (row i on the points whose `labels` entry is one of sets[sel[2i], sel[2i] + sel[2i + 1]))
 struct LaunchFilter {
   const uint32_t* bits = nullptr;
   const uint32_t* const* table = nullptr;
   const uint32_t* sel = nullptr;
   const uint32_t* labels = nullptr;
+  const uint32_t* sets = nullptr;
 };
 
 // Resident filters (hnsw_b200_filter_new, filter_store.cu): a FilterT materialised once per handle, as one bitmap per
@@ -207,9 +209,10 @@ struct AnswerArrays {
 
 // What the rows of a batch may return: every point (NONE); the points a FilterT admits (FILTER_T: `mode` 1 sorted
 // origin-id list, 2 callback, as make_filter_bits reads it); one resident filter for every row (RESIDENT); a resident
-// filter per row, -1 = none (ROW_FILTERS); or a label per row, LABEL_NONE = none (ROW_LABELS)
+// filter per row, -1 = none (ROW_FILTERS); a label per row, LABEL_NONE = none (ROW_LABELS); or a set of labels per row,
+// row i's the values qset[qset_off[i], qset_off[i + 1]) in any order and with repeats, {LABEL_NONE} = none (ROW_LABEL_SETS)
 struct Restriction {
-  enum Kind { NONE, FILTER_T, RESIDENT, ROW_FILTERS, ROW_LABELS } kind = NONE;
+  enum Kind { NONE, FILTER_T, RESIDENT, ROW_FILTERS, ROW_LABELS, ROW_LABEL_SETS } kind = NONE;
   int mode = 0;
   const uint64_t* ids = nullptr;
   size_t nids = 0;
@@ -218,7 +221,17 @@ struct Restriction {
   int64_t resident = -1;
   const int64_t* filters = nullptr;  // [nq]
   const uint32_t* labels = nullptr;  // [nq]
-  bool per_row() const { return kind == ROW_FILTERS || kind == ROW_LABELS; }
+  const uint64_t* qset_off = nullptr;  // [nq + 1]
+  const uint32_t* qset = nullptr;
+  bool per_row() const { return kind == ROW_FILTERS || kind == ROW_LABELS || kind == ROW_LABEL_SETS; }
+  bool by_label() const { return kind == ROW_LABELS || kind == ROW_LABEL_SETS; }
+};
+
+// The distinct label sets of a ROW_LABEL_SETS batch (Index::sort_rows): set j is values[off[j], off[j + 1]), ascending
+// and without repeats
+struct LabelSets {
+  std::vector<uint32_t> values;
+  std::vector<size_t> off;
 };
 
 // One host search batch: flat queries or one pointer per query (rows), k answers each into `out`.  `exact`: the exact
@@ -236,20 +249,26 @@ struct HostBatch {
 
 // A leg's restriction (Index::resolve): its rows [0, plain) are unrestricted, and `runs` cover the rest, each a range of
 // consecutive rows under one restriction.  A run is a resident filter's bitmap on the leg's device, a FilterT's host bits
-// (uploaded into the context when the leg begins), or a label on `labels` (the label array on the leg's device); in an
-// exact batch, the points it scans.  A batch-wide filter is a plan with no prefix and one run over every row.
+// (uploaded into the context when the leg begins), a label on `labels` (the label array on the leg's device), or a label
+// set (label_sets) on `labels`; in an exact batch, the points it scans, and for a label set the slices of the label CSR
+// they are the union of, joined into one list in the context when there are several (stage_plan).  A batch-wide filter
+// is a plan with no prefix and one run over every row.
 struct LegPlan {
   struct Run {
     size_t first, count;
     const uint32_t* bits = nullptr;
     const uint32_t* host_bits = nullptr;
     uint32_t label = LABEL_NONE;
+    const uint32_t* set = nullptr;  // label_sets: the run's set, nset values of a LabelSets
+    uint32_t nset = 0;
     ExactScan scan;
+    std::vector<ExactScan> slices;
   };
   bool exact = false;
   size_t plain = 0;
   std::vector<Run> runs;
   const uint32_t* labels = nullptr;
+  bool label_sets = false;
 };
 
 // One Index's part of a batch: queries [first, first + count) searched on rx (the handle, a replica, or partition `part`)
@@ -309,7 +328,7 @@ class Index {
   int search_host_finish(int c, const NeighbourOut** out, const int32_t** counts);
   // host search batches (host_search.cu): synchronous, or submitted now and collected by finish_batch.  A ticket is a
   // batch planned into legs, with what the legs read until they are collected: a per-row batch's caller row of each
-  // sorted row (out.perm) and its sorted rows, and a FilterT's host bits per partition.
+  // sorted row (out.perm) and its sorted rows, a FilterT's host bits per partition, and a label-set batch's sets.
   struct Ticket {
     std::vector<Leg> legs;
     size_t k = 0;
@@ -317,6 +336,7 @@ class Index {
     std::vector<size_t> perm;
     std::vector<const void*> rows;
     std::vector<std::vector<uint32_t>> bits;
+    LabelSets sets;
   };
   int search_batch(const HostBatch& b);
   int64_t submit_batch(const HostBatch& b);  // a ticket id, or < 0
@@ -326,18 +346,21 @@ class Index {
   void drain_pending() const {
     while (pending_.load() != 0) std::this_thread::yield();
   }
-  // the plan of each of legs[0, n) under `rs`; `sorted` holds a per-row restriction's keys (a filter id or a label, -1:
-  // none) in the order the legs run the rows (sort_rows).  A FilterT's host bits are made on the calling thread once per
-  // partition (a replica shares the handle's internal ids, and so its bits) into `bits`; a resident filter is its copy
-  // on each leg's device; a label needs the label array on the leg's device.  `exact`: each run's ExactScan (a filter's
-  // id list or a label's CSR slice on the leg's device).  Nonzero when a leg could not have its plan; that leg's rc is
-  // set (legs_fail reports it).
+  // the plan of each of legs[0, n) under `rs`; `sorted` holds a per-row restriction's keys (a filter id, a label or a
+  // set of `sets`, -1: none) in the order the legs run the rows (sort_rows).  A FilterT's host bits are made on the
+  // calling thread once per partition (a replica shares the handle's internal ids, and so its bits) into `bits`; a
+  // resident filter is its copy on each leg's device; a label or label set needs the label array on the leg's device.
+  // `exact`: each run's ExactScan (a filter's id list or a label's CSR slice on the leg's device; a label set's slices).
+  // Nonzero when a leg could not have its plan; that leg's rc is set (legs_fail reports it).
   int resolve(const Restriction& rs, bool exact, const std::vector<int64_t>& sorted, Leg* legs, size_t n,
-              std::vector<std::vector<uint32_t>>& bits);
+              std::vector<std::vector<uint32_t>>& bits, const LabelSets* sets = nullptr);
   // a per-row restriction: every filter of rs.filters[0, nq) is -1 or a live, current filter of this handle (else the
   // first bad position is refused), and `perm` orders the rows stably by filter, the unfiltered ones first; labels by
-  // label, LABEL_NONE first.  sorted[j]: the filter or label of sorted row j (-1: none).
-  int sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm, std::vector<int64_t>& sorted);
+  // label, LABEL_NONE first; label sets, each made ascending without repeats into `sets`, by set, {LABEL_NONE} first
+  // (a decreasing offset, or LABEL_NONE with another label, refuses the first such row).  sorted[j]: the filter, label
+  // or set of sorted row j (-1: none).
+  int sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm, std::vector<int64_t>& sorted,
+                LabelSets& sets);
 
   // ---- point labels (labels.cu).  One u32 per point (GraphStore LABEL and its host mirror h_label), LABEL_NONE until
   // set_labels names one; label_version counts the calls that changed them (a replica: the handle's version it copied).
@@ -349,6 +372,9 @@ class Index {
   int labels_on_device(const Index* src, const uint32_t** d_labels);
   // the exact scan of the points labelled `label`: a slice of this Index's label CSR, rebuilt when the labels changed
   int label_scan(uint32_t label, ExactScan* scan);
+  // the points whose label is one of set[0, nset) (ascending): one slice of the label CSR per label that some point
+  // carries, slices that follow each other in the CSR joined into one
+  int label_set_scan(const uint32_t* set, size_t nset, std::vector<ExactScan>& slices);
   // device queries in, device answers out; the restriction is none or a resident filter.  `exact`: the exact scan (ef
   // unused).
   int search_device(const Restriction& rs, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef,
@@ -413,7 +439,8 @@ class Index {
     unsigned int* d_counter = nullptr;
     int* d_status = nullptr;
     VisitedPool vis, fvis;  // unfiltered / filtered searches
-    void *d_fbits = nullptr, *d_cbuf = nullptr;  // the call's filter bits (or its bitmap table and selectors) / C
+    // the call's filter bits (or its bitmap table and selectors; exact: its label sets' joined id lists) / C
+    void *d_fbits = nullptr, *d_cbuf = nullptr;
     size_t d_fbits_bytes = 0, d_cbuf_bytes = 0;
     void *d_xq = nullptr, *d_xpart = nullptr;  // exact scan: the host batch's queries on the device / tickets and slice lists
     size_t d_xq_bytes = 0, d_xpart_bytes = 0;
@@ -524,7 +551,7 @@ class Index {
   int legs_fail(const Leg* legs, size_t n, bool replicas_first);
 
   // ---- point labels (labels.cu).  The CSR of the exact path: the internal ids of every labelled point on this device,
-  // grouped by label and ascending within a group; groups[label] = (offset, count).  Made from h_label at label version
+  // grouped by label in ascending label order and ascending within a group; groups[label] = (offset, count).  Made from h_label at label version
   // `version` (~0: never), at the first exact labelled search after the labels changed.  A point added since has no
   // label, so inserts leave it current.  label_mu_ guards it and a replica's copy of the labels.
   struct LabelCsr {

@@ -67,6 +67,10 @@ struct SearchParams {
   // filtered search with a label per query (labels != nullptr): query i admits the points p with labels[p] ==
   // filter_sel[i] (never LABEL_NONE) instead of a bitmap.  Appended like the two above.
   const uint32_t* labels;  // [points]
+  // filtered search with a label set per query (labels and label_sets != nullptr): filter_sel is [nq][2], and query i
+  // admits the points p whose labels[p] is one of label_sets[filter_sel[2i], filter_sel[2i] + filter_sel[2i + 1]),
+  // sorted ascending, none LABEL_NONE (filter_sel[2i] is never LABEL_NONE).  Appended like the fields above.
+  const uint32_t* label_sets;
 };
 
 // the label of a point that has none (hnsw_b200_set_labels): no label admits it

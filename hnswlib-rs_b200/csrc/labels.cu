@@ -1,7 +1,8 @@
 // Point labels (index.h "point labels"): one u32 per point, next to the graph, that a search can restrict each query to.
 // No kernel of its own.  A graph search with a label per query runs the filtered query kernel (filter.cu), whose
-// admission test reads the label array instead of a bitmap.  An exact search runs the exact scan over one slice per
-// label of a CSR of internal ids grouped by label, made on the host.
+// admission test reads the label array instead of a bitmap, or with a label set per query, looks the point's label up in
+// the query's set.  An exact search runs the exact scan over one slice per label of a CSR of internal ids grouped by
+// label, made on the host; a label set's points are its labels' slices, joined into one list by copies (stage_plan).
 #include <algorithm>
 
 #include "index.h"
@@ -46,7 +47,8 @@ int Index::label_scan(uint32_t label, ExactScan* scan) {
   std::lock_guard<std::mutex> lk(label_mu_);
   LabelCsr& c = label_csr_;
   if (c.version != label_version) {
-    // counts per label, then each group's offset, then the ids in ascending order into their groups
+    // counts per label, then each group's offset in ascending label order (so that a label set's adjacent labels are
+    // one slice), then the ids in ascending order into their groups
     c.groups.clear();
     size_t total = 0;
     for (size_t i = 0; i < n; ++i)
@@ -54,10 +56,15 @@ int Index::label_scan(uint32_t label, ExactScan* scan) {
         c.groups[h_label[i]].second++;
         total++;
       }
+    std::vector<uint32_t> order;
+    order.reserve(c.groups.size());
+    for (const auto& g : c.groups) order.push_back(g.first);
+    std::sort(order.begin(), order.end());
     uint32_t off = 0;
-    for (auto& g : c.groups) {
-      g.second.first = off;
-      off += g.second.second;
+    for (uint32_t L : order) {
+      auto& g = c.groups[L];
+      g.first = off;
+      off += g.second;
     }
     std::vector<uint32_t> ids(total);
     std::unordered_map<uint32_t, uint32_t> at;
@@ -85,6 +92,21 @@ int Index::label_scan(uint32_t label, ExactScan* scan) {
   const uint32_t off = g == c.groups.end() ? 0 : g->second.first, cnt = g == c.groups.end() ? 0 : g->second.second;
   scan->ids = (const uint32_t*)c.d_ids + off;
   scan->n = cnt;
+  return 0;
+}
+
+int Index::label_set_scan(const uint32_t* set, size_t nset, std::vector<ExactScan>& slices) {
+  slices.clear();
+  for (size_t j = 0; j < nset; ++j) {
+    ExactScan s;
+    int r;
+    if ((r = label_scan(set[j], &s))) return r;
+    if (s.n == 0) continue;
+    if (!slices.empty() && slices.back().ids + slices.back().n == s.ids)
+      slices.back().n += s.n;
+    else
+      slices.push_back(s);
+  }
   return 0;
 }
 

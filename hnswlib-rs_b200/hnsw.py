@@ -107,6 +107,8 @@ def load_library():
     L.hnsw_b200_get_labels.argtypes = [vp, u64, u64, vp]
     L.hnsw_b200_search_flat_labeled.argtypes = [vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_exact_labeled.argtypes = [vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_flat_label_sets.argtypes = [vp, vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_exact_label_sets.argtypes = [vp, vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_get_stats.argtypes = [vp, vp, i32]
     L.hnsw_b200_set_stream.argtypes = [vp, vp]
     L.hnsw_b200_join.argtypes = [vp]
@@ -245,6 +247,28 @@ def _labels(labels, n, what):
     if a.size and (a.min() < 0 or a.max() > LABEL_NONE):
         raise ValueError(f"{what}: labels are unsigned 32-bit integers")
     return np.ascontiguousarray(a, np.uint32)
+
+
+def _label_sets(sets, nq):
+    """the sets argument of the label-set searches, as (offsets u64[nq + 1], values u32[>= 1]): a sequence of nq
+    iterables of labels, or a tuple (offsets, values) as the C calls take it (query i: values[offsets[i]:offsets[i + 1]])"""
+    if isinstance(sets, tuple):
+        off, vals = sets
+        off, vals = np.asarray(off).reshape(-1), np.asarray(vals).reshape(-1)
+        if off.shape != (nq + 1,):
+            raise ValueError(f"sets: {off.size} offsets for {nq} queries, expected {nq + 1}")
+        if off.size and (off.dtype.kind not in "iu" or off.min() < 0 or off.max() > vals.size):
+            raise ValueError(f"sets: offsets must be integers in [0, {vals.size}], the number of values")
+        off = np.ascontiguousarray(off, np.uint64)
+    else:
+        if len(sets) != nq:
+            raise ValueError(f"sets has {len(sets)} entries for {nq} queries")
+        parts = [np.asarray(x if isinstance(x, np.ndarray) else list(x), np.int64).reshape(-1) for x in sets]
+        off = np.zeros(nq + 1, np.uint64)
+        off[1:] = np.cumsum([x.size for x in parts])
+        vals = np.concatenate(parts) if parts else np.zeros(0, np.int64)
+    vals = _labels(vals, vals.size, "sets")
+    return off, vals if vals.size else np.zeros(1, np.uint32)   # never a NULL pointer
 
 
 class Hnsw:
@@ -490,6 +514,24 @@ class Hnsw:
         q = np.ascontiguousarray(queries, self.dtype)
         lab = _labels(labels, q.shape[0], "labels")
         return self._host_search(self._L.hnsw_b200_search_exact_labeled, (_p(lab),), q, knbn, (), with_internal, with_pid)
+
+    def search_flat_label_sets(self, queries, knbn, ef, sets, with_internal=True, with_pid=True):
+        """hnsw_b200_search_flat_label_sets: one batch, query i restricted to the points whose label is in sets[i] (any
+        order, repeats allowed; [LABEL_NONE]: every point; empty: none).  sets is a sequence of iterables of labels, or
+        a tuple (offsets, values).  Row i equals search_flat with a resident filter admitting exactly those points.
+        Returns search_flat's (origin, dist, internal | None, pid | None, counts)."""
+        q = np.ascontiguousarray(queries, self.dtype)
+        off, vals = _label_sets(sets, q.shape[0])
+        return self._host_search(self._L.hnsw_b200_search_flat_label_sets, (_p(off), _p(vals)), q, knbn, (int(ef),),
+                                 with_internal, with_pid)
+
+    def search_exact_label_sets(self, queries, knbn, sets, with_internal=True, with_pid=True):
+        """hnsw_b200_search_exact_label_sets: the exact knbn nearest of query i among the points whose label is in
+        sets[i] (as search_flat_label_sets takes it), in one batch.  Returns search_exact's tuple."""
+        q = np.ascontiguousarray(queries, self.dtype)
+        off, vals = _label_sets(sets, q.shape[0])
+        return self._host_search(self._L.hnsw_b200_search_exact_label_sets, (_p(off), _p(vals)), q, knbn, (),
+                                 with_internal, with_pid)
 
     def make_filter(self, filter):
         """hnsw_b200_filter_new: materialise a FilterT (sorted id sequence or callable(id)->bool, as search_flat takes)

@@ -92,6 +92,13 @@ extern "C" {
     fn hnsw_b200_search_exact_labeled(h: *const HnswApif32, qlabels: *const u32, queries: *const f32, nq: u64, dim: u64,
                                       knbn: u64, out_ids: *mut u64, out_dist: *mut f32, out_internal: *mut u32,
                                       out_pid: *mut i32, out_counts: *mut i32) -> c_int;
+    // label sets (include/hnsw_b200.h "Label sets"): query i's set is qset[qset_off[i] .. qset_off[i + 1]]
+    fn hnsw_b200_search_flat_label_sets(h: *const HnswApif32, qset_off: *const u64, qset: *const u32, queries: *const f32,
+                                        nq: u64, dim: u64, knbn: u64, ef: u64, out_ids: *mut u64, out_dist: *mut f32,
+                                        out_internal: *mut u32, out_pid: *mut i32, out_counts: *mut i32) -> c_int;
+    fn hnsw_b200_search_exact_label_sets(h: *const HnswApif32, qset_off: *const u64, qset: *const u32, queries: *const f32,
+                                         nq: u64, dim: u64, knbn: u64, out_ids: *mut u64, out_dist: *mut f32,
+                                         out_internal: *mut u32, out_pid: *mut i32, out_counts: *mut i32) -> c_int;
 }
 
 /// The label of a point that has none (include/hnsw_b200.h HNSW_B200_LABEL_NONE): no label admits it.
@@ -310,6 +317,38 @@ impl<D: DistName> Hnsw<D> {
             }
         };
         assert_eq!(r, 0, "hnsw_b200_search_flat_labeled / _exact_labeled failed");
+        (0..nq).map(|i| (0..cnt[i] as usize).map(|j| {
+            let s = i * knbn + j;
+            Neighbour { d_id: ids[s] as usize, distance: ds[s], p_id: PointId(pid[2 * s] as u8, pid[2 * s + 1]) }
+        }).collect()).collect()
+    }
+    /// Extension: one batch, request i restricted to the points whose label is one of `sets[i]` (any order, repeats
+    /// allowed; `[LABEL_NONE]`: every point; empty: none); answer i is what search_resident returns with a filter
+    /// admitting exactly those points.  Graph search with `Some(ef)`, the exact scan with None.
+    pub fn search_label_sets(&self, datas: &[Vec<f32>], knbn: usize, ef: Option<usize>, sets: &[Vec<u32>]) -> Vec<Vec<Neighbour>> {
+        assert_eq!(datas.len(), sets.len(), "one label set per request");
+        if datas.is_empty() { return Vec::new(); }
+        let (nq, dim) = (datas.len(), datas[0].len());
+        let flat: Vec<f32> = datas.iter().flat_map(|d| d.iter().copied()).collect();
+        let mut off = vec![0u64; nq + 1];
+        for (i, s) in sets.iter().enumerate() { off[i + 1] = off[i] + s.len() as u64; }
+        let mut vals: Vec<u32> = sets.iter().flat_map(|s| s.iter().copied()).collect();
+        vals.push(LABEL_NONE);  // never empty, so never a null pointer; past every set's end
+        let mut ids = vec![0u64; nq * knbn];
+        let mut ds = vec![0f32; nq * knbn];
+        let mut pid = vec![0i32; 2 * nq * knbn];
+        let mut cnt = vec![0i32; nq];
+        let r = unsafe {
+            match ef {
+                Some(ef) => hnsw_b200_search_flat_label_sets(self.h, off.as_ptr(), vals.as_ptr(), flat.as_ptr(), nq as u64, dim as u64,
+                                                             knbn as u64, ef as u64, ids.as_mut_ptr(), ds.as_mut_ptr(),
+                                                             std::ptr::null_mut(), pid.as_mut_ptr(), cnt.as_mut_ptr()),
+                None => hnsw_b200_search_exact_label_sets(self.h, off.as_ptr(), vals.as_ptr(), flat.as_ptr(), nq as u64, dim as u64,
+                                                          knbn as u64, ids.as_mut_ptr(), ds.as_mut_ptr(), std::ptr::null_mut(),
+                                                          pid.as_mut_ptr(), cnt.as_mut_ptr()),
+            }
+        };
+        assert_eq!(r, 0, "hnsw_b200_search_flat_label_sets / _exact_label_sets failed");
         (0..nq).map(|i| (0..cnt[i] as usize).map(|j| {
             let s = i * knbn + j;
             Neighbour { d_id: ids[s] as usize, distance: ds[s], p_id: PointId(pid[2 * s] as u8, pid[2 * s + 1]) }

@@ -403,6 +403,26 @@ int hnsw_b200_search_exact_labeled(const void* h, const uint32_t* qlabels, const
                                    uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                    int32_t* out_pid, int32_t* out_counts);
 
+/* ---- Label sets: searches in which each query is restricted to the points of several labels (a user in several groups,
+ * a category filter IN (a, b, c)).  Points keep one label each; a point that belongs to several groups is labelled with
+ * the id of its distinct group set, and a query names every set id that holds one of its groups (INTEGRATION.md).
+ *   Sets: query i's set S_i is the distinct values of qset[qset_off[i], qset_off[i + 1]), in any order and with repeats.
+ *   Answers: row i is, bit for bit, what search_flat_filtered / search_exact return for query i with a resident filter
+ *     that admits exactly the points whose label is in S_i (ids, distance bits, internal ids, PointIds, count).  S_i =
+ *     {HNSW_B200_LABEL_NONE} gives the unfiltered search_flat / search_exact row, which follows the tie mode; an empty
+ *     S_i admits no point (count 0); a one-label set {L} gives the search_flat_labeled / search_exact_labeled row for L.
+ *     With statistics on, one call adds what the single-filter calls over the same queries add together.
+ *   Checks, before anything runs: qset_off must not decrease, and HNSW_B200_LABEL_NONE may not share a set with another
+ *     label; the first bad row refuses the whole call, and the message names it.  qset_off or qset NULL with nq > 0 is
+ *     refused; nq == 0 returns 0.
+ *   Handles, locks and every other argument and output: as search_flat_labeled / search_exact_labeled. */
+int hnsw_b200_search_flat_label_sets(const void* h, const uint64_t* qset_off, const uint32_t* qset, const void* queries,
+                                     uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search, uint64_t* out_ids,
+                                     float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
+int hnsw_b200_search_exact_label_sets(const void* h, const uint64_t* qset_off, const uint32_t* qset, const void* queries,
+                                      uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids, float* out_dist,
+                                      uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
+
 /* Run this handle's kernels and copies on a caller-owned CUDA stream (cudaStream_t passed as void*; NULL
  * restores the handle's own stream), e.g. so that torch.cuda.Event on torch's current stream brackets them. */
 int hnsw_b200_join(void* h);
