@@ -4,6 +4,7 @@
 #include <exception>
 #include <cstring>
 #include <mutex>
+#include <numeric>
 #include <shared_mutex>
 #include <string>
 #include <vector>
@@ -619,7 +620,6 @@ static int64_t search_call(const void* h, Via via, const char* name, const Restr
     return pass(ix, ix->search_device(rs, exact, queries, nq, knbn, ef, out.nb, out.counts, sync != 0, kernel_ms));
   if (via == HOST && nq == 0) return 0;
   if (rs.kind == Restriction::ROW_FILTERS && !rs.filters) return set_err("filters is NULL");
-  if (rs.kind == Restriction::ROW_LABELS && !rs.labels) return set_err("qlabels is NULL");
   if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset_off) return set_err("qset_off is NULL");
   if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset) return set_err("qset is NULL");
   if (!queries || !out.ids || !out.dist || !out.counts || knbn == 0 || nq == 0) return set_err("bad argument");
@@ -643,11 +643,8 @@ static Restriction filter_t(int mode, const uint64_t* ids, uint64_t nids, hnsw_b
 static Restriction resident(int64_t f) { return {Restriction::RESIDENT, 0, nullptr, 0, nullptr, nullptr, f}; }
 static Restriction resident_or_all(int64_t f) { return f == -1 ? Restriction() : resident(f); }  // -1: every point
 static Restriction row_filters(const int64_t* f) { return {Restriction::ROW_FILTERS, 0, nullptr, 0, nullptr, nullptr, -1, f}; }
-static Restriction row_labels(const uint32_t* l) {
-  return {Restriction::ROW_LABELS, 0, nullptr, 0, nullptr, nullptr, -1, nullptr, l};
-}
 static Restriction row_label_sets(const uint64_t* off, const uint32_t* set) {
-  return {Restriction::ROW_LABEL_SETS, 0, nullptr, 0, nullptr, nullptr, -1, nullptr, nullptr, off, set};
+  return {Restriction::ROW_LABEL_SETS, 0, nullptr, 0, nullptr, nullptr, -1, nullptr, off, set};
 }
 
 // hnsw_b200_search_flat and _search_flat_filtered: the filter is the FilterT arguments (filter_mode 1, 2) or one of the
@@ -779,18 +776,25 @@ int hnsw_b200_get_labels(const void* h, uint64_t first, uint64_t n, uint32_t* ou
 }
 
 // A label per query: labels[i] is the label query i is restricted to, or LABEL_NONE for none; the graph search
-// (ef_search) or the exact scan.
+// (ef_search) or the exact scan.  Query i's label set is {qlabels[i]}: offsets 0, 1, ..., nq over qlabels itself.
+static int labeled_call(const void* h, const char* name, const uint32_t* qlabels, bool exact, const void* queries,
+                        uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef, const AnswerArrays& out) {
+  if (h && nq && !qlabels) return set_err("qlabels is NULL");  // search_call answers a NULL handle and nq == 0 first
+  std::vector<uint64_t> off(nq + 1);
+  std::iota(off.begin(), off.end(), (uint64_t)0);
+  return (int)search_call(h, HOST, name, row_label_sets(off.data(), qlabels), exact, queries, nq, dim, knbn, ef, out);
+}
 int hnsw_b200_search_flat_labeled(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim,
                                   uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                   uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_flat_labeled", row_labels(qlabels), false, queries, nq, dim, knbn, ef_search,
-                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return labeled_call(h, "search_flat_labeled", qlabels, false, queries, nq, dim, knbn, ef_search,
+                      columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 int hnsw_b200_search_exact_labeled(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim,
                                    uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                    int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_exact_labeled", row_labels(qlabels), true, queries, nq, dim, knbn, 0,
-                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return labeled_call(h, "search_exact_labeled", qlabels, true, queries, nq, dim, knbn, 0,
+                      columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 
 // A label set per query: query i is restricted to the points whose label is one of qset[qset_off[i], qset_off[i + 1])
@@ -818,12 +822,7 @@ int64_t hnsw_b200_filter_new(const void* h, int filter_mode, const uint64_t* fil
                              hnsw_b200_filter_fn fn, void* ctx) {
   HB_HS(h);  // shared: the points cannot change while the bitmap is made
   HB_NOT_VIEW(ix);
-  if (ix->parts) {
-    HB_PARTS_SHARED(ix);
-    const int64_t id = ix->new_filter(filter_mode, filter_ids, nfilter, fn, ctx);
-    if (id < 0) g_err = ix->err();
-    return id;
-  }
+  HB_PARTS_SHARED_IF(ix);
   const int64_t id = ix->new_filter(filter_mode, filter_ids, nfilter, fn, ctx);
   if (id < 0) g_err = ix->err();
   return id;

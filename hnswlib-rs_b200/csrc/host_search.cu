@@ -12,7 +12,6 @@
 //     each replica's leg by that replica's worker.
 #include <algorithm>
 #include <cstring>
-#include <map>
 #include <numeric>
 #include <set>
 
@@ -197,20 +196,26 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
       }
     }
   }
-  // run u of leg l under `key`, a resident filter, a label or a label set
-  auto restrict_run = [&](const Leg& l, int64_t key, LegPlan::Run& u) {
+  // run u of leg l under `key`, a resident filter or a label set; exact: its slices appended to the plan's
+  auto restrict_run = [&](Leg& l, int64_t key, LegPlan::Run& u) {
     if (rs.kind == Restriction::FILTER_T) {
       u.host_bits = bits[l.part].data();
       return 0;
     }
+    std::vector<ExactScan>& slices = l.plan.slices;
+    u.slice = slices.size();
+    int r;
     if (rs.kind == Restriction::ROW_LABEL_SETS) {
       u.set = sets->values.data() + sets->off[key];
       u.nset = (uint32_t)(sets->off[key + 1] - sets->off[key]);
-      return exact ? l.rx->label_set_scan(u.set, u.nset, u.slices) : 0;
+      r = exact ? l.rx->label_set_scan(u.set, u.nset, slices) : 0;
+    } else {
+      ExactScan list;
+      r = filters.use(key, l.part, P, l.rx, &u.bits, exact ? &list : nullptr);
+      if (!r && exact) slices.push_back(list);
     }
-    if (rs.kind != Restriction::ROW_LABELS) return filters.use(key, l.part, P, l.rx, &u.bits, exact ? &u.scan : nullptr);
-    u.label = (uint32_t)key;
-    return exact ? l.rx->label_scan(u.label, &u.scan) : 0;
+    u.nslices = slices.size() - u.slice;
+    return r;
   };
   int r = 0;
   for (Leg* l = legs; l < legs + n; ++l) {  // every leg, so that the caller reports the failure it chooses
@@ -229,12 +234,12 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
     const int64_t* key = sorted.data() + l->first;
     while (pl.plain < l->count && key[pl.plain] == -1) ++pl.plain;
     // labels: the leg's own, or on a replica its copy of the handle's, made current first
-    pl.label_sets = rs.kind == Restriction::ROW_LABEL_SETS;
-    if (rs.by_label() && pl.plain < l->count && l->rx->labels_on_device(parts ? l->rx : this, &pl.labels)) {
+    if (rs.kind == Restriction::ROW_LABEL_SETS && pl.plain < l->count &&
+        l->rx->labels_on_device(parts ? l->rx : this, &pl.labels)) {
       r = l->rc = -1;
       continue;
     }
-    for (size_t j = pl.plain, e; j < l->count; j = e) {  // one run per filter, label or label set
+    for (size_t j = pl.plain, e; j < l->count; j = e) {  // one run per filter or label set
       for (e = j + 1; e < l->count && key[e] == key[j];) ++e;
       LegPlan::Run u{j, e - j};
       if (restrict_run(*l, key[j], u)) {
@@ -247,65 +252,72 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
   return r;
 }
 
-// The label sets of rows [0, nq): each row's values made ascending without repeats and checked, the distinct sets into
-// `sets` in lexicographic order, and key[i] the set of row i, or -1 for {LABEL_NONE}.  The first row whose offsets
-// decrease or whose set holds LABEL_NONE with another label refuses the call.
-static int label_set_keys(const Restriction& rs, size_t nq, std::vector<int64_t>& key, LabelSets& sets, std::string& err) {
-  std::map<std::vector<uint32_t>, int64_t> distinct;
-  std::vector<const std::vector<uint32_t>*> row_set(nq, nullptr);
-  std::vector<uint32_t> v;
+// sort_rows for label sets, or the refusal of the first bad row: the rows copied into one array (a longer row sorted and
+// de-duplicated), their indices sorted once, and one walk over them that numbers the distinct sets into `sets`
+static std::string label_set_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm,
+                                  std::vector<int64_t>& sorted, LabelSets& sets) {
+  std::vector<uint32_t> v;  // row i's set is v[at[i], at[i + 1])
+  v.reserve(nq);
+  std::vector<size_t> at(nq + 1);
+  // key[i]: -1 for {LABEL_NONE} (the only accepted set that holds it), 0 for the empty set, else 1 + the set's smallest
+  // value; rows of one key are ordered by the rest of their sets, which only rows of several labels have (`longer`)
+  std::vector<int64_t> key(nq);
+  bool longer = false;
   for (size_t i = 0; i < nq; ++i) {
     const uint64_t lo = rs.qset_off[i], hi = rs.qset_off[i + 1];
-    if (hi < lo) {
-      err = "label set " + std::to_string(i) + ": qset_off[" + std::to_string(i + 1) + "] = " + std::to_string(hi) +
-            " is below qset_off[" + std::to_string(i) + "] = " + std::to_string(lo);
-      return -1;
+    if (hi < lo)
+      return "label set " + std::to_string(i) + ": qset_off[" + std::to_string(i + 1) + "] = " + std::to_string(hi) +
+             " is below qset_off[" + std::to_string(i) + "] = " + std::to_string(lo);
+    at[i] = v.size();
+    v.insert(v.end(), rs.qset + lo, rs.qset + hi);
+    if (hi - lo > 1) {
+      std::sort(v.begin() + at[i], v.end());
+      v.erase(std::unique(v.begin() + at[i], v.end()), v.end());
+      if (v.size() - at[i] > 1 && v.back() == LABEL_NONE)
+        return "label set " + std::to_string(i) + " holds LABEL_NONE together with another label";
+      longer |= v.size() - at[i] > 1;
     }
-    v.assign(rs.qset + lo, rs.qset + hi);
-    std::sort(v.begin(), v.end());
-    v.erase(std::unique(v.begin(), v.end()), v.end());
-    if (!v.empty() && v.back() == LABEL_NONE) {
-      if (v.size() > 1) {
-        err = "label set " + std::to_string(i) + " holds LABEL_NONE together with another label";
-        return -1;
-      }
-      continue;  // {LABEL_NONE}: every point
-    }
-    row_set[i] = &distinct.emplace(v, 0).first->first;
+    key[i] = at[i] == v.size() ? 0 : v[at[i]] == LABEL_NONE ? -1 : 1 + (int64_t)v[at[i]];
   }
+  at[nq] = v.size();
+  auto less = [&](size_t a, size_t b) {
+    if (key[a] != key[b] || !longer || key[a] <= 0) return key[a] < key[b];
+    return std::lexicographical_compare(v.begin() + at[a] + 1, v.begin() + at[a + 1], v.begin() + at[b] + 1,
+                                        v.begin() + at[b + 1]);
+  };
+  perm.resize(nq);
+  std::iota(perm.begin(), perm.end(), (size_t)0);
+  std::stable_sort(perm.begin(), perm.end(), less);
+  sorted.resize(nq);
   sets.values.clear();
   sets.off.assign(1, 0);
-  for (auto& d : distinct) {
-    d.second = (int64_t)sets.off.size() - 1;
-    sets.values.insert(sets.values.end(), d.first.begin(), d.first.end());
-    sets.off.push_back(sets.values.size());
+  for (size_t j = 0; j < nq; ++j) {
+    const size_t i = perm[j];
+    if (key[i] == -1) {
+      sorted[j] = -1;
+      continue;
+    }
+    if (j == 0 || less(perm[j - 1], i)) {  // a set the sorted rows have not had yet
+      sets.values.insert(sets.values.end(), v.begin() + at[i], v.begin() + at[i + 1]);
+      sets.off.push_back(sets.values.size());
+    }
+    sorted[j] = (int64_t)sets.off.size() - 2;
   }
-  key.resize(nq);
-  for (size_t i = 0; i < nq; ++i) key[i] = row_set[i] ? distinct.find(*row_set[i])->second : -1;
-  return 0;
+  return {};
 }
 
 // Every filter is checked on every partition before anything runs, so that a bad entry refuses the whole call, named by
-// its first position.  The sort is stable: rows of one filter keep their order, and -1 (no filter) sorts first.  A label
-// needs no check; LABEL_NONE sorts first as -1.  A label set is checked and made canonical (label_set_keys); {LABEL_NONE}
-// sorts first as -1.
+// its first position.  The sort is stable: rows of one filter keep their order, and -1 (no filter) sorts first.
 int Index::sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm, std::vector<int64_t>& sorted,
                      LabelSets& sets) {
-  const int P = parts ? parts->count() : 1;
-  const bool labels = rs.by_label();
-  std::vector<int64_t> key;
-  const int64_t* fid = rs.filters;
-  if (rs.kind == Restriction::ROW_LABELS) {
-    key.resize(nq);
-    for (size_t i = 0; i < nq; ++i) key[i] = rs.labels[i] == LABEL_NONE ? -1 : (int64_t)rs.labels[i];
-    fid = key.data();
-  } else if (rs.kind == Restriction::ROW_LABEL_SETS) {
-    std::string e;
-    if (label_set_keys(rs, nq, key, sets, e)) return fail(e);
-    fid = key.data();
+  if (rs.kind == Restriction::ROW_LABEL_SETS) {
+    const std::string e = label_set_rows(rs, nq, perm, sorted, sets);
+    return e.empty() ? 0 : fail(e);
   }
+  const int P = parts ? parts->count() : 1;
+  const int64_t* fid = rs.filters;
   std::set<int64_t> checked;
-  for (size_t i = 0; !labels && i < nq; ++i) {
+  for (size_t i = 0; i < nq; ++i) {
     if (fid[i] == -1 || checked.count(fid[i])) continue;
     for (int p = 0; p < P; ++p) {
       Index* rx = parts ? parts->part(p) : this;
@@ -367,7 +379,7 @@ int Index::end_leg(Leg& l, size_t k, const AnswerArrays& out) {
 
 // ------------------------------------------------------------------------------------------------ batches
 // The batch `call` planned into t's legs, each with its plan; `b` is the batch as the legs run it.  A per-row restriction:
-// the batch is planned over the rows sorted by filter or label, gathered through row pointers, and each answer goes back
+// the batch is planned over the rows sorted by filter or label set, gathered through row pointers, and each answer goes back
 // to its caller's row.  A leg that could not have its plan is reported in leg order, or the replicas' first.
 int Index::prepare_batch(const HostBatch& call, HostBatch& b, Ticket& t, bool replicas_first) {
   if (parts && dim != 0 && call.d != dim) return fail("query length differs from the index dimension");

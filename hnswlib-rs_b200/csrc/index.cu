@@ -891,11 +891,12 @@ int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** 
 }
 
 // A single bitmap run goes to the launch as its filter bits (a FilterT's host bits uploaded into the context first), as
-// a batch-wide filter does; several as a table of their bitmaps and each row's entry in it, label runs as the label
-// array and each row's label, and label-set runs as the label array, the sets' values and each row's (offset, count) in
-// them, uploaded into the context ahead of the launches.  Exact: a group of every point for the unrestricted rows, and
-// one per run; a label set scans its one CSR slice, or its slices copied one after the other into the context (a point
-// has one label, so they are disjoint, and the exact scan orders by (distance, id), so their order does not matter).
+// a batch-wide filter does; several as a table of their bitmaps and each row's entry in it.  Label-set runs go as the
+// label array and each row's label when every set is one label (the kernel compares labels), else each row's (offset,
+// count) in the sets' values, uploaded into the context ahead of the launches.  Exact: a group of every point for the
+// unrestricted rows, and one per run; a run of one slice scans it in place, any other its slices copied one after the
+// other into the context (a point has one label, so a label set's slices are disjoint, and the exact scan orders by
+// (distance, id), so their order does not matter).
 int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
   cudaStream_t st = c.stream;
   int r;
@@ -904,33 +905,37 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
   if (plan.exact) {
     if (plan.plain) L.groups.push_back(ExactGroup{0, plan.plain, ExactScan()});
     size_t joined = 0;  // ids copied into the context
-    if (plan.label_sets) {
-      for (const LegPlan::Run& u : plan.runs)
-        if (u.slices.size() != 1)
-          for (const ExactScan& x : u.slices) joined += x.n;
-      if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, std::max<size_t>(joined, 1) * 4, st))) return r;  // never null
-    }
+    for (const LegPlan::Run& u : plan.runs)
+      if (u.nslices != 1)
+        for (size_t s = u.slice; s < u.slice + u.nslices; ++s) joined += plan.slices[s].n;
+    // never null, also for a run of no points: a null list means every point
+    if (!plan.runs.empty() && (r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, std::max<size_t>(joined, 1) * 4, st)))
+      return r;
     uint32_t* at = (uint32_t*)c.d_fbits;
     for (const LegPlan::Run& u : plan.runs) {
-      ExactScan scan = u.scan;
-      if (plan.label_sets && u.slices.size() == 1) {
-        scan = u.slices[0];
-      } else if (plan.label_sets) {
-        scan = ExactScan{at, 0};
-        for (const ExactScan& x : u.slices) {
+      ExactScan scan{at, 0};
+      if (u.nslices == 1)
+        scan = plan.slices[u.slice];
+      else
+        for (size_t s = u.slice; s < u.slice + u.nslices; ++s) {
+          const ExactScan& x = plan.slices[s];
           HB_CUDA(cudaMemcpyAsync(at, x.ids, x.n * 4, cudaMemcpyDeviceToDevice, st));
           at += x.n;
           scan.n += x.n;
         }
-      }
       L.groups.push_back(ExactGroup{u.first, u.count, scan});
     }
     return 0;
   }
   if (plan.runs.empty()) return 0;
-  if (plan.label_sets) {
-    std::vector<uint32_t> sel, vals;  // sel: (offset, count) per row
+  if (plan.labels) {
+    const bool single = std::all_of(plan.runs.begin(), plan.runs.end(), [](const LegPlan::Run& u) { return u.nset == 1; });
+    std::vector<uint32_t> sel, vals;  // sel: the label, or (offset, count), per row
     for (const LegPlan::Run& u : plan.runs) {
+      if (single) {
+        sel.insert(sel.end(), u.count, u.set[0]);
+        continue;
+      }
       if (vals.size() >= LABEL_NONE - u.nset) return fail("label sets: too many distinct labels in one batch");
       for (size_t j = 0; j < u.count; ++j) sel.insert(sel.end(), {(uint32_t)vals.size(), u.nset});
       vals.insert(vals.end(), u.set, u.set + u.nset);
@@ -940,11 +945,11 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
     HB_CUDA(cudaMemcpyAsync(c.d_fbits, sel.data(), sel.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
     if (vb) HB_CUDA(cudaMemcpyAsync((char*)c.d_fbits + sb, vals.data(), vb, cudaMemcpyHostToDevice, st));
     L.filter.sel = (const uint32_t*)c.d_fbits;
-    L.filter.sets = (const uint32_t*)((char*)c.d_fbits + sb);
+    L.filter.sets = single ? nullptr : (const uint32_t*)((char*)c.d_fbits + sb);
     L.filter.labels = plan.labels;
     return 0;
   }
-  if (plan.runs.size() == 1 && !plan.labels) {
+  if (plan.runs.size() == 1) {
     L.filter.bits = plan.runs[0].bits;  // a resident filter: already on this device
     if (plan.runs[0].host_bits) {
       const size_t fb = ((n + 31) / 32) * 4;
@@ -957,16 +962,15 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
   std::vector<const uint32_t*> table;
   std::vector<uint32_t> sel;
   for (const LegPlan::Run& u : plan.runs) {
-    sel.insert(sel.end(), u.count, plan.labels ? u.label : (uint32_t)table.size());
-    if (!plan.labels) table.push_back(u.bits);
+    sel.insert(sel.end(), u.count, (uint32_t)table.size());
+    table.push_back(u.bits);
   }
   const size_t tb = round128(table.size() * sizeof(void*)), sb = sel.size() * sizeof(uint32_t);
   if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, tb + sb, st))) return r;
-  if (tb) HB_CUDA(cudaMemcpyAsync(c.d_fbits, table.data(), table.size() * sizeof(void*), cudaMemcpyHostToDevice, st));
+  HB_CUDA(cudaMemcpyAsync(c.d_fbits, table.data(), table.size() * sizeof(void*), cudaMemcpyHostToDevice, st));
   HB_CUDA(cudaMemcpyAsync((char*)c.d_fbits + tb, sel.data(), sb, cudaMemcpyHostToDevice, st));
-  L.filter.table = plan.labels ? nullptr : (const uint32_t* const*)c.d_fbits;
+  L.filter.table = (const uint32_t* const*)c.d_fbits;
   L.filter.sel = (const uint32_t*)((char*)c.d_fbits + tb);
-  L.filter.labels = plan.labels;
   return 0;
 }
 

@@ -209,10 +209,10 @@ struct AnswerArrays {
 
 // What the rows of a batch may return: every point (NONE); the points a FilterT admits (FILTER_T: `mode` 1 sorted
 // origin-id list, 2 callback, as make_filter_bits reads it); one resident filter for every row (RESIDENT); a resident
-// filter per row, -1 = none (ROW_FILTERS); a label per row, LABEL_NONE = none (ROW_LABELS); or a set of labels per row,
-// row i's the values qset[qset_off[i], qset_off[i + 1]) in any order and with repeats, {LABEL_NONE} = none (ROW_LABEL_SETS)
+// filter per row, -1 = none (ROW_FILTERS); or a set of labels per row (a label per row: sets of one), row i's the values
+// qset[qset_off[i], qset_off[i + 1]) in any order and with repeats, {LABEL_NONE} = none (ROW_LABEL_SETS)
 struct Restriction {
-  enum Kind { NONE, FILTER_T, RESIDENT, ROW_FILTERS, ROW_LABELS, ROW_LABEL_SETS } kind = NONE;
+  enum Kind { NONE, FILTER_T, RESIDENT, ROW_FILTERS, ROW_LABEL_SETS } kind = NONE;
   int mode = 0;
   const uint64_t* ids = nullptr;
   size_t nids = 0;
@@ -220,11 +220,9 @@ struct Restriction {
   void* ctx = nullptr;
   int64_t resident = -1;
   const int64_t* filters = nullptr;  // [nq]
-  const uint32_t* labels = nullptr;  // [nq]
   const uint64_t* qset_off = nullptr;  // [nq + 1]
   const uint32_t* qset = nullptr;
-  bool per_row() const { return kind == ROW_FILTERS || kind == ROW_LABELS || kind == ROW_LABEL_SETS; }
-  bool by_label() const { return kind == ROW_LABELS || kind == ROW_LABEL_SETS; }
+  bool per_row() const { return kind == ROW_FILTERS || kind == ROW_LABEL_SETS; }
 };
 
 // The distinct label sets of a ROW_LABEL_SETS batch (Index::sort_rows): set j is values[off[j], off[j + 1]), ascending
@@ -248,27 +246,24 @@ struct HostBatch {
 };
 
 // A leg's restriction (Index::resolve): its rows [0, plain) are unrestricted, and `runs` cover the rest, each a range of
-// consecutive rows under one restriction.  A run is a resident filter's bitmap on the leg's device, a FilterT's host bits
-// (uploaded into the context when the leg begins), a label on `labels` (the label array on the leg's device), or a label
-// set (label_sets) on `labels`; in an exact batch, the points it scans, and for a label set the slices of the label CSR
-// they are the union of, joined into one list in the context when there are several (stage_plan).  A batch-wide filter
-// is a plan with no prefix and one run over every row.
+// consecutive rows under one restriction: a bitmap (a resident filter's on the leg's device, or a FilterT's host bits,
+// uploaded into the context when the leg begins) or a label set on `labels` (the label array on the leg's device).  In
+// an exact batch its points are slices [slice, slice + nslices): a filter's id list, or a label set's CSR slices.  A
+// batch-wide filter is a plan with no prefix and one run over every row.
 struct LegPlan {
   struct Run {
     size_t first, count;
     const uint32_t* bits = nullptr;
     const uint32_t* host_bits = nullptr;
-    uint32_t label = LABEL_NONE;
-    const uint32_t* set = nullptr;  // label_sets: the run's set, nset values of a LabelSets
+    const uint32_t* set = nullptr;  // the run's label set, nset values of a LabelSets
     uint32_t nset = 0;
-    ExactScan scan;
-    std::vector<ExactScan> slices;
+    size_t slice = 0, nslices = 0;
   };
   bool exact = false;
   size_t plain = 0;
   std::vector<Run> runs;
+  std::vector<ExactScan> slices;
   const uint32_t* labels = nullptr;
-  bool label_sets = false;
 };
 
 // One Index's part of a batch: queries [first, first + count) searched on rx (the handle, a replica, or partition `part`)
@@ -346,19 +341,19 @@ class Index {
   void drain_pending() const {
     while (pending_.load() != 0) std::this_thread::yield();
   }
-  // the plan of each of legs[0, n) under `rs`; `sorted` holds a per-row restriction's keys (a filter id, a label or a
-  // set of `sets`, -1: none) in the order the legs run the rows (sort_rows).  A FilterT's host bits are made on the
-  // calling thread once per partition (a replica shares the handle's internal ids, and so its bits) into `bits`; a
-  // resident filter is its copy on each leg's device; a label or label set needs the label array on the leg's device.
-  // `exact`: each run's ExactScan (a filter's id list or a label's CSR slice on the leg's device; a label set's slices).
-  // Nonzero when a leg could not have its plan; that leg's rc is set (legs_fail reports it).
+  // the plan of each of legs[0, n) under `rs`; `sorted` holds a per-row restriction's keys (a filter id or a set of
+  // `sets`, -1: none) in the order the legs run the rows (sort_rows).  A FilterT's host bits are made on the calling
+  // thread once per partition (a replica shares the handle's internal ids, and so its bits) into `bits`; a resident
+  // filter is its copy on each leg's device; a label set needs the label array on the leg's device.  `exact`: each
+  // run's slices (a filter's id list on the leg's device; a label set's CSR slices).  Nonzero when a leg could not have
+  // its plan; that leg's rc is set (legs_fail reports it).
   int resolve(const Restriction& rs, bool exact, const std::vector<int64_t>& sorted, Leg* legs, size_t n,
               std::vector<std::vector<uint32_t>>& bits, const LabelSets* sets = nullptr);
   // a per-row restriction: every filter of rs.filters[0, nq) is -1 or a live, current filter of this handle (else the
-  // first bad position is refused), and `perm` orders the rows stably by filter, the unfiltered ones first; labels by
-  // label, LABEL_NONE first; label sets, each made ascending without repeats into `sets`, by set, {LABEL_NONE} first
-  // (a decreasing offset, or LABEL_NONE with another label, refuses the first such row).  sorted[j]: the filter, label
-  // or set of sorted row j (-1: none).
+  // first bad position is refused), and `perm` orders the rows stably by filter, the unfiltered ones first; label sets,
+  // each made ascending without repeats into `sets`, by set in lexicographic order, {LABEL_NONE} first (a decreasing
+  // offset, or LABEL_NONE with another label, refuses the first such row).  sorted[j]: the filter or set of sorted row
+  // j (-1: none).
   int sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm, std::vector<int64_t>& sorted,
                 LabelSets& sets);
 
@@ -370,10 +365,8 @@ class Index {
   // the label array on this Index's device, as current as `src`'s (a replica's copy of the handle's labels, refreshed
   // when src's changed; src == this: its own)
   int labels_on_device(const Index* src, const uint32_t** d_labels);
-  // the exact scan of the points labelled `label`: a slice of this Index's label CSR, rebuilt when the labels changed
-  int label_scan(uint32_t label, ExactScan* scan);
-  // the points whose label is one of set[0, nset) (ascending): one slice of the label CSR per label that some point
-  // carries, slices that follow each other in the CSR joined into one
+  // the points whose label is one of set[0, nset) (ascending), appended to `slices`: one slice of the label CSR (rebuilt
+  // when the labels changed) per label that some point carries, slices that follow each other in the CSR joined
   int label_set_scan(const uint32_t* set, size_t nset, std::vector<ExactScan>& slices);
   // device queries in, device answers out; the restriction is none or a resident filter.  `exact`: the exact scan (ef
   // unused).

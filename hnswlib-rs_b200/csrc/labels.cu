@@ -1,8 +1,8 @@
 // Point labels (index.h "point labels"): one u32 per point, next to the graph, that a search can restrict each query to.
-// No kernel of its own.  A graph search with a label per query runs the filtered query kernel (filter.cu), whose
-// admission test reads the label array instead of a bitmap, or with a label set per query, looks the point's label up in
-// the query's set.  An exact search runs the exact scan over one slice per label of a CSR of internal ids grouped by
-// label, made on the host; a label set's points are its labels' slices, joined into one list by copies (stage_plan).
+// No kernel of its own.  A graph search with a label set per query runs the filtered query kernel (filter.cu), whose
+// admission test reads the label array and looks the point's label up in the query's set (or compares it, when every
+// set is one label).  An exact search scans a label set's slices of a CSR of internal ids grouped by label, made on
+// the host, joined into one list by copies when there are several (stage_plan).
 #include <algorithm>
 
 #include "index.h"
@@ -43,7 +43,7 @@ int Index::labels_on_device(const Index* src, const uint32_t** d_labels) {
   return 0;
 }
 
-int Index::label_scan(uint32_t label, ExactScan* scan) {
+int Index::label_set_scan(const uint32_t* set, size_t nset, std::vector<ExactScan>& slices) {
   std::lock_guard<std::mutex> lk(label_mu_);
   LabelCsr& c = label_csr_;
   if (c.version != label_version) {
@@ -88,21 +88,12 @@ int Index::label_scan(uint32_t label, ExactScan* scan) {
     }
     c.version = label_version;
   }
-  auto g = c.groups.find(label);
-  const uint32_t off = g == c.groups.end() ? 0 : g->second.first, cnt = g == c.groups.end() ? 0 : g->second.second;
-  scan->ids = (const uint32_t*)c.d_ids + off;
-  scan->n = cnt;
-  return 0;
-}
-
-int Index::label_set_scan(const uint32_t* set, size_t nset, std::vector<ExactScan>& slices) {
-  slices.clear();
+  const size_t first = slices.size();
   for (size_t j = 0; j < nset; ++j) {
-    ExactScan s;
-    int r;
-    if ((r = label_scan(set[j], &s))) return r;
-    if (s.n == 0) continue;
-    if (!slices.empty() && slices.back().ids + slices.back().n == s.ids)
+    auto g = c.groups.find(set[j]);  // a group holds at least one point
+    if (g == c.groups.end()) continue;
+    const ExactScan s{(const uint32_t*)c.d_ids + g->second.first, g->second.second};
+    if (slices.size() > first && slices.back().ids + slices.back().n == s.ids)
       slices.back().n += s.n;
     else
       slices.push_back(s);
