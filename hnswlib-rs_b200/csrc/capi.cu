@@ -452,6 +452,20 @@ int hnsw_b200_last_kernel(char* buf, size_t cap) {
   return (int)len;
 }
 
+int hnsw_b200_last_kernel_shape(int64_t* out3) {
+  if (!out3) return set_err("NULL output");
+  out3[0] = out3[1] = out3[2] = 0;
+  if (!hb::last_launched_kernel) return 0;
+  int bps = 0;
+  cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, hb::last_launched_kernel, hb::last_launched_threads,
+                                                                hb::last_launched_smem);
+  if (e != cudaSuccess) return set_err(std::string("cudaOccupancyMaxActiveBlocksPerMultiprocessor: ") + cudaGetErrorString(e));
+  out3[0] = (int64_t)hb::last_launched_smem;
+  out3[1] = hb::last_launched_threads;
+  out3[2] = bps;
+  return 1;
+}
+
 int hnsw_b200_device_count(void) {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;

@@ -562,6 +562,34 @@ __device__ __forceinline__ void warp_dists_staged(const uint4* __restrict__ vec,
 }
 
 // ------------------------------------------------------------------------------------------------
+// Shared memory through 32-bit window addresses (the lean kernel, and a visited first stage in shared memory).  The
+// addresses are produced once by pin(), an opaque move the compiler can neither see through nor re-derive from the
+// thread index inside the loop (it did, at ~6 instructions and one S2R per access, when the addresses were ordinary
+// pointers).
+__device__ __forceinline__ uint32_t pin(uint32_t v) {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %1;" : "=r"(r) : "r"(v));
+  return r;
+}
+__device__ __forceinline__ uint64_t lds64(uint32_t a) {
+  uint64_t v;
+  asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void sts64(uint32_t a, uint64_t v) { asm volatile("st.shared.u64 [%0], %1;" ::"r"(a), "l"(v) : "memory"); }
+__device__ __forceinline__ uint32_t lds32(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+__device__ __forceinline__ uint4 lds128(uint32_t a) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a) : "memory");
+  return v;
+}
+
+// ------------------------------------------------------------------------------------------------
 // Visited set: one open-addressing table per resident warp ("warp slot") in global memory.  Entry =
 // (epoch << id_bits) | id; an entry whose epoch differs from the current one is free, so a new search only bumps the
 // epoch instead of clearing.  Exact (no false positives).
@@ -571,9 +599,11 @@ __device__ __forceinline__ void warp_dists_staged(const uint4* __restrict__ vec,
 // hot in L2 is about (slots x small) entries, not (slots x cap).  At the SIFT1M shape (M = 16, ef = 64: cap = 8192,
 // 21 one-warp CTAs x 132 SMs = 2 772 slots) full-size tables alone were 91 MB per search context against a 50 MB L2;
 // a search touched every line of its 32 KB table, so table lines were evicted between probes and re-read from HBM, and
-// they crowded out the rows and adjacency lists the kernel prefetches for itself.
+// they crowded out the rows and adjacency lists the kernel prefetches for itself.  Global first stages still kept ~23 MB
+// per context in L2; the lean kernel therefore keeps its first stage in shared memory (FirstStage::Shared), where a
+// query that never moves touches no table line in L2 at all.
 struct VisitedCfg {
-  uint32_t* tables;   // [n_slots][small + cap]: first stage, then full stage
+  uint32_t* tables;   // [n_slots][small + cap]: first stage (unused when it lives in shared memory), then full stage
   uint32_t* epochs;   // [n_slots] persisted across launches
   uint32_t cap;       // full stage, power of two
   int shift;          // 32 - log2(cap)
@@ -582,49 +612,106 @@ struct VisitedCfg {
   int id_bits;        // bits needed for ids
 };
 
+// Where a slot's first stage lives.  Global: in the slot's table, before the full stage (every kernel but the lean one).
+// Shared: in a window of the warp's shared memory, `small` words at a 32-bit shared address, zeroed when the warp starts;
+// the full stage stays in the slot's global table.  A window does not outlive its CTA, so its entries never carry over
+// between launches; zero is never a live entry (begin() makes the epoch >= 1).
+enum class FirstStage { Global, Shared };
+
 // The state of one warp's set is what changes during a search: the current stage (table pointer and hash shift; its
 // capacity is 2^(32 - shift)), epoch and insert count.  The stage sizes and the epoch / id split are read from the
 // launch's VisitedCfg (kernel parameters) where they are used.  Every function is warp-collective and takes the caller's
-// lane (the lean kernel pins it, see lean_common.cuh pin()).
-struct Visited {
-  uint32_t* tab;  // current stage: the slot's first stage, or its full stage (= first + small)
+// lane (the lean kernel pins it, see pin()).  With FS = Shared the current stage is the window while shift != c.shift (a
+// warp-uniform test), else the global full stage.
+template <FirstStage FS>
+struct VisitedWindow {};  // Global: no window, so that the state stays four words
+template <>
+struct VisitedWindow<FirstStage::Shared> {
+  uint32_t win;  // shared address of the first-stage window
+};
+template <FirstStage FS>
+struct VisitedT : VisitedWindow<FS> {
+  static constexpr bool WINDOW = FS == FirstStage::Shared;
+  uint32_t* tab;  // Global: current stage, the slot's first stage or its full stage (= first + small).  Shared: full stage
   int shift;
   uint32_t epoch;
   uint32_t used;  // insertions of the current search (warp-uniform)
 
   __device__ __forceinline__ void init(const VisitedCfg& c, uint32_t slot) {
+    static_assert(!WINDOW, "a shared first stage is initialised with its window");
     tab = c.tables + (size_t)slot * (c.small + c.cap);
     shift = c.small_shift;
     epoch = c.epochs[slot];
     used = 0;
+  }
+  // Shared: `window` holds c.small words; they are zeroed here, once per warp
+  __device__ __forceinline__ void init(const VisitedCfg& c, uint32_t slot, uint32_t window, int lane) {
+    static_assert(WINDOW, "a global first stage has no window");
+    tab = c.tables + (size_t)slot * (c.small + c.cap) + c.small;
+    shift = c.small_shift;
+    epoch = c.epochs[slot];
+    used = 0;
+    this->win = window;
+    for (uint32_t i = lane; i < c.small; i += 32) sts32(window + 4 * i, 0u);
+    __syncwarp();
   }
   __device__ __forceinline__ void save(const VisitedCfg& c, uint32_t slot, int lane) const {
     if (lane == 0) c.epochs[slot] = epoch;
   }
   __device__ __forceinline__ uint32_t mask() const { return 0xFFFFFFFFu >> shift; }
   __device__ __forceinline__ uint32_t home(uint32_t id) const { return (id * 2654435761u) >> shift; }
+  // Entry h of the current stage.  With a window the stage is chosen by predicated instructions, not a branch, so that
+  // the probe loops and the lean kernel's look-ahead (issued between row loads and their use) stay straight-line code.
+  __device__ __forceinline__ uint32_t probe(const VisitedCfg& c, uint32_t h, uint64_t pol_keep) const {
+    if constexpr (WINDOW) {
+      uint32_t v;
+      asm volatile(
+          "{\n .reg .pred w;\n setp.ne.s32 w, %1, %2;\n @w ld.shared.u32 %0, [%3];\n"
+          " @!w ld.global.cg.L2::cache_hint.u32 %0, [%4], %5;\n}"
+          : "=r"(v)
+          : "r"(shift), "r"(c.shift), "r"(this->win + 4 * h), "l"(tab + h), "l"(pol_keep)
+          : "memory");
+      return v;
+    }
+    return ld_keep(tab + h, pol_keep);
+  }
+  __device__ __forceinline__ void put(const VisitedCfg& c, uint32_t h, uint32_t v, uint64_t pol_keep) const {
+    if constexpr (WINDOW) {
+      asm volatile(
+          "{\n .reg .pred w;\n setp.ne.s32 w, %0, %1;\n @w st.shared.u32 [%2], %4;\n"
+          " @!w st.global.cg.L2::cache_hint.u32 [%3], %4, %5;\n}" ::"r"(shift),
+          "r"(c.shift), "r"(this->win + 4 * h), "l"(tab + h), "r"(v), "l"(pol_keep)
+          : "memory");
+      return;
+    }
+    st_keep(tab + h, v, pol_keep);
+  }
   // Start a new search from `entry` (hnsw.rs:955-956) in the first stage: bump the epoch instead of clearing the tables
   // (both stages are cleared only when the epoch wraps), then record the entry.  The stage holds nothing of the new
   // epoch yet, so the entry's home slot is free.
   __device__ __forceinline__ void begin(const VisitedCfg& c, uint32_t entry, int lane) {
-    if (shift != c.small_shift) tab -= c.small;  // the last search moved to the full stage
+    if (!WINDOW && shift != c.small_shift) tab -= c.small;  // the last search moved to the full stage
     shift = c.small_shift;
     const uint32_t epoch_max = (c.id_bits >= 32) ? 0u : ((1u << (32 - c.id_bits)) - 1u);
     if (epoch >= epoch_max) {
-      for (uint32_t i = lane; i < c.small + c.cap; i += 32) tab[i] = 0u;
+      // the whole global slot, also an unused global first stage, which a kernel with FS = Global may use later
+      uint32_t* slot_tab = WINDOW ? tab - c.small : tab;
+      for (uint32_t i = lane; i < c.small + c.cap; i += 32) slot_tab[i] = 0u;
+      if constexpr (WINDOW)
+        for (uint32_t i = lane; i < c.small; i += 32) sts32(this->win + 4 * i, 0u);
       epoch = 0;
     }
     epoch += 1;
     used = 1;
     __syncwarp();
-    if (lane == 0) st_keep(tab + home(entry), (epoch << c.id_bits) | entry, l2_policy_evict_last());
+    if (lane == 0) put(c, home(entry), (epoch << c.id_bits) | entry, l2_policy_evict_last());
     __syncwarp();
   }
   // Test-and-set of up to 32 ids (one per lane, `valid` lanes only).  Returns true in the lanes whose id was not yet in
   // the set (it is afterwards).  The table is private to this warp, so no atomics are needed: lanes that find the same
-  // free slot in the same round elect the lowest lane (match_any); the others probe on.  One L2 round trip per round,
-  // and almost always one round.  The first probe may have been done ahead of time (`pre`: slot pre_h was read as
-  // pre_cv after the last store to the table).
+  // free slot in the same round elect the lowest lane (match_any); the others probe on.  One L2 round trip per round
+  // (one shared-memory load in a window), and almost always one round.  The first probe may have been done ahead of time
+  // (`pre`: slot pre_h was read as pre_cv after the last store to the table).
   __device__ __forceinline__ bool test_and_set(const VisitedCfg& c, int lane, uint32_t id, bool valid, bool pre = false,
                                                uint32_t pre_h = 0, uint32_t pre_cv = 0) {
     const uint32_t want = (epoch << c.id_bits) | id;
@@ -633,7 +720,7 @@ struct Visited {
     bool pending = valid, fresh = false, first = pre;
     while (__any_sync(FULL, pending)) {
       uint32_t cur = 0;
-      if (pending) cur = first ? pre_cv : ld_keep(tab + h, pol_keep);
+      if (pending) cur = first ? pre_cv : probe(c, h, pol_keep);
       first = false;
       bool claim = false;
       if (pending) {
@@ -651,7 +738,7 @@ struct Visited {
         const int leader = __ffs(same) - 1;
         const uint32_t lead_id = __shfl_sync(claimers, id, leader);
         if (lane == leader) {
-          st_keep(tab + h, want, pol_keep);
+          put(c, h, want, pol_keep);
           fresh = true;
           pending = false;
         } else if (lead_id == id) {
@@ -675,25 +762,31 @@ struct Visited {
     return grow_or_overflow(c, lane, none);
   }
 };
+typedef VisitedT<FirstStage::Global> Visited;
 
 // Move a search to the full stage: re-insert the live entries (current epoch) of the first stage, 32 per round; the last
 // searches' stale entries are skipped.  The full stage holds nothing of the current epoch before.  Returns the full
 // stage's state.  Out of line: it is the rare path, and inlined it took registers from the search loops around it.
-static __device__ __noinline__ Visited visited_migrate(const VisitedCfg c, const Visited from, int lane) {
-  Visited v{from.tab + c.small, c.shift, from.epoch, 0};  // `used` is counted again by the re-inserts
+template <FirstStage FS>
+static __device__ __noinline__ VisitedT<FS> visited_migrate(const VisitedCfg c, const VisitedT<FS> from, int lane) {
+  VisitedT<FS> v = from;  // the window stays; `used` is counted again by the re-inserts
+  if constexpr (!VisitedT<FS>::WINDOW) v.tab = from.tab + c.small;
+  v.shift = c.shift;
+  v.used = 0;
   const uint64_t pol_keep = l2_policy_evict_last();
 #pragma unroll 1
   for (uint32_t i = lane; i < c.small; i += 32) {
-    const uint32_t e = ld_keep(from.tab + i, pol_keep);
+    const uint32_t e = from.probe(c, i, pol_keep);
     v.test_and_set(c, lane, e & ((1u << c.id_bits) - 1u), (e >> c.id_bits) == v.epoch);
   }
   return v;
 }
 // `probed_ahead` is cleared when the search moves: a probe read ahead of time came from the first stage.
-__device__ __forceinline__ bool Visited::grow_or_overflow(const VisitedCfg& c, int lane, bool& probed_ahead) {
+template <FirstStage FS>
+__device__ __forceinline__ bool VisitedT<FS>::grow_or_overflow(const VisitedCfg& c, int lane, bool& probed_ahead) {
   if (shift == c.shift) return used >= c.cap - (c.cap >> 2);
   if (used >= c.small - (c.small >> 2)) {
-    *this = visited_migrate(c, *this, lane);
+    *this = visited_migrate<FS>(c, *this, lane);
     probed_ahead = false;
   }
   return false;

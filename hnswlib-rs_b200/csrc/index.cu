@@ -222,7 +222,11 @@ int Index::fill_visited_cfg(VisitedPool& v, VisitedCfg& c, bool staged, cudaStre
 //     decides it.  H100 SXM 80 GB, 700 W, bench.py, staged vs one stage: c2 (first stage 2 048 = 0.40 of 5 120, 91 MB of
 //     tables) +9 %; c3 (4 096 = 0.30 of 13 824, 181 MB) -15 %; c4 (8 192 = 0.30 of 27 648) -1 %.
 // Inserts keep one stage: their ef_construction searches mostly outgrow a first stage.
-bool Index::visited_staged(size_t slots, size_t cap, size_t need) const {
+// The lean kernel keeps its first stage in shared memory (FirstStage::Shared, common.cuh): it is staged only where that
+// window fits at the kernel's occupancy (`first_fits`: as many CTAs per SM as without it), in every mode; else it runs
+// single-stage.  At c2 the window is 8 KB and fits; c1, c3 and c4 are single-stage by the rule above anyway.
+bool Index::visited_staged(size_t slots, size_t cap, size_t need, bool first_fits) const {
+  if (!first_fits) return false;
   if (visited_stages_ != 0) return visited_stages_ == 1;
   return slots * cap * sizeof(uint32_t) > l2_bytes_ && visited_first_stage(cap) * 5 >= need * 2;
 }
@@ -742,18 +746,21 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.threads = wpb * 32;
   p.cbuf = nullptr;
   p.ccap = 0;
-  int bps = 0;
-  {
+  // CTAs per SM that the runtime grants the kernel with `bytes` of dynamic shared memory
+  auto occupancy = [&](size_t bytes, int& out) -> int {
     std::lock_guard<std::mutex> lk(occ_mu_);
-    const auto key = std::make_tuple(kind, p.q_kind, p.q_smem, wpb, p.g.d4, smem);
+    const auto key = std::make_tuple(kind, p.q_kind, p.q_smem, wpb, p.g.d4, bytes);
     auto it = occ_cache_.find(key);
     if (it != occ_cache_.end()) {
-      bps = it->second;
+      out = it->second;
     } else {
-      HB_CUDA(launch_query(kind, p, metric, dtype, 0, smem, st, &bps));
-      occ_cache_[key] = bps;
+      HB_CUDA(launch_query(kind, p, metric, dtype, 0, bytes, st, &out));
+      occ_cache_[key] = out;
     }
-  }
+    return 0;
+  };
+  int bps = 0;
+  if (int r = occupancy(smem, bps)) return r;
   if (bps < 1) return fail("search kernel does not fit on an SM");
   const size_t per_cta = (size_t)wpb;
   int grid = (int)std::min<size_t>((size_t)sm_count_ * bps, (nq + per_cta - 1) / per_cta);
@@ -774,7 +781,20 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
     }
     if ((r = ensure_visited(pool, (size_t)grid * per_cta, vcap, st))) return r;
     const size_t need = (size_t)2 * (p.ef + 16) * deg;  // the sizing estimate vcap was rounded up from
-    if ((r = fill_visited_cfg(pool, p.vis, visited_staged((size_t)grid * per_cta, pool.cap, need), st))) return r;
+    // the lean kernel keeps a first stage in its shared memory: a window that would cost CTAs per SM is not taken
+    size_t window_smem = 0;
+    bool first_fits = true;
+    if (kind == QueryKernel::Lean) {
+      const CtaShape wcta = cta_shape(lean_layout(p.q_smem, (uint32_t)visited_first_stage(pool.cap)).bytes, 1);
+      int wbps = 0;
+      if (wcta.warps && (r = occupancy(wcta.smem, wbps))) return r;
+      first_fits = wcta.warps && wbps >= bps;
+      window_smem = wcta.smem;
+    }
+    const bool staged = visited_staged((size_t)grid * per_cta, pool.cap, need, first_fits);
+    if ((r = fill_visited_cfg(pool, p.vis, staged, st))) return r;
+    const size_t launch_smem = staged && kind == QueryKernel::Lean ? window_smem : smem;
+    p.smem_per_warp = (int)(launch_smem / wpb);
     if (kind == QueryKernel::Filtered || kind == QueryKernel::StdTie) {  // candidate queue C: one region per warp slot
       if ((r = ensure_scratch(&c.d_cbuf, &c.d_cbuf_bytes, (size_t)grid * wpb * pool.cap * 8, st))) return r;
       p.cbuf = (uint64_t*)c.d_cbuf;
@@ -782,7 +802,7 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
     }
     HB_CUDA(cudaMemsetAsync(c.d_counter, 0, sizeof(unsigned int), st));
     HB_CUDA(cudaEventRecord(c.ev0, st));
-    HB_CUDA(launch_query(kind, p, metric, dtype, grid, smem, st, nullptr));
+    HB_CUDA(launch_query(kind, p, metric, dtype, grid, launch_smem, st, nullptr));
     HB_CUDA(cudaEventRecord(c.ev1, st));
     if (!sync) break;
     int status = 0;

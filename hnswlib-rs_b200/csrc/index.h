@@ -527,7 +527,7 @@ class Index {
   InsertShape insert_shape() const;
   int ensure_visited(VisitedPool& v, size_t slots, size_t cap_entries, cudaStream_t st);
   int fill_visited_cfg(VisitedPool& v, VisitedCfg& c, bool staged, cudaStream_t st);
-  bool visited_staged(size_t slots, size_t cap, size_t need) const;
+  bool visited_staged(size_t slots, size_t cap, size_t need, bool first_fits) const;
   int ensure_scratch(void** p, size_t* cur, size_t need, cudaStream_t st);
   int ensure_pinned(void** p, size_t* cur, size_t need, unsigned int flags);
   int grow_plevel(uint32_t id, int new_plevel);

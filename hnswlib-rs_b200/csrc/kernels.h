@@ -19,13 +19,16 @@ constexpr size_t SMEM_BUDGET = 220 * 1024;  // dynamic shared memory one CTA may
 // power limit, bench.py c2, one run each: 4.60 M queries/s at 20 (96 registers, 0 spill bytes; one launch of 100 000
 // queries 22.0 ms), 4.74 M at 24 (80 registers, 26 bytes spilled; 21.6 ms), 4.59 M at 28 (72 registers, 70 bytes spilled;
 // 22.8 ms).  24 is not taken: it spills in the production kernel.  (The sweep with full-size tables, 400 W: 25.8 ms at 20,
-// 26.7 at 24, 28.3 at 28, 32.4 at 32.)
+// 26.7 at 24, 28.3 at 28, 32.4 at 32.)  With the first stage in shared memory (8 960 bytes per CTA at c2) the production
+// kernel has 95 registers and 0 spill bytes, and the runtime grants 20 CTAs per SM, as without the window.
 constexpr int LEAN_MIN_BLOCKS = 20;
 
 // Visited tables (Visited, common.cuh): a search starts in a first stage of cap / VISITED_FIRST_DIV entries and moves to
 // the full stage of `cap` entries when the first one is 3/4 full.  H100 SXM 80 GB, 700 W, bench.py c2 (cap = 8 192): 4.35 M
 // queries/s at cap / 8 (65-74 % of queries move), 4.60 M at cap / 4 (7-10 % move), 4.54 M at cap / 2 (none moves); 4.21 M
-// with one full-size table per slot.
+// with one full-size table per slot.  Those first stages were global (~23 MB per search context resident in L2); the lean
+// kernel's first stage is now in shared memory (8 KB per warp at c2, none in L2): 4.58-4.59 -> 5.72-5.73 M queries/s,
+// same card and power limit, one session.
 constexpr int VISITED_FIRST_DIV = 4;
 inline size_t visited_first_stage(size_t cap) { return cap / VISITED_FIRST_DIV; }
 inline size_t visited_slot_entries(size_t cap) { return cap + visited_first_stage(cap); }
@@ -114,12 +117,13 @@ __host__ __device__ inline StdLayout std_layout(int d4, int q_smem) {
 }
 
 // lean kernel (search_lean.cuh): [queue keys, also the query's staging buffer][chunk ids][chunk distances]
+// [visited first stage, `small` words (VisitedCfg.small; none for a single-stage launch)]
 struct LeanLayout {
-  uint32_t queue, cand_id, cand_d, bytes;
+  uint32_t queue, cand_id, cand_d, visited, bytes;
 };
-__host__ __device__ constexpr LeanLayout lean_layout(int q_smem) {
-  const uint32_t cand_id = (uint32_t)q_smem * 8, cand_d = cand_id + 32 * 4;
-  return LeanLayout{0, cand_id, cand_d, (uint32_t)round128(cand_d + 32 * 4)};
+__host__ __device__ constexpr LeanLayout lean_layout(int q_smem, uint32_t small = 0) {
+  const uint32_t cand_id = (uint32_t)q_smem * 8, cand_d = cand_id + 32 * 4, visited = cand_d + 32 * 4;
+  return LeanLayout{0, cand_id, cand_d, visited, (uint32_t)round128(visited + (size_t)small * 4)};
 }
 
 // insert kernel (build.cu): [TMA stage][new point][point of a selection step][queue keys][chunk ids][chunk distances]
@@ -231,6 +235,9 @@ struct InsertParams {
 // The kernel this host thread last launched through launch_kernel (hnsw_b200_last_kernel reports its name), so that a
 // test can tell which template instantiation served a call.
 inline thread_local const void* last_launched_kernel = nullptr;
+// its dynamic shared memory and threads per CTA (hnsw_b200_last_kernel_shape)
+inline thread_local size_t last_launched_smem = 0;
+inline thread_local int last_launched_threads = 0;
 
 // Every launcher below sets the kernel's dynamic shared-memory limit to `smem`, then either launches it (blocks_per_sm ==
 // nullptr) or only reports how many CTAs of `threads` threads fit on one SM.
@@ -241,6 +248,8 @@ cudaError_t launch_kernel(void (*kern)(P), const P& p, int grid, int threads, si
   if (blocks_per_sm) return cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, kern, threads, smem);
   kern<<<grid, threads, smem, st>>>(p);
   last_launched_kernel = reinterpret_cast<const void*>(kern);
+  last_launched_smem = smem;
+  last_launched_threads = threads;
   return cudaGetLastError();
 }
 

@@ -1,5 +1,5 @@
 // Building blocks of the lean query kernel (search_lean.cuh): the reduction arithmetic of the distance functors by type, the "still unexpanded" bit masks that stand for the reference's candidate heap C
-// (/root/reference/src/hnsw.rs:940-1001), and shared-memory access through pinned 32-bit window addresses.
+// (/root/reference/src/hnsw.rs:940-1001).  Shared-memory access through pinned 32-bit window addresses is in common.cuh.
 #pragma once
 #include "common.cuh"
 
@@ -55,31 +55,5 @@ template <int QC>
 struct MaskSel;
 template <> struct MaskSel<64> { typedef Mask64 type; };
 template <> struct MaskSel<128> { typedef Mask128 type; };
-
-// ---- shared memory through 32-bit window addresses.  The addresses are produced once by pin(), an opaque move the
-// compiler can neither see through nor re-derive from the thread index inside the loop (it did, at ~6 instructions
-// and one S2R per access, when the addresses were ordinary pointers).
-__device__ __forceinline__ uint32_t pin(uint32_t v) {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %1;" : "=r"(r) : "r"(v));
-  return r;
-}
-__device__ __forceinline__ uint64_t lds64(uint32_t a) {
-  uint64_t v;
-  asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(a) : "memory");
-  return v;
-}
-__device__ __forceinline__ void sts64(uint32_t a, uint64_t v) { asm volatile("st.shared.u64 [%0], %1;" ::"r"(a), "l"(v) : "memory"); }
-__device__ __forceinline__ uint32_t lds32(uint32_t a) {
-  uint32_t v;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
-  return v;
-}
-__device__ __forceinline__ void sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
-__device__ __forceinline__ uint4 lds128(uint32_t a) {
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a) : "memory");
-  return v;
-}
 
 }  // namespace hb

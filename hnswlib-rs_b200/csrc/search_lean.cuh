@@ -17,6 +17,8 @@
 //     eight are prefetched to L2 the moment the list is known, so that only the first pass pays the HBM latency
 //     (issuing one bulk copy per row costs ~8 instructions per row: the copy engine takes uniform operands);
 //   * two rows per lane group are reduced with one transposed reduction (3 shuffles for 2 rows, same sums);
+//   * a staged launch keeps the visited set's first stage in the warp's shared memory (VisitedT<FirstStage::Shared>):
+//     a probe is a shared-memory load, and a query that never moves touches no table line in L2;
 //   * the traversal counters are a template parameter: the production instantiation does not carry them.
 #pragma once
 #include "kernels.h"
@@ -139,15 +141,16 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
   const GraphView& G = p.g;
   const int lane = (int)pin(threadIdx.x & 31);
   const int g = lane & 7, r = lane >> 3;
-  const uint32_t wa = pin(smem_u32(smem_raw) + (uint32_t)(threadIdx.x >> 5) * L.bytes + L.queue);
+  // the warp's region is p.smem_per_warp bytes: lean_layout(QC, p.vis.small)
+  const uint32_t wa = pin(smem_u32(smem_raw) + (uint32_t)(threadIdx.x >> 5) * (uint32_t)p.smem_per_warp + L.queue);
   const uint32_t ca = wa + L.cand_id, da = wa + L.cand_d;
   const char* const vecb = reinterpret_cast<const char*>(G.vec);
   constexpr uint32_t row_bytes = (uint32_t)CH * 128u;
   const uint64_t pol_rows = l2_policy_evict_first();
 
   const uint32_t slot = blockIdx.x * (LEAN_THREADS / 32) + (threadIdx.x >> 5);
-  Visited vis;
-  vis.init(p.vis, slot);
+  VisitedT<FirstStage::Shared> vis;  // first stage in the warp's shared memory, full stage in its global slot
+  vis.init(p.vis, slot, wa - L.queue + L.visited, lane);
   unsigned evals = 0, expans = 0, adjr = 0;
   const int cap = p.ef;
 
@@ -284,7 +287,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
             pre_nid = (lane < pcap) ? pids[lane] : INVALID_ID;
             pre_h = vis.home(pre_nid);
             pre_cv = 0;
-            if (pre_nid != INVALID_ID) pre_cv = ld_keep(vis.tab + pre_h, l2_policy_evict_last());
+            if (pre_nid != INVALID_ID) pre_cv = vis.probe(p.vis, pre_h, l2_policy_evict_last());
             pre_ok = true;
           }
         };
@@ -323,10 +326,15 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
   }
 }
 
+// A launch whose `smem` holds a visited first stage asks for the largest shared-memory carveout, so that the windows do
+// not cost CTAs per SM (c2: 20 CTAs x (8 960 + 1 024 reserved) bytes = 195 KB); one without leaves the split to the driver.
 template <class Op, int CH, int QC>
 static cudaError_t launch_lean_kernel(const SearchParams& p, int grid, size_t smem, cudaStream_t st, int* blocks_per_sm) {
-  if (p.stats) return launch_kernel(search_lean_kernel<Op, CH, QC, true>, p, grid, LEAN_THREADS, smem, st, blocks_per_sm);
-  return launch_kernel(search_lean_kernel<Op, CH, QC, false>, p, grid, LEAN_THREADS, smem, st, blocks_per_sm);
+  void (*kern)(SearchParams) = p.stats ? search_lean_kernel<Op, CH, QC, true> : search_lean_kernel<Op, CH, QC, false>;
+  const int carveout = smem > lean_layout(QC).bytes ? (int)cudaSharedmemCarveoutMaxShared : (int)cudaSharedmemCarveoutDefault;
+  cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, carveout);
+  if (e != cudaSuccess) return e;
+  return launch_kernel(kern, p, grid, LEAN_THREADS, smem, st, blocks_per_sm);
 }
 
 template <class Op, int QC>

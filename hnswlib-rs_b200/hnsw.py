@@ -70,6 +70,7 @@ def load_library():
     L.hnsw_b200_drop.argtypes = [vp]
     L.hnsw_b200_last_error.restype = C.c_char_p
     L.hnsw_b200_last_kernel.argtypes = [C.c_char_p, sz]
+    L.hnsw_b200_last_kernel_shape.argtypes = [vp]
     L.hnsw_b200_device_count.restype = i32
     L.hnsw_b200_set_device.argtypes = [i32]
     L.hnsw_b200_free_neighbourhood.argtypes = [vp]
@@ -158,6 +159,16 @@ def last_kernel():
     buf = C.create_string_buffer(n + 1)
     L.hnsw_b200_last_kernel(buf, n + 1)
     return buf.value.decode()
+
+
+def last_kernel_shape():
+    """(dynamic shared memory per CTA in bytes, threads per CTA, CTAs per SM the runtime grants) of that same kernel,
+    (0, 0, 0) before the first launch"""
+    L = load_library()
+    out = np.zeros(3, np.int64)
+    if L.hnsw_b200_last_kernel_shape(_p(out)) < 0:
+        raise HnswError(last_error())
+    return tuple(int(v) for v in out)
 
 
 def _p(a):

@@ -200,6 +200,10 @@ const char* hnsw_b200_last_error(void);
  * search, dist_batch and bruteforce kernels; occupancy queries do not count), written NUL-terminated and truncated to
  * cap bytes.  Returns the full length of the name, 0 when this thread has launched none, -1 on a CUDA error. */
 int hnsw_b200_last_kernel(char* buf, size_t cap);
+/* Diagnostics: of that same kernel, out3 = {dynamic shared memory per CTA in bytes, threads per CTA, CTAs per SM the
+ * runtime grants it (cudaOccupancyMaxActiveBlocksPerMultiprocessor, under the kernel's current attributes)}.  Returns 1,
+ * 0 (and zeros) when this thread has launched none, -1 on a CUDA error. */
+int hnsw_b200_last_kernel_shape(int64_t* out3);
 int hnsw_b200_device_count(void);
 /* Limits: max_nb_connection <= 256; fewer than 2^31 points; one query (or insert) must fit 220 KB of shared memory:
  * 16 * ceil(dim * sizeof(T) / 128) * 8 bytes for the query (twice that for an insert) plus 8 bytes per ef (ef_construction)

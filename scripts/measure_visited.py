@@ -1,6 +1,8 @@
 """Visited tables at the c2 shape (1 M x 128 f32 L2, M = 16, ef_c = 200, k = 10, ef = 64): per-launch kernel ms of the
-lean search for 10 000 and 100 000 queries (search_device, best of 5 after a warm-up launch), and how many queries
-outgrow a first stage of cap / 8, cap / 4 and cap / 2 entries.  A search moves when its layer-0 insertions (one per
+lean search for 10 000 and 100 000 queries (search_device, best of 5 after a warm-up launch), the launch's dynamic shared
+memory per CTA (with the first stage in shared memory when the launch is staged) and the CTAs per SM the runtime grants
+it (cudaOccupancyMaxActiveBlocksPerMultiprocessor), and how many queries outgrow a first stage of cap / 8, cap / 4 and
+cap / 2 entries (cap / 4 is the one the searches use).  A search moves when its layer-0 insertions (one per
 layer-0 evaluation, the entry included) reach 3/4 of the first stage; the counters give evaluations per query including
 the descent's (at most 1 + max_level * M), so the moved count is given as a range.  HNSW_B200_LIB selects a build."""
 import importlib
@@ -25,6 +27,9 @@ for nq in (10000, 100000):
     h.search_device(q.data_ptr(), nq, k, ef, out.data_ptr(), cnt.data_ptr(), sync=True)
     ms = [h.search_device(q.data_ptr(), nq, k, ef, out.data_ptr(), cnt.data_ptr(), sync=True) for _ in range(5)]
     print(f"{nq} queries per launch: kernel {min(ms):.3f} ms (best of 5), {nq / min(ms) / 1e3:.2f} M queries/s", flush=True)
+    smem, threads, bps = pkg.last_kernel_shape()
+    print(f"  {pkg.last_kernel()}: {smem} bytes of dynamic shared memory per {threads}-thread CTA, {bps} CTAs per SM",
+          flush=True)
 
 Q = pkg.datagen.make("clustered", 500, d, 3)
 h.enable_stats(True)
