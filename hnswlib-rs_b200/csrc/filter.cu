@@ -16,24 +16,6 @@
 
 namespace hb {
 
-// A query's filter, kept in its warp's mbarrier slot (unused by this kernel) and read at each use, so that the search
-// loop holds no extra register: a bitmap (label == LABEL_NONE), or the label array and the label the query admits, or
-// (the launch's SearchParams::label_sets set) the label array and the query's set, label_sets[label, label + nset).
-struct FilterSlot {
-  const uint32_t* ptr;
-  uint32_t label;
-  uint32_t nset;
-};
-
-// The launch's label_sets (nullptr: none), kept by lane 0 in the 16 bytes just below the slot: the tail of the
-// candidate-distance region, whose first 32 of 64 reserved entries are all this kernel scores into.  Read there, the
-// admission test needs neither a register nor an argument for it; as an argument it pushed the generic (CH = 0)
-// kernels of f32 L2 and cosine into spilling.
-__device__ __forceinline__ const uint32_t** set_base(FilterSlot* f) { return reinterpret_cast<const uint32_t**>(f) - 2; }
-__device__ __forceinline__ const uint32_t* set_base(const FilterSlot* f) {
-  return *(reinterpret_cast<const uint32_t* const*>(f) - 2);
-}
-
 // x is one of the sorted values v[0, n): a binary search in global memory
 __device__ __forceinline__ bool in_sorted(const uint32_t* v, uint32_t n, uint32_t x) {
   while (n) {
@@ -65,21 +47,21 @@ template <> struct SetLookupCall<OpJaccard<uint16_t>> { static constexpr bool va
 
 // the one admission test: the point's label against the query's label or set, or its bit of the bitmap
 template <class Op>
-__device__ __forceinline__ bool filter_pass(const FilterSlot* f, uint32_t id) {
+__device__ __forceinline__ bool filter_pass(const RowFilter* f, uint32_t id) {
   const uint32_t want = f->label;
   if (want != LABEL_NONE) {
     const uint32_t lab = __ldg(f->ptr + id);
-    const uint32_t* sets = set_base(f);
-    if (!sets) return lab == want;
-    if constexpr (SetLookupCall<Op>::value) return in_sorted_call(sets + want, f->nset, lab);
-    return in_sorted(sets + want, f->nset, lab);
+    const uint32_t* set = f->set;
+    if (!set) return lab == want;
+    if constexpr (SetLookupCall<Op>::value) return in_sorted_call(set, f->nset, lab);
+    return in_sorted(set, f->nset, lab);
   }
   return (__ldg(f->ptr + (id >> 5)) >> (id & 31)) & 1u;
 }
 
 // keeps the keys w[0, n) whose points pass the filter, in order, at the front of w; returns how many there are
 template <class Op>
-__device__ __forceinline__ int keep_passing(uint64_t* w, int n, const FilterSlot* fslot) {
+__device__ __forceinline__ int keep_passing(uint64_t* w, int n, const RowFilter* fslot) {
   const int lane = lane_id();
   int out = 0;
   for (int b = 0; b < n; b += 32) {
@@ -102,7 +84,7 @@ __device__ __forceinline__ int keep_passing(uint64_t* w, int n, const FilterSlot
 template <class Op, int CH, int U>
 __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const WarpSmem& s, const VisitedCfg& vc, Visited& vis,
                                                       SortedQueue& W, uint64_t* cbuf, uint32_t ccap,
-                                                      const FilterSlot* fslot, uint32_t ep, int ef, int layer,
+                                                      const RowFilter* fslot, uint32_t ep, int ef, int layer,
                                                       Stats& st, bool& overflow) {
   const int lane = lane_id();
   const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
@@ -216,7 +198,9 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
   const QueryLayout L = query_layout(g.d4, p.q_smem);  // search.cu's layout; the stage is unused here
   const WarpSmem s{reinterpret_cast<uint4*>(base + L.query), reinterpret_cast<uint64_t*>(base + L.queue),
                    reinterpret_cast<uint32_t*>(base + L.cand_id), reinterpret_cast<float*>(base + L.cand_d)};
-  FilterSlot* fslot = reinterpret_cast<FilterSlot*>(base + L.bar);
+  // the query's filter, read at each use so that the search loop holds no register for it: in the upper half of the
+  // candidate-distance region, whose first 32 of 64 reserved entries are all this kernel scores into
+  RowFilter* fslot = reinterpret_cast<RowFilter*>(base + L.cand_d + 32 * 4);
   const uint32_t slot = blockIdx.x * (blockDim.x >> 5) + warp;  // the host launches fewer warps per CTA when shared memory is short
   Visited vis;
   vis.init(p.vis, slot);
@@ -228,23 +212,7 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
     const uint32_t qi = next_item(p.work_counter, lane);
     if (qi >= p.nq) break;
     stage_row_bytes(s.q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes, p.q_bytes, g.d4 * 16);
-    // this query's filter: the launch's one bitmap, its own entry of the bitmap table, its own label or label set
-    if (lane == 0) {
-      if (p.labels) {
-        fslot->ptr = p.labels;
-        *set_base(fslot) = p.label_sets;
-        if (p.label_sets) {
-          const uint2 s2 = reinterpret_cast<const uint2*>(p.filter_sel)[qi];
-          fslot->label = s2.x;
-          fslot->nset = s2.y;
-        } else {
-          fslot->label = p.filter_sel[qi];
-        }
-      } else {
-        fslot->ptr = p.filter_sel ? p.filter_table[p.filter_sel[qi]] : p.filter_bits;
-        fslot->label = LABEL_NONE;
-      }
-    }
+    if (lane == 0) *fslot = p.filter_sel ? p.filter_table[p.filter_sel[qi]] : p.filter;
     __syncwarp();
     int count = 0;
     bool overflow = false;

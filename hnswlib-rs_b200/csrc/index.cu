@@ -722,14 +722,12 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.work_counter = c.d_counter;
   p.out_nb = d_out;
   p.out_count = d_counts;
-  p.filter_bits = f.bits;
   p.filter_table = f.table;
   p.filter_sel = f.sel;
-  p.labels = f.labels;
-  p.label_sets = f.sets;
+  p.filter = f.filter;
   p.stats = stats_on_ ? d_stats_ : nullptr;
   p.status = c.d_status;
-  const bool filtered = f.bits != nullptr || f.sel != nullptr;
+  const bool filtered = f.sel != nullptr || f.filter.ptr != nullptr;
   QueryKernel kind = QueryKernel::Generic;
   if (filtered) kind = QueryKernel::Filtered;
   else if (tie_std_) kind = QueryKernel::StdTie;  // unfiltered searches only
@@ -910,13 +908,12 @@ int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** 
   return run_plan(c, p.run, true, nullptr);  // grows the tables
 }
 
-// A single bitmap run goes to the launch as its filter bits (a FilterT's host bits uploaded into the context first), as
-// a batch-wide filter does; several as a table of their bitmaps and each row's entry in it.  Label-set runs go as the
-// label array and each row's label when every set is one label (the kernel compares labels), else each row's (offset,
-// count) in the sets' values, uploaded into the context ahead of the launches.  Exact: a group of every point for the
-// unrestricted rows, and one per run; a run of one slice scans it in place, any other its slices copied one after the
-// other into the context (a point has one label, so a label set's slices are disjoint, and the exact scan orders by
-// (distance, id), so their order does not matter).
+// Graph: one RowFilter per run, a bitmap (a FilterT's host bits uploaded into the context first), a label (a set of one,
+// which the kernel compares) or a set (its values uploaded).  One run goes to the launch by value, as a batch-wide
+// filter does; several as a table of them and each row's entry in it, uploaded into the context's filter scratch ahead
+// of the words the runs read there.  Exact: a group of every point for the unrestricted rows, and one per run; a run of
+// one slice scans it in place, any other its slices copied one after the other into the context (a point has one label,
+// so a label set's slices are disjoint, and the exact scan orders by (distance, id), so their order does not matter).
 int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
   cudaStream_t st = c.stream;
   int r;
@@ -948,49 +945,39 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
     return 0;
   }
   if (plan.runs.empty()) return 0;
-  if (plan.labels) {
-    const bool single = std::all_of(plan.runs.begin(), plan.runs.end(), [](const LegPlan::Run& u) { return u.nset == 1; });
-    std::vector<uint32_t> sel, vals;  // sel: the label, or (offset, count), per row
-    for (const LegPlan::Run& u : plan.runs) {
-      if (single) {
-        sel.insert(sel.end(), u.count, u.set[0]);
-        continue;
-      }
-      if (vals.size() >= LABEL_NONE - u.nset) return fail("label sets: too many distinct labels in one batch");
-      for (size_t j = 0; j < u.count; ++j) sel.insert(sel.end(), {(uint32_t)vals.size(), u.nset});
+  const bool several = plan.runs.size() > 1;
+  const size_t fw = (n + 31) / 32, rows = L.nq - plan.plain;
+  const size_t tb = several ? round128(plan.runs.size() * sizeof(RowFilter)) : 0, sb = several ? round128(rows * 4) : 0;
+  size_t words = 0;
+  for (const LegPlan::Run& u : plan.runs) words += u.host_bits ? fw : u.nset != 1 ? u.nset : 0;
+  // never null, also with no words: an empty set's values are there
+  if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, tb + sb + std::max<size_t>(words, 1) * 4, st))) return r;
+  uint32_t* const at = (uint32_t*)((char*)c.d_fbits + tb + sb);
+  std::vector<RowFilter> table;
+  std::vector<uint32_t> sel, vals;  // vals: the host words to upload at `at`
+  for (const LegPlan::Run& u : plan.runs) {
+    RowFilter f{u.bits, nullptr, LABEL_NONE, 0};  // a resident filter: already on this device
+    if (u.host_bits) {
+      f.ptr = at + vals.size();
+      vals.insert(vals.end(), u.host_bits, u.host_bits + fw);
+    } else if (u.nset == 1) {
+      f = RowFilter{plan.labels, nullptr, u.set[0], 0};
+    } else if (plan.labels) {
+      f = RowFilter{plan.labels, at + vals.size(), 0, u.nset};
       vals.insert(vals.end(), u.set, u.set + u.nset);
     }
-    const size_t sb = round128(sel.size() * sizeof(uint32_t)), vb = vals.size() * sizeof(uint32_t);
-    if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, sb + vb, st))) return r;
-    HB_CUDA(cudaMemcpyAsync(c.d_fbits, sel.data(), sel.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
-    if (vb) HB_CUDA(cudaMemcpyAsync((char*)c.d_fbits + sb, vals.data(), vb, cudaMemcpyHostToDevice, st));
-    L.filter.sel = (const uint32_t*)c.d_fbits;
-    L.filter.sets = single ? nullptr : (const uint32_t*)((char*)c.d_fbits + sb);
-    L.filter.labels = plan.labels;
-    return 0;
+    if (several) sel.insert(sel.end(), u.count, (uint32_t)table.size());
+    table.push_back(f);
   }
-  if (plan.runs.size() == 1) {
-    L.filter.bits = plan.runs[0].bits;  // a resident filter: already on this device
-    if (plan.runs[0].host_bits) {
-      const size_t fb = ((n + 31) / 32) * 4;
-      if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, fb, st))) return r;
-      HB_CUDA(cudaMemcpyAsync(c.d_fbits, plan.runs[0].host_bits, fb, cudaMemcpyHostToDevice, st));
-      L.filter.bits = (const uint32_t*)c.d_fbits;
-    }
-    return 0;
+  if (several) {
+    HB_CUDA(cudaMemcpyAsync(c.d_fbits, table.data(), table.size() * sizeof(RowFilter), cudaMemcpyHostToDevice, st));
+    HB_CUDA(cudaMemcpyAsync((char*)c.d_fbits + tb, sel.data(), rows * 4, cudaMemcpyHostToDevice, st));
+    L.filter.table = (const RowFilter*)c.d_fbits;
+    L.filter.sel = (const uint32_t*)((char*)c.d_fbits + tb);
+  } else {
+    L.filter.filter = table[0];
   }
-  std::vector<const uint32_t*> table;
-  std::vector<uint32_t> sel;
-  for (const LegPlan::Run& u : plan.runs) {
-    sel.insert(sel.end(), u.count, (uint32_t)table.size());
-    table.push_back(u.bits);
-  }
-  const size_t tb = round128(table.size() * sizeof(void*)), sb = sel.size() * sizeof(uint32_t);
-  if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, tb + sb, st))) return r;
-  HB_CUDA(cudaMemcpyAsync(c.d_fbits, table.data(), table.size() * sizeof(void*), cudaMemcpyHostToDevice, st));
-  HB_CUDA(cudaMemcpyAsync((char*)c.d_fbits + tb, sel.data(), sb, cudaMemcpyHostToDevice, st));
-  L.filter.table = (const uint32_t* const*)c.d_fbits;
-  L.filter.sel = (const uint32_t*)((char*)c.d_fbits + tb);
+  if (!vals.empty()) HB_CUDA(cudaMemcpyAsync(at, vals.data(), vals.size() * 4, cudaMemcpyHostToDevice, st));
   return 0;
 }
 

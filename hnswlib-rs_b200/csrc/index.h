@@ -119,15 +119,12 @@ struct ExactGroup {
   ExactScan scan;
 };
 
-// The restriction of one search launch, as SearchParams reads it: none, one bitmap for every row (bits), a bitmap per row
-// (row i on table[sel[i]]), a label per row (row i on the points whose `labels` entry is sel[i]), or a label set per row
-// (row i on the points whose `labels` entry is one of sets[sel[2i], sel[2i] + sel[2i + 1]))
+// The restriction of one search launch, as SearchParams reads it: none (sel and filter.ptr null), `filter` for every row,
+// or row i under table[sel[i]]
 struct LaunchFilter {
-  const uint32_t* bits = nullptr;
-  const uint32_t* const* table = nullptr;
+  RowFilter filter{nullptr, nullptr, LABEL_NONE, 0};
+  const RowFilter* table = nullptr;
   const uint32_t* sel = nullptr;
-  const uint32_t* labels = nullptr;
-  const uint32_t* sets = nullptr;
 };
 
 // Resident filters (hnsw_b200_filter_new, filter_store.cu): a FilterT materialised once per handle, as one bitmap per
@@ -432,7 +429,7 @@ class Index {
     unsigned int* d_counter = nullptr;
     int* d_status = nullptr;
     VisitedPool vis, fvis;  // unfiltered / filtered searches
-    // the call's filter bits (or its bitmap table and selectors; exact: its label sets' joined id lists) / C
+    // what the call's restriction uploads (stage_plan; exact: its label sets' joined id lists) / C
     void *d_fbits = nullptr, *d_cbuf = nullptr;
     size_t d_fbits_bytes = 0, d_cbuf_bytes = 0;
     void *d_xq = nullptr, *d_xpart = nullptr;  // exact scan: the host batch's queries on the device / tickets and slice lists

@@ -41,6 +41,16 @@ struct NeighbourOut {
   uint32_t internal;
 };
 
+// the restriction of one row of a filtered launch: a bitmap over internal ids (label == LABEL_NONE), or the label array
+// and the one label the row admits (set == nullptr), or the label array and the row's set, set[0, nset) ascending (set
+// is not nullptr, also when the set is empty, and label is then any value but LABEL_NONE)
+struct RowFilter {
+  const uint32_t* ptr;
+  const uint32_t* set;
+  uint32_t label;
+  uint32_t nset;
+};
+
 struct SearchParams {
   GraphView g;
   const void* queries;  // device, raw element bytes, row i at i * q_stride_bytes
@@ -54,7 +64,7 @@ struct SearchParams {
   unsigned int* work_counter;
   NeighbourOut* out_nb;  // [nq][k]
   int32_t* out_count;    // [nq]
-  const uint32_t* filter_bits;  // nullptr = no filter; bit per internal id
+  const RowFilter* filter_table;  // filtered search: one entry per run of rows
   unsigned long long* stats;    // nullptr or [3]: evals, expansions, adjacency ids read
   int* status;                  // set to 1 on visited-table overflow
   int smem_per_warp;
@@ -63,17 +73,9 @@ struct SearchParams {
   int q_kind;  // QueueSel kind
   uint64_t* cbuf;  // filtered search only: candidate queue C, [slots][ccap] keys
   uint32_t ccap;
-  // filtered search with a filter per query (filter_sel != nullptr): query i uses the bitmap filter_table[filter_sel[i]]
-  // instead of filter_bits.  Appended, so that every field above keeps its offset.
-  const uint32_t* const* filter_table;
+  // filtered search: query i's restriction is filter_table[filter_sel[i]], or `filter` when filter_sel is nullptr
   const uint32_t* filter_sel;  // [nq]
-  // filtered search with a label per query (labels != nullptr): query i admits the points p with labels[p] ==
-  // filter_sel[i] (never LABEL_NONE) instead of a bitmap.  Appended like the two above.
-  const uint32_t* labels;  // [points]
-  // filtered search with a label set per query (labels and label_sets != nullptr): filter_sel is [nq][2], and query i
-  // admits the points p whose labels[p] is one of label_sets[filter_sel[2i], filter_sel[2i] + filter_sel[2i + 1]),
-  // sorted ascending, none LABEL_NONE (filter_sel[2i] is never LABEL_NONE).  Appended like the fields above.
-  const uint32_t* label_sets;
+  RowFilter filter;
 };
 
 // the label of a point that has none (hnsw_b200_set_labels): no label admits it
