@@ -67,7 +67,7 @@ struct ExactParams {
   const void* queries;   // device, [nq][q_bytes] raw element bytes
   int q_bytes;
   uint32_t nq;
-  const uint32_t* list;  // sorted internal ids, or nullptr: the points 0 .. npts - 1
+  const uint32_t* list;  // distinct internal ids in any order (the queues keep the k smallest keys), or nullptr: 0 .. npts - 1
   uint32_t npts;
   int k;
   int tq, rows, stages;  // queries per tile, rows per ring block (divides 32), ring blocks

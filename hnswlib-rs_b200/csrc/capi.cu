@@ -634,8 +634,10 @@ static int64_t search_call(const void* h, Via via, const char* name, const Restr
     return pass(ix, ix->search_device(rs, exact, queries, nq, knbn, ef, out.nb, out.counts, sync != 0, kernel_ms));
   if (via == HOST && nq == 0) return 0;
   if (rs.kind == Restriction::ROW_FILTERS && !rs.filters) return set_err("filters is NULL");
-  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset_off) return set_err("qset_off is NULL");
-  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset) return set_err("qset is NULL");
+  // with ranges, qset_off and qset may both be NULL: every row's set is then {LABEL_NONE}
+  const bool no_sets = rs.qrange && !rs.qset_off && !rs.qset;
+  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset_off && !no_sets) return set_err("qset_off is NULL");
+  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset && !no_sets) return set_err("qset is NULL");
   if (!queries || !out.ids || !out.dist || !out.counts || knbn == 0 || nq == 0) return set_err("bad argument");
   HB_PARTS_SHARED_IF(ix);
   HostBatch b{queries, nullptr, nq, (int)dim, knbn, ef, rs, out};
@@ -657,8 +659,8 @@ static Restriction filter_t(int mode, const uint64_t* ids, uint64_t nids, hnsw_b
 static Restriction resident(int64_t f) { return {Restriction::RESIDENT, 0, nullptr, 0, nullptr, nullptr, f}; }
 static Restriction resident_or_all(int64_t f) { return f == -1 ? Restriction() : resident(f); }  // -1: every point
 static Restriction row_filters(const int64_t* f) { return {Restriction::ROW_FILTERS, 0, nullptr, 0, nullptr, nullptr, -1, f}; }
-static Restriction row_label_sets(const uint64_t* off, const uint32_t* set) {
-  return {Restriction::ROW_LABEL_SETS, 0, nullptr, 0, nullptr, nullptr, -1, nullptr, off, set};
+static Restriction row_label_sets(const uint64_t* off, const uint32_t* set, const int64_t* range = nullptr) {
+  return {Restriction::ROW_LABEL_SETS, 0, nullptr, 0, nullptr, nullptr, -1, nullptr, off, set, range};
 }
 
 // hnsw_b200_search_flat and _search_flat_filtered: the filter is the FilterT arguments (filter_mode 1, 2) or one of the
@@ -735,11 +737,12 @@ int hnsw_b200_search_exact_per_query(const void* h, const int64_t* filters, cons
                           columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 
-// Point labels.  On a partitioned handle point g (its insertion rank) is local point g / P of partition g % P.
-static int label_range(const Index* ix, uint64_t first, uint64_t n) {
+// Point labels (and attributes).  On a partitioned handle point g (its insertion rank) is local point g / P of partition
+// g % P.
+static int label_range(const Index* ix, uint64_t first, uint64_t n, const char* what = "labels") {
   const uint64_t have = nb_point(ix);
   if (first > have || n > have - first)
-    return set_err("labels [" + std::to_string(first) + ", " + std::to_string(first + n) + ") are out of range: the " +
+    return set_err(std::string(what) + " [" + std::to_string(first) + ", " + std::to_string(first + n) + ") are out of range: the " +
                    (ix->owner ? "partition" : "index") + " holds " + std::to_string(have) + " points");
   return 0;
 }
@@ -757,25 +760,36 @@ static int for_label_range(Index* ix, uint64_t first, uint64_t n,
   }
   return 0;
 }
-int hnsw_b200_set_labels(void* h, uint64_t first, uint64_t n, const uint32_t* labels) {
+// set_labels / set_attributes: values[0, n) for the points [first, first + n), under the handle's lock and every
+// partition's, each taken exclusively; a partition's share is gathered from every P-th value
+extern "C++" {
+namespace {
+template <class T>
+int set_per_point(void* h, uint64_t first, uint64_t n, const T* values, const char* what, const char* null_msg,
+                  int (Index::*set)(size_t, size_t, const T*)) {
   HB_H(h);
   HB_NOT_VIEW(ix);
-  if (label_range(ix, first, n)) return -1;
+  if (label_range(ix, first, n, what)) return -1;
   if (n == 0) return 0;
-  if (!labels) return set_err("labels is NULL");
+  if (!values) return set_err(null_msg);
   hb::DeviceRestore keep;
   const auto pl__ = ix->parts ? ix->parts->lock_exclusive() : std::vector<std::unique_lock<std::shared_mutex>>();
-  std::vector<uint32_t> mine;
+  std::vector<T> mine;
   return for_label_range(ix, first, n, [&](Index* x, int part, uint64_t lo, uint64_t cnt, uint64_t stride, uint64_t at) {
-    const uint32_t* src = labels + at;
+    const T* src = values + at;
     if (stride != 1) {
       mine.resize(cnt);
-      for (uint64_t i = 0; i < cnt; ++i) mine[i] = labels[at + i * stride];
+      for (uint64_t i = 0; i < cnt; ++i) mine[i] = values[at + i * stride];
       src = mine.data();
     }
-    const int r = x->set_labels(lo, cnt, src);
+    const int r = (x->*set)(lo, cnt, src);
     return pass(ix, r && ix->parts ? ix->parts->fail(part, x->err()) : r);
   });
+}
+}  // namespace
+}  // extern "C++"
+int hnsw_b200_set_labels(void* h, uint64_t first, uint64_t n, const uint32_t* labels) {
+  return set_per_point(h, first, n, labels, "labels", "labels is NULL", &Index::set_labels);
 }
 int hnsw_b200_get_labels(const void* h, uint64_t first, uint64_t n, uint32_t* out) {
   HB_HS(h);
@@ -785,6 +799,22 @@ int hnsw_b200_get_labels(const void* h, uint64_t first, uint64_t n, uint32_t* ou
   HB_PARTS_SHARED_IF(ix);
   return for_label_range(ix, first, n, [&](Index* x, int, uint64_t lo, uint64_t cnt, uint64_t stride, uint64_t at) {
     for (uint64_t i = 0; i < cnt; ++i) out[at + i * stride] = x->h_label[lo + i];
+    return 0;
+  });
+}
+
+// Point attributes: addressed as labels are
+int hnsw_b200_set_attributes(void* h, uint64_t first, uint64_t n, const int64_t* values) {
+  return set_per_point(h, first, n, values, "attributes", "values is NULL", &Index::set_attributes);
+}
+int hnsw_b200_get_attributes(const void* h, uint64_t first, uint64_t n, int64_t* out) {
+  HB_HS(h);
+  if (label_range(ix, first, n, "attributes")) return -1;
+  if (n == 0) return 0;
+  if (!out) return set_err("out is NULL");
+  HB_PARTS_SHARED_IF(ix);
+  return for_label_range(ix, first, n, [&](Index* x, int, uint64_t lo, uint64_t cnt, uint64_t stride, uint64_t at) {
+    for (uint64_t i = 0; i < cnt; ++i) out[at + i * stride] = hb::attr_unbias(x->h_attr[lo + i]);
     return 0;
   });
 }
@@ -824,6 +854,30 @@ int hnsw_b200_search_exact_label_sets(const void* h, const uint64_t* qset_off, c
                                       uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
   return (int)search_call(h, HOST, "search_exact_label_sets", row_label_sets(qset_off, qset), true, queries, nq, dim, knbn,
                           0, columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+}
+
+// Attribute ranges.  Query i is restricted to the points whose attribute is in [qrange[2i], qrange[2i + 1]]
+// ([INT64_MIN, INT64_MAX]: every point, also those without one) and whose label is one of qset[qset_off[i],
+// qset_off[i + 1]) ({LABEL_NONE}: any; qset_off and qset both NULL: {LABEL_NONE} for every query); the graph search
+// (ef_search) or the exact scan.
+static int ranged_call(const void* h, const char* name, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                       bool exact, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef,
+                       const AnswerArrays& out) {
+  if (h && nq && !qrange) return set_err("qrange is NULL");  // search_call answers a NULL handle and nq == 0 first
+  return (int)search_call(h, HOST, name, row_label_sets(qset_off, qset, qrange), exact, queries, nq, dim, knbn, ef, out);
+}
+int hnsw_b200_search_flat_ranges(const void* h, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                                 const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
+                                 uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
+                                 int32_t* out_counts) {
+  return ranged_call(h, "search_flat_ranges", qrange, qset_off, qset, false, queries, nq, dim, knbn, ef_search,
+                     columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+}
+int hnsw_b200_search_exact_ranges(const void* h, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                                  const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids,
+                                  float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+  return ranged_call(h, "search_exact_ranges", qrange, qset_off, qset, true, queries, nq, dim, knbn, 0,
+                     columns(out_ids, out_dist, out_internal, out_pid, out_counts));
 }
 
 int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,

@@ -10,7 +10,8 @@
 // So here C is a real queue: an unsorted array of keys per warp in global memory, pop = warp-wide min scan
 // (consumed entries are overwritten with ~0).  W is the same sorted shared-memory array as elsewhere.
 // The FilterT predicate (filter.rs:7-24) is a device bitmap over internal ids, materialised by the host, or a point
-// label: the predicate label(p) == L, or label(p) in a set S of labels, over the label array of the graph store.
+// label: the predicate label(p) == L, or label(p) in a set S of labels, over the label array of the graph store; and,
+// alone or with a label part, a range lo <= attr(p) <= hi over the attribute array of the graph store.
 #include "kernels.h"
 #include "search_core.cuh"
 
@@ -45,9 +46,16 @@ template <> struct SetLookupCall<OpCast<uint32_t, OpL2>> { static constexpr bool
 template <> struct SetLookupCall<OpJaccard<uint8_t>> { static constexpr bool value = true; };
 template <> struct SetLookupCall<OpJaccard<uint16_t>> { static constexpr bool value = true; };
 
-// the one admission test: the point's label against the query's label or set, or its bit of the bitmap
+// the one admission test: the point's attribute against the query's range, then the point's label against the query's
+// label or set, or its bit of the bitmap
 template <class Op>
 __device__ __forceinline__ bool filter_pass(const RowFilter* f, uint32_t id) {
+  const uint64_t* attr = f->attr;
+  if (attr) {
+    const uint64_t v = __ldg(attr + id);
+    if (v < f->lo || v > f->hi) return false;
+  }
+  if (!f->ptr) return true;
   const uint32_t want = f->label;
   if (want != LABEL_NONE) {
     const uint32_t lab = __ldg(f->ptr + id);
@@ -200,6 +208,7 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
                    reinterpret_cast<uint32_t*>(base + L.cand_id), reinterpret_cast<float*>(base + L.cand_d)};
   // the query's filter, read at each use so that the search loop holds no register for it: in the upper half of the
   // candidate-distance region, whose first 32 of 64 reserved entries are all this kernel scores into
+  static_assert(sizeof(RowFilter) <= 32 * 4, "a RowFilter fits the upper half of the candidate-distance region");
   RowFilter* fslot = reinterpret_cast<RowFilter*>(base + L.cand_d + 32 * 4);
   const uint32_t slot = blockIdx.x * (blockDim.x >> 5) + warp;  // the host launches fewer warps per CTA when shared memory is short
   Visited vis;

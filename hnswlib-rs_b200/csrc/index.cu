@@ -97,6 +97,8 @@ Index::~Index() {
   for (void* a : graph_.p) cudaFree(a);
   cudaFree(vis_.tab); cudaFree(vis_.epoch); cudaFree(d_counter_); cudaFree(d_status_); cudaFree(d_stats_); cudaFree(d_mask_);
   cudaFree(label_csr_.d_ids);
+  cudaFree(by_value_.d_ids);
+  cudaFree(by_label_value_.d_ids);
   if (h_pin_) cudaFreeHost(h_pin_);
   for (SearchCtx& c : ctx_) {
     if (c.stream) cudaStreamSynchronize(c.stream);
@@ -355,6 +357,7 @@ void Index::resize_points(size_t count) {
   h_rank.resize(count);
   h_origin.resize(count);
   h_label.resize(count, LABEL_NONE);
+  h_attr.resize(count, attr_bias(ATTR_NONE));
   h_upoff.resize(count);
 }
 
@@ -370,6 +373,7 @@ int Index::upload_points(size_t first, size_t count) {
   HB_CUDA(cudaMemcpyAsync(graph_.at<uint64_t>(GS::ORIGIN) + first, h_origin.data() + first, count * 8, cudaMemcpyHostToDevice, stream_));
   HB_CUDA(cudaMemcpyAsync(graph_.at<uint32_t>(GS::UP_OFF) + first, h_upoff.data() + first, count * 4, cudaMemcpyHostToDevice, stream_));
   HB_CUDA(cudaMemcpyAsync(graph_.at<uint32_t>(GS::LABEL) + first, h_label.data() + first, count * 4, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.at<uint64_t>(GS::ATTR) + first, h_attr.data() + first, count * 8, cudaMemcpyHostToDevice, stream_));
   return 0;
 }
 
@@ -727,7 +731,7 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.filter = f.filter;
   p.stats = stats_on_ ? d_stats_ : nullptr;
   p.status = c.d_status;
-  const bool filtered = f.sel != nullptr || f.filter.ptr != nullptr;
+  const bool filtered = f.sel != nullptr || f.filter.ptr != nullptr || f.filter.attr != nullptr;
   QueryKernel kind = QueryKernel::Generic;
   if (filtered) kind = QueryKernel::Filtered;
   else if (tie_std_) kind = QueryKernel::StdTie;  // unfiltered searches only
@@ -909,11 +913,12 @@ int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** 
 }
 
 // Graph: one RowFilter per run, a bitmap (a FilterT's host bits uploaded into the context first), a label (a set of one,
-// which the kernel compares) or a set (its values uploaded).  One run goes to the launch by value, as a batch-wide
-// filter does; several as a table of them and each row's entry in it, uploaded into the context's filter scratch ahead
-// of the words the runs read there.  Exact: a group of every point for the unrestricted rows, and one per run; a run of
-// one slice scans it in place, any other its slices copied one after the other into the context (a point has one label,
-// so a label set's slices are disjoint, and the exact scan orders by (distance, id), so their order does not matter).
+// which the kernel compares), a set (its values uploaded) or none ({LABEL_NONE}), each with the run's attribute range
+// if it has one.  One run goes to the launch by value, as a batch-wide filter does; several as a table of them and each
+// row's entry in it, uploaded into the context's filter scratch ahead of the words the runs read there.  Exact: a group
+// of every point for the unrestricted rows, and one per run; a run of one slice scans it in place, any other its slices
+// copied one after the other into the context (a point has one label, so a label set's slices are disjoint, and the
+// exact scan keeps the k smallest (distance, id) keys, so the order of the ids does not matter).
 int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
   cudaStream_t st = c.stream;
   int r;
@@ -956,15 +961,22 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
   std::vector<RowFilter> table;
   std::vector<uint32_t> sel, vals;  // vals: the host words to upload at `at`
   for (const LegPlan::Run& u : plan.runs) {
-    RowFilter f{u.bits, nullptr, LABEL_NONE, 0};  // a resident filter: already on this device
+    RowFilter f{u.bits, nullptr, LABEL_NONE, 0, nullptr, 0, 0};  // a resident filter: already on this device
     if (u.host_bits) {
       f.ptr = at + vals.size();
       vals.insert(vals.end(), u.host_bits, u.host_bits + fw);
+    } else if (u.nset == 1 && u.set[0] == LABEL_NONE) {
+      f.ptr = nullptr;  // a range alone
     } else if (u.nset == 1) {
-      f = RowFilter{plan.labels, nullptr, u.set[0], 0};
+      f = RowFilter{plan.labels, nullptr, u.set[0], 0, nullptr, 0, 0};
     } else if (plan.labels) {
-      f = RowFilter{plan.labels, at + vals.size(), 0, u.nset};
+      f = RowFilter{plan.labels, at + vals.size(), 0, u.nset, nullptr, 0, 0};
       vals.insert(vals.end(), u.set, u.set + u.nset);
+    }
+    if (u.ranged) {
+      f.attr = plan.attrs;
+      f.lo = u.lo;
+      f.hi = u.hi;
     }
     if (several) sel.insert(sel.end(), u.count, (uint32_t)table.size());
     table.push_back(f);

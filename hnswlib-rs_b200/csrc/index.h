@@ -61,9 +61,9 @@ struct DevBuf {  // device memory freed on scope exit, so that no early return l
 };
 
 // The device arrays that hold the graph.  Replication blob i is array i, in this order (the order is part of the blob
-// protocol between processes); the per-point insert locks and labels come last and are not replicated.
+// protocol between processes); the per-point insert locks, labels and attributes come last and are not replicated.
 struct GraphStore {
-  enum Array { VEC, ADJ0, ADJU, UP_OFF, PLEVEL, LEVEL, ORIGIN, ADJ0_D, ADJU_D, LOCKS, LABEL, COUNT };
+  enum Array { VEC, ADJ0, ADJU, UP_OFF, PLEVEL, LEVEL, ORIGIN, ADJ0_D, ADJU_D, LOCKS, LABEL, ATTR, COUNT };
   static constexpr int BLOBS = LOCKS;
   // elements per point: a vector row (row_bytes), a layer-0 list (2M), one; or per upper-layer list: a list (M)
   enum Row { VEC_ROW, LIST0, ONE, LISTU };
@@ -84,6 +84,7 @@ struct GraphStore {
       {4, LISTU, 0},     // ADJU_D
       {4, ONE, 0},       // LOCKS
       {4, ONE, 0xFF},    // LABEL: the point's label, LABEL_NONE = none
+      {8, ONE, 0},       // ATTR: the point's attribute, attr_bias(value), 0 = none (attr_bias(ATTR_NONE))
   };
   void* p[COUNT] = {};
   size_t cap = 0, cap_ul = 0;  // points / upper-layer lists allocated
@@ -106,8 +107,8 @@ int dtype_from_type_name(const std::string& s);
 
 class Index;
 
-// The points an exact scan (exact_knn_kernel, aux.cu) covers: `ids`, n sorted internal ids on the scanning device, or
-// every stored point (ids == nullptr)
+// The points an exact scan (exact_knn_kernel, aux.cu) covers: `ids`, n distinct internal ids on the scanning device in
+// any order, or every stored point (ids == nullptr)
 struct ExactScan {
   const uint32_t* ids = nullptr;
   size_t n = 0;
@@ -119,10 +120,10 @@ struct ExactGroup {
   ExactScan scan;
 };
 
-// The restriction of one search launch, as SearchParams reads it: none (sel and filter.ptr null), `filter` for every row,
-// or row i under table[sel[i]]
+// The restriction of one search launch, as SearchParams reads it: none (sel, filter.ptr and filter.attr null), `filter`
+// for every row, or row i under table[sel[i]]
 struct LaunchFilter {
-  RowFilter filter{nullptr, nullptr, LABEL_NONE, 0};
+  RowFilter filter{nullptr, nullptr, LABEL_NONE, 0, nullptr, 0, 0};
   const RowFilter* table = nullptr;
   const uint32_t* sel = nullptr;
 };
@@ -207,7 +208,9 @@ struct AnswerArrays {
 // What the rows of a batch may return: every point (NONE); the points a FilterT admits (FILTER_T: `mode` 1 sorted
 // origin-id list, 2 callback, as make_filter_bits reads it); one resident filter for every row (RESIDENT); a resident
 // filter per row, -1 = none (ROW_FILTERS); or a set of labels per row (a label per row: sets of one), row i's the values
-// qset[qset_off[i], qset_off[i + 1]) in any order and with repeats, {LABEL_NONE} = none (ROW_LABEL_SETS)
+// qset[qset_off[i], qset_off[i + 1]) in any order and with repeats, {LABEL_NONE} = none (ROW_LABEL_SETS), each within an
+// attribute range when qrange is set: row i's [qrange[2i], qrange[2i + 1]], inclusive, [INT64_MIN, INT64_MAX] = none.
+// qset_off and qset both null with qrange: every row's set is {LABEL_NONE}.
 struct Restriction {
   enum Kind { NONE, FILTER_T, RESIDENT, ROW_FILTERS, ROW_LABEL_SETS } kind = NONE;
   int mode = 0;
@@ -219,14 +222,17 @@ struct Restriction {
   const int64_t* filters = nullptr;  // [nq]
   const uint64_t* qset_off = nullptr;  // [nq + 1]
   const uint32_t* qset = nullptr;
+  const int64_t* qrange = nullptr;  // [2 nq]
   bool per_row() const { return kind == ROW_FILTERS || kind == ROW_LABEL_SETS; }
 };
 
-// The distinct label sets of a ROW_LABEL_SETS batch (Index::sort_rows): set j is values[off[j], off[j + 1]), ascending
-// and without repeats
+// The distinct (label set, range) pairs of a ROW_LABEL_SETS batch (Index::sort_rows): set j is values[off[j], off[j + 1]),
+// ascending and without repeats, within the biased attribute range [range[2j], range[2j + 1]] (attr_bias; lo >= 1); with
+// no range when range is empty (a batch without ranges) or range[2j] is 0
 struct LabelSets {
   std::vector<uint32_t> values;
   std::vector<size_t> off;
+  std::vector<uint64_t> range;
 };
 
 // One host search batch: flat queries or one pointer per query (rows), k answers each into `out`.  `exact`: the exact
@@ -244,8 +250,9 @@ struct HostBatch {
 
 // A leg's restriction (Index::resolve): its rows [0, plain) are unrestricted, and `runs` cover the rest, each a range of
 // consecutive rows under one restriction: a bitmap (a resident filter's on the leg's device, or a FilterT's host bits,
-// uploaded into the context when the leg begins) or a label set on `labels` (the label array on the leg's device).  In
-// an exact batch its points are slices [slice, slice + nslices): a filter's id list, or a label set's CSR slices.  A
+// uploaded into the context when the leg begins) or a label set on `labels` (the label array on the leg's device), the
+// latter within an attribute range on `attrs` when it is `ranged`.  In an exact batch its points are slices [slice,
+// slice + nslices): a filter's id list, a label set's CSR slices, or a ranged run's slices of the attribute orders.  A
 // batch-wide filter is a plan with no prefix and one run over every row.
 struct LegPlan {
   struct Run {
@@ -254,6 +261,8 @@ struct LegPlan {
     const uint32_t* host_bits = nullptr;
     const uint32_t* set = nullptr;  // the run's label set, nset values of a LabelSets
     uint32_t nset = 0;
+    bool ranged = false;  // the run's attribute range, biased bounds of a LabelSets
+    uint64_t lo = 0, hi = 0;
     size_t slice = 0, nslices = 0;
   };
   bool exact = false;
@@ -261,6 +270,7 @@ struct LegPlan {
   std::vector<Run> runs;
   std::vector<ExactScan> slices;
   const uint32_t* labels = nullptr;
+  const uint64_t* attrs = nullptr;  // the attribute array on the leg's device, when a run has a range
 };
 
 // One Index's part of a batch: queries [first, first + count) searched on rx (the handle, a replica, or partition `part`)
@@ -303,6 +313,7 @@ class Index {
   std::vector<int32_t> h_rank;
   std::vector<uint64_t> h_origin;
   std::vector<uint32_t> h_label;  // LABEL_NONE = none (labels.cu)
+  std::vector<uint64_t> h_attr;   // attr_bias(value), 0 = none (labels.cu)
   std::vector<uint32_t> h_upoff;
 
   // ---- operations (return 0 or a negative status; message in err())
@@ -365,6 +376,18 @@ class Index {
   // the points whose label is one of set[0, nset) (ascending), appended to `slices`: one slice of the label CSR (rebuilt
   // when the labels changed) per label that some point carries, slices that follow each other in the CSR joined
   int label_set_scan(const uint32_t* set, size_t nset, std::vector<ExactScan>& slices);
+  // ---- point attributes (labels.cu).  One int64 per point (GraphStore ATTR and its host mirror h_attr, both biased by
+  // attr_bias), ATTR_NONE until set_attributes names one; attr_version counts the calls that changed them (a replica: the
+  // handle's version it copied).
+  uint64_t attr_version = 0;
+  // values[0, count) for the points [first, first + count) of this Index (the caller checked the range)
+  int set_attributes(size_t first, size_t count, const int64_t* values);
+  // the attribute array on this Index's device, as current as `src`'s (labels_on_device's twin)
+  int attrs_on_device(const Index* src, const uint64_t** d_attrs);
+  // the points whose attribute is in [lo, hi] (biased, lo >= 1) and, unless set is {LABEL_NONE}, whose label is one of
+  // set[0, nset) (ascending), appended to `slices`: one slice of the value order, or one of the label-value order per
+  // label of the set (each order rebuilt when what it sorts by changed), slices that follow each other joined
+  int attr_range_scan(const uint32_t* set, size_t nset, uint64_t lo, uint64_t hi, std::vector<ExactScan>& slices);
   // device queries in, device answers out; the restriction is none or a resident filter.  `exact`: the exact scan (ef
   // unused).
   int search_device(const Restriction& rs, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef,
@@ -503,7 +526,7 @@ class Index {
   // ---- point ledger: the host mirrors (h_level ... h_upoff) and the per-layer counts
   void resize_points(size_t count);
   void rank_points();  // layer_count and h_rank from h_level, in internal-id order
-  int upload_points(size_t first, size_t count);  // level, plevel, origin, up_off, label of [first, first + count)
+  int upload_points(size_t first, size_t count);  // level, plevel, origin, up_off, label, attr of [first, first + count)
   // ---- graph export
   struct ListRef {  // a point's list at one layer: adj0 (layer 0) or adjU from element `at`, `cap` slots (0: none)
     size_t at, cap;
@@ -550,6 +573,19 @@ class Index {
     uint64_t version = ~0ull;
     std::unordered_map<uint32_t, std::pair<uint32_t, uint32_t>> groups;
   } label_csr_;
+  // The orders of the exact ranged path, made from h_attr (and h_label) at the first exact ranged search after what they
+  // sort by changed: the internal ids of every point with an attribute by (value, id), and of every point with a label
+  // and an attribute by (label, value, id) with each label's (offset, count).  The sorted values stay on the host for the
+  // binary searches, the ids go to the device.  A point added since has neither, so inserts leave them current.
+  struct AttrOrder {
+    void* d_ids = nullptr;
+    size_t bytes = 0;
+    uint64_t version = ~0ull, lversion = ~0ull;  // attr_version (and label_version) it was made at
+    std::vector<uint64_t> values;                // biased, in the order of the ids
+    std::unordered_map<uint32_t, std::pair<uint32_t, uint32_t>> groups;
+  } by_value_, by_label_value_;
+  int make_attr_order(AttrOrder& o, bool by_label);
+  // label_mu_ guards the label CSR, both attribute orders and a replica's copy of the labels and attributes
   std::mutex label_mu_;
 
   int broadcast_to_replicas();

@@ -41,14 +41,19 @@ struct NeighbourOut {
   uint32_t internal;
 };
 
-// the restriction of one row of a filtered launch: a bitmap over internal ids (label == LABEL_NONE), or the label array
-// and the one label the row admits (set == nullptr), or the label array and the row's set, set[0, nset) ascending (set
-// is not nullptr, also when the set is empty, and label is then any value but LABEL_NONE)
+// the restriction of one row of a filtered launch, two parts that both must admit a point:
+//   * none (ptr == nullptr), a bitmap over internal ids (label == LABEL_NONE), or the label array and the one label the
+//     row admits (set == nullptr), or the label array and the row's set, set[0, nset) ascending (set is not nullptr,
+//     also when the set is empty, and label is then any value but LABEL_NONE);
+//   * none (attr == nullptr), or the attribute array (attr_bias values) and the range lo <= attr[p] <= hi, biased
+//     bounds with lo >= 1, so that a point without an attribute (0) is never in it.
 struct RowFilter {
   const uint32_t* ptr;
   const uint32_t* set;
   uint32_t label;
   uint32_t nset;
+  const uint64_t* attr;
+  uint64_t lo, hi;
 };
 
 struct SearchParams {
@@ -80,6 +85,13 @@ struct SearchParams {
 
 // the label of a point that has none (hnsw_b200_set_labels): no label admits it
 constexpr uint32_t LABEL_NONE = 0xFFFFFFFFu;
+
+// A point's int64 attribute (hnsw_b200_set_attributes) is stored as its bits with the sign bit flipped, so that the
+// unsigned order of the stored values is the signed order of the attributes and HNSW_B200_ATTR_NONE (INT64_MIN), the
+// attribute of a point that has none, is 0: the byte the graph store fills new space with.
+__host__ __device__ constexpr uint64_t attr_bias(int64_t v) { return (uint64_t)v ^ 0x8000000000000000ull; }
+__host__ __device__ constexpr int64_t attr_unbias(uint64_t b) { return (int64_t)(b ^ 0x8000000000000000ull); }
+constexpr int64_t ATTR_NONE = (int64_t)0x8000000000000000ull;
 
 // rows of up to 512 bytes are (partly) staged by TMA: STAGE_ROWS rows + an mbarrier per warp
 __host__ __device__ inline size_t stage_bytes(int d4) { return d4 <= 32 ? (size_t)STAGE_ROWS * d4 * 16 : 0; }
@@ -170,7 +182,7 @@ __host__ __device__ inline ExactLayout exact_layout(int d4, int k, int tq, int r
 }
 
 // one tile of an exact launch whose tiles differ (a filter per query): queries [q0, q0 + nq) of the launch, scanned over
-// `list` (npts sorted internal ids) or, with list == nullptr, over the points 0 .. npts - 1
+// `list` (npts distinct internal ids, in any order) or, with list == nullptr, over the points 0 .. npts - 1
 struct ExactTile {
   uint32_t q0, nq;
   const uint32_t* list;

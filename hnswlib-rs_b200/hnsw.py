@@ -110,6 +110,10 @@ def load_library():
     L.hnsw_b200_search_exact_labeled.argtypes = [vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_flat_label_sets.argtypes = [vp, vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_exact_label_sets.argtypes = [vp, vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_set_attributes.argtypes = [vp, u64, u64, vp]
+    L.hnsw_b200_get_attributes.argtypes = [vp, u64, u64, vp]
+    L.hnsw_b200_search_flat_ranges.argtypes = [vp, vp, vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_exact_ranges.argtypes = [vp, vp, vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_get_stats.argtypes = [vp, vp, i32]
     L.hnsw_b200_set_stream.argtypes = [vp, vp]
     L.hnsw_b200_join.argtypes = [vp]
@@ -280,6 +284,36 @@ def _label_sets(sets, nq):
         vals = np.concatenate(parts) if parts else np.zeros(0, np.int64)
     vals = _labels(vals, vals.size, "sets")
     return off, vals if vals.size else np.zeros(1, np.uint32)   # never a NULL pointer
+
+
+ATTR_NONE = -(1 << 63)   # hnsw_b200.h HNSW_B200_ATTR_NONE: the attribute of a point that has none
+RANGE_ALL = (-(1 << 63), (1 << 63) - 1)   # the range of a query that has none: every point, also those without one
+
+
+def attr_of_float(x):
+    """an int64 attribute for the float x, in x's order, so that scores or prices can be attributes: the bits of x for
+    x >= 0, and for x < 0 the bits with their 63 low bits flipped; -0.0 is taken as +0.0.  Never ATTR_NONE.  A float
+    array gives an int64 array.  NaN is refused."""
+    a = np.asarray(x, np.float64)
+    if np.isnan(a).any():
+        raise ValueError("attr_of_float: NaN has no place in the order")
+    b = (a + 0.0).view(np.int64)   # -0.0 + 0.0 is +0.0
+    out = np.where(b < 0, b ^ np.int64((1 << 63) - 1), b)
+    return int(out) if out.ndim == 0 else out
+
+
+def _ranges(ranges, nq):
+    """the ranges argument of the ranged searches: an (nq, 2) int64 array or a sequence of nq (lo, hi) pairs, as a
+    contiguous int64 array of 2 nq bounds"""
+    a = np.asarray(ranges)
+    if a.shape != (nq, 2) and not (nq == 0 and a.size == 0):
+        raise ValueError(f"ranges has shape {a.shape}, expected ({nq}, 2)")
+    if a.size and a.dtype.kind not in "iu":
+        raise ValueError("ranges: bounds are 64-bit integers (attr_of_float maps floats)")
+    if a.size and a.dtype.kind == "u" and a.max() > np.iinfo(np.int64).max:
+        raise ValueError("ranges: bounds are signed 64-bit integers")
+    a = np.ascontiguousarray(a, np.int64).reshape(-1)
+    return a if a.size else np.zeros(2, np.int64)   # never a NULL pointer
 
 
 class Hnsw:
@@ -543,6 +577,44 @@ class Hnsw:
         off, vals = _label_sets(sets, q.shape[0])
         return self._host_search(self._L.hnsw_b200_search_exact_label_sets, (_p(off), _p(vals)), q, knbn, (),
                                  with_internal, with_pid)
+
+    def set_attributes(self, first, values):
+        """hnsw_b200_set_attributes: the int64 attributes of the points with insertion ranks first .. first +
+        len(values) - 1 (ATTR_NONE clears one).  Every point starts without an attribute."""
+        v = np.asarray(values).reshape(-1)
+        if v.size and v.dtype.kind not in "iu":
+            raise ValueError("attributes are 64-bit integers (attr_of_float maps floats)")
+        if v.size and v.dtype.kind == "u" and v.max() > np.iinfo(np.int64).max:
+            raise ValueError("attributes are signed 64-bit integers")
+        v = np.ascontiguousarray(v, np.int64)
+        self._chk(self._L.hnsw_b200_set_attributes(self._h, int(first), v.size, _p(v)))
+
+    def get_attributes(self, first, n):
+        """hnsw_b200_get_attributes: the attributes of the points first .. first + n - 1, as int64 (ATTR_NONE: none)"""
+        out = np.empty(int(n), np.int64)
+        self._chk(self._L.hnsw_b200_get_attributes(self._h, int(first), int(n), _p(out)))
+        return out
+
+    def _ranged(self, fn, queries, knbn, mid, ranges, sets, with_internal, with_pid):
+        q = np.ascontiguousarray(queries, self.dtype)
+        rg = _ranges(ranges, q.shape[0])
+        off, vals = (None, None) if sets is None else _label_sets(sets, q.shape[0])
+        return self._host_search(fn, (_p(rg), _p(off), _p(vals)), q, knbn, mid, with_internal, with_pid)
+
+    def search_flat_ranges(self, queries, knbn, ef, ranges, sets=None, with_internal=True, with_pid=True):
+        """hnsw_b200_search_flat_ranges: one batch, query i restricted to the points whose attribute lies in
+        ranges[i] = (lo, hi), inclusive (RANGE_ALL: every point, also those without one; lo > hi: none), and, with sets
+        (as search_flat_label_sets takes it), whose label is in sets[i].  Row i equals search_flat with a resident
+        filter admitting exactly those points.  Returns search_flat's (origin, dist, internal | None, pid | None,
+        counts)."""
+        return self._ranged(self._L.hnsw_b200_search_flat_ranges, queries, knbn, (int(ef),), ranges, sets, with_internal,
+                            with_pid)
+
+    def search_exact_ranges(self, queries, knbn, ranges, sets=None, with_internal=True, with_pid=True):
+        """hnsw_b200_search_exact_ranges: the exact knbn nearest of query i among the points search_flat_ranges
+        admits for it, in one batch.  Returns search_exact's tuple."""
+        return self._ranged(self._L.hnsw_b200_search_exact_ranges, queries, knbn, (), ranges, sets, with_internal,
+                            with_pid)
 
     def make_filter(self, filter):
         """hnsw_b200_filter_new: materialise a FilterT (sorted id sequence or callable(id)->bool, as search_flat takes)

@@ -99,7 +99,21 @@ extern "C" {
     fn hnsw_b200_search_exact_label_sets(h: *const HnswApif32, qset_off: *const u64, qset: *const u32, queries: *const f32,
                                          nq: u64, dim: u64, knbn: u64, out_ids: *mut u64, out_dist: *mut f32,
                                          out_internal: *mut u32, out_pid: *mut i32, out_counts: *mut i32) -> c_int;
+    // attribute ranges (include/hnsw_b200.h "Attribute ranges"): query i's range is qrange[2i] ..= qrange[2i + 1]
+    fn hnsw_b200_set_attributes(h: *mut HnswApif32, first: u64, n: u64, values: *const i64) -> c_int;
+    fn hnsw_b200_get_attributes(h: *const HnswApif32, first: u64, n: u64, out: *mut i64) -> c_int;
+    fn hnsw_b200_search_flat_ranges(h: *const HnswApif32, qrange: *const i64, qset_off: *const u64, qset: *const u32,
+                                    queries: *const f32, nq: u64, dim: u64, knbn: u64, ef: u64, out_ids: *mut u64,
+                                    out_dist: *mut f32, out_internal: *mut u32, out_pid: *mut i32, out_counts: *mut i32) -> c_int;
+    fn hnsw_b200_search_exact_ranges(h: *const HnswApif32, qrange: *const i64, qset_off: *const u64, qset: *const u32,
+                                     queries: *const f32, nq: u64, dim: u64, knbn: u64, out_ids: *mut u64, out_dist: *mut f32,
+                                     out_internal: *mut u32, out_pid: *mut i32, out_counts: *mut i32) -> c_int;
 }
+
+/// The attribute of a point that has none (include/hnsw_b200.h HNSW_B200_ATTR_NONE): no range admits it.
+pub const ATTR_NONE: i64 = i64::MIN;
+/// The range of a request that has none: every point, also those without an attribute.
+pub const RANGE_ALL: (i64, i64) = (i64::MIN, i64::MAX);
 
 /// The label of a point that has none (include/hnsw_b200.h HNSW_B200_LABEL_NONE): no label admits it.
 pub const LABEL_NONE: u32 = 0xFFFF_FFFF;
@@ -349,6 +363,59 @@ impl<D: DistName> Hnsw<D> {
             }
         };
         assert_eq!(r, 0, "hnsw_b200_search_flat_label_sets / _exact_label_sets failed");
+        (0..nq).map(|i| (0..cnt[i] as usize).map(|j| {
+            let s = i * knbn + j;
+            Neighbour { d_id: ids[s] as usize, distance: ds[s], p_id: PointId(pid[2 * s] as u8, pid[2 * s + 1]) }
+        }).collect()).collect()
+    }
+    /// Extension: give the points with insertion ranks `first .. first + values.len()` an int64 attribute (ATTR_NONE
+    /// clears one).  Every point starts without one; attributes are not written into dumps.  Err when the range passes
+    /// nb_point.
+    pub fn set_attributes(&mut self, first: usize, values: &[i64]) -> Result<(), i32> {
+        let r = unsafe { hnsw_b200_set_attributes(self.h, first as u64, values.len() as u64, values.as_ptr()) };
+        if r == 0 { Ok(()) } else { Err(r) }
+    }
+    /// Extension: the attributes of the points `first .. first + n`
+    pub fn get_attributes(&self, first: usize, n: usize) -> Result<Vec<i64>, i32> {
+        let mut out = vec![0i64; n];
+        let r = unsafe { hnsw_b200_get_attributes(self.h, first as u64, n as u64, out.as_mut_ptr()) };
+        if r == 0 { Ok(out) } else { Err(r) }
+    }
+    /// Extension: one batch, request i restricted to the points whose attribute lies in `ranges[i]` (inclusive;
+    /// RANGE_ALL: every point, also those without one) and, with `sets`, whose label is one of `sets[i]` (as
+    /// search_label_sets takes it); answer i is what search_resident returns with a filter admitting exactly those
+    /// points.  Graph search with `Some(ef)`, the exact scan with None.
+    pub fn search_ranges(&self, datas: &[Vec<f32>], knbn: usize, ef: Option<usize>, ranges: &[(i64, i64)],
+                         sets: Option<&[Vec<u32>]>) -> Vec<Vec<Neighbour>> {
+        assert_eq!(datas.len(), ranges.len(), "one range per request");
+        if let Some(s) = sets { assert_eq!(datas.len(), s.len(), "one label set per request"); }
+        if datas.is_empty() { return Vec::new(); }
+        let (nq, dim) = (datas.len(), datas[0].len());
+        let flat: Vec<f32> = datas.iter().flat_map(|d| d.iter().copied()).collect();
+        let qrange: Vec<i64> = ranges.iter().flat_map(|&(lo, hi)| [lo, hi]).collect();
+        let (mut off, mut vals) = (Vec::new(), Vec::new());
+        if let Some(sets) = sets {
+            off = vec![0u64; nq + 1];
+            for (i, s) in sets.iter().enumerate() { off[i + 1] = off[i] + s.len() as u64; }
+            vals = sets.iter().flat_map(|s| s.iter().copied()).collect();
+            vals.push(LABEL_NONE);  // never empty, so never a null pointer; past every set's end
+        }
+        let (po, pv) = if sets.is_some() { (off.as_ptr(), vals.as_ptr()) } else { (std::ptr::null(), std::ptr::null()) };
+        let mut ids = vec![0u64; nq * knbn];
+        let mut ds = vec![0f32; nq * knbn];
+        let mut pid = vec![0i32; 2 * nq * knbn];
+        let mut cnt = vec![0i32; nq];
+        let r = unsafe {
+            match ef {
+                Some(ef) => hnsw_b200_search_flat_ranges(self.h, qrange.as_ptr(), po, pv, flat.as_ptr(), nq as u64, dim as u64,
+                                                         knbn as u64, ef as u64, ids.as_mut_ptr(), ds.as_mut_ptr(),
+                                                         std::ptr::null_mut(), pid.as_mut_ptr(), cnt.as_mut_ptr()),
+                None => hnsw_b200_search_exact_ranges(self.h, qrange.as_ptr(), po, pv, flat.as_ptr(), nq as u64, dim as u64,
+                                                      knbn as u64, ids.as_mut_ptr(), ds.as_mut_ptr(), std::ptr::null_mut(),
+                                                      pid.as_mut_ptr(), cnt.as_mut_ptr()),
+            }
+        };
+        assert_eq!(r, 0, "hnsw_b200_search_flat_ranges / _exact_ranges failed");
         (0..nq).map(|i| (0..cnt[i] as usize).map(|j| {
             let s = i * knbn + j;
             Neighbour { d_id: ids[s] as usize, distance: ds[s], p_id: PointId(pid[2 * s] as u8, pid[2 * s + 1]) }

@@ -427,6 +427,42 @@ int hnsw_b200_search_exact_label_sets(const void* h, const uint64_t* qset_off, c
                                       uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids, float* out_dist,
                                       uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
 
+/* ---- Attribute ranges: one int64 attribute per point (a timestamp, a version, a price), and searches in which each
+ * query is restricted to a range of it, alone or within a label set ("this tenant, this week").  An attribute costs 8
+ * bytes per point on the device and on the host, a query names its own range, and no insert makes it stale.  The exact
+ * ranged search also keeps, from its first call on, two orders of the points per index: up to 4 + 4 bytes per point
+ * of ids on the device and 8 + 8 bytes per point of sorted values on the host (by value, and by label and value, each
+ * over the points with an attribute, the second only over those that also have a label).
+ *   Attributes: every point starts with HNSW_B200_ATTR_NONE (new inserts, imports, reloaded dumps and replication
+ *     blobs).  They are not written into the dump files (get_attributes reads them back) and nccl_broadcast_index does
+ *     not broadcast them.  set_attributes / get_attributes address insertion ranks [first, first + n) exactly as
+ *     set_labels / get_labels do, with the same range check, locks and partition placement; HNSW_B200_ATTR_NONE clears
+ *     an attribute.  No attribute call reads or changes labels or resident filters, and no label or filter call reads or
+ *     changes attributes.
+ *   Rows: query i's range is [qrange[2i], qrange[2i + 1]], inclusive, and its label set S_i is as search_*_label_sets
+ *     take it (qset_off and qset both NULL: S_i = {HNSW_B200_LABEL_NONE} for every query).  Row i admits point p when
+ *     p's label is in S_i or S_i = {HNSW_B200_LABEL_NONE}, and p has an attribute with qrange[2i] <= value(p) <=
+ *     qrange[2i + 1].  The full range [INT64_MIN, INT64_MAX] is no range: it also admits points without an attribute,
+ *     so with S_i = {HNSW_B200_LABEL_NONE} it gives the unfiltered search_flat / search_exact row (which follows the tie
+ *     mode), and with any other S_i the search_*_label_sets row.  lo > hi admits no point (count 0).
+ *   Answers: row i is, bit for bit, what search_flat_filtered / search_exact return for query i with a resident filter
+ *     that admits exactly the points row i admits (ids, distance bits, internal ids, PointIds, count); restricted rows
+ *     ignore the tie mode.  With statistics on, the counters add up as search_*_label_sets' do.
+ *   Checks: those of search_*_label_sets, with their wording; qrange NULL with nq > 0 is refused, and so is exactly one
+ *     of qset_off and qset NULL.  A NULL handle is refused and nq == 0 returns 0 before any other check.
+ *   Handles: as search_*_label_sets; a replica's device gets a copy of the attributes at its first ranged search after
+ *     they changed, and a partition view searches with its own partition's attributes and reports local ids. */
+#define HNSW_B200_ATTR_NONE INT64_MIN /* the attribute of a point that has none */
+int hnsw_b200_set_attributes(void* h, uint64_t first, uint64_t n, const int64_t* values);
+int hnsw_b200_get_attributes(const void* h, uint64_t first, uint64_t n, int64_t* out);
+int hnsw_b200_search_flat_ranges(const void* h, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                                 const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
+                                 uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
+                                 int32_t* out_counts);
+int hnsw_b200_search_exact_ranges(const void* h, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                                  const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids,
+                                  float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
+
 /* Run this handle's kernels and copies on a caller-owned CUDA stream (cudaStream_t passed as void*; NULL
  * restores the handle's own stream), e.g. so that torch.cuda.Event on torch's current stream brackets them. */
 int hnsw_b200_join(void* h);
