@@ -634,10 +634,8 @@ static int64_t search_call(const void* h, Via via, const char* name, const Restr
     return pass(ix, ix->search_device(rs, exact, queries, nq, knbn, ef, out.nb, out.counts, sync != 0, kernel_ms));
   if (via == HOST && nq == 0) return 0;
   if (rs.kind == Restriction::ROW_FILTERS && !rs.filters) return set_err("filters is NULL");
-  // with ranges, qset_off and qset may both be NULL: every row's set is then {LABEL_NONE}
-  const bool no_sets = rs.qrange && !rs.qset_off && !rs.qset;
-  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset_off && !no_sets) return set_err("qset_off is NULL");
-  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset && !no_sets) return set_err("qset is NULL");
+  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset_off) return set_err("qset_off is NULL");
+  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset) return set_err("qset is NULL");
   if (!queries || !out.ids || !out.dist || !out.counts || knbn == 0 || nq == 0) return set_err("bad argument");
   HB_PARTS_SHARED_IF(ix);
   HostBatch b{queries, nullptr, nq, (int)dim, knbn, ef, rs, out};
@@ -760,13 +758,15 @@ static int for_label_range(Index* ix, uint64_t first, uint64_t n,
   }
   return 0;
 }
-// set_labels / set_attributes: values[0, n) for the points [first, first + n), under the handle's lock and every
-// partition's, each taken exclusively; a partition's share is gathered from every P-th value
+// set_labels / set_attributes: column `col` of the points [first, first + n) set to value(0), ..., value(n - 1), under
+// the handle's lock and every partition's, each taken exclusively; a partition's share is every P-th value.
+// get_labels / get_attributes: out[i] = value(x, p) for the point p of Index x that is point first + i, under the
+// handle's lock and every partition's, each taken shared.
 extern "C++" {
 namespace {
-template <class T>
-int set_per_point(void* h, uint64_t first, uint64_t n, const T* values, const char* what, const char* null_msg,
-                  int (Index::*set)(size_t, size_t, const T*)) {
+template <class T, class F>
+int set_per_point(void* h, uint64_t first, uint64_t n, const void* values, const char* what, const char* null_msg,
+                  hb::PointColumn<T> Index::*col, F value) {
   HB_H(h);
   HB_NOT_VIEW(ix);
   if (label_range(ix, first, n, what)) return -1;
@@ -774,49 +774,41 @@ int set_per_point(void* h, uint64_t first, uint64_t n, const T* values, const ch
   if (!values) return set_err(null_msg);
   hb::DeviceRestore keep;
   const auto pl__ = ix->parts ? ix->parts->lock_exclusive() : std::vector<std::unique_lock<std::shared_mutex>>();
-  std::vector<T> mine;
   return for_label_range(ix, first, n, [&](Index* x, int part, uint64_t lo, uint64_t cnt, uint64_t stride, uint64_t at) {
-    const T* src = values + at;
-    if (stride != 1) {
-      mine.resize(cnt);
-      for (uint64_t i = 0; i < cnt; ++i) mine[i] = values[at + i * stride];
-      src = mine.data();
-    }
-    const int r = (x->*set)(lo, cnt, src);
+    const int r = x->set_points(x->*col, lo, cnt, [&](size_t i) { return value(at + i * stride); });
     return pass(ix, r && ix->parts ? ix->parts->fail(part, x->err()) : r);
+  });
+}
+template <class T, class F>
+int get_per_point(const void* h, uint64_t first, uint64_t n, T* out, const char* what, F value) {
+  HB_HS(h);
+  if (label_range(ix, first, n, what)) return -1;
+  if (n == 0) return 0;
+  if (!out) return set_err("out is NULL");
+  HB_PARTS_SHARED_IF(ix);
+  return for_label_range(ix, first, n, [&](Index* x, int, uint64_t lo, uint64_t cnt, uint64_t stride, uint64_t at) {
+    for (uint64_t i = 0; i < cnt; ++i) out[at + i * stride] = value(x, lo + i);
+    return 0;
   });
 }
 }  // namespace
 }  // extern "C++"
 int hnsw_b200_set_labels(void* h, uint64_t first, uint64_t n, const uint32_t* labels) {
-  return set_per_point(h, first, n, labels, "labels", "labels is NULL", &Index::set_labels);
+  return set_per_point(h, first, n, labels, "labels", "labels is NULL", &Index::labels,
+                       [&](size_t i) { return labels[i]; });
 }
 int hnsw_b200_get_labels(const void* h, uint64_t first, uint64_t n, uint32_t* out) {
-  HB_HS(h);
-  if (label_range(ix, first, n)) return -1;
-  if (n == 0) return 0;
-  if (!out) return set_err("out is NULL");
-  HB_PARTS_SHARED_IF(ix);
-  return for_label_range(ix, first, n, [&](Index* x, int, uint64_t lo, uint64_t cnt, uint64_t stride, uint64_t at) {
-    for (uint64_t i = 0; i < cnt; ++i) out[at + i * stride] = x->h_label[lo + i];
-    return 0;
-  });
+  return get_per_point(h, first, n, out, "labels", [](const Index* x, size_t p) { return x->labels.host[p]; });
 }
 
-// Point attributes: addressed as labels are
+// Point attributes: addressed as labels are, stored biased
 int hnsw_b200_set_attributes(void* h, uint64_t first, uint64_t n, const int64_t* values) {
-  return set_per_point(h, first, n, values, "attributes", "values is NULL", &Index::set_attributes);
+  return set_per_point(h, first, n, values, "attributes", "values is NULL", &Index::attrs,
+                       [&](size_t i) { return hb::attr_bias(values[i]); });
 }
 int hnsw_b200_get_attributes(const void* h, uint64_t first, uint64_t n, int64_t* out) {
-  HB_HS(h);
-  if (label_range(ix, first, n, "attributes")) return -1;
-  if (n == 0) return 0;
-  if (!out) return set_err("out is NULL");
-  HB_PARTS_SHARED_IF(ix);
-  return for_label_range(ix, first, n, [&](Index* x, int, uint64_t lo, uint64_t cnt, uint64_t stride, uint64_t at) {
-    for (uint64_t i = 0; i < cnt; ++i) out[at + i * stride] = hb::attr_unbias(x->h_attr[lo + i]);
-    return 0;
-  });
+  return get_per_point(h, first, n, out, "attributes",
+                       [](const Index* x, size_t p) { return hb::attr_unbias(x->attrs.host[p]); });
 }
 
 // A label per query: labels[i] is the label query i is restricted to, or LABEL_NONE for none; the graph search
@@ -858,12 +850,21 @@ int hnsw_b200_search_exact_label_sets(const void* h, const uint64_t* qset_off, c
 
 // Attribute ranges.  Query i is restricted to the points whose attribute is in [qrange[2i], qrange[2i + 1]]
 // ([INT64_MIN, INT64_MAX]: every point, also those without one) and whose label is one of qset[qset_off[i],
-// qset_off[i + 1]) ({LABEL_NONE}: any; qset_off and qset both NULL: {LABEL_NONE} for every query); the graph search
-// (ef_search) or the exact scan.
+// qset_off[i + 1]) ({LABEL_NONE}: any; qset_off and qset both NULL: {LABEL_NONE} for every query, passed as offsets 0,
+// 1, ..., nq over nq LABEL_NONE values); the graph search (ef_search) or the exact scan.
 static int ranged_call(const void* h, const char* name, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
                        bool exact, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef,
                        const AnswerArrays& out) {
   if (h && nq && !qrange) return set_err("qrange is NULL");  // search_call answers a NULL handle and nq == 0 first
+  std::vector<uint64_t> off;
+  std::vector<uint32_t> none;
+  if (!qset_off && !qset) {
+    off.resize(nq + 1);
+    std::iota(off.begin(), off.end(), (uint64_t)0);
+    none.assign(nq, hb::LABEL_NONE);
+    qset_off = off.data();
+    qset = none.data();
+  }
   return (int)search_call(h, HOST, name, row_label_sets(qset_off, qset, qrange), exact, queries, nq, dim, knbn, ef, out);
 }
 int hnsw_b200_search_flat_ranges(const void* h, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,

@@ -208,12 +208,9 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
     if (rs.kind == Restriction::ROW_LABEL_SETS) {
       u.set = sets->values.data() + sets->off[key];
       u.nset = (uint32_t)(sets->off[key + 1] - sets->off[key]);
-      u.ranged = !sets->range.empty() && sets->range[2 * key] != 0;
-      if (u.ranged) {
-        u.lo = sets->range[2 * key];
-        u.hi = sets->range[2 * key + 1];
-      }
-      r = !exact ? 0 : u.ranged ? l.rx->attr_range_scan(u.set, u.nset, u.lo, u.hi, slices) : l.rx->label_set_scan(u.set, u.nset, slices);
+      u.lo = sets->range[2 * key];
+      u.hi = sets->range[2 * key + 1];
+      r = exact ? l.rx->scan_slices(u.set, u.nset, u.lo, u.hi, slices) : 0;
     } else {
       ExactScan list;
       r = filters.use(key, l.part, P, l.rx, &u.bits, exact ? &list : nullptr);
@@ -241,7 +238,7 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
     // labels and attributes: the leg's own, or on a replica its copies of the handle's, made current first
     const Index* src = parts ? l->rx : this;
     if (rs.kind == Restriction::ROW_LABEL_SETS && pl.plain < l->count &&
-        (l->rx->labels_on_device(src, &pl.labels) || (rs.qrange && l->rx->attrs_on_device(src, &pl.attrs)))) {
+        (l->rx->on_device(&Index::labels, src, &pl.labels) || (rs.qrange && l->rx->on_device(&Index::attrs, src, &pl.attrs)))) {
       r = l->rc = -1;
       continue;
     }
@@ -260,10 +257,9 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
 
 // sort_rows for label sets, or the refusal of the first bad row: the rows copied into one array (a longer row sorted and
 // de-duplicated), their indices sorted once, and one walk over them that numbers the distinct (set, range) pairs into
-// `sets`.  Without qset_off and qset every row's set is {LABEL_NONE}.
+// `sets`.
 static std::string label_set_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm,
                                   std::vector<int64_t>& sorted, LabelSets& sets) {
-  static const uint32_t none = LABEL_NONE;
   std::vector<uint32_t> v;  // row i's set is v[at[i], at[i + 1])
   v.reserve(nq);
   std::vector<size_t> at(nq + 1);
@@ -272,16 +268,15 @@ static std::string label_set_rows(const Restriction& rs, size_t nq, std::vector<
   // then by their ranges
   std::vector<int64_t> key(nq);
   // row i's range, biased: (0, ~0) for none, which sorts first; else lo >= 1, and (1, 0) for every empty one
-  std::vector<uint64_t> rg(rs.qrange ? 2 * nq : 0);
+  std::vector<uint64_t> rg(2 * nq);
   bool longer = false;
   for (size_t i = 0; i < nq; ++i) {
-    const uint64_t lo = rs.qset_off ? rs.qset_off[i] : 0, hi = rs.qset_off ? rs.qset_off[i + 1] : 1;
+    const uint64_t lo = rs.qset_off[i], hi = rs.qset_off[i + 1];
     if (hi < lo)
       return "label set " + std::to_string(i) + ": qset_off[" + std::to_string(i + 1) + "] = " + std::to_string(hi) +
              " is below qset_off[" + std::to_string(i) + "] = " + std::to_string(lo);
     at[i] = v.size();
-    const uint32_t* src = rs.qset_off ? rs.qset : &none;
-    v.insert(v.end(), src + lo, src + hi);
+    v.insert(v.end(), rs.qset + lo, rs.qset + hi);
     if (hi - lo > 1) {
       std::sort(v.begin() + at[i], v.end());
       v.erase(std::unique(v.begin() + at[i], v.end()), v.end());
@@ -290,17 +285,15 @@ static std::string label_set_rows(const Restriction& rs, size_t nq, std::vector<
       longer |= v.size() - at[i] > 1;
     }
     key[i] = at[i] == v.size() ? 0 : v[at[i]] == LABEL_NONE ? -1 : 1 + (int64_t)v[at[i]];
-    if (rs.qrange) {
-      const int64_t a = rs.qrange[2 * i], b = rs.qrange[2 * i + 1];
-      uint64_t blo = 0, bhi = ~0ull;
-      if (a != INT64_MIN || b != INT64_MAX) {
-        blo = std::max<uint64_t>(attr_bias(a), 1);  // ATTR_NONE is no value: a range never admits a point without one
-        bhi = attr_bias(b);
-        if (blo > bhi) blo = 1, bhi = 0;
-      }
-      rg[2 * i] = blo;
-      rg[2 * i + 1] = bhi;
+    const int64_t* q = rs.qrange ? rs.qrange + 2 * i : nullptr;
+    uint64_t blo = 0, bhi = ~0ull;
+    if (q && (q[0] != INT64_MIN || q[1] != INT64_MAX)) {
+      blo = std::max<uint64_t>(attr_bias(q[0]), 1);  // ATTR_NONE is no value: a range never admits a point without one
+      bhi = attr_bias(q[1]);
+      if (blo > bhi) blo = 1, bhi = 0;
     }
+    rg[2 * i] = blo;
+    rg[2 * i + 1] = bhi;
   }
   at[nq] = v.size();
   auto less = [&](size_t a, size_t b) {
@@ -310,7 +303,7 @@ static std::string label_set_rows(const Restriction& rs, size_t nq, std::vector<
       if (std::lexicographical_compare(a0, a1, b0, b1)) return true;
       if (std::lexicographical_compare(b0, b1, a0, a1)) return false;
     }
-    return !rg.empty() && std::make_pair(rg[2 * a], rg[2 * a + 1]) < std::make_pair(rg[2 * b], rg[2 * b + 1]);
+    return std::make_pair(rg[2 * a], rg[2 * a + 1]) < std::make_pair(rg[2 * b], rg[2 * b + 1]);
   };
   perm.resize(nq);
   std::iota(perm.begin(), perm.end(), (size_t)0);
@@ -321,14 +314,14 @@ static std::string label_set_rows(const Restriction& rs, size_t nq, std::vector<
   sets.range.clear();
   for (size_t j = 0; j < nq; ++j) {
     const size_t i = perm[j];
-    if (key[i] == -1 && (rg.empty() || rg[2 * i] == 0)) {  // every point
+    if (key[i] == -1 && rg[2 * i] == 0) {  // every point
       sorted[j] = -1;
       continue;
     }
     if (j == 0 || less(perm[j - 1], i)) {  // a (set, range) the sorted rows have not had yet
       sets.values.insert(sets.values.end(), v.begin() + at[i], v.begin() + at[i + 1]);
       sets.off.push_back(sets.values.size());
-      if (!rg.empty()) sets.range.insert(sets.range.end(), {rg[2 * i], rg[2 * i + 1]});
+      sets.range.insert(sets.range.end(), {rg[2 * i], rg[2 * i + 1]});
     }
     sorted[j] = (int64_t)sets.off.size() - 2;
   }

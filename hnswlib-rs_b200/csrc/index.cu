@@ -96,7 +96,7 @@ Index::~Index() {
   if (stream_) cudaStreamSynchronize(stream_);
   for (void* a : graph_.p) cudaFree(a);
   cudaFree(vis_.tab); cudaFree(vis_.epoch); cudaFree(d_counter_); cudaFree(d_status_); cudaFree(d_stats_); cudaFree(d_mask_);
-  cudaFree(label_csr_.d_ids);
+  cudaFree(by_label_.d_ids);
   cudaFree(by_value_.d_ids);
   cudaFree(by_label_value_.d_ids);
   if (h_pin_) cudaFreeHost(h_pin_);
@@ -356,8 +356,8 @@ void Index::resize_points(size_t count) {
   h_plevel.resize(count);
   h_rank.resize(count);
   h_origin.resize(count);
-  h_label.resize(count, LABEL_NONE);
-  h_attr.resize(count, attr_bias(ATTR_NONE));
+  labels.host.resize(count, labels.none);
+  attrs.host.resize(count, attrs.none);
   h_upoff.resize(count);
 }
 
@@ -372,8 +372,8 @@ int Index::upload_points(size_t first, size_t count) {
   HB_CUDA(cudaMemcpyAsync(graph_.at<uint8_t>(GS::PLEVEL) + first, h_plevel.data() + first, count, cudaMemcpyHostToDevice, stream_));
   HB_CUDA(cudaMemcpyAsync(graph_.at<uint64_t>(GS::ORIGIN) + first, h_origin.data() + first, count * 8, cudaMemcpyHostToDevice, stream_));
   HB_CUDA(cudaMemcpyAsync(graph_.at<uint32_t>(GS::UP_OFF) + first, h_upoff.data() + first, count * 4, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(graph_.at<uint32_t>(GS::LABEL) + first, h_label.data() + first, count * 4, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(graph_.at<uint64_t>(GS::ATTR) + first, h_attr.data() + first, count * 8, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.at<uint32_t>(GS::LABEL) + first, labels.host.data() + first, count * 4, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.at<uint64_t>(GS::ATTR) + first, attrs.host.data() + first, count * 8, cudaMemcpyHostToDevice, stream_));
   return 0;
 }
 
@@ -973,7 +973,7 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
       f = RowFilter{plan.labels, at + vals.size(), 0, u.nset, nullptr, 0, 0};
       vals.insert(vals.end(), u.set, u.set + u.nset);
     }
-    if (u.ranged) {
+    if (u.lo) {
       f.attr = plan.attrs;
       f.lo = u.lo;
       f.hi = u.hi;

@@ -92,6 +92,16 @@ struct GraphStore {
   T* at(Array a) const { return static_cast<T*>(p[a]); }
 };
 
+// A value per point kept next to the graph (labels.cu): graph store array `array` and its host mirror, `none` for every
+// point until it is set; `version` counts the calls that changed it (a replica: the handle's version it copied).
+template <class T>
+struct PointColumn {
+  GraphStore::Array array;
+  T none;
+  std::vector<T> host{};
+  uint64_t version = 0;
+};
+
 struct DumpDescription {  // Description, /root/reference/src/hnswio.rs:846-870
   int format_version = 0;
   uint8_t dumpmode = 0, max_nb_connection = 0, nb_layer = 0;
@@ -210,7 +220,6 @@ struct AnswerArrays {
 // filter per row, -1 = none (ROW_FILTERS); or a set of labels per row (a label per row: sets of one), row i's the values
 // qset[qset_off[i], qset_off[i + 1]) in any order and with repeats, {LABEL_NONE} = none (ROW_LABEL_SETS), each within an
 // attribute range when qrange is set: row i's [qrange[2i], qrange[2i + 1]], inclusive, [INT64_MIN, INT64_MAX] = none.
-// qset_off and qset both null with qrange: every row's set is {LABEL_NONE}.
 struct Restriction {
   enum Kind { NONE, FILTER_T, RESIDENT, ROW_FILTERS, ROW_LABEL_SETS } kind = NONE;
   int mode = 0;
@@ -227,8 +236,8 @@ struct Restriction {
 };
 
 // The distinct (label set, range) pairs of a ROW_LABEL_SETS batch (Index::sort_rows): set j is values[off[j], off[j + 1]),
-// ascending and without repeats, within the biased attribute range [range[2j], range[2j + 1]] (attr_bias; lo >= 1); with
-// no range when range is empty (a batch without ranges) or range[2j] is 0
+// ascending and without repeats, within the biased attribute range [range[2j], range[2j + 1]] (attr_bias; lo >= 1), or
+// with no range when that is (0, ~0)
 struct LabelSets {
   std::vector<uint32_t> values;
   std::vector<size_t> off;
@@ -251,9 +260,9 @@ struct HostBatch {
 // A leg's restriction (Index::resolve): its rows [0, plain) are unrestricted, and `runs` cover the rest, each a range of
 // consecutive rows under one restriction: a bitmap (a resident filter's on the leg's device, or a FilterT's host bits,
 // uploaded into the context when the leg begins) or a label set on `labels` (the label array on the leg's device), the
-// latter within an attribute range on `attrs` when it is `ranged`.  In an exact batch its points are slices [slice,
-// slice + nslices): a filter's id list, a label set's CSR slices, or a ranged run's slices of the attribute orders.  A
-// batch-wide filter is a plan with no prefix and one run over every row.
+// latter within an attribute range on `attrs` unless its lo is 0.  In an exact batch its points are slices [slice,
+// slice + nslices): a filter's id list, or a label set's and range's slices of an exact-scan order.  A batch-wide filter
+// is a plan with no prefix and one run over every row.
 struct LegPlan {
   struct Run {
     size_t first, count;
@@ -261,8 +270,7 @@ struct LegPlan {
     const uint32_t* host_bits = nullptr;
     const uint32_t* set = nullptr;  // the run's label set, nset values of a LabelSets
     uint32_t nset = 0;
-    bool ranged = false;  // the run's attribute range, biased bounds of a LabelSets
-    uint64_t lo = 0, hi = 0;
+    uint64_t lo = 0, hi = 0;  // the run's attribute range, biased bounds of a LabelSets (lo == 0: none)
     size_t slice = 0, nslices = 0;
   };
   bool exact = false;
@@ -312,8 +320,6 @@ class Index {
   std::vector<uint8_t> h_level, h_plevel;
   std::vector<int32_t> h_rank;
   std::vector<uint64_t> h_origin;
-  std::vector<uint32_t> h_label;  // LABEL_NONE = none (labels.cu)
-  std::vector<uint64_t> h_attr;   // attr_bias(value), 0 = none (labels.cu)
   std::vector<uint32_t> h_upoff;
 
   // ---- operations (return 0 or a negative status; message in err())
@@ -353,7 +359,7 @@ class Index {
   // `sets`, -1: none) in the order the legs run the rows (sort_rows).  A FilterT's host bits are made on the calling
   // thread once per partition (a replica shares the handle's internal ids, and so its bits) into `bits`; a resident
   // filter is its copy on each leg's device; a label set needs the label array on the leg's device.  `exact`: each
-  // run's slices (a filter's id list on the leg's device; a label set's CSR slices).  Nonzero when a leg could not have
+  // run's slices (a filter's id list on the leg's device; a label set's scan_slices).  Nonzero when a leg could not have
   // its plan; that leg's rc is set (legs_fail reports it).
   int resolve(const Restriction& rs, bool exact, const std::vector<int64_t>& sorted, Leg* legs, size_t n,
               std::vector<std::vector<uint32_t>>& bits, const LabelSets* sets = nullptr);
@@ -365,29 +371,33 @@ class Index {
   int sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm, std::vector<int64_t>& sorted,
                 LabelSets& sets);
 
-  // ---- point labels (labels.cu).  One u32 per point (GraphStore LABEL and its host mirror h_label), LABEL_NONE until
-  // set_labels names one; label_version counts the calls that changed them (a replica: the handle's version it copied).
-  uint64_t label_version = 0;
-  // labels[0, count) for the points [first, first + count) of this Index (the caller checked the range)
-  int set_labels(size_t first, size_t count, const uint32_t* labels);
-  // the label array on this Index's device, as current as `src`'s (a replica's copy of the handle's labels, refreshed
-  // when src's changed; src == this: its own)
-  int labels_on_device(const Index* src, const uint32_t** d_labels);
-  // the points whose label is one of set[0, nset) (ascending), appended to `slices`: one slice of the label CSR (rebuilt
-  // when the labels changed) per label that some point carries, slices that follow each other in the CSR joined
-  int label_set_scan(const uint32_t* set, size_t nset, std::vector<ExactScan>& slices);
-  // ---- point attributes (labels.cu).  One int64 per point (GraphStore ATTR and its host mirror h_attr, both biased by
-  // attr_bias), ATTR_NONE until set_attributes names one; attr_version counts the calls that changed them (a replica: the
-  // handle's version it copied).
-  uint64_t attr_version = 0;
-  // values[0, count) for the points [first, first + count) of this Index (the caller checked the range)
-  int set_attributes(size_t first, size_t count, const int64_t* values);
-  // the attribute array on this Index's device, as current as `src`'s (labels_on_device's twin)
-  int attrs_on_device(const Index* src, const uint64_t** d_attrs);
-  // the points whose attribute is in [lo, hi] (biased, lo >= 1) and, unless set is {LABEL_NONE}, whose label is one of
-  // set[0, nset) (ascending), appended to `slices`: one slice of the value order, or one of the label-value order per
-  // label of the set (each order rebuilt when what it sorts by changed), slices that follow each other joined
-  int attr_range_scan(const uint32_t* set, size_t nset, uint64_t lo, uint64_t hi, std::vector<ExactScan>& slices);
+  // ---- point labels and attributes (labels.cu): a u32 label per point, LABEL_NONE = none, and an int64 attribute per
+  // point, stored as attr_bias(value), 0 = none (ATTR_NONE)
+  PointColumn<uint32_t> labels{GraphStore::LABEL, LABEL_NONE};
+  PointColumn<uint64_t> attrs{GraphStore::ATTR, attr_bias(ATTR_NONE)};
+  // c's values of the points [first, first + count) of this Index (the caller checked the range): value(i) for point
+  // first + i.  Copied on the handle's stream and waited for, so that no search launched after this returns reads the old
+  // values.
+  template <class T, class F>
+  int set_points(PointColumn<T>& c, size_t first, size_t count, F value) {
+    if (count == 0) return 0;
+    HB_CUDA(cudaSetDevice(device));
+    for (size_t i = 0; i < count; ++i) c.host[first + i] = value(i);
+    HB_CUDA(cudaMemcpyAsync(graph_.at<T>(c.array) + first, c.host.data() + first, count * sizeof(T), cudaMemcpyHostToDevice,
+                            stream_));
+    HB_CUDA(cudaStreamSynchronize(stream_));
+    ++c.version;
+    return 0;
+  }
+  // column `col`'s array on this Index's device, as current as src's (src == this: its own; a replica: its copy of the
+  // handle's, refreshed when the handle's changed)
+  template <class T>
+  int on_device(PointColumn<T> Index::*col, const Index* src, const T** d);
+  // the points of one run, appended to `slices`: those whose label is one of set[0, nset) (ascending; {LABEL_NONE}: any
+  // label) and, unless lo is 0, whose attribute is in the biased range [lo, hi] (lo >= 1).  They are slices of one
+  // exact-scan order (rebuilt when a column it is keyed on changed): per label of the set, its group, narrowed to the
+  // range by binary search in a value-keyed order; slices that follow each other in the order are joined.
+  int scan_slices(const uint32_t* set, size_t nset, uint64_t lo, uint64_t hi, std::vector<ExactScan>& slices);
   // device queries in, device answers out; the restriction is none or a resident filter.  `exact`: the exact scan (ef
   // unused).
   int search_device(const Restriction& rs, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef,
@@ -563,29 +573,23 @@ class Index {
   int end_leg(Leg& l, size_t k, const AnswerArrays& out);
   int legs_fail(const Leg* legs, size_t n, bool replicas_first);
 
-  // ---- point labels (labels.cu).  The CSR of the exact path: the internal ids of every labelled point on this device,
-  // grouped by label in ascending label order and ascending within a group; groups[label] = (offset, count).  Made from h_label at label version
-  // `version` (~0: never), at the first exact labelled search after the labels changed.  A point added since has no
-  // label, so inserts leave it current.  label_mu_ guards it and a replica's copy of the labels.
-  struct LabelCsr {
+  // ---- exact-scan orders (labels.cu): the internal ids of this Index's points that have what the order is keyed on (a
+  // label, an attribute, or both), in groups per label (groups[label] = (offset, count)) laid out in ascending label
+  // order; a value-only order is one group, LABEL_NONE's.  Within a group the ids ascend, or in a value-keyed order go
+  // by (value, id), whose biased values stay on the host for the binary searches.  The ids go to the device.  Made from
+  // the columns at the first exact search that needs the order after a column it is keyed on changed (the versions it
+  // was made at, ~0: never).  A point added since has neither a label nor an attribute, so inserts leave it current.
+  struct ScanOrder {
+    bool by_label, by_value;
     void* d_ids = nullptr;
     size_t bytes = 0;
-    uint64_t version = ~0ull;
-    std::unordered_map<uint32_t, std::pair<uint32_t, uint32_t>> groups;
-  } label_csr_;
-  // The orders of the exact ranged path, made from h_attr (and h_label) at the first exact ranged search after what they
-  // sort by changed: the internal ids of every point with an attribute by (value, id), and of every point with a label
-  // and an attribute by (label, value, id) with each label's (offset, count).  The sorted values stay on the host for the
-  // binary searches, the ids go to the device.  A point added since has neither, so inserts leave them current.
-  struct AttrOrder {
-    void* d_ids = nullptr;
-    size_t bytes = 0;
-    uint64_t version = ~0ull, lversion = ~0ull;  // attr_version (and label_version) it was made at
-    std::vector<uint64_t> values;                // biased, in the order of the ids
-    std::unordered_map<uint32_t, std::pair<uint32_t, uint32_t>> groups;
-  } by_value_, by_label_value_;
-  int make_attr_order(AttrOrder& o, bool by_label);
-  // label_mu_ guards the label CSR, both attribute orders and a replica's copy of the labels and attributes
+    uint64_t label_version = ~0ull, attr_version = ~0ull;
+    std::unordered_map<uint32_t, std::pair<uint32_t, uint32_t>> groups{};
+    std::vector<uint64_t> values{};
+  };
+  ScanOrder by_label_{true, false}, by_value_{false, true}, by_label_value_{true, true};
+  int make_order(ScanOrder& o);
+  // label_mu_ guards the orders and a replica's copy of the labels and attributes
   std::mutex label_mu_;
 
   int broadcast_to_replicas();

@@ -302,17 +302,23 @@ def attr_of_float(x):
     return int(out) if out.ndim == 0 else out
 
 
+def _int64s(a, what):
+    """the integer array a as a contiguous int64 array; floats and unsigned values above INT64_MAX are refused ("<what>
+    64-bit integers")"""
+    if a.size and a.dtype.kind not in "iu":
+        raise ValueError(f"{what} 64-bit integers (attr_of_float maps floats)")
+    if a.size and a.dtype.kind == "u" and a.max() > np.iinfo(np.int64).max:
+        raise ValueError(f"{what} signed 64-bit integers")
+    return np.ascontiguousarray(a, np.int64)
+
+
 def _ranges(ranges, nq):
     """the ranges argument of the ranged searches: an (nq, 2) int64 array or a sequence of nq (lo, hi) pairs, as a
     contiguous int64 array of 2 nq bounds"""
     a = np.asarray(ranges)
     if a.shape != (nq, 2) and not (nq == 0 and a.size == 0):
         raise ValueError(f"ranges has shape {a.shape}, expected ({nq}, 2)")
-    if a.size and a.dtype.kind not in "iu":
-        raise ValueError("ranges: bounds are 64-bit integers (attr_of_float maps floats)")
-    if a.size and a.dtype.kind == "u" and a.max() > np.iinfo(np.int64).max:
-        raise ValueError("ranges: bounds are signed 64-bit integers")
-    a = np.ascontiguousarray(a, np.int64).reshape(-1)
+    a = _int64s(a, "ranges: bounds are").reshape(-1)
     return a if a.size else np.zeros(2, np.int64)   # never a NULL pointer
 
 
@@ -581,12 +587,7 @@ class Hnsw:
     def set_attributes(self, first, values):
         """hnsw_b200_set_attributes: the int64 attributes of the points with insertion ranks first .. first +
         len(values) - 1 (ATTR_NONE clears one).  Every point starts without an attribute."""
-        v = np.asarray(values).reshape(-1)
-        if v.size and v.dtype.kind not in "iu":
-            raise ValueError("attributes are 64-bit integers (attr_of_float maps floats)")
-        if v.size and v.dtype.kind == "u" and v.max() > np.iinfo(np.int64).max:
-            raise ValueError("attributes are signed 64-bit integers")
-        v = np.ascontiguousarray(v, np.int64)
+        v = _int64s(np.asarray(values).reshape(-1), "attributes are")
         self._chk(self._L.hnsw_b200_set_attributes(self._h, int(first), v.size, _p(v)))
 
     def get_attributes(self, first, n):

@@ -251,6 +251,11 @@ def test_attributes_follow_inserts_and_changes(pkg, po):
     check(lab, attr, "new values and cleared ones")
     assert np.array_equal(h.get_attributes(0, n), attr)
     assert np.array_equal(h.get_labels(0, n), lab)   # attributes leave labels alone
+    relabelled = rng.choice(n, 500, replace=False)   # points that have a label get another one: only the label-keyed
+    lab[relabelled] = (lab[relabelled] + rng.integers(1, 4, 500)) % 4   # exact orders go stale
+    h.set_labels(0, lab)
+    check(lab, attr, "relabelled, attributes unchanged")
+    assert np.array_equal(h.get_attributes(0, n), attr)   # labels leave attributes alone
 
 
 @pytest.mark.parametrize("P", [2, 3])
