@@ -6,6 +6,7 @@
 //                       truth), and the exact search over a resident filter (hnsw_b200_search_exact).
 #include "index.h"
 #include "kernels.h"
+#include "search_core.cuh"
 
 namespace hb {
 
@@ -77,6 +78,8 @@ struct ExactParams {
   NeighbourOut* out;     // [nq][k]
   int32_t* counts;       // [nq]
   const ExactTile* tiles;  // nullptr: tile t is queries [t * tq, t * tq + tq) over (list, npts); else tile t is tiles[t]
+  const uint64_t* q_ids;     // as SearchParams' (a search by stored point)
+  const uint64_t* skip_ids;  // as SearchParams': k is knbn + 1 and each row of `out` knbn wide
 };
 
 // keys[0, c) (~0 = none) into the warp's sorted queue Q, 32 at a time: those Q accepts, inserted in lane order.  The keys
@@ -132,7 +135,7 @@ __global__ void __launch_bounds__(256, 2) exact_knn_kernel(ExactParams p) {
   if (threadIdx.x == 0)
     for (int s = 0; s < NS; ++s) mbar_init(bar + s, 1);
   for (int q = warp; q < tq; q += 8)
-    stage_row_bytes(qs + (size_t)q * d4, reinterpret_cast<const char*>(p.queries) + (size_t)(q < nqt ? q0 + q : 0) * p.q_bytes,
+    stage_row_bytes(qs + (size_t)q * d4, query_row(p.g, p.q_ids, p.queries, p.q_bytes, q < nqt ? q0 + q : 0),
                     q < nqt ? p.q_bytes : 0, (int)row_bytes);
   for (int q = threadIdx.x; q < tq; q += blockDim.x) {
     thr[q] = ~0ull;
@@ -210,18 +213,9 @@ __global__ void __launch_bounds__(256, 2) exact_knn_kernel(ExactParams p) {
     __syncthreads();
   }
 
-  // answers: (origin, distance, internal id) for the first n keys, then (~0, +inf, INVALID_ID)
+  // answers: the first n keys (write_row)
   auto write = [&](int q, const uint64_t* w, int n) {
-    NeighbourOut* o = p.out + (size_t)(q0 + q) * k;
-    for (int j = lane; j < k; j += 32) {
-      if (j < n) {
-        const uint32_t it = key_id(w[j]);
-        o[j] = NeighbourOut{p.g.origin[it], key_dist(w[j]), it};
-      } else {
-        o[j] = NeighbourOut{~0ull, __int_as_float(0x7f800000), INVALID_ID};
-      }
-    }
-    if (lane == 0) p.counts[q0 + q] = n;
+    write_row(p.out, p.counts, p.g.origin, k, p.skip_ids, q0 + q, lane, n, [&](int j) { return w[j]; }, KeepAll());
   };
   if (p.slices == 1) {
     for (int q = warp; q < nqt; q += 8) write(q, queue + (size_t)q * k, qn[q]);
@@ -279,7 +273,8 @@ static bool exact_shape(int d4, size_t k, size_t nq, ExactParams& p, size_t& sme
 }
 
 int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const std::vector<ExactGroup>& groups,
-                        NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms) {
+                        NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* q_ids,
+                        const uint64_t* skip) {
   if (k == 0) return fail("knbn must be positive");
   if (poisoned_) return fail(poison_msg_);
   cudaStream_t st = c.stream;
@@ -298,11 +293,16 @@ int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k
   p.nq = (uint32_t)nq;
   p.list = scan.ids;
   p.npts = (uint32_t)(scan.ids ? scan.n : n);
+  p.q_ids = q_ids;
+  p.skip_ids = skip;
+  k += skip ? 1 : 0;  // the scan keeps k + 1 keys, each row is k wide (write_row)
   p.k = (int)k;
   size_t widest_group = 0;
   for (const ExactGroup& gr : groups) widest_group = std::max(widest_group, gr.count);
   size_t smem = 0;
-  if (!exact_shape(p.g.d4, k, widest_group, p, smem)) return fail("k / dimension too large for the exact search kernel");
+  if (!exact_shape(p.g.d4, k, widest_group, p, smem))
+    return fail(skip ? "k + 1 / dimension too large for the exact search kernel (exclude_self searches k + 1)"
+                     : "k / dimension too large for the exact search kernel");
   auto launch = [&](int grid, int* blocks_per_sm) {
     return dispatch_op(metric, dtype, [&](auto tag) -> cudaError_t {
       return launch_exact_for_op<typename decltype(tag)::type>(p, grid, smem, st, blocks_per_sm);

@@ -625,21 +625,34 @@ int hnsw_b200_insert_flat(void* h, const void* vecs, uint64_t n, uint64_t dim, c
 // `name` is the entry point a refusal on a partitioned handle names.  `rs` is what each query may return, `exact` the
 // exact scan of those points instead of the graph search (ef unused).
 enum Via { HOST, SUBMIT, DEVICE };
+// By stored point (qids, checked by the caller to be non-NULL): the queries are the stored vectors of qids[0, nq), each
+// below the handle's nb_point, and `dim` is the handle's; exclude_self: each row leaves its own point out.
 static int64_t search_call(const void* h, Via via, const char* name, const Restriction& rs, bool exact, const void* queries,
                            uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef, const AnswerArrays& out, int sync = 1,
-                           float* kernel_ms = nullptr) {
+                           float* kernel_ms = nullptr, const uint64_t* qids = nullptr, bool exclude_self = false) {
   HB_HS(h);
   if (via != HOST) HB_NOT_PARTITIONED(ix, name);
   if (via == DEVICE)
-    return pass(ix, ix->search_device(rs, exact, queries, nq, knbn, ef, out.nb, out.counts, sync != 0, kernel_ms));
+    return pass(ix, ix->search_device(rs, exact, queries, nq, knbn, ef, out.nb, out.counts, sync != 0, kernel_ms, qids,
+                                      exclude_self));
   if (via == HOST && nq == 0) return 0;
+  HB_PARTS_SHARED_IF(ix);
+  if (qids) {
+    const uint64_t have = nb_point(ix);
+    for (uint64_t i = 0; i < nq; ++i)
+      if (qids[i] >= have)
+        return set_err(std::string(name) + ": qids[" + std::to_string(i) + "] = " + std::to_string(qids[i]) +
+                       " is not below nb_point = " + std::to_string(have));
+    dim = (uint64_t)ix->dim;
+  }
   if (rs.kind == Restriction::ROW_FILTERS && !rs.filters) return set_err("filters is NULL");
   if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset_off) return set_err("qset_off is NULL");
   if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset) return set_err("qset is NULL");
-  if (!queries || !out.ids || !out.dist || !out.counts || knbn == 0 || nq == 0) return set_err("bad argument");
-  HB_PARTS_SHARED_IF(ix);
+  if (!(queries || qids) || !out.ids || !out.dist || !out.counts || knbn == 0 || nq == 0) return set_err("bad argument");
   HostBatch b{queries, nullptr, nq, (int)dim, knbn, ef, rs, out};
   b.exact = exact;
+  b.qids = qids;
+  b.exclude_self = exclude_self;
   if (via == HOST) return pass(ix, ix->search_batch(b));
   const int64_t t = ix->submit_batch(b);
   if (t < 0) g_err = ix->err();
@@ -885,6 +898,66 @@ int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_q
                                   void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
   return (int)search_call(h, DEVICE, "search_exact_device", resident_or_all(filter), true, d_queries, nq, 0, knbn, 0,
                           on_device(d_out, d_counts), sync, kernel_ms);
+}
+
+// Search by stored point: the restriction of a by-id call (-1 and no sets or ranges: none), refused when a resident
+// filter comes with sets or ranges; a range without sets is a range within {LABEL_NONE} per query, as ranged_call reads
+// it, and sets without ranges are the label-sets call's
+static int by_id_call(const void* h, Via via, const char* name, bool exact, const uint64_t* qids, uint64_t nq, uint64_t knbn,
+                      uint64_t ef, int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                      const uint32_t* qset, const AnswerArrays& out, int sync = 1, float* kernel_ms = nullptr) {
+  if (!h) return set_err("NULL handle");
+  if (nq == 0) return 0;
+  if (!qids) return set_err(std::string(name) + ": qids is NULL");
+  const bool rows = qrange || qset_off || qset;
+  if (filter != -1 && rows)
+    return set_err(std::string(name) + ": a resident filter cannot be combined with label sets or ranges");
+  std::vector<uint64_t> off;
+  std::vector<uint32_t> none;
+  if (qrange && !qset_off && !qset) {
+    off.resize(nq + 1);
+    std::iota(off.begin(), off.end(), (uint64_t)0);
+    none.assign(nq, hb::LABEL_NONE);
+    qset_off = off.data();
+    qset = none.data();
+  }
+  const Restriction rs = rows ? row_label_sets(qset_off, qset, qrange) : resident_or_all(filter);
+  return (int)search_call(h, via, name, rs, exact, nullptr, nq, 0, knbn, ef, out, sync, kernel_ms, qids, exclude_self != 0);
+}
+int hnsw_b200_search_flat_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, uint64_t ef_search,
+                                int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                                const uint32_t* qset, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                                int32_t* out_pid, int32_t* out_counts) {
+  return by_id_call(h, HOST, "search_flat_by_id", false, qids, nq, knbn, ef_search, exclude_self, filter, qrange, qset_off,
+                    qset, columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+}
+int hnsw_b200_search_exact_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, int exclude_self,
+                                 int64_t filter, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                                 uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
+                                 int32_t* out_counts) {
+  return by_id_call(h, HOST, "search_exact_by_id", true, qids, nq, knbn, 0, exclude_self, filter, qrange, qset_off, qset,
+                    columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+}
+int hnsw_b200_search_device_by_id(const void* h, int exact, int64_t filter, const uint64_t* d_qids, uint64_t nq,
+                                  uint64_t knbn, uint64_t ef_search, int exclude_self, void* d_out, int32_t* d_counts,
+                                  int sync, float* kernel_ms) {
+  return by_id_call(h, DEVICE, "search_device_by_id", exact != 0, d_qids, nq, knbn, exact ? 0 : ef_search, exclude_self,
+                    filter, nullptr, nullptr, nullptr, on_device(d_out, d_counts), sync, kernel_ms);
+}
+
+int hnsw_b200_get_vectors(const void* h, const uint64_t* ranks, uint64_t n, void* out) {
+  HB_HS(h);
+  if (n == 0) return 0;
+  if (!ranks) return set_err("get_vectors: ranks is NULL");
+  if (!out) return set_err("get_vectors: out is NULL");
+  HB_PARTS_SHARED_IF(ix);
+  const uint64_t have = nb_point(ix);
+  for (uint64_t i = 0; i < n; ++i)
+    if (ranks[i] >= have)
+      return set_err("get_vectors: ranks[" + std::to_string(i) + "] = " + std::to_string(ranks[i]) +
+                     " is not below nb_point = " + std::to_string(have));
+  hb::DeviceRestore keep;
+  return pass(ix, ix->get_vectors(ranks, n, out));
 }
 
 int64_t hnsw_b200_filter_new(const void* h, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,

@@ -220,7 +220,7 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
   for (;;) {
     const uint32_t qi = next_item(p.work_counter, lane);
     if (qi >= p.nq) break;
-    stage_row_bytes(s.q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes, p.q_bytes, g.d4 * 16);
+    stage_row_bytes(s.q4, query_row(g, p.q_ids, p.queries, p.q_stride_bytes, qi), p.q_bytes, g.d4 * 16);
     if (lane == 0) *fslot = p.filter_sel ? p.filter_table[p.filter_sel[qi]] : p.filter;
     __syncwarp();
     int count = 0;
@@ -238,26 +238,8 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
       count = 0;
     }
     // post-filter AFTER truncation (hnsw.rs:1549-1563): only the entry point can fail here
-    const size_t ob = (size_t)qi * p.k;
-    int outn = 0;
-    for (int b = 0; b < count; b += 32) {
-      const int j = b + lane;
-      uint64_t key = 0;
-      bool keep = false;
-      if (j < count) {
-        key = W.w[j];
-        keep = filter_pass<Op>(fslot, key_id(key));
-      }
-      const unsigned m = __ballot_sync(FULL, keep);
-      if (keep) {
-        const uint32_t id = key_id(key);
-        p.out_nb[ob + outn + __popc(m & ((1u << lane) - 1u))] = NeighbourOut{g.origin[id], key_dist(key), id};
-      }
-      outn += __popc(m);
-    }
-    for (int j = outn + lane; j < p.k; j += 32) p.out_nb[ob + j] = NeighbourOut{~0ull, __int_as_float(0x7f800000), INVALID_ID};
-    if (lane == 0) p.out_count[qi] = outn;
-    __syncwarp();
+    write_row(p.out_nb, p.out_count, g.origin, p.k, p.skip_ids, qi, lane, count, [&](int j) { return W.w[j]; },
+              [&](uint32_t id) { return filter_pass<Op>(fslot, id); });
   }
   vis.save(p.vis, slot, lane);
   flush_stats(p.stats, st, lane);

@@ -372,8 +372,20 @@ int Index::legs_fail(const Leg* legs, size_t n, bool replicas_first) {
 
 void Index::begin_leg(const HostBatch& b, Leg& l) {
   if (l.ctx < 0) l.ctx = l.rx->acquire_ctx();
-  const void* q = b.rows ? nullptr : (const char*)b.queries + l.first * (size_t)b.d * es;
-  l.rc = l.rx->search_host_begin(l.ctx, q, b.rows ? b.rows + l.first : nullptr, l.count, b.d, b.k, b.ef, l.plan);
+  const uint64_t* ids = b.qids ? b.qids + l.first : nullptr;
+  const uint64_t* skip = b.exclude_self ? ids : nullptr;
+  std::vector<uint64_t> local;
+  if (parts && ids) {  // the rows were gathered into b.queries; a row leaves out its point on the partition that holds it
+    const uint64_t P = (uint64_t)parts->count();
+    if (skip) {
+      local.resize(l.count);
+      for (size_t i = 0; i < l.count; ++i) local[i] = ids[i] % P == (uint64_t)l.part ? ids[i] / P : ~0ull;
+      skip = local.data();
+    }
+    ids = nullptr;
+  }
+  const void* q = b.rows || ids ? nullptr : (const char*)b.queries + l.first * (size_t)b.d * es;
+  l.rc = l.rx->search_host_begin(l.ctx, q, b.rows ? b.rows + l.first : nullptr, ids, skip, l.count, b.d, b.k, b.ef, l.plan);
   l.begun = l.rc == 0;
 }
 
@@ -401,19 +413,33 @@ int Index::end_leg(Leg& l, size_t k, const AnswerArrays& out) {
 
 // ------------------------------------------------------------------------------------------------ batches
 // The batch `call` planned into t's legs, each with its plan; `b` is the batch as the legs run it.  A per-row restriction:
-// the batch is planned over the rows sorted by filter or label set, gathered through row pointers, and each answer goes back
-// to its caller's row.  A leg that could not have its plan is reported in leg order, or the replicas' first.
+// the batch is planned over the rows sorted by filter or label set, gathered through row pointers (by stored point: its
+// ids permuted), and each answer goes back to its caller's row.  A batch by stored point on a partitioned handle has its
+// rows gathered from their partitions first, since no device reads another partition's store, and is then searched as
+// host queries.  A leg that could not have its plan is reported in leg order, or the replicas' first.
 int Index::prepare_batch(const HostBatch& call, HostBatch& b, Ticket& t, bool replicas_first) {
   if (parts && dim != 0 && call.d != dim) return fail("query length differs from the index dimension");
   int r;
   b = call;
+  if (parts && call.qids) {
+    t.gathered.resize(call.nq * (size_t)dim * es);
+    if ((r = get_vectors(call.qids, call.nq, t.gathered.data()))) return r;
+    b.queries = t.gathered.data();
+  }
   std::vector<int64_t> sorted;
   if (call.restriction.per_row()) {
     if ((r = sort_rows(call.restriction, call.nq, t.perm, sorted, t.sets))) return r;
-    t.rows.resize(call.nq);
-    for (size_t j = 0; j < call.nq; ++j)
-      t.rows[j] = call.rows ? call.rows[t.perm[j]] : (const char*)call.queries + t.perm[j] * (size_t)call.d * es;
-    b.rows = t.rows.data();
+    if (call.qids) {
+      t.qids.resize(call.nq);
+      for (size_t j = 0; j < call.nq; ++j) t.qids[j] = call.qids[t.perm[j]];
+      b.qids = t.qids.data();
+    }
+    if (!call.qids || parts) {
+      t.rows.resize(call.nq);
+      for (size_t j = 0; j < call.nq; ++j)
+        t.rows[j] = b.rows ? b.rows[t.perm[j]] : (const char*)b.queries + t.perm[j] * (size_t)b.d * es;
+      b.rows = t.rows.data();
+    }
     b.out.perm = t.perm.data();
   }
   t.k = b.k;

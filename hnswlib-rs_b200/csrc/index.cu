@@ -1,6 +1,7 @@
 // Host-side index: HBM allocation, insert-batch scheduling, query launches, import/export.
 // See index.h for what it replaces in the reference.
 #include "index.h"
+#include "partition.h"
 
 #include <algorithm>
 #include <cmath>
@@ -652,15 +653,27 @@ void Index::release_ctx(int c) {
 // check_status, set_stream, any synchronous call's own synchronisation) makes it do so; stream_wait_last() makes any
 // stream wait for the most recent launch alone.  The same for the exact scan (`exact`).
 int Index::search_device(const Restriction& rs, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef_arg,
-                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms) {
+                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* d_qids,
+                         bool exclude_self) {
   Leg leg{this, 0, 0, nq};
   std::vector<std::vector<uint32_t>> bits;
   int r;
   if (resolve(rs, exact, {}, &leg, 1, bits)) return legs_fail(&leg, 1, false);
   if (nq == 0) return 0;
   HB_CUDA(cudaSetDevice(device));
+  if (d_qids) {
+    // the ids are checked before anything runs: read back once the work already on the handle's stream (which may
+    // write them) is done
+    std::vector<uint64_t> ids(nq);
+    HB_CUDA(cudaMemcpyAsync(ids.data(), d_qids, nq * sizeof(uint64_t), cudaMemcpyDeviceToHost, stream_));
+    HB_CUDA(cudaStreamSynchronize(stream_));
+    for (size_t i = 0; i < nq; ++i)
+      if (ids[i] >= n)
+        return fail("qids[" + std::to_string(i) + "] = " + std::to_string(ids[i]) + " is not below nb_point = " +
+                    std::to_string(n));
+  }
   auto run = [&](SearchCtx& c, bool s, float* ms) {
-    SearchCtx::Launch L{d_queries, nq, k, ef_arg, d_out, d_counts, false, 0, {}, {}};
+    SearchCtx::Launch L{d_queries, nq, k, ef_arg, d_out, d_counts, false, 0, {}, {}, d_qids, exclude_self ? d_qids : nullptr};
     const int e = stage_plan(c, leg.plan, L);
     return e ? e : run_plan(c, L, s, ms);
   };
@@ -702,7 +715,8 @@ int Index::stream_wait_last(cudaStream_t s) {
 }
 
 int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const LaunchFilter& f,
-                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms) {
+                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* q_ids,
+                         const uint64_t* skip) {
   if (k == 0) return fail("knbn must be positive");
   if (poisoned_) return fail(poison_msg_);
   cudaStream_t st = c.stream;
@@ -717,6 +731,9 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.q_bytes = dim * es;
   p.q_stride_bytes = dim * es;
   p.nq = (uint32_t)nq;
+  p.q_ids = q_ids;
+  p.skip_ids = skip;
+  k += skip ? 1 : 0;  // the search takes k + 1, each row is k wide (write_row)
   p.k = (int)k;
   p.ef = (int)std::max(ef_arg, k);  // hnsw.rs:1531
   int layer0 = 0;                   // hnsw.rs:1534-1540
@@ -742,7 +759,8 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.smem_per_warp = (int)spw;
   const CtaShape cta = cta_shape(spw, query_threads(kind) / 32);
   if (!cta.warps)
-    return fail("ef / dimension too large: one query needs " + std::to_string(spw) + " bytes of shared memory (limit 220 KB)");
+    return fail(std::string(skip ? "exclude_self searches knbn + 1: " : "") + "ef / dimension too large: one query needs " +
+                std::to_string(spw) + " bytes of shared memory (limit 220 KB)");
   const int wpb = cta.warps;
   const size_t smem = cta.smem;
   p.threads = wpb * 32;
@@ -839,14 +857,14 @@ static const void* device_view_of_host(const void* p) {
 // are being searched), and the answers are written by the kernel straight into the context's pinned result buffer: one
 // synchronisation.  Pageable queries and row pointers are gathered into the context's own pinned staging buffer first
 // (the only host-side copy), which the kernel then reads the same way.
-int Index::search_host_begin(int ci, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                             const LegPlan& plan) {
+int Index::search_host_begin(int ci, const void* queries, const void* const* rows, const uint64_t* qids,
+                             const uint64_t* skip, size_t nq, int d, size_t k, size_t ef, const LegPlan& plan) {
   SearchCtx& c = ctx_[ci];
   cudaStream_t st = c.stream;
   c.pend = SearchCtx::Pending();
   if (nq == 0) return 0;
   HB_CUDA(cudaSetDevice(device));
-  if (dim != 0 && d != dim) return fail("query length differs from the index dimension");
+  if (!qids && dim != 0 && d != dim) return fail("query length differs from the index dimension");
   int r;
   const size_t out_bytes = nq * k * sizeof(NeighbourOut), cnt_bytes = nq * sizeof(int32_t);
   if ((r = ensure_pinned(&c.h_res, &c.h_res_bytes, out_bytes + cnt_bytes + 16, cudaHostAllocMapped | cudaHostAllocPortable))) return r;
@@ -865,31 +883,44 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
     for (size_t i = 0; i < nq * k; ++i) hout[i] = NeighbourOut{~0ull, __builtin_inff(), INVALID_ID};
     return 0;
   }
-  const size_t qbytes = nq * (size_t)dim * es;
-  const void* d_queries = rows ? nullptr : device_view_of_host(queries);  // what the kernel reads
-  if (!d_queries) {
+  char* dv = (char*)device_view_of_host(c.h_res);  // where the kernel writes
+  if (!dv) return fail("the pinned result buffer has no device address");
+  L.out = (NeighbourOut*)dv;
+  L.counts = (int32_t*)(dv + out_bytes);
+  // by stored point: the ids, and the ids the rows leave out, cross the bus in place of the rows (16 bytes a query at
+  // most); they go after the query staging in the pinned buffer and after an exact launch's rows in device memory
+  const size_t qbytes = qids ? 0 : nq * (size_t)dim * es, ib = nq * sizeof(uint64_t);
+  const int nid = (qids ? 1 : 0) + (skip && skip != qids ? 1 : 0);
+  const void* d_queries = qids || rows ? nullptr : device_view_of_host(queries);  // what the kernel reads
+  const size_t staged = qids || d_queries ? 0 : round128(qbytes);
+  if (staged + nid * ib) {
     // gather into pinned staging (rows: one pointer per query, libext.rs parallel_search_neighbours_<ty>)
-    if ((r = ensure_pinned(&c.h_pin, &c.h_pin_bytes, qbytes, cudaHostAllocMapped | cudaHostAllocPortable))) return r;
+    if ((r = ensure_pinned(&c.h_pin, &c.h_pin_bytes, staged + nid * ib, cudaHostAllocMapped | cudaHostAllocPortable))) return r;
     unsigned char* stage = (unsigned char*)c.h_pin;
     if (rows)
       for (size_t i = 0; i < nq; ++i) memcpy(stage + i * (size_t)dim * es, rows[i], (size_t)dim * es);
-    else
+    else if (staged)
       memcpy(stage, queries, qbytes);
-    d_queries = device_view_of_host(stage);
-    if (!d_queries) return fail("the pinned query staging buffer has no device address");
+    if (staged) {
+      d_queries = device_view_of_host(stage);
+      if (!d_queries) return fail("the pinned query staging buffer has no device address");
+    }
+    if (qids) memcpy(stage + staged, qids, ib);
+    if (skip && skip != qids) memcpy(stage + staged + (qids ? ib : 0), skip, ib);
   }
-  char* dv = (char*)device_view_of_host(c.h_res);  // where the kernel writes
-  if (!dv) return fail("the pinned result buffer has no device address");
   L.d_queries = d_queries;
-  L.out = (NeighbourOut*)dv;
-  L.counts = (int32_t*)(dv + out_bytes);
-  if (plan.exact) {
-    // an exact launch may run many CTAs per query (row slices): the queries cross the bus once, into device memory
-    if ((r = ensure_scratch(&c.d_xq, &c.d_xq_bytes, qbytes, st))) return r;
-    HB_CUDA(cudaMemcpyAsync(c.d_xq, d_queries, qbytes, cudaMemcpyDefault, st));
-    L.d_queries = c.d_xq;
-    *hstatus = 0;
+  // an exact launch may run many CTAs per query (row slices): the queries cross the bus once, into device memory
+  const size_t xq = plan.exact ? round128(qbytes) : 0;
+  if (xq + nid * ib) {
+    if ((r = ensure_scratch(&c.d_xq, &c.d_xq_bytes, xq + nid * ib, st))) return r;
+    if (xq) HB_CUDA(cudaMemcpyAsync(c.d_xq, d_queries, qbytes, cudaMemcpyDefault, st));
+    if (xq) L.d_queries = c.d_xq;
+    const uint64_t* ids = (const uint64_t*)((char*)c.d_xq + xq);
+    if (nid) HB_CUDA(cudaMemcpyAsync((void*)ids, (char*)c.h_pin + staged, nid * ib, cudaMemcpyHostToDevice, st));
+    L.q_ids = qids ? ids : nullptr;
+    L.skip = !skip ? nullptr : skip == qids ? ids : ids + (qids ? nq : 0);
   }
+  if (plan.exact) *hstatus = 0;
   // one enqueue (the plan's uploads, the launches, the status); search_host_finish synchronises once and takes the slow
   // path (a visited table overflowed: grow and re-run) only when the status says so
   c.pend.enqueued = true;
@@ -994,13 +1025,16 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
 }
 
 int Index::run_plan(SearchCtx& c, const SearchCtx::Launch& L, bool sync, float* kernel_ms) {
-  if (L.exact) return exact_on_ctx(c, L.d_queries, L.nq, L.k, L.groups, L.out, L.counts, sync, kernel_ms);
+  if (L.exact) return exact_on_ctx(c, L.d_queries, L.nq, L.k, L.groups, L.out, L.counts, sync, kernel_ms, L.q_ids, L.skip);
   int r;
-  if (L.plain && (r = search_on_ctx(c, L.d_queries, L.plain, L.k, L.ef, LaunchFilter(), L.out, L.counts, sync, kernel_ms)))
+  if (L.plain && (r = search_on_ctx(c, L.d_queries, L.plain, L.k, L.ef, LaunchFilter(), L.out, L.counts, sync, kernel_ms,
+                                    L.q_ids, L.skip)))
     return r;
   if (L.plain == L.nq) return 0;
-  const char* q = (const char*)L.d_queries + L.plain * (size_t)dim * es;
-  return search_on_ctx(c, q, L.nq - L.plain, L.k, L.ef, L.filter, L.out + L.plain * L.k, L.counts + L.plain, sync, kernel_ms);
+  const size_t j = L.plain;
+  const char* q = L.q_ids ? nullptr : (const char*)L.d_queries + j * (size_t)dim * es;
+  return search_on_ctx(c, q, L.nq - j, L.k, L.ef, L.filter, L.out + j * L.k, L.counts + j, sync, kernel_ms,
+                       L.q_ids ? L.q_ids + j : nullptr, L.skip ? L.skip + j : nullptr);
 }
 
 int Index::make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx,
@@ -1110,6 +1144,21 @@ int Index::export_vectors(void* out) const {
   if (n == 0) return 0;
   cudaSetDevice(device);
   HB_CUDA(cudaMemcpy2D(out, (size_t)dim * es, graph_.p[GS::VEC], (size_t)row_bytes, (size_t)dim * es, n, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// one 2-D copy per run of consecutive ids of one partition
+int Index::get_vectors(const uint64_t* ranks, size_t count, void* out) const {
+  const uint64_t P = parts ? (uint64_t)parts->count() : 1;
+  const size_t rb = (size_t)dim * es;
+  for (size_t i = 0, e; i < count; i = e) {
+    const uint64_t p = ranks[i] % P, first = ranks[i] / P;
+    for (e = i + 1; e < count && ranks[e] % P == p && ranks[e] / P == first + (e - i);) ++e;
+    const Index* x = parts ? parts->part((int)p) : this;
+    HB_CUDA(cudaSetDevice(x->device));
+    HB_CUDA(cudaMemcpy2D((char*)out + i * rb, rb, (const char*)x->graph_.p[GS::VEC] + first * x->row_bytes,
+                         (size_t)x->row_bytes, rb, e - i, cudaMemcpyDeviceToHost));
+  }
   return 0;
 }
 

@@ -245,7 +245,9 @@ struct LabelSets {
 };
 
 // One host search batch: flat queries or one pointer per query (rows), k answers each into `out`.  `exact`: the exact
-// scan of the points each row may return (ef unused) instead of the graph search.
+// scan of the points each row may return (ef unused) instead of the graph search.  By stored point: query i is the
+// stored vector of qids[i] (an insertion rank; a partitioned handle's global one), and with exclude_self its row leaves
+// that point out (write_row, search_core.cuh).
 struct HostBatch {
   const void* queries = nullptr;
   const void* const* rows = nullptr;
@@ -255,6 +257,8 @@ struct HostBatch {
   Restriction restriction;
   AnswerArrays out;
   bool exact = false;
+  const uint64_t* qids = nullptr;
+  bool exclude_self = false;
 };
 
 // A leg's restriction (Index::resolve): its rows [0, plain) are unrestricted, and `runs` cover the rest, each a range of
@@ -332,8 +336,10 @@ class Index {
                    const float* const* dists);
   // host queries (flat or row pointers) on leased context c under the leg's plan, answers left in the context's pinned
   // buffer (valid until it is released)
-  int search_host_begin(int c, const void* queries, const void* const* rows, size_t nq, int d, size_t k, size_t ef,
-                        const LegPlan& plan);
+  // By stored point (qids, insertion ranks of this Index, instead of queries and rows), and with skip[i] the id row i
+  // leaves out (~0: none; skip may be qids itself).
+  int search_host_begin(int c, const void* queries, const void* const* rows, const uint64_t* qids, const uint64_t* skip,
+                        size_t nq, int d, size_t k, size_t ef, const LegPlan& plan);
   int search_host_finish(int c, const NeighbourOut** out, const int32_t** counts);
   // host search batches (host_search.cu): synchronous, or submitted now and collected by finish_batch.  A ticket is a
   // batch planned into legs, with what the legs read until they are collected: a per-row batch's caller row of each
@@ -344,6 +350,8 @@ class Index {
     AnswerArrays out;
     std::vector<size_t> perm;
     std::vector<const void*> rows;
+    std::vector<uint64_t> qids;  // a per-row batch by stored point: the ids in sorted-row order
+    std::vector<unsigned char> gathered;  // a partitioned batch by stored point: the query rows read from their partitions
     std::vector<std::vector<uint32_t>> bits;
     LabelSets sets;
   };
@@ -399,9 +407,14 @@ class Index {
   // range by binary search in a value-keyed order; slices that follow each other in the order are joined.
   int scan_slices(const uint32_t* set, size_t nset, uint64_t lo, uint64_t hi, std::vector<ExactScan>& slices);
   // device queries in, device answers out; the restriction is none or a resident filter.  `exact`: the exact scan (ef
-  // unused).
+  // unused).  By stored point: d_qids (device, insertion ranks) in place of d_queries, each row without its own point
+  // when exclude_self is set.
   int search_device(const Restriction& rs, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef,
-                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms);
+                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* d_qids = nullptr,
+                    bool exclude_self = false);
+  // the stored vectors of ranks[0, n) into out[n][dim], a partitioned handle's global ranks each from its partition (the
+  // caller checked the ranks)
+  int get_vectors(const uint64_t* ranks, size_t n, void* out) const;
   // filter materialisation: bit per internal id from a sorted origin-id list or a callback
   int make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx,
                        std::vector<uint32_t>& bits) const;
@@ -482,6 +495,8 @@ class Index {
       size_t plain = 0;
       LaunchFilter filter;
       std::vector<ExactGroup> groups;
+      const uint64_t* q_ids = nullptr;  // a search by stored point: in place of d_queries
+      const uint64_t* skip = nullptr;   // per row the id it leaves out: the launches search k + 1
     };
     struct Pending {  // a host search enqueued by search_host_begin, completed by search_host_finish
       Launch run;
@@ -614,13 +629,16 @@ class Index {
 
   VisitedPool vis_;  // visited tables of the insert kernel (searches: SearchCtx)
   SearchCtx ctx_[NCTX + NASYNC];
-  // one graph search launch (the filtered kernel when `f` restricts it)
+  // one graph search launch (the filtered kernel when `f` restricts it).  q_ids: the queries are those stored rows;
+  // skip: rows k wide from a search of k + 1 (SearchParams)
   int search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const LaunchFilter& f,
-                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms);
+                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* q_ids,
+                    const uint64_t* skip);
   // the exact k nearest of device queries, each group's rows among that group's points (aux.cu); the slices' scratch is
-  // sized before the launch
+  // sized before the launch.  q_ids and skip as search_on_ctx takes them.
   int exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const std::vector<ExactGroup>& groups,
-                   NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms);
+                   NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* q_ids,
+                   const uint64_t* skip);
   // the device view of a leg's plan in `run`, with what it needs uploaded into context c
   int stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& run);
   // the launches of `run` on context c: the unrestricted rows as an ordinary unfiltered launch, then the restricted ones

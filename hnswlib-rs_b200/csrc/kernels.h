@@ -81,6 +81,10 @@ struct SearchParams {
   // filtered search: query i's restriction is filter_table[filter_sel[i]], or `filter` when filter_sel is nullptr
   const uint32_t* filter_sel;  // [nq]
   RowFilter filter;
+  // a search by stored point: query i is row q_ids[i] of g.vec instead of `queries` (query_row, search_core.cuh)
+  const uint64_t* q_ids;
+  // nullptr, or per row the id the row leaves out (~0: none): k is knbn + 1 and each row knbn wide (write_row)
+  const uint64_t* skip_ids;
 };
 
 // the label of a point that has none (hnsw_b200_set_labels): no label admits it

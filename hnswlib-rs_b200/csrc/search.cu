@@ -35,7 +35,7 @@ __global__ void __launch_bounds__(SEARCH_THREADS, 4) search_kernel(SearchParams 
     const uint32_t qi = next_item(p.work_counter, lane);
     if (qi >= p.nq) break;
     // stage the query (zero padded to d_pad)
-    stage_row_bytes(s.q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes, p.q_bytes, g.d4 * 16);
+    stage_row_bytes(s.q4, query_row(g, p.q_ids, p.queries, p.q_stride_bytes, qi), p.q_bytes, g.d4 * 16);
     int count = 0;
     bool overflow = false;
     if (g.entry != INVALID_ID) {  // hnsw.rs:1498-1503

@@ -163,26 +163,61 @@ __device__ __forceinline__ Entry descend(const GraphView& g, int lane, Stats& st
   return Entry{pivot, best};
 }
 
-// The answers of query qi (hnsw.rs:1544-1579): key_at(j) for j < count, ascending, then (~0, +inf, INVALID_ID) up to k.
-// A query whose visited table overflowed answers nothing and raises the launch's status flag (the host re-runs it).
+// Where query qi of a launch is: row q_ids[qi] of the store for a search by stored point (rows are zero padded to whole
+// lines, so staging one gives the bytes its vector would), else row qi of `queries`, `stride` bytes apart.
+__device__ __forceinline__ const char* query_row(const GraphView& g, const uint64_t* q_ids, const void* queries, size_t stride,
+                                                 uint32_t qi) {
+  if (q_ids) return reinterpret_cast<const char*>(g.vec) + (size_t)q_ids[qi] * ((size_t)g.d4 * 16);
+  return reinterpret_cast<const char*>(queries) + (size_t)qi * stride;
+}
+
+// Row qi of a launch's answers from its keys key_at(0 .. count - 1), ascending: those keep(id) admits, as (origin,
+// distance, internal id), then (~0, +inf, INVALID_ID) to the row's width, and their count.  Without skip ids a row is k
+// wide.  With them (a search by stored point that leaves the point out) the launch searched k = knbn + 1 and a row is
+// k - 1 wide: the key whose id is skip[qi] is left out and the rest cut to that width, which is the k-row without that
+// entry, or without its last one when it does not hold it.
+template <class KeyAt, class Keep>
+__device__ __forceinline__ void write_row(NeighbourOut* out, int32_t* counts, const uint64_t* origin, int k,
+                                          const uint64_t* skip, uint32_t qi, int lane, int count, KeyAt&& key_at, Keep&& keep) {
+  const uint64_t skip_id = skip ? skip[qi] : ~0ull;
+  const int w = skip ? k - 1 : k;
+  NeighbourOut* o = out + (size_t)qi * w;
+  int n = 0;
+  for (int b = 0; b < count && n < w; b += 32) {  // warp-uniform trip count
+    const int j = b + lane;
+    uint64_t key = 0;
+    bool in = false;
+    if (j < count) {
+      key = key_at(j);
+      in = key_id(key) != skip_id && keep(key_id(key));
+    }
+    const unsigned m = __ballot_sync(FULL, in);
+    const int at = n + __popc(m & ((1u << lane) - 1u));
+    if (in && at < w) {
+      const uint32_t id = key_id(key);
+      o[at] = NeighbourOut{origin[id], key_dist(key), id};
+    }
+    n += __popc(m);
+  }
+  n = min(n, w);
+  for (int j = n + lane; j < w; j += 32) o[j] = NeighbourOut{~0ull, __int_as_float(0x7f800000), INVALID_ID};
+  if (lane == 0) counts[qi] = n;
+  __syncwarp();
+}
+
+struct KeepAll {
+  __device__ __forceinline__ bool operator()(uint32_t) const { return true; }
+};
+
+// The answers of query qi (hnsw.rs:1544-1579): key_at(j) for j < count, ascending (write_row).  A query whose visited
+// table overflowed answers nothing and raises the launch's status flag (the host re-runs it).
 template <class KeyAt>
 __device__ __forceinline__ void write_answers(const SearchParams& p, int lane, uint32_t qi, bool overflow, int count, KeyAt&& key_at) {
   if (overflow) {
     if (lane == 0) atomicExch(p.status, 1);
     count = 0;
   }
-  const size_t ob = (size_t)qi * p.k;
-  for (int j = lane; j < p.k; j += 32) {
-    if (j < count) {
-      const uint64_t key = key_at(j);
-      const uint32_t id = key_id(key);
-      p.out_nb[ob + j] = NeighbourOut{p.g.origin[id], key_dist(key), id};
-    } else {
-      p.out_nb[ob + j] = NeighbourOut{~0ull, __int_as_float(0x7f800000), INVALID_ID};
-    }
-  }
-  if (lane == 0) p.out_count[qi] = count;
-  __syncwarp();
+  write_row(p.out_nb, p.out_count, p.g.origin, p.k, p.skip_ids, qi, lane, count, key_at, KeepAll());
 }
 
 // the traversal counters of one warp into the launch's totals (the counters are warp-uniform)

@@ -159,7 +159,7 @@ __global__ void __launch_bounds__(LEAN_THREADS, LEAN_MIN_BLOCKS) search_lean_ker
     if (qi >= p.nq) break;
     // ---- the lane's chunks of the query (zero padded) -> registers, through the queue buffer
     {
-      const char* src = reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_stride_bytes;
+      const char* src = query_row(G, p.q_ids, p.queries, p.q_stride_bytes, qi);
       const int nw = p.q_bytes >> 2;
       if ((reinterpret_cast<size_t>(src) & 3) == 0) {
         const uint32_t* s32 = reinterpret_cast<const uint32_t*>(src);

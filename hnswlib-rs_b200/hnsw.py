@@ -114,6 +114,10 @@ def load_library():
     L.hnsw_b200_get_attributes.argtypes = [vp, u64, u64, vp]
     L.hnsw_b200_search_flat_ranges.argtypes = [vp, vp, vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_exact_ranges.argtypes = [vp, vp, vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_get_vectors.argtypes = [vp, vp, u64, vp]
+    L.hnsw_b200_search_flat_by_id.argtypes = [vp, vp, u64, u64, u64, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_exact_by_id.argtypes = [vp, vp, u64, u64, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_device_by_id.argtypes = [vp, i32, i64, vp, u64, u64, u64, i32, vp, vp, i32, vp]
     L.hnsw_b200_get_stats.argtypes = [vp, vp, i32]
     L.hnsw_b200_set_stream.argtypes = [vp, vp]
     L.hnsw_b200_join.argtypes = [vp]
@@ -616,6 +620,77 @@ class Hnsw:
         admits for it, in one batch.  Returns search_exact's tuple."""
         return self._ranged(self._L.hnsw_b200_search_exact_ranges, queries, knbn, (), ranges, sets, with_internal,
                             with_pid)
+
+    # ---- search by stored point (include/hnsw_b200.h "Search by stored point")
+    def get_vectors(self, ranks):
+        """hnsw_b200_get_vectors: the stored vectors of the points with insertion ranks `ranks` (a partitioned handle:
+        global ranks), as an [n, dim] array"""
+        r = np.ascontiguousarray(ranks, np.uint64).reshape(-1)
+        out = np.empty((r.size, self.get_data_dimension()), self.dtype)
+        self._chk(self._L.hnsw_b200_get_vectors(self._h, _p(r), r.size, _p(out)))
+        return out
+
+    def get_point_data(self, p_id):
+        """Hnsw::get_point_data (hnsw.rs:587-598): the stored vector of the point whose PointId is p_id = (level, rank
+        in that level), or None when no point has that PointId"""
+        level, rank = int(p_id[0]), int(p_id[1])
+        if level < 0 or rank < 0:
+            return None
+        lv, rk, _, _ = self.export_points()
+        hit = np.flatnonzero((lv == level) & (rk == rank))
+        return self.get_vectors(hit[:1])[0] if hit.size else None
+
+    def _by_id(self, fn, qids, knbn, mid, exclude_self, filter, sets, ranges, with_internal, with_pid):
+        q = np.ascontiguousarray(qids, np.uint64).reshape(-1)
+        nq = q.size
+        rg = None if ranges is None else _ranges(ranges, nq)
+        off, vals = (None, None) if sets is None else _label_sets(sets, nq)
+        ans = self._answers(nq, knbn, with_internal, with_pid)
+        self._chk(fn(self._h, _p(q), nq, int(knbn), *mid, int(bool(exclude_self)), _filter_id(filter), _p(rg), _p(off),
+                     _p(vals), *map(_p, ans)))
+        return ans
+
+    def search_by_id(self, qids, knbn, ef, filter=None, sets=None, ranges=None, exclude_self=False, with_internal=True,
+                     with_pid=True):
+        """hnsw_b200_search_flat_by_id: query i is the stored point qids[i] (an insertion rank).  Row i equals
+        search_flat (filter: a ResidentFilter), search_flat_label_sets (sets) or search_flat_ranges (ranges, optionally
+        with sets) on get_vectors(qids[i]).  exclude_self: the row of knbn + 1 without the point itself (or without its
+        last entry when it does not hold the point), cut to knbn.  Returns search_flat's tuple."""
+        return self._by_id(self._L.hnsw_b200_search_flat_by_id, qids, knbn, (int(ef),), exclude_self, filter, sets, ranges,
+                           with_internal, with_pid)
+
+    def search_exact_by_id(self, qids, knbn, filter=None, sets=None, ranges=None, exclude_self=False, with_internal=True,
+                           with_pid=True):
+        """hnsw_b200_search_exact_by_id: search_by_id with the exact searches in place of the graph ones"""
+        return self._by_id(self._L.hnsw_b200_search_exact_by_id, qids, knbn, (), exclude_self, filter, sets, ranges,
+                           with_internal, with_pid)
+
+    def search_device_by_id(self, d_qids_ptr, nq, knbn, ef, d_out_ptr, d_counts_ptr, exclude_self=False, exact=False,
+                            sync=True, filter=None):
+        """hnsw_b200_search_device_by_id: search_device (exact: search_exact_device) with query i the stored point
+        whose insertion rank is the uint64 d_qids[i] on the device.  Returns the kernel's CUDA-event time in ms when sync
+        is true."""
+        ms = C.c_float(0.0)
+        self._chk(self._L.hnsw_b200_search_device_by_id(self._h, int(bool(exact)), _filter_id(filter), C.c_void_p(d_qids_ptr),
+                                                        int(nq), int(knbn), int(ef), int(bool(exclude_self)),
+                                                        C.c_void_p(d_out_ptr), C.c_void_p(d_counts_ptr), int(bool(sync)),
+                                                        C.byref(ms) if sync else None))
+        return float(ms.value)
+
+    def knn_graph(self, k, ef=None, exact=False, batch=65536):
+        """every stored point's k nearest other points, by insertion rank: (internal ids u32[n, k], distances
+        f32[n, k]), a row's slots past its count holding (0xFFFFFFFF, +inf).  Batches of `batch` points through
+        search_by_id (ef: default k) or, exact, search_exact_by_id, each with exclude_self."""
+        n = self.get_nb_point()
+        ids, ds = np.empty((n, k), np.uint32), np.empty((n, k), np.float32)
+        for s in range(0, n, int(batch)):
+            q = np.arange(s, min(n, s + int(batch)), dtype=np.uint64)
+            if exact:
+                _, d, it, _, _ = self.search_exact_by_id(q, k, exclude_self=True, with_pid=False)
+            else:
+                _, d, it, _, _ = self.search_by_id(q, k, k if ef is None else ef, exclude_self=True, with_pid=False)
+            ids[s:s + q.size], ds[s:s + q.size] = it, d
+        return ids, ds
 
     def make_filter(self, filter):
         """hnsw_b200_filter_new: materialise a FilterT (sorted id sequence or callable(id)->bool, as search_flat takes)

@@ -463,6 +463,45 @@ int hnsw_b200_search_exact_ranges(const void* h, const int64_t* qrange, const ui
                                   const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids,
                                   float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
 
+/* ---- Search by stored point: the queries are points of the index, named by id, and their vectors are read where they
+ * are stored ("more like this", near-duplicates, the k-NN graph of the data).  Nothing but 8 bytes per query crosses
+ * the bus on the way in.
+ *   Ids: insertion ranks, the ids set_labels / set_attributes address and out_internal reports.  On a partitioned handle
+ *     they are global ranks (point g is local point g / P of partition g % P); on a partition view, its local ids.
+ *   get_vectors: out[i] is the stored vector of ranks[i] (dim elements each); a partitioned handle reads each from its
+ *     partition.  n == 0 returns 0; NULL ranks or out, and the first ranks[i] >= nb_point (named with i), are refused.
+ *   Rows: row i is, bit for bit, what the call below returns for the query "get_vectors of qids[i]" (ids, distance bits,
+ *     internal ids, PointIds, counts and, with statistics on, the traversal counters):
+ *       search_flat_by_id: search_flat with no restriction (filter -1, qrange, qset_off and qset NULL), which follows
+ *         the tie mode; search_flat_filtered with resident filter `filter`; search_flat_label_sets (qrange NULL) or
+ *         search_flat_ranges (qrange set; qset_off and qset both NULL: {HNSW_B200_LABEL_NONE} per query), with the
+ *         sets and ranges read as those calls read them;
+ *       search_exact_by_id: search_exact, search_exact_label_sets or search_exact_ranges likewise.
+ *   exclude_self != 0: row i is the row of that same call with knbn + 1 (so ef becomes max(ef_search, knbn + 1)),
+ *     without the entry whose internal id is qids[i], or without its last entry when it does not hold that id, cut to
+ *     knbn.  Other points with an identical vector stay.  Under DistDot, or under a restriction that does not admit the
+ *     point, the point may be absent from its row; the rule holds all the same.  The rows stay knbn wide.
+ *   Checks, before anything runs: a NULL handle is refused; nq == 0 returns 0; qids NULL is refused; the first
+ *     qids[i] >= nb_point is refused, naming i and the value; filter != -1 together with qrange, qset_off or qset is
+ *     refused; with exclude_self, a knbn + 1 beyond a kernel's limit is refused.  Otherwise the checks of the call the
+ *     row is defined by apply (stale, foreign or unknown filters, bad set offsets).
+ *   search_device_by_id: d_qids on the device, answers as search_device / search_exact_device (exact != 0) leave them,
+ *     no restriction or one resident filter, with their sync, join, stream_wait_last, check_status and overflow rules.
+ *     To check the ids it reads them back once the work already on the handle's stream is done.  Refused on a
+ *     partitioned handle. */
+int hnsw_b200_get_vectors(const void* h, const uint64_t* ranks, uint64_t n, void* out /* [n][dim] elements */);
+int hnsw_b200_search_flat_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, uint64_t ef_search,
+                                int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                                const uint32_t* qset, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                                int32_t* out_pid, int32_t* out_counts);
+int hnsw_b200_search_exact_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, int exclude_self,
+                                 int64_t filter, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                                 uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
+                                 int32_t* out_counts);
+int hnsw_b200_search_device_by_id(const void* h, int exact, int64_t filter, const uint64_t* d_qids, uint64_t nq,
+                                  uint64_t knbn, uint64_t ef_search, int exclude_self, void* d_out, int32_t* d_counts,
+                                  int sync, float* kernel_ms);
+
 /* Run this handle's kernels and copies on a caller-owned CUDA stream (cudaStream_t passed as void*; NULL
  * restores the handle's own stream), e.g. so that torch.cuda.Event on torch's current stream brackets them. */
 int hnsw_b200_join(void* h);
