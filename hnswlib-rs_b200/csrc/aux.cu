@@ -63,6 +63,13 @@ static cudaError_t launch_dist_batch_for_op(const AuxParams& p, int grid, size_t
 // bit-identical to warp_dists'.  A key that beats its query's threshold goes to a per-query candidate list; after each
 // block the warp that owns the query (query % 8) merges the list into the query's sorted queue.  With slices > 1 every
 // CTA leaves its top k in `part` and the last CTA of a tile to finish (ticket) merges the slices' lists.
+// Radius mode (radius != nullptr): a query's threshold is its radius key, (bits(r) << 32) | 0xFFFFFFFF, which a key
+// beats exactly when its distance is <= r (distances are >= 0, common.cuh).  It does not tighten when the queue is full,
+// so every key within the radius reaches the candidate list (at most `rows` per query and block, as in k-NN mode), and
+// the queue still keeps the k smallest of them (queue_offer admits only what it accepts).  The merging warp counts each
+// list's keys other than the row's skip id into a register of the lane that holds that query (lane j: the warp's query
+// warp + 8j), and each CTA adds its counts to `totals` once at the end.  The scoring loop and the shared-memory layout
+// are those of k-NN mode.
 struct ExactParams {
   GraphView g;
   const void* queries;   // device, [nq][q_bytes] raw element bytes
@@ -80,6 +87,8 @@ struct ExactParams {
   const ExactTile* tiles;  // nullptr: tile t is queries [t * tq, t * tq + tq) over (list, npts); else tile t is tiles[t]
   const uint64_t* q_ids;     // as SearchParams' (a search by stored point)
   const uint64_t* skip_ids;  // as SearchParams': k is knbn + 1 and each row of `out` knbn wide
+  const float* radius;       // radius mode: [nq] per launch row, each >= 0 and not NaN (nullptr: k-NN)
+  uint32_t* totals;          // radius mode: [nq] per launch row, zero at launch: the admitted points within the radius
 };
 
 // keys[0, c) (~0 = none) into the warp's sorted queue Q, 32 at a time: those Q accepts, inserted in lane order.  The keys
@@ -141,7 +150,13 @@ __global__ void __launch_bounds__(256, 2) exact_knn_kernel(ExactParams p) {
     thr[q] = ~0ull;
     ccount[q] = 0;
     qn[q] = 0;
+    if (p.radius && q < nqt) thr[q] = ((uint64_t)__float_as_uint(p.radius[q0 + q]) << 32) | 0xFFFFFFFFull;
   }
+  // radius mode: lane j's count of keys within the radius, and the id it leaves out, for this warp's query warp + 8j
+  const bool radius = p.radius != nullptr;
+  const int my_q = warp + 8 * lane;
+  uint32_t within = 0;
+  const uint32_t my_skip = radius && p.skip_ids && lane < 4 && my_q < nqt ? (uint32_t)p.skip_ids[q0 + my_q] : INVALID_ID;
   __syncthreads();
 
   // warp 0: block b of the slice into ring slot b % NS, one bulk copy per row (lane i: row i)
@@ -203,15 +218,23 @@ __global__ void __launch_bounds__(256, 2) exact_knn_kernel(ExactParams p) {
       Q.w = queue + (size_t)q * k;
       Q.n = qn[q];
       Q.cap = k;
+      if (radius) {  // every candidate is within the radius
+        const int j = (q - warp) >> 3;
+        const uint32_t skip = __shfl_sync(FULL, my_skip, j);
+        const unsigned in = __ballot_sync(FULL, lane < c && key_id(cand[q * B + lane]) != skip);
+        if (lane == j) within += __popc(in);
+      }
       queue_offer(Q, cand + q * B, c, false);
       if (lane == 0) {
         qn[q] = Q.n;
-        thr[q] = Q.n < k ? ~0ull : Q.w[k - 1];
+        if (!radius) thr[q] = Q.n < k ? ~0ull : Q.w[k - 1];
         ccount[q] = 0;
       }
     }
     __syncthreads();
   }
+
+  if (radius && lane < 4 && my_q < nqt && within) atomicAdd(p.totals + q0 + my_q, within);
 
   // answers: the first n keys (write_row)
   auto write = [&](int q, const uint64_t* w, int n) {
@@ -274,10 +297,11 @@ static bool exact_shape(int d4, size_t k, size_t nq, ExactParams& p, size_t& sme
 
 int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const std::vector<ExactGroup>& groups,
                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* q_ids,
-                        const uint64_t* skip) {
+                        const uint64_t* skip, const float* radius, uint32_t* totals) {
   if (k == 0) return fail("knbn must be positive");
   if (poisoned_) return fail(poison_msg_);
   cudaStream_t st = c.stream;
+  if (radius) HB_CUDA(cudaMemsetAsync(totals, 0, nq * sizeof(uint32_t), st));
   if (dim == 0) {  // empty index: every answer is empty
     HB_CUDA(cudaMemsetAsync(d_counts, 0, nq * sizeof(int32_t), st));
     if (sync) HB_CUDA(cudaStreamSynchronize(st));
@@ -295,6 +319,8 @@ int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k
   p.npts = (uint32_t)(scan.ids ? scan.n : n);
   p.q_ids = q_ids;
   p.skip_ids = skip;
+  p.radius = radius;
+  p.totals = totals;
   k += skip ? 1 : 0;  // the scan keeps k + 1 keys, each row is k wide (write_row)
   p.k = (int)k;
   size_t widest_group = 0;

@@ -1,5 +1,7 @@
 // extern "C" surface of libhnsw_b200.so: the reference's libext.rs symbols (f32) + extensions.
 // Declarations and the reference file:line each one replaces are in include/hnsw_b200.h.
+#include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <exception>
 #include <cstring>
@@ -626,10 +628,12 @@ int hnsw_b200_insert_flat(void* h, const void* vecs, uint64_t n, uint64_t dim, c
 // exact scan of those points instead of the graph search (ef unused).
 enum Via { HOST, SUBMIT, DEVICE };
 // By stored point (qids, checked by the caller to be non-NULL): the queries are the stored vectors of qids[0, nq), each
-// below the handle's nb_point, and `dim` is the handle's; exclude_self: each row leaves its own point out.
+// below the handle's nb_point, and `dim` is the handle's; exclude_self: each row leaves its own point out.  Radius (an
+// exact HOST call, checked by the caller): row i holds only the points within radius[i], and out.total their number.
 static int64_t search_call(const void* h, Via via, const char* name, const Restriction& rs, bool exact, const void* queries,
                            uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef, const AnswerArrays& out, int sync = 1,
-                           float* kernel_ms = nullptr, const uint64_t* qids = nullptr, bool exclude_self = false) {
+                           float* kernel_ms = nullptr, const uint64_t* qids = nullptr, bool exclude_self = false,
+                           const float* radius = nullptr) {
   HB_HS(h);
   if (via != HOST) HB_NOT_PARTITIONED(ix, name);
   if (via == DEVICE)
@@ -653,6 +657,7 @@ static int64_t search_call(const void* h, Via via, const char* name, const Restr
   b.exact = exact;
   b.qids = qids;
   b.exclude_self = exclude_self;
+  b.radius = radius;
   if (via == HOST) return pass(ix, ix->search_batch(b));
   const int64_t t = ix->submit_batch(b);
   if (t < 0) g_err = ix->err();
@@ -900,20 +905,14 @@ int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_q
                           on_device(d_out, d_counts), sync, kernel_ms);
 }
 
-// Search by stored point: the restriction of a by-id call (-1 and no sets or ranges: none), refused when a resident
-// filter comes with sets or ranges; a range without sets is a range within {LABEL_NONE} per query, as ranged_call reads
-// it, and sets without ranges are the label-sets call's
-static int by_id_call(const void* h, Via via, const char* name, bool exact, const uint64_t* qids, uint64_t nq, uint64_t knbn,
-                      uint64_t ef, int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
-                      const uint32_t* qset, const AnswerArrays& out, int sync = 1, float* kernel_ms = nullptr) {
-  if (!h) return set_err("NULL handle");
-  if (nq == 0) return 0;
-  if (!qids) return set_err(std::string(name) + ": qids is NULL");
+// The restriction of a by-id or radius call (-1 and no sets or ranges: none), refused when a resident filter comes with
+// sets or ranges; a range without sets is a range within {LABEL_NONE} per query, as ranged_call reads it (the offsets
+// and values made in off and none), and sets without ranges are the label-sets call's
+static int one_restriction(const char* name, uint64_t nq, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                           const uint32_t* qset, std::vector<uint64_t>& off, std::vector<uint32_t>& none, Restriction& rs) {
   const bool rows = qrange || qset_off || qset;
   if (filter != -1 && rows)
     return set_err(std::string(name) + ": a resident filter cannot be combined with label sets or ranges");
-  std::vector<uint64_t> off;
-  std::vector<uint32_t> none;
   if (qrange && !qset_off && !qset) {
     off.resize(nq + 1);
     std::iota(off.begin(), off.end(), (uint64_t)0);
@@ -921,7 +920,21 @@ static int by_id_call(const void* h, Via via, const char* name, bool exact, cons
     qset_off = off.data();
     qset = none.data();
   }
-  const Restriction rs = rows ? row_label_sets(qset_off, qset, qrange) : resident_or_all(filter);
+  rs = rows ? row_label_sets(qset_off, qset, qrange) : resident_or_all(filter);
+  return 0;
+}
+
+// Search by stored point, under one_restriction's restriction
+static int by_id_call(const void* h, Via via, const char* name, bool exact, const uint64_t* qids, uint64_t nq, uint64_t knbn,
+                      uint64_t ef, int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                      const uint32_t* qset, const AnswerArrays& out, int sync = 1, float* kernel_ms = nullptr) {
+  if (!h) return set_err("NULL handle");
+  if (nq == 0) return 0;
+  if (!qids) return set_err(std::string(name) + ": qids is NULL");
+  std::vector<uint64_t> off;
+  std::vector<uint32_t> none;
+  Restriction rs;
+  if (one_restriction(name, nq, filter, qrange, qset_off, qset, off, none, rs)) return -1;
   return (int)search_call(h, via, name, rs, exact, nullptr, nq, 0, knbn, ef, out, sync, kernel_ms, qids, exclude_self != 0);
 }
 int hnsw_b200_search_flat_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, uint64_t ef_search,
@@ -943,6 +956,61 @@ int hnsw_b200_search_device_by_id(const void* h, int exact, int64_t filter, cons
                                   int sync, float* kernel_ms) {
   return by_id_call(h, DEVICE, "search_device_by_id", exact != 0, d_qids, nq, knbn, exact ? 0 : ef_search, exclude_self,
                     filter, nullptr, nullptr, nullptr, on_device(d_out, d_counts), sync, kernel_ms);
+}
+
+// Radius search: the exact scan of host queries (qids == nullptr) or of stored points, under one_restriction's
+// restriction, each row cut at its radius and its total of points within it into out_total (may be NULL).  Every radius
+// is checked before anything runs: >= 0 and not NaN, -0 read as 0 (whose key is the smallest).  knbn == 0 counts only:
+// the scan runs at k = 1 into scratch rows, the caller's row arrays may be NULL, and every count is 0.
+static int radius_call(const void* h, const char* name, bool by_id, const void* queries, uint64_t dim, const uint64_t* qids,
+                       uint64_t nq, const float* radius, uint64_t knbn, int exclude_self, int64_t filter,
+                       const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset, AnswerArrays out,
+                       uint64_t* out_total) {
+  if (!h) return set_err("NULL handle");
+  if (nq == 0) return 0;
+  if (by_id && !qids) return set_err(std::string(name) + ": qids is NULL");
+  if (!radius) return set_err(std::string(name) + ": radius is NULL");
+  std::vector<float> r(nq);
+  for (uint64_t i = 0; i < nq; ++i) {
+    if (std::isnan(radius[i]) || radius[i] < 0)
+      return set_err(std::string(name) + ": radius[" + std::to_string(i) + "] = " + std::to_string(radius[i]) + " is " +
+                     (std::isnan(radius[i]) ? "NaN" : "negative"));
+    r[i] = radius[i] == 0 ? 0.0f : radius[i];
+  }
+  std::vector<uint64_t> off;
+  std::vector<uint32_t> none;
+  Restriction rs;
+  if (one_restriction(name, nq, filter, qrange, qset_off, qset, off, none, rs)) return -1;
+  std::vector<uint64_t> scratch_ids;
+  std::vector<float> scratch_dist;
+  if (knbn == 0) {
+    scratch_ids.resize(nq);
+    scratch_dist.resize(nq);
+    out.ids = scratch_ids.data();
+    out.dist = scratch_dist.data();
+    out.internal = nullptr;
+    out.pid = nullptr;
+  }
+  out.total = out_total;
+  const int rc = (int)search_call(h, HOST, name, rs, true, queries, nq, dim, knbn ? knbn : 1, 0, out, 1, nullptr, qids,
+                                  exclude_self != 0, r.data());
+  if (rc == 0 && knbn == 0) std::fill(out.counts, out.counts + nq, 0);
+  return rc;
+}
+int hnsw_b200_search_exact_radius(const void* h, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                                  const uint32_t* qset, const void* queries, uint64_t nq, uint64_t dim,
+                                  const float* radius, uint64_t knbn, uint64_t* out_ids, float* out_dist,
+                                  uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts, uint64_t* out_total) {
+  return radius_call(h, "search_exact_radius", false, queries, dim, nullptr, nq, radius, knbn, 0, filter, qrange, qset_off,
+                     qset, columns(out_ids, out_dist, out_internal, out_pid, out_counts), out_total);
+}
+int hnsw_b200_search_exact_radius_by_id(const void* h, const uint64_t* qids, uint64_t nq, const float* radius,
+                                        uint64_t knbn, int exclude_self, int64_t filter, const int64_t* qrange,
+                                        const uint64_t* qset_off, const uint32_t* qset, uint64_t* out_ids,
+                                        float* out_dist, uint32_t* out_internal, int32_t* out_pid,
+                                        int32_t* out_counts, uint64_t* out_total) {
+  return radius_call(h, "search_exact_radius_by_id", true, nullptr, 0, qids, nq, radius, knbn, exclude_self, filter, qrange,
+                     qset_off, qset, columns(out_ids, out_dist, out_internal, out_pid, out_counts), out_total);
 }
 
 int hnsw_b200_get_vectors(const void* h, const uint64_t* ranks, uint64_t n, void* out) {

@@ -86,11 +86,13 @@ static inline void point_id(const Index* rx, uint32_t it, int32_t* pid2) {
 }
 
 // rows [first, first + count) of `out` from one leg's answers (k slots each, as the kernels left them: the slots beyond a
-// query's count hold (~0, +inf, INVALID_ID)): plain copies
+// query's count hold (~0, +inf, INVALID_ID)), and a radius batch's totals: plain copies
 static void put_rows(const AnswerArrays& out, const Index* rx, size_t first, size_t count, size_t k, const NeighbourOut* a,
-                     const int32_t* cnts) {
+                     const int32_t* cnts, const uint32_t* tots) {
   if (count == 0) return;
   memcpy(out.counts + first, cnts, count * sizeof(int32_t));
+  if (out.total && tots)
+    for (size_t i = 0; i < count; ++i) out.total[first + i] = tots[i];
   const size_t o = first * k, tot = count * k;
   if (out.nb) {
     memcpy(out.nb + o, a, tot * sizeof(NeighbourOut));
@@ -114,9 +116,10 @@ static void put_rows(const AnswerArrays& out, const Index* rx, size_t first, siz
 
 // queries [first, first + count) of the batch from one leg's answers, each to its row of `out` (out.perm)
 static void put_slice(const AnswerArrays& out, const Index* rx, size_t first, size_t count, size_t k, const NeighbourOut* a,
-                      const int32_t* cnts) {
-  if (!out.perm) return put_rows(out, rx, first, count, k, a, cnts);
-  for (size_t i = 0; i < count; ++i) put_rows(out, rx, out.perm[first + i], 1, k, a + i * k, cnts + i);
+                      const int32_t* cnts, const uint32_t* tots) {
+  if (!out.perm) return put_rows(out, rx, first, count, k, a, cnts, tots);
+  for (size_t i = 0; i < count; ++i)
+    put_rows(out, rx, out.perm[first + i], 1, k, a + i * k, cnts + i, tots ? tots + i : nullptr);
 }
 
 // slot s of `out` from answer e of index rx, reported with internal id `internal` (a partitioned handle's global rank)
@@ -132,9 +135,11 @@ static inline void put_answer(const AnswerArrays& out, size_t s, const Index* rx
 }
 
 // every query of the batch from the answers of P partition legs, merged by merge_lists, to its row of `out` (out.perm);
-// the slots past a query's count are padded with (~0, +inf, INVALID_ID) and PointId (-1, -1)
+// the slots past a query's count are padded with (~0, +inf, INVALID_ID) and PointId (-1, -1).  A radius batch's total is
+// the sum of the partitions' (t: each leg's totals).
 static void put_merged(const AnswerArrays& out, const std::vector<Leg>& legs, size_t nq, size_t k,
-                       const std::vector<const NeighbourOut*>& a, const std::vector<const int32_t*>& c) {
+                       const std::vector<const NeighbourOut*>& a, const std::vector<const int32_t*>& c,
+                       const std::vector<const uint32_t*>& t) {
   const int P = (int)legs.size();
   const NeighbourOut pad{~0ull, __builtin_inff(), INVALID_ID};
   int32_t cnt[Partitions::MAX_PARTS];
@@ -149,6 +154,11 @@ static void put_merged(const AnswerArrays& out, const std::vector<Leg>& legs, si
         });
     for (size_t j = total; j < k; ++j) put_answer(out, w + j, nullptr, pad, INVALID_ID);
     out.counts[row] = (int32_t)total;
+    if (out.total && t[0]) {
+      uint64_t sum = 0;
+      for (int p = 0; p < P; ++p) sum += t[p][q];
+      out.total[row] = sum;
+    }
   }
 }
 
@@ -385,7 +395,8 @@ void Index::begin_leg(const HostBatch& b, Leg& l) {
     ids = nullptr;
   }
   const void* q = b.rows || ids ? nullptr : (const char*)b.queries + l.first * (size_t)b.d * es;
-  l.rc = l.rx->search_host_begin(l.ctx, q, b.rows ? b.rows + l.first : nullptr, ids, skip, l.count, b.d, b.k, b.ef, l.plan);
+  l.rc = l.rx->search_host_begin(l.ctx, q, b.rows ? b.rows + l.first : nullptr, ids, skip, l.count, b.d, b.k, b.ef, l.plan,
+                                 b.radius ? b.radius + l.first : nullptr);
   l.begun = l.rc == 0;
 }
 
@@ -404,8 +415,9 @@ int Index::end_leg(Leg& l, size_t k, const AnswerArrays& out) {
   if (l.begun) {
     const NeighbourOut* a = nullptr;
     const int32_t* c = nullptr;
-    l.rc = l.rx->search_host_finish(l.ctx, &a, &c);
-    if (!l.rc) put_slice(out, l.rx, l.first, l.count, k, a, c);
+    const uint32_t* t = nullptr;
+    l.rc = l.rx->search_host_finish(l.ctx, &a, &c, &t);
+    if (!l.rc) put_slice(out, l.rx, l.first, l.count, k, a, c, t);
   }
   release_leg(l);
   return l.rc;
@@ -414,7 +426,7 @@ int Index::end_leg(Leg& l, size_t k, const AnswerArrays& out) {
 // ------------------------------------------------------------------------------------------------ batches
 // The batch `call` planned into t's legs, each with its plan; `b` is the batch as the legs run it.  A per-row restriction:
 // the batch is planned over the rows sorted by filter or label set, gathered through row pointers (by stored point: its
-// ids permuted), and each answer goes back to its caller's row.  A batch by stored point on a partitioned handle has its
+// ids and radii permuted), and each answer goes back to its caller's row.  A batch by stored point on a partitioned handle has its
 // rows gathered from their partitions first, since no device reads another partition's store, and is then searched as
 // host queries.  A leg that could not have its plan is reported in leg order, or the replicas' first.
 int Index::prepare_batch(const HostBatch& call, HostBatch& b, Ticket& t, bool replicas_first) {
@@ -433,6 +445,11 @@ int Index::prepare_batch(const HostBatch& call, HostBatch& b, Ticket& t, bool re
       t.qids.resize(call.nq);
       for (size_t j = 0; j < call.nq; ++j) t.qids[j] = call.qids[t.perm[j]];
       b.qids = t.qids.data();
+    }
+    if (call.radius) {
+      t.radius.resize(call.nq);
+      for (size_t j = 0; j < call.nq; ++j) t.radius[j] = call.radius[t.perm[j]];
+      b.radius = t.radius.data();
     }
     if (!call.qids || parts) {
       t.rows.resize(call.nq);
@@ -481,11 +498,12 @@ int Index::search_batch(const HostBatch& call) {
   }
   std::vector<const NeighbourOut*> a(n);
   std::vector<const int32_t*> c(n);
+  std::vector<const uint32_t*> tot(n);
   for (int p = 0; p < n; ++p) {
-    if (legs[p].begun) legs[p].rc = legs[p].rx->search_host_finish(legs[p].ctx, &a[p], &c[p]);
+    if (legs[p].begun) legs[p].rc = legs[p].rx->search_host_finish(legs[p].ctx, &a[p], &c[p], &tot[p]);
     if (legs[p].rc && bad < 0) bad = p;
   }
-  if (bad < 0) put_merged(b.out, legs, b.nq, b.k, a, c);
+  if (bad < 0) put_merged(b.out, legs, b.nq, b.k, a, c, tot);
   for (Leg& l : legs) release_leg(l);
   return bad < 0 ? 0 : legs_fail(&legs[bad], 1, false);
 }

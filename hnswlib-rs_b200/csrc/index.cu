@@ -858,7 +858,8 @@ static const void* device_view_of_host(const void* p) {
 // synchronisation.  Pageable queries and row pointers are gathered into the context's own pinned staging buffer first
 // (the only host-side copy), which the kernel then reads the same way.
 int Index::search_host_begin(int ci, const void* queries, const void* const* rows, const uint64_t* qids,
-                             const uint64_t* skip, size_t nq, int d, size_t k, size_t ef, const LegPlan& plan) {
+                             const uint64_t* skip, size_t nq, int d, size_t k, size_t ef, const LegPlan& plan,
+                             const float* radius) {
   SearchCtx& c = ctx_[ci];
   cudaStream_t st = c.stream;
   c.pend = SearchCtx::Pending();
@@ -866,20 +867,26 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
   HB_CUDA(cudaSetDevice(device));
   if (!qids && dim != 0 && d != dim) return fail("query length differs from the index dimension");
   int r;
+  // [answers][counts][status, 16 bytes][radius mode: totals]
   const size_t out_bytes = nq * k * sizeof(NeighbourOut), cnt_bytes = nq * sizeof(int32_t);
-  if ((r = ensure_pinned(&c.h_res, &c.h_res_bytes, out_bytes + cnt_bytes + 16, cudaHostAllocMapped | cudaHostAllocPortable))) return r;
+  const size_t rb = radius ? nq * sizeof(float) : 0;  // radii or totals, 4 bytes a row
+  if ((r = ensure_pinned(&c.h_res, &c.h_res_bytes, out_bytes + cnt_bytes + 16 + rb, cudaHostAllocMapped | cudaHostAllocPortable)))
+    return r;
   NeighbourOut* hout = (NeighbourOut*)c.h_res;
   int32_t* hcnt = (int32_t*)((char*)c.h_res + out_bytes);
   int32_t* hstatus = hcnt + nq;
+  uint32_t* htot = radius ? (uint32_t*)((char*)c.h_res + out_bytes + cnt_bytes + 16) : nullptr;
   SearchCtx::Launch& L = c.pend.run;
   c.pend.hout = hout;
   c.pend.hcnt = hcnt;
   c.pend.hstatus = hstatus;
+  c.pend.htot = htot;
   L.nq = nq;
   L.k = k;
   L.ef = ef;
   if (dim == 0) {  // empty index: every answer is empty (hnsw.rs:1498-1500)
     for (size_t i = 0; i < nq; ++i) hcnt[i] = 0;
+    if (htot) std::fill(htot, htot + nq, 0u);
     for (size_t i = 0; i < nq * k; ++i) hout[i] = NeighbourOut{~0ull, __builtin_inff(), INVALID_ID};
     return 0;
   }
@@ -888,14 +895,16 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
   L.out = (NeighbourOut*)dv;
   L.counts = (int32_t*)(dv + out_bytes);
   // by stored point: the ids, and the ids the rows leave out, cross the bus in place of the rows (16 bytes a query at
-  // most); they go after the query staging in the pinned buffer and after an exact launch's rows in device memory
+  // most); they go after the query staging in the pinned buffer and after an exact launch's rows in device memory, and
+  // a radius launch's radii after them (in device memory followed by its totals)
   const size_t qbytes = qids ? 0 : nq * (size_t)dim * es, ib = nq * sizeof(uint64_t);
   const int nid = (qids ? 1 : 0) + (skip && skip != qids ? 1 : 0);
   const void* d_queries = qids || rows ? nullptr : device_view_of_host(queries);  // what the kernel reads
   const size_t staged = qids || d_queries ? 0 : round128(qbytes);
-  if (staged + nid * ib) {
+  if (staged + nid * ib + rb) {
     // gather into pinned staging (rows: one pointer per query, libext.rs parallel_search_neighbours_<ty>)
-    if ((r = ensure_pinned(&c.h_pin, &c.h_pin_bytes, staged + nid * ib, cudaHostAllocMapped | cudaHostAllocPortable))) return r;
+    if ((r = ensure_pinned(&c.h_pin, &c.h_pin_bytes, staged + nid * ib + rb, cudaHostAllocMapped | cudaHostAllocPortable)))
+      return r;
     unsigned char* stage = (unsigned char*)c.h_pin;
     if (rows)
       for (size_t i = 0; i < nq; ++i) memcpy(stage + i * (size_t)dim * es, rows[i], (size_t)dim * es);
@@ -907,18 +916,22 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
     }
     if (qids) memcpy(stage + staged, qids, ib);
     if (skip && skip != qids) memcpy(stage + staged + (qids ? ib : 0), skip, ib);
+    if (radius) memcpy(stage + staged + nid * ib, radius, rb);
   }
   L.d_queries = d_queries;
   // an exact launch may run many CTAs per query (row slices): the queries cross the bus once, into device memory
   const size_t xq = plan.exact ? round128(qbytes) : 0;
-  if (xq + nid * ib) {
-    if ((r = ensure_scratch(&c.d_xq, &c.d_xq_bytes, xq + nid * ib, st))) return r;
+  if (xq + nid * ib + rb) {
+    if ((r = ensure_scratch(&c.d_xq, &c.d_xq_bytes, xq + nid * ib + 2 * rb, st))) return r;
     if (xq) HB_CUDA(cudaMemcpyAsync(c.d_xq, d_queries, qbytes, cudaMemcpyDefault, st));
     if (xq) L.d_queries = c.d_xq;
     const uint64_t* ids = (const uint64_t*)((char*)c.d_xq + xq);
-    if (nid) HB_CUDA(cudaMemcpyAsync((void*)ids, (char*)c.h_pin + staged, nid * ib, cudaMemcpyHostToDevice, st));
+    if (nid * ib + rb)
+      HB_CUDA(cudaMemcpyAsync((void*)ids, (char*)c.h_pin + staged, nid * ib + rb, cudaMemcpyHostToDevice, st));
     L.q_ids = qids ? ids : nullptr;
     L.skip = !skip ? nullptr : skip == qids ? ids : ids + (qids ? nq : 0);
+    L.radius = radius ? (const float*)(ids + nid * nq) : nullptr;
+    L.totals = radius ? (uint32_t*)(ids + nid * nq) + nq : nullptr;
   }
   if (plan.exact) *hstatus = 0;
   // one enqueue (the plan's uploads, the launches, the status); search_host_finish synchronises once and takes the slow
@@ -926,15 +939,17 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
   c.pend.enqueued = true;
   if ((r = stage_plan(c, plan, L)) || (r = run_plan(c, L, false, nullptr))) return r;
   if (!plan.exact) HB_CUDA(cudaMemcpyAsync(hstatus, c.d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (radius) HB_CUDA(cudaMemcpyAsync(htot, L.totals, rb, cudaMemcpyDeviceToHost, st));
   return 0;
 }
 
-int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** counts) {
+int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** counts, const uint32_t** totals) {
   SearchCtx& c = ctx_[ci];
   cudaStream_t st = c.stream;
   SearchCtx::Pending& p = c.pend;
   *out = p.hout;
   *counts = p.hcnt;
+  if (totals) *totals = p.htot;
   if (!p.enqueued) return 0;  // empty batch or empty index: the answers (if any) were filled by search_host_begin
   HB_CUDA(cudaSetDevice(device));
   HB_CUDA(cudaStreamSynchronize(st));
@@ -1025,7 +1040,9 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
 }
 
 int Index::run_plan(SearchCtx& c, const SearchCtx::Launch& L, bool sync, float* kernel_ms) {
-  if (L.exact) return exact_on_ctx(c, L.d_queries, L.nq, L.k, L.groups, L.out, L.counts, sync, kernel_ms, L.q_ids, L.skip);
+  if (L.exact)
+    return exact_on_ctx(c, L.d_queries, L.nq, L.k, L.groups, L.out, L.counts, sync, kernel_ms, L.q_ids, L.skip, L.radius,
+                        L.totals);
   int r;
   if (L.plain && (r = search_on_ctx(c, L.d_queries, L.plain, L.k, L.ef, LaunchFilter(), L.out, L.counts, sync, kernel_ms,
                                     L.q_ids, L.skip)))

@@ -204,7 +204,7 @@ class WorkerGroup {
 // ---- host searches (host_search.cu)
 // Where a host search writes its [nq][k] answer slots and counts[nq]: either the reference entry points' answer blocks
 // (`nb`: Neighbour_api with the internal id in its tail padding) or hnsw_b200_search_flat's arrays (internal and pid
-// optional).
+// optional).  A radius batch also writes each row's total, the number of its points within its radius (optional).
 struct AnswerArrays {
   NeighbourOut* nb = nullptr;
   uint64_t* ids = nullptr;
@@ -213,6 +213,7 @@ struct AnswerArrays {
   int32_t* pid = nullptr;
   int32_t* counts = nullptr;
   const size_t* perm = nullptr;  // row j of the batch is written to row perm[j] (nullptr: to row j)
+  uint64_t* total = nullptr;
 };
 
 // What the rows of a batch may return: every point (NONE); the points a FilterT admits (FILTER_T: `mode` 1 sorted
@@ -247,7 +248,8 @@ struct LabelSets {
 // One host search batch: flat queries or one pointer per query (rows), k answers each into `out`.  `exact`: the exact
 // scan of the points each row may return (ef unused) instead of the graph search.  By stored point: query i is the
 // stored vector of qids[i] (an insertion rank; a partitioned handle's global one), and with exclude_self its row leaves
-// that point out (write_row, search_core.cuh).
+// that point out (write_row, search_core.cuh).  Radius (an exact batch): row i holds only the points within radius[i]
+// (>= 0, not NaN) and reports how many of its points are (out.total).
 struct HostBatch {
   const void* queries = nullptr;
   const void* const* rows = nullptr;
@@ -259,6 +261,7 @@ struct HostBatch {
   bool exact = false;
   const uint64_t* qids = nullptr;
   bool exclude_self = false;
+  const float* radius = nullptr;
 };
 
 // A leg's restriction (Index::resolve): its rows [0, plain) are unrestricted, and `runs` cover the rest, each a range of
@@ -337,10 +340,11 @@ class Index {
   // host queries (flat or row pointers) on leased context c under the leg's plan, answers left in the context's pinned
   // buffer (valid until it is released)
   // By stored point (qids, insertion ranks of this Index, instead of queries and rows), and with skip[i] the id row i
-  // leaves out (~0: none; skip may be qids itself).
+  // leaves out (~0: none; skip may be qids itself).  An exact plan with radii: row i within radius[i], and its count of
+  // points within the radius left in the pinned buffer next to the counts.
   int search_host_begin(int c, const void* queries, const void* const* rows, const uint64_t* qids, const uint64_t* skip,
-                        size_t nq, int d, size_t k, size_t ef, const LegPlan& plan);
-  int search_host_finish(int c, const NeighbourOut** out, const int32_t** counts);
+                        size_t nq, int d, size_t k, size_t ef, const LegPlan& plan, const float* radius = nullptr);
+  int search_host_finish(int c, const NeighbourOut** out, const int32_t** counts, const uint32_t** totals = nullptr);
   // host search batches (host_search.cu): synchronous, or submitted now and collected by finish_batch.  A ticket is a
   // batch planned into legs, with what the legs read until they are collected: a per-row batch's caller row of each
   // sorted row (out.perm) and its sorted rows, a FilterT's host bits per partition, and a label-set batch's sets.
@@ -351,6 +355,7 @@ class Index {
     std::vector<size_t> perm;
     std::vector<const void*> rows;
     std::vector<uint64_t> qids;  // a per-row batch by stored point: the ids in sorted-row order
+    std::vector<float> radius;   // a per-row radius batch: the radii in sorted-row order
     std::vector<unsigned char> gathered;  // a partitioned batch by stored point: the query rows read from their partitions
     std::vector<std::vector<uint32_t>> bits;
     LabelSets sets;
@@ -497,11 +502,14 @@ class Index {
       std::vector<ExactGroup> groups;
       const uint64_t* q_ids = nullptr;  // a search by stored point: in place of d_queries
       const uint64_t* skip = nullptr;   // per row the id it leaves out: the launches search k + 1
+      const float* radius = nullptr;    // exact, radius mode: per row its radius, and where its total goes
+      uint32_t* totals = nullptr;
     };
     struct Pending {  // a host search enqueued by search_host_begin, completed by search_host_finish
       Launch run;
       NeighbourOut* hout = nullptr;
       int32_t *hcnt = nullptr, *hstatus = nullptr;
+      uint32_t* htot = nullptr;  // radius mode
       bool enqueued = false;
     } pend;
   };
@@ -635,10 +643,11 @@ class Index {
                     NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* q_ids,
                     const uint64_t* skip);
   // the exact k nearest of device queries, each group's rows among that group's points (aux.cu); the slices' scratch is
-  // sized before the launch.  q_ids and skip as search_on_ctx takes them.
+  // sized before the launch.  q_ids and skip as search_on_ctx takes them.  Radius mode (radius, device, per row): only
+  // the points within each row's radius, and their number per row into the device array totals.
   int exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const std::vector<ExactGroup>& groups,
                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* q_ids,
-                   const uint64_t* skip);
+                   const uint64_t* skip, const float* radius = nullptr, uint32_t* totals = nullptr);
   // the device view of a leg's plan in `run`, with what it needs uploaded into context c
   int stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& run);
   // the launches of `run` on context c: the unrestricted rows as an ordinary unfiltered launch, then the restricted ones

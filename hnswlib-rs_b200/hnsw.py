@@ -118,6 +118,8 @@ def load_library():
     L.hnsw_b200_search_flat_by_id.argtypes = [vp, vp, u64, u64, u64, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_exact_by_id.argtypes = [vp, vp, u64, u64, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_device_by_id.argtypes = [vp, i32, i64, vp, u64, u64, u64, i32, vp, vp, i32, vp]
+    L.hnsw_b200_search_exact_radius.argtypes = [vp, i64, vp, vp, vp, vp, u64, u64, vp, u64, vp, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_exact_radius_by_id.argtypes = [vp, vp, u64, vp, u64, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.hnsw_b200_get_stats.argtypes = [vp, vp, i32]
     L.hnsw_b200_set_stream.argtypes = [vp, vp]
     L.hnsw_b200_join.argtypes = [vp]
@@ -691,6 +693,76 @@ class Hnsw:
                 _, d, it, _, _ = self.search_by_id(q, k, k if ef is None else ef, exclude_self=True, with_pid=False)
             ids[s:s + q.size], ds[s:s + q.size] = it, d
         return ids, ds
+
+    # ---- radius search (include/hnsw_b200.h "Radius search")
+    def _radius(self, fn, lead, nq, radius, knbn, filter, sets, ranges, with_internal, with_pid):
+        r = np.ascontiguousarray(np.broadcast_to(np.asarray(radius, np.float32), (nq,)))
+        rg = None if ranges is None else _ranges(ranges, nq)
+        off, vals = (None, None) if sets is None else _label_sets(sets, nq)
+        knbn = int(knbn)
+        ans = self._answers(nq, knbn, with_internal, with_pid)
+        totals = np.empty(nq, np.uint64)
+        restriction = (_filter_id(filter), _p(rg), _p(off), _p(vals))
+        self._chk(fn(self._h, *lead(restriction, _p(r)), *map(_p, ans), _p(totals)))
+        return ans + (totals,)
+
+    def search_exact_radius(self, queries, radius, knbn, filter=None, sets=None, ranges=None, with_internal=True,
+                            with_pid=True):
+        """hnsw_b200_search_exact_radius: the points within radius of each query (a scalar or one value per query),
+        under the restriction search_exact_by_id takes (filter: a ResidentFilter; sets; ranges, optionally with sets).
+        Row i is search_exact's row of knbn for query i cut after its last entry within radius[i].  knbn = 0 counts
+        only.  Returns search_exact's (origin, dist, internal | None, pid | None, counts) and totals u64[nq], the number
+        of admitted points within each radius."""
+        q = np.ascontiguousarray(queries, self.dtype)
+        nq, d = q.shape
+        return self._radius(self._L.hnsw_b200_search_exact_radius,
+                            lambda rs, r: rs + (_p(q), nq, d, r, int(knbn)),
+                            nq, radius, knbn, filter, sets, ranges, with_internal, with_pid)
+
+    def search_exact_radius_by_id(self, qids, radius, knbn, exclude_self=False, filter=None, sets=None, ranges=None,
+                                  with_internal=True, with_pid=True):
+        """hnsw_b200_search_exact_radius_by_id: search_exact_radius with query i the stored point qids[i] (an insertion
+        rank).  exclude_self: search_exact_by_id's exclude_self row cut at the radius, and a total without the point
+        itself.  Returns search_exact_radius's tuple."""
+        ids = np.ascontiguousarray(qids, np.uint64).reshape(-1)
+        nq = ids.size
+        return self._radius(self._L.hnsw_b200_search_exact_radius_by_id,
+                            lambda rs, r: (_p(ids), nq, r, int(knbn), int(bool(exclude_self))) + rs,
+                            nq, radius, knbn, filter, sets, ranges, with_internal, with_pid)
+
+    def radius_graph(self, radius, knbn=64, batch=65536):
+        """every stored point's complete list of the other points within radius, by insertion rank, as CSR
+        (offsets u64[n + 1], internal ids u32[], distances f32[]), each list in (distance, id) order.  One
+        search_exact_radius_by_id pass with exclude_self per batch of `batch` points at knbn, then the rows whose total
+        exceeded knbn again with knbn set to their largest total.  A total beyond the exact kernel's limit raises
+        HnswError naming the point; a list is never returned truncated."""
+        n = self.get_nb_point()
+        counts = np.zeros(n, np.uint64)
+        ids, ds = [None] * n, [None] * n
+        knbn = int(knbn)
+        for s in range(0, n, int(batch)):
+            q = np.arange(s, min(n, s + int(batch)), dtype=np.uint64)
+            _, d, it, _, c, tot = self.search_exact_radius_by_id(q, radius, knbn, exclude_self=True, with_pid=False)
+            for j in range(q.size):
+                ids[s + j], ds[s + j] = it[j, :c[j]], d[j, :c[j]]
+            counts[s:s + q.size] = tot
+            over = np.flatnonzero(tot > np.uint64(knbn))
+            if over.size:
+                want = int(tot[over].max())
+                try:
+                    _, d2, it2, _, c2, tot2 = self.search_exact_radius_by_id(q[over], radius, want, exclude_self=True,
+                                                                             with_pid=False)
+                except HnswError as e:
+                    j = int(over[np.argmax(tot[over])])
+                    raise HnswError(f"radius_graph: point {s + j} has {int(tot[j])} points within the radius, beyond "
+                                    f"the exact search's limit: {e}") from None
+                assert np.array_equal(c2.astype(np.uint64), tot2)
+                for m, j in enumerate(over):
+                    ids[s + j], ds[s + j] = it2[m, :c2[m]], d2[m, :c2[m]]
+        off = np.zeros(n + 1, np.uint64)
+        np.cumsum(counts, out=off[1:])
+        cat = lambda parts, dt: np.concatenate(parts).astype(dt, copy=False) if n else np.empty(0, dt)
+        return off, cat(ids, np.uint32), cat(ds, np.float32)
 
     def make_filter(self, filter):
         """hnsw_b200_filter_new: materialise a FilterT (sorted id sequence or callable(id)->bool, as search_flat takes)

@@ -122,6 +122,15 @@ extern "C" {
     fn hnsw_b200_search_device_by_id(h: *const HnswApif32, exact: c_int, filter: i64, d_qids: *const u64, nq: u64,
                                      knbn: u64, ef: u64, exclude_self: c_int, d_out: *mut c_void, d_counts: *mut i32,
                                      sync: c_int, kernel_ms: *mut f32) -> c_int;
+    fn hnsw_b200_search_exact_radius(h: *const HnswApif32, filter: i64, qrange: *const i64, qset_off: *const u64,
+                                     qset: *const u32, queries: *const c_void, nq: u64, dim: u64, radius: *const f32,
+                                     knbn: u64, out_ids: *mut u64, out_dist: *mut f32, out_internal: *mut u32,
+                                     out_pid: *mut i32, out_counts: *mut i32, out_total: *mut u64) -> c_int;
+    fn hnsw_b200_search_exact_radius_by_id(h: *const HnswApif32, qids: *const u64, nq: u64, radius: *const f32,
+                                           knbn: u64, exclude_self: c_int, filter: i64, qrange: *const i64,
+                                           qset_off: *const u64, qset: *const u32, out_ids: *mut u64,
+                                           out_dist: *mut f32, out_internal: *mut u32, out_pid: *mut i32,
+                                           out_counts: *mut i32, out_total: *mut u64) -> c_int;
 }
 
 /// The attribute of a point that has none (include/hnsw_b200.h HNSW_B200_ATTR_NONE): no range admits it.

@@ -350,6 +350,42 @@ int hnsw_b200_search_exact(const void* h, int64_t filter, const void* queries, u
 int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                   void* d_out, int32_t* d_counts, int sync, float* kernel_ms);
 
+/* ---- Radius search: every admitted point within each query's own distance, counted in the exact scan (threshold
+ * retrieval, near-duplicates, the epsilon-neighbourhoods of density clustering).
+ *   Restriction: as hnsw_b200_search_exact_by_id reads it: none (filter = -1, qrange, qset_off and qset NULL), one
+ *     resident filter, label sets, or ranges with optional sets.  Call row i's admitted points A_i.
+ *   Rows: W_i is the points of A_i whose distance to query i is <= radius[i], that distance being the one
+ *     hnsw_b200_dist_batch reports for the pair, bit for bit.  Row i holds the first min(knbn, |W_i|) points of W_i by
+ *     (distance, internal id): the row search_exact / _label_sets / _ranges (same restriction, same knbn) returns for
+ *     query i, cut after its last entry within radius[i], bit for bit (ids, distance bits, internal ids, PointIds,
+ *     count).  Slots past the count are padded as in every exact call.
+ *   Totals: out_total[i] = |W_i|, also when the row was cut at knbn (a row is complete exactly when its count equals
+ *     its total).  out_total may be NULL.
+ *   knbn = 0 counts only: no slot is written, out_ids, out_dist, out_internal and out_pid may be NULL, every count is 0
+ *     and the totals are filled.
+ *   By stored point (_by_id): query i is the stored vector of qids[i], as for search_exact_by_id.  With exclude_self,
+ *     row i is that call's exclude_self row cut at the radius, and the total leaves qids[i] out; other points with an
+ *     identical vector stay in both.
+ *   Radii: radius[i] = +inf admits every point of A_i; -0 is read as 0.  A NaN or negative radius[i] refuses the whole
+ *     call, naming i, before anything runs; radius NULL with nq > 0 is refused; nq == 0 returns 0.
+ *   Checks, before anything runs: those of search_exact_by_id with its wording (a NULL handle, qids NULL, qids out of
+ *     range, a filter together with sets or ranges, stale, foreign or unknown filters, bad set offsets), and knbn (with
+ *     exclude_self knbn + 1) beyond search_exact's limit at this dimension, refused with its message.  A refused call
+ *     leaves the outputs untouched.
+ *   Ignored: the tie mode and statistics, as for every exact call.  There is no device variant.
+ *   Handles: a partitioned handle merges the partitions' rows by the partitioned rule (distance, then partition, then
+ *     position), reports global ranks and sums the partitions' totals; a replicated handle shards the batch like
+ *     search_exact; a partition view uses its local ids.  The handle is taken shared. */
+int hnsw_b200_search_exact_radius(const void* h, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                                  const uint32_t* qset, const void* queries, uint64_t nq, uint64_t dim,
+                                  const float* radius, uint64_t knbn, uint64_t* out_ids, float* out_dist,
+                                  uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts, uint64_t* out_total);
+int hnsw_b200_search_exact_radius_by_id(const void* h, const uint64_t* qids, uint64_t nq, const float* radius,
+                                        uint64_t knbn, int exclude_self, int64_t filter, const int64_t* qrange,
+                                        const uint64_t* qset_off, const uint32_t* qset, uint64_t* out_ids,
+                                        float* out_dist, uint32_t* out_internal, int32_t* out_pid,
+                                        int32_t* out_counts, uint64_t* out_total);
+
 /* ---- A filter per query: one batch whose query i uses resident filter filters[i] of h, or no filter (-1).  A batch
  * that mixes tenants, users or categories runs as one call (one launch per leg for the filtered rows) instead of one
  * call per distinct filter.
