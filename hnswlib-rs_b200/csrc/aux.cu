@@ -295,40 +295,33 @@ static bool exact_shape(int d4, size_t k, size_t nq, ExactParams& p, size_t& sme
   return false;
 }
 
-int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const std::vector<ExactGroup>& groups,
-                        NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* q_ids,
-                        const uint64_t* skip, const float* radius, uint32_t* totals) {
-  if (k == 0) return fail("knbn must be positive");
-  if (poisoned_) return fail(poison_msg_);
+int Index::exact_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, size_t k,
+                        const std::vector<ExactGroup>& groups, bool sync, float* kernel_ms) {
   cudaStream_t st = c.stream;
-  if (radius) HB_CUDA(cudaMemsetAsync(totals, 0, nq * sizeof(uint32_t), st));
-  if (dim == 0) {  // empty index: every answer is empty
-    HB_CUDA(cudaMemsetAsync(d_counts, 0, nq * sizeof(int32_t), st));
-    if (sync) HB_CUDA(cudaStreamSynchronize(st));
-    return 0;
-  }
   // one group over every row: equal tiles over its points, taken from blockIdx (no tile table); else a tile table
   const bool tiled = !(groups.size() == 1 && groups[0].first == 0 && groups[0].count == nq);
   const ExactScan scan = tiled ? ExactScan() : groups[0].scan;
   ExactParams p{};
   p.g = view();
-  p.queries = d_queries;
+  p.queries = rows.d_queries;
   p.q_bytes = dim * es;
   p.nq = (uint32_t)nq;
   p.list = scan.ids;
   p.npts = (uint32_t)(scan.ids ? scan.n : n);
-  p.q_ids = q_ids;
-  p.skip_ids = skip;
-  p.radius = radius;
-  p.totals = totals;
-  k += skip ? 1 : 0;  // the scan keeps k + 1 keys, each row is k wide (write_row)
+  p.q_ids = rows.q_ids;
+  p.skip_ids = rows.skip;
+  p.radius = rows.radius;
+  p.totals = rows.totals;
+  p.out = rows.out;
+  p.counts = rows.counts;
+  k += rows.skip ? 1 : 0;  // the scan keeps k + 1 keys, each row is k wide (write_row)
   p.k = (int)k;
   size_t widest_group = 0;
   for (const ExactGroup& gr : groups) widest_group = std::max(widest_group, gr.count);
   size_t smem = 0;
   if (!exact_shape(p.g.d4, k, widest_group, p, smem))
-    return fail(skip ? "k + 1 / dimension too large for the exact search kernel (exclude_self searches k + 1)"
-                     : "k / dimension too large for the exact search kernel");
+    return fail(rows.skip ? "k + 1 / dimension too large for the exact search kernel (exclude_self searches k + 1)"
+                          : "k / dimension too large for the exact search kernel");
   auto launch = [&](int grid, int* blocks_per_sm) {
     return dispatch_op(metric, dtype, [&](auto tag) -> cudaError_t {
       return launch_exact_for_op<typename decltype(tag)::type>(p, grid, smem, st, blocks_per_sm);
@@ -390,8 +383,6 @@ int Index::exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k
     p.part = (uint64_t*)((char*)c.d_xpart + tile_bytes + tick_bytes);
     HB_CUDA(cudaMemsetAsync(p.tickets, 0, tiles * 4, st));
   }
-  p.out = d_out;
-  p.counts = d_counts;
   HB_CUDA(cudaEventRecord(c.ev0, st));
   HB_CUDA(launch((int)(tiles * p.slices), nullptr));
   HB_CUDA(cudaEventRecord(c.ev1, st));
@@ -437,16 +428,8 @@ int Index::bruteforce(const void* queries, size_t nq, int d, size_t k, uint32_t*
   if (nq == 0 || k == 0) return 0;
   if (d != dim) return fail("query length differs from the index dimension");
   std::vector<int32_t> counts(nq);
-  HostBatch b;
-  b.queries = queries;
-  b.nq = nq;
-  b.d = d;
-  b.k = k;
-  b.exact = true;
-  b.out.internal = out_ids;
-  b.out.dist = out_dist;
-  b.out.counts = counts.data();
-  return search_batch(b);
+  return search_batch(
+      {{queries}, nq, d, k, 0, Restriction(), true, {nullptr, nullptr, out_dist, out_ids, nullptr, counts.data()}});
 }
 
 }  // namespace hb

@@ -165,7 +165,7 @@ static const Neighbourhood_api* search_any(const void* hv, size_t len, const voi
   Neighbour_api* nb = (Neighbour_api*)malloc(sizeof(Neighbour_api) * knbn);
   int32_t cnt = 0;
   const AnswerArrays ans{(NeighbourOut*)nb, nullptr, nullptr, nullptr, nullptr, &cnt};
-  if (pass(h->ix, h->ix->search_batch(HostBatch{data, nullptr, 1, (int)len, knbn, ef_search, Restriction(), ans}))) {
+  if (pass(h->ix, h->ix->search_batch(HostBatch{{data}, 1, (int)len, knbn, ef_search, Restriction(), false, ans}))) {
     free(nb);
     return nullptr;
   }
@@ -196,7 +196,7 @@ static const Vec_api_Neighbourhood_api* parallel_search_any(const void* hv, size
   std::vector<int32_t> cnt(nb_vec);
   const AnswerArrays out{(NeighbourOut*)box->block, nullptr, nullptr, nullptr, nullptr, cnt.data()};
   // with replicas, every device answers its slice of the batch in place
-  if (pass(h->ix, h->ix->search_batch(HostBatch{nullptr, data, nb_vec, (int)vec_len, knbn, ef_search, Restriction(), out}))) {
+  if (pass(h->ix, h->ix->search_batch(HostBatch{{nullptr, data}, nb_vec, (int)vec_len, knbn, ef_search, Restriction(), false, out}))) {
     free(box->hoods);
     free(box->block);
     free(box);
@@ -616,48 +616,37 @@ int hnsw_b200_insert_flat(void* h, const void* vecs, uint64_t n, uint64_t dim, c
 }
 
 // ---- searches.  Every search entry point below is one call of search_call, which takes the handle's lock shared (and
-// every partition's), checks the arguments and runs the batch:
-//   * HOST: host queries in, host answers out (`out`), through the host batch driver; a partitioned handle searches
-//     every partition;
+// every partition's), checks the arguments and runs the batch b:
+//   * HOST: host rows in, host answers out, through the host batch driver; a partitioned handle searches every partition;
 //   * SUBMIT: the same, split in two (hnsw_b200_search_flat_wait collects it), so that one host thread keeps several
 //     batches in flight.  With replicas (hnsw_b200_replicate) every device gets its contiguous share enqueued at submit
 //     time.  Refused on a partitioned handle;
-//   * DEVICE: device queries in, device answers out (out.nb, out.counts), `sync` and `kernel_ms` as
-//     hnsw_b200_search_device takes them.  Refused on a partitioned handle.
-// `name` is the entry point a refusal on a partitioned handle names.  `rs` is what each query may return, `exact` the
-// exact scan of those points instead of the graph search (ef unused).
+//   * DEVICE: device rows in, device answers out (b.out.nb, b.out.counts), `sync` and `kernel_ms` as
+//     hnsw_b200_search_device takes them (the other two ignore them).  Refused on a partitioned handle.
+// `name` is the entry point a refusal on a partitioned handle names.  By stored point (b.in.qids, non-NULL) the queries
+// are the stored vectors of qids[0, nq), each below nb_point, in the handle's dimension; radii (b.in.radius, an exact
+// HOST call) are checked by the caller.
 enum Via { HOST, SUBMIT, DEVICE };
-// By stored point (qids, checked by the caller to be non-NULL): the queries are the stored vectors of qids[0, nq), each
-// below the handle's nb_point, and `dim` is the handle's; exclude_self: each row leaves its own point out.  Radius (an
-// exact HOST call, checked by the caller): row i holds only the points within radius[i], and out.total their number.
-static int64_t search_call(const void* h, Via via, const char* name, const Restriction& rs, bool exact, const void* queries,
-                           uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef, const AnswerArrays& out, int sync = 1,
-                           float* kernel_ms = nullptr, const uint64_t* qids = nullptr, bool exclude_self = false,
-                           const float* radius = nullptr) {
+static int64_t search_call(const void* h, Via via, const char* name, HostBatch b, int sync, float* kernel_ms) {
   HB_HS(h);
   if (via != HOST) HB_NOT_PARTITIONED(ix, name);
-  if (via == DEVICE)
-    return pass(ix, ix->search_device(rs, exact, queries, nq, knbn, ef, out.nb, out.counts, sync != 0, kernel_ms, qids,
-                                      exclude_self));
-  if (via == HOST && nq == 0) return 0;
+  if (via == DEVICE) return pass(ix, ix->search_device(b, sync != 0, kernel_ms));
+  if (via == HOST && b.nq == 0) return 0;
   HB_PARTS_SHARED_IF(ix);
-  if (qids) {
+  if (const uint64_t* qids = b.in.qids) {
     const uint64_t have = nb_point(ix);
-    for (uint64_t i = 0; i < nq; ++i)
+    for (uint64_t i = 0; i < b.nq; ++i)
       if (qids[i] >= have)
         return set_err(std::string(name) + ": qids[" + std::to_string(i) + "] = " + std::to_string(qids[i]) +
                        " is not below nb_point = " + std::to_string(have));
-    dim = (uint64_t)ix->dim;
+    b.d = ix->dim;
   }
+  const Restriction& rs = b.restriction;
   if (rs.kind == Restriction::ROW_FILTERS && !rs.filters) return set_err("filters is NULL");
   if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset_off) return set_err("qset_off is NULL");
   if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset) return set_err("qset is NULL");
-  if (!(queries || qids) || !out.ids || !out.dist || !out.counts || knbn == 0 || nq == 0) return set_err("bad argument");
-  HostBatch b{queries, nullptr, nq, (int)dim, knbn, ef, rs, out};
-  b.exact = exact;
-  b.qids = qids;
-  b.exclude_self = exclude_self;
-  b.radius = radius;
+  if (!(b.in.queries || b.in.qids) || !b.out.ids || !b.out.dist || !b.out.counts || b.k == 0 || b.nq == 0)
+    return set_err("bad argument");
   if (via == HOST) return pass(ix, ix->search_batch(b));
   const int64_t t = ix->submit_batch(b);
   if (t < 0) g_err = ix->err();
@@ -685,27 +674,28 @@ int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint6
                           uint64_t ef_search, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,
                           hnsw_b200_filter_fn fn, void* ctx, uint64_t* out_ids, float* out_dist,
                           uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_flat", filter_t(filter_mode, filter_ids, nfilter, fn, ctx), false, queries, nq,
-                          dim, knbn, ef_search, columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return (int)search_call(h, HOST, "search_flat",
+                          {{queries}, nq, (int)dim, knbn, ef_search, filter_t(filter_mode, filter_ids, nfilter, fn, ctx),
+                           false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
 }
 int hnsw_b200_search_flat_filtered(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim,
                                    uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                    uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_flat_filtered", resident(filter), false, queries, nq, dim, knbn, ef_search,
-                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return (int)search_call(h, HOST, "search_flat_filtered", {{queries}, nq, (int)dim, knbn, ef_search, resident(filter),
+                          false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
 }
 
 int64_t hnsw_b200_search_flat_submit(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
                                      uint64_t ef_search, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                      int32_t* out_pid, int32_t* out_counts) {
-  return search_call(h, SUBMIT, "search_flat_submit", Restriction(), false, queries, nq, dim, knbn, ef_search,
-                     columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return search_call(h, SUBMIT, "search_flat_submit", {{queries}, nq, (int)dim, knbn, ef_search, Restriction(), false,
+                     columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
 }
 int64_t hnsw_b200_search_flat_submit_filtered(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim,
                                               uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                               uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return search_call(h, SUBMIT, "search_flat_submit_filtered", resident(filter), false, queries, nq, dim, knbn, ef_search,
-                     columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return search_call(h, SUBMIT, "search_flat_submit_filtered", {{queries}, nq, (int)dim, knbn, ef_search,
+                     resident(filter), false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
 }
 
 int hnsw_b200_search_flat_wait(const void* h, int64_t ticket) {
@@ -721,21 +711,21 @@ int hnsw_b200_search_flat_wait(const void* h, int64_t ticket) {
 
 int hnsw_b200_search_device(const void* h, const void* d_queries, uint64_t nq, uint64_t knbn,
                             uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
-  return (int)search_call(h, DEVICE, "search_device", Restriction(), false, d_queries, nq, 0, knbn, ef_search,
-                          on_device(d_out, d_counts), sync, kernel_ms);
+  return (int)search_call(h, DEVICE, "search_device", {{d_queries}, nq, 0, knbn, ef_search, Restriction(), false,
+                          on_device(d_out, d_counts)}, sync, kernel_ms);
 }
 int hnsw_b200_search_device_filtered(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                      uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
-  return (int)search_call(h, DEVICE, "search_device_filtered", resident(filter), false, d_queries, nq, 0, knbn, ef_search,
-                          on_device(d_out, d_counts), sync, kernel_ms);
+  return (int)search_call(h, DEVICE, "search_device_filtered", {{d_queries}, nq, 0, knbn, ef_search, resident(filter),
+                          false, on_device(d_out, d_counts)}, sync, kernel_ms);
 }
 
 // Exact search: the exact scan of the points a resident filter admits (filter >= 0) or of every point (-1), through the
 // same batch driver and device-resident path as the graph searches
 int hnsw_b200_search_exact(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
                            uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_exact", resident_or_all(filter), true, queries, nq, dim, knbn, 0,
-                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return (int)search_call(h, HOST, "search_exact", {{queries}, nq, (int)dim, knbn, 0, resident_or_all(filter), true,
+                          columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
 }
 
 // A filter per query: filters[i] is a resident filter of the handle or -1; the graph search (ef_search) or the exact
@@ -743,14 +733,15 @@ int hnsw_b200_search_exact(const void* h, int64_t filter, const void* queries, u
 int hnsw_b200_search_flat_per_query(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim,
                                     uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                     uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_flat_per_query", row_filters(filters), false, queries, nq, dim, knbn, ef_search,
-                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return (int)search_call(h, HOST, "search_flat_per_query", {{queries}, nq, (int)dim, knbn, ef_search,
+                          row_filters(filters), false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1,
+                          nullptr);
 }
 int hnsw_b200_search_exact_per_query(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim,
                                      uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                      int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_exact_per_query", row_filters(filters), true, queries, nq, dim, knbn, 0,
-                          columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return (int)search_call(h, HOST, "search_exact_per_query", {{queries}, nq, (int)dim, knbn, 0, row_filters(filters),
+                          true, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
 }
 
 // Point labels (and attributes).  On a partitioned handle point g (its insertion rank) is local point g / P of partition
@@ -829,14 +820,40 @@ int hnsw_b200_get_attributes(const void* h, uint64_t first, uint64_t n, int64_t*
                        [](const Index* x, size_t p) { return hb::attr_unbias(x->attrs.host[p]); });
 }
 
+// Label sets of one label per query, for the calls that give no offsets: query i's set is {labels[i]}, or {LABEL_NONE}
+// (any label) when labels is NULL; the offsets 0, 1, ..., nq, and the nq LABEL_NONE values, are kept here
+struct OneLabelSets {
+  std::vector<uint64_t> off;
+  std::vector<uint32_t> none;
+  Restriction rows(uint64_t nq, const uint32_t* labels, const int64_t* qrange) {
+    off.resize(nq + 1);
+    std::iota(off.begin(), off.end(), (uint64_t)0);
+    if (!labels) none.assign(nq, hb::LABEL_NONE);
+    return row_label_sets(off.data(), labels ? labels : none.data(), qrange);
+  }
+};
+
+// The restriction of a call that takes sets and ranges (-1 and no sets or ranges: none), refused when a resident filter
+// comes with sets or ranges; a range without sets is a range within {LABEL_NONE} per query (made in `one`), and sets
+// without ranges are the label-sets call's
+static int one_restriction(const char* name, uint64_t nq, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                           const uint32_t* qset, OneLabelSets& one, Restriction& rs) {
+  const bool rows = qrange || qset_off || qset;
+  if (filter != -1 && rows)
+    return set_err(std::string(name) + ": a resident filter cannot be combined with label sets or ranges");
+  rs = !rows ? resident_or_all(filter)
+             : qset_off || qset ? row_label_sets(qset_off, qset, qrange) : one.rows(nq, nullptr, qrange);
+  return 0;
+}
+
 // A label per query: labels[i] is the label query i is restricted to, or LABEL_NONE for none; the graph search
-// (ef_search) or the exact scan.  Query i's label set is {qlabels[i]}: offsets 0, 1, ..., nq over qlabels itself.
+// (ef_search) or the exact scan.  Query i's label set is {qlabels[i]}.
 static int labeled_call(const void* h, const char* name, const uint32_t* qlabels, bool exact, const void* queries,
                         uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef, const AnswerArrays& out) {
   if (h && nq && !qlabels) return set_err("qlabels is NULL");  // search_call answers a NULL handle and nq == 0 first
-  std::vector<uint64_t> off(nq + 1);
-  std::iota(off.begin(), off.end(), (uint64_t)0);
-  return (int)search_call(h, HOST, name, row_label_sets(off.data(), qlabels), exact, queries, nq, dim, knbn, ef, out);
+  OneLabelSets one;
+  return (int)search_call(h, HOST, name, {{queries}, nq, (int)dim, knbn, ef, one.rows(nq, qlabels, nullptr), exact, out}, 1,
+                          nullptr);
 }
 int hnsw_b200_search_flat_labeled(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim,
                                   uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
@@ -856,34 +873,30 @@ int hnsw_b200_search_exact_labeled(const void* h, const uint32_t* qlabels, const
 int hnsw_b200_search_flat_label_sets(const void* h, const uint64_t* qset_off, const uint32_t* qset, const void* queries,
                                      uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search, uint64_t* out_ids,
                                      float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_flat_label_sets", row_label_sets(qset_off, qset), false, queries, nq, dim, knbn,
-                          ef_search, columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return (int)search_call(h, HOST, "search_flat_label_sets", {{queries}, nq, (int)dim, knbn, ef_search,
+                          row_label_sets(qset_off, qset), false, columns(out_ids, out_dist, out_internal, out_pid,
+                          out_counts)}, 1, nullptr);
 }
 int hnsw_b200_search_exact_label_sets(const void* h, const uint64_t* qset_off, const uint32_t* qset, const void* queries,
                                       uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids, float* out_dist,
                                       uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_exact_label_sets", row_label_sets(qset_off, qset), true, queries, nq, dim, knbn,
-                          0, columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return (int)search_call(h, HOST, "search_exact_label_sets", {{queries}, nq, (int)dim, knbn, 0,
+                          row_label_sets(qset_off, qset), true, columns(out_ids, out_dist, out_internal, out_pid,
+                          out_counts)}, 1, nullptr);
 }
 
 // Attribute ranges.  Query i is restricted to the points whose attribute is in [qrange[2i], qrange[2i + 1]]
 // ([INT64_MIN, INT64_MAX]: every point, also those without one) and whose label is one of qset[qset_off[i],
-// qset_off[i + 1]) ({LABEL_NONE}: any; qset_off and qset both NULL: {LABEL_NONE} for every query, passed as offsets 0,
-// 1, ..., nq over nq LABEL_NONE values); the graph search (ef_search) or the exact scan.
+// qset_off[i + 1]) ({LABEL_NONE}: any; qset_off and qset both NULL: {LABEL_NONE} for every query); the graph search
+// (ef_search) or the exact scan.
 static int ranged_call(const void* h, const char* name, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
                        bool exact, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef,
                        const AnswerArrays& out) {
   if (h && nq && !qrange) return set_err("qrange is NULL");  // search_call answers a NULL handle and nq == 0 first
-  std::vector<uint64_t> off;
-  std::vector<uint32_t> none;
-  if (!qset_off && !qset) {
-    off.resize(nq + 1);
-    std::iota(off.begin(), off.end(), (uint64_t)0);
-    none.assign(nq, hb::LABEL_NONE);
-    qset_off = off.data();
-    qset = none.data();
-  }
-  return (int)search_call(h, HOST, name, row_label_sets(qset_off, qset, qrange), exact, queries, nq, dim, knbn, ef, out);
+  OneLabelSets one;
+  Restriction rs;
+  one_restriction(name, nq, -1, qrange, qset_off, qset, one, rs);  // no resident filter: never refused
+  return (int)search_call(h, HOST, name, {{queries}, nq, (int)dim, knbn, ef, rs, exact, out}, 1, nullptr);
 }
 int hnsw_b200_search_flat_ranges(const void* h, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
                                  const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
@@ -901,116 +914,105 @@ int hnsw_b200_search_exact_ranges(const void* h, const int64_t* qrange, const ui
 
 int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                   void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
-  return (int)search_call(h, DEVICE, "search_exact_device", resident_or_all(filter), true, d_queries, nq, 0, knbn, 0,
-                          on_device(d_out, d_counts), sync, kernel_ms);
+  return (int)search_call(h, DEVICE, "search_exact_device", {{d_queries}, nq, 0, knbn, 0, resident_or_all(filter), true,
+                          on_device(d_out, d_counts)}, sync, kernel_ms);
 }
 
-// The restriction of a by-id or radius call (-1 and no sets or ranges: none), refused when a resident filter comes with
-// sets or ranges; a range without sets is a range within {LABEL_NONE} per query, as ranged_call reads it (the offsets
-// and values made in off and none), and sets without ranges are the label-sets call's
-static int one_restriction(const char* name, uint64_t nq, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
-                           const uint32_t* qset, std::vector<uint64_t>& off, std::vector<uint32_t>& none, Restriction& rs) {
-  const bool rows = qrange || qset_off || qset;
-  if (filter != -1 && rows)
-    return set_err(std::string(name) + ": a resident filter cannot be combined with label sets or ranges");
-  if (qrange && !qset_off && !qset) {
-    off.resize(nq + 1);
-    std::iota(off.begin(), off.end(), (uint64_t)0);
-    none.assign(nq, hb::LABEL_NONE);
-    qset_off = off.data();
-    qset = none.data();
+// The checks a by-id or radius call starts with, in the header's order, before its restriction's: the NULL handle, then
+// nq == 0 (1: nothing to run), qids (by stored point), and a radius call's radii (r: as run, -0 read as 0, whose key is
+// the smallest; NULL: not a radius call).  -1: refused, 0: go on.
+static int first_checks(const void* h, const char* name, uint64_t nq, bool by_id, const uint64_t* qids,
+                        const float* radius, std::vector<float>* r) {
+  if (!h) return set_err("NULL handle");
+  if (nq == 0) return 1;
+  if (by_id && !qids) return set_err(std::string(name) + ": qids is NULL");
+  if (!r) return 0;
+  if (!radius) return set_err(std::string(name) + ": radius is NULL");
+  r->resize(nq);
+  for (uint64_t i = 0; i < nq; ++i) {
+    if (std::isnan(radius[i]) || radius[i] < 0)
+      return set_err(std::string(name) + ": radius[" + std::to_string(i) + "] = " + std::to_string(radius[i]) + " is " +
+                     (std::isnan(radius[i]) ? "NaN" : "negative"));
+    (*r)[i] = radius[i] == 0 ? 0.0f : radius[i];
   }
-  rs = rows ? row_label_sets(qset_off, qset, qrange) : resident_or_all(filter);
   return 0;
 }
 
-// Search by stored point, under one_restriction's restriction
-static int by_id_call(const void* h, Via via, const char* name, bool exact, const uint64_t* qids, uint64_t nq, uint64_t knbn,
-                      uint64_t ef, int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
-                      const uint32_t* qset, const AnswerArrays& out, int sync = 1, float* kernel_ms = nullptr) {
-  if (!h) return set_err("NULL handle");
-  if (nq == 0) return 0;
-  if (!qids) return set_err(std::string(name) + ": qids is NULL");
-  std::vector<uint64_t> off;
-  std::vector<uint32_t> none;
-  Restriction rs;
-  if (one_restriction(name, nq, filter, qrange, qset_off, qset, off, none, rs)) return -1;
-  return (int)search_call(h, via, name, rs, exact, nullptr, nq, 0, knbn, ef, out, sync, kernel_ms, qids, exclude_self != 0);
+// Search by stored point (b.in.qids, and b.in.skip for exclude_self), under one_restriction's restriction
+static int by_id_call(const void* h, Via via, const char* name, HostBatch b, int64_t filter, const int64_t* qrange,
+                      const uint64_t* qset_off, const uint32_t* qset, int sync, float* kernel_ms) {
+  OneLabelSets one;
+  if (int s = first_checks(h, name, b.nq, true, b.in.qids, nullptr, nullptr)) return s < 0 ? -1 : 0;
+  if (one_restriction(name, b.nq, filter, qrange, qset_off, qset, one, b.restriction)) return -1;
+  return (int)search_call(h, via, name, b, sync, kernel_ms);
 }
 int hnsw_b200_search_flat_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, uint64_t ef_search,
                                 int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
                                 const uint32_t* qset, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                 int32_t* out_pid, int32_t* out_counts) {
-  return by_id_call(h, HOST, "search_flat_by_id", false, qids, nq, knbn, ef_search, exclude_self, filter, qrange, qset_off,
-                    qset, columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return by_id_call(h, HOST, "search_flat_by_id", {{nullptr, nullptr, qids, exclude_self ? qids : nullptr}, nq, 0, knbn,
+                    ef_search, Restriction(), false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)},
+                    filter, qrange, qset_off, qset, 1, nullptr);
 }
 int hnsw_b200_search_exact_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, int exclude_self,
                                  int64_t filter, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
                                  uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
                                  int32_t* out_counts) {
-  return by_id_call(h, HOST, "search_exact_by_id", true, qids, nq, knbn, 0, exclude_self, filter, qrange, qset_off, qset,
-                    columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return by_id_call(h, HOST, "search_exact_by_id", {{nullptr, nullptr, qids, exclude_self ? qids : nullptr}, nq, 0, knbn,
+                    0, Restriction(), true, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, filter,
+                    qrange, qset_off, qset, 1, nullptr);
 }
 int hnsw_b200_search_device_by_id(const void* h, int exact, int64_t filter, const uint64_t* d_qids, uint64_t nq,
                                   uint64_t knbn, uint64_t ef_search, int exclude_self, void* d_out, int32_t* d_counts,
                                   int sync, float* kernel_ms) {
-  return by_id_call(h, DEVICE, "search_device_by_id", exact != 0, d_qids, nq, knbn, exact ? 0 : ef_search, exclude_self,
-                    filter, nullptr, nullptr, nullptr, on_device(d_out, d_counts), sync, kernel_ms);
+  return by_id_call(h, DEVICE, "search_device_by_id", {{nullptr, nullptr, d_qids, exclude_self ? d_qids : nullptr}, nq, 0,
+                    knbn, exact ? 0 : ef_search, Restriction(), exact != 0, on_device(d_out, d_counts)}, filter, nullptr,
+                    nullptr, nullptr, sync, kernel_ms);
 }
 
-// Radius search: the exact scan of host queries (qids == nullptr) or of stored points, under one_restriction's
-// restriction, each row cut at its radius and its total of points within it into out_total (may be NULL).  Every radius
-// is checked before anything runs: >= 0 and not NaN, -0 read as 0 (whose key is the smallest).  knbn == 0 counts only:
-// the scan runs at k = 1 into scratch rows, the caller's row arrays may be NULL, and every count is 0.
-static int radius_call(const void* h, const char* name, bool by_id, const void* queries, uint64_t dim, const uint64_t* qids,
-                       uint64_t nq, const float* radius, uint64_t knbn, int exclude_self, int64_t filter,
-                       const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset, AnswerArrays out,
-                       uint64_t* out_total) {
-  if (!h) return set_err("NULL handle");
-  if (nq == 0) return 0;
-  if (by_id && !qids) return set_err(std::string(name) + ": qids is NULL");
-  if (!radius) return set_err(std::string(name) + ": radius is NULL");
-  std::vector<float> r(nq);
-  for (uint64_t i = 0; i < nq; ++i) {
-    if (std::isnan(radius[i]) || radius[i] < 0)
-      return set_err(std::string(name) + ": radius[" + std::to_string(i) + "] = " + std::to_string(radius[i]) + " is " +
-                     (std::isnan(radius[i]) ? "NaN" : "negative"));
-    r[i] = radius[i] == 0 ? 0.0f : radius[i];
-  }
-  std::vector<uint64_t> off;
-  std::vector<uint32_t> none;
-  Restriction rs;
-  if (one_restriction(name, nq, filter, qrange, qset_off, qset, off, none, rs)) return -1;
+// Radius search: the exact scan of host queries or of stored points (by_id), under one_restriction's restriction, each
+// row cut at its radius and its total of points within it into out_total (may be NULL).  knbn == 0 counts only: the
+// scan runs at k = 1 into scratch rows, the caller's row arrays may be NULL, and every count is 0.
+static int radius_call(const void* h, const char* name, bool by_id, HostBatch b, const float* radius, int64_t filter,
+                       const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset, uint64_t* out_total) {
+  std::vector<float> r;
+  OneLabelSets one;
+  if (int s = first_checks(h, name, b.nq, by_id, b.in.qids, radius, &r)) return s < 0 ? -1 : 0;
+  if (one_restriction(name, b.nq, filter, qrange, qset_off, qset, one, b.restriction)) return -1;
+  b.in.radius = r.data();
+  const size_t knbn = b.k;
   std::vector<uint64_t> scratch_ids;
   std::vector<float> scratch_dist;
   if (knbn == 0) {
-    scratch_ids.resize(nq);
-    scratch_dist.resize(nq);
-    out.ids = scratch_ids.data();
-    out.dist = scratch_dist.data();
-    out.internal = nullptr;
-    out.pid = nullptr;
+    scratch_ids.resize(b.nq);
+    scratch_dist.resize(b.nq);
+    b.k = 1;
+    b.out.ids = scratch_ids.data();
+    b.out.dist = scratch_dist.data();
+    b.out.internal = nullptr;
+    b.out.pid = nullptr;
   }
-  out.total = out_total;
-  const int rc = (int)search_call(h, HOST, name, rs, true, queries, nq, dim, knbn ? knbn : 1, 0, out, 1, nullptr, qids,
-                                  exclude_self != 0, r.data());
-  if (rc == 0 && knbn == 0) std::fill(out.counts, out.counts + nq, 0);
+  b.out.total = out_total;
+  const int rc = (int)search_call(h, HOST, name, b, 1, nullptr);
+  if (rc == 0 && knbn == 0) std::fill(b.out.counts, b.out.counts + b.nq, 0);
   return rc;
 }
 int hnsw_b200_search_exact_radius(const void* h, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
                                   const uint32_t* qset, const void* queries, uint64_t nq, uint64_t dim,
                                   const float* radius, uint64_t knbn, uint64_t* out_ids, float* out_dist,
                                   uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts, uint64_t* out_total) {
-  return radius_call(h, "search_exact_radius", false, queries, dim, nullptr, nq, radius, knbn, 0, filter, qrange, qset_off,
-                     qset, columns(out_ids, out_dist, out_internal, out_pid, out_counts), out_total);
+  return radius_call(h, "search_exact_radius", false, {{queries}, nq, (int)dim, knbn, 0, Restriction(), true,
+                     columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, radius, filter, qrange, qset_off,
+                     qset, out_total);
 }
 int hnsw_b200_search_exact_radius_by_id(const void* h, const uint64_t* qids, uint64_t nq, const float* radius,
                                         uint64_t knbn, int exclude_self, int64_t filter, const int64_t* qrange,
                                         const uint64_t* qset_off, const uint32_t* qset, uint64_t* out_ids,
                                         float* out_dist, uint32_t* out_internal, int32_t* out_pid,
                                         int32_t* out_counts, uint64_t* out_total) {
-  return radius_call(h, "search_exact_radius_by_id", true, nullptr, 0, qids, nq, radius, knbn, exclude_self, filter, qrange,
-                     qset_off, qset, columns(out_ids, out_dist, out_internal, out_pid, out_counts), out_total);
+  return radius_call(h, "search_exact_radius_by_id", true, {{nullptr, nullptr, qids, exclude_self ? qids : nullptr}, nq, 0,
+                     knbn, 0, Restriction(), true, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, radius,
+                     filter, qrange, qset_off, qset, out_total);
 }
 
 int hnsw_b200_get_vectors(const void* h, const uint64_t* ranks, uint64_t n, void* out) {

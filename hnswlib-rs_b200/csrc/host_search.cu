@@ -85,41 +85,39 @@ static inline void point_id(const Index* rx, uint32_t it, int32_t* pid2) {
   pid2[1] = it != INVALID_ID ? rx->h_rank[it] : -1;
 }
 
-// rows [first, first + count) of `out` from one leg's answers (k slots each, as the kernels left them: the slots beyond a
-// query's count hold (~0, +inf, INVALID_ID)), and a radius batch's totals: plain copies
-static void put_rows(const AnswerArrays& out, const Index* rx, size_t first, size_t count, size_t k, const NeighbourOut* a,
-                     const int32_t* cnts, const uint32_t* tots) {
+// rows [first, first + count) of `out` from one leg's answers `ans` (k slots each, as the kernels left them: the slots
+// beyond a query's count hold (~0, +inf, INVALID_ID)), and a radius batch's totals: plain copies
+static void put_rows(const AnswerArrays& out, const Index* rx, size_t first, size_t count, size_t k, const HostAnswers& ans) {
   if (count == 0) return;
-  memcpy(out.counts + first, cnts, count * sizeof(int32_t));
-  if (out.total && tots)
-    for (size_t i = 0; i < count; ++i) out.total[first + i] = tots[i];
+  memcpy(out.counts + first, ans.counts, count * sizeof(int32_t));
+  if (out.total && ans.totals)
+    for (size_t i = 0; i < count; ++i) out.total[first + i] = ans.totals[i];
   const size_t o = first * k, tot = count * k;
   if (out.nb) {
-    memcpy(out.nb + o, a, tot * sizeof(NeighbourOut));
+    memcpy(out.nb + o, ans.slots, tot * sizeof(NeighbourOut));
     return;
   }
   if (out.ids) {
     uint64_t* ids = out.ids + o;
-    for (size_t s = 0; s < tot; ++s) ids[s] = a[s].origin;
+    for (size_t s = 0; s < tot; ++s) ids[s] = ans.slots[s].origin;
   }
   float* dist = out.dist + o;
-  for (size_t s = 0; s < tot; ++s) dist[s] = a[s].dist;
+  for (size_t s = 0; s < tot; ++s) dist[s] = ans.slots[s].dist;
   if (out.internal) {
     uint32_t* internal = out.internal + o;
-    for (size_t s = 0; s < tot; ++s) internal[s] = a[s].internal;
+    for (size_t s = 0; s < tot; ++s) internal[s] = ans.slots[s].internal;
   }
   if (out.pid) {
     int32_t* pid = out.pid + 2 * o;
-    for (size_t s = 0; s < tot; ++s) point_id(rx, a[s].internal, pid + 2 * s);
+    for (size_t s = 0; s < tot; ++s) point_id(rx, ans.slots[s].internal, pid + 2 * s);
   }
 }
 
 // queries [first, first + count) of the batch from one leg's answers, each to its row of `out` (out.perm)
-static void put_slice(const AnswerArrays& out, const Index* rx, size_t first, size_t count, size_t k, const NeighbourOut* a,
-                      const int32_t* cnts, const uint32_t* tots) {
-  if (!out.perm) return put_rows(out, rx, first, count, k, a, cnts, tots);
+static void put_slice(const AnswerArrays& out, const Index* rx, size_t first, size_t count, size_t k, const HostAnswers& a) {
+  if (!out.perm) return put_rows(out, rx, first, count, k, a);
   for (size_t i = 0; i < count; ++i)
-    put_rows(out, rx, out.perm[first + i], 1, k, a + i * k, cnts + i, tots ? tots + i : nullptr);
+    put_rows(out, rx, out.perm[first + i], 1, k, {a.slots + i * k, a.counts + i, a.totals ? a.totals + i : nullptr});
 }
 
 // slot s of `out` from answer e of index rx, reported with internal id `internal` (a partitioned handle's global rank)
@@ -136,27 +134,26 @@ static inline void put_answer(const AnswerArrays& out, size_t s, const Index* rx
 
 // every query of the batch from the answers of P partition legs, merged by merge_lists, to its row of `out` (out.perm);
 // the slots past a query's count are padded with (~0, +inf, INVALID_ID) and PointId (-1, -1).  A radius batch's total is
-// the sum of the partitions' (t: each leg's totals).
+// the sum of the partitions'.  a[p]: leg p's answers.
 static void put_merged(const AnswerArrays& out, const std::vector<Leg>& legs, size_t nq, size_t k,
-                       const std::vector<const NeighbourOut*>& a, const std::vector<const int32_t*>& c,
-                       const std::vector<const uint32_t*>& t) {
+                       const std::vector<HostAnswers>& a) {
   const int P = (int)legs.size();
   const NeighbourOut pad{~0ull, __builtin_inff(), INVALID_ID};
   int32_t cnt[Partitions::MAX_PARTS];
   for (size_t q = 0; q < nq; ++q) {
-    for (int p = 0; p < P; ++p) cnt[p] = c[p][q];
+    for (int p = 0; p < P; ++p) cnt[p] = a[p].counts[q];
     const size_t o = q * k, row = out.perm ? out.perm[q] : q, w = row * k;
     const size_t total = merge_lists(
-        P, k, cnt, [&](int p, int i) { return a[p][o + i].dist; },
+        P, k, cnt, [&](int p, int i) { return a[p].slots[o + i].dist; },
         [&](size_t j, int p, int i) {
-          const NeighbourOut& e = a[p][o + i];
+          const NeighbourOut& e = a[p].slots[o + i];
           put_answer(out, w + j, legs[p].rx, e, e.internal * (uint32_t)P + (uint32_t)p);
         });
     for (size_t j = total; j < k; ++j) put_answer(out, w + j, nullptr, pad, INVALID_ID);
     out.counts[row] = (int32_t)total;
-    if (out.total && t[0]) {
+    if (out.total && a[0].totals) {
       uint64_t sum = 0;
-      for (int p = 0; p < P; ++p) sum += t[p][q];
+      for (int p = 0; p < P; ++p) sum += a[p].totals[q];
       out.total[row] = sum;
     }
   }
@@ -380,23 +377,55 @@ int Index::legs_fail(const Leg* legs, size_t n, bool replicas_first) {
   return 0;
 }
 
+// The batch's rows in sorted-row order (row j: caller row perm[j]): every present column copied in that order into
+// `store`, flat queries as row pointers into them (q_bytes apart), and skip still the ids when it was
+static HostRows sorted_rows(const HostRows& in, const std::vector<size_t>& perm, size_t q_bytes,
+                            std::vector<unsigned char>& store) {
+  const size_t nq = perm.size();
+  store.resize(nq * (sizeof(void*) + 2 * sizeof(uint64_t) + sizeof(float)));  // room for every column, 8-byte ones first
+  unsigned char* at = store.data();
+  auto column = [&](auto value) {  // the next column of `store`: row j holds value(perm[j])
+    unsigned char* c = at;
+    for (size_t j = 0; j < nq; ++j, at += sizeof(value(0))) {
+      const auto v = value(perm[j]);
+      memcpy(at, &v, sizeof(v));
+    }
+    return c;
+  };
+  HostRows s;
+  if (in.queries || in.rows)
+    s.rows = (const void* const*)column([&](size_t i) {
+      return in.rows ? in.rows[i] : (const void*)((const char*)in.queries + i * q_bytes);
+    });
+  if (in.qids) s.qids = (const uint64_t*)column([&](size_t i) { return in.qids[i]; });
+  if (in.skip) s.skip = in.skip == in.qids ? s.qids : (const uint64_t*)column([&](size_t i) { return in.skip[i]; });
+  if (in.radius) s.radius = (const float*)column([&](size_t i) { return in.radius[i]; });
+  return s;
+}
+
+// Leg l's rows: rows [l.first, l.first + l.count) of the batch's, flat queries q_bytes apart.  A batch by stored point on
+// a partitioned handle (P partitions; 0: none) runs on its rows gathered into the queries, and a row leaves out its
+// point only on the partition that holds it, as that partition's local id (made in `local`).
+static HostRows leg_rows(const HostRows& in, const Leg& l, size_t q_bytes, uint64_t P, std::vector<uint64_t>& local) {
+  const size_t j = l.first;
+  HostRows s{in.queries ? (const char*)in.queries + j * q_bytes : nullptr, in.rows ? in.rows + j : nullptr,
+             in.qids ? in.qids + j : nullptr, in.skip ? in.skip + j : nullptr, in.radius ? in.radius + j : nullptr};
+  if (P && s.qids) {
+    if (s.skip) {
+      local.resize(l.count);
+      for (size_t i = 0; i < l.count; ++i) local[i] = s.skip[i] % P == (uint64_t)l.part ? s.skip[i] / P : ~0ull;
+      s.skip = local.data();
+    }
+    s.qids = nullptr;
+  }
+  return s;
+}
+
 void Index::begin_leg(const HostBatch& b, Leg& l) {
   if (l.ctx < 0) l.ctx = l.rx->acquire_ctx();
-  const uint64_t* ids = b.qids ? b.qids + l.first : nullptr;
-  const uint64_t* skip = b.exclude_self ? ids : nullptr;
   std::vector<uint64_t> local;
-  if (parts && ids) {  // the rows were gathered into b.queries; a row leaves out its point on the partition that holds it
-    const uint64_t P = (uint64_t)parts->count();
-    if (skip) {
-      local.resize(l.count);
-      for (size_t i = 0; i < l.count; ++i) local[i] = ids[i] % P == (uint64_t)l.part ? ids[i] / P : ~0ull;
-      skip = local.data();
-    }
-    ids = nullptr;
-  }
-  const void* q = b.rows || ids ? nullptr : (const char*)b.queries + l.first * (size_t)b.d * es;
-  l.rc = l.rx->search_host_begin(l.ctx, q, b.rows ? b.rows + l.first : nullptr, ids, skip, l.count, b.d, b.k, b.ef, l.plan,
-                                 b.radius ? b.radius + l.first : nullptr);
+  const HostRows in = leg_rows(b.in, l, (size_t)b.d * es, parts ? parts->count() : 0, local);
+  l.rc = l.rx->search_host_begin(l.ctx, in, l.count, b.d, b.k, b.ef, l.plan);
   l.begun = l.rc == 0;
 }
 
@@ -410,57 +439,39 @@ void Index::release_leg(Leg& l) {
   l.ctx = -1;
 }
 
-// collects a leg, writes its slice of `out` and releases its context
-int Index::end_leg(Leg& l, size_t k, const AnswerArrays& out) {
+// collects a leg, writes its slice of b.out and releases its context
+int Index::end_leg(Leg& l, const HostBatch& b) {
   if (l.begun) {
-    const NeighbourOut* a = nullptr;
-    const int32_t* c = nullptr;
-    const uint32_t* t = nullptr;
-    l.rc = l.rx->search_host_finish(l.ctx, &a, &c, &t);
-    if (!l.rc) put_slice(out, l.rx, l.first, l.count, k, a, c, t);
+    const HostAnswers a = l.rx->search_host_finish(l.ctx);
+    l.rc = a.rc;
+    if (!l.rc) put_slice(b.out, l.rx, l.first, l.count, b.k, a);
   }
   release_leg(l);
   return l.rc;
 }
 
 // ------------------------------------------------------------------------------------------------ batches
-// The batch `call` planned into t's legs, each with its plan; `b` is the batch as the legs run it.  A per-row restriction:
-// the batch is planned over the rows sorted by filter or label set, gathered through row pointers (by stored point: its
-// ids and radii permuted), and each answer goes back to its caller's row.  A batch by stored point on a partitioned handle has its
-// rows gathered from their partitions first, since no device reads another partition's store, and is then searched as
-// host queries.  A leg that could not have its plan is reported in leg order, or the replicas' first.
-int Index::prepare_batch(const HostBatch& call, HostBatch& b, Ticket& t, bool replicas_first) {
+// The batch `call` planned into t's legs, each with its plan; t.b is the batch as the legs run it.  A per-row
+// restriction: the batch is planned over the rows sorted by filter or label set (sorted_rows), and each answer goes
+// back to its caller's row.  A batch by stored point on a partitioned handle has its rows gathered from their
+// partitions first, since no device reads another partition's store, and is then searched as host queries.  A leg that
+// could not have its plan is reported in leg order, or the replicas' first.
+int Index::prepare_batch(const HostBatch& call, Ticket& t, bool replicas_first) {
   if (parts && dim != 0 && call.d != dim) return fail("query length differs from the index dimension");
   int r;
+  HostBatch& b = t.b;
   b = call;
-  if (parts && call.qids) {
+  if (parts && call.in.qids) {
     t.gathered.resize(call.nq * (size_t)dim * es);
-    if ((r = get_vectors(call.qids, call.nq, t.gathered.data()))) return r;
-    b.queries = t.gathered.data();
+    if ((r = get_vectors(call.in.qids, call.nq, t.gathered.data()))) return r;
+    b.in.queries = t.gathered.data();
   }
   std::vector<int64_t> sorted;
   if (call.restriction.per_row()) {
     if ((r = sort_rows(call.restriction, call.nq, t.perm, sorted, t.sets))) return r;
-    if (call.qids) {
-      t.qids.resize(call.nq);
-      for (size_t j = 0; j < call.nq; ++j) t.qids[j] = call.qids[t.perm[j]];
-      b.qids = t.qids.data();
-    }
-    if (call.radius) {
-      t.radius.resize(call.nq);
-      for (size_t j = 0; j < call.nq; ++j) t.radius[j] = call.radius[t.perm[j]];
-      b.radius = t.radius.data();
-    }
-    if (!call.qids || parts) {
-      t.rows.resize(call.nq);
-      for (size_t j = 0; j < call.nq; ++j)
-        t.rows[j] = b.rows ? b.rows[t.perm[j]] : (const char*)b.queries + t.perm[j] * (size_t)b.d * es;
-      b.rows = t.rows.data();
-    }
+    b.in = sorted_rows(b.in, t.perm, (size_t)b.d * es, t.rows);
     b.out.perm = t.perm.data();
   }
-  t.k = b.k;
-  t.out = b.out;
   if ((r = plan(b.nq, t.legs))) return r;
   if (resolve(b.restriction, b.exact, sorted, t.legs.data(), t.legs.size(), t.bits, &t.sets))
     return legs_fail(t.legs.data(), t.legs.size(), replicas_first && !parts);
@@ -469,21 +480,21 @@ int Index::prepare_batch(const HostBatch& call, HostBatch& b, Ticket& t, bool re
 
 int Index::search_batch(const HostBatch& call) {
   if (call.nq == 0) return 0;
-  HostBatch b;
   Ticket t;
   int r;
-  if ((r = prepare_batch(call, b, t, true))) return r;
+  if ((r = prepare_batch(call, t, true))) return r;
+  const HostBatch& b = t.b;
   std::vector<Leg>& legs = t.legs;
   const int n = (int)legs.size();
   const bool sharded = n > 1 && !parts;
   if (n == 1 && !parts) {
     begin_leg(b, legs[0]);
-    return end_leg(legs[0], b.k, b.out);
+    return end_leg(legs[0], b);
   }
   if (sharded) {  // leg i on worker i - 1
     workers_.run(n, [&](int i) {
       begin_leg(b, legs[i]);
-      return end_leg(legs[i], b.k, b.out);
+      return end_leg(legs[i], b);
     });
     return legs_fail(legs.data(), n, true);
   }
@@ -496,31 +507,31 @@ int Index::search_batch(const HostBatch& call) {
     begin_leg(b, legs[p]);
     if (legs[p].rc) bad = p;
   }
-  std::vector<const NeighbourOut*> a(n);
-  std::vector<const int32_t*> c(n);
-  std::vector<const uint32_t*> tot(n);
+  std::vector<HostAnswers> a(n);
   for (int p = 0; p < n; ++p) {
-    if (legs[p].begun) legs[p].rc = legs[p].rx->search_host_finish(legs[p].ctx, &a[p], &c[p], &tot[p]);
+    if (legs[p].begun) {
+      a[p] = legs[p].rx->search_host_finish(legs[p].ctx);
+      legs[p].rc = a[p].rc;
+    }
     if (legs[p].rc && bad < 0) bad = p;
   }
-  if (bad < 0) put_merged(b.out, legs, b.nq, b.k, a, c, tot);
+  if (bad < 0) put_merged(b.out, legs, b.nq, b.k, a);
   for (Leg& l : legs) release_leg(l);
   return bad < 0 ? 0 : legs_fail(&legs[bad], 1, false);
 }
 
 int64_t Index::submit_batch(const HostBatch& call) {
   DeviceRestore keep;  // the legs switch to their devices on the calling thread
-  HostBatch b;
   Ticket t;
   int r;
-  if ((r = prepare_batch(call, b, t, false))) return r;
+  if ((r = prepare_batch(call, t, false))) return r;
   int bad = -1;
   for (size_t i = 0; i < t.legs.size() && bad < 0; ++i) {  // one after the other, on the calling thread
-    begin_leg(b, t.legs[i]);
+    begin_leg(t.b, t.legs[i]);
     if (t.legs[i].rc) bad = (int)i;
   }
   if (bad >= 0) {
-    for (Leg& l : t.legs) end_leg(l, t.k, t.out);  // collect what was enqueued before the failure
+    for (Leg& l : t.legs) end_leg(l, t.b);  // collect what was enqueued before the failure
     return legs_fail(&t.legs[bad], 1, false);
   }
   pending_.fetch_add(1);
@@ -528,8 +539,8 @@ int64_t Index::submit_batch(const HostBatch& call) {
 }
 
 int Index::finish_batch(Ticket& t) {
-  if (t.legs.size() == 1) return end_leg(t.legs[0], t.k, t.out);
-  workers_.run((int)t.legs.size(), [&](int i) { return end_leg(t.legs[i], t.k, t.out); });
+  if (t.legs.size() == 1) return end_leg(t.legs[0], t.b);
+  workers_.run((int)t.legs.size(), [&](int i) { return end_leg(t.legs[i], t.b); });
   return legs_fail(t.legs.data(), t.legs.size(), false);
 }
 

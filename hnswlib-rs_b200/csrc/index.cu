@@ -652,28 +652,27 @@ void Index::release_ctx(int c) {
 // context streams, so that two consecutive launches overlap.  The handle's stream does NOT wait for it: join() (or
 // check_status, set_stream, any synchronous call's own synchronisation) makes it do so; stream_wait_last() makes any
 // stream wait for the most recent launch alone.  The same for the exact scan (`exact`).
-int Index::search_device(const Restriction& rs, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef_arg,
-                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* d_qids,
-                         bool exclude_self) {
-  Leg leg{this, 0, 0, nq};
+int Index::search_device(const HostBatch& b, bool sync, float* kernel_ms) {
+  Leg leg{this, 0, 0, b.nq};
   std::vector<std::vector<uint32_t>> bits;
   int r;
-  if (resolve(rs, exact, {}, &leg, 1, bits)) return legs_fail(&leg, 1, false);
-  if (nq == 0) return 0;
+  if (resolve(b.restriction, b.exact, {}, &leg, 1, bits)) return legs_fail(&leg, 1, false);
+  if (b.nq == 0) return 0;
   HB_CUDA(cudaSetDevice(device));
-  if (d_qids) {
+  if (const uint64_t* d_qids = b.in.qids) {
     // the ids are checked before anything runs: read back once the work already on the handle's stream (which may
     // write them) is done
-    std::vector<uint64_t> ids(nq);
-    HB_CUDA(cudaMemcpyAsync(ids.data(), d_qids, nq * sizeof(uint64_t), cudaMemcpyDeviceToHost, stream_));
+    std::vector<uint64_t> ids(b.nq);
+    HB_CUDA(cudaMemcpyAsync(ids.data(), d_qids, b.nq * sizeof(uint64_t), cudaMemcpyDeviceToHost, stream_));
     HB_CUDA(cudaStreamSynchronize(stream_));
-    for (size_t i = 0; i < nq; ++i)
+    for (size_t i = 0; i < b.nq; ++i)
       if (ids[i] >= n)
         return fail("qids[" + std::to_string(i) + "] = " + std::to_string(ids[i]) + " is not below nb_point = " +
                     std::to_string(n));
   }
   auto run = [&](SearchCtx& c, bool s, float* ms) {
-    SearchCtx::Launch L{d_queries, nq, k, ef_arg, d_out, d_counts, false, 0, {}, {}, d_qids, exclude_self ? d_qids : nullptr};
+    SearchCtx::Launch L{{b.in.queries, b.in.qids, b.in.skip, nullptr, nullptr, b.out.nb, b.out.counts}, b.nq, b.k, b.ef,
+                        false, 0, {}, {}};
     const int e = stage_plan(c, leg.plan, L);
     return e ? e : run_plan(c, L, s, ms);
   };
@@ -714,26 +713,18 @@ int Index::stream_wait_last(cudaStream_t s) {
   return 0;
 }
 
-int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const LaunchFilter& f,
-                         NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* q_ids,
-                         const uint64_t* skip) {
-  if (k == 0) return fail("knbn must be positive");
-  if (poisoned_) return fail(poison_msg_);
+int Index::search_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, size_t k, size_t ef_arg,
+                         const LaunchFilter& f, bool sync, float* kernel_ms) {
   cudaStream_t st = c.stream;
-  if (dim == 0) {  // empty index: every answer is empty (hnsw.rs:1498-1503)
-    HB_CUDA(cudaMemsetAsync(d_counts, 0, nq * sizeof(int32_t), st));
-    if (sync) HB_CUDA(cudaStreamSynchronize(st));
-    return 0;
-  }
   SearchParams p;
   p.g = view();
-  p.queries = d_queries;
+  p.queries = rows.d_queries;
   p.q_bytes = dim * es;
   p.q_stride_bytes = dim * es;
   p.nq = (uint32_t)nq;
-  p.q_ids = q_ids;
-  p.skip_ids = skip;
-  k += skip ? 1 : 0;  // the search takes k + 1, each row is k wide (write_row)
+  p.q_ids = rows.q_ids;
+  p.skip_ids = rows.skip;
+  k += rows.skip ? 1 : 0;  // the search takes k + 1, each row is k wide (write_row)
   p.k = (int)k;
   p.ef = (int)std::max(ef_arg, k);  // hnsw.rs:1531
   int layer0 = 0;                   // hnsw.rs:1534-1540
@@ -741,8 +732,8 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   if (n == 0) layer0 = 0;
   p.layer0 = layer0;
   p.work_counter = c.d_counter;
-  p.out_nb = d_out;
-  p.out_count = d_counts;
+  p.out_nb = rows.out;
+  p.out_count = rows.counts;
   p.filter_table = f.table;
   p.filter_sel = f.sel;
   p.filter = f.filter;
@@ -759,7 +750,7 @@ int Index::search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t 
   p.smem_per_warp = (int)spw;
   const CtaShape cta = cta_shape(spw, query_threads(kind) / 32);
   if (!cta.warps)
-    return fail(std::string(skip ? "exclude_self searches knbn + 1: " : "") + "ef / dimension too large: one query needs " +
+    return fail(std::string(rows.skip ? "exclude_self searches knbn + 1: " : "") + "ef / dimension too large: one query needs " +
                 std::to_string(spw) + " bytes of shared memory (limit 220 KB)");
   const int wpb = cta.warps;
   const size_t smem = cta.smem;
@@ -857,30 +848,35 @@ static const void* device_view_of_host(const void* p) {
 // are being searched), and the answers are written by the kernel straight into the context's pinned result buffer: one
 // synchronisation.  Pageable queries and row pointers are gathered into the context's own pinned staging buffer first
 // (the only host-side copy), which the kernel then reads the same way.
-int Index::search_host_begin(int ci, const void* queries, const void* const* rows, const uint64_t* qids,
-                             const uint64_t* skip, size_t nq, int d, size_t k, size_t ef, const LegPlan& plan,
-                             const float* radius) {
+int Index::search_host_begin(int ci, const HostRows& in, size_t nq, int d, size_t k, size_t ef, const LegPlan& plan) {
   SearchCtx& c = ctx_[ci];
   cudaStream_t st = c.stream;
   c.pend = SearchCtx::Pending();
   if (nq == 0) return 0;
   HB_CUDA(cudaSetDevice(device));
-  if (!qids && dim != 0 && d != dim) return fail("query length differs from the index dimension");
+  if (!in.qids && dim != 0 && d != dim) return fail("query length differs from the index dimension");
   int r;
-  // [answers][counts][status, 16 bytes][radius mode: totals]
-  const size_t out_bytes = nq * k * sizeof(NeighbourOut), cnt_bytes = nq * sizeof(int32_t);
-  const size_t rb = radius ? nq * sizeof(float) : 0;  // radii or totals, 4 bytes a row
-  if ((r = ensure_pinned(&c.h_res, &c.h_res_bytes, out_bytes + cnt_bytes + 16 + rb, cudaHostAllocMapped | cudaHostAllocPortable)))
+  // Per-row columns: by stored point the ids, and the ids the rows leave out, cross the bus in place of the rows (16 bytes
+  // a query at most), as do a radius launch's radii.  Those go in with one copy, from after the queries in the pinned
+  // buffer to after an exact launch's rows in device memory; the totals follow there and come back after the status.
+  enum { IDS, SKIP, RADIUS, TOTALS, COLUMNS };
+  struct Column {
+    const void* host;  // the values that go in (the totals come out; skip == qids is the ids' column)
+    size_t bytes;      // a row (0: absent)
+  } col[COLUMNS] = {{in.qids, in.qids ? 8u : 0u}, {in.skip, in.skip && in.skip != in.qids ? 8u : 0u},
+                    {in.radius, in.radius ? 4u : 0u}, {nullptr, in.radius ? 4u : 0u}};
+  size_t at[COLUMNS + 1] = {};  // column i at at[i]: at[TOTALS] bytes go in, at[COLUMNS] in all
+  for (int i = 0; i < COLUMNS; ++i) at[i + 1] = at[i] + col[i].bytes * nq;
+  // [answers][counts][status, 16 bytes][totals]
+  const size_t out_bytes = nq * k * sizeof(NeighbourOut), cnt_bytes = nq * sizeof(int32_t), tot_bytes = at[COLUMNS] - at[TOTALS];
+  if ((r = ensure_pinned(&c.h_res, &c.h_res_bytes, out_bytes + cnt_bytes + 16 + tot_bytes, cudaHostAllocMapped | cudaHostAllocPortable)))
     return r;
   NeighbourOut* hout = (NeighbourOut*)c.h_res;
   int32_t* hcnt = (int32_t*)((char*)c.h_res + out_bytes);
-  int32_t* hstatus = hcnt + nq;
-  uint32_t* htot = radius ? (uint32_t*)((char*)c.h_res + out_bytes + cnt_bytes + 16) : nullptr;
+  uint32_t* htot = tot_bytes ? (uint32_t*)((char*)c.h_res + out_bytes + cnt_bytes + 16) : nullptr;
+  c.pend.ans = HostAnswers{hout, hcnt, htot};
+  c.pend.hstatus = hcnt + nq;
   SearchCtx::Launch& L = c.pend.run;
-  c.pend.hout = hout;
-  c.pend.hcnt = hcnt;
-  c.pend.hstatus = hstatus;
-  c.pend.htot = htot;
   L.nq = nq;
   L.k = k;
   L.ef = ef;
@@ -892,70 +888,65 @@ int Index::search_host_begin(int ci, const void* queries, const void* const* row
   }
   char* dv = (char*)device_view_of_host(c.h_res);  // where the kernel writes
   if (!dv) return fail("the pinned result buffer has no device address");
-  L.out = (NeighbourOut*)dv;
-  L.counts = (int32_t*)(dv + out_bytes);
-  // by stored point: the ids, and the ids the rows leave out, cross the bus in place of the rows (16 bytes a query at
-  // most); they go after the query staging in the pinned buffer and after an exact launch's rows in device memory, and
-  // a radius launch's radii after them (in device memory followed by its totals)
-  const size_t qbytes = qids ? 0 : nq * (size_t)dim * es, ib = nq * sizeof(uint64_t);
-  const int nid = (qids ? 1 : 0) + (skip && skip != qids ? 1 : 0);
-  const void* d_queries = qids || rows ? nullptr : device_view_of_host(queries);  // what the kernel reads
-  const size_t staged = qids || d_queries ? 0 : round128(qbytes);
-  if (staged + nid * ib + rb) {
+  L.rows.out = (NeighbourOut*)dv;
+  L.rows.counts = (int32_t*)(dv + out_bytes);
+  const size_t qbytes = in.qids ? 0 : nq * (size_t)dim * es;
+  const void* d_queries = in.qids || in.rows ? nullptr : device_view_of_host(in.queries);  // what the kernel reads
+  const size_t staged = in.qids || d_queries ? 0 : round128(qbytes);
+  if (staged + at[TOTALS]) {
     // gather into pinned staging (rows: one pointer per query, libext.rs parallel_search_neighbours_<ty>)
-    if ((r = ensure_pinned(&c.h_pin, &c.h_pin_bytes, staged + nid * ib + rb, cudaHostAllocMapped | cudaHostAllocPortable)))
+    if ((r = ensure_pinned(&c.h_pin, &c.h_pin_bytes, staged + at[TOTALS], cudaHostAllocMapped | cudaHostAllocPortable)))
       return r;
     unsigned char* stage = (unsigned char*)c.h_pin;
-    if (rows)
-      for (size_t i = 0; i < nq; ++i) memcpy(stage + i * (size_t)dim * es, rows[i], (size_t)dim * es);
+    if (in.rows)
+      for (size_t i = 0; i < nq; ++i) memcpy(stage + i * (size_t)dim * es, in.rows[i], (size_t)dim * es);
     else if (staged)
-      memcpy(stage, queries, qbytes);
+      memcpy(stage, in.queries, qbytes);
     if (staged) {
       d_queries = device_view_of_host(stage);
       if (!d_queries) return fail("the pinned query staging buffer has no device address");
     }
-    if (qids) memcpy(stage + staged, qids, ib);
-    if (skip && skip != qids) memcpy(stage + staged + (qids ? ib : 0), skip, ib);
-    if (radius) memcpy(stage + staged + nid * ib, radius, rb);
+    for (int i = IDS; i < TOTALS; ++i)
+      if (col[i].bytes) memcpy(stage + staged + at[i], col[i].host, col[i].bytes * nq);
   }
-  L.d_queries = d_queries;
+  L.rows.d_queries = d_queries;
   // an exact launch may run many CTAs per query (row slices): the queries cross the bus once, into device memory
   const size_t xq = plan.exact ? round128(qbytes) : 0;
-  if (xq + nid * ib + rb) {
-    if ((r = ensure_scratch(&c.d_xq, &c.d_xq_bytes, xq + nid * ib + 2 * rb, st))) return r;
+  if (xq + at[COLUMNS]) {
+    if ((r = ensure_scratch(&c.d_xq, &c.d_xq_bytes, xq + at[COLUMNS], st))) return r;
     if (xq) HB_CUDA(cudaMemcpyAsync(c.d_xq, d_queries, qbytes, cudaMemcpyDefault, st));
-    if (xq) L.d_queries = c.d_xq;
-    const uint64_t* ids = (const uint64_t*)((char*)c.d_xq + xq);
-    if (nid * ib + rb)
-      HB_CUDA(cudaMemcpyAsync((void*)ids, (char*)c.h_pin + staged, nid * ib + rb, cudaMemcpyHostToDevice, st));
-    L.q_ids = qids ? ids : nullptr;
-    L.skip = !skip ? nullptr : skip == qids ? ids : ids + (qids ? nq : 0);
-    L.radius = radius ? (const float*)(ids + nid * nq) : nullptr;
-    L.totals = radius ? (uint32_t*)(ids + nid * nq) + nq : nullptr;
+    if (xq) L.rows.d_queries = c.d_xq;
+    char* cols = (char*)c.d_xq + xq;
+    if (at[TOTALS]) HB_CUDA(cudaMemcpyAsync(cols, (char*)c.h_pin + staged, at[TOTALS], cudaMemcpyHostToDevice, st));
+    auto on_device = [&](int i) -> void* { return col[i].bytes ? cols + at[i] : nullptr; };
+    L.rows.q_ids = (const uint64_t*)on_device(IDS);
+    L.rows.skip = (const uint64_t*)on_device(in.skip == in.qids ? IDS : SKIP);
+    L.rows.radius = (const float*)on_device(RADIUS);
+    L.rows.totals = (uint32_t*)on_device(TOTALS);
   }
-  if (plan.exact) *hstatus = 0;
+  if (plan.exact) *c.pend.hstatus = 0;
   // one enqueue (the plan's uploads, the launches, the status); search_host_finish synchronises once and takes the slow
   // path (a visited table overflowed: grow and re-run) only when the status says so
   c.pend.enqueued = true;
   if ((r = stage_plan(c, plan, L)) || (r = run_plan(c, L, false, nullptr))) return r;
-  if (!plan.exact) HB_CUDA(cudaMemcpyAsync(hstatus, c.d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  if (radius) HB_CUDA(cudaMemcpyAsync(htot, L.totals, rb, cudaMemcpyDeviceToHost, st));
+  if (!plan.exact) HB_CUDA(cudaMemcpyAsync(c.pend.hstatus, c.d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (htot) HB_CUDA(cudaMemcpyAsync(htot, L.rows.totals, tot_bytes, cudaMemcpyDeviceToHost, st));
   return 0;
 }
 
-int Index::search_host_finish(int ci, const NeighbourOut** out, const int32_t** counts, const uint32_t** totals) {
+HostAnswers Index::search_host_finish(int ci) {
   SearchCtx& c = ctx_[ci];
-  cudaStream_t st = c.stream;
   SearchCtx::Pending& p = c.pend;
-  *out = p.hout;
-  *counts = p.hcnt;
-  if (totals) *totals = p.htot;
-  if (!p.enqueued) return 0;  // empty batch or empty index: the answers (if any) were filled by search_host_begin
-  HB_CUDA(cudaSetDevice(device));
-  HB_CUDA(cudaStreamSynchronize(st));
-  if (p.run.exact || *p.hstatus == 0) return 0;  // an exact scan has no status and nothing to re-run
-  HB_CUDA(cudaMemsetAsync(c.d_status, 0, sizeof(int), st));
-  return run_plan(c, p.run, true, nullptr);  // grows the tables
+  HostAnswers a = p.ans;
+  a.rc = [&] {
+    if (!p.enqueued) return 0;  // empty batch or empty index: the answers (if any) were filled by search_host_begin
+    HB_CUDA(cudaSetDevice(device));
+    HB_CUDA(cudaStreamSynchronize(c.stream));
+    if (p.run.exact || *p.hstatus == 0) return 0;  // an exact scan has no status and nothing to re-run
+    HB_CUDA(cudaMemsetAsync(c.d_status, 0, sizeof(int), c.stream));
+    return run_plan(c, p.run, true, nullptr);  // grows the tables
+  }();
+  return a;
 }
 
 // Graph: one RowFilter per run, a bitmap (a FilterT's host bits uploaded into the context first), a label (a set of one,
@@ -1040,18 +1031,20 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
 }
 
 int Index::run_plan(SearchCtx& c, const SearchCtx::Launch& L, bool sync, float* kernel_ms) {
-  if (L.exact)
-    return exact_on_ctx(c, L.d_queries, L.nq, L.k, L.groups, L.out, L.counts, sync, kernel_ms, L.q_ids, L.skip, L.radius,
-                        L.totals);
+  if (L.k == 0) return fail("knbn must be positive");
+  if (poisoned_) return fail(poison_msg_);
+  cudaStream_t st = c.stream;
+  if (L.rows.radius) HB_CUDA(cudaMemsetAsync(L.rows.totals, 0, L.nq * sizeof(uint32_t), st));
+  if (dim == 0) {  // empty index: every answer is empty (hnsw.rs:1498-1503)
+    HB_CUDA(cudaMemsetAsync(L.rows.counts, 0, L.nq * sizeof(int32_t), st));
+    if (sync) HB_CUDA(cudaStreamSynchronize(st));
+    return 0;
+  }
+  if (L.exact) return exact_on_ctx(c, L.rows, L.nq, L.k, L.groups, sync, kernel_ms);
   int r;
-  if (L.plain && (r = search_on_ctx(c, L.d_queries, L.plain, L.k, L.ef, LaunchFilter(), L.out, L.counts, sync, kernel_ms,
-                                    L.q_ids, L.skip)))
-    return r;
+  if (L.plain && (r = search_on_ctx(c, L.rows, L.plain, L.k, L.ef, LaunchFilter(), sync, kernel_ms))) return r;
   if (L.plain == L.nq) return 0;
-  const size_t j = L.plain;
-  const char* q = L.q_ids ? nullptr : (const char*)L.d_queries + j * (size_t)dim * es;
-  return search_on_ctx(c, q, L.nq - j, L.k, L.ef, L.filter, L.out + j * L.k, L.counts + j, sync, kernel_ms,
-                       L.q_ids ? L.q_ids + j : nullptr, L.skip ? L.skip + j : nullptr);
+  return search_on_ctx(c, L.rows.from(L.plain, (size_t)dim * es, L.k), L.nq - L.plain, L.k, L.ef, L.filter, sync, kernel_ms);
 }
 
 int Index::make_filter_bits(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx,

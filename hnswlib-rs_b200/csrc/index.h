@@ -245,23 +245,38 @@ struct LabelSets {
   std::vector<uint64_t> range;
 };
 
-// One host search batch: flat queries or one pointer per query (rows), k answers each into `out`.  `exact`: the exact
-// scan of the points each row may return (ef unused) instead of the graph search.  By stored point: query i is the
-// stored vector of qids[i] (an insertion rank; a partitioned handle's global one), and with exclude_self its row leaves
-// that point out (write_row, search_core.cuh).  Radius (an exact batch): row i holds only the points within radius[i]
-// (>= 0, not NaN) and reports how many of its points are (out.total).
-struct HostBatch {
+// What each row of a host batch brings in, a column per field (nullptr: absent): its query (flat, a row pointer, or by
+// stored point the stored vector of qids[i], an insertion rank, a partitioned handle's global one); the id it leaves out
+// (skip, ~0: none; qids itself for exclude_self; write_row, search_core.cuh); and in an exact batch the radius it holds
+// the points within (>= 0, not NaN), reporting how many of its points are.  A new column is a field here and in
+// SearchCtx::Rows, a line in sorted_rows and leg_rows (host_search.cu), and an entry in search_host_begin's staging list.
+struct HostRows {
   const void* queries = nullptr;
   const void* const* rows = nullptr;
+  const uint64_t* qids = nullptr;
+  const uint64_t* skip = nullptr;
+  const float* radius = nullptr;
+};
+
+// What each row of a leg takes out (search_host_finish): k answer slots and a count per row, and a radius batch's
+// totals, in the context's pinned result buffer (valid until it is released); rc: 0, or the leg's failure
+struct HostAnswers {
+  const NeighbourOut* slots = nullptr;
+  const int32_t* counts = nullptr;
+  const uint32_t* totals = nullptr;
+  int rc = 0;
+};
+
+// One host search batch: the rows `in`, k answers each into `out`.  `exact`: the exact scan of the points each row may
+// return (ef unused) instead of the graph search.
+struct HostBatch {
+  HostRows in;
   size_t nq = 0;
   int d = 0;
   size_t k = 0, ef = 0;
   Restriction restriction;
-  AnswerArrays out;
   bool exact = false;
-  const uint64_t* qids = nullptr;
-  bool exclude_self = false;
-  const float* radius = nullptr;
+  AnswerArrays out;
 };
 
 // A leg's restriction (Index::resolve): its rows [0, plain) are unrestricted, and `runs` cover the rest, each a range of
@@ -337,25 +352,18 @@ class Index {
   int import_graph(const void* vecs, size_t n_new, int d, const uint64_t* origin, const uint8_t* levels,
                    int64_t entry_id, int nlayers, const uint64_t* const* offsets, const uint32_t* const* ids,
                    const float* const* dists);
-  // host queries (flat or row pointers) on leased context c under the leg's plan, answers left in the context's pinned
-  // buffer (valid until it is released)
-  // By stored point (qids, insertion ranks of this Index, instead of queries and rows), and with skip[i] the id row i
-  // leaves out (~0: none; skip may be qids itself).  An exact plan with radii: row i within radius[i], and its count of
-  // points within the radius left in the pinned buffer next to the counts.
-  int search_host_begin(int c, const void* queries, const void* const* rows, const uint64_t* qids, const uint64_t* skip,
-                        size_t nq, int d, size_t k, size_t ef, const LegPlan& plan, const float* radius = nullptr);
-  int search_host_finish(int c, const NeighbourOut** out, const int32_t** counts, const uint32_t** totals = nullptr);
+  // the rows `in` of one leg (by stored point: ranks of this Index) on leased context c under the leg's plan, answers
+  // left in the context's pinned buffer
+  int search_host_begin(int c, const HostRows& in, size_t nq, int d, size_t k, size_t ef, const LegPlan& plan);
+  HostAnswers search_host_finish(int c);
   // host search batches (host_search.cu): synchronous, or submitted now and collected by finish_batch.  A ticket is a
-  // batch planned into legs, with what the legs read until they are collected: a per-row batch's caller row of each
+  // batch `b` planned into legs, with what the legs read until they are collected: a per-row batch's caller row of each
   // sorted row (out.perm) and its sorted rows, a FilterT's host bits per partition, and a label-set batch's sets.
   struct Ticket {
     std::vector<Leg> legs;
-    size_t k = 0;
-    AnswerArrays out;
+    HostBatch b;
     std::vector<size_t> perm;
-    std::vector<const void*> rows;
-    std::vector<uint64_t> qids;  // a per-row batch by stored point: the ids in sorted-row order
-    std::vector<float> radius;   // a per-row radius batch: the radii in sorted-row order
+    std::vector<unsigned char> rows;      // a per-row batch: its HostRows columns in sorted-row order
     std::vector<unsigned char> gathered;  // a partitioned batch by stored point: the query rows read from their partitions
     std::vector<std::vector<uint32_t>> bits;
     LabelSets sets;
@@ -411,12 +419,9 @@ class Index {
   // exact-scan order (rebuilt when a column it is keyed on changed): per label of the set, its group, narrowed to the
   // range by binary search in a value-keyed order; slices that follow each other in the order are joined.
   int scan_slices(const uint32_t* set, size_t nset, uint64_t lo, uint64_t hi, std::vector<ExactScan>& slices);
-  // device queries in, device answers out; the restriction is none or a resident filter.  `exact`: the exact scan (ef
-  // unused).  By stored point: d_qids (device, insertion ranks) in place of d_queries, each row without its own point
-  // when exclude_self is set.
-  int search_device(const Restriction& rs, bool exact, const void* d_queries, size_t nq, size_t k, size_t ef,
-                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* d_qids = nullptr,
-                    bool exclude_self = false);
+  // the batch b with device rows in and device answers out (b.in: queries, or qids and skip; b.out: nb and counts); the
+  // restriction is none or a resident filter
+  int search_device(const HostBatch& b, bool sync, float* kernel_ms);
   // the stored vectors of ranks[0, n) into out[n][dim], a partitioned handle's global ranks each from its partition (the
   // caller checked the ranks)
   int get_vectors(const uint64_t* ranks, size_t n, void* out) const;
@@ -488,28 +493,36 @@ class Index {
     void *h_pin = nullptr, *h_res = nullptr;  // pinned, mapped: query staging / answers
     size_t h_pin_bytes = 0, h_res_bytes = 0;
     bool busy = false;
-    // The launches of one leg on the context (run_plan): device queries and answers, and the device view of the leg's
-    // plan (stage_plan).  Graph: rows [0, plain) unrestricted, the others under `filter`.  Exact: the rows by the points
-    // they scan.
-    struct Launch {
+    // The per-row device arrays of a launch: queries (by stored point q_ids, stored rows), the id each row leaves out
+    // (skip: the launch searches k + 1), a radius launch's radii and totals, and k answer slots and a count per row
+    struct Rows {
       const void* d_queries = nullptr;
-      size_t nq = 0, k = 0, ef = 0;
+      const uint64_t* q_ids = nullptr;
+      const uint64_t* skip = nullptr;
+      const float* radius = nullptr;
+      uint32_t* totals = nullptr;
       NeighbourOut* out = nullptr;
       int32_t* counts = nullptr;
+      Rows from(size_t j, size_t q_bytes, size_t k) const {  // the same rows from row j on: only present arrays move
+        return {d_queries ? (const char*)d_queries + j * q_bytes : nullptr, q_ids ? q_ids + j : nullptr, skip ? skip + j : nullptr,
+                radius ? radius + j : nullptr, totals ? totals + j : nullptr, out ? out + j * k : nullptr,
+                counts ? counts + j : nullptr};
+      }
+    };
+    // The launches of one leg on the context (run_plan): its rows, and the device view of the leg's plan (stage_plan).
+    // Graph: rows [0, plain) unrestricted, the others under `filter`.  Exact: the rows by the points they scan.
+    struct Launch {
+      Rows rows;
+      size_t nq = 0, k = 0, ef = 0;
       bool exact = false;
       size_t plain = 0;
       LaunchFilter filter;
       std::vector<ExactGroup> groups;
-      const uint64_t* q_ids = nullptr;  // a search by stored point: in place of d_queries
-      const uint64_t* skip = nullptr;   // per row the id it leaves out: the launches search k + 1
-      const float* radius = nullptr;    // exact, radius mode: per row its radius, and where its total goes
-      uint32_t* totals = nullptr;
     };
     struct Pending {  // a host search enqueued by search_host_begin, completed by search_host_finish
       Launch run;
-      NeighbourOut* hout = nullptr;
-      int32_t *hcnt = nullptr, *hstatus = nullptr;
-      uint32_t* htot = nullptr;  // radius mode
+      HostAnswers ans;
+      int32_t* hstatus = nullptr;
       bool enqueued = false;
     } pend;
   };
@@ -590,10 +603,10 @@ class Index {
 
   // ---- host search batches (host_search.cu)
   int plan(size_t nq, std::vector<Leg>& legs);
-  int prepare_batch(const HostBatch& call, HostBatch& b, Ticket& t, bool replicas_first);
+  int prepare_batch(const HostBatch& call, Ticket& t, bool replicas_first);
   void begin_leg(const HostBatch& b, Leg& l);
   void release_leg(Leg& l);
-  int end_leg(Leg& l, size_t k, const AnswerArrays& out);
+  int end_leg(Leg& l, const HostBatch& b);
   int legs_fail(const Leg* legs, size_t n, bool replicas_first);
 
   // ---- exact-scan orders (labels.cu): the internal ids of this Index's points that have what the order is keyed on (a
@@ -637,21 +650,18 @@ class Index {
 
   VisitedPool vis_;  // visited tables of the insert kernel (searches: SearchCtx)
   SearchCtx ctx_[NCTX + NASYNC];
-  // one graph search launch (the filtered kernel when `f` restricts it).  q_ids: the queries are those stored rows;
-  // skip: rows k wide from a search of k + 1 (SearchParams)
-  int search_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, size_t ef_arg, const LaunchFilter& f,
-                    NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* q_ids,
-                    const uint64_t* skip);
-  // the exact k nearest of device queries, each group's rows among that group's points (aux.cu); the slices' scratch is
-  // sized before the launch.  q_ids and skip as search_on_ctx takes them.  Radius mode (radius, device, per row): only
-  // the points within each row's radius, and their number per row into the device array totals.
-  int exact_on_ctx(SearchCtx& c, const void* d_queries, size_t nq, size_t k, const std::vector<ExactGroup>& groups,
-                   NeighbourOut* d_out, int32_t* d_counts, bool sync, float* kernel_ms, const uint64_t* q_ids,
-                   const uint64_t* skip, const float* radius = nullptr, uint32_t* totals = nullptr);
+  // one graph search launch of rows [0, nq) of r (the filtered kernel when `f` restricts it; SearchParams)
+  int search_on_ctx(SearchCtx& c, const SearchCtx::Rows& r, size_t nq, size_t k, size_t ef_arg, const LaunchFilter& f,
+                    bool sync, float* kernel_ms);
+  // the exact k nearest of rows [0, nq) of r, each group's rows among that group's points (aux.cu; the slices' scratch
+  // sized before the launch); radius mode (r.radius): only those within each row's radius, their number into r.totals
+  int exact_on_ctx(SearchCtx& c, const SearchCtx::Rows& r, size_t nq, size_t k, const std::vector<ExactGroup>& groups,
+                   bool sync, float* kernel_ms);
   // the device view of a leg's plan in `run`, with what it needs uploaded into context c
   int stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& run);
-  // the launches of `run` on context c: the unrestricted rows as an ordinary unfiltered launch, then the restricted ones
-  // in one filtered launch (exact: one launch over the groups).  Both share the context's status, so an overflow in either
+  // the launches of `run` on context c, after what they share (the checks, a radius launch's totals zeroed, an empty
+  // index's empty rows): the unrestricted rows as an ordinary unfiltered launch, then the restricted ones in one
+  // filtered launch (exact: one launch over the groups).  Both share the context's status, so an overflow in either
   // re-runs both (sync: growing the tables).
   int run_plan(SearchCtx& c, const SearchCtx::Launch& run, bool sync, float* kernel_ms);
   std::mutex ctx_mu_;
