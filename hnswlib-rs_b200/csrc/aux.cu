@@ -25,13 +25,14 @@ template <class Op, int CH, int U>
 __global__ void __launch_bounds__(256) dist_batch_kernel(AuxParams p) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t wpb = blockDim.x >> 5;  // 8, or fewer for wide rows (cta_shape)
   unsigned char* base = smem_raw + (size_t)warp * p.smem_per_warp;
   uint4* q4 = reinterpret_cast<uint4*>(base);
   uint32_t* cid = reinterpret_cast<uint32_t*>(base + (size_t)p.g.d4 * 16);
   float* cd = reinterpret_cast<float*>(cid + 32);
   const uint4* vec4 = reinterpret_cast<const uint4*>(p.g.vec);
-  const uint32_t wstride = gridDim.x * 8;
-  for (uint32_t qi = blockIdx.x * 8 + warp; qi < p.nq; qi += wstride) {
+  const uint32_t wstride = gridDim.x * wpb;
+  for (uint32_t qi = blockIdx.x * wpb + warp; qi < p.nq; qi += wstride) {
     __syncwarp();
     stage_row_bytes(q4, reinterpret_cast<const char*>(p.queries) + (size_t)qi * p.q_bytes, p.q_bytes, p.g.d4 * 16);
     for (uint32_t b = 0; b < p.m; b += 32) {
@@ -47,13 +48,13 @@ __global__ void __launch_bounds__(256) dist_batch_kernel(AuxParams p) {
 }
 
 template <class Op>
-static cudaError_t launch_dist_batch_for_op(const AuxParams& p, int grid, size_t smem, cudaStream_t st) {
+static cudaError_t launch_dist_batch_for_op(const AuxParams& p, int grid, int threads, size_t smem, cudaStream_t st) {
   const int ch = p.g.d4 / 8;
   if constexpr (Specialise<Op>::value) {
-    if (ch == 1) return launch_kernel(dist_batch_kernel<Op, 1, 4>, p, grid, 256, smem, st, nullptr);
-    if (ch == 4) return launch_kernel(dist_batch_kernel<Op, 4, 2>, p, grid, 256, smem, st, nullptr);
+    if (ch == 1) return launch_kernel(dist_batch_kernel<Op, 1, 4>, p, grid, threads, smem, st, nullptr);
+    if (ch == 4) return launch_kernel(dist_batch_kernel<Op, 4, 2>, p, grid, threads, smem, st, nullptr);
   }
-  return launch_kernel(dist_batch_kernel<Op, 0, 2>, p, grid, 256, smem, st, nullptr);
+  return launch_kernel(dist_batch_kernel<Op, 0, 2>, p, grid, threads, smem, st, nullptr);
 }
 
 // ------------------------------------------------------------------------------------------------ exact k-NN scan
@@ -397,6 +398,12 @@ int Index::dist_batch(const void* queries, size_t nq, int d, const uint32_t* can
   if (d != dim) return fail("query length differs from the index dimension");
   for (size_t i = 0; i < nq * m; ++i)
     if (cand[i] >= n) return fail("candidate id out of range");
+  // 8 warps (one query each) per CTA, fewer when 8 query rows do not fit the shared-memory budget
+  const int smem_per_warp = (int)(row_bytes + 256);  // [query row][32 candidate ids][32 distances]
+  const CtaShape cta = cta_shape((size_t)smem_per_warp, 8);
+  if (!cta.warps)
+    return fail("dimension too large for dist_batch: one query row needs " + std::to_string(smem_per_warp) +
+                " bytes of shared memory (limit 220 KB)");
   HB_CUDA(cudaSetDevice(device));
   DevBuf dq, dc, dout;
   HB_CUDA(cudaMalloc(&dq.p, nq * d * es));
@@ -412,11 +419,10 @@ int Index::dist_batch(const void* queries, size_t nq, int d, const uint32_t* can
   p.cand = (const uint32_t*)dc.p;
   p.m = (uint32_t)m;
   p.out = (float*)dout.p;
-  p.smem_per_warp = p.g.d4 * 16 + 256;
-  const size_t smem = (size_t)p.smem_per_warp * 8;
-  const int grid = (int)std::min<size_t>((size_t)sm_count_ * 8, (nq + 7) / 8);
+  p.smem_per_warp = smem_per_warp;
+  const int grid = (int)std::min<size_t>((size_t)sm_count_ * 8, (nq + cta.warps - 1) / cta.warps);
   HB_CUDA(dispatch_op(metric, dtype, [&](auto tag) -> cudaError_t {
-    return launch_dist_batch_for_op<typename decltype(tag)::type>(p, grid, smem, stream_);
+    return launch_dist_batch_for_op<typename decltype(tag)::type>(p, grid, cta.warps * 32, cta.smem, stream_);
   }));
   HB_CUDA(cudaMemcpyAsync(out, dout.p, nq * m * 4, cudaMemcpyDeviceToHost, stream_));
   HB_CUDA(cudaStreamSynchronize(stream_));

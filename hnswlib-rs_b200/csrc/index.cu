@@ -311,19 +311,6 @@ int Index::grow_plevel(uint32_t id, int new_pl) {
   return 0;
 }
 
-// Launch shape for a kernel built for up to `max_warps` warps per CTA: fewer warps when one warp's share of shared
-// memory is large (wide rows, big ef).  warps == 0: a single warp does not fit.
-struct CtaShape {
-  int warps;
-  size_t smem;
-};
-static CtaShape cta_shape(size_t smem_per_warp, int max_warps) {
-  int w = max_warps;
-  while (w > 1 && smem_per_warp * w > SMEM_BUDGET) w >>= 1;
-  if (smem_per_warp * w > SMEM_BUDGET) return {0, 0};
-  return {w, smem_per_warp * w};
-}
-
 // the insert kernel's queue (it is built for the 128 / 256-slot queues and the generic one only) and shared memory
 Index::InsertShape Index::insert_shape() const {
   InsertShape s;

@@ -230,6 +230,19 @@ inline size_t query_smem_per_warp(QueryKernel kind, int d4, int q_smem) {
 }
 inline int query_threads(QueryKernel kind) { return kind == QueryKernel::Lean ? LEAN_THREADS : SEARCH_THREADS; }
 
+// Launch shape for a kernel built for up to `max_warps` warps per CTA: fewer warps when one warp's share of shared
+// memory is large (wide rows, big ef).  warps == 0: a single warp does not fit.
+struct CtaShape {
+  int warps;
+  size_t smem;
+};
+inline CtaShape cta_shape(size_t smem_per_warp, int max_warps) {
+  int w = max_warps;
+  while (w > 1 && smem_per_warp * w > SMEM_BUDGET) w >>= 1;
+  if (smem_per_warp * w > SMEM_BUDGET) return {0, 0};
+  return {w, smem_per_warp * w};
+}
+
 struct InsertParams {
   GraphView g;
   uint32_t first;   // internal id of the first point of the batch

@@ -228,22 +228,3 @@ def test_submit_wait_pipelines_batches(pkg, po):
     for a, b in zip(want[0], res):
         assert np.array_equal(a, b)                               # the ticket saw the index as it was at submit time
 
-
-def test_very_wide_rows_run_with_fewer_warps_per_block(pkg, po):
-    """d = 7000 f32 (28 KB per row): 8 warps' worth of query rows no longer fit one block's shared memory; the kernels run
-    fewer warps per block instead of failing (ADVICE r1), and the answers still equal the oracle's"""
-    n, d = 400, 7000
-    X = pkg.datagen.uniform(n, d, 1)
-    o = po.Oracle(8, n, 16, 40, "DistL2", d, mode=po.MODE_DET, order=po.ORDER_GPU)
-    lv = o.draw_levels(n)
-    o.insert_batch(X, levels=lv)
-    h = pkg.Hnsw(8, n, 16, 40, "DistL2")
-    h.set_insert_batching(1 << 30, 1)
-    h.insert_flat(X, levels=lv)
-    for a, b in zip(h.export_layer(0)[:2], o.export_layer(0)[:2]):   # (above layer 0 the oracle also keeps never-read lists)
-        assert np.array_equal(a, b)
-    Q = pkg.datagen.uniform(40, d, 2)
-    go, gd, gi, _, gc = h.search_flat(Q, 5, 32)
-    oo, od, oi, _, oc = o.search_batch(Q, 5, 32)
-    assert np.array_equal(gi, oi) and np.array_equal(gd.view(np.uint32), od.view(np.uint32))
-    assert pkg.load_library().hnsw_b200_get_extend_candidates(h._h) == 0

@@ -243,7 +243,9 @@ def test_probability_metric_kernels(pkg, po, metric):
 
 
 # ---------------------------------------------------------------- distances against the float64 formulas
-GPU_DIMS = [1, 3, 15, 17, 33, 100, 129, 257]    # f32 rows of 128 (CH 1), 256, 512 (CH 4) and more bytes
+# f32 rows of 128 (CH 1), 256, 512 (CH 4) and more bytes; 7201 and 28801 are rows too wide for 8 warps of dist_batch
+# (every element type at 28801: f32 4 warps at 7201 and 1 at 28801, u16 2 and u8 4 at 28801)
+GPU_DIMS = [1, 3, 15, 17, 33, 100, 129, 257, 7201, 28801]
 LOG_METRICS = ("DistJeffreys", "DistJensenShannon")
 DIST_CASES = [(dt, m) for dt in (np.float32, np.uint8, np.uint16, np.uint32, np.int32)
               for m in distref.F32_METRICS + ["DistHamming", "DistJaccard"] if distref.supported(dt, m)]
