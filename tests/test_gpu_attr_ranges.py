@@ -10,11 +10,10 @@ import tempfile
 import numpy as np
 import pytest
 
-from test_gpu_exact import expected
-from test_gpu_label_sets import free, unrestricted
-from test_gpu_labels import GRAPH_CASES, NONE, point_labels
-from test_gpu_matrix import data, same
-from test_gpu_per_query_filter import N, build, origin_ids, per_group, rows_of, stats_sum
+from answers import per_group, same, same_as_single_filter_calls
+from exactref import expected, origin_ids
+from graphs import data
+from restrict import GRAPH_CASES, NONE, N, build, free, point_labels, unrestricted
 
 pytestmark = pytest.mark.gpu
 
@@ -77,27 +76,9 @@ def test_rows_equal_filter_calls(pkg, po, dtype, metric, d):
     sel = np.random.default_rng(d).integers(0, len(ROWS), len(Q))
     rg, qs = args(sel)
     g = selector(sel)
-    for tie in (0, 1):   # tie mode 1 changes the kernel of the unrestricted rows only
-        h.set_tie_mode(tie)
-        for k, ef in ((1, 1), (10, 64), (40, 257)):
-            what = f"tie={tie} k={k} ef={ef}"
-            single = lambda q, rf: h.search_flat(q, k, ef, filter=rf)   # noqa: E731
-            want = per_group(single, Q, g, rfs, None)
-            same(h.search_flat_ranges(Q, k, ef, rg, qs), want, what)
-            h.enable_stats(True)
-            h.get_stats()
-            got = h.search_flat_ranges(Q, k, ef, rg, qs)
-            s_rng = h.get_stats()
-            parts = []
-            for j in np.unique(g):
-                single(Q[rows_of(g, j)], None if j < 0 else rfs[j])
-                parts.append(h.get_stats())
-            h.enable_stats(False)
-            same(got, want, what + " stats on")
-            assert s_rng == stats_sum(parts), (what, s_rng, parts)
-        for k in (1, 10):
-            same(h.search_exact_ranges(Q, k, rg, qs),
-                 per_group(lambda q, rf: h.search_exact(q, k, filter=rf), Q, g, rfs, None), f"tie={tie} exact k={k}")
+    # tie mode 1 changes the kernel of the unrestricted rows only
+    same_as_single_filter_calls(h, Q, g, rfs, lambda k, ef: h.search_flat_ranges(Q, k, ef, rg, qs),
+                                lambda k: h.search_exact_ranges(Q, k, rg, qs))
     free(rfs)
 
 
@@ -113,10 +94,10 @@ def test_ranges_without_sets(pkg, po):
     sel = np.arange(len(Q)) % len(rows)
     rg, _ = args(sel, rows)
     g = selector(sel, rows)
-    same(h.search_flat_ranges(Q, 10, 64, rg), per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs, None),
+    same(h.search_flat_ranges(Q, 10, 64, rg), per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs),
          "graph")
     same(h.search_exact_ranges(Q, 10, [tuple(r) for r in rg]),
-         per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs, None), "exact, pairs")
+         per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs), "exact, pairs")
     free(rfs)
 
 
@@ -162,9 +143,9 @@ def test_every_row_its_own_window(pkg, po):
     rg, qs = args(sel, rows)
     g = selector(sel, rows)
     assert np.all(g >= 0) and len(np.unique(g)) == len(Q)
-    same(h.search_flat_ranges(Q, 10, 64, rg, qs), per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs, None),
+    same(h.search_flat_ranges(Q, 10, 64, rg, qs), per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs),
          "graph")
-    same(h.search_exact_ranges(Q, 10, rg, qs), per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs, None),
+    same(h.search_exact_ranges(Q, 10, rg, qs), per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs),
          "exact")
     free(rfs)
 
@@ -194,7 +175,7 @@ def test_overflow_grows_and_reruns(pkg, po):
     assert first["evals"] > again["evals"] and first["queries"] > again["queries"], (first, again)
     with h.make_filter(og[[5, 9000, 19999]]) as three, h.make_filter(np.sort(og[attr < 500])) as half:
         sel = np.arange(len(Q)) % 3 - 1
-        same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, [three, half], 10), "overflow")
+        same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, [three, half]), "overflow")
     assert np.all(got[4][1::3] <= 3)
 
 
@@ -218,8 +199,8 @@ def test_attributes_follow_inserts_and_changes(pkg, po):
 
     def check(lab, attr, what):
         rfs = filters_for(h, lab, attr, og[: len(lab)], rows)
-        want = per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs, 10)
-        want_x = per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs, 10)
+        want = per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs)
+        want_x = per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs)
         got, got_x = h.search_flat_ranges(Q, 10, 64, rg, qs), h.search_exact_ranges(Q, 10, rg, qs)
         same(got, want, what)
         same(got_x, want_x, what + ", exact")
@@ -276,9 +257,9 @@ def test_partitioned_handle_and_view(pkg, po, P):
     rg, qs = args(sel)
     g = selector(sel)
     got = h.search_flat_ranges(Q, 10, 64, rg, qs)
-    same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs, None), f"P={P} graph")
+    same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs), f"P={P} graph")
     assert np.all(got[2][got[2] != NONE] < N)   # global ranks
-    same(h.search_exact_ranges(Q, 10, rg, qs), per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs, None),
+    same(h.search_exact_ranges(Q, 10, rg, qs), per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs),
          f"P={P} exact")
     free(rfs)
     v = h.partition_view(1)

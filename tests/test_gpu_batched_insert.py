@@ -5,7 +5,7 @@ A of a batch (insert_search_kernel) searches the graph as it stood when the batc
 files the back-links under per-point locks; DESIGN.md §4.3 argues the result is deterministic.  pyoracle's
 insert_batched restates those semantics, so every batched build here must equal it exactly:
   * entry point, levels, ranks and origins equal, every materialised list equal, layer-0 link distances bit-equal
-    (test_gpu_matrix.assert_same_graph);
+    (graphs.assert_same_graph);
   * the insert path's traversal counters `expansions` and `adj_read` equal the oracle's.  `evals` is not compared: the
     kernel does not count dist_to_entry (hnsw.rs:1110-1112) or the recompute at hnsw.rs:1146, and it evaluates every
     kept neighbour of a selection step at once, where the oracle stops at the first one that rejects the candidate.
@@ -18,7 +18,6 @@ partitions building concurrently on one device; the row-pointer upload across it
 c2 graph at full size.  test_zz_every_insert_kernel_ran_batched checks that every compiled insert_search_kernel entry
 point ran in a bit-exact case of this module.
 """
-import os
 import re
 import subprocess
 import time
@@ -26,8 +25,10 @@ import time
 import numpy as np
 import pytest
 
-from batched import engine_batches, entry_level_after, promoting_levels
-from test_gpu_matrix import CASES, INSERT_CASES, LOG_METRICS, assert_same_graph, case_id, cuobjdump, data, same
+from answers import same
+from batched import engine_batches, promoting_levels
+from graphs import (CASES, INSERT_CASES, LOG_METRICS, NTH, State, assert_same_graph, case_id, cuobjdump, data,
+                    insert_both, make_engine, make_oracle)
 from util import oracle_layers
 
 pytestmark = pytest.mark.gpu
@@ -35,54 +36,8 @@ pytestmark = pytest.mark.gpu
 T0 = time.time()
 LEDGER = set()   # insert_search_kernel instantiations that ran in a case compared bit for bit
 DONE = []        # ids of the cases that ran to the end
-N, M, NTH = 1000, 8, os.cpu_count() or 8
+N, M = 1000, 8
 STALE = (1, 1 << 30)   # every batch as large as the graph before it
-
-
-def make_oracle(po, dtype, metric, d, M, efc, n, extend=False, keep_pruned=False):
-    o = po.Oracle(M, n, 16, efc, metric, d, dtype=dtype, mode=po.MODE_DET, order=po.ORDER_GPU)
-    o.set_extend_candidates(extend)
-    o.set_keeping_pruned(keep_pruned)
-    return o
-
-
-def make_engine(pkg, dtype, metric, M, efc, n, sched=None, extend=False, keep_pruned=False, link_mode=0):
-    h = pkg.Hnsw(M, n, 16, efc, metric, dtype=dtype)
-    h.set_extend_candidates(extend)
-    h.set_keeping_pruned(keep_pruned)
-    h.set_link_mode(link_mode)
-    if sched is not None:
-        h.set_insert_batching(*sched)
-    return h
-
-
-class State:
-    """the handle's point count and entry level, which the next call's schedule starts from"""
-
-    def __init__(self):
-        self.n, self.top = 0, -1
-
-    def batches(self, levels, sched=None):
-        out = engine_batches(self.n, self.top, levels, *(sched or ()))
-        self.top = entry_level_after(self.n, self.top, levels)
-        self.n += len(levels)
-        return out
-
-
-def insert_both(pkg, h, o, X, levels, st, sched=None, ids=None, link_mode=0, record=True):
-    """one insert call on the engine (stats on) and the same call, batch for batch, on the oracle; the counters equal"""
-    o.counters()
-    o.insert_batched(X, ids=ids, levels=levels, batches=st.batches(levels, sched), nthreads=NTH, link_mode=link_mode)
-    co = o.counters()
-    h.enable_stats(True)
-    h.get_stats()
-    h.insert_flat(X, ids=ids, levels=levels)
-    if record:
-        LEDGER.add(pkg.last_kernel())
-    cg = h.get_stats()
-    h.enable_stats(False)
-    for key in ("expansions", "adj_read"):
-        assert cg[key] == co[key], ("insert", key, cg, co)
 
 
 def same_with_counters(h, o, Q, k, ef, what):
@@ -106,7 +61,7 @@ def prob_data(n, d, seed):
 def build_and_search(pkg, po, dtype, metric, d, efc, X, levels, sched=None, n=N):
     o = make_oracle(po, dtype, metric, d, M, efc, n)
     h = make_engine(pkg, dtype, metric, M, efc, n, sched)
-    insert_both(pkg, h, o, X, levels, State(), sched)
+    insert_both(pkg, h, o, X, levels, State(), sched, ledger=LEDGER)
     assert_same_graph(h, o, n)
     Q = X[::10][:100].copy() if metric == "DistHellinger" else data(dtype, metric, 100, d, d + 100)
     Q[:10] = X[:10]
@@ -153,7 +108,7 @@ def test_long_lists(pkg, po, M2, efc):
     lv = promoting_levels(po, n, M2)
     o = make_oracle(po, np.float32, "DistL2", d, M2, efc, n)
     h = make_engine(pkg, np.float32, "DistL2", M2, efc, n, STALE)
-    insert_both(pkg, h, o, X, lv, State(), STALE)
+    insert_both(pkg, h, o, X, lv, State(), STALE, ledger=LEDGER)
     assert_same_graph(h, o, n)
     assert int(np.diff(h.export_layer(0)[0].astype(np.int64)).max()) > 32
     DONE.append(f"long-{M2}-{efc}")
@@ -166,7 +121,7 @@ def test_extend_candidates_and_keep_pruned(pkg, po, sched):
     lv = promoting_levels(po, N, 21)
     o = make_oracle(po, np.float32, "DistL2", d, M, efc, N, extend=True, keep_pruned=True)
     h = make_engine(pkg, np.float32, "DistL2", M, efc, N, sched, extend=True, keep_pruned=True)
-    insert_both(pkg, h, o, X, lv, State(), sched)
+    insert_both(pkg, h, o, X, lv, State(), sched, ledger=LEDGER)
     assert_same_graph(h, o, N)
     DONE.append(f"ext-kp-{sched}")
 
@@ -178,7 +133,7 @@ def test_link_mode1(pkg, po, sched):
     lv = promoting_levels(po, N, 22)
     o = make_oracle(po, np.float32, "DistL2", d, M, efc, N)
     h = make_engine(pkg, np.float32, "DistL2", M, efc, N, sched, link_mode=1)
-    insert_both(pkg, h, o, X, lv, State(), sched, link_mode=1)
+    insert_both(pkg, h, o, X, lv, State(), sched, link_mode=1, ledger=LEDGER)
     assert_same_graph(h, o, N)
     DONE.append(f"mode1-{sched}")
 
@@ -190,9 +145,9 @@ def test_link_mode_switch_between_calls(pkg, po):
     o = make_oracle(po, np.float32, "DistL2", d, M, efc, N)
     h = make_engine(pkg, np.float32, "DistL2", M, efc, N)
     st = State()
-    insert_both(pkg, h, o, X[:half], lv[:half], st)
+    insert_both(pkg, h, o, X[:half], lv[:half], st, ledger=LEDGER)
     h.set_link_mode(1)
-    insert_both(pkg, h, o, X[half:], lv[half:], st, ids=np.arange(half, N), link_mode=1)
+    insert_both(pkg, h, o, X[half:], lv[half:], st, ids=np.arange(half, N), link_mode=1, ledger=LEDGER)
     assert_same_graph(h, o, N)
     DONE.append("mode-switch")
 
@@ -208,7 +163,7 @@ def test_incremental_calls_and_capacity_growth(pkg, po):
     h = make_engine(pkg, np.float32, "DistL2", M, efc, 16)
     st, pos = State(), 0
     for sz in (1, 1, 3, 50, 700, 1, 2000, 2244):
-        insert_both(pkg, h, o, X[pos:pos + sz], lv[pos:pos + sz], st, ids=np.arange(pos, pos + sz))
+        insert_both(pkg, h, o, X[pos:pos + sz], lv[pos:pos + sz], st, ids=np.arange(pos, pos + sz), ledger=LEDGER)
         pos += sz
     assert pos == n and h.get_nb_point() == n
     assert_same_graph(h, o, n)
@@ -231,7 +186,7 @@ def test_batched_insert_into_imported_graph(pkg, po):
     st.n, st.top = n0, int(lv0[src.entry])
     lv1 = np.minimum(promoting_levels(po, n1, 43), int(lv0.max()))
     lv1[700] = int(lv0.max()) + 1   # one promotion in the middle of the call
-    insert_both(pkg, h, o, X[n0:], lv1, st, ids=np.arange(n0, n0 + n1))
+    insert_both(pkg, h, o, X[n0:], lv1, st, ids=np.arange(n0, n0 + n1), ledger=LEDGER)
     assert_same_graph(h, o, n0 + n1)
     DONE.append("imported")
 
@@ -252,7 +207,7 @@ def test_layer_mask_per_point(pkg, po):
     assert 311 in starts and 330 in starts and 320 not in starts
     o = make_oracle(po, np.float32, "DistL2", d, M, efc, n)
     h = make_engine(pkg, np.float32, "DistL2", M, efc, n)
-    insert_both(pkg, h, o, X, lv, State())
+    insert_both(pkg, h, o, X, lv, State(), ledger=LEDGER)
     assert_same_graph(h, o, n)
     DONE.append("masks")
 

@@ -8,7 +8,7 @@ candidate buffer from it.  Those shapes arise only with wide rows or a large ef 
 the host's choice (stage_bytes, the per-warp layouts, the queue kinds, cta_shape) and for every launch:
   * checks that the kernel was of the expected family, with warps x 32 threads and warps x the layout's bytes;
   * compares every answer with the oracle (ids, distance bits, PointIds, counts, and the traversal counters with stats
-    on), and with float64 (test_gpu_exact_shapes.F64): each returned distance within its bound and, where the search is
+    on), and with float64 (exactref.F64): each returned distance within its bound and, where the search is
     exhaustive (fewer points than ef), no returned point beyond the float64 k-th nearest plus both bounds;
   * compares every GPU build with the oracle's: serial with its MODE_DET build, batched with its batch-synchronous one.
 It also checks the largest ef / ef_construction / dimension that one warp fits, the refusal one step past it, and
@@ -21,9 +21,9 @@ import pytest
 import scipy.sparse
 import scipy.sparse.csgraph
 
-from test_gpu_batched_insert import State, insert_both, make_engine, make_oracle
-from test_gpu_exact_shapes import F64, check_f64
-from test_gpu_matrix import assert_same_graph, data, same
+from answers import same
+from exactref import F64, check_f64, d4_of
+from graphs import State, assert_same_graph, data, insert_both, make_engine, make_oracle
 from util import oracle_layers
 
 pytestmark = pytest.mark.gpu
@@ -41,11 +41,6 @@ MAX_WARPS = {"generic": 8, "filtered": 8, "std": 8, "insert": 4, "dist": 8}   # 
 KERNEL = {"generic": "search_kernel", "filtered": "search_filter_kernel", "std": "search_std_kernel",
           "insert": "insert_search_kernel", "dist": "dist_batch_kernel"}
 COMMON = ("DistL1", "DistL2", "DistDot", "DistCosine")
-
-
-def d4_of(d, dtype):
-    """16-byte units of a stored row: dim * element size rounded up to whole 128-byte lines (Index::row_bytes / 16)"""
-    return (d * np.dtype(dtype).itemsize + 127) // 128 * 8
 
 
 def round128(b):
@@ -349,7 +344,7 @@ def builds(pkg, po, dtype, metric, X, M, efc, warps, extend=False, keep_pruned=F
     assert_same_graph(h, o, n)
     ob = make_oracle(po, dtype, metric, d, M, efc, n, extend, keep_pruned)
     hb = make_engine(pkg, dtype, metric, M, efc, n, None, extend, keep_pruned)
-    insert_both(pkg, hb, ob, X, levels, State(), record=False)
+    insert_both(pkg, hb, ob, X, levels, State())
     check_launch(pkg, "insert", d4, metric, dtype, efc, M, what=f"{what} batched", warps=warps)
     assert_same_graph(hb, ob, n)
     hb.close()

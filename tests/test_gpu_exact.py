@@ -9,62 +9,16 @@ import numpy as np
 import pytest
 import torch  # device buffers; imported first, so that torch's own NCCL is the one the library binds at run time
 
-from test_gpu_matrix import data, same
-from test_gpu_resident_filter import device_answers, same_host_device
+from answers import device_answers, same, same_host_device
+from exactref import EXACT_CASES, INVALID, expected, filter_sets, handle, origin_ids
+from graphs import case_id, data
 
 pytestmark = pytest.mark.gpu
 
 N, NQ, M = 1500, 40, 8
-INVALID = 0xFFFFFFFF
 
 
-def origin_ids(n):
-    return np.arange(n, dtype=np.uint64) * 5 + 2   # distinct from the internal ids, so a mix-up shows
-
-
-def handle(pkg, X, metric, ids=None):
-    """the points X stored in internal-id order (no graph: the exact search does not read one)"""
-    n = len(X)
-    h = pkg.Hnsw(M, n, 16, 48, metric, dtype=X.dtype)
-    h.import_graph(X, origin_ids(n) if ids is None else ids, np.zeros(n, np.uint8), 0,
-                   [(np.zeros(n + 1, np.uint64), np.zeros(0, np.uint32), None)])
-    return h
-
-
-def expected(po, h, X, Q, k, metric, adm):
-    """the oracle's exact k nearest among X[adm], as search_exact reports them on handle h"""
-    lv, rk, og, _ = h.export_points()
-    nq = len(Q)
-    o = np.full((nq, k), np.iinfo(np.uint64).max, np.uint64)
-    d = np.full((nq, k), np.inf, np.float32)
-    it = np.full((nq, k), INVALID, np.uint32)
-    pid = np.full((nq, k, 2), -1, np.int32)
-    c = min(k, len(adm))
-    if c:
-        ti, td = po.bruteforce(X[adm], Q, k, metric, po.ORDER_GPU)
-        g = adm[ti[:, :c].astype(np.int64)]
-        it[:, :c], o[:, :c], d[:, :c] = g, og[g], td[:, :c]
-        pid[:, :c, 0], pid[:, :c, 1] = lv[g], rk[g]
-    return o, d, it, pid, np.full(nq, c, np.int32)
-
-
-def filter_sets(n, seed):
-    """internal ids admitted: none, one, three, ~5 %, ~50 %, all"""
-    rng = np.random.default_rng(seed)
-    return {"0": np.zeros(0, np.int64), "1": np.array([n // 2]), "3": np.array([0, n // 3, n - 1]),
-            "5%": np.sort(rng.choice(n, n // 20, replace=False)), "50%": np.sort(rng.choice(n, n // 2, replace=False)),
-            "all": np.arange(n)}
-
-
-CASES = ([(np.float32, m, d, False) for m in ("DistL1", "DistL2", "DistDot", "DistCosine") for d in (24, 48, 100, 150)]
-         + [(np.uint8, m, 100, False) for m in ("DistL1", "DistL2", "DistHamming", "DistJaccard")]
-         + [(np.uint16, m, 200, False) for m in ("DistL1", "DistL2", "DistHamming", "DistJaccard")]
-         + [(np.uint32, "DistJaccard", 24, False), (np.int32, "DistL2", 24, False)]
-         + [(np.float32, "DistL2", 24, True), (np.float32, "DistCosine", 100, True)])
-
-
-@pytest.mark.parametrize("dtype,metric,d,ties", CASES,
-                         ids=[f"{np.dtype(c[0]).name}-{c[1]}-d{c[2]}" + ("-ties" if c[3] else "") for c in CASES])
+@pytest.mark.parametrize("dtype,metric,d,ties", EXACT_CASES, ids=[case_id(c) for c in EXACT_CASES])
 def test_exact_equals_oracle(pkg, po, dtype, metric, d, ties):
     X = data(dtype, metric, N, d, d + 3, ties)
     Q = data(dtype, metric, NQ, d, d + 103)

@@ -8,7 +8,9 @@ entries of the Neighbour_api answers, and the traversal counters of get_stats.""
 import numpy as np
 import pytest
 
-from test_gpu_matrix import data, same
+from answers import same
+from exactref import origin_ids
+from graphs import data
 
 pytestmark = pytest.mark.gpu
 
@@ -17,11 +19,7 @@ INV = 0xFFFFFFFF
 CASES = [(np.float32, "DistL2", 24), (np.uint8, "DistHamming", 100)]
 
 
-def origin_ids(n):
-    return np.arange(n, dtype=np.uint64) * 5 + 2   # distinct from the internal ids, so a mix-up shows
-
-
-def handle(pkg, dtype, metric, d, P):
+def inserted_handle(pkg, dtype, metric, d, P):
     X = data(dtype, metric, N, d, d + P)
     h = pkg.Hnsw(M, N, 16, EFC, metric, dtype=dtype)
     if P:
@@ -82,7 +80,7 @@ def twice(h, call):
 @pytest.mark.parametrize("P", [0, 1, 2, 3], ids=["unpartitioned", "P1", "P2", "P3"])
 @pytest.mark.parametrize("dtype,metric,d", CASES, ids=[f"{np.dtype(c[0]).name}-{c[1]}-d{c[2]}" for c in CASES])
 def test_host_paths_agree(pkg, dtype, metric, d, P):
-    h, Q = handle(pkg, dtype, metric, d, P)
+    h, Q = inserted_handle(pkg, dtype, metric, d, P)
     ids = origin_ids(N)
     allow = ids[1::3]
     allowed = set(allow.tolist())

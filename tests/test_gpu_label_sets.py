@@ -7,20 +7,16 @@ and with statistics on the counters equal the sum over those calls.  A set of on
 import numpy as np
 import pytest
 
-from test_gpu_exact import expected
-from test_gpu_labels import GRAPH_CASES, NONE, point_labels
-from test_gpu_matrix import data, same
-from test_gpu_per_query_filter import N, build, origin_ids, per_group, rows_of, stats_sum
+from answers import per_group, same, same_as_single_filter_calls
+from exactref import expected, origin_ids
+from graphs import data
+from restrict import GRAPH_CASES, NONE, N, build, free, point_labels, unrestricted
 
 pytestmark = pytest.mark.gpu
 
 # point_labels carries 0 (~40 %), 1 (~30 %), 2, 7 (one point) and 8 (three points); 99 no point carries.  Sets out of
 # order, with repeats, empty, and [NONE] with a repeat.
 SETS = [[0, 1], [2, 7], [8, 2, 8], [7], [1, 99], [99], [], [NONE], [NONE, NONE], [2, 1, 0, 7, 8], [8, 7], [1, 0]]
-
-
-def unrestricted(s):
-    return len(s) > 0 and set(s) == {NONE}
 
 
 def filters_for(h, lab, og, sets=SETS):
@@ -31,12 +27,6 @@ def filters_for(h, lab, og, sets=SETS):
 def selector(sets, sel):
     """per_group's selector: -1 for the rows of an unrestricted set"""
     return np.array([-1 if unrestricted(sets[g]) else g for g in sel], np.int64)
-
-
-def free(rfs):
-    for rf in rfs:
-        if rf is not None:
-            rf.free()
 
 
 def row_sets(sel, sets=SETS):
@@ -52,27 +42,9 @@ def test_rows_equal_filter_calls(pkg, po, dtype, metric, d):
     rfs = filters_for(h, lab, og)
     sel = np.random.default_rng(d).integers(0, len(SETS), len(Q))
     qs, g = row_sets(sel), selector(SETS, sel)
-    for tie in (0, 1):   # tie mode 1 changes the kernel of the [LABEL_NONE] rows only
-        h.set_tie_mode(tie)
-        for k, ef in ((1, 1), (10, 64), (40, 257)):
-            what = f"tie={tie} k={k} ef={ef}"
-            single = lambda q, rf: h.search_flat(q, k, ef, filter=rf)   # noqa: E731
-            want = per_group(single, Q, g, rfs, None)
-            same(h.search_flat_label_sets(Q, k, ef, qs), want, what)
-            h.enable_stats(True)
-            h.get_stats()
-            got = h.search_flat_label_sets(Q, k, ef, qs)
-            s_sets = h.get_stats()
-            parts = []
-            for j in np.unique(g):
-                single(Q[rows_of(g, j)], None if j < 0 else rfs[j])
-                parts.append(h.get_stats())
-            h.enable_stats(False)
-            same(got, want, what + " stats on")
-            assert s_sets == stats_sum(parts), (what, s_sets, parts)
-        for k in (1, 10):
-            same(h.search_exact_label_sets(Q, k, qs),
-                 per_group(lambda q, rf: h.search_exact(q, k, filter=rf), Q, g, rfs, None), f"tie={tie} exact k={k}")
+    # tie mode 1 changes the kernel of the [LABEL_NONE] rows only
+    same_as_single_filter_calls(h, Q, g, rfs, lambda k, ef: h.search_flat_label_sets(Q, k, ef, qs),
+                                lambda k: h.search_exact_label_sets(Q, k, qs))
     free(rfs)
 
 
@@ -130,7 +102,7 @@ def test_overflow_grows_and_reruns(pkg, po):
     assert first["evals"] > again["evals"] and first["queries"] > again["queries"], (first, again)
     with h.make_filter(og[[5, 9000, 19999]]) as three, h.make_filter(np.sort(og[lab == 2])) as half:
         sel = np.arange(len(Q)) % 3 - 1
-        same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, [three, half], 10), "overflow")
+        same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, [three, half]), "overflow")
     assert np.all(got[4][1::3] <= 3)
 
 
@@ -150,8 +122,8 @@ def test_sets_follow_inserts_and_relabels(pkg, po):
 
     def check(labels, what):
         rfs = filters_for(h, labels, og[: len(labels)], sets)
-        want = per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs, 10)
-        want_x = per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs, 10)
+        want = per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs)
+        want_x = per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs)
         got, got_x = h.search_flat_label_sets(Q, 10, 64, qs), h.search_exact_label_sets(Q, 10, qs)
         same(got, want, what)
         same(got_x, want_x, what + ", exact")
@@ -192,9 +164,9 @@ def test_partitioned_handle_and_view(pkg, po, P):
     sel = np.random.default_rng(P).integers(0, len(SETS), len(Q))
     qs, g = row_sets(sel), selector(SETS, sel)
     got = h.search_flat_label_sets(Q, 10, 64, qs)
-    same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs, None), f"P={P} graph")
+    same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, g, rfs), f"P={P} graph")
     assert np.all(got[2][got[2] != NONE] < N)   # global ranks
-    same(h.search_exact_label_sets(Q, 10, qs), per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs, None),
+    same(h.search_exact_label_sets(Q, 10, qs), per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, g, rfs),
          f"P={P} exact")
     free(rfs)
     v = h.partition_view(1)

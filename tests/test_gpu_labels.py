@@ -10,23 +10,12 @@ import threading
 import numpy as np
 import pytest
 
-from test_gpu_exact import expected
-from test_gpu_matrix import data, same
-from test_gpu_per_query_filter import N, build, origin_ids, per_group, rows_of, stats_sum
+from answers import per_group, same, same_as_single_filter_calls
+from exactref import expected, origin_ids
+from graphs import data
+from restrict import GRAPH_CASES, NONE, N, build, free, point_labels
 
 pytestmark = pytest.mark.gpu
-
-NONE = 0xFFFFFFFF
-
-
-def point_labels(n, seed):
-    """large labels (0: ~40 %, 1: ~30 %), tiny ones (7: one point, 8: three), the rest without a label"""
-    rng = np.random.default_rng(seed)
-    lab = rng.choice(np.array([0, 0, 0, 0, 1, 1, 1, 2, NONE, NONE], np.uint32), n)
-    lab[lab == 7] = NONE
-    lab[rng.choice(n, 4, replace=False)] = [7, 8, 8, 8]
-    return lab
-
 
 QLABELS = np.array([0, 1, 2, 7, 8, 99, NONE], np.uint32)   # 99: a label no point carries
 
@@ -36,19 +25,9 @@ def filters_for(h, lab, og):
     return [None if L == NONE else h.make_filter(np.sort(og[lab == L])) for L in QLABELS]
 
 
-def reference(h, Q, sel, rfs, call):
-    """the single-filter call on each label's rows, in the batch's row order"""
-    return per_group(lambda q, rf: call(q, rf), Q, np.where(QLABELS[sel] == NONE, -1, sel), rfs, None)
-
-
-def free(rfs):
-    for rf in rfs:
-        if rf is not None:
-            rf.free()
-
-
-GRAPH_CASES = [(np.float32, "DistL2", 128), (np.float32, "DistL2", 100), (np.uint8, "DistHamming", 100),
-               (np.uint16, "DistL1", 100), (np.int32, "DistL2", 24)]
+def selector(sel):
+    """per_group's selector for rows of the labels QLABELS[sel]: -1 for the LABEL_NONE rows"""
+    return np.where(QLABELS[sel] == NONE, -1, sel)
 
 
 @pytest.mark.parametrize("dtype,metric,d", GRAPH_CASES, ids=[f"{np.dtype(c[0]).name}-{c[1]}-d{c[2]}" for c in GRAPH_CASES])
@@ -61,27 +40,9 @@ def test_rows_equal_filter_calls(pkg, po, dtype, metric, d):
     rfs = filters_for(h, lab, og)
     sel = np.random.default_rng(d).integers(0, len(QLABELS), len(Q))
     ql = QLABELS[sel]
-    for tie in (0, 1):   # tie mode 1 changes the kernel of the LABEL_NONE rows only
-        h.set_tie_mode(tie)
-        for k, ef in ((1, 1), (10, 64), (40, 257)):
-            what = f"tie={tie} k={k} ef={ef}"
-            single = lambda q, rf: h.search_flat(q, k, ef, filter=rf)   # noqa: E731
-            want = reference(h, Q, sel, rfs, single)
-            same(h.search_flat_labeled(Q, k, ef, ql), want, what)
-            h.enable_stats(True)
-            h.get_stats()
-            got = h.search_flat_labeled(Q, k, ef, ql)
-            s_lab = h.get_stats()
-            parts = []
-            for g in np.unique(sel):
-                single(Q[rows_of(sel, g)], rfs[g])
-                parts.append(h.get_stats())
-            h.enable_stats(False)
-            same(got, want, what + " stats on")
-            assert s_lab == stats_sum(parts), (what, s_lab, parts)
-        for k in (1, 10):
-            same(h.search_exact_labeled(Q, k, ql), reference(h, Q, sel, rfs, lambda q, rf: h.search_exact(q, k, filter=rf)),
-                 f"tie={tie} exact k={k}")
+    # tie mode 1 changes the kernel of the LABEL_NONE rows only
+    same_as_single_filter_calls(h, Q, selector(sel), rfs, lambda k, ef: h.search_flat_labeled(Q, k, ef, ql),
+                                lambda k: h.search_exact_labeled(Q, k, ql))
     assert np.all(h.search_flat_labeled(Q, 10, 64, np.full(len(Q), 99, np.uint32))[4] == 0)
     free(rfs)
 
@@ -115,8 +76,8 @@ def test_labels_follow_inserts_and_relabels(pkg, po):
     def check(labels, what):
         rfs = [h.make_filter(np.sort(og[: len(labels)][labels == L])) for L in range(3)]
         sel = np.where(ql == NONE, -1, ql.astype(np.int64))
-        want = per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, rfs, 10)
-        want_x = per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, sel, rfs, 10)
+        want = per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, rfs)
+        want_x = per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, sel, rfs)
         got, got_x = h.search_flat_labeled(Q, 10, 64, ql), h.search_exact_labeled(Q, 10, ql)
         same(got, want, what)
         same(got_x, want_x, what + ", exact")
@@ -165,7 +126,7 @@ def test_overflow_grows_and_reruns(pkg, po):
     assert h.check_status() == 0
     with h.make_filter(og[[5, 9000, 19999]]) as three, h.make_filter(np.sort(og[lab == 2])) as half:
         sel = np.arange(len(Q)) % 3 - 1
-        same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, [three, half], 10), "overflow")
+        same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, [three, half]), "overflow")
     assert np.all(got[4][ql == 0] <= 3)
 
 
@@ -185,9 +146,9 @@ def test_partitioned_handle_and_view(pkg, po, P):
     sel = np.random.default_rng(P).integers(0, len(QLABELS), len(Q))
     ql = QLABELS[sel]
     got = h.search_flat_labeled(Q, 10, 64, ql)
-    same(got, reference(h, Q, sel, rfs, lambda q, rf: h.search_flat(q, 10, 64, filter=rf)), f"P={P} graph")
+    same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, selector(sel), rfs), f"P={P} graph")
     assert np.all(got[2][got[2] != NONE] < N)   # global ranks
-    same(h.search_exact_labeled(Q, 10, ql), reference(h, Q, sel, rfs, lambda q, rf: h.search_exact(q, 10, filter=rf)),
+    same(h.search_exact_labeled(Q, 10, ql), per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, selector(sel), rfs),
          f"P={P} exact")
     free(rfs)
     v = h.partition_view(1)

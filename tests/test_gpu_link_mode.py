@@ -14,6 +14,7 @@ rule).
 import numpy as np
 import pytest
 
+from answers import same
 from linkgraph import insert_link_mode1, without_layer0_inlink
 from util import csr_lists, recall_ids
 
@@ -22,7 +23,8 @@ pytestmark = pytest.mark.gpu
 N, M = 1000, 8
 
 
-def data(dtype, metric, n, d, seed):
+def numpy_data(dtype, metric, n, d, seed):
+    """rows from numpy's generator (f32 in [0, 1)), not datagen's as graphs.data draws them"""
     rng = np.random.default_rng(seed)
     dt = np.dtype(dtype)
     if dt == np.float32:
@@ -57,7 +59,8 @@ def engine(pkg, dtype, metric, d, efc, n=N, extend=False, keep_pruned=False):
     return h
 
 
-def assert_same_graph(h, o):
+def assert_same_lists(h, o):
+    """graphs.assert_same_graph's rule, with the link distances of the upper layers compared too"""
     lv, rk, og, entry = h.export_points()
     olv, ork, oog = o.export_points()
     assert entry == o.entry
@@ -72,16 +75,6 @@ def assert_same_graph(h, o):
                 continue
             assert gl[p] == ol[p], (layer, p, gl[p], ol[p])
             assert gd[p] == od[p], ("link distances", layer, p)
-
-
-def same(got, want, what):
-    go, gd, gi, gpid, gc = got
-    oo, od, oi, opid, oc = want
-    assert np.array_equal(gc, oc), f"{what}: counts differ"
-    assert np.array_equal(gi, oi), f"{what}: internal ids differ"
-    assert np.array_equal(go, oo), f"{what}: origin ids differ"
-    assert np.array_equal(gd.view(np.uint32), od.view(np.uint32)), f"{what}: distances are not bit-identical"
-    assert np.array_equal(gpid, opid), f"{what}: PointIds differ"
 
 
 def same_with_counters(h, o, Q, k, ef, what, filt=None):
@@ -112,7 +105,7 @@ SERIAL_CASES = [
                          ids=[f"{np.dtype(c[0]).name}-{c[1]}-d{c[2]}-efc{c[3]}" + ("-ext-kp" if c[4] else "")
                               for c in SERIAL_CASES])
 def test_serial_mode1_build_and_search_equal_oracle(pkg, po, dtype, metric, d, efc, options):
-    X = data(dtype, metric, N, d, d + efc)
+    X = numpy_data(dtype, metric, N, d, d + efc)
     levels = promoting_levels(po, N, d)
     o = oracle(po, dtype, metric, d, efc, extend=options, keep_pruned=options)
     insert_link_mode1(o, X, levels)
@@ -120,8 +113,8 @@ def test_serial_mode1_build_and_search_equal_oracle(pkg, po, dtype, metric, d, e
     h.set_link_mode(1)
     h.insert_flat(X, levels=levels)
     assert h.get_link_mode() == 1
-    assert_same_graph(h, o)
-    Q = data(dtype, metric, 100, d, d + 1)
+    assert_same_lists(h, o)
+    Q = numpy_data(dtype, metric, 100, d, d + 1)
     Q[:10] = X[:10]
     same_with_counters(h, o, Q, 10, 64, "lean")
     same_with_counters(h, o, Q, 10, 129, "generic")
@@ -133,7 +126,7 @@ def test_serial_mode1_build_and_search_equal_oracle(pkg, po, dtype, metric, d, e
 
 def test_mode_switch_between_inserts_equals_oracle(pkg, po):
     d, efc = 24, 200
-    X = data(np.float32, "DistL2", N, d, 5)
+    X = numpy_data(np.float32, "DistL2", N, d, 5)
     levels = promoting_levels(po, N, 5)
     half = N // 2
     o = oracle(po, np.float32, "DistL2", d, efc)
@@ -143,7 +136,7 @@ def test_mode_switch_between_inserts_equals_oracle(pkg, po):
     h.set_link_mode(1)
     insert_link_mode1(o, X[half:], levels[half:])
     h.insert_flat(X[half:], ids=np.arange(half, N), levels=levels[half:])
-    assert_same_graph(h, o)
+    assert_same_lists(h, o)
 
 
 @pytest.mark.parametrize("n,d,kind", [(20000, 25, "uniform"), (20000, 128, "clustered")])
@@ -195,7 +188,7 @@ def test_link_mode_settings(pkg):
 @pytest.mark.parametrize("when", ["before", "after"])
 def test_partitions_build_in_mode1(pkg, po, when):
     P, n, d, efc = 2, 2000, 24, 200
-    X = data(np.float32, "DistL2", n, d, 9)
+    X = numpy_data(np.float32, "DistL2", n, d, 9)
     levels = po.Oracle(M, n, 16, efc, "DistL2", d).draw_levels(n)
     h = pkg.Hnsw(M, n, 16, efc, "DistL2")
     h.set_insert_batching(1 << 30, 1)
@@ -213,13 +206,13 @@ def test_partitions_build_in_mode1(pkg, po, when):
             v.set_link_mode(0)
         o = oracle(po, np.float32, "DistL2", d, efc, n=len(X[p::P]))
         insert_link_mode1(o, X[p::P], levels[p::P], ids=np.arange(p, n, P))
-        assert_same_graph(v, o)
+        assert_same_lists(v, o)
 
 
 def test_mode1_dump_reload_and_insert(tmp_path, pkg, po):
     import dumpfmt
     n, d, efc = 1200, 20, 48
-    X = data(np.float32, "DistL2", n, d, 13)
+    X = numpy_data(np.float32, "DistL2", n, d, 13)
     levels = promoting_levels(po, n, 13)
     h = engine(pkg, np.float32, "DistL2", d, efc)
     h.set_link_mode(1)
@@ -240,7 +233,7 @@ def test_mode1_dump_reload_and_insert(tmp_path, pkg, po):
     # reload: mode 0 (dumps store no mode), same answers
     h2 = pkg.Hnsw.load(tmp_path, "lm1", "DistL2")
     assert h2.get_link_mode() == 0
-    Q = data(np.float32, "DistL2", 100, d, 14)
+    Q = numpy_data(np.float32, "DistL2", 100, d, 14)
     a1, a2 = h.search_flat(Q, 10, 48), h2.search_flat(Q, 10, 48)
     assert np.array_equal(a1[0], a2[0]) and np.array_equal(a1[1].view(np.uint32), a2[1].view(np.uint32))
     # an insert into the reloaded handle in mode 1 equals the oracle's on the same graph
@@ -248,11 +241,11 @@ def test_mode1_dump_reload_and_insert(tmp_path, pkg, po):
     o = po.Oracle(M, n + 50, 16, efc, "DistL2", d, mode=po.MODE_DET, order=po.ORDER_GPU)
     o.import_graph(h2.export_vectors(), og2, lv2, entry2, {l: h2.export_layer(l) for l in range(int(lv2.max()) + 1)})
     o.set_extend_candidates(True)   # a reload turns extend_candidates on (hnswio.rs:510, 599); set it on both explicitly
-    extra = data(np.float32, "DistL2", 50, d, 15)
+    extra = numpy_data(np.float32, "DistL2", 50, d, 15)
     xlev = np.minimum(po.Oracle(M, 50, 16, efc, "DistL2", d, seed=16).draw_levels(50), 2)
     insert_link_mode1(o, extra, xlev, ids=np.arange(7000, 7050))
     h2.set_extend_candidates(True)
     h2.set_insert_batching(1 << 30, 1)
     h2.set_link_mode(1)
     h2.insert_flat(extra, ids=np.arange(7000, 7050), levels=xlev)
-    assert_same_graph(h2, o)
+    assert_same_lists(h2, o)

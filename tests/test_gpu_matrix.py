@@ -14,9 +14,7 @@ points `cuobjdump -symbols` lists for the loaded library and names every compile
 It also covers the visited tables' two rare paths (overflow then grow and re-run; epoch wrap-around with its table clear)
 and checks the device's dist_batch against the float64 formulas of tests/distref.py at every row-chunk size.
 """
-import os
 import re
-import shutil
 import subprocess
 import time
 
@@ -24,7 +22,9 @@ import numpy as np
 import pytest
 
 import distref
-from util import csr_lists, oracle_layers, recall_ids
+from answers import same
+from graphs import CASES, INSERT_CASES, LOG_METRICS, build_both, case_id, cuobjdump, data
+from util import oracle_layers, recall_ids
 
 pytestmark = pytest.mark.gpu
 
@@ -38,82 +38,13 @@ def launched(pkg, result=None):
     return result
 
 
-def same(got, want, what):
-    go, gd, gi, gpid, gc = got
-    oo, od, oi, opid, oc = want
-    assert np.array_equal(gc, oc), f"{what}: counts differ"
-    assert np.array_equal(gi, oi), f"{what}: internal ids differ"
-    assert np.array_equal(go, oo), f"{what}: origin ids differ"
-    assert np.array_equal(gd.view(np.uint32), od.view(np.uint32)), f"{what}: distances are not bit-identical"
-    assert np.array_equal(gpid, opid), f"{what}: PointIds differ"
-
-
-def assert_same_graph(h, o, n):
-    lv, rk, og, entry = h.export_points()
-    olv, ork, oog = o.export_points()
-    assert entry == o.entry
-    assert np.array_equal(lv, olv) and np.array_equal(rk, ork) and np.array_equal(og, oog)
-    for layer in range(0, int(olv.max()) + 1):
-        goff, gids, gds = h.export_layer(layer)
-        ooff, oids, ods = o.export_layer(layer)
-        if layer == 0:
-            assert np.array_equal(goff, ooff) and np.array_equal(gids, oids), "layer 0 differs"
-            assert np.array_equal(gds.view(np.uint32), ods.view(np.uint32)), "layer-0 link distances differ"
-            continue
-        gl, ol = csr_lists(goff, gids), csr_lists(ooff, oids)
-        for p in range(n):
-            if not gl[p] and olv[p] < layer:   # a list no search can reach, which the engine does not store
-                continue
-            assert gl[p] == ol[p], (layer, p, gl[p], ol[p])
-
-
-def data(dtype, metric, n, d, seed, ties=False):
-    rng = np.random.default_rng(seed)
-    dt = np.dtype(dtype)
-    if dt == np.float32:
-        kind = "unit" if metric == "DistDot" else "uniform"
-        import importlib
-        dg = importlib.import_module("hnswlib-rs_b200").datagen
-        if ties:   # every vector stored 4 times: the kernels must order equal distances by id
-            base = dg.make(kind, (n + 3) // 4, d, seed)
-            return np.repeat(base, 4, axis=0)[:n].copy()
-        return dg.make(kind, n, d, seed)
-    hi = {"DistHamming": 3, "DistJaccard": 16 if dt == np.uint8 else 1000}.get(metric)
-    if hi is None:
-        hi = {np.dtype(np.uint8): 256, np.dtype(np.uint16): 5000, np.dtype(np.uint32): 100000}.get(dt, 2000)
-    lo = -hi if dt == np.int32 and metric != "DistHamming" else 0
-    return rng.integers(lo, hi, (n, d)).astype(dt)
-
-
-def build_both(pkg, po, dtype, metric, n, d, M, efc, seed, ties=False, max_elements=None):
-    X = data(dtype, metric, n, d, seed, ties)
-    o = po.Oracle(M, n, 16, efc, metric, d, dtype=dtype, mode=po.MODE_DET, order=po.ORDER_GPU)
-    levels = o.draw_levels(n)
-    o.insert_batch(X, levels=levels)
-    h = pkg.Hnsw(M, max_elements or n, 16, efc, metric, dtype=dtype)
-    h.set_insert_batching(1 << 30, 1)   # one insert in flight: a deterministic serial build
-    launched(pkg, h.insert_flat(X, levels=levels))
-    assert_same_graph(h, o, n)
-    return X, o, h
-
-
 def queries(X, dtype, metric, nq, seed):
     Q = data(dtype, metric, nq, X.shape[1], seed + 100)
     Q[: nq // 10] = X[: nq // 10]   # stored points: distance-0 answers
     return Q
 
 
-# ---------------------------------------------------------------- the matrix
-F32_OPS = ["DistL1", "DistL2", "DistDot", "DistCosine"]
-F32_DIMS = [24, 48, 100, 150]          # rows of 128 / 256 / 512 / 640 bytes: CH = 1, 2, 4, generic
-U8_DIMS = [100, 200, 400, 600]
-U16_DIMS = [50, 100, 200, 300]
-CASES = ([(np.float32, m, d, False) for m in F32_OPS for d in F32_DIMS]
-         + [(np.float32, "DistL2", 24, True), (np.float32, "DistCosine", 100, True)]
-         + [(np.uint8, m, d, False) for m in distref.INT_METRICS for d in U8_DIMS]
-         + [(np.uint16, m, d, False) for m in distref.INT_METRICS for d in U16_DIMS]
-         + [(np.uint32, m, 24, False) for m in distref.INT_METRICS]
-         + [(np.int32, m, 24, False) for m in ("DistL1", "DistL2", "DistHamming")])
+# ---------------------------------------------------------------- the matrix (graphs.CASES, graphs.INSERT_CASES)
 N, NQ, M = 1000, 100, 8
 KS = [1, 10, 40, 128]
 EFS = [1, 64, 65, 128, 129, 256, 257]
@@ -124,13 +55,10 @@ def k_ef_pairs():
     return sorted({(k, max(ef, k)) for k in KS for ef in EFS + [k - 1] if ef >= k - 1})
 
 
-def case_id(c):
-    return f"{np.dtype(c[0]).name}-{c[1]}-d{c[2]}" + ("-ties" if c[3] else "")
-
-
 @pytest.mark.parametrize("dtype,metric,d,ties", CASES, ids=[case_id(c) for c in CASES])
 def test_instantiation_matrix(pkg, po, dtype, metric, d, ties):
-    X, o, h = build_both(pkg, po, dtype, metric, N, d, M, 200 if np.dtype(dtype) == np.float32 else 48, seed=d + 7, ties=ties)
+    X, o, h = build_both(pkg, po, dtype, metric, N, d, M, 200 if np.dtype(dtype) == np.float32 else 48, seed=d + 7,
+                         ties=ties, ledger=LEDGER)
     Q = queries(X, dtype, metric, NQ, d)
     # unfiltered search, stats off and on: same answers, and with stats the oracle's traversal counters
     for k, ef in k_ef_pairs():
@@ -179,14 +107,11 @@ def test_instantiation_matrix(pkg, po, dtype, metric, d, ties):
     DONE.append(case_id((dtype, metric, d, ties)))
 
 
-INSERT_CASES = [(m, d, efc) for m in F32_OPS for d in F32_DIMS for efc in (48, 300)]
-
-
 @pytest.mark.parametrize("metric,d,efc", INSERT_CASES)
 def test_insert_queue_kinds(pkg, po, metric, d, efc):
     """the f32 insert kernel's other queues: 128 slots (ef_construction <= 128) and the generic one (> 256); the
     256-slot queue (129..256) builds the graphs of test_instantiation_matrix"""
-    X, o, h = build_both(pkg, po, np.float32, metric, 600, d, M, efc, seed=d + efc)
+    X, o, h = build_both(pkg, po, np.float32, metric, 600, d, M, efc, seed=d + efc, ledger=LEDGER)
     Q = queries(X, np.float32, metric, 50, d + 1)
     same(launched(pkg, h.search_flat(Q, 10, 300)), o.search_batch(Q, 10, 300), "search")
     DONE.append(f"insert-{metric}-{d}-{efc}")
@@ -246,7 +171,6 @@ def test_probability_metric_kernels(pkg, po, metric):
 # f32 rows of 128 (CH 1), 256, 512 (CH 4) and more bytes; 7201 and 28801 are rows too wide for 8 warps of dist_batch
 # (every element type at 28801: f32 4 warps at 7201 and 1 at 28801, u16 2 and u8 4 at 28801)
 GPU_DIMS = [1, 3, 15, 17, 33, 100, 129, 257, 7201, 28801]
-LOG_METRICS = ("DistJeffreys", "DistJensenShannon")
 DIST_CASES = [(dt, m) for dt in (np.float32, np.uint8, np.uint16, np.uint32, np.int32)
               for m in distref.F32_METRICS + ["DistHamming", "DistJaccard"] if distref.supported(dt, m)]
 
@@ -322,7 +246,7 @@ def test_visited_epoch_wraps(pkg, po):
         8 slots, so some slot sees >= 2100 > 2 * 1023.
     Every answer is compared with the oracle."""
     n, d = 4200, 24
-    X, o, h = build_both(pkg, po, np.float32, "DistL2", n, d, M, 48, seed=11, max_elements=1 << 22)
+    X, o, h = build_both(pkg, po, np.float32, "DistL2", n, d, M, 48, seed=11, max_elements=1 << 22, ledger=LEDGER)
     calls = 2100
     Q = data(np.float32, "DistL2", 8 * calls, d, 12)
     allow = np.arange(0, n, 2)
@@ -359,15 +283,6 @@ NOT_RECORDED = {
         "launched directly after every insert search (run_insert_range), not through launch_kernel, so that the insert "
         "search kernel stays the recorded one",
 }
-
-
-def cuobjdump():
-    exe = shutil.which("cuobjdump")
-    if exe is None:
-        for root in (os.environ.get("CUDA_HOME"), os.environ.get("CUDA_PATH"), "/usr/local/cuda"):
-            if root and os.path.exists(os.path.join(root, "bin", "cuobjdump")):
-                return os.path.join(root, "bin", "cuobjdump")
-    return exe
 
 
 def test_zz_every_compiled_kernel_was_reached(pkg):

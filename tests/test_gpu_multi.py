@@ -8,7 +8,7 @@ import ctypes
 import numpy as np
 import pytest
 
-from test_gpu_search import build_pair
+from graphs import build_pair
 
 pytestmark = pytest.mark.gpu
 

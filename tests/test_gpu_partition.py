@@ -9,7 +9,8 @@ import threading
 import numpy as np
 import pytest
 
-from test_gpu_matrix import assert_same_graph, data, same
+from answers import same
+from graphs import assert_same_graph, data
 from util import recall_ids
 
 pytestmark = pytest.mark.gpu
@@ -18,7 +19,7 @@ N, NQ, M = 2000, 60, 8
 INV = 0xFFFFFFFF
 
 
-def origin_ids(n):
+def partition_origin_ids(n):
     return (np.arange(n, dtype=np.uint64) * 7 + 3)   # distinct from every rank, so a mix-up shows
 
 
@@ -34,7 +35,7 @@ def oracle_parts(po, X, ids, levels, P, metric, efc, dtype):
 def build(pkg, po, dtype, metric, d, efc, P, devices=None, serial=True, seed=1, n=N):
     X = data(dtype, metric, n, d, seed)
     levels = po.Oracle(M, n, 16, efc, metric, d, dtype=dtype, mode=po.MODE_DET, order=po.ORDER_GPU).draw_levels(n)
-    ids = origin_ids(n)
+    ids = partition_origin_ids(n)
     h = pkg.Hnsw(M, n, 16, efc, metric, dtype=dtype)
     if serial:
         h.set_insert_batching(1 << 30, 1)   # set before partition(): copied to every partition
@@ -160,7 +161,7 @@ def test_reference_entry_points_on_a_partitioned_handle(pkg, po):
     P, n = 3, 600
     X = data(np.float32, "DistL2", n, 24, 9)
     Q = queries(X, np.float32, "DistL2", 9)
-    ids = origin_ids(n)
+    ids = partition_origin_ids(n)
     hs = []
     for mixed in (False, True):
         h = pkg.Hnsw(M, n, 16, 64, "DistL2")

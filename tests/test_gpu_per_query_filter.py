@@ -10,32 +10,12 @@ import threading
 import numpy as np
 import pytest
 
-from test_gpu_exact import expected, handle
-from test_gpu_matrix import data, same
-from util import oracle_layers
+from answers import per_group, rows_of, same, same_as_single_filter_calls
+from exactref import expected, handle, origin_ids
+from graphs import data
+from restrict import EFC, M, N, build
 
 pytestmark = pytest.mark.gpu
-
-N, M, EFC = 2000, 8, 48
-
-
-def origin_ids(n):
-    return np.arange(n, dtype=np.uint64) * 5 + 2   # distinct from the internal ids, so a mix-up shows
-
-
-def build(pkg, po, dtype, metric, d, nq=300, seed=1):
-    """an oracle graph imported into the engine.  Points 0..399 come in identical pairs, so that a filter admitting
-    them has an equal-distance twin for every answer."""
-    X = data(dtype, metric, N, d, seed)
-    X[1:400:2] = X[0:400:2]
-    o = po.Oracle(M, N, 16, EFC, metric, d, dtype=dtype, mode=po.MODE_DET, order=po.ORDER_GPU)
-    o.insert_batch(X, ids=origin_ids(N))
-    lv, rk, og = o.export_points()
-    h = pkg.Hnsw(M, N, 16, EFC, metric, dtype=dtype)
-    h.import_graph(X, og, lv, o.entry, oracle_layers(o))
-    Q = data(dtype, metric, nq, d, seed + 100)
-    Q[:20] = X[:40:2]   # stored points with a twin: distance-0 ties
-    return X, Q, o, h
 
 
 def graph_filters(h):
@@ -45,30 +25,8 @@ def graph_filters(h):
     return [(name, allow, h.make_filter(allow)) for name, allow in sets]
 
 
-def rows_of(sel, g):
-    return np.flatnonzero(sel == g)
-
-
 def take(res, rows):
     return tuple(None if x is None else x[rows] for x in res)
-
-
-def per_group(call, Q, sel, rfs, k):
-    """the single-filter call on each group's rows, assembled in the batch's row order; sel[i] = -1 or an index of rfs"""
-    out = None
-    for g in np.unique(sel):
-        rows = rows_of(sel, g)
-        res = call(Q[rows], None if g < 0 else rfs[g])
-        if out is None:
-            out = tuple(None if x is None else np.empty((len(Q),) + x.shape[1:], x.dtype) for x in res)
-        for o, x in zip(out, res):
-            if o is not None:
-                o[rows] = x
-    return out
-
-
-def stats_sum(dicts):
-    return {key: sum(d[key] for d in dicts) for key in dicts[0]}
 
 
 GRAPH_CASES = [(np.float32, "DistL2", 24), (np.float32, "DistL2", 100), (np.uint8, "DistHamming", 100)]
@@ -81,25 +39,8 @@ def test_graph_rows_equal_single_filter_calls(pkg, po, dtype, metric, d):
     rfs = [rf for _, _, rf in fl]
     sel = np.random.default_rng(d).integers(-1, len(fl), len(Q))
     filters = [None if g < 0 else rfs[g] for g in sel]
-    for tie in (0, 1):   # tie mode 1 changes the kernel of the -1 rows only
-        h.set_tie_mode(tie)
-        for k, ef in ((1, 1), (10, 64), (40, 257)):
-            what = f"tie={tie} k={k} ef={ef}"
-            single = lambda q, rf: h.search_flat(q, k, ef, filter=rf)   # noqa: E731
-            want = per_group(single, Q, sel, rfs, k)
-            same(h.search_flat_per_query(Q, k, ef, filters), want, what)
-            # statistics: every run above grew the contexts' tables, so none of these overflows and re-runs
-            h.enable_stats(True)
-            h.get_stats()
-            got = h.search_flat_per_query(Q, k, ef, filters)
-            s_pq = h.get_stats()
-            parts = []
-            for g in np.unique(sel):
-                single(Q[rows_of(sel, g)], None if g < 0 else rfs[g])
-                parts.append(h.get_stats())
-            h.enable_stats(False)
-            same(got, want, what + " stats on")
-            assert s_pq == stats_sum(parts), (what, s_pq, parts)
+    # tie mode 1 changes the kernel of the -1 rows only
+    same_as_single_filter_calls(h, Q, sel, rfs, lambda k, ef: h.search_flat_per_query(Q, k, ef, filters))
     # one group straight against the oracle's filtered search
     h.set_tie_mode(0)
     name, allow, rf = fl[2]
@@ -136,7 +77,7 @@ def test_exact_rows_equal_single_filter_calls(pkg, po, k):
     filters = [None if g < 0 else rfs[g] for g in sel]
     got = h.search_exact_per_query(Q, k, filters)
     kern = pkg.last_kernel()
-    same(got, per_group(lambda q, rf: h.search_exact(q, k, filter=rf), Q, sel, rfs, k), f"k={k}")
+    same(got, per_group(lambda q, rf: h.search_exact(q, k, filter=rf), Q, sel, rfs), f"k={k}")
     h.search_exact(Q[:4], k, filter=rfs[0])
     assert "exact_knn_kernel" in kern and pkg.last_kernel() == kern
     for g in np.unique(sel):
@@ -198,9 +139,9 @@ def test_many_filters(pkg, po):
     sel = rng.integers(-1, 200, len(Q))
     filters = [None if g < 0 else rfs[g] for g in sel]
     same(h.search_flat_per_query(Q, 10, 64, filters),
-         per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, rfs, 10), "graph, 200 filters")
+         per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, rfs), "graph, 200 filters")
     same(h.search_exact_per_query(Q, 10, filters),
-         per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, sel, rfs, 10), "exact, 200 filters")
+         per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, sel, rfs), "exact, 200 filters")
     for rf in rfs:
         rf.free()
 
@@ -219,7 +160,7 @@ def test_overflow_grows_and_reruns(pkg, po):
         rfs = [three, half]
         got = h.search_flat_per_query(Q, 10, 64, [None if g < 0 else rfs[g] for g in sel])
         assert h.check_status() == 0
-        same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, rfs, 10), "overflow")
+        same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, rfs), "overflow")
         assert np.all(got[4][sel == 0] <= 3)
 
 
@@ -235,10 +176,10 @@ def test_partitioned_handle_and_view(pkg, po):
         sel = np.random.default_rng(8).integers(-1, 2, len(Q))
         filters = [None if g < 0 else rfs[g] for g in sel]
         got = h.search_flat_per_query(Q, 10, 64, filters)
-        same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, rfs, 10), "P=2 graph")
+        same(got, per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, rfs), "P=2 graph")
         assert np.all(got[2][got[2] != 0xFFFFFFFF] < N)   # global ranks
         same(h.search_exact_per_query(Q, 10, filters),
-             per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, sel, rfs, 10), "P=2 exact")
+             per_group(lambda q, rf: h.search_exact(q, 10, filter=rf), Q, sel, rfs), "P=2 exact")
         v = h.partition_view(0)
         same(v.search_flat_per_query(Q, 10, 64, [None] * len(Q)), v.search_flat(Q, 10, 64), "view, -1")
         with pytest.raises(pkg.HnswError, match=r"filters\[0\]"):
@@ -305,7 +246,7 @@ def test_refusals_leave_the_handle_unchanged(pkg, po):
     mixed = [fresh if i % 2 else None for i in range(len(Q))]
     sel = np.where(np.arange(len(Q)) % 2, 0, -1)
     same(h.search_flat_per_query(Q, 10, 64, mixed),
-         per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, [fresh], 10), "after an insert, with a new filter")
+         per_group(lambda q, rf: h.search_flat(q, 10, 64, filter=rf), Q, sel, [fresh]), "after an insert, with a new filter")
     for rf in (good, stale, fresh):
         rf.free()
     foreign.free()

@@ -11,14 +11,14 @@ import numpy as np
 import pytest
 import torch  # imported first, so that torch's own NCCL is the one the library binds at run time
 
-from test_gpu_exact import CASES, expected, filter_sets, handle, origin_ids
-from test_gpu_exact_shapes import SHAPE_CASES, d4_of, exact_shape, exact_slices, points, stored_queries, tile_points
-from test_gpu_matrix import data, same
+from answers import same
+from exactref import (EXACT_CASES, INVALID, SHAPE_CASES, d4_of, exact_shape, exact_slices, expected, filter_sets, handle,
+                      origin_ids, points, shape_case_id, stored_queries, tile_points)
+from graphs import case_id, data
 
 pytestmark = pytest.mark.gpu
 
 N, NQ = 1500, 40
-INVALID = 0xFFFFFFFF
 NONE = 0xFFFFFFFF
 I64_MIN, I64_MAX = np.iinfo(np.int64).min, np.iinfo(np.int64).max
 LEDGER = set()  # (pass, tq, rows, stages, S > 1) of every radius launch of the shape cases
@@ -107,8 +107,7 @@ def oracle(po, h, X, Q, k, metric, adms, r):
 
 
 # ---------------------------------------------------------------- 1. oracle parity
-@pytest.mark.parametrize("dtype,metric,d,ties", CASES,
-                         ids=[f"{np.dtype(c[0]).name}-{c[1]}-d{c[2]}" + ("-ties" if c[3] else "") for c in CASES])
+@pytest.mark.parametrize("dtype,metric,d,ties", EXACT_CASES, ids=[case_id(c) for c in EXACT_CASES])
 def test_radius_equals_oracle(pkg, po, dtype, metric, d, ties):
     X = data(dtype, metric, N, d, d + 3, ties)
     Q = data(dtype, metric, NQ, d, d + 103)
@@ -191,13 +190,9 @@ def test_split_launches(pkg, po):
 
 
 # ---------------------------------------------------------------- 4. instantiations and shapes
-def shape_case_id(c):
-    return f"{np.dtype(c[0]).name}-{c[1]}-d{c[2]}-n{c[3]}-nq{c[4]}-k{c[5]}"
-
-
 @pytest.mark.parametrize("dtype,metric,d,n,nq,k", SHAPE_CASES, ids=[shape_case_id(c) for c in SHAPE_CASES])
 def test_shapes(pkg, po, dtype, metric, d, n, nq, k):
-    """a radius launch has the k-NN launch's shape and shared memory (test_gpu_exact_shapes' restatement of
+    """a radius launch has the k-NN launch's shape and shared memory (exactref's restatement of
     exact_layout / exact_shape / cost(S), which radius mode does not change) and runs its instantiation; its rows are
     the k-NN rows cut at a radius halfway down them"""
     X = points(dtype, metric, n, d, d + n)

@@ -12,16 +12,14 @@ import numpy as np
 import pytest
 import torch  # device buffers; imported first, so that torch's own NCCL is the one the library binds at run time
 
-from test_gpu_matrix import data, same
+from answers import device_answers, same, same_host_device
+from exactref import origin_ids
+from graphs import data
 from util import oracle_layers
 
 pytestmark = pytest.mark.gpu
 
 N, NQ, M, EFC = 2000, 60, 8, 48
-
-
-def origin_ids(n):
-    return np.arange(n, dtype=np.uint64) * 5 + 2   # distinct from the internal ids, so a mix-up shows
 
 
 def build(pkg, po, dtype, metric, d, n=N, seed=1):
@@ -35,23 +33,6 @@ def build(pkg, po, dtype, metric, d, n=N, seed=1):
     Q = data(dtype, metric, NQ, d, seed + 100)
     Q[: NQ // 10] = X[: NQ // 10]   # stored points: distance-0 answers
     return X, Q, o, h
-
-
-def device_answers(raw, cnt):
-    """Neighbour_api[nq][k] (origin u64, dist f32, internal id in the tail padding) + counts, as search_flat's arrays"""
-    a = raw.cpu().numpy()
-    o = a[..., 0:8].copy().view(np.uint64)[..., 0]
-    d = a[..., 8:12].copy().view(np.float32)[..., 0]
-    it = a[..., 12:16].copy().view(np.uint32)[..., 0]
-    return o, d, it, cnt.cpu().numpy()
-
-
-def same_host_device(host, dev, what):
-    o, d, it, c = dev
-    assert np.array_equal(c, host[4]), f"{what}: counts differ"
-    assert np.array_equal(it, host[2]), f"{what}: internal ids differ"
-    assert np.array_equal(o, host[0]), f"{what}: origin ids differ"
-    assert np.array_equal(d.view(np.uint32), host[1].view(np.uint32)), f"{what}: distances are not bit-identical"
 
 
 CASES = [(np.float32, "DistL2", 24), (np.float32, "DistL2", 100), (np.uint8, "DistHamming", 100)]

@@ -9,19 +9,10 @@ BASELINE.json names: recall@k within 1e-3, distances within 1e-5 relative.
 import numpy as np
 import pytest
 
+from graphs import build_pair
 from util import gpu_layers, oracle_layers, recall_ids
 
 pytestmark = pytest.mark.gpu
-
-
-def build_pair(pkg, po, n, d, M, efc, metric, kind="uniform", max_layer=16, seed=1):
-    X = pkg.datagen.make(kind, n, d, seed)
-    o = po.Oracle(M, n, max_layer, efc, metric, d, mode=po.MODE_DET, order=po.ORDER_GPU)
-    o.insert_batch(X)
-    lv, rk, og = o.export_points()
-    h = pkg.Hnsw(M, n, max_layer, efc, metric)
-    h.import_graph(X, og, lv, o.entry, oracle_layers(o))
-    return X, o, h
 
 
 CASES = [

@@ -7,20 +7,17 @@ exclude_self it must equal that call with knbn + 1, without the point's own entr
 row does not hold the point), cut to knbn; that rule is computed here in numpy."""
 import numpy as np
 import pytest
+import torch  # device buffers; imported first, so that torch's own NCCL is the one the library binds at run time
 
-from test_gpu_exact import expected
-from test_gpu_matrix import data, same
+from answers import same
+from exactref import INVALID, expected, origin_ids
+from graphs import data
 from util import oracle_layers
 
 pytestmark = pytest.mark.gpu
 
 N, M, EFC = 1200, 8, 64
-INVALID = 0xFFFFFFFF
 NONE = 0xFFFFFFFF
-
-
-def origin_ids(n):
-    return np.arange(n, dtype=np.uint64) * 5 + 2   # distinct from the internal ids, so a mix-up shows
 
 
 def build(pkg, po, dtype, metric, d, seed, ties=False, n=N):
@@ -155,7 +152,6 @@ def test_exclude_self(pkg, po, metric):
 
 
 def test_device_variant(pkg, po):
-    import torch
     X, o, h = build(pkg, po, np.float32, "DistL2", 100, seed=23)
     qids = some_ids(N, 4)
     nq, k, ef = len(qids), 10, 64
@@ -209,7 +205,6 @@ def test_partitions(pkg, po, P):
     same(h.search_by_id(qids, 10, 64, sets=sets), h.search_flat_label_sets(V, 10, 64, sets), "partitioned sets")
     same(h.search_by_id(qids, 10, 64, sets=sets, exclude_self=True),
          minus_self(h.search_flat_label_sets(V, 11, 64, sets), qids, 10), "partitioned sets exclude_self")
-    import torch
     d_q = torch.zeros(1, dtype=torch.int64, device="cuda")
     out = torch.empty((1, 20), dtype=torch.int64, device="cuda")
     cnt = torch.empty(1, dtype=torch.int32, device="cuda")

@@ -10,11 +10,12 @@ distance bits, PointIds, counts and traversal counters against the oracle and ag
 import numpy as np
 import pytest
 
-from test_gpu_visited_stages import ALWAYS, EF, K, NEVER, build_both, move_at, same
+from answers import same
+from visited import ALWAYS, EF, K, NEVER, move_at, staged_graph
 
 pytestmark = pytest.mark.gpu
 
-M4 = 4  # build_both's M
+M4 = 4  # staged_graph's M
 
 
 def lean_bytes(ef):
@@ -63,7 +64,7 @@ def evals_per_query(o, Q, ef):
 
 @pytest.fixture(scope="module")
 def graph(pkg, po):
-    return build_both(pkg, po, 6000, 24, seed=41)
+    return staged_graph(pkg, po, 6000, 24, seed=41)
 
 
 def test_stay_in_window_and_move(pkg, po, graph):
@@ -117,7 +118,7 @@ def test_overflow_reruns(pkg, po):
 def test_epoch_wrap(pkg, po):
     """max_elements = 1 << 22 gives id_bits = 22 and 1023 epochs per slot; 1-query calls all land on slot 0 of search
     context 0, so 1100 of them wrap its epoch once, with searches that stay in the window and searches that moved"""
-    X, o, h, top = build_both(pkg, po, 6000, 24, seed=45, max_elements=1 << 22)
+    X, o, h, top = staged_graph(pkg, po, 6000, 24, seed=45, max_elements=1 << 22)
     calls = 1100
     Q = pkg.datagen.make("uniform", calls, 24, 46)
     Q[:100] = X[:100]

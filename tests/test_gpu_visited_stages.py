@@ -13,57 +13,10 @@ PointIds, counts and traversal counters must equal the oracle's.
 import numpy as np
 import pytest
 
-from util import csr_lists
+from answers import same
+from visited import ALWAYS, AUTO, EF, EFC, K, M, NEVER, move_at, staged_graph
 
 pytestmark = pytest.mark.gpu
-
-M, EFC, EF, K = 4, 48, 16, 10
-ALWAYS, NEVER, AUTO = 1, 2, 0
-
-
-def move_at(ef):
-    """insertions at which a search moves: 3/4 of a first stage of cap / 4"""
-    cap = max(1024, 1 << (2 * (ef + 16) * 2 * M - 1).bit_length())
-    return (cap // 4) * 3 // 4
-
-
-def same(got, want, what):
-    go, gd, gi, gpid, gc = got
-    oo, od, oi, opid, oc = want
-    assert np.array_equal(gc, oc), f"{what}: counts differ"
-    assert np.array_equal(gi, oi), f"{what}: internal ids differ"
-    assert np.array_equal(go, oo), f"{what}: origin ids differ"
-    assert np.array_equal(gd.view(np.uint32), od.view(np.uint32)), f"{what}: distances are not bit-identical"
-    assert np.array_equal(gpid, opid), f"{what}: PointIds differ"
-
-
-def build_both(pkg, po, n, d, seed, max_elements=None):
-    """the same graph serially on the GPU (one insert in flight) and in the oracle; the two must be equal list for list"""
-    X = pkg.datagen.make("uniform", n, d, seed)
-    o = po.Oracle(M, n, 16, EFC, "DistL2", d, mode=po.MODE_DET, order=po.ORDER_GPU)
-    levels = o.draw_levels(n)
-    o.insert_batch(X, levels=levels)
-    h = pkg.Hnsw(M, max_elements or n, 16, EFC, "DistL2")
-    h.set_insert_batching(1 << 30, 1)
-    h.insert_flat(X, levels=levels)
-    lv, rk, og, entry = h.export_points()
-    olv, ork, oog = o.export_points()
-    assert entry == o.entry
-    assert np.array_equal(lv, olv) and np.array_equal(rk, ork) and np.array_equal(og, oog)
-    for layer in range(int(olv.max()) + 1):
-        goff, gids, gds = h.export_layer(layer)
-        ooff, oids, ods = o.export_layer(layer)
-        if layer == 0:
-            assert np.array_equal(goff, ooff) and np.array_equal(gids, oids), "layer 0 differs"
-            assert np.array_equal(gds.view(np.uint32), ods.view(np.uint32)), "layer-0 link distances differ"
-            continue
-        gl, ol = csr_lists(goff, gids), csr_lists(ooff, oids)
-        for p in range(n):
-            if gl[p] or olv[p] >= layer:
-                assert gl[p] == ol[p], (layer, p)
-    h.set_visited_stages(ALWAYS)
-    return X, o, h, int(olv.max())
-
 
 def assert_mix(o, Q, ef, top, what, filt=None, some_stay=True):
     """the oracle's evaluations of each query: some pass the move point even after the descent's evaluations (at most
@@ -95,7 +48,7 @@ def check(h, o, Q, ef, what, filt=None, stats=True):
 
 @pytest.fixture(scope="module")
 def graph(pkg, po):
-    return build_both(pkg, po, 6000, 24, seed=21)
+    return staged_graph(pkg, po, 6000, 24, seed=21)
 
 
 def test_lean_every_mode_and_back(pkg, po, graph):
@@ -139,7 +92,7 @@ def test_filtered_kernel(pkg, po, graph):
 
 def test_generic_wide_rows(pkg, po):
     """rows of 640 bytes: the generic kernel at ef = 16, the same 256 / 1024-entry stages"""
-    X, o, h, top = build_both(pkg, po, 3000, 150, seed=25)
+    X, o, h, top = staged_graph(pkg, po, 3000, 150, seed=25)
     Q = pkg.datagen.make("uniform", 300, 150, 26)
     assert_mix(o, Q, EF, top, "generic wide rows")
     check(h, o, Q, EF, "generic wide rows")
@@ -169,7 +122,7 @@ def test_epoch_wrap_with_both_stages(pkg, po):
     """max_elements = 1 << 22 gives id_bits = 22 and 1023 epochs per table; 1-query lean calls all land on slot 0 of
     search context 0, so 1100 of them wrap its epoch once, with entries of moved searches left in the full stage.  A
     full stage that the wrap did not clear would hold entries of the restarted epochs, which the counters would show."""
-    X, o, h, top = build_both(pkg, po, 6000, 24, seed=29, max_elements=1 << 22)
+    X, o, h, top = staged_graph(pkg, po, 6000, 24, seed=29, max_elements=1 << 22)
     calls = 1100
     Q = pkg.datagen.make("uniform", calls, 24, 30)
     o.counters()
