@@ -371,17 +371,14 @@ int Index::exact_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, si
   const size_t tile_bytes = round128(tl.size() * sizeof(ExactTile));
   const size_t tick_bytes = p.slices > 1 ? round128(tiles * 4) : 0;
   const size_t part_bytes = p.slices > 1 ? tiles * p.slices * p.tq * k * 8 : 0;
-  if (tile_bytes + tick_bytes + part_bytes) {
-    int r;
-    if ((r = ensure_scratch(&c.d_xpart, &c.d_xpart_bytes, tile_bytes + tick_bytes + part_bytes, st))) return r;
-  }
+  if (tile_bytes + tick_bytes + part_bytes) HB_CUDA(c.d_xpart.grow(tile_bytes + tick_bytes + part_bytes, st));
   if (tiled) {
-    p.tiles = (const ExactTile*)c.d_xpart;
-    HB_CUDA(cudaMemcpyAsync(c.d_xpart, tl.data(), tl.size() * sizeof(ExactTile), cudaMemcpyHostToDevice, st));
+    p.tiles = c.d_xpart.as<const ExactTile>();
+    HB_CUDA(cudaMemcpyAsync(c.d_xpart.as(), tl.data(), tl.size() * sizeof(ExactTile), cudaMemcpyHostToDevice, st));
   }
   if (p.slices > 1) {
-    p.tickets = (unsigned*)((char*)c.d_xpart + tile_bytes);
-    p.part = (uint64_t*)((char*)c.d_xpart + tile_bytes + tick_bytes);
+    p.tickets = (unsigned*)(c.d_xpart.as<char>() + tile_bytes);
+    p.part = (uint64_t*)(c.d_xpart.as<char>() + tile_bytes + tick_bytes);
     HB_CUDA(cudaMemsetAsync(p.tickets, 0, tiles * 4, st));
   }
   HB_CUDA(cudaEventRecord(c.ev0, st));
@@ -405,26 +402,26 @@ int Index::dist_batch(const void* queries, size_t nq, int d, const uint32_t* can
     return fail("dimension too large for dist_batch: one query row needs " + std::to_string(smem_per_warp) +
                 " bytes of shared memory (limit 220 KB)");
   HB_CUDA(cudaSetDevice(device));
-  DevBuf dq, dc, dout;
-  HB_CUDA(cudaMalloc(&dq.p, nq * d * es));
-  HB_CUDA(cudaMalloc(&dc.p, nq * m * 4));
-  HB_CUDA(cudaMalloc(&dout.p, nq * m * 4));
-  HB_CUDA(cudaMemcpyAsync(dq.p, queries, nq * d * es, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(dc.p, cand, nq * m * 4, cudaMemcpyHostToDevice, stream_));
+  DeviceBuffer dq, dc, dout;
+  HB_CUDA(dq.reset(nq * d * es));
+  HB_CUDA(dc.reset(nq * m * 4));
+  HB_CUDA(dout.reset(nq * m * 4));
+  HB_CUDA(cudaMemcpyAsync(dq.as(), queries, nq * d * es, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(dc.as(), cand, nq * m * 4, cudaMemcpyHostToDevice, stream_));
   AuxParams p{};
   p.g = view();
-  p.queries = dq.p;
+  p.queries = dq.as();
   p.q_bytes = d * es;
   p.nq = (uint32_t)nq;
-  p.cand = (const uint32_t*)dc.p;
+  p.cand = dc.as<const uint32_t>();
   p.m = (uint32_t)m;
-  p.out = (float*)dout.p;
+  p.out = dout.as<float>();
   p.smem_per_warp = smem_per_warp;
   const int grid = (int)std::min<size_t>((size_t)sm_count_ * 8, (nq + cta.warps - 1) / cta.warps);
   HB_CUDA(dispatch_op(metric, dtype, [&](auto tag) -> cudaError_t {
     return launch_dist_batch_for_op<typename decltype(tag)::type>(p, grid, cta.warps * 32, cta.smem, stream_);
   }));
-  HB_CUDA(cudaMemcpyAsync(out, dout.p, nq * m * 4, cudaMemcpyDeviceToHost, stream_));
+  HB_CUDA(cudaMemcpyAsync(out, dout.as(), nq * m * 4, cudaMemcpyDeviceToHost, stream_));
   HB_CUDA(cudaStreamSynchronize(stream_));
   return 0;
 }

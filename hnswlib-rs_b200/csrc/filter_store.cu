@@ -13,20 +13,13 @@ static std::string unknown_filter(int64_t id) {
   return "filter " + std::to_string(id) + " is not a live filter of this handle (freed, or made on another handle)";
 }
 
-static void free_device_copies(FilterStore::Filter& f) {
-  for (auto& d : f.dev) {
-    cudaSetDevice(d.first.second);
-    cudaFree(d.second);
-  }
-  for (auto& d : f.ids) {
-    cudaSetDevice(d.first.second);
-    cudaFree(d.second.first);
-  }
-}
-
-FilterStore::~FilterStore() {
+// a copy of `words` on `device`, never null: an empty id list is not a null list (every point)
+static cudaError_t upload(const std::vector<uint32_t>& words, int device, DeviceBuffer& out) {
   DeviceRestore keep;
-  for (auto& kv : f_) free_device_copies(kv.second);
+  cudaError_t e;
+  if ((e = cudaSetDevice(device)) != cudaSuccess || (e = out.reset(std::max<size_t>(1, words.size()) * 4)) != cudaSuccess)
+    return e;
+  return cudaMemcpy(out.as(), words.data(), words.size() * 4, cudaMemcpyHostToDevice);
 }
 
 int64_t FilterStore::add(Filter&& f) {
@@ -60,44 +53,27 @@ int FilterStore::use(int64_t id, int p, int nparts, const Index* rx, const uint3
       std::vector<uint32_t> ids;
       for (size_t i = 0; i < f.counts[p]; ++i)
         if ((b[i >> 5] >> (i & 31)) & 1u) ids.push_back((uint32_t)i);
-      DeviceRestore keep;
-      void* ptr = nullptr;
-      cudaError_t e;
-      if ((e = cudaSetDevice(rx->device)) != cudaSuccess || (e = cudaMalloc(&ptr, std::max<size_t>(1, ids.size()) * 4)) != cudaSuccess ||
-          (e = cudaMemcpy(ptr, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice)) != cudaSuccess) {
-        cudaFree(ptr);
-        return rx->cuda_fail(e, "filter id list upload");
-      }
-      l = f.ids.emplace(key, std::make_pair(ptr, ids.size())).first;
+      DeviceBuffer copy;
+      if (cudaError_t e = upload(ids, rx->device, copy)) return rx->cuda_fail(e, "filter id list upload");
+      l = f.ids.emplace(key, std::make_pair(std::move(copy), ids.size())).first;
     }
-    list->ids = (const uint32_t*)l->second.first;
+    list->ids = l->second.first.as<const uint32_t>();
     list->n = l->second.second;
     return 0;
   }
   auto d = f.dev.find(key);
   if (d == f.dev.end()) {  // first use on this device: one copy, kept until the filter is freed
-    DeviceRestore keep;
-    const std::vector<uint32_t>& b = f.bits[p];
-    void* ptr = nullptr;
-    cudaError_t e;
-    if ((e = cudaSetDevice(rx->device)) != cudaSuccess || (e = cudaMalloc(&ptr, b.size() * 4)) != cudaSuccess ||
-        (e = cudaMemcpy(ptr, b.data(), b.size() * 4, cudaMemcpyHostToDevice)) != cudaSuccess) {
-      cudaFree(ptr);
-      return rx->cuda_fail(e, "filter upload");
-    }
-    d = f.dev.emplace(key, ptr).first;
+    DeviceBuffer copy;
+    if (cudaError_t e = upload(f.bits[p], rx->device, copy)) return rx->cuda_fail(e, "filter upload");
+    d = f.dev.emplace(key, std::move(copy)).first;
   }
-  *d_bits = (const uint32_t*)d->second;
+  *d_bits = d->second.as<const uint32_t>();
   return 0;
 }
 
-void FilterStore::erase(int64_t id) {
+void FilterStore::erase(int64_t id) {  // each device copy is freed on its device
   std::lock_guard<std::mutex> lk(mu_);
-  auto it = f_.find(id);
-  if (it == f_.end()) return;
-  DeviceRestore keep;
-  free_device_copies(it->second);
-  f_.erase(it);
+  f_.erase(id);
 }
 
 int64_t Index::new_filter(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx) {

@@ -56,17 +56,16 @@ Index::Index(int M_, size_t max_elements_, int max_layer_, int ef_c_, int metric
     err_ = "device index out of range";
     return;
   }
-  if ((e = cudaSetDevice(device)) != cudaSuccess || (e = cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking)) != cudaSuccess) {
+  if ((e = cudaSetDevice(device)) != cudaSuccess || (e = own_stream_.create(cudaStreamNonBlocking)) != cudaSuccess) {
     err_ = std::string("CUDA init failed: ") + cudaGetErrorString(e);
     return;
   }
+  stream_ = own_stream_;
   for (SearchCtx& c : ctx_) {
-    if ((e = cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking)) != cudaSuccess ||
-        (e = cudaEventCreateWithFlags(&c.fork, cudaEventDisableTiming)) != cudaSuccess ||
-        (e = cudaEventCreateWithFlags(&c.join, cudaEventDisableTiming)) != cudaSuccess ||
-        (e = cudaEventCreate(&c.ev0)) != cudaSuccess || (e = cudaEventCreate(&c.ev1)) != cudaSuccess ||
-        (e = cudaMalloc(&c.d_counter, sizeof(unsigned int))) != cudaSuccess || (e = cudaMalloc(&c.d_status, sizeof(int))) != cudaSuccess ||
-        (e = cudaMemset(c.d_status, 0, sizeof(int))) != cudaSuccess) {
+    if ((e = c.stream.create(cudaStreamNonBlocking)) != cudaSuccess || (e = c.fork.create(cudaEventDisableTiming)) != cudaSuccess ||
+        (e = c.join.create(cudaEventDisableTiming)) != cudaSuccess || (e = c.ev0.create(cudaEventDefault)) != cudaSuccess ||
+        (e = c.ev1.create(cudaEventDefault)) != cudaSuccess || (e = c.d_counter.reset(sizeof(unsigned int))) != cudaSuccess ||
+        (e = c.d_status.reset(sizeof(int))) != cudaSuccess || (e = cudaMemset(c.d_status.as(), 0, sizeof(int))) != cudaSuccess) {
       err_ = std::string("CUDA init failed: ") + cudaGetErrorString(e);
       return;
     }
@@ -76,44 +75,55 @@ Index::Index(int M_, size_t max_elements_, int max_layer_, int ef_c_, int metric
     err_ = std::string("cudaGetDeviceProperties: ") + cudaGetErrorString(e);
     return;
   }
-  own_stream_ = stream_;
   sm_count_ = prop.multiProcessorCount;
   l2_bytes_ = (size_t)prop.l2CacheSize;
-  if ((e = cudaMalloc(&d_counter_, sizeof(unsigned int))) != cudaSuccess || (e = cudaMalloc(&d_status_, sizeof(int))) != cudaSuccess ||
-      (e = cudaMalloc(&d_stats_, 4 * sizeof(unsigned long long))) != cudaSuccess) {
+  if ((e = d_counter_.reset(sizeof(unsigned int))) != cudaSuccess || (e = d_status_.reset(sizeof(int))) != cudaSuccess ||
+      (e = d_stats_.reset(4 * sizeof(unsigned long long))) != cudaSuccess) {
     err_ = std::string("cudaMalloc: ") + cudaGetErrorString(e);
     return;
   }
-  cudaMemset(d_stats_, 0, 4 * sizeof(unsigned long long));
-  cudaMemset(d_status_, 0, sizeof(int));
+  cudaMemset(d_stats_.as(), 0, 4 * sizeof(unsigned long long));
+  cudaMemset(d_status_.as(), 0, sizeof(int));
   ok_ = true;
 }
 
+// The members free themselves, each on its own device; before they do, every stream that may still read them is idle.
 Index::~Index() {
   DeviceRestore keep;
   drop_replicas();
   nccl_destroy();
   cudaSetDevice(device);
   if (stream_) cudaStreamSynchronize(stream_);
-  for (void* a : graph_.p) cudaFree(a);
-  cudaFree(vis_.tab); cudaFree(vis_.epoch); cudaFree(d_counter_); cudaFree(d_status_); cudaFree(d_stats_); cudaFree(d_mask_);
-  cudaFree(by_label_.d_ids);
-  cudaFree(by_value_.d_ids);
-  cudaFree(by_label_value_.d_ids);
-  if (h_pin_) cudaFreeHost(h_pin_);
-  for (SearchCtx& c : ctx_) {
+  for (SearchCtx& c : ctx_)
     if (c.stream) cudaStreamSynchronize(c.stream);
-    cudaFree(c.vis.tab); cudaFree(c.vis.epoch); cudaFree(c.fvis.tab); cudaFree(c.fvis.epoch); cudaFree(c.d_counter); cudaFree(c.d_status);
-    cudaFree(c.d_fbits); cudaFree(c.d_cbuf); cudaFree(c.d_xq); cudaFree(c.d_xpart);
-    if (c.h_pin) cudaFreeHost(c.h_pin);
-    if (c.h_res) cudaFreeHost(c.h_res);
-    if (c.fork) cudaEventDestroy(c.fork);
-    if (c.join) cudaEventDestroy(c.join);
-    if (c.ev0) cudaEventDestroy(c.ev0);
-    if (c.ev1) cudaEventDestroy(c.ev1);
-    if (c.stream) cudaStreamDestroy(c.stream);
-  }
-  if (own_stream_) cudaStreamDestroy(own_stream_);
+}
+
+template <bool Pinned>
+void CudaBuffer<Pinned>::release() {
+  if (!p_) return;
+  DeviceRestore keep;
+  cudaSetDevice(dev_);
+  (Pinned ? cudaFreeHost : cudaFree)(p_);
+  p_ = nullptr;
+  bytes_ = 0;
+}
+
+template <bool Pinned>
+cudaError_t CudaBuffer<Pinned>::reset(size_t bytes, unsigned int flags) {
+  release();
+  cudaError_t e = cudaGetDevice(&dev_);
+  if (e == cudaSuccess) e = Pinned ? cudaHostAlloc(&p_, bytes, flags) : cudaMalloc(&p_, bytes);
+  if (e != cudaSuccess) p_ = nullptr;
+  bytes_ = e == cudaSuccess ? bytes : 0;
+  return e;
+}
+template class CudaBuffer<false>;
+template class CudaBuffer<true>;
+
+cudaError_t DeviceBuffer::grow(size_t need, cudaStream_t st) {
+  if (need <= size()) return cudaSuccess;
+  const cudaError_t e = cudaStreamSynchronize(st);
+  return e != cudaSuccess ? e : reset(std::max(need, (size_t)4096));
 }
 
 size_t Index::row_size(int a) const {
@@ -126,12 +136,12 @@ int Index::grow_store(bool per_list, size_t cap, size_t keep) {
   for (int a = 0; a < GS::COUNT; ++a) {
     if ((GS::DESC[a].row == GS::LISTU) != per_list) continue;
     const size_t row = row_size(a);
-    DevBuf grown;
-    HB_CUDA(cudaMalloc(&grown.p, cap * row));
-    HB_CUDA(cudaMemsetAsync(grown.p, GS::DESC[a].fill, cap * row, stream_));
-    if (keep && graph_.p[a]) HB_CUDA(cudaMemcpyAsync(grown.p, graph_.p[a], keep * row, cudaMemcpyDeviceToDevice, stream_));
+    DeviceBuffer grown;
+    HB_CUDA(grown.reset(cap * row));
+    HB_CUDA(cudaMemsetAsync(grown.as(), GS::DESC[a].fill, cap * row, stream_));
+    if (keep && graph_.p[a].size()) HB_CUDA(cudaMemcpyAsync(grown.as(), graph_.p[a].as(), keep * row, cudaMemcpyDeviceToDevice, stream_));
     HB_CUDA(cudaStreamSynchronize(stream_));
-    std::swap(graph_.p[a], grown.p);  // the old array is freed with `grown`
+    graph_.p[a] = std::move(grown);  // the old array is freed with `grown`
   }
   return 0;
 }
@@ -179,15 +189,12 @@ int Index::ensure_visited(VisitedPool& v, size_t slots, size_t cap_entries, cuda
   }
   const size_t bytes = ns * visited_slot_entries(nc) * sizeof(uint32_t);
   HB_CUDA(cudaStreamSynchronize(st));
-  cudaFree(v.tab);
-  cudaFree(v.epoch);
-  v.tab = v.epoch = nullptr;
   v.slots = v.cap = 0;
-  HB_CUDA(cudaMalloc(&v.tab, bytes));
-  HB_CUDA(cudaMalloc(&v.epoch, ns * sizeof(uint32_t)));
-  HB_CUDA(cudaMemsetAsync(v.tab, 0, bytes, st));
+  HB_CUDA(v.tab.reset(bytes));
+  HB_CUDA(v.epoch.reset(ns * sizeof(uint32_t)));
+  HB_CUDA(cudaMemsetAsync(v.tab.as(), 0, bytes, st));
   // epoch = max forces a table clear on first use whatever id_bits is (Visited::begin)
-  HB_CUDA(cudaMemsetAsync(v.epoch, 0xFF, ns * sizeof(uint32_t), st));
+  HB_CUDA(cudaMemsetAsync(v.epoch.as(), 0xFF, ns * sizeof(uint32_t), st));
   v.slots = ns;
   v.cap = nc;
   return 0;
@@ -201,12 +208,12 @@ int Index::fill_visited_cfg(VisitedPool& v, VisitedCfg& c, bool staged, cudaStre
   // entries are (epoch << id_bits) | id at slot offsets of one layout: a new split or a new layout invalidates every table
   // (epoch = max clears a slot's tables at its next begin())
   if (id_bits != v.id_bits || staged != v.staged) {
-    HB_CUDA(cudaMemsetAsync(v.epoch, 0xFF, v.slots * sizeof(uint32_t), st));
+    HB_CUDA(cudaMemsetAsync(v.epoch.as(), 0xFF, v.slots * sizeof(uint32_t), st));
     v.id_bits = id_bits;
     v.staged = staged;
   }
-  c.tables = v.tab;
-  c.epochs = v.epoch;
+  c.tables = v.tab.as<uint32_t>();
+  c.epochs = v.epoch.as<uint32_t>();
   c.cap = (uint32_t)v.cap;
   c.shift = 32 - ilog2(v.cap);
   c.small = staged ? (uint32_t)visited_first_stage(v.cap) : 0u;
@@ -234,32 +241,9 @@ bool Index::visited_staged(size_t slots, size_t cap, size_t need, bool first_fit
   return slots * cap * sizeof(uint32_t) > l2_bytes_ && visited_first_stage(cap) * 5 >= need * 2;
 }
 
-int Index::ensure_scratch(void** p, size_t* cur, size_t need, cudaStream_t st) {
-  if (need <= *cur) return 0;
-  HB_CUDA(cudaStreamSynchronize(st));
-  cudaFree(*p);
-  *p = nullptr;
-  *cur = 0;
-  size_t nb = std::max(need, (size_t)4096);
-  HB_CUDA(cudaMalloc(p, nb));
-  *cur = nb;
-  return 0;
-}
-
-// the same for a pinned host buffer, allocated with cudaHostAlloc `flags`
-int Index::ensure_pinned(void** p, size_t* cur, size_t need, unsigned int flags) {
-  if (need <= *cur) return 0;
-  if (*p) cudaFreeHost(*p);
-  *p = nullptr;
-  *cur = 0;
-  HB_CUDA(cudaHostAlloc(p, need, flags));
-  *cur = need;
-  return 0;
-}
-
 GraphView Index::view() const {
   GraphView g;
-  g.vec = graph_.p[GS::VEC];
+  g.vec = graph_.at<void>(GS::VEC);
   g.d4 = row_bytes / 16;
   g.dim = dim;
   g.adj0 = graph_.at<uint32_t>(GS::ADJ0);
@@ -370,15 +354,15 @@ int Index::run_insert_range(size_t first, size_t count, size_t mask_off) {
   p.g = view();
   p.first = (uint32_t)first;
   p.count = (uint32_t)count;
-  p.layer_mask = reinterpret_cast<const uint16_t*>(d_mask_) + mask_off;
+  p.layer_mask = d_mask_.as<const uint16_t>() + mask_off;
   p.ef_c = ef_c;
   p.keep_pruned = keep_pruned ? 1 : 0;
   p.extend = extend_candidates ? 1 : 0;
   p.link_mode = link_mode;
-  p.work_counter = d_counter_;
+  p.work_counter = d_counter_.as<unsigned int>();
   p.locks = graph_.at<int>(GS::LOCKS);
-  p.stats = stats_on_ ? d_stats_ : nullptr;  // insert-path distance evaluations / expansions / adjacency ids read
-  p.status = d_status_;
+  p.stats = stats_on_ ? d_stats_.as<unsigned long long>() : nullptr;  // insert-path distance evaluations / expansions / adjacency ids read
+  p.status = d_status_.as<int>();
   const InsertShape s = insert_shape();
   p.q_kind = s.q_kind;
   p.q_smem = s.q_smem;
@@ -397,14 +381,14 @@ int Index::run_insert_range(size_t first, size_t count, size_t mask_off) {
     int r;
     if ((r = ensure_visited(vis_, (size_t)grid * wpb, vcap, stream_))) return r;
     if ((r = fill_visited_cfg(vis_, p.vis, false, stream_))) return r;  // inserts: one stage (see visited_staged)
-    HB_CUDA(cudaMemsetAsync(d_counter_, 0, sizeof(unsigned int), stream_));
+    HB_CUDA(cudaMemsetAsync(d_counter_.as(), 0, sizeof(unsigned int), stream_));
     HB_CUDA(launch_insert_search(p, metric, dtype, grid, smem, stream_, nullptr));
     int status = 0;
-    HB_CUDA(cudaMemcpyAsync(&status, d_status_, sizeof(int), cudaMemcpyDeviceToHost, stream_));
+    HB_CUDA(cudaMemcpyAsync(&status, d_status_.as(), sizeof(int), cudaMemcpyDeviceToHost, stream_));
     HB_CUDA(cudaStreamSynchronize(stream_));
     if (status == 0) break;
     if (attempt >= 8) return fail("visited table overflow persists");
-    HB_CUDA(cudaMemsetAsync(d_status_, 0, sizeof(int), stream_));
+    HB_CUDA(cudaMemsetAsync(d_status_.as(), 0, sizeof(int), stream_));
     vcap = vis_.cap * 2;  // rare: a search wandered further than 2*(ef+16)*degree nodes
   }
   int lgrid = (int)std::min<size_t>((size_t)sm_count_ * 8, (count + wpb - 1) / wpb);
@@ -459,10 +443,10 @@ int Index::insert_batch(const void* vecs, size_t n_new, size_t stride, const voi
   if (rows) {
     const size_t rb = (size_t)dim * es;  // bytes of one user row
     const size_t chunk = std::max<size_t>(1, (size_t)(8u << 20) / rb);
-    if ((r = ensure_pinned(&h_pin_, &h_pin_bytes_, chunk * rb, cudaHostAllocDefault))) return r;
+    HB_CUDA(h_pin_.grow(chunk * rb, cudaHostAllocDefault));
     for (size_t b = 0; b < n_new; b += chunk) {
       const size_t c = std::min(chunk, n_new - b);
-      unsigned char* st = (unsigned char*)h_pin_;
+      unsigned char* st = h_pin_.as<unsigned char>();
       for (size_t i = 0; i < c; ++i) memcpy(st + i * rb, rows[b + i], rb);
       HB_CUDA(cudaMemcpy2DAsync(graph_.at<unsigned char>(GS::VEC) + (first + b) * (size_t)row_bytes, (size_t)row_bytes, st, rb, rb, c,
                                 cudaMemcpyHostToDevice, stream_));
@@ -473,8 +457,8 @@ int Index::insert_batch(const void* vecs, size_t n_new, size_t stride, const voi
                               (size_t)dim * es, n_new, cudaMemcpyHostToDevice, stream_));
   }
   if ((r = upload_points(first, n_new))) return r;
-  if ((r = ensure_scratch(&d_mask_, &d_mask_bytes_, n_new * 2, stream_))) return r;
-  HB_CUDA(cudaMemcpyAsync(d_mask_, masks.data(), n_new * 2, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(d_mask_.grow(n_new * 2, stream_));
+  HB_CUDA(cudaMemcpyAsync(d_mask_.as(), masks.data(), n_new * 2, cudaMemcpyHostToDevice, stream_));
   n = first + n_new;  // stored; points become reachable as their batch links them
   // ---- schedule batches
   size_t done = 0;
@@ -595,13 +579,13 @@ int Index::import_graph(const void* vecs, size_t n_new, int d, const uint64_t* o
         if (dists && dists[l]) ad[j - b] = dists[l][j];
       }
     }
-  HB_CUDA(cudaMemcpy2DAsync(graph_.p[GS::VEC], (size_t)row_bytes, vecs, (size_t)dim * es, (size_t)dim * es, n_new,
+  HB_CUDA(cudaMemcpy2DAsync(graph_.at<void>(GS::VEC), (size_t)row_bytes, vecs, (size_t)dim * es, (size_t)dim * es, n_new,
                             cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(graph_.p[GS::ADJ0], a0.data(), a0.size() * 4, cudaMemcpyHostToDevice, stream_));
-  HB_CUDA(cudaMemcpyAsync(graph_.p[GS::ADJ0_D], a0d.data(), a0d.size() * 4, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.at<void>(GS::ADJ0), a0.data(), a0.size() * 4, cudaMemcpyHostToDevice, stream_));
+  HB_CUDA(cudaMemcpyAsync(graph_.at<void>(GS::ADJ0_D), a0d.data(), a0d.size() * 4, cudaMemcpyHostToDevice, stream_));
   if (n_ul) {
-    HB_CUDA(cudaMemcpyAsync(graph_.p[GS::ADJU], aU.data(), n_ul * M * 4, cudaMemcpyHostToDevice, stream_));
-    HB_CUDA(cudaMemcpyAsync(graph_.p[GS::ADJU_D], aUd.data(), n_ul * M * 4, cudaMemcpyHostToDevice, stream_));
+    HB_CUDA(cudaMemcpyAsync(graph_.at<void>(GS::ADJU), aU.data(), n_ul * M * 4, cudaMemcpyHostToDevice, stream_));
+    HB_CUDA(cudaMemcpyAsync(graph_.at<void>(GS::ADJU_D), aUd.data(), n_ul * M * 4, cudaMemcpyHostToDevice, stream_));
   }
   if ((r = upload_points(0, n_new))) return r;
   HB_CUDA(cudaStreamSynchronize(stream_));
@@ -718,14 +702,14 @@ int Index::search_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, s
   while (layer0 < MAX_LAYERS - 1 && layer_count[layer0] == 0) layer0++;
   if (n == 0) layer0 = 0;
   p.layer0 = layer0;
-  p.work_counter = c.d_counter;
+  p.work_counter = c.d_counter.as<unsigned int>();
   p.out_nb = rows.out;
   p.out_count = rows.counts;
   p.filter_table = f.table;
   p.filter_sel = f.sel;
   p.filter = f.filter;
-  p.stats = stats_on_ ? d_stats_ : nullptr;
-  p.status = c.d_status;
+  p.stats = stats_on_ ? d_stats_.as<unsigned long long>() : nullptr;
+  p.status = c.d_status.as<int>();
   const bool filtered = f.sel != nullptr || f.filter.ptr != nullptr || f.filter.attr != nullptr;
   QueryKernel kind = QueryKernel::Generic;
   if (filtered) kind = QueryKernel::Filtered;
@@ -794,24 +778,24 @@ int Index::search_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, s
     const size_t launch_smem = staged && kind == QueryKernel::Lean ? window_smem : smem;
     p.smem_per_warp = (int)(launch_smem / wpb);
     if (kind == QueryKernel::Filtered || kind == QueryKernel::StdTie) {  // candidate queue C: one region per warp slot
-      if ((r = ensure_scratch(&c.d_cbuf, &c.d_cbuf_bytes, (size_t)grid * wpb * pool.cap * 8, st))) return r;
-      p.cbuf = (uint64_t*)c.d_cbuf;
+      HB_CUDA(c.d_cbuf.grow((size_t)grid * wpb * pool.cap * 8, st));
+      p.cbuf = c.d_cbuf.as<uint64_t>();
       p.ccap = (uint32_t)pool.cap;
     }
-    HB_CUDA(cudaMemsetAsync(c.d_counter, 0, sizeof(unsigned int), st));
+    HB_CUDA(cudaMemsetAsync(c.d_counter.as(), 0, sizeof(unsigned int), st));
     HB_CUDA(cudaEventRecord(c.ev0, st));
     HB_CUDA(launch_query(kind, p, metric, dtype, grid, launch_smem, st, nullptr));
     HB_CUDA(cudaEventRecord(c.ev1, st));
     if (!sync) break;
     int status = 0;
-    HB_CUDA(cudaMemcpyAsync(&status, c.d_status, sizeof(int), cudaMemcpyDeviceToHost, st));
+    HB_CUDA(cudaMemcpyAsync(&status, c.d_status.as(), sizeof(int), cudaMemcpyDeviceToHost, st));
     HB_CUDA(cudaStreamSynchronize(st));
     if (status == 0) {
       if (kernel_ms) HB_CUDA(cudaEventElapsedTime(kernel_ms, c.ev0, c.ev1));
       break;
     }
     if (attempt >= 24) return fail("visited table overflow persists");
-    HB_CUDA(cudaMemsetAsync(c.d_status, 0, sizeof(int), st));
+    HB_CUDA(cudaMemsetAsync(c.d_status.as(), 0, sizeof(int), st));
     vcap = pool.cap * 2;
   }
   if (stats_on_) stat_queries_ += nq;
@@ -856,11 +840,10 @@ int Index::search_host_begin(int ci, const HostRows& in, size_t nq, int d, size_
   for (int i = 0; i < COLUMNS; ++i) at[i + 1] = at[i] + col[i].bytes * nq;
   // [answers][counts][status, 16 bytes][totals]
   const size_t out_bytes = nq * k * sizeof(NeighbourOut), cnt_bytes = nq * sizeof(int32_t), tot_bytes = at[COLUMNS] - at[TOTALS];
-  if ((r = ensure_pinned(&c.h_res, &c.h_res_bytes, out_bytes + cnt_bytes + 16 + tot_bytes, cudaHostAllocMapped | cudaHostAllocPortable)))
-    return r;
-  NeighbourOut* hout = (NeighbourOut*)c.h_res;
-  int32_t* hcnt = (int32_t*)((char*)c.h_res + out_bytes);
-  uint32_t* htot = tot_bytes ? (uint32_t*)((char*)c.h_res + out_bytes + cnt_bytes + 16) : nullptr;
+  HB_CUDA(c.h_res.grow(out_bytes + cnt_bytes + 16 + tot_bytes, cudaHostAllocMapped | cudaHostAllocPortable));
+  NeighbourOut* hout = c.h_res.as<NeighbourOut>();
+  int32_t* hcnt = (int32_t*)(c.h_res.as<char>() + out_bytes);
+  uint32_t* htot = tot_bytes ? (uint32_t*)(c.h_res.as<char>() + out_bytes + cnt_bytes + 16) : nullptr;
   c.pend.ans = HostAnswers{hout, hcnt, htot};
   c.pend.hstatus = hcnt + nq;
   SearchCtx::Launch& L = c.pend.run;
@@ -873,7 +856,7 @@ int Index::search_host_begin(int ci, const HostRows& in, size_t nq, int d, size_
     for (size_t i = 0; i < nq * k; ++i) hout[i] = NeighbourOut{~0ull, __builtin_inff(), INVALID_ID};
     return 0;
   }
-  char* dv = (char*)device_view_of_host(c.h_res);  // where the kernel writes
+  char* dv = (char*)device_view_of_host(c.h_res.as());  // where the kernel writes
   if (!dv) return fail("the pinned result buffer has no device address");
   L.rows.out = (NeighbourOut*)dv;
   L.rows.counts = (int32_t*)(dv + out_bytes);
@@ -882,9 +865,8 @@ int Index::search_host_begin(int ci, const HostRows& in, size_t nq, int d, size_
   const size_t staged = in.qids || d_queries ? 0 : round128(qbytes);
   if (staged + at[TOTALS]) {
     // gather into pinned staging (rows: one pointer per query, libext.rs parallel_search_neighbours_<ty>)
-    if ((r = ensure_pinned(&c.h_pin, &c.h_pin_bytes, staged + at[TOTALS], cudaHostAllocMapped | cudaHostAllocPortable)))
-      return r;
-    unsigned char* stage = (unsigned char*)c.h_pin;
+    HB_CUDA(c.h_pin.grow(staged + at[TOTALS], cudaHostAllocMapped | cudaHostAllocPortable));
+    unsigned char* stage = c.h_pin.as<unsigned char>();
     if (in.rows)
       for (size_t i = 0; i < nq; ++i) memcpy(stage + i * (size_t)dim * es, in.rows[i], (size_t)dim * es);
     else if (staged)
@@ -900,11 +882,11 @@ int Index::search_host_begin(int ci, const HostRows& in, size_t nq, int d, size_
   // an exact launch may run many CTAs per query (row slices): the queries cross the bus once, into device memory
   const size_t xq = plan.exact ? round128(qbytes) : 0;
   if (xq + at[COLUMNS]) {
-    if ((r = ensure_scratch(&c.d_xq, &c.d_xq_bytes, xq + at[COLUMNS], st))) return r;
-    if (xq) HB_CUDA(cudaMemcpyAsync(c.d_xq, d_queries, qbytes, cudaMemcpyDefault, st));
-    if (xq) L.rows.d_queries = c.d_xq;
-    char* cols = (char*)c.d_xq + xq;
-    if (at[TOTALS]) HB_CUDA(cudaMemcpyAsync(cols, (char*)c.h_pin + staged, at[TOTALS], cudaMemcpyHostToDevice, st));
+    HB_CUDA(c.d_xq.grow(xq + at[COLUMNS], st));
+    if (xq) HB_CUDA(cudaMemcpyAsync(c.d_xq.as(), d_queries, qbytes, cudaMemcpyDefault, st));
+    if (xq) L.rows.d_queries = c.d_xq.as();
+    char* cols = c.d_xq.as<char>() + xq;
+    if (at[TOTALS]) HB_CUDA(cudaMemcpyAsync(cols, c.h_pin.as<char>() + staged, at[TOTALS], cudaMemcpyHostToDevice, st));
     auto on_device = [&](int i) -> void* { return col[i].bytes ? cols + at[i] : nullptr; };
     L.rows.q_ids = (const uint64_t*)on_device(IDS);
     L.rows.skip = (const uint64_t*)on_device(in.skip == in.qids ? IDS : SKIP);
@@ -916,7 +898,7 @@ int Index::search_host_begin(int ci, const HostRows& in, size_t nq, int d, size_
   // path (a visited table overflowed: grow and re-run) only when the status says so
   c.pend.enqueued = true;
   if ((r = stage_plan(c, plan, L)) || (r = run_plan(c, L, false, nullptr))) return r;
-  if (!plan.exact) HB_CUDA(cudaMemcpyAsync(c.pend.hstatus, c.d_status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  if (!plan.exact) HB_CUDA(cudaMemcpyAsync(c.pend.hstatus, c.d_status.as(), sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   if (htot) HB_CUDA(cudaMemcpyAsync(htot, L.rows.totals, tot_bytes, cudaMemcpyDeviceToHost, st));
   return 0;
 }
@@ -930,7 +912,7 @@ HostAnswers Index::search_host_finish(int ci) {
     HB_CUDA(cudaSetDevice(device));
     HB_CUDA(cudaStreamSynchronize(c.stream));
     if (p.run.exact || *p.hstatus == 0) return 0;  // an exact scan has no status and nothing to re-run
-    HB_CUDA(cudaMemsetAsync(c.d_status, 0, sizeof(int), c.stream));
+    HB_CUDA(cudaMemsetAsync(c.d_status.as(), 0, sizeof(int), c.stream));
     return run_plan(c, p.run, true, nullptr);  // grows the tables
   }();
   return a;
@@ -945,7 +927,6 @@ HostAnswers Index::search_host_finish(int ci) {
 // exact scan keeps the k smallest (distance, id) keys, so the order of the ids does not matter).
 int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
   cudaStream_t st = c.stream;
-  int r;
   L.exact = plan.exact;
   L.plain = plan.plain;
   if (plan.exact) {
@@ -955,9 +936,8 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
       if (u.nslices != 1)
         for (size_t s = u.slice; s < u.slice + u.nslices; ++s) joined += plan.slices[s].n;
     // never null, also for a run of no points: a null list means every point
-    if (!plan.runs.empty() && (r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, std::max<size_t>(joined, 1) * 4, st)))
-      return r;
-    uint32_t* at = (uint32_t*)c.d_fbits;
+    if (!plan.runs.empty()) HB_CUDA(c.d_fbits.grow(std::max<size_t>(joined, 1) * 4, st));
+    uint32_t* at = c.d_fbits.as<uint32_t>();
     for (const LegPlan::Run& u : plan.runs) {
       ExactScan scan{at, 0};
       if (u.nslices == 1)
@@ -980,8 +960,8 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
   size_t words = 0;
   for (const LegPlan::Run& u : plan.runs) words += u.host_bits ? fw : u.nset != 1 ? u.nset : 0;
   // never null, also with no words: an empty set's values are there
-  if ((r = ensure_scratch(&c.d_fbits, &c.d_fbits_bytes, tb + sb + std::max<size_t>(words, 1) * 4, st))) return r;
-  uint32_t* const at = (uint32_t*)((char*)c.d_fbits + tb + sb);
+  HB_CUDA(c.d_fbits.grow(tb + sb + std::max<size_t>(words, 1) * 4, st));
+  uint32_t* const at = (uint32_t*)(c.d_fbits.as<char>() + tb + sb);
   std::vector<RowFilter> table;
   std::vector<uint32_t> sel, vals;  // vals: the host words to upload at `at`
   for (const LegPlan::Run& u : plan.runs) {
@@ -1006,10 +986,10 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
     table.push_back(f);
   }
   if (several) {
-    HB_CUDA(cudaMemcpyAsync(c.d_fbits, table.data(), table.size() * sizeof(RowFilter), cudaMemcpyHostToDevice, st));
-    HB_CUDA(cudaMemcpyAsync((char*)c.d_fbits + tb, sel.data(), rows * 4, cudaMemcpyHostToDevice, st));
-    L.filter.table = (const RowFilter*)c.d_fbits;
-    L.filter.sel = (const uint32_t*)((char*)c.d_fbits + tb);
+    HB_CUDA(cudaMemcpyAsync(c.d_fbits.as(), table.data(), table.size() * sizeof(RowFilter), cudaMemcpyHostToDevice, st));
+    HB_CUDA(cudaMemcpyAsync(c.d_fbits.as<char>() + tb, sel.data(), rows * 4, cudaMemcpyHostToDevice, st));
+    L.filter.table = c.d_fbits.as<const RowFilter>();
+    L.filter.sel = (const uint32_t*)(c.d_fbits.as<char>() + tb);
   } else {
     L.filter.filter = table[0];
   }
@@ -1073,14 +1053,14 @@ int Index::export_layers(int lo, int hi, std::vector<LayerCsr>& out) const {
   if (lo == 0 && n) {
     a0.resize(n * 2 * M);
     a0d.resize(a0.size());
-    HB_CUDA(cudaMemcpy(a0.data(), graph_.p[GS::ADJ0], a0.size() * 4, cudaMemcpyDeviceToHost));
-    HB_CUDA(cudaMemcpy(a0d.data(), graph_.p[GS::ADJ0_D], a0d.size() * 4, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(a0.data(), graph_.at<void>(GS::ADJ0), a0.size() * 4, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(a0d.data(), graph_.at<void>(GS::ADJ0_D), a0d.size() * 4, cudaMemcpyDeviceToHost));
   }
   if (hi > 0 && n_ul) {
     aU.resize(n_ul * M);
     aUd.resize(aU.size());
-    HB_CUDA(cudaMemcpy(aU.data(), graph_.p[GS::ADJU], aU.size() * 4, cudaMemcpyDeviceToHost));
-    HB_CUDA(cudaMemcpy(aUd.data(), graph_.p[GS::ADJU_D], aUd.size() * 4, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(aU.data(), graph_.at<void>(GS::ADJU), aU.size() * 4, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(aUd.data(), graph_.at<void>(GS::ADJU_D), aUd.size() * 4, cudaMemcpyDeviceToHost));
   }
   out.assign(hi - lo + 1, LayerCsr());
   for (int l = lo; l <= hi; ++l) {
@@ -1140,7 +1120,7 @@ int Index::flatten(std::vector<uint64_t>& offsets, std::vector<uint64_t>& nb_ori
 int Index::export_vectors(void* out) const {
   if (n == 0) return 0;
   cudaSetDevice(device);
-  HB_CUDA(cudaMemcpy2D(out, (size_t)dim * es, graph_.p[GS::VEC], (size_t)row_bytes, (size_t)dim * es, n, cudaMemcpyDeviceToHost));
+  HB_CUDA(cudaMemcpy2D(out, (size_t)dim * es, graph_.at<void>(GS::VEC), (size_t)row_bytes, (size_t)dim * es, n, cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -1153,7 +1133,7 @@ int Index::get_vectors(const uint64_t* ranks, size_t count, void* out) const {
     for (e = i + 1; e < count && ranks[e] % P == p && ranks[e] / P == first + (e - i);) ++e;
     const Index* x = parts ? parts->part((int)p) : this;
     HB_CUDA(cudaSetDevice(x->device));
-    HB_CUDA(cudaMemcpy2D((char*)out + i * rb, rb, (const char*)x->graph_.p[GS::VEC] + first * x->row_bytes,
+    HB_CUDA(cudaMemcpy2D((char*)out + i * rb, rb, x->graph_.at<const char>(GS::VEC) + first * x->row_bytes,
                          (size_t)x->row_bytes, rb, e - i, cudaMemcpyDeviceToHost));
   }
   return 0;
@@ -1173,9 +1153,9 @@ int Index::check_status() {
   int any = 0;
   for (SearchCtx& c : ctx_) {
     int status = 0;
-    HB_CUDA(cudaMemcpyAsync(&status, c.d_status, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+    HB_CUDA(cudaMemcpyAsync(&status, c.d_status.as(), sizeof(int), cudaMemcpyDeviceToHost, c.stream));
     HB_CUDA(cudaStreamSynchronize(c.stream));
-    if (status) HB_CUDA(cudaMemset(c.d_status, 0, sizeof(int)));
+    if (status) HB_CUDA(cudaMemset(c.d_status.as(), 0, sizeof(int)));
     any |= status;
   }
   return any ? 1 : 0;
@@ -1190,13 +1170,13 @@ int Index::get_stats(uint64_t* out4, bool reset) {
   cudaSetDevice(device);
   unsigned long long h[4];
   HB_CUDA(cudaStreamSynchronize(stream_));
-  HB_CUDA(cudaMemcpy(h, d_stats_, sizeof(h), cudaMemcpyDeviceToHost));
+  HB_CUDA(cudaMemcpy(h, d_stats_.as(), sizeof(h), cudaMemcpyDeviceToHost));
   out4[0] = h[0];
   out4[1] = h[1];
   out4[2] = h[2];
   out4[3] = stat_queries_;
   if (reset) {
-    HB_CUDA(cudaMemset(d_stats_, 0, sizeof(h)));
+    HB_CUDA(cudaMemset(d_stats_.as(), 0, sizeof(h)));
     stat_queries_ = 0;
   }
   return 0;
@@ -1244,7 +1224,7 @@ int Index::blob_alloc(const uint64_t* h) {
 
 int Index::blob_info(int i, void** p, uint64_t* bytes) const {
   if (i < 0 || i >= GS::BLOBS) return fail("bad blob index");
-  *p = graph_.p[i];
+  *p = graph_.p[i].as();
   *bytes = (GS::DESC[i].row == GS::LISTU ? n_ul : n) * row_size(i);
   return 0;
 }
@@ -1253,10 +1233,10 @@ int Index::blob_commit() {
   cudaSetDevice(device);
   resize_points(n);
   if (n) {
-    HB_CUDA(cudaMemcpy(h_level.data(), graph_.p[GS::LEVEL], n, cudaMemcpyDeviceToHost));
-    HB_CUDA(cudaMemcpy(h_plevel.data(), graph_.p[GS::PLEVEL], n, cudaMemcpyDeviceToHost));
-    HB_CUDA(cudaMemcpy(h_origin.data(), graph_.p[GS::ORIGIN], n * 8, cudaMemcpyDeviceToHost));
-    HB_CUDA(cudaMemcpy(h_upoff.data(), graph_.p[GS::UP_OFF], n * 4, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(h_level.data(), graph_.at<void>(GS::LEVEL), n, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(h_plevel.data(), graph_.at<void>(GS::PLEVEL), n, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(h_origin.data(), graph_.at<void>(GS::ORIGIN), n * 8, cudaMemcpyDeviceToHost));
+    HB_CUDA(cudaMemcpy(h_upoff.data(), graph_.at<void>(GS::UP_OFF), n * 4, cudaMemcpyDeviceToHost));
   }
   rank_points();
   return 0;

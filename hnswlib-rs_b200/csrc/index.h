@@ -52,13 +52,69 @@ struct DeviceRestore {
     if (e__ != cudaSuccess) return cuda_fail(e__, #call); \
   } while (0)
 
-struct DevBuf {  // device memory freed on scope exit, so that no early return leaks it
-  void* p = nullptr;
-  DevBuf() = default;
-  DevBuf(const DevBuf&) = delete;
-  DevBuf& operator=(const DevBuf&) = delete;
-  ~DevBuf() { cudaFree(p); }
+// One allocation, owned: device memory (cudaMalloc) or, Pinned, page-locked host memory (cudaHostAlloc with the
+// caller's flags).  It is made on the current device and freed on that device, the caller's current device kept; an
+// empty one makes no CUDA call.  reset frees, then allocates exactly `bytes`; contents are not kept.  A failed
+// allocation leaves it empty (size 0), so that the next call allocates again.  A move swaps: the moved-from object
+// frees what the target held.
+template <bool Pinned>
+class CudaBuffer {
+ public:
+  CudaBuffer() = default;
+  CudaBuffer(CudaBuffer&& o) noexcept { *this = std::move(o); }
+  CudaBuffer& operator=(CudaBuffer&& o) noexcept {
+    std::swap(p_, o.p_), std::swap(bytes_, o.bytes_), std::swap(dev_, o.dev_);
+    return *this;
+  }
+  ~CudaBuffer() { release(); }
+  cudaError_t reset(size_t bytes, unsigned int flags = 0);
+  size_t size() const { return bytes_; }
+  template <class T = void>
+  T* as() const { return static_cast<T*>(p_); }
+
+ private:
+  void release();
+  void* p_ = nullptr;
+  size_t bytes_ = 0;
+  int dev_ = -1;
 };
+
+struct DeviceBuffer : CudaBuffer<false> {
+  // at least `need` bytes: a smaller buffer is replaced by max(need, 4 KB) once `st`, which may still read it, is idle
+  cudaError_t grow(size_t need, cudaStream_t st);
+};
+
+struct PinnedBuffer : CudaBuffer<true> {
+  cudaError_t grow(size_t need, unsigned int flags) { return need <= size() ? cudaSuccess : reset(need, flags); }
+};
+
+// A stream or an event, owned: created on the current device and destroyed on it, the caller's current device kept;
+// it reads as its handle.  An empty one makes no CUDA call.
+template <class H, cudaError_t (*Create)(H*, unsigned int), cudaError_t (*Destroy)(H)>
+class CudaHandle {
+ public:
+  CudaHandle() = default;
+  CudaHandle(const CudaHandle&) = delete;
+  CudaHandle& operator=(const CudaHandle&) = delete;
+  ~CudaHandle() {
+    if (!h_) return;
+    DeviceRestore keep;
+    cudaSetDevice(dev_);
+    Destroy(h_);
+  }
+  cudaError_t create(unsigned int flags) {
+    cudaError_t e = cudaGetDevice(&dev_);
+    if (e == cudaSuccess && (e = Create(&h_, flags)) != cudaSuccess) h_ = nullptr;
+    return e;
+  }
+  operator H() const { return h_; }
+
+ private:
+  H h_ = nullptr;
+  int dev_ = -1;
+};
+using Stream = CudaHandle<cudaStream_t, cudaStreamCreateWithFlags, cudaStreamDestroy>;
+using Event = CudaHandle<cudaEvent_t, cudaEventCreateWithFlags, cudaEventDestroy>;
 
 // The device arrays that hold the graph.  Replication blob i is array i, in this order (the order is part of the blob
 // protocol between processes); the per-point insert locks, labels and attributes come last and are not replicated.
@@ -86,10 +142,10 @@ struct GraphStore {
       {4, ONE, 0xFF},    // LABEL: the point's label, LABEL_NONE = none
       {8, ONE, 0},       // ATTR: the point's attribute, attr_bias(value), 0 = none (attr_bias(ATTR_NONE))
   };
-  void* p[COUNT] = {};
+  DeviceBuffer p[COUNT];
   size_t cap = 0, cap_ul = 0;  // points / upper-layer lists allocated
   template <class T>
-  T* at(Array a) const { return static_cast<T*>(p[a]); }
+  T* at(Array a) const { return p[a].as<T>(); }
 };
 
 // A value per point kept next to the graph (labels.cu): graph store array `array` and its host mirror, `none` for every
@@ -148,15 +204,11 @@ class FilterStore {
   struct Filter {
     std::vector<std::vector<uint32_t>> bits;  // [partition] bit per internal id (make_filter_bits)
     std::vector<size_t> counts;               // [partition] points stored when the filter was made
-    std::map<std::pair<int, int>, void*> dev;  // (partition, device) -> device copy of bits[partition]
+    std::map<std::pair<int, int>, DeviceBuffer> dev;  // (partition, device) -> device copy of bits[partition]
     // (partition, device) -> the admitted internal ids of bits[partition], sorted, on the device, and their count; made
     // at the first exact search with the filter there
-    std::map<std::pair<int, int>, std::pair<void*, size_t>> ids;
+    std::map<std::pair<int, int>, std::pair<DeviceBuffer, size_t>> ids;
   };
-  FilterStore() = default;
-  FilterStore(const FilterStore&) = delete;
-  FilterStore& operator=(const FilterStore&) = delete;
-  ~FilterStore();  // frees every device copy (the owner has synchronised its streams)
   int64_t add(Filter&& f);
   bool has(int64_t id);
   // the device copy of partition p's bitmap on rx's device (copied there on first use), after checking that the filter
@@ -473,25 +525,20 @@ class Index {
   // launches, whose last queries then overlap the next launch's first (a launch ends with a few long searches that
   // leave most SMs idle).
   struct VisitedPool {
-    uint32_t* tab = nullptr;
-    uint32_t* epoch = nullptr;
+    DeviceBuffer tab, epoch;
     size_t slots = 0, cap = 0;  // cap: the full stage; a slot also holds a first stage (visited_first_stage)
     int id_bits = 0;
     bool staged = false;  // the layout of the last launch: [first stage + full stage] per slot, or the full stage alone
   };
   struct SearchCtx {
-    cudaStream_t stream = nullptr;
-    cudaEvent_t fork = nullptr, join = nullptr, ev0 = nullptr, ev1 = nullptr;
-    unsigned int* d_counter = nullptr;
-    int* d_status = nullptr;
+    Stream stream;
+    Event fork, join, ev0, ev1;
+    DeviceBuffer d_counter, d_status;  // unsigned int, int
     VisitedPool vis, fvis;  // unfiltered / filtered searches
     // what the call's restriction uploads (stage_plan; exact: its label sets' joined id lists) / C
-    void *d_fbits = nullptr, *d_cbuf = nullptr;
-    size_t d_fbits_bytes = 0, d_cbuf_bytes = 0;
-    void *d_xq = nullptr, *d_xpart = nullptr;  // exact scan: the host batch's queries on the device / tickets and slice lists
-    size_t d_xq_bytes = 0, d_xpart_bytes = 0;
-    void *h_pin = nullptr, *h_res = nullptr;  // pinned, mapped: query staging / answers
-    size_t h_pin_bytes = 0, h_res_bytes = 0;
+    DeviceBuffer d_fbits, d_cbuf;
+    DeviceBuffer d_xq, d_xpart;  // exact scan: the host batch's queries on the device / tickets and slice lists
+    PinnedBuffer h_pin, h_res;   // pinned, mapped: query staging / answers
     bool busy = false;
     // The per-row device arrays of a launch: queries (by stored point q_ids, stored rows), the id each row leaves out
     // (skip: the launch searches k + 1), a radius launch's radii and totals, and k answer slots and a count per row
@@ -594,8 +641,6 @@ class Index {
   int ensure_visited(VisitedPool& v, size_t slots, size_t cap_entries, cudaStream_t st);
   int fill_visited_cfg(VisitedPool& v, VisitedCfg& c, bool staged, cudaStream_t st);
   bool visited_staged(size_t slots, size_t cap, size_t need, bool first_fits) const;
-  int ensure_scratch(void** p, size_t* cur, size_t need, cudaStream_t st);
-  int ensure_pinned(void** p, size_t* cur, size_t need, unsigned int flags);
   int grow_plevel(uint32_t id, int new_plevel);
   int run_insert_range(size_t first, size_t count, size_t mask_off);
   int check_insert_fit();
@@ -617,8 +662,7 @@ class Index {
   // was made at, ~0: never).  A point added since has neither a label nor an attribute, so inserts leave it current.
   struct ScanOrder {
     bool by_label, by_value;
-    void* d_ids = nullptr;
-    size_t bytes = 0;
+    DeviceBuffer d_ids{};
     uint64_t label_version = ~0ull, attr_version = ~0ull;
     std::unordered_map<uint32_t, std::pair<uint32_t, uint32_t>> groups{};
     std::vector<uint64_t> values{};
@@ -642,7 +686,8 @@ class Index {
   std::string poison_msg_;
   mutable std::string err_;
   mutable std::mutex err_mu_;
-  cudaStream_t stream_ = nullptr, own_stream_ = nullptr;
+  cudaStream_t stream_ = nullptr;  // own_stream_, or the caller's (set_stream)
+  Stream own_stream_;
   int sm_count_ = 0;
   size_t l2_bytes_ = 0;
 
@@ -674,19 +719,14 @@ class Index {
   std::mutex occ_mu_;
 
   // small device scratch (insert path; searches: SearchCtx)
-  unsigned int* d_counter_ = nullptr;
-  int* d_status_ = nullptr;
-  unsigned long long* d_stats_ = nullptr;
+  DeviceBuffer d_counter_, d_status_, d_stats_;  // unsigned int, int, unsigned long long[4]
   bool stats_on_ = false;
   std::atomic<uint64_t> stat_queries_{0};
 
-  // staging of the insert path
-  void* h_pin_ = nullptr;
-  size_t h_pin_bytes_ = 0;
+  PinnedBuffer h_pin_;  // staging of the insert path
   // (kernel, queue kind, queue slots, warps per CTA, d4, shared memory per CTA) -> CTAs per SM
   std::map<std::tuple<QueryKernel, int, int, int, int, size_t>, int> occ_cache_;
-  void* d_mask_ = nullptr;
-  size_t d_mask_bytes_ = 0;
+  DeviceBuffer d_mask_;
 };
 
 }  // namespace hb

@@ -76,17 +76,9 @@ int Index::make_order(ScanOrder& o) {
   }
   DeviceRestore keep;
   HB_CUDA(cudaSetDevice(device));
-  const size_t need = std::max<size_t>(total, 1) * 4;  // never null: a null list means every point
-  if (need > o.bytes) {
-    HB_CUDA(cudaStreamSynchronize(stream_));
-    cudaFree(o.d_ids);
-    o.d_ids = nullptr;
-    o.bytes = 0;
-    HB_CUDA(cudaMalloc(&o.d_ids, need));
-    o.bytes = need;
-  }
+  HB_CUDA(o.d_ids.grow(std::max<size_t>(total, 1) * 4, stream_));  // never null: a null list means every point
   if (total) {
-    HB_CUDA(cudaMemcpyAsync(o.d_ids, ids.data(), total * 4, cudaMemcpyHostToDevice, stream_));
+    HB_CUDA(cudaMemcpyAsync(o.d_ids.as(), ids.data(), total * 4, cudaMemcpyHostToDevice, stream_));
     HB_CUDA(cudaStreamSynchronize(stream_));
   }
   o.label_version = labels.version;
@@ -110,7 +102,7 @@ int Index::scan_slices(const uint32_t* set, size_t nset, uint64_t lo, uint64_t h
       e = std::upper_bound(v + b, v + e, hi) - v;
       if (b == e) continue;
     }
-    const ExactScan s{(const uint32_t*)o.d_ids + b, e - b};
+    const ExactScan s{o.d_ids.as<const uint32_t>() + b, e - b};
     if (slices.size() > first && slices.back().ids + slices.back().n == s.ids)
       slices.back().n += s.n;
     else

@@ -233,9 +233,9 @@ int Index::nccl_broadcast_index(int root) {
   if (!comm_) return fail("nccl_broadcast_index: call hnsw_b200_nccl_init first");
   if (root < 0 || root >= nranks_) return fail("nccl_broadcast_index: bad root");
   HB_CUDA(cudaSetDevice(device));
-  DevBuf hdr;
-  HB_CUDA(cudaMalloc(&hdr.p, 16 * sizeof(uint64_t)));
-  uint64_t* d_hdr = (uint64_t*)hdr.p;
+  DeviceBuffer hdr;
+  HB_CUDA(hdr.reset(16 * sizeof(uint64_t)));
+  uint64_t* d_hdr = hdr.as<uint64_t>();
   uint64_t header[16];
   if (rank_ == root) {
     blob_header(header);
