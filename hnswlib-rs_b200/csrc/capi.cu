@@ -45,37 +45,52 @@ static int pass(Index* ix, int r) {
   return r;
 }
 
-// HB_H: exclusive access (anything that may change the index); HB_HS: shared access (searches, read-only queries)
-#define HB_H(h) \
-  if (!(h)) return set_err("NULL handle"); \
-  Index* ix = ((const AnyApi*)(h))->ix;    \
-  std::unique_lock<std::shared_mutex> g__(ix->mu); \
-  ix->drain_pending()
-#define HB_HS(h) \
-  if (!(h)) return set_err("NULL handle"); \
-  Index* ix = ((const AnyApi*)(h))->ix;    \
-  std::shared_lock<std::shared_mutex> g__(ix->mu)
+// The locks of one call on handle h, held for the guard's scope: the handle's `mu`, then on a partitioned handle every
+// partition's in partition order, all shared (searches, read-only queries) or all exclusive (anything that may change
+// the index).  Exclusive also waits for the searches submitted on each (drain_pending).  A NULL handle is refused, and
+// the guard reads as a null Index*.
+enum Mode { SHARED, EXCLUSIVE };
+class Locked {
+ public:
+  Locked(const void* h, Mode mode) : ix_(h ? ((const AnyApi*)h)->ix : nullptr) {
+    if (!ix_) {
+      set_err("NULL handle");
+      return;
+    }
+    take(ix_, mode);
+    for (Index* x : ix_->holders())
+      if (x != ix_) take(x, mode);
+  }
+  operator Index*() const { return ix_; }
+  Index* operator->() const { return ix_; }
+
+ private:
+  void take(Index* x, Mode mode) {
+    if (mode == SHARED) {
+      shared_.emplace_back(x->mu);
+      return;
+    }
+    exclusive_.emplace_back(x->mu);
+    x->drain_pending();
+  }
+  Index* ix_;
+  std::vector<std::shared_lock<std::shared_mutex>> shared_;
+  std::vector<std::unique_lock<std::shared_mutex>> exclusive_;
+};
 
 // Partitioned handles (partition.h) and their views.  A view serves read-only calls only; a call the partitioned handle
-// cannot serve is refused before it changes anything.  A partitioned call holds the handle's lock, then every
-// partition's in partition order (HB_PARTS_SHARED for searches, HB_PARTS_EXCLUSIVE for inserts and settings).
+// cannot serve is refused before it changes anything.
 #define HB_NOT_VIEW(ix) \
   if ((ix)->owner) return set_err("a partition view is read-only")
 #define HB_NOT_PARTITIONED(ix, what) \
-  if ((ix)->parts) return set_err(std::string(what) + " is not available on a partitioned handle")
-#define HB_PARTS_SHARED(ix) const auto pl__ = (ix)->parts->lock_shared()
-#define HB_PARTS_SHARED_IF(ix) \
-  const auto pl__ = (ix)->parts ? (ix)->parts->lock_shared() : std::vector<std::shared_lock<std::shared_mutex>>()
-#define HB_PARTS_EXCLUSIVE(ix) const auto pl__ = (ix)->parts->lock_exclusive()
+  if ((ix)->partitioned()) return set_err(std::string(what) + " is not available on a partitioned handle")
 
-// a setting: on a partitioned handle it is applied to the handle and to every partition
+// a setting, applied to the handle and to every partition (the caller holds them all exclusively)
 static void apply(Index* ix, const std::function<void(Index*)>& set) {
   set(ix);
-  if (!ix->parts) return;
-  HB_PARTS_EXCLUSIVE(ix);
-  for (int p = 0; p < ix->parts->count(); ++p) set(ix->parts->part(p));
+  for (Index* x : ix->holders())
+    if (x != ix) set(x);
 }
-static uint64_t nb_point(const Index* ix) { return ix->parts ? ix->parts->nb_point() : ix->n; }
 
 static int metric_from_name(const uint8_t* name, size_t len) {
   return hb::metric_from_name(std::string((const char*)name, len));
@@ -120,16 +135,9 @@ static void insert_any(void* hv, size_t len, const void* data, size_t id) {
     set_err("insert: a partition view is read-only");
     return;
   }
-  std::unique_lock<std::shared_mutex> g(h->ix->mu);
-  h->ix->drain_pending();
+  Locked ix(h, EXCLUSIVE);
   uint64_t id64 = id;
-  if (h->ix->parts) {
-    HB_PARTS_EXCLUSIVE(h->ix);
-    pass(h->ix, h->ix->parts->insert(data, 1, len, nullptr, &id64, nullptr, (int)len));
-    return;
-  }
-  if (pass(h->ix, h->ix->set_dim((int)len))) return;
-  pass(h->ix, h->ix->insert_batch(data, 1, len, nullptr, &id64, nullptr));
+  pass(ix, ix->insert(data, 1, len, nullptr, &id64, nullptr, (int)len));
 }
 
 static void parallel_insert_any(void* hv, size_t nb_vec, size_t vec_len, const void* const* datas, const size_t* ids) {
@@ -142,16 +150,9 @@ static void parallel_insert_any(void* hv, size_t nb_vec, size_t vec_len, const v
     set_err("parallel_insert: a partition view is read-only");
     return;
   }
-  std::unique_lock<std::shared_mutex> g(h->ix->mu);
-  h->ix->drain_pending();
+  Locked ix(h, EXCLUSIVE);
   std::vector<uint64_t> id64(ids, ids + nb_vec);
-  if (h->ix->parts) {
-    HB_PARTS_EXCLUSIVE(h->ix);
-    pass(h->ix, h->ix->parts->insert(nullptr, nb_vec, vec_len, datas, id64.data(), nullptr, (int)vec_len));
-    return;
-  }
-  if (pass(h->ix, h->ix->set_dim((int)vec_len))) return;
-  pass(h->ix, h->ix->insert_batch(nullptr, nb_vec, vec_len, datas, id64.data(), nullptr));
+  pass(ix, ix->insert(nullptr, nb_vec, vec_len, datas, id64.data(), nullptr, (int)vec_len));
 }
 
 static const Neighbourhood_api* search_any(const void* hv, size_t len, const void* data, size_t knbn, size_t ef_search) {
@@ -160,12 +161,11 @@ static const Neighbourhood_api* search_any(const void* hv, size_t len, const voi
     set_err("search_neighbours: bad argument");
     return nullptr;
   }
-  std::shared_lock<std::shared_mutex> g(h->ix->mu);
-  HB_PARTS_SHARED_IF(h->ix);
+  Locked ix(h, SHARED);
   Neighbour_api* nb = (Neighbour_api*)malloc(sizeof(Neighbour_api) * knbn);
   int32_t cnt = 0;
   const AnswerArrays ans{(NeighbourOut*)nb, nullptr, nullptr, nullptr, nullptr, &cnt};
-  if (pass(h->ix, h->ix->search_batch(HostBatch{{data}, 1, (int)len, knbn, ef_search, Restriction(), false, ans}))) {
+  if (pass(ix, ix->search_batch(HostBatch{{data}, 1, (int)len, knbn, ef_search, Restriction(), false, ans}))) {
     free(nb);
     return nullptr;
   }
@@ -188,15 +188,14 @@ static const Vec_api_Neighbourhood_api* parallel_search_any(const void* hv, size
     set_err("parallel_search_neighbours: bad argument");
     return nullptr;
   }
-  std::shared_lock<std::shared_mutex> g(h->ix->mu);
-  HB_PARTS_SHARED_IF(h->ix);
+  Locked ix(h, SHARED);
   VecApiBox* box = (VecApiBox*)malloc(sizeof(VecApiBox));
   box->hoods = (Neighbourhood_api*)malloc(sizeof(Neighbourhood_api) * (nb_vec ? nb_vec : 1));
   box->block = (Neighbour_api*)malloc(sizeof(Neighbour_api) * (nb_vec ? nb_vec * knbn : 1));
   std::vector<int32_t> cnt(nb_vec);
   const AnswerArrays out{(NeighbourOut*)box->block, nullptr, nullptr, nullptr, nullptr, cnt.data()};
   // with replicas, every device answers its slice of the batch in place
-  if (pass(h->ix, h->ix->search_batch(HostBatch{{nullptr, data}, nb_vec, (int)vec_len, knbn, ef_search, Restriction(), false, out}))) {
+  if (pass(ix, ix->search_batch(HostBatch{{nullptr, data}, nb_vec, (int)vec_len, knbn, ef_search, Restriction(), false, out}))) {
     free(box->hoods);
     free(box->block);
     free(box);
@@ -290,11 +289,11 @@ static int64_t file_dump_any(const void* hv, size_t namelen, const uint8_t* file
     set_err("file_dump: NULL argument");
     return -1;
   }
-  HB_NOT_PARTITIONED(h->ix, "file_dump (dump each partition_view)");
-  std::shared_lock<std::shared_mutex> g(h->ix->mu);
+  Locked ix(h, SHARED);
+  HB_NOT_PARTITIONED(ix, "file_dump (dump each partition_view)");
   std::string used;
   // api.rs:76-78: the reference refuses to overwrite only while a dump is memory-mapped; nothing is mapped here
-  if (pass(h->ix, h->ix->file_dump(".", std::string((const char*)filename, namelen), true, &used))) return -1;
+  if (pass(ix, ix->file_dump(".", std::string((const char*)filename, namelen), true, &used))) return -1;
   return 1;
 }
 
@@ -387,7 +386,8 @@ void* hnsw_b200_load_dump(HnswIo* io, int dtype, size_t namelen, const uint8_t* 
 
 int hnsw_b200_file_dump(const void* h, const char* dir, const char* basename, int overwrite, char* used_basename,
                         size_t used_cap) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_PARTITIONED(ix, "file_dump (dump each partition_view)");
   if (!dir || !basename) return set_err("NULL path");
   std::string used;
@@ -497,7 +497,8 @@ void hnsw_b200_free_vec_api(const Vec_api_Neighbourhood_api* p) {
 
 
 int hnsw_b200_set_extend_candidates(void* h, int flag) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   if (flag && ix->ef_c <= 2 * ix->M)
     return set_err("extend_candidates needs ef_construction > 2*max_nb_connection in this engine (otherwise the "
@@ -510,35 +511,40 @@ int hnsw_b200_get_extend_candidates(const void* h) {
   return ((const AnyApi*)h)->ix->extend_candidates ? 1 : 0;
 }
 int hnsw_b200_set_keeping_pruned(void* h, int flag) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   apply(ix, [=](Index* x) { x->keep_pruned = flag != 0; });
   return 0;
 }
 int hnsw_b200_modify_level_scale(void* h, double scale) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
-  if (nb_point(ix) > 0) return set_err("modify_level_scale: index already holds points (hnsw.rs:881-888)");
+  if (ix->nb_point() > 0) return set_err("modify_level_scale: index already holds points (hnsw.rs:881-888)");
   if (!(scale >= 0.2 && scale <= 1.0)) return set_err("modify_level_scale: factor must be in [0.2, 1]");  // hnsw.rs:889-900
   apply(ix, [=](Index* x) { x->level_scale = scale / std::log((double)x->M); });
   return 0;
 }
 int hnsw_b200_set_tie_mode(void* h, int mode) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   if (mode != 0 && mode != 1) return set_err("tie mode must be 0 (distance, id) or 1 (reference std heaps)");
   apply(ix, [=](Index* x) { x->tie_std_ = mode == 1; });
   return 0;
 }
 int hnsw_b200_set_visited_stages(void* h, int mode) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   if (mode < 0 || mode > 2) return set_err("visited stages must be 0 (auto), 1 (always) or 2 (never)");
   apply(ix, [=](Index* x) { x->visited_stages_ = mode; });
   return 0;
 }
 int hnsw_b200_set_link_mode(void* h, int mode) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   if (mode != 0 && mode != 1) return set_err("link mode must be 0 (reference: new point's level) or 1 (per layer)");
   apply(ix, [=](Index* x) { x->link_mode = mode; });
@@ -549,26 +555,25 @@ int hnsw_b200_get_link_mode(const void* h) {
   return ((const AnyApi*)h)->ix->link_mode;
 }
 int hnsw_b200_set_searching_mode(void* h, int flag) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   apply(ix, [=](Index* x) { x->searching = flag != 0; });
   return 0;
 }
 int hnsw_b200_set_level_seed(void* h, uint64_t seed) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   ix->rng.s = seed;  // a partitioned handle draws every level itself, in global insertion order
   return 0;
 }
-uint64_t hnsw_b200_get_nb_point(const void* h) { return h ? nb_point(((const AnyApi*)h)->ix) : 0; }
-int hnsw_b200_get_max_level_observed(const void* h) {
-  if (!h) return 0;
-  const Index* ix = ((const AnyApi*)h)->ix;
-  return ix->parts ? ix->parts->max_level() : std::max(ix->entry_level, 0);
-}
+uint64_t hnsw_b200_get_nb_point(const void* h) { return h ? ((const AnyApi*)h)->ix->nb_point() : 0; }
+int hnsw_b200_get_max_level_observed(const void* h) { return h ? ((const AnyApi*)h)->ix->max_level() : 0; }
 int hnsw_b200_get_dim(const void* h) { return h ? ((const AnyApi*)h)->ix->dim : 0; }
 int hnsw_b200_set_insert_batching(void* h, uint32_t ratio, uint32_t max_batch) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   if (ratio == 0 || max_batch == 0) return set_err("ratio and max_batch must be positive");
   apply(ix, [=](Index* x) {
@@ -579,7 +584,8 @@ int hnsw_b200_set_insert_batching(void* h, uint32_t ratio, uint32_t max_batch) {
 }
 
 int hnsw_b200_partition(void* h, int nparts, const int* devices) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   return pass(ix, hb::Partitions::create(ix, nparts, devices));
 }
 int hnsw_b200_partition_count(const void* h) {
@@ -602,21 +608,16 @@ const void* hnsw_b200_partition_view(const void* h, int p) {
 
 int hnsw_b200_insert_flat(void* h, const void* vecs, uint64_t n, uint64_t dim, const uint64_t* ids,
                           const int32_t* levels) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   if (n == 0) return 0;
   if (!vecs) return set_err("vecs is NULL");
-  if (ix->parts) {
-    HB_PARTS_EXCLUSIVE(ix);
-    return pass(ix, ix->parts->insert(vecs, n, dim, nullptr, ids, levels, (int)dim));
-  }
-  int r;
-  if ((r = pass(ix, ix->set_dim((int)dim)))) return r;
-  return pass(ix, ix->insert_batch(vecs, n, dim, nullptr, ids, levels));
+  return pass(ix, ix->insert(vecs, n, dim, nullptr, ids, levels, (int)dim));
 }
 
-// ---- searches.  Every search entry point below is one call of search_call, which takes the handle's lock shared (and
-// every partition's), checks the arguments and runs the batch b:
+// ---- searches.  Every search entry point below is one call of search_call, which holds the handle shared (Locked),
+// checks the arguments and runs the batch b:
 //   * HOST: host rows in, host answers out, through the host batch driver; a partitioned handle searches every partition;
 //   * SUBMIT: the same, split in two (hnsw_b200_search_flat_wait collects it), so that one host thread keeps several
 //     batches in flight.  With replicas (hnsw_b200_replicate) every device gets its contiguous share enqueued at submit
@@ -628,13 +629,13 @@ int hnsw_b200_insert_flat(void* h, const void* vecs, uint64_t n, uint64_t dim, c
 // HOST call) are checked by the caller.
 enum Via { HOST, SUBMIT, DEVICE };
 static int64_t search_call(const void* h, Via via, const char* name, HostBatch b, int sync, float* kernel_ms) {
-  HB_HS(h);
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
   if (via != HOST) HB_NOT_PARTITIONED(ix, name);
   if (via == DEVICE) return pass(ix, ix->search_device(b, sync != 0, kernel_ms));
   if (via == HOST && b.nq == 0) return 0;
-  HB_PARTS_SHARED_IF(ix);
   if (const uint64_t* qids = b.in.qids) {
-    const uint64_t have = nb_point(ix);
+    const uint64_t have = ix->nb_point();
     for (uint64_t i = 0; i < b.nq; ++i)
       if (qids[i] >= have)
         return set_err(std::string(name) + ": qids[" + std::to_string(i) + "] = " + std::to_string(qids[i]) +
@@ -744,59 +745,47 @@ int hnsw_b200_search_exact_per_query(const void* h, const int64_t* filters, cons
                           true, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
 }
 
-// Point labels (and attributes).  On a partitioned handle point g (its insertion rank) is local point g / P of partition
-// g % P.
+// Point labels (and attributes), addressed by insertion rank; on a partitioned handle each partition holds its share of
+// a range by the placement rule (partition.h).
 static int label_range(const Index* ix, uint64_t first, uint64_t n, const char* what = "labels") {
-  const uint64_t have = nb_point(ix);
+  const uint64_t have = ix->nb_point();
   if (first > have || n > have - first)
     return set_err(std::string(what) + " [" + std::to_string(first) + ", " + std::to_string(first + n) + ") are out of range: the " +
                    (ix->owner ? "partition" : "index") + " holds " + std::to_string(have) + " points");
   return 0;
 }
-// calls f(index, partition, local first, count, stride, at) for each Index that holds some of the points [first, first + n):
-// its points lo .. lo + count - 1 are entries at, at + stride, ... of the caller's array
-static int for_label_range(Index* ix, uint64_t first, uint64_t n,
-                           const std::function<int(Index*, int, uint64_t, uint64_t, uint64_t, uint64_t)>& f) {
-  if (!ix->parts) return f(ix, 0, first, n, 1, 0);
-  const uint64_t P = (uint64_t)ix->parts->count();
-  for (uint64_t p = 0; p < P; ++p) {
-    const uint64_t g0 = first + (p + P - first % P) % P;  // the first rank of partition p in the range
-    if (g0 >= first + n) continue;
-    int r = f(ix->parts->part((int)p), (int)p, g0 / P, (first + n - g0 + P - 1) / P, P, g0 - first);
-    if (r) return r;
-  }
-  return 0;
-}
 // set_labels / set_attributes: column `col` of the points [first, first + n) set to value(0), ..., value(n - 1), under
-// the handle's lock and every partition's, each taken exclusively; a partition's share is every P-th value.
+// the handle's locks taken exclusively; a partition's share is every P-th value.
 // get_labels / get_attributes: out[i] = value(x, p) for the point p of Index x that is point first + i, under the
-// handle's lock and every partition's, each taken shared.
+// handle's locks taken shared.
 extern "C++" {
 namespace {
 template <class T, class F>
 int set_per_point(void* h, uint64_t first, uint64_t n, const void* values, const char* what, const char* null_msg,
                   hb::PointColumn<T> Index::*col, F value) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   if (label_range(ix, first, n, what)) return -1;
   if (n == 0) return 0;
   if (!values) return set_err(null_msg);
   hb::DeviceRestore keep;
-  const auto pl__ = ix->parts ? ix->parts->lock_exclusive() : std::vector<std::unique_lock<std::shared_mutex>>();
-  return for_label_range(ix, first, n, [&](Index* x, int part, uint64_t lo, uint64_t cnt, uint64_t stride, uint64_t at) {
-    const int r = x->set_points(x->*col, lo, cnt, [&](size_t i) { return value(at + i * stride); });
-    return pass(ix, r && ix->parts ? ix->parts->fail(part, x->err()) : r);
+  const std::vector<Index*>& hs = ix->holders();
+  return hb::for_each_share(first, n, hs.size(), [&](int p, uint64_t lo, uint64_t cnt, uint64_t at, uint64_t step) {
+    const int r = hs[p]->set_points(hs[p]->*col, lo, cnt, [&](size_t i) { return value(at + i * step); });
+    return pass(ix, r ? ix->holder_fail(p, r) : 0);
   });
 }
 template <class T, class F>
 int get_per_point(const void* h, uint64_t first, uint64_t n, T* out, const char* what, F value) {
-  HB_HS(h);
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
   if (label_range(ix, first, n, what)) return -1;
   if (n == 0) return 0;
   if (!out) return set_err("out is NULL");
-  HB_PARTS_SHARED_IF(ix);
-  return for_label_range(ix, first, n, [&](Index* x, int, uint64_t lo, uint64_t cnt, uint64_t stride, uint64_t at) {
-    for (uint64_t i = 0; i < cnt; ++i) out[at + i * stride] = value(x, lo + i);
+  const std::vector<Index*>& hs = ix->holders();
+  return hb::for_each_share(first, n, hs.size(), [&](int p, uint64_t lo, uint64_t cnt, uint64_t at, uint64_t step) {
+    for (uint64_t i = 0; i < cnt; ++i) out[at + i * step] = value(hs[p], lo + i);
     return 0;
   });
 }
@@ -1016,12 +1005,12 @@ int hnsw_b200_search_exact_radius_by_id(const void* h, const uint64_t* qids, uin
 }
 
 int hnsw_b200_get_vectors(const void* h, const uint64_t* ranks, uint64_t n, void* out) {
-  HB_HS(h);
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
   if (n == 0) return 0;
   if (!ranks) return set_err("get_vectors: ranks is NULL");
   if (!out) return set_err("get_vectors: out is NULL");
-  HB_PARTS_SHARED_IF(ix);
-  const uint64_t have = nb_point(ix);
+  const uint64_t have = ix->nb_point();
   for (uint64_t i = 0; i < n; ++i)
     if (ranks[i] >= have)
       return set_err("get_vectors: ranks[" + std::to_string(i) + "] = " + std::to_string(ranks[i]) +
@@ -1032,55 +1021,59 @@ int hnsw_b200_get_vectors(const void* h, const uint64_t* ranks, uint64_t n, void
 
 int64_t hnsw_b200_filter_new(const void* h, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,
                              hnsw_b200_filter_fn fn, void* ctx) {
-  HB_HS(h);  // shared: the points cannot change while the bitmap is made
+  Locked ix(h, SHARED);  // shared: the points cannot change while the bitmap is made
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
-  HB_PARTS_SHARED_IF(ix);
   const int64_t id = ix->new_filter(filter_mode, filter_ids, nfilter, fn, ctx);
   if (id < 0) g_err = ix->err();
   return id;
 }
 int hnsw_b200_filter_free(const void* h, int64_t filter) {
-  HB_H(h);  // exclusive: waits for every search under the shared lock and every outstanding ticket
+  Locked ix(h, EXCLUSIVE);  // exclusive: waits for every search under the shared lock and every outstanding ticket
+  if (!ix) return -1;
   return pass(ix, ix->free_filter(filter));
 }
 
 int hnsw_b200_join(void* h) {
-  HB_HS(h);
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
   return pass(ix, ix->join());
 }
 int hnsw_b200_stream_wait_last(void* h, void* cuda_stream) {
-  HB_HS(h);
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
   return pass(ix, ix->stream_wait_last((cudaStream_t)cuda_stream));
 }
 int hnsw_b200_set_stream(void* h, void* cuda_stream) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   return pass(ix, ix->set_stream((cudaStream_t)cuda_stream));
 }
 int hnsw_b200_check_status(void* h) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   int r = ix->check_status();
   if (r < 0) g_err = ix->err();
   return r;
 }
 
 int hnsw_b200_enable_stats(void* h, int enable) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   apply(ix, [=](Index* x) { x->enable_stats(enable != 0); });
   return 0;
 }
 int hnsw_b200_get_stats(const void* h, uint64_t* out4, int reset) {
-  HB_H(h);
-  if (ix->parts) {  // the sum over the partitions: out4[3] counts a query once per partition
-    HB_PARTS_EXCLUSIVE(ix);
-    return pass(ix, ix->parts->get_stats(out4, reset != 0));
-  }
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   return pass(ix, ix->get_stats(out4, reset != 0));
 }
 
 int hnsw_b200_export_points(const void* h, uint8_t* levels, int32_t* ranks, uint64_t* origin, int64_t* entry) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_PARTITIONED(ix, "export_points (export each partition_view)");
   for (size_t i = 0; i < ix->n; ++i) {
     if (levels) levels[i] = ix->h_level[i];
@@ -1091,17 +1084,17 @@ int hnsw_b200_export_points(const void* h, uint8_t* levels, int32_t* ranks, uint
   return 0;
 }
 int hnsw_b200_export_vectors(const void* h, void* out) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_PARTITIONED(ix, "export_vectors (export each partition_view)");
   return pass(ix, ix->export_vectors(out));
 }
 // FlatNeighborhood::from(&hnsw) + get_neighbours(DataId) (flatten.rs:93-126): neighbours of `origin_id` over all
 // layers, ascending distance.  Returns the number written (<= cap), -1 when the id is unknown.
 int64_t hnsw_b200_flat_neighbours(const void* h, uint64_t origin_id, Neighbour_api* out, uint64_t cap) {
-  if (!h) return set_err("NULL handle");
-  Index* ix = ((const AnyApi*)h)->ix;
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
   HB_NOT_PARTITIONED(ix, "flatten (flatten each partition_view)");
-  std::shared_lock<std::shared_mutex> g(ix->mu);
   std::vector<uint64_t> off, nbo;
   std::vector<float> nbd;
   if (pass(ix, ix->flatten(off, nbo, nbd))) return -1;
@@ -1117,10 +1110,9 @@ int64_t hnsw_b200_flat_neighbours(const void* h, uint64_t origin_id, Neighbour_a
 // whole flattened graph: offsets[nb_point+1] (internal-id order), neighbour origin ids and distances; pass NULL
 // arrays to get the total neighbour count only
 int64_t hnsw_b200_flatten(const void* h, uint64_t* offsets, uint64_t* nb_origin, float* nb_dist) {
-  if (!h) return set_err("NULL handle");
-  Index* ix = ((const AnyApi*)h)->ix;
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
   HB_NOT_PARTITIONED(ix, "flatten (flatten each partition_view)");
-  std::shared_lock<std::shared_mutex> g(ix->mu);
   std::vector<uint64_t> off, nbo;
   std::vector<float> nbd;
   if (pass(ix, ix->flatten(off, nbo, nbd))) return -1;
@@ -1131,35 +1123,38 @@ int64_t hnsw_b200_flatten(const void* h, uint64_t* offsets, uint64_t* nb_origin,
 }
 
 int64_t hnsw_b200_layer_edges(const void* h, int layer) {
-  if (!h) return set_err("NULL handle");
-  Index* ix = ((const AnyApi*)h)->ix;
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
   HB_NOT_PARTITIONED(ix, "layer_edges (export each partition_view)");
-  std::shared_lock<std::shared_mutex> g(ix->mu);
   int64_t total = 0;
   if (pass(ix, ix->export_layer(layer, nullptr, nullptr, nullptr, &total))) return -1;
   return total;
 }
 int hnsw_b200_export_layer(const void* h, int layer, uint64_t* offsets, uint32_t* ids, float* dists) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_PARTITIONED(ix, "export_layer (export each partition_view)");
   return pass(ix, ix->export_layer(layer, offsets, ids, dists, nullptr));
 }
 int hnsw_b200_import_graph(void* h, const void* vecs, uint64_t n, uint64_t dim, const uint64_t* origin,
                            const uint8_t* levels, int64_t entry, int nlayers, const uint64_t* const* offsets,
                            const uint32_t* const* ids, const float* const* dists) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   HB_NOT_PARTITIONED(ix, "import_graph");
   return pass(ix, ix->import_graph(vecs, n, (int)dim, origin, levels, entry, nlayers, offsets, ids, dists));
 }
 
 int hnsw_b200_blob_header(const void* h, uint64_t* header16) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_PARTITIONED(ix, "blob_header");
   return ix->blob_header(header16);
 }
 int hnsw_b200_blob_alloc(void* h, const uint64_t* header16) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   HB_NOT_PARTITIONED(ix, "blob_alloc");
   return pass(ix, ix->blob_alloc(header16));
@@ -1170,12 +1165,14 @@ int hnsw_b200_blob_count(const void* h) {
   return ((const AnyApi*)h)->ix->blob_count();
 }
 int hnsw_b200_blob_info(const void* h, int i, void** dev_ptr, uint64_t* nbytes) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_PARTITIONED(ix, "blob_info");
   return pass(ix, ix->blob_info(i, dev_ptr, nbytes));
 }
 int hnsw_b200_blob_commit(void* h) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   HB_NOT_PARTITIONED(ix, "blob_commit");
   return pass(ix, ix->blob_commit());
@@ -1183,7 +1180,8 @@ int hnsw_b200_blob_commit(void* h) {
 
 // ---- multi-GPU (multi.cu)
 int hnsw_b200_replicate(void* h, int ndev, const int* devices) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   HB_NOT_PARTITIONED(ix, "replicate");
   return pass(ix, ix->replicate(ndev, devices));
@@ -1194,37 +1192,39 @@ int hnsw_b200_nccl_unique_id(uint8_t* id128) {
   return Index::nccl_unique_id(id128) ? set_err("NCCL is not available (libnccl.so.2)") : 0;
 }
 int hnsw_b200_nccl_init(void* h, int nranks, int rank, const uint8_t* id128) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   HB_NOT_PARTITIONED(ix, "nccl_init");
   if (!id128) return set_err("NULL argument");
   return pass(ix, ix->nccl_init(nranks, rank, id128));
 }
 int hnsw_b200_nccl_broadcast_index(void* h, int root) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_VIEW(ix);
   HB_NOT_PARTITIONED(ix, "nccl_broadcast_index");
   return pass(ix, ix->nccl_broadcast_index(root));
 }
 int hnsw_b200_nccl_allgather(void* h, const void* d_send, void* d_recv, uint64_t bytes_per_rank, void* cuda_stream) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_PARTITIONED(ix, "nccl_allgather");
   return pass(ix, ix->nccl_allgather(d_send, d_recv, bytes_per_rank, (cudaStream_t)cuda_stream));
 }
 
 int hnsw_b200_dist_batch(const void* h, const void* queries, uint64_t nq, uint64_t dim, const uint32_t* cand,
                          uint64_t m, float* out) {
-  HB_H(h);
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
   HB_NOT_PARTITIONED(ix, "dist_batch");
   return pass(ix, ix->dist_batch(queries, nq, (int)dim, cand, m, out));
 }
 int hnsw_b200_bruteforce(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t k,
                          uint32_t* out_ids, float* out_dist) {
-  HB_H(h);
-  if (ix->parts) {  // every partition's exact answers, merged like a search; ids are global insertion ranks
-    HB_PARTS_EXCLUSIVE(ix);
-    return pass(ix, ix->parts->bruteforce(queries, nq, (int)dim, k, out_ids, out_dist));
-  }
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
+  // a partitioned handle's ids are global insertion ranks (the partitions' answers merged like a search's)
   return pass(ix, ix->bruteforce(queries, nq, (int)dim, k, out_ids, out_dist));
 }
 

@@ -3,7 +3,6 @@
 // a bitmap that is already on the device instead of one uploaded for the call.  An exact search with it runs the exact
 // scan over the filter's sorted id list, made from the bitmap at the first exact search on a device.
 #include "index.h"
-#include "partition.h"
 
 namespace hb {
 
@@ -79,11 +78,7 @@ void FilterStore::erase(int64_t id) {  // each device copy is freed on its devic
 int64_t Index::new_filter(int mode, const uint64_t* sorted_ids, size_t nids, int (*fn)(uint64_t, void*), void* ctx) {
   if (mode != 1 && mode != 2) return fail("filter_mode must be 1 (sorted origin-id list) or 2 (callback)");
   if (mode == 1 && nids && !sorted_ids) return fail("filter_ids is NULL");
-  std::vector<Index*> part;  // the Index objects that hold the points, in partition order
-  if (parts)
-    for (int p = 0; p < parts->count(); ++p) part.push_back(parts->part(p));
-  else
-    part.push_back(this);
+  const std::vector<Index*>& part = holders();
   const int P = (int)part.size();
   FilterStore::Filter f;
   f.bits.resize(P);

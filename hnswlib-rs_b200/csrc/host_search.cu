@@ -147,7 +147,7 @@ static void put_merged(const AnswerArrays& out, const std::vector<Leg>& legs, si
         P, k, cnt, [&](int p, int i) { return a[p].slots[o + i].dist; },
         [&](size_t j, int p, int i) {
           const NeighbourOut& e = a[p].slots[o + i];
-          put_answer(out, w + j, legs[p].rx, e, e.internal * (uint32_t)P + (uint32_t)p);
+          put_answer(out, w + j, legs[p].rx, e, (uint32_t)global_rank(p, e.internal, P));
         });
     for (size_t j = total; j < k; ++j) put_answer(out, w + j, nullptr, pad, INVALID_ID);
     out.counts[row] = (int32_t)total;
@@ -191,11 +191,12 @@ int Index::plan(size_t nq, std::vector<Leg>& legs) {
 
 int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>& sorted, Leg* legs, size_t n,
                    std::vector<std::vector<uint32_t>>& bits, const LabelSets* sets) {
-  const int P = parts ? parts->count() : 1;
+  const std::vector<Index*>& hs = holders();
+  const int P = (int)hs.size();
   if (rs.kind == Restriction::FILTER_T) {
     bits.resize(P);
     for (int p = 0; p < P; ++p) {
-      Index* rx = parts ? parts->part(p) : this;
+      Index* rx = hs[p];
       if (rx->make_filter_bits(rs.mode, rs.ids, rs.nids, rs.fn, rs.ctx, bits[p])) {
         for (Leg* l = legs; l < legs + n; ++l)
           if (l->rx == rx) l->rc = -1;
@@ -343,16 +344,16 @@ int Index::sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm
     const std::string e = label_set_rows(rs, nq, perm, sorted, sets);
     return e.empty() ? 0 : fail(e);
   }
-  const int P = parts ? parts->count() : 1;
+  const std::vector<Index*>& hs = holders();
+  const int P = (int)hs.size();
   const int64_t* fid = rs.filters;
   std::set<int64_t> checked;
   for (size_t i = 0; i < nq; ++i) {
     if (fid[i] == -1 || checked.count(fid[i])) continue;
     for (int p = 0; p < P; ++p) {
-      Index* rx = parts ? parts->part(p) : this;
       const uint32_t* bits = nullptr;
-      if (filters.use(fid[i], p, P, rx, &bits))
-        return fail("filters[" + std::to_string(i) + "] = " + std::to_string(fid[i]) + ": " + rx->err());
+      if (filters.use(fid[i], p, P, hs[p], &bits))
+        return fail("filters[" + std::to_string(i) + "] = " + std::to_string(fid[i]) + ": " + hs[p]->err());
     }
     checked.insert(fid[i]);
   }
@@ -413,7 +414,10 @@ static HostRows leg_rows(const HostRows& in, const Leg& l, size_t q_bytes, uint6
   if (P && s.qids) {
     if (s.skip) {
       local.resize(l.count);
-      for (size_t i = 0; i < l.count; ++i) local[i] = s.skip[i] % P == (uint64_t)l.part ? s.skip[i] / P : ~0ull;
+      for (size_t i = 0; i < l.count; ++i) {
+        const Placed at = place(s.skip[i], P);
+        local[i] = at.part == l.part ? at.local : ~0ull;
+      }
       s.skip = local.data();
     }
     s.qids = nullptr;

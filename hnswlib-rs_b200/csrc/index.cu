@@ -1126,14 +1126,14 @@ int Index::export_vectors(void* out) const {
 
 // one 2-D copy per run of consecutive ids of one partition
 int Index::get_vectors(const uint64_t* ranks, size_t count, void* out) const {
-  const uint64_t P = parts ? (uint64_t)parts->count() : 1;
+  const std::vector<Index*>& hs = holders();
   const size_t rb = (size_t)dim * es;
   for (size_t i = 0, e; i < count; i = e) {
-    const uint64_t p = ranks[i] % P, first = ranks[i] / P;
-    for (e = i + 1; e < count && ranks[e] % P == p && ranks[e] / P == first + (e - i);) ++e;
-    const Index* x = parts ? parts->part((int)p) : this;
+    const Placed at = place(ranks[i], hs.size());
+    for (e = i + 1; e < count && ranks[e] == global_rank(at.part, at.local + (e - i), hs.size());) ++e;
+    const Index* x = hs[at.part];
     HB_CUDA(cudaSetDevice(x->device));
-    HB_CUDA(cudaMemcpy2D((char*)out + i * rb, rb, x->graph_.at<const char>(GS::VEC) + first * x->row_bytes,
+    HB_CUDA(cudaMemcpy2D((char*)out + i * rb, rb, x->graph_.at<const char>(GS::VEC) + at.local * x->row_bytes,
                          (size_t)x->row_bytes, rb, e - i, cudaMemcpyDeviceToHost));
   }
   return 0;
@@ -1166,7 +1166,31 @@ int Index::enable_stats(bool on) {
   return 0;
 }
 
+size_t Index::nb_point() const {
+  size_t s = 0;
+  for (const Index* x : holders()) s += x->n;
+  return s;
+}
+
+int Index::max_level() const {
+  int m = 0;
+  for (const Index* x : holders()) m = std::max(m, x->entry_level);
+  return m;
+}
+
 int Index::get_stats(uint64_t* out4, bool reset) {
+  DeviceRestore keep;
+  const std::vector<Index*>& hs = holders();
+  std::fill(out4, out4 + 4, 0);
+  for (size_t p = 0; p < hs.size(); ++p) {
+    uint64_t s[4];
+    if (int r = hs[p]->own_stats(s, reset)) return holder_fail((int)p, r);
+    for (int i = 0; i < 4; ++i) out4[i] += s[i];
+  }
+  return 0;
+}
+
+int Index::own_stats(uint64_t* out4, bool reset) {
   cudaSetDevice(device);
   unsigned long long h[4];
   HB_CUDA(cudaStreamSynchronize(stream_));

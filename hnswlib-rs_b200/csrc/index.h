@@ -401,6 +401,10 @@ class Index {
   int draw_level();
   int insert_batch(const void* vecs, size_t n_new, size_t stride, const void* const* rows, const uint64_t* ids,
                    const int32_t* levels);
+  // a batch of the handle's, in dimension d: split over the partitions by placement (Partitions::insert), or set_dim and
+  // insert_batch on an unpartitioned handle
+  int insert(const void* vecs, size_t n_new, size_t stride, const void* const* rows, const uint64_t* ids,
+             const int32_t* levels, int d);
   int import_graph(const void* vecs, size_t n_new, int d, const uint64_t* origin, const uint8_t* levels,
                    int64_t entry_id, int nlayers, const uint64_t* const* offsets, const uint32_t* const* ids,
                    const float* const* dists);
@@ -496,6 +500,7 @@ class Index {
   int file_dump(const std::string& dir, const std::string& basename, bool overwrite, std::string* used_basename);
   int load_dump(const std::string& dir, const std::string& basename);
   int enable_stats(bool on);
+  // the work counters summed over the holders (a query counts once per partition)
   int get_stats(uint64_t* out4, bool reset);
 
   // replication blobs
@@ -605,12 +610,22 @@ class Index {
   // each partition is an Index of its own whose `owner` is that handle (the C ABI serves it read-only, as a view).
   std::unique_ptr<Partitions, PartitionsDeleter> parts;
   const Index* owner = nullptr;
+  bool partitioned() const { return parts != nullptr; }
+  // the Index objects that hold the handle's points: its partitions in partition order, or the handle itself
+  const std::vector<Index*>& holders() const;
+  // the handle's status for a failure r of holders()[p]: r itself, or on a partitioned handle its error "partition p
+  // (device D): why"
+  int holder_fail(int p, int r) const;
+  size_t nb_point() const;  // over the holders
+  int max_level() const;    // the highest level a point has, 0 when there is none
 
  private:
   friend class Partitions;
   friend class FilterStore;
   int fail(const std::string& m) const;
   int cuda_fail(cudaError_t e, const char* what) const;
+  std::vector<Index*> self_{this};  // holders() of an unpartitioned handle
+  int own_stats(uint64_t* out4, bool reset);  // this Index's counters
   // ---- graph store
   size_t row_size(int a) const;  // bytes of array a per point (per upper-layer list for ADJU, ADJU_D)
   int grow_store(bool per_list, size_t cap, size_t keep);

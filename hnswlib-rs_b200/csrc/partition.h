@@ -9,6 +9,26 @@
 
 namespace hb {
 
+// The placement rule over P partitions (P = 1: an unpartitioned handle, where a rank is its own local id).  Global rank
+// g is local id g / P of partition g % P.
+struct Placed {
+  int part;
+  uint64_t local;
+};
+inline Placed place(uint64_t g, uint64_t P) { return {(int)(g % P), g / P}; }
+inline uint64_t global_rank(int part, uint64_t local, uint64_t P) { return local * P + (uint64_t)part; }
+// f(p, lo, count, at, step) for each partition p that holds some of the ranks [first, first + n): its local ids lo ..
+// lo + count - 1 are the ranks first + at, first + at + step, ...  Returns the first nonzero f, or 0.
+template <class F>
+int for_each_share(uint64_t first, uint64_t n, uint64_t P, const F& f) {
+  for (uint64_t p = 0; p < P; ++p) {
+    const uint64_t g0 = first + (p + P - first % P) % P;  // the first rank of partition p in the range
+    if (g0 >= first + n) continue;
+    if (int r = f((int)p, g0 / P, (first + n - g0 + P - 1) / P, g0 - first, P)) return r;
+  }
+  return 0;
+}
+
 class Partitions {
  public:
   static constexpr int MAX_PARTS = 64;
@@ -16,22 +36,13 @@ class Partitions {
   static int create(Index* parent, int nparts, const int* devices);
   int count() const { return (int)ix_.size(); }
   Index* part(int p) const { return ix_[p].get(); }
+  const std::vector<Index*>& all() const { return views_; }
   // a C ABI handle on partition p: the address of a pointer to it, which is the layout of every handle
   const void* view_handle(int p) const { return &views_[p]; }
 
-  // every partition's lock in partition order (the caller holds the handle's own first); exclusive also waits for
-  // submitted searches on the partitions' views
-  std::vector<std::shared_lock<std::shared_mutex>> lock_shared() const;
-  std::vector<std::unique_lock<std::shared_mutex>> lock_exclusive() const;
-
-  size_t nb_point() const;
-  int max_level() const;
   // a batch in the engine's insert form (flat `vecs` with `stride` elements per row, or `rows`), split by placement
   int insert(const void* vecs, size_t n_new, size_t stride, const void* const* rows, const uint64_t* ids,
              const int32_t* levels, int d);
-  // exact k nearest over all partitions, merged like a search (host_search.cu); out_ids are global insertion ranks
-  int bruteforce(const void* queries, size_t nq, int d, size_t k, uint32_t* out_ids, float* out_dist);
-  int get_stats(uint64_t* out4, bool reset);
   // the handle's error "partition p (device D): why"
   int fail(int p, const std::string& why) const;
 

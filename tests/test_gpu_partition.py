@@ -67,7 +67,8 @@ def merged(answers, k):
 
 def queries(X, dtype, metric, seed):
     Q = data(dtype, metric, NQ, X.shape[1], seed + 100)
-    Q[: NQ // 10] = X[: NQ // 10]   # stored points: distance-0 answers
+    s = min(NQ // 10, len(X))
+    Q[:s] = X[:s]   # stored points: distance-0 answers
     return Q
 
 
@@ -193,15 +194,19 @@ def test_reference_entry_points_on_a_partitioned_handle(pkg, po):
 
 
 def test_bruteforce_and_recall(pkg, po):
-    # ground truth: bruteforce on a partitioned handle is exact kNN over all points, with global insertion ranks
-    X, ids, levels, h = build(pkg, po, np.float32, "DistL2", 24, 48, 3, serial=False)
-    Q = queries(X, np.float32, "DistL2", 3)
-    bi, bd = h.bruteforce(Q, 10)
-    d64 = np.sqrt(((Q[:, None, :].astype(np.float64) - X[None, :, :]) ** 2).sum(-1))   # DistL2 is the Euclidean norm
-    assert np.array_equal(bi, np.argsort(d64, axis=1, kind="stable")[:, :10].astype(np.uint32))
-    assert np.allclose(bd, np.sort(d64, axis=1)[:, :10], rtol=1e-4, atol=1e-5)
-    ti, td = po.bruteforce(X, Q, 10, "DistL2", po.ORDER_GPU)
-    assert np.array_equal(bi, ti) and np.array_equal(bd.view(np.uint32), td.view(np.uint32))
+    # ground truth: bruteforce on a partitioned handle is exact kNN over all points, with global insertion ranks; with
+    # fewer points than partitions some partitions are empty, and a query has fewer than k answers, the rest padded
+    for P, n in ((3, N), (4, 3)):
+        X, ids, levels, h = build(pkg, po, np.float32, "DistL2", 24, 48, P, serial=False, n=n)
+        Q = queries(X, np.float32, "DistL2", 3)
+        bi, bd = h.bruteforce(Q, 10)
+        d64 = np.sqrt(((Q[:, None, :].astype(np.float64) - X[None, :, :]) ** 2).sum(-1))   # DistL2 is the Euclidean norm
+        m = min(n, 10)
+        assert np.array_equal(bi[:, :m], np.argsort(d64, axis=1, kind="stable")[:, :m].astype(np.uint32)), P
+        assert np.allclose(bd[:, :m], np.sort(d64, axis=1)[:, :m], rtol=1e-4, atol=1e-5), P
+        assert (bi[:, m:] == INV).all() and np.isinf(bd[:, m:]).all(), P
+        ti, td = po.bruteforce(X, Q, 10, "DistL2", po.ORDER_GPU)
+        assert np.array_equal(bi, ti) and np.array_equal(bd.view(np.uint32), td.view(np.uint32)), P
     # recall on 50 000 clustered points, four partitions on one device, against the unpartitioned index
     n, d = 50000, 64
     X = pkg.datagen.clustered(n, d, 21)
