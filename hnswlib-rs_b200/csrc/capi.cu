@@ -85,13 +85,6 @@ class Locked {
 #define HB_NOT_PARTITIONED(ix, what) \
   if ((ix)->partitioned()) return set_err(std::string(what) + " is not available on a partitioned handle")
 
-// a setting, applied to the handle and to every partition (the caller holds them all exclusively)
-static void apply(Index* ix, const std::function<void(Index*)>& set) {
-  set(ix);
-  for (Index* x : ix->holders())
-    if (x != ix) set(x);
-}
-
 static int metric_from_name(const uint8_t* name, size_t len) {
   return hb::metric_from_name(std::string((const char*)name, len));
 }
@@ -503,18 +496,18 @@ int hnsw_b200_set_extend_candidates(void* h, int flag) {
   if (flag && ix->ef_c <= 2 * ix->M)
     return set_err("extend_candidates needs ef_construction > 2*max_nb_connection in this engine (otherwise the "
                    "extension set of hnsw.rs:1336-1362 is not provably empty)");
-  apply(ix, [=](Index* x) { x->extend_candidates = flag != 0; });
+  ix->settings().extend_candidates = flag != 0;
   return 0;
 }
 int hnsw_b200_get_extend_candidates(const void* h) {
   if (!h) return set_err("NULL handle");
-  return ((const AnyApi*)h)->ix->extend_candidates ? 1 : 0;
+  return ((const AnyApi*)h)->ix->settings().extend_candidates ? 1 : 0;
 }
 int hnsw_b200_set_keeping_pruned(void* h, int flag) {
   Locked ix(h, EXCLUSIVE);
   if (!ix) return -1;
   HB_NOT_VIEW(ix);
-  apply(ix, [=](Index* x) { x->keep_pruned = flag != 0; });
+  ix->settings().keep_pruned = flag != 0;
   return 0;
 }
 int hnsw_b200_modify_level_scale(void* h, double scale) {
@@ -523,7 +516,7 @@ int hnsw_b200_modify_level_scale(void* h, double scale) {
   HB_NOT_VIEW(ix);
   if (ix->nb_point() > 0) return set_err("modify_level_scale: index already holds points (hnsw.rs:881-888)");
   if (!(scale >= 0.2 && scale <= 1.0)) return set_err("modify_level_scale: factor must be in [0.2, 1]");  // hnsw.rs:889-900
-  apply(ix, [=](Index* x) { x->level_scale = scale / std::log((double)x->M); });
+  ix->settings().level_scale = scale / std::log((double)ix->M);
   return 0;
 }
 int hnsw_b200_set_tie_mode(void* h, int mode) {
@@ -531,7 +524,7 @@ int hnsw_b200_set_tie_mode(void* h, int mode) {
   if (!ix) return -1;
   HB_NOT_VIEW(ix);
   if (mode != 0 && mode != 1) return set_err("tie mode must be 0 (distance, id) or 1 (reference std heaps)");
-  apply(ix, [=](Index* x) { x->tie_std_ = mode == 1; });
+  ix->settings().tie_std = mode == 1;
   return 0;
 }
 int hnsw_b200_set_visited_stages(void* h, int mode) {
@@ -539,7 +532,7 @@ int hnsw_b200_set_visited_stages(void* h, int mode) {
   if (!ix) return -1;
   HB_NOT_VIEW(ix);
   if (mode < 0 || mode > 2) return set_err("visited stages must be 0 (auto), 1 (always) or 2 (never)");
-  apply(ix, [=](Index* x) { x->visited_stages_ = mode; });
+  ix->settings().visited_stages = mode;
   return 0;
 }
 int hnsw_b200_set_link_mode(void* h, int mode) {
@@ -547,18 +540,17 @@ int hnsw_b200_set_link_mode(void* h, int mode) {
   if (!ix) return -1;
   HB_NOT_VIEW(ix);
   if (mode != 0 && mode != 1) return set_err("link mode must be 0 (reference: new point's level) or 1 (per layer)");
-  apply(ix, [=](Index* x) { x->link_mode = mode; });
+  ix->settings().link_mode = mode;
   return 0;
 }
 int hnsw_b200_get_link_mode(const void* h) {
   if (!h) return set_err("NULL handle");
-  return ((const AnyApi*)h)->ix->link_mode;
+  return ((const AnyApi*)h)->ix->settings().link_mode;
 }
-int hnsw_b200_set_searching_mode(void* h, int flag) {
+int hnsw_b200_set_searching_mode(void* h, int) {  // nothing in this engine depends on the mode
   Locked ix(h, EXCLUSIVE);
   if (!ix) return -1;
   HB_NOT_VIEW(ix);
-  apply(ix, [=](Index* x) { x->searching = flag != 0; });
   return 0;
 }
 int hnsw_b200_set_level_seed(void* h, uint64_t seed) {
@@ -576,10 +568,8 @@ int hnsw_b200_set_insert_batching(void* h, uint32_t ratio, uint32_t max_batch) {
   if (!ix) return -1;
   HB_NOT_VIEW(ix);
   if (ratio == 0 || max_batch == 0) return set_err("ratio and max_batch must be positive");
-  apply(ix, [=](Index* x) {
-    x->batch_ratio = ratio;
-    x->batch_max = max_batch;
-  });
+  ix->settings().batch_ratio = ratio;
+  ix->settings().batch_max = max_batch;
   return 0;
 }
 
@@ -1062,7 +1052,7 @@ int hnsw_b200_enable_stats(void* h, int enable) {
   Locked ix(h, EXCLUSIVE);
   if (!ix) return -1;
   HB_NOT_VIEW(ix);
-  apply(ix, [=](Index* x) { x->enable_stats(enable != 0); });
+  ix->settings().stats = enable != 0;
   return 0;
 }
 int hnsw_b200_get_stats(const void* h, uint64_t* out4, int reset) {

@@ -127,7 +127,7 @@ int Index::file_dump(const std::string& dir, const std::string& basename_default
   g.put<uint32_t>(MAGICDESCR_4);
   g.put<uint8_t>(1);                 // DumpMode::Full
   g.put<uint8_t>((uint8_t)M);        // get_max_nb_connection() as u8 (256 wraps to 0 upstream too)
-  g.put<double>(level_scale);        // v4: level scale
+  g.put<double>(settings().level_scale);  // v4: level scale
   g.put<uint8_t>((uint8_t)max_layer);
   g.put<uint64_t>((uint64_t)ef_c);
   g.put<uint64_t>((uint64_t)n);
@@ -367,10 +367,10 @@ int Index::load_dump(const std::string& dir, const std::string& basename) {
   ef_c = (int)de.ef;
   // the reference re-applies the stored scale as a FACTOR of 1/ln(M) on reload (hnswio.rs:773-777 with
   // hnsw.rs:339-352): levels drawn for points inserted after a reload follow that law, mirrored here
-  level_scale = (1.0 / std::log((double)M)) * de.level_scale;
+  settings().level_scale = (1.0 / std::log((double)M)) * de.level_scale;
   int r = import_graph(vecs.data(), N, (int)D, origin.data(), levels.data(), entry_id, nl, po.data(), pi.data(), pd.data());
   if (r) return r;
-  if (ef_c > 2 * M) extend_candidates = true;  // hnswio.rs:510,599: reloaded indexes extend candidates
+  if (ef_c > 2 * M) settings().extend_candidates = true;  // hnswio.rs:510,599: reloaded indexes extend candidates
   return 0;
 }
 

@@ -45,7 +45,7 @@ Index::Index(int M_, size_t max_elements_, int max_layer_, int ef_c_, int metric
       es(dtype_size(dtype_)), device(device_),
       max_elements(max_elements_) {
   for (int l = 0; l < MAX_LAYERS; ++l) layer_count[l] = 0;
-  level_scale = 1.0 / std::log((double)M);  // hnsw.rs:327
+  settings_.level_scale = 1.0 / std::log((double)M);  // hnsw.rs:327
   int ndev = 0;
   cudaError_t e = cudaGetDeviceCount(&ndev);
   if (e != cudaSuccess || ndev <= 0) {
@@ -85,6 +85,11 @@ Index::Index(int M_, size_t max_elements_, int max_layer_, int ef_c_, int metric
   cudaMemset(d_stats_.as(), 0, 4 * sizeof(unsigned long long));
   cudaMemset(d_status_.as(), 0, sizeof(int));
   ok_ = true;
+}
+
+Index::Index(Index* handle, size_t max_elements_, int device_)
+    : Index(handle->M, max_elements_, handle->max_layer, handle->ef_c, handle->metric, handle->dtype, device_) {
+  handle_ = handle;
 }
 
 // The members free themselves, each on its own device; before they do, every stream that may still read them is idle.
@@ -237,7 +242,8 @@ int Index::fill_visited_cfg(VisitedPool& v, VisitedCfg& c, bool staged, cudaStre
 // single-stage.  At c2 the window is 8 KB and fits; c1, c3 and c4 are single-stage by the rule above anyway.
 bool Index::visited_staged(size_t slots, size_t cap, size_t need, bool first_fits) const {
   if (!first_fits) return false;
-  if (visited_stages_ != 0) return visited_stages_ == 1;
+  const int mode = settings().visited_stages;
+  if (mode != 0) return mode == 1;
   return slots * cap * sizeof(uint32_t) > l2_bytes_ && visited_first_stage(cap) * 5 >= need * 2;
 }
 
@@ -266,7 +272,7 @@ GraphView Index::view() const {
 int Index::draw_level() {
   double xsi = rng.unif();
   if (xsi <= 0.) xsi = 1e-300;
-  double level = -std::log(xsi) * level_scale;
+  double level = -std::log(xsi) * settings().level_scale;
   size_t ul = (size_t)std::floor(level);
   if (ul >= (size_t)max_layer) ul = (size_t)(rng.next() % (uint64_t)max_layer);
   return (int)ul;
@@ -356,12 +362,13 @@ int Index::run_insert_range(size_t first, size_t count, size_t mask_off) {
   p.count = (uint32_t)count;
   p.layer_mask = d_mask_.as<const uint16_t>() + mask_off;
   p.ef_c = ef_c;
-  p.keep_pruned = keep_pruned ? 1 : 0;
-  p.extend = extend_candidates ? 1 : 0;
-  p.link_mode = link_mode;
+  const Settings& set = settings();
+  p.keep_pruned = set.keep_pruned ? 1 : 0;
+  p.extend = set.extend_candidates ? 1 : 0;
+  p.link_mode = set.link_mode;
   p.work_counter = d_counter_.as<unsigned int>();
   p.locks = graph_.at<int>(GS::LOCKS);
-  p.stats = stats_on_ ? d_stats_.as<unsigned long long>() : nullptr;  // insert-path distance evaluations / expansions / adjacency ids read
+  p.stats = set.stats ? d_stats_.as<unsigned long long>() : nullptr;  // insert-path distance evaluations / expansions / adjacency ids read
   p.status = d_status_.as<int>();
   const InsertShape s = insert_shape();
   p.q_kind = s.q_kind;
@@ -471,7 +478,8 @@ int Index::insert_batch(const void* vecs, size_t n_new, size_t stride, const voi
       continue;
     }
     const size_t linked = first + done;
-    size_t nb = std::min<size_t>(std::max<size_t>(linked / std::max<uint32_t>(batch_ratio, 1), 1), batch_max);
+    const Settings& set = settings();
+    size_t nb = std::min<size_t>(std::max<size_t>(linked / std::max<uint32_t>(set.batch_ratio, 1), 1), set.batch_max);
     nb = std::min(nb, n_new - done);
     bool promo = false;
     for (size_t j = 0; j < nb; ++j) {
@@ -687,6 +695,7 @@ int Index::stream_wait_last(cudaStream_t s) {
 int Index::search_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, size_t k, size_t ef_arg,
                          const LaunchFilter& f, bool sync, float* kernel_ms) {
   cudaStream_t st = c.stream;
+  const Settings& set = settings();
   SearchParams p;
   p.g = view();
   p.queries = rows.d_queries;
@@ -708,12 +717,12 @@ int Index::search_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, s
   p.filter_table = f.table;
   p.filter_sel = f.sel;
   p.filter = f.filter;
-  p.stats = stats_on_ ? d_stats_.as<unsigned long long>() : nullptr;
+  p.stats = set.stats ? d_stats_.as<unsigned long long>() : nullptr;
   p.status = c.d_status.as<int>();
   const bool filtered = f.sel != nullptr || f.filter.ptr != nullptr || f.filter.attr != nullptr;
   QueryKernel kind = QueryKernel::Generic;
   if (filtered) kind = QueryKernel::Filtered;
-  else if (tie_std_) kind = QueryKernel::StdTie;  // unfiltered searches only
+  else if (set.tie_std) kind = QueryKernel::StdTie;  // unfiltered searches only
   else if (entry != INVALID_ID && lean_eligible(p.g.d4, p.ef) && lean_op_supported(metric, dtype)) kind = QueryKernel::Lean;
   p.q_kind = kind == QueryKernel::Generic ? queue_kind(p.ef, metric, dtype) : 0;
   p.q_smem = query_queue_slots(kind, p.q_kind, p.ef);
@@ -798,7 +807,7 @@ int Index::search_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, s
     HB_CUDA(cudaMemsetAsync(c.d_status.as(), 0, sizeof(int), st));
     vcap = pool.cap * 2;
   }
-  if (stats_on_) stat_queries_ += nq;
+  if (set.stats) stat_queries_ += nq;
   return 0;
 }
 
@@ -1161,11 +1170,6 @@ int Index::check_status() {
   return any ? 1 : 0;
 }
 
-int Index::enable_stats(bool on) {
-  stats_on_ = on;
-  return 0;
-}
-
 size_t Index::nb_point() const {
   size_t s = 0;
   for (const Index* x : holders()) s += x->n;
@@ -1180,13 +1184,18 @@ int Index::max_level() const {
 
 int Index::get_stats(uint64_t* out4, bool reset) {
   DeviceRestore keep;
-  const std::vector<Index*>& hs = holders();
   std::fill(out4, out4 + 4, 0);
-  for (size_t p = 0; p < hs.size(); ++p) {
+  auto add = [&](Index* x) {
     uint64_t s[4];
-    if (int r = hs[p]->own_stats(s, reset)) return holder_fail((int)p, r);
-    for (int i = 0; i < 4; ++i) out4[i] += s[i];
-  }
+    const int r = x->own_stats(s, reset);
+    for (int i = 0; r == 0 && i < 4; ++i) out4[i] += s[i];
+    return r;
+  };
+  const std::vector<Index*>& hs = holders();
+  for (size_t p = 0; p < hs.size(); ++p)
+    if (int r = add(hs[p])) return holder_fail((int)p, r);
+  for (auto& rep : replicas_)
+    if (add(rep.get())) return fail("replica: " + rep->err());
   return 0;
 }
 

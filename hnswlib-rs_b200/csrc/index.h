@@ -367,22 +367,34 @@ struct Leg {
   LegPlan plan;
 };
 
+// A handle's settings (its setters, hnsw.rs:810-905).  One value, on the handle; its partitions and replicas read it
+// through Index::settings(), so a setting made before or after partitioning or replicating applies to all of them.
+struct Settings {
+  bool extend_candidates = false, keep_pruned = false;
+  int link_mode = 0;       // hnsw_b200_set_link_mode: 0 back-links under the new point's level (hnsw.rs:1257), 1 per layer
+  bool tie_std = false;    // hnsw_b200_set_tie_mode: equal-distance ties resolved like the reference's std BinaryHeaps (search_std.cu)
+  int visited_stages = 0;  // hnsw_b200_set_visited_stages: 0 auto (first stage when the tables outgrow L2), 1 always, 2 never
+  bool stats = false;      // hnsw_b200_enable_stats: launches add their work to the counters of the Index they run on
+  double level_scale;      // 1/ln(M) * factor (the Index constructor sets factor 1)
+  uint32_t batch_ratio = 16, batch_max = 16384;  // hnsw_b200_set_insert_batching
+};
+
 class Index {
  public:
   Index(int M, size_t max_elements, int max_layer, int ef_c, int metric, int dtype, int device);
+  // a partition or replica of `handle` on `device`, sized for max_elements points: the handle's configuration, and the
+  // handle's settings through settings()
+  Index(Index* handle, size_t max_elements, int device);
   ~Index();
   bool ok() const { return ok_; }
 
-  // ---- configuration (Hnsw::new and setters, hnsw.rs:771-905)
+  // ---- configuration (Hnsw::new, hnsw.rs:771-790)
   int M, max_layer, ef_c, metric, dtype, es, device;  // es = bytes per element
   size_t max_elements;
-  bool extend_candidates = false, keep_pruned = false, searching = false;
-  int link_mode = 0;      // hnsw_b200_set_link_mode: 0 back-links under the new point's level (hnsw.rs:1257), 1 per layer
-  int visited_stages_ = 0;  // hnsw_b200_set_visited_stages: 0 auto (first stage when the tables outgrow L2), 1 always, 2 never
-  bool tie_std_ = false;  // hnsw_b200_set_tie_mode: equal-distance ties resolved like the reference's std BinaryHeaps (search_std.cu)
-  double level_scale;  // 1/ln(M) * factor
   SplitMix64 rng{397};
-  uint32_t batch_ratio = 16, batch_max = 16384;
+  // the settings of the handle this Index serves: its own on a handle, the handle's on a partition or a replica
+  const Settings& settings() const { return handle_->settings_; }
+  Settings& settings() { return handle_->settings_; }
 
   // ---- state
   int dim = 0, row_bytes = 0;  // row_bytes = dim*es rounded up to whole 128-byte lines
@@ -499,8 +511,7 @@ class Index {
   // dump / reload in the reference's two-file format (hnswio.cu)
   int file_dump(const std::string& dir, const std::string& basename, bool overwrite, std::string* used_basename);
   int load_dump(const std::string& dir, const std::string& basename);
-  int enable_stats(bool on);
-  // the work counters summed over the holders (a query counts once per partition)
+  // the work counters summed over the holders (a query counts once per partition) and the replicas
   int get_stats(uint64_t* out4, bool reset);
 
   // replication blobs
@@ -607,7 +618,8 @@ class Index {
   mutable std::shared_mutex mu;
 
   // ---- partitions (partition.cu).  A partitioned handle keeps its settings and level RNG here and its points in `parts`;
-  // each partition is an Index of its own whose `owner` is that handle (the C ABI serves it read-only, as a view).
+  // each partition is an Index of its own whose `owner` is that handle (the C ABI serves it read-only, as a view).  A
+  // replica has no owner: it is never handed out.
   std::unique_ptr<Partitions, PartitionsDeleter> parts;
   const Index* owner = nullptr;
   bool partitioned() const { return parts != nullptr; }
@@ -624,6 +636,8 @@ class Index {
   friend class FilterStore;
   int fail(const std::string& m) const;
   int cuda_fail(cudaError_t e, const char* what) const;
+  Settings settings_;       // a handle's settings (unused on a partition or a replica)
+  Index* handle_ = this;    // the handle whose settings_ settings() reads
   std::vector<Index*> self_{this};  // holders() of an unpartitioned handle
   int own_stats(uint64_t* out4, bool reset);  // this Index's counters
   // ---- graph store
@@ -735,7 +749,6 @@ class Index {
 
   // small device scratch (insert path; searches: SearchCtx)
   DeviceBuffer d_counter_, d_status_, d_stats_;  // unsigned int, int, unsigned long long[4]
-  bool stats_on_ = false;
   std::atomic<uint64_t> stat_queries_{0};
 
   PinnedBuffer h_pin_;  // staging of the insert path

@@ -93,10 +93,15 @@ int Index::broadcast_to_replicas() {
   blob_header(header);
   int r;
   for (auto& rep : replicas_) {
-    if (rep->n != 0) {  // a stale copy: start from an empty index of the same configuration
+    if (rep->n != 0) {  // a stale copy: start from an empty replica on the same device, with the old one's counters
+      uint64_t s[4];
+      if ((r = rep->own_stats(s, false))) return fail("replica: " + rep->err());
       const int dev = rep->device;
-      rep.reset(new Index(M, max_elements, max_layer, ef_c, metric, dtype, dev));
+      rep.reset(new Index(this, max_elements, dev));
       if (!rep->ok()) return fail("replica: " + rep->err());
+      HB_CUDA(cudaSetDevice(dev));
+      HB_CUDA(cudaMemcpy(rep->d_stats_.as(), s, 3 * sizeof(uint64_t), cudaMemcpyHostToDevice));
+      rep->stat_queries_ = s[3];
     }
     if ((r = rep->blob_alloc(header))) return fail("replica: " + rep->err());
   }
@@ -126,7 +131,6 @@ int Index::broadcast_to_replicas() {
     HB_CUDA(cudaSetDevice(rep->device));
     HB_CUDA(cudaStreamSynchronize(rep->stream_));
     if ((r = rep->blob_commit())) return fail("replica: " + rep->err());
-    rep->searching = true;
   }
   HB_CUDA(cudaSetDevice(device));
   replicas_stale_ = false;
@@ -149,7 +153,7 @@ int Index::replicate(int ndev, const int* devices) {
   drop_replicas();
   if (ndev == 1) return 0;
   for (int i = 1; i < ndev; ++i) {
-    replicas_.emplace_back(new Index(M, max_elements, max_layer, ef_c, metric, dtype, devices[i]));
+    replicas_.emplace_back(new Index(this, max_elements, devices[i]));
     if (!replicas_.back()->ok()) {
       const std::string why = replicas_.back()->err();
       drop_replicas();
@@ -253,10 +257,7 @@ int Index::nccl_broadcast_index(int root) {
     if (bytes) HB_NCCL(nc.Broadcast(ptr, ptr, bytes, ncclChar, root, (ncclComm_t)comm_, stream_));
   }
   HB_CUDA(cudaStreamSynchronize(stream_));
-  if (rank_ != root) {
-    if ((r = blob_commit())) return r;
-    searching = true;
-  }
+  if (rank_ != root && (r = blob_commit())) return r;
   return 0;
 }
 

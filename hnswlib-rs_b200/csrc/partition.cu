@@ -41,19 +41,9 @@ int Partitions::create(Index* parent, int nparts, const int* devices) {
   std::unique_ptr<Partitions, PartitionsDeleter> ps(new Partitions(parent));
   const size_t cap = (parent->max_elements + nparts - 1) / nparts;
   for (int p = 0; p < nparts; ++p) {
-    std::unique_ptr<Index> ix(new Index(parent->M, cap, parent->max_layer, parent->ef_c, parent->metric, parent->dtype, devices[p]));
+    // the level RNG stays with the handle (levels are drawn in global order)
+    std::unique_ptr<Index> ix(new Index(parent, cap, devices[p]));
     if (!ix->ok()) return parent->fail("partition " + std::to_string(p) + ": " + ix->err());
-    // the settings made on the handle so far; the level RNG stays with the handle (levels are drawn in global order)
-    ix->extend_candidates = parent->extend_candidates;
-    ix->keep_pruned = parent->keep_pruned;
-    ix->link_mode = parent->link_mode;
-    ix->searching = parent->searching;
-    ix->tie_std_ = parent->tie_std_;
-    ix->visited_stages_ = parent->visited_stages_;
-    ix->level_scale = parent->level_scale;
-    ix->batch_ratio = parent->batch_ratio;
-    ix->batch_max = parent->batch_max;
-    ix->stats_on_ = parent->stats_on_;
     if (parent->dim) ix->set_dim(parent->dim);
     ix->owner = parent;
     ps->ix_.push_back(std::move(ix));

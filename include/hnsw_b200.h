@@ -595,7 +595,8 @@ int hnsw_b200_blob_commit(void* h); /* after the broadcasts: pull the small host
  * device) to devices[1..ndev) with ncclBroadcast.  Afterwards hnsw_b200_search_flat and parallel_search_neighbours_<ty> on
  * `h` split a batch of >= 64 * ndev queries into ndev contiguous shards; every device copies its shard in, searches it and
  * writes its slice of the caller's output arrays (input order kept, no gather step).  Inserting into `h` marks the copies
- * stale; they are re-broadcast before the next sharded search.  ndev = 1 drops the copies. */
+ * stale; they are re-broadcast before the next sharded search.  ndev = 1 drops the copies.  Settings made on `h` before
+ * or after this call apply on every device, and hnsw_b200_get_stats sums the counters of every device. */
 int hnsw_b200_replicate(void* h, int ndev, const int* devices);
 int hnsw_b200_replica_count(const void* h);
 /* One process per GPU.  Rank 0 calls hnsw_b200_nccl_unique_id and hands the 128 bytes to the other ranks by the host's own
@@ -614,7 +615,7 @@ int hnsw_b200_nccl_allgather(void* h, const void* d_send, void* d_recv, uint64_t
  *
  * Split an EMPTY handle into nparts partitions, partition p on devices[p] (devices[0] = the handle's device).
  * A device may be named more than once: several partitions then share one GPU.  Refused on a non-empty, replicated or
- * NCCL-initialised handle.  Settings made before the call are copied to the partitions.
+ * NCCL-initialised handle.  Settings made on the handle before or after the call apply to every partition.
  *   Placement: the g-th point inserted into the handle, counted over all insert calls, goes to partition g % P as that
  *     partition's local id g / P.  Levels are drawn once, in global insertion order, from the handle's RNG (explicit
  *     levels are passed through), so a partitioned build draws the levels an unpartitioned build of the same sequence
@@ -630,7 +631,7 @@ int hnsw_b200_nccl_allgather(void* h, const void* d_send, void* d_recv, uint64_t
  *     insertion rank; out_pid is the PointId (level, rank) in the answering partition's own graph.  A filter callback
  *     (mode 2) is called on the calling thread only, once per stored origin id over all partitions.
  *   hnsw_b200_bruteforce merges every partition's exact answers by the same rule and returns global insertion ranks.
- *   Setters apply to every partition.  get_nb_point is the sum over the partitions, get_max_level_observed the max,
+ *   get_nb_point is the sum over the partitions, get_max_level_observed the max,
  *     get_stats the sum (out[3] counts each query once per partition).
  *   Refused with an error and no change: hnsw_b200_replicate, hnsw_b200_nccl_*, search_flat_submit / _wait,
  *     search_device, dist_batch, file_dump*, export_*, layer_edges, flatten, flat_neighbours, import_graph, blob_*.
