@@ -90,6 +90,11 @@ struct ExactParams {
   const uint64_t* skip_ids;  // as SearchParams': k is knbn + 1 and each row of `out` knbn wide
   const float* radius;       // radius mode: [nq] per launch row, each >= 0 and not NaN (nullptr: k-NN)
   uint32_t* totals;          // radius mode: [nq] per launch row, zero at launch: the admitted points within the radius
+  // nullptr, or per launch row its excluded points in excluded_ids (as SearchParams'): a key is a candidate only when it
+  // beats its query's threshold and its id is not in the row's list, so the list is searched only for keys that would
+  // enter the queue
+  const ExcludedRow* excluded;
+  const uint32_t* excluded_ids;
 };
 
 // keys[0, c) (~0 = none) into the warp's sorted queue Q, 32 at a time: those Q accepts, inserted in lane order.  The keys
@@ -108,6 +113,10 @@ __device__ __forceinline__ void queue_offer(SortedQueue& Q, const uint64_t* keys
     }
   }
   __syncwarp();
+}
+
+__device__ __forceinline__ bool in_excluded(ExcludedRow x, const uint32_t* ids, uint32_t id) {
+  return x.n && in_sorted(ids + x.off, x.n, id);
 }
 
 template <class Op, int CH>
@@ -207,7 +216,8 @@ __global__ void __launch_bounds__(256, 2) exact_knn_kernel(ExactParams p) {
       const float dist = reduce8<Op>(a, p.g.dim);
       if (g == 0 && row_ok && q < nqt) {
         const uint64_t key = make_key(Op::post(dist), id);
-        if (key < thr[q]) cand[q * B + atomicAdd(&ccount[q], 1)] = key;
+        if (key < thr[q] && !(p.excluded && in_excluded(p.excluded[q0 + q], p.excluded_ids, id)))
+          cand[q * B + atomicAdd(&ccount[q], 1)] = key;
       }
     }
     __syncthreads();  // the slot is read and the candidates are in
@@ -313,6 +323,8 @@ int Index::exact_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, si
   p.skip_ids = rows.skip;
   p.radius = rows.radius;
   p.totals = rows.totals;
+  p.excluded = rows.excluded;
+  p.excluded_ids = rows.excluded_ids;
   p.out = rows.out;
   p.counts = rows.counts;
   k += rows.skip ? 1 : 0;  // the scan keeps k + 1 keys, each row is k wide (write_row)

@@ -949,6 +949,36 @@ int hnsw_b200_search_device_by_id(const void* h, int exact, int64_t filter, cons
                     nullptr, nullptr, sync, kernel_ms);
 }
 
+// Excluded points per query: host queries under one_restriction's restriction, row i without the points of qx[qx_off[i],
+// qx_off[i + 1]) (insertion ranks; their check against nb_point runs under the handle's lock, Index::exclusion_lists)
+static int excluding_call(const void* h, const char* name, HostBatch b, const uint64_t* qx_off, const uint64_t* qx,
+                          int64_t filter, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset) {
+  OneLabelSets one;
+  if (int s = first_checks(h, name, b.nq, false, nullptr, nullptr, nullptr)) return s < 0 ? -1 : 0;
+  if (!qx_off) return set_err(std::string(name) + ": qx_off is NULL");
+  if (!qx) return set_err(std::string(name) + ": qx is NULL");
+  if (one_restriction(name, b.nq, filter, qrange, qset_off, qset, one, b.restriction)) return -1;
+  b.excluded = {qx_off, qx};
+  return (int)search_call(h, HOST, name, b, 1, nullptr);
+}
+int hnsw_b200_search_flat_excluding(const void* h, const uint64_t* qx_off, const uint64_t* qx, int64_t filter,
+                                    const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                                    const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
+                                    uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
+                                    int32_t* out_counts) {
+  return excluding_call(h, "search_flat_excluding", {{queries}, nq, (int)dim, knbn, ef_search, Restriction(), false,
+                        columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, qx_off, qx, filter, qrange,
+                        qset_off, qset);
+}
+int hnsw_b200_search_exact_excluding(const void* h, const uint64_t* qx_off, const uint64_t* qx, int64_t filter,
+                                     const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                                     const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids,
+                                     float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
+  return excluding_call(h, "search_exact_excluding", {{queries}, nq, (int)dim, knbn, 0, Restriction(), true,
+                        columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, qx_off, qx, filter, qrange,
+                        qset_off, qset);
+}
+
 // Radius search: the exact scan of host queries or of stored points (by_id), under one_restriction's restriction, each
 // row cut at its radius and its total of points within it into out_total (may be NULL).  knbn == 0 counts only: the
 // scan runs at k = 1 into scratch rows, the caller's row arrays may be NULL, and every count is 0.

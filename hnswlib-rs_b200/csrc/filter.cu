@@ -11,26 +11,12 @@
 // (consumed entries are overwritten with ~0).  W is the same sorted shared-memory array as elsewhere.
 // The FilterT predicate (filter.rs:7-24) is a device bitmap over internal ids, materialised by the host, or a point
 // label: the predicate label(p) == L, or label(p) in a set S of labels, over the label array of the graph store; and,
-// alone or with a label part, a range lo <= attr(p) <= hi over the attribute array of the graph store.
+// alone or with a label part, a range lo <= attr(p) <= hi over the attribute array of the graph store.  A row may also
+// name points it never admits (its excluded list, binary-searched), on top of its run's predicate or alone.
 #include "kernels.h"
 #include "search_core.cuh"
 
 namespace hb {
-
-// x is one of the sorted values v[0, n): a binary search in global memory
-__device__ __forceinline__ bool in_sorted(const uint32_t* v, uint32_t n, uint32_t x) {
-  while (n) {
-    const uint32_t h = n >> 1, m = __ldg(v + h);
-    if (m == x) return true;
-    if (m < x) {
-      v += h + 1;
-      n -= h + 1;
-    } else {
-      n = h;
-    }
-  }
-  return false;
-}
 
 __device__ __noinline__ bool in_sorted_call(const uint32_t* v, uint32_t n, uint32_t x) { return in_sorted(v, n, x); }
 
@@ -45,9 +31,20 @@ template <> struct SetLookupCall<OpCast<int32_t, OpL2>> { static constexpr bool 
 template <> struct SetLookupCall<OpCast<uint32_t, OpL2>> { static constexpr bool value = true; };
 template <> struct SetLookupCall<OpJaccard<uint8_t>> { static constexpr bool value = true; };
 template <> struct SetLookupCall<OpJaccard<uint16_t>> { static constexpr bool value = true; };
+// A row's excluded points (RowFilter::excl) are looked up once per point, where it is scored: for a chunk of fresh
+// neighbours before their distances (excluded_flags), and for the entry point when the search starts (xep).  Every
+// other point of W entered it past that test, so W's later tests (keep_passing, the single-element clear, write_row's
+// post-filter) only compare the id with xep (member_pass).  A lookup inside filter_pass at those sites made the generic
+// u16 L1 and u32 Jaccard kernels spill (78 / 74 registers became 64 and 100 / 84 bytes spilled, inlined or called
+// alike).
+template <class Op>
+__device__ __forceinline__ bool in_excluded(const RowFilter* f, uint32_t id) {
+  if constexpr (SetLookupCall<Op>::value) return in_sorted_call(f->excl, f->nexcl, id);
+  return in_sorted(f->excl, f->nexcl, id);
+}
 
-// the one admission test: the point's attribute against the query's range, then the point's label against the query's
-// label or set, or its bit of the bitmap
+// the admission test of the run's predicate: the point's attribute against the query's range, then its label against
+// the query's label or set, or its bit of the bitmap
 template <class Op>
 __device__ __forceinline__ bool filter_pass(const RowFilter* f, uint32_t id) {
   const uint64_t* attr = f->attr;
@@ -67,6 +64,12 @@ __device__ __forceinline__ bool filter_pass(const RowFilter* f, uint32_t id) {
   return (__ldg(f->ptr + (id >> 5)) >> (id & 31)) & 1u;
 }
 
+// the admission test of a member of W: not the excluded entry point, and the run's predicate
+template <class Op>
+__device__ __forceinline__ bool member_pass(const RowFilter* f, uint32_t id) {
+  return id != f->xep && filter_pass<Op>(f, id);
+}
+
 // keeps the keys w[0, n) whose points pass the filter, in order, at the front of w; returns how many there are
 template <class Op>
 __device__ __forceinline__ int keep_passing(uint64_t* w, int n, const RowFilter* fslot) {
@@ -78,7 +81,7 @@ __device__ __forceinline__ int keep_passing(uint64_t* w, int n, const RowFilter*
     bool keep = false;
     if (i < n) {
       v = w[i];
-      keep = filter_pass<Op>(fslot, key_id(v));
+      keep = member_pass<Op>(fslot, key_id(v));
     }
     const unsigned m = __ballot_sync(FULL, keep);
     __syncwarp();
@@ -92,7 +95,7 @@ __device__ __forceinline__ int keep_passing(uint64_t* w, int n, const RowFilter*
 template <class Op, int CH, int U>
 __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const WarpSmem& s, const VisitedCfg& vc, Visited& vis,
                                                       SortedQueue& W, uint64_t* cbuf, uint32_t ccap,
-                                                      const RowFilter* fslot, uint32_t ep, int ef, int layer,
+                                                      RowFilter* fslot, uint32_t ep, int ef, int layer,
                                                       Stats& st, bool& overflow) {
   const int lane = lane_id();
   const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
@@ -107,6 +110,8 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
   }
   W.n = 1;
   uint32_t cn = 1;
+  // ep enters W before any test; if the row excludes it, every later test of W's members rejects it (member_pass)
+  if (lane == 0 && fslot->nexcl && in_excluded<Op>(fslot, ep)) fslot->xep = ep;
   __syncwarp();
   for (;;) {
     // ---- C.pop(): nearest candidate (hnsw.rs:971)
@@ -156,13 +161,17 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
       if (cnt) {
         const int pos = __popc(m & ((1u << lane) - 1u));
         if (fresh) s.cand_id[pos] = nid;
+        // the chunk's excluded flags, in the unused upper half of the candidate-id region (nothing stays in a register
+        // across the distances)
+        uint32_t* const excluded_flags = s.cand_id + 32;
+        if (fresh && fslot->nexcl) excluded_flags[pos] = in_excluded<Op>(fslot, nid);
         __syncwarp();
         warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, cnt, s.cand_d);  // 1026
         __syncwarp();
         st.evals += cnt;
         const uint32_t my_id = lane < cnt ? s.cand_id[lane] : 0u;
         const uint64_t key = lane < cnt ? make_key(Op::post(s.cand_d[lane]), my_id) : ~0ull;
-        const bool my_pass = lane < cnt && filter_pass<Op>(fslot, my_id);
+        const bool my_pass = lane < cnt && !(fslot->nexcl && excluded_flags[lane]) && filter_pass<Op>(fslot, my_id);
         const unsigned passmask = __ballot_sync(FULL, my_pass);
         for (int j = 0; j < cnt; ++j) {  // strictly in list order: the accept rule sees the W of that moment
           if (W.n == 0) {                // 1019-1024
@@ -179,7 +188,7 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
             if (lane == 0) __stcg(cbuf + cn, kj);  // 1035-1036: every accepted candidate goes to C
             cn += 1;
             if ((passmask >> j) & 1u) {  // 1040-1049
-              if (W.n == 1 && !filter_pass<Op>(fslot, key_id(W.w[0]))) W.n = 0;
+              if (W.n == 1 && !member_pass<Op>(fslot, key_id(W.w[0]))) W.n = 0;
               __syncwarp();
               W.insert(kj);  // push, and pop the farthest when over ef (1051-1053)
             }
@@ -221,7 +230,15 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
     const uint32_t qi = next_item(p.work_counter, lane);
     if (qi >= p.nq) break;
     stage_row_bytes(s.q4, query_row(g, p.q_ids, p.queries, p.q_stride_bytes, qi), p.q_bytes, g.d4 * 16);
-    if (lane == 0) *fslot = p.filter_sel ? p.filter_table[p.filter_sel[qi]] : p.filter;
+    if (lane == 0) {
+      *fslot = p.filter_sel ? p.filter_table[p.filter_sel[qi]] : p.filter;
+      fslot->xep = INVALID_ID;
+      if (p.excluded) {  // the row's own part: its excluded points
+        const ExcludedRow x = p.excluded[qi];
+        fslot->excl = p.excluded_ids + x.off;
+        fslot->nexcl = x.n;
+      }
+    }
     __syncwarp();
     int count = 0;
     bool overflow = false;
@@ -239,7 +256,7 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
     }
     // post-filter AFTER truncation (hnsw.rs:1549-1563): only the entry point can fail here
     write_row(p.out_nb, p.out_count, g.origin, p.k, p.skip_ids, qi, lane, count, [&](int j) { return W.w[j]; },
-              [&](uint32_t id) { return filter_pass<Op>(fslot, id); });
+              [&](uint32_t id) { return member_pass<Op>(fslot, id); });
   }
   vis.save(p.vis, slot, lane);
   flush_stats(p.stats, st, lane);

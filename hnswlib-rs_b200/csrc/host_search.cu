@@ -204,7 +204,7 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
       }
     }
   }
-  // run u of leg l under `key`, a resident filter or a label set; exact: its slices appended to the plan's
+  // run u of leg l under `key`, a resident filter, a label set or every point; exact: its slices appended to the plan's
   auto restrict_run = [&](Leg& l, int64_t key, LegPlan::Run& u) {
     if (rs.kind == Restriction::FILTER_T) {
       u.host_bits = bits[l.part].data();
@@ -212,8 +212,10 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
     }
     std::vector<ExactScan>& slices = l.plan.slices;
     u.slice = slices.size();
-    int r;
-    if (rs.kind == Restriction::ROW_LABEL_SETS) {
+    int r = 0;
+    if (key == EVERY_POINT) {  // graph batches only: an exact batch applies its lists in the scan (prepare_batch)
+      u.every = true;
+    } else if (rs.kind == Restriction::ROW_LABEL_SETS) {
       u.set = sets->values.data() + sets->off[key];
       u.nset = (uint32_t)(sets->off[key + 1] - sets->off[key]);
       u.lo = sets->range[2 * key];
@@ -231,7 +233,7 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
   for (Leg* l = legs; l < legs + n; ++l) {  // every leg, so that the caller reports the failure it chooses
     LegPlan& pl = l->plan;
     pl.exact = exact;
-    if (!rs.per_row()) {  // every row unrestricted, or one run over every row
+    if (!rs.per_row() && sorted.empty()) {  // every row unrestricted, or one run over every row
       LegPlan::Run u{0, l->count};
       if (rs.kind == Restriction::NONE)
         pl.plain = l->count;
@@ -365,6 +367,33 @@ int Index::sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm
   return 0;
 }
 
+// Row i's list is copied, sorted and de-duplicated (as label_set_rows treats a set) after its ranks are checked.  The
+// ranks are this Index's: a partitioned handle's global ones, split per partition by leg_rows.
+int Index::exclusion_lists(const Exclusions& x, size_t nq, Ticket& t) {
+  const uint64_t have = nb_point();
+  t.xrows.resize(nq);
+  t.xids.clear();
+  for (size_t i = 0; i < nq; ++i) {
+    const uint64_t lo = x.off[i], hi = x.off[i + 1];
+    if (hi < lo)
+      return fail("excluded list " + std::to_string(i) + ": qx_off[" + std::to_string(i + 1) + "] = " + std::to_string(hi) +
+                  " is below qx_off[" + std::to_string(i) + "] = " + std::to_string(lo));
+    for (uint64_t j = lo; j < hi; ++j)
+      if (x.ids[j] >= have)
+        return fail("excluded list " + std::to_string(i) + ": qx[" + std::to_string(j) + "] = " + std::to_string(x.ids[j]) +
+                    " is not below nb_point = " + std::to_string(have));
+    const size_t at = t.xids.size();
+    t.xids.insert(t.xids.end(), x.ids + lo, x.ids + hi);  // below nb_point, so below 2^32
+    if (hi - lo > 1) {
+      std::sort(t.xids.begin() + at, t.xids.end());
+      t.xids.erase(std::unique(t.xids.begin() + at, t.xids.end()), t.xids.end());
+    }
+    if (t.xids.size() > UINT32_MAX) return fail("the excluded lists hold more than 2^32 - 1 distinct ids in all");
+    t.xrows[i] = ExcludedRow{(uint32_t)at, (uint32_t)(t.xids.size() - at)};
+  }
+  return 0;
+}
+
 // The handle's error for the first failed leg of legs[0, n) (0 if none failed): in leg order, or the replicas' before the
 // root's (replicas_first, the synchronous sharded search's order).  A partition's and a replica's message name it.
 int Index::legs_fail(const Leg* legs, size_t n, bool replicas_first) {
@@ -379,11 +408,13 @@ int Index::legs_fail(const Leg* legs, size_t n, bool replicas_first) {
 }
 
 // The batch's rows in sorted-row order (row j: caller row perm[j]): every present column copied in that order into
-// `store`, flat queries as row pointers into them (q_bytes apart), and skip still the ids when it was
+// `store`, flat queries as row pointers into them (q_bytes apart), skip still the ids when it was, and the excluded ids
+// where they were
 static HostRows sorted_rows(const HostRows& in, const std::vector<size_t>& perm, size_t q_bytes,
                             std::vector<unsigned char>& store) {
   const size_t nq = perm.size();
-  store.resize(nq * (sizeof(void*) + 2 * sizeof(uint64_t) + sizeof(float)));  // room for every column, 8-byte ones first
+  // room for every column, 8-byte ones first
+  store.resize(nq * (sizeof(void*) + 2 * sizeof(uint64_t) + sizeof(ExcludedRow) + sizeof(float)));
   unsigned char* at = store.data();
   auto column = [&](auto value) {  // the next column of `store`: row j holds value(perm[j])
     unsigned char* c = at;
@@ -400,17 +431,39 @@ static HostRows sorted_rows(const HostRows& in, const std::vector<size_t>& perm,
     });
   if (in.qids) s.qids = (const uint64_t*)column([&](size_t i) { return in.qids[i]; });
   if (in.skip) s.skip = in.skip == in.qids ? s.qids : (const uint64_t*)column([&](size_t i) { return in.skip[i]; });
+  if (in.excluded) s.excluded = (const ExcludedRow*)column([&](size_t i) { return in.excluded[i]; });
   if (in.radius) s.radius = (const float*)column([&](size_t i) { return in.radius[i]; });
+  s.excluded_ids = in.excluded_ids;
+  s.nexcluded_ids = in.nexcluded_ids;
   return s;
 }
 
 // Leg l's rows: rows [l.first, l.first + l.count) of the batch's, flat queries q_bytes apart.  A batch by stored point on
 // a partitioned handle (P partitions; 0: none) runs on its rows gathered into the queries, and a row leaves out its
-// point only on the partition that holds it, as that partition's local id (made in `local`).
-static HostRows leg_rows(const HostRows& in, const Leg& l, size_t q_bytes, uint64_t P, std::vector<uint64_t>& local) {
+// point only on the partition that holds it, as that partition's local id (made in `local`).  On a partitioned handle
+// a row's excluded points are those of its list that the leg's partition holds, as its local ids (made in `xrows` and
+// `xids`; the list ascends, and so does its part: local id g / P of global rank g).
+static HostRows leg_rows(const HostRows& in, const Leg& l, size_t q_bytes, uint64_t P, std::vector<uint64_t>& local,
+                         std::vector<ExcludedRow>& xrows, std::vector<uint32_t>& xids) {
   const size_t j = l.first;
   HostRows s{in.queries ? (const char*)in.queries + j * q_bytes : nullptr, in.rows ? in.rows + j : nullptr,
-             in.qids ? in.qids + j : nullptr, in.skip ? in.skip + j : nullptr, in.radius ? in.radius + j : nullptr};
+             in.qids ? in.qids + j : nullptr, in.skip ? in.skip + j : nullptr, in.radius ? in.radius + j : nullptr,
+             in.excluded ? in.excluded + j : nullptr, in.excluded_ids, in.nexcluded_ids};
+  if (P && s.excluded) {
+    xrows.resize(l.count);
+    for (size_t i = 0; i < l.count; ++i) {
+      const ExcludedRow x = s.excluded[i];
+      const size_t at = xids.size();
+      for (uint32_t e = 0; e < x.n; ++e) {
+        const Placed g = place(s.excluded_ids[x.off + e], P);
+        if (g.part == l.part) xids.push_back((uint32_t)g.local);
+      }
+      xrows[i] = ExcludedRow{(uint32_t)at, (uint32_t)(xids.size() - at)};
+    }
+    s.excluded = xrows.data();
+    s.excluded_ids = xids.data();
+    s.nexcluded_ids = xids.size();
+  }
   if (P && s.qids) {
     if (s.skip) {
       local.resize(l.count);
@@ -428,7 +481,9 @@ static HostRows leg_rows(const HostRows& in, const Leg& l, size_t q_bytes, uint6
 void Index::begin_leg(const HostBatch& b, Leg& l) {
   if (l.ctx < 0) l.ctx = l.rx->acquire_ctx();
   std::vector<uint64_t> local;
-  const HostRows in = leg_rows(b.in, l, (size_t)b.d * es, parts ? parts->count() : 0, local);
+  std::vector<ExcludedRow> xrows;
+  std::vector<uint32_t> xids;
+  const HostRows in = leg_rows(b.in, l, (size_t)b.d * es, parts ? parts->count() : 0, local, xrows, xids);
   l.rc = l.rx->search_host_begin(l.ctx, in, l.count, b.d, b.k, b.ef, l.plan);
   l.begun = l.rc == 0;
 }
@@ -458,8 +513,10 @@ int Index::end_leg(Leg& l, const HostBatch& b) {
 // The batch `call` planned into t's legs, each with its plan; t.b is the batch as the legs run it.  A per-row
 // restriction: the batch is planned over the rows sorted by filter or label set (sorted_rows), and each answer goes
 // back to its caller's row.  A batch by stored point on a partitioned handle has its rows gathered from their
-// partitions first, since no device reads another partition's store, and is then searched as host queries.  A leg that
-// could not have its plan is reported in leg order, or the replicas' first.
+// partitions first, since no device reads another partition's store, and is then searched as host queries.  Excluded
+// points ride with their rows; in a graph batch the unrestricted rows that exclude points are moved from the
+// unrestricted prefix into a run over every point, after the rows that stay there.  A leg that could not have its plan
+// is reported in leg order, or the replicas' first.
 int Index::prepare_batch(const HostBatch& call, Ticket& t, bool replicas_first) {
   if (parts && dim != 0 && call.d != dim) return fail("query length differs from the index dimension");
   int r;
@@ -470,9 +527,29 @@ int Index::prepare_batch(const HostBatch& call, Ticket& t, bool replicas_first) 
     if ((r = get_vectors(call.in.qids, call.nq, t.gathered.data()))) return r;
     b.in.queries = t.gathered.data();
   }
+  const Restriction& rs = call.restriction;
+  if (call.excluded.off) {
+    if ((r = exclusion_lists(call.excluded, call.nq, t))) return r;
+    b.in.excluded = t.xrows.data();
+    b.in.excluded_ids = t.xids.data();
+    b.in.nexcluded_ids = t.xids.size();
+  }
+  const bool every = call.excluded.off && !call.exact && (rs.kind == Restriction::NONE || rs.per_row());
   std::vector<int64_t> sorted;
-  if (call.restriction.per_row()) {
-    if ((r = sort_rows(call.restriction, call.nq, t.perm, sorted, t.sets))) return r;
+  if (rs.per_row() || every) {
+    if (rs.per_row() && (r = sort_rows(rs, call.nq, t.perm, sorted, t.sets))) return r;
+    if (!rs.per_row()) {
+      t.perm.resize(call.nq);
+      std::iota(t.perm.begin(), t.perm.end(), (size_t)0);
+      sorted.assign(call.nq, -1);
+    }
+    if (every) {
+      size_t plain = 0;
+      while (plain < call.nq && sorted[plain] == -1) ++plain;
+      const auto listed = std::stable_partition(t.perm.begin(), t.perm.begin() + plain,
+                                                [&](size_t i) { return t.xrows[i].n == 0; });
+      std::fill(sorted.begin() + (listed - t.perm.begin()), sorted.begin() + plain, EVERY_POINT);
+    }
     b.in = sorted_rows(b.in, t.perm, (size_t)b.d * es, t.rows);
     b.out.perm = t.perm.data();
   }

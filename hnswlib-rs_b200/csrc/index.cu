@@ -704,6 +704,8 @@ int Index::search_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, s
   p.nq = (uint32_t)nq;
   p.q_ids = rows.q_ids;
   p.skip_ids = rows.skip;
+  p.excluded = rows.excluded;
+  p.excluded_ids = rows.excluded_ids;
   k += rows.skip ? 1 : 0;  // the search takes k + 1, each row is k wide (write_row)
   p.k = (int)k;
   p.ef = (int)std::max(ef_arg, k);  // hnsw.rs:1531
@@ -719,7 +721,8 @@ int Index::search_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, s
   p.filter = f.filter;
   p.stats = set.stats ? d_stats_.as<unsigned long long>() : nullptr;
   p.status = c.d_status.as<int>();
-  const bool filtered = f.sel != nullptr || f.filter.ptr != nullptr || f.filter.attr != nullptr;
+  // rows with excluded points run filtered, also under a filter that admits every point (LegPlan::Run::every)
+  const bool filtered = f.sel != nullptr || f.filter.ptr != nullptr || f.filter.attr != nullptr || rows.excluded != nullptr;
   QueryKernel kind = QueryKernel::Generic;
   if (filtered) kind = QueryKernel::Filtered;
   else if (set.tie_std) kind = QueryKernel::StdTie;  // unfiltered searches only
@@ -837,16 +840,21 @@ int Index::search_host_begin(int ci, const HostRows& in, size_t nq, int d, size_
   if (!in.qids && dim != 0 && d != dim) return fail("query length differs from the index dimension");
   int r;
   // Per-row columns: by stored point the ids, and the ids the rows leave out, cross the bus in place of the rows (16 bytes
-  // a query at most), as do a radius launch's radii.  Those go in with one copy, from after the queries in the pinned
-  // buffer to after an exact launch's rows in device memory; the totals follow there and come back after the status.
-  enum { IDS, SKIP, RADIUS, TOTALS, COLUMNS };
+  // a query at most), as do a radius launch's radii and the rows' excluded points (a row's offset and count, and the
+  // one list of them all).  Those go in with one copy, from after the queries in the pinned buffer to after an exact
+  // launch's rows in device memory; the totals follow there and come back after the status.
+  enum { IDS, SKIP, EXCLUDED, RADIUS, EXCLUDED_IDS, TOTALS, COLUMNS };
   struct Column {
     const void* host;  // the values that go in (the totals come out; skip == qids is the ids' column)
-    size_t bytes;      // a row (0: absent)
-  } col[COLUMNS] = {{in.qids, in.qids ? 8u : 0u}, {in.skip, in.skip && in.skip != in.qids ? 8u : 0u},
-                    {in.radius, in.radius ? 4u : 0u}, {nullptr, in.radius ? 4u : 0u}};
+    size_t bytes;      // all rows' (0: absent); the 8-byte columns come first
+  } col[COLUMNS] = {{in.qids, in.qids ? 8 * nq : 0},
+                    {in.skip, in.skip && in.skip != in.qids ? 8 * nq : 0},
+                    {in.excluded, in.excluded ? sizeof(ExcludedRow) * nq : 0},
+                    {in.radius, in.radius ? 4 * nq : 0},
+                    {in.excluded_ids, in.excluded ? 4 * in.nexcluded_ids : 0},
+                    {nullptr, in.radius ? 4 * nq : 0}};
   size_t at[COLUMNS + 1] = {};  // column i at at[i]: at[TOTALS] bytes go in, at[COLUMNS] in all
-  for (int i = 0; i < COLUMNS; ++i) at[i + 1] = at[i] + col[i].bytes * nq;
+  for (int i = 0; i < COLUMNS; ++i) at[i + 1] = at[i] + col[i].bytes;
   // [answers][counts][status, 16 bytes][totals]
   const size_t out_bytes = nq * k * sizeof(NeighbourOut), cnt_bytes = nq * sizeof(int32_t), tot_bytes = at[COLUMNS] - at[TOTALS];
   HB_CUDA(c.h_res.grow(out_bytes + cnt_bytes + 16 + tot_bytes, cudaHostAllocMapped | cudaHostAllocPortable));
@@ -885,7 +893,7 @@ int Index::search_host_begin(int ci, const HostRows& in, size_t nq, int d, size_
       if (!d_queries) return fail("the pinned query staging buffer has no device address");
     }
     for (int i = IDS; i < TOTALS; ++i)
-      if (col[i].bytes) memcpy(stage + staged + at[i], col[i].host, col[i].bytes * nq);
+      if (col[i].bytes) memcpy(stage + staged + at[i], col[i].host, col[i].bytes);
   }
   L.rows.d_queries = d_queries;
   // an exact launch may run many CTAs per query (row slices): the queries cross the bus once, into device memory
@@ -900,6 +908,8 @@ int Index::search_host_begin(int ci, const HostRows& in, size_t nq, int d, size_
     L.rows.q_ids = (const uint64_t*)on_device(IDS);
     L.rows.skip = (const uint64_t*)on_device(in.skip == in.qids ? IDS : SKIP);
     L.rows.radius = (const float*)on_device(RADIUS);
+    L.rows.excluded = (const ExcludedRow*)on_device(EXCLUDED);
+    L.rows.excluded_ids = (const uint32_t*)on_device(EXCLUDED_IDS);
     L.rows.totals = (uint32_t*)on_device(TOTALS);
   }
   if (plan.exact) *c.pend.hstatus = 0;
@@ -978,6 +988,8 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
     if (u.host_bits) {
       f.ptr = at + vals.size();
       vals.insert(vals.end(), u.host_bits, u.host_bits + fw);
+    } else if (u.every) {
+      f.ptr = nullptr;  // no predicate: each row's excluded points alone
     } else if (u.nset == 1 && u.set[0] == LABEL_NONE) {
       f.ptr = nullptr;  // a range alone
     } else if (u.nset == 1) {
@@ -1018,7 +1030,9 @@ int Index::run_plan(SearchCtx& c, const SearchCtx::Launch& L, bool sync, float* 
   }
   if (L.exact) return exact_on_ctx(c, L.rows, L.nq, L.k, L.groups, sync, kernel_ms);
   int r;
-  if (L.plain && (r = search_on_ctx(c, L.rows, L.plain, L.k, L.ef, LaunchFilter(), sync, kernel_ms))) return r;
+  SearchCtx::Rows plain = L.rows;
+  plain.excluded = nullptr;  // the unrestricted rows exclude no point (prepare_batch)
+  if (L.plain && (r = search_on_ctx(c, plain, L.plain, L.k, L.ef, LaunchFilter(), sync, kernel_ms))) return r;
   if (L.plain == L.nq) return 0;
   return search_on_ctx(c, L.rows.from(L.plain, (size_t)dim * es, L.k), L.nq - L.plain, L.k, L.ef, L.filter, sync, kernel_ms);
 }

@@ -299,15 +299,27 @@ struct LabelSets {
 
 // What each row of a host batch brings in, a column per field (nullptr: absent): its query (flat, a row pointer, or by
 // stored point the stored vector of qids[i], an insertion rank, a partitioned handle's global one); the id it leaves out
-// (skip, ~0: none; qids itself for exclude_self; write_row, search_core.cuh); and in an exact batch the radius it holds
-// the points within (>= 0, not NaN), reporting how many of its points are.  A new column is a field here and in
-// SearchCtx::Rows, a line in sorted_rows and leg_rows (host_search.cu), and an entry in search_host_begin's staging list.
+// (skip, ~0: none; qids itself for exclude_self; write_row, search_core.cuh); in an exact batch the radius it holds
+// the points within (>= 0, not NaN), reporting how many of its points are; and the points it never returns (excluded:
+// an ExcludedRow per row into excluded_ids[0, nexcluded_ids), the one list of every row's ascending, distinct internal
+// ids, which stays in place when the rows are permuted or sliced).  A new column is a field here and in SearchCtx::Rows,
+// a line in sorted_rows and leg_rows (host_search.cu), and an entry in search_host_begin's staging list.
 struct HostRows {
   const void* queries = nullptr;
   const void* const* rows = nullptr;
   const uint64_t* qids = nullptr;
   const uint64_t* skip = nullptr;
   const float* radius = nullptr;
+  const ExcludedRow* excluded = nullptr;
+  const uint32_t* excluded_ids = nullptr;
+  size_t nexcluded_ids = 0;
+};
+
+// The caller's excluded points of a batch: row i's are the distinct values of ids[off[i], off[i + 1]) in any order,
+// insertion ranks (a partitioned handle's global ones); off == nullptr: none (Index::exclusion_lists reads them)
+struct Exclusions {
+  const uint64_t* off = nullptr;
+  const uint64_t* ids = nullptr;
 };
 
 // What each row of a leg takes out (search_host_finish): k answer slots and a count per row, and a radius batch's
@@ -320,7 +332,8 @@ struct HostAnswers {
 };
 
 // One host search batch: the rows `in`, k answers each into `out`.  `exact`: the exact scan of the points each row may
-// return (ef unused) instead of the graph search.
+// return (ef unused) instead of the graph search.  `excluded`: each row's points left out on top of its restriction
+// (made into in.excluded when the batch is planned).
 struct HostBatch {
   HostRows in;
   size_t nq = 0;
@@ -329,6 +342,7 @@ struct HostBatch {
   Restriction restriction;
   bool exact = false;
   AnswerArrays out;
+  Exclusions excluded;
 };
 
 // A leg's restriction (Index::resolve): its rows [0, plain) are unrestricted, and `runs` cover the rest, each a range of
@@ -336,10 +350,12 @@ struct HostBatch {
 // uploaded into the context when the leg begins) or a label set on `labels` (the label array on the leg's device), the
 // latter within an attribute range on `attrs` unless its lo is 0.  In an exact batch its points are slices [slice,
 // slice + nslices): a filter's id list, or a label set's and range's slices of an exact-scan order.  A batch-wide filter
-// is a plan with no prefix and one run over every row.
+// is a plan with no prefix and one run over every row.  Graph rows that exclude points and have no other restriction
+// are a run over every point (`every`), so that they run in the filtered kernel, which reads their lists.
 struct LegPlan {
   struct Run {
     size_t first, count;
+    bool every = false;
     const uint32_t* bits = nullptr;
     const uint32_t* host_bits = nullptr;
     const uint32_t* set = nullptr;  // the run's label set, nset values of a LabelSets
@@ -426,7 +442,8 @@ class Index {
   HostAnswers search_host_finish(int c);
   // host search batches (host_search.cu): synchronous, or submitted now and collected by finish_batch.  A ticket is a
   // batch `b` planned into legs, with what the legs read until they are collected: a per-row batch's caller row of each
-  // sorted row (out.perm) and its sorted rows, a FilterT's host bits per partition, and a label-set batch's sets.
+  // sorted row (out.perm) and its sorted rows, a FilterT's host bits per partition, a label-set batch's sets, and the
+  // rows' excluded points.
   struct Ticket {
     std::vector<Leg> legs;
     HostBatch b;
@@ -435,6 +452,8 @@ class Index {
     std::vector<unsigned char> gathered;  // a partitioned batch by stored point: the query rows read from their partitions
     std::vector<std::vector<uint32_t>> bits;
     LabelSets sets;
+    std::vector<ExcludedRow> xrows;  // per caller row, into xids (exclusion_lists)
+    std::vector<uint32_t> xids;
   };
   int search_batch(const HostBatch& b);
   int64_t submit_batch(const HostBatch& b);  // a ticket id, or < 0
@@ -445,7 +464,8 @@ class Index {
     while (pending_.load() != 0) std::this_thread::yield();
   }
   // the plan of each of legs[0, n) under `rs`; `sorted` holds a per-row restriction's keys (a filter id or a set of
-  // `sets`, -1: none) in the order the legs run the rows (sort_rows).  A FilterT's host bits are made on the calling
+  // `sets`, -1: none, EVERY_POINT: rows that only exclude points) in the order the legs run the rows (sort_rows,
+  // prepare_batch), also for an unrestricted graph batch with excluded points.  A FilterT's host bits are made on the calling
   // thread once per partition (a replica shares the handle's internal ids, and so its bits) into `bits`; a resident
   // filter is its copy on each leg's device; a label set needs the label array on the leg's device.  `exact`: each
   // run's slices (a filter's id list on the leg's device; a label set's scan_slices).  Nonzero when a leg could not have
@@ -459,6 +479,11 @@ class Index {
   // j (-1: none).
   int sort_rows(const Restriction& rs, size_t nq, std::vector<size_t>& perm, std::vector<int64_t>& sorted,
                 LabelSets& sets);
+  // the excluded points of rows [0, nq) as t.xrows / t.xids: each row's ranks checked below nb_point, then sorted and
+  // de-duplicated.  A decreasing offset refuses its row; the first rank out of range refuses its row and position.
+  int exclusion_lists(const Exclusions& x, size_t nq, Ticket& t);
+  // the key sort_rows' keys leave free, which resolve makes a run over every point (LegPlan::Run::every)
+  static constexpr int64_t EVERY_POINT = -2;
 
   // ---- point labels and attributes (labels.cu): a u32 label per point, LABEL_NONE = none, and an int64 attribute per
   // point, stored as attr_bias(value), 0 = none (ATTR_NONE)
@@ -557,7 +582,8 @@ class Index {
     PinnedBuffer h_pin, h_res;   // pinned, mapped: query staging / answers
     bool busy = false;
     // The per-row device arrays of a launch: queries (by stored point q_ids, stored rows), the id each row leaves out
-    // (skip: the launch searches k + 1), a radius launch's radii and totals, and k answer slots and a count per row
+    // (skip: the launch searches k + 1), a radius launch's radii and totals, k answer slots and a count per row, and each
+    // row's excluded points (into excluded_ids, which does not move with the rows)
     struct Rows {
       const void* d_queries = nullptr;
       const uint64_t* q_ids = nullptr;
@@ -566,10 +592,12 @@ class Index {
       uint32_t* totals = nullptr;
       NeighbourOut* out = nullptr;
       int32_t* counts = nullptr;
+      const ExcludedRow* excluded = nullptr;
+      const uint32_t* excluded_ids = nullptr;
       Rows from(size_t j, size_t q_bytes, size_t k) const {  // the same rows from row j on: only present arrays move
         return {d_queries ? (const char*)d_queries + j * q_bytes : nullptr, q_ids ? q_ids + j : nullptr, skip ? skip + j : nullptr,
                 radius ? radius + j : nullptr, totals ? totals + j : nullptr, out ? out + j * k : nullptr,
-                counts ? counts + j : nullptr};
+                counts ? counts + j : nullptr, excluded ? excluded + j : nullptr, excluded_ids};
       }
     };
     // The launches of one leg on the context (run_plan): its rows, and the device view of the leg's plan (stage_plan).

@@ -46,7 +46,10 @@ struct NeighbourOut {
 //     row admits (set == nullptr), or the label array and the row's set, set[0, nset) ascending (set is not nullptr,
 //     also when the set is empty, and label is then any value but LABEL_NONE);
 //   * none (attr == nullptr), or the attribute array (attr_bias values) and the range lo <= attr[p] <= hi, biased
-//     bounds with lo >= 1, so that a point without an attribute (0) is never in it.
+//     bounds with lo >= 1, so that a point without an attribute (0) is never in it;
+// and the row's own excluded points, excl[0, nexcl) ascending and distinct, which it never admits (nexcl == 0: none),
+// with xep the search's entry point when it is one of them (else INVALID_ID).  Those three are filled per row by the
+// filtered kernel (excl / nexcl from SearchParams::excluded) and are never part of a run's entry.
 struct RowFilter {
   const uint32_t* ptr;
   const uint32_t* set;
@@ -54,6 +57,15 @@ struct RowFilter {
   uint32_t nset;
   const uint64_t* attr;
   uint64_t lo, hi;
+  const uint32_t* excl;
+  uint32_t nexcl;
+  uint32_t xep;
+};
+
+// One row's excluded points (hnsw_b200_search_*_excluding): ids[off, off + n) of its launch's concatenated id list,
+// internal ids of the searched Index, ascending and distinct
+struct ExcludedRow {
+  uint32_t off, n;
 };
 
 struct SearchParams {
@@ -85,6 +97,9 @@ struct SearchParams {
   const uint64_t* q_ids;
   // nullptr, or per row the id the row leaves out (~0: none): k is knbn + 1 and each row knbn wide (write_row)
   const uint64_t* skip_ids;
+  // filtered search: nullptr, or per row its excluded points in excluded_ids (RowFilter::excl)
+  const ExcludedRow* excluded;
+  const uint32_t* excluded_ids;
 };
 
 // the label of a point that has none (hnsw_b200_set_labels): no label admits it

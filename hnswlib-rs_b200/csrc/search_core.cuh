@@ -171,6 +171,21 @@ __device__ __forceinline__ const char* query_row(const GraphView& g, const uint6
   return reinterpret_cast<const char*>(queries) + (size_t)qi * stride;
 }
 
+// x is one of the sorted values v[0, n): a binary search in global memory
+__device__ __forceinline__ bool in_sorted(const uint32_t* v, uint32_t n, uint32_t x) {
+  while (n) {
+    const uint32_t h = n >> 1, m = __ldg(v + h);
+    if (m == x) return true;
+    if (m < x) {
+      v += h + 1;
+      n -= h + 1;
+    } else {
+      n = h;
+    }
+  }
+  return false;
+}
+
 // Row qi of a launch's answers from its keys key_at(0 .. count - 1), ascending: those keep(id) admits, as (origin,
 // distance, internal id), then (~0, +inf, INVALID_ID) to the row's width, and their count.  Without skip ids a row is k
 // wide.  With them (a search by stored point that leaves the point out) the launch searched k = knbn + 1 and a row is

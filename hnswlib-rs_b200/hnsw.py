@@ -120,6 +120,8 @@ def load_library():
     L.hnsw_b200_search_device_by_id.argtypes = [vp, i32, i64, vp, u64, u64, u64, i32, vp, vp, i32, vp]
     L.hnsw_b200_search_exact_radius.argtypes = [vp, i64, vp, vp, vp, vp, u64, u64, vp, u64, vp, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_exact_radius_by_id.argtypes = [vp, vp, u64, vp, u64, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_flat_excluding.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_exact_excluding.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_get_stats.argtypes = [vp, vp, i32]
     L.hnsw_b200_set_stream.argtypes = [vp, vp]
     L.hnsw_b200_join.argtypes = [vp]
@@ -290,6 +292,29 @@ def _label_sets(sets, nq):
         vals = np.concatenate(parts) if parts else np.zeros(0, np.int64)
     vals = _labels(vals, vals.size, "sets")
     return off, vals if vals.size else np.zeros(1, np.uint32)   # never a NULL pointer
+
+
+def _excluded(excluded, nq):
+    """the excluded argument of the excluding searches, as (offsets u64[nq + 1], ranks u64[>= 1]): a sequence of nq
+    iterables of insertion ranks, or a tuple (offsets, ranks) as the C calls take it (query i: ranks[offsets[i]:
+    offsets[i + 1]])"""
+    if isinstance(excluded, tuple):
+        off, ids = excluded
+        off, ids = np.asarray(off).reshape(-1), np.asarray(ids).reshape(-1)
+        if off.shape != (nq + 1,):
+            raise ValueError(f"excluded: {off.size} offsets for {nq} queries, expected {nq + 1}")
+    else:
+        if len(excluded) != nq:
+            raise ValueError(f"excluded has {len(excluded)} entries for {nq} queries")
+        parts = [np.asarray(x if isinstance(x, np.ndarray) else list(x), np.int64).reshape(-1) for x in excluded]
+        off = np.zeros(nq + 1, np.uint64)
+        off[1:] = np.cumsum([x.size for x in parts])
+        ids = np.concatenate(parts) if parts else np.zeros(0, np.int64)
+    for what, a in (("offsets", off), ("ranks", ids)):
+        if a.size and (a.dtype.kind not in "iu" or a.min() < 0):
+            raise ValueError(f"excluded: {what} must be non-negative integers")
+    ids = np.ascontiguousarray(ids, np.uint64)
+    return np.ascontiguousarray(off, np.uint64), ids if ids.size else np.zeros(1, np.uint64)   # never a NULL pointer
 
 
 ATTR_NONE = -(1 << 63)   # hnsw_b200.h HNSW_B200_ATTR_NONE: the attribute of a point that has none
@@ -622,6 +647,33 @@ class Hnsw:
         admits for it, in one batch.  Returns search_exact's tuple."""
         return self._ranged(self._L.hnsw_b200_search_exact_ranges, queries, knbn, (), ranges, sets, with_internal,
                             with_pid)
+
+    # ---- excluded points per query (include/hnsw_b200.h "Excluded points per query")
+    def _excluding(self, fn, queries, knbn, mid, excluded, filter, sets, ranges, with_internal, with_pid):
+        q = np.ascontiguousarray(queries, self.dtype)
+        nq = q.shape[0]
+        off, ids = _excluded(excluded, nq)
+        rg = None if ranges is None else _ranges(ranges, nq)
+        sets_off, vals = (None, None) if sets is None else _label_sets(sets, nq)
+        return self._host_search(fn, (_p(off), _p(ids), _filter_id(filter), _p(rg), _p(sets_off), _p(vals)), q, knbn, mid,
+                                 with_internal, with_pid)
+
+    def search_flat_excluding(self, queries, knbn, ef, excluded, filter=None, sets=None, ranges=None, with_internal=True,
+                              with_pid=True):
+        """hnsw_b200_search_flat_excluding: query i without the points excluded[i] (insertion ranks, any order,
+        repeats allowed; a partitioned handle: global ranks), under the restriction search_by_id takes (filter: a
+        ResidentFilter; sets; ranges, optionally with sets).  excluded is a sequence of nq iterables of ranks, or a
+        tuple (offsets, ranks).  Row i equals search_flat with a resident filter admitting exactly the points its
+        restriction admits minus excluded[i].  Returns search_flat's (origin, dist, internal | None, pid | None,
+        counts)."""
+        return self._excluding(self._L.hnsw_b200_search_flat_excluding, queries, knbn, (int(ef),), excluded, filter, sets,
+                               ranges, with_internal, with_pid)
+
+    def search_exact_excluding(self, queries, knbn, excluded, filter=None, sets=None, ranges=None, with_internal=True,
+                               with_pid=True):
+        """hnsw_b200_search_exact_excluding: search_flat_excluding with the exact search in place of the graph one"""
+        return self._excluding(self._L.hnsw_b200_search_exact_excluding, queries, knbn, (), excluded, filter, sets, ranges,
+                               with_internal, with_pid)
 
     # ---- search by stored point (include/hnsw_b200.h "Search by stored point")
     def get_vectors(self, ranks):

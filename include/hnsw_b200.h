@@ -538,6 +538,42 @@ int hnsw_b200_search_device_by_id(const void* h, int exact, int64_t filter, cons
                                   uint64_t knbn, uint64_t ef_search, int exclude_self, void* d_out, int32_t* d_counts,
                                   int sync, float* kernel_ms);
 
+/* ---- Excluded points per query: each query names its own points to leave out of its answers ("not these points":
+ * items a user has already seen, the ids an earlier page returned, a query's known copies, the rest of a basket).  The
+ * lists cost nothing per stored point, cross the bus with the batch, and never go stale.
+ *   Lists: query i's list E_i is the distinct values of qx[qx_off[i], qx_off[i + 1]), in any order and with repeats.
+ *     They are insertion ranks, the ids set_labels, set_attributes, the _by_id calls and out_internal use: on a
+ *     partitioned handle global ranks (a list is split by placement, g to partition g % P as local id g / P), on a
+ *     partition view its local ids.  A caller who keys points by origin id maps them to ranks: with ids == NULL at
+ *     insert the two are equal, and hnsw_b200_export_points gives the origin id of every rank.
+ *   Restriction: as hnsw_b200_search_exact_by_id reads it: none (filter = -1, qrange, qset_off and qset NULL), one
+ *     resident filter, label sets, or ranges with optional sets.  Call row i's admitted points A_i.
+ *   Answers: row i is, bit for bit, what search_flat_filtered / search_exact return for query i with a resident filter
+ *     that admits exactly A_i \ E_i (ids, distance bits, internal ids, PointIds, count and, with statistics on, the
+ *     traversal counters).  A row with an empty E_i is the row of the call for its restriction alone (search_flat /
+ *     _filtered / _label_sets / _ranges, or the exact twins), so an unrestricted row with an empty list follows the tie
+ *     mode; a row with a non-empty list ignores it, as every filtered row does.  An E_i that covers A_i gives count 0.
+ *   Checks, before anything runs: a NULL handle is refused; nq == 0 returns 0; qx_off or qx NULL is refused (a batch
+ *     without lists passes nq + 1 zero offsets and any non-NULL qx); a decreasing qx_off refuses the first such row,
+ *     named; the first rank >= nb_point refuses the call, naming the row, the position in qx and the value; filter !=
+ *     -1 together with qrange, qset_off or qset is refused.  Otherwise the checks of the call the row is defined by
+ *     apply, with their wording (stale, foreign or unknown filters, bad set offsets).  A refused call leaves the
+ *     outputs untouched.
+ *   Handles: a partitioned handle merges each row over the partitions by the partitioned rule (distance, then
+ *     partition, then position) and reports global ranks; a replicated handle shards the batch like search_flat; a
+ *     partition view uses its local ids.  The handle is taken shared, and hnsw_b200_filter_free waits for the call.
+ *   Not offered: by-stored-point (_by_id) variants, radius search, submit / wait and device-resident variants.
+ * Every other argument and output is that of hnsw_b200_search_flat_ranges / hnsw_b200_search_exact_ranges. */
+int hnsw_b200_search_flat_excluding(const void* h, const uint64_t* qx_off, const uint64_t* qx, int64_t filter,
+                                    const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                                    const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
+                                    uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
+                                    int32_t* out_counts);
+int hnsw_b200_search_exact_excluding(const void* h, const uint64_t* qx_off, const uint64_t* qx, int64_t filter,
+                                     const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                                     const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids,
+                                     float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
+
 /* Run this handle's kernels and copies on a caller-owned CUDA stream (cudaStream_t passed as void*; NULL
  * restores the handle's own stream), e.g. so that torch.cuda.Event on torch's current stream brackets them. */
 int hnsw_b200_join(void* h);
