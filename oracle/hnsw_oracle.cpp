@@ -903,6 +903,11 @@ float oracle_dist(int dtype, int metric, int order, const void* a, const void* b
   return NAN;
 }
 
+// ---- the natural logarithm each order uses: device_logf in ORDER_GPU, the C library's in ORDER_REF
+void oracle_logf(int order, const float* x, float* out, uint64_t n) {
+  for (uint64_t i = 0; i < n; ++i) out[i] = order == ORDER_GPU ? device_logf(x[i]) : std::log(x[i]);
+}
+
 // ---- exact brute force (ground truth for recall): ascending (dist, id), nthreads workers
 void oracle_bruteforce(int dtype, int metric, int order, const void* base, uint64_t n, const void* qs, uint64_t nq,
                        uint64_t d, uint64_t k, int nthreads, uint32_t* out_ids, float* out_dist) {

@@ -62,6 +62,7 @@ def lib():
         L.oracle_import_layer.argtypes = [vp, i32, vp, vp, vp, u64]
         L.oracle_dist.restype = C.c_float
         L.oracle_dist.argtypes = [i32, i32, i32, vp, vp, u64]
+        L.oracle_logf.argtypes = [i32, vp, vp, u64]
         L.oracle_bruteforce.argtypes = [i32, i32, i32, vp, u64, vp, u64, u64, u64, i32, vp, vp]
         L.oracle_numa_interleave.restype = i32
         L.oracle_numa_interleave.argtypes = [i32]
@@ -84,6 +85,15 @@ def dist(a, b, metric, order=ORDER_REF):
     a = np.ascontiguousarray(a)
     b = np.ascontiguousarray(b, dtype=a.dtype)
     return float(lib().oracle_dist(DTYPES[a.dtype], METRICS[metric], order, _p(a), _p(b), a.size))
+
+
+def logf(x, order=ORDER_REF):
+    """float32 natural logarithm of every element of x as `order` computes it: the device's logf (ORDER_GPU) or the C
+    library's (ORDER_REF)"""
+    x = np.ascontiguousarray(x, np.float32)
+    out = np.empty_like(x)
+    lib().oracle_logf(int(order), _p(x), _p(out), x.size)
+    return out
 
 
 def bruteforce(base, queries, k, metric, order=ORDER_REF, nthreads=None):

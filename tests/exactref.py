@@ -17,6 +17,7 @@ EXACT_CASES = ([(np.float32, m, d, False) for m in ("DistL1", "DistL2", "DistDot
                + [(np.uint8, m, 100, False) for m in ("DistL1", "DistL2", "DistHamming", "DistJaccard")]
                + [(np.uint16, m, 200, False) for m in ("DistL1", "DistL2", "DistHamming", "DistJaccard")]
                + [(np.uint32, "DistJaccard", 24, False), (np.int32, "DistL2", 24, False)]
+               + [(np.float32, m, 32, False) for m in ("DistHellinger", "DistJeffreys", "DistJensenShannon")]
                + [(np.float32, "DistL2", 24, True), (np.float32, "DistCosine", 100, True)])
 
 
@@ -132,6 +133,8 @@ SHAPE_CASES = [
     (np.float32, "DistL2", 11000, 3000, 2, 10),      # (1, 2, 1, 2)
     (np.float32, "DistL2", 12000, 3000, 3, 10),      # (1, 1, 1, 2)
     (np.float32, "DistCosine", 3000, 3000, 33, 100),  # generic row loop (CH = 0), f64 accumulation
+    (np.float32, "DistJeffreys", 3000, 3000, 33, 100),     # (1, 8, 4, 2): logarithms, zeros at Jeffreys' clamp
+    (np.float32, "DistJensenShannon", 24, 3000, 200, 10),  # (0, 32, 32, 3): zero terms
     (np.uint8, "DistHamming", 16384, 3000, 33, 10),   # (1, 8, 2, 2), integer ops on 16 KB rows
     (np.uint8, "DistJaccard", 16384, 3000, 33, 10),
     (np.uint16, "DistL2", 8192, 3000, 33, 10),
@@ -164,7 +167,8 @@ U = distref.U
 
 
 class F64:
-    """float64 distances of stored points to a query, with tests/distref.py's formulas and bounds (L2 squared)"""
+    """float64 distances of stored points to a query, with tests/distref.py's formulas and bounds; the metrics distref
+    compares squared (L2, Hellinger, Jensen-Shannon) give their squares"""
 
     def __init__(self, X, metric):
         self.X, self.metric, self.d = X, metric, X.shape[1]
@@ -194,6 +198,25 @@ class F64:
             mx = np.maximum(self.X[ids], q).sum(1, dtype=np.int64)
             v = (1.0 - mn / np.maximum(mx, 1)).astype(np.float32).astype(np.float64)
             return np.where(mx == 0, 0.0, v), np.zeros(len(ids))
+        g = (d + 4) * U
+        if self.metric == "DistHellinger":
+            t = self._rows(ids, lambda x: np.sqrt(x * q64).sum(1))
+            return np.maximum(0.0, 1.0 - t), (g + 3 * U) * (t + 1.0)
+        if self.metric == "DistJeffreys":
+            def f(x):
+                lr = np.log(np.maximum(x, distref.EPS_CLAMP) / np.maximum(q64, distref.EPS_CLAMP))
+                return np.stack([((x - q64) * lr).sum(1), (np.abs(x - q64) * (1.0 + np.abs(lr))).sum(1)], 1)
+            v = self._rows(ids, f)
+            return v[:, 0], g * v[:, 1]
+        if self.metric == "DistJensenShannon":
+            def f(x):
+                m = 0.5 * (x + q64)
+                with np.errstate(divide="ignore", invalid="ignore"):
+                    la = np.where(x > 0, np.log(np.where(x > 0, x, 1.0) / np.where(m > 0, m, 1.0)), 0.0)
+                    lb = np.where(q64 > 0, np.log(np.where(q64 > 0, q64, 1.0) / np.where(m > 0, m, 1.0)), 0.0)
+                return np.stack([(x * la + q64 * lb).sum(1), ((x + q64) * (1.0 + np.abs(la) + np.abs(lb))).sum(1)], 1)
+            v = self._rows(ids, f)
+            return np.maximum(0.0, 0.5 * v[:, 0]), (g + 3 * U) * v[:, 1]
         raise ValueError(self.metric)
 
     def kth(self, adm, q, c):
@@ -225,7 +248,7 @@ def check_f64(F, Q, got, k, adms, what):
         assert np.isclose(rv * rv if sq else rv, v[0], rtol=1e-9, atol=1e-12) and np.isclose(rb, b[0], rtol=1e-9, atol=1e-12), \
             f"{what}, row {i}: the block formula gives {v[0]!r} +- {b[0]!r}, distref.reference {rv!r} +- {rb!r} (squared: {sq})"
         g = dist[i, :c].astype(np.float64)
-        if F.metric == "DistL2":
+        if sq:
             g = g * g
         bad = np.flatnonzero(np.abs(g - v) > b)
         assert not len(bad), f"{what}, row {i}, slot {bad[0]}: got {g[bad[0]]!r}, float64 {v[bad[0]]!r} +- {b[bad[0]]:.3g}"

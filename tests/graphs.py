@@ -19,16 +19,19 @@ NTH = os.cpu_count() or 8   # oracle threads of insert_both
 # ---------------------------------------------------------------- the instantiation matrix's cases
 F32_OPS = ["DistL1", "DistL2", "DistDot", "DistCosine"]
 F32_DIMS = [24, 48, 100, 150]          # rows of 128 / 256 / 512 / 640 bytes: CH = 1, 2, 4, generic
+PROB_OPS = ["DistHellinger", "DistJeffreys", "DistJensenShannon"]   # generic row loop only, at every dimension
+PROB_DIMS = [24, 100, 150]             # one 128-byte chunk column, four, and five with a partial last one
 U8_DIMS = [100, 200, 400, 600]
 U16_DIMS = [50, 100, 200, 300]
 CASES = ([(np.float32, m, d, False) for m in F32_OPS for d in F32_DIMS]
-         + [(np.float32, "DistL2", 24, True), (np.float32, "DistCosine", 100, True)]
+         + [(np.float32, m, d, False) for m in PROB_OPS for d in PROB_DIMS]
+         + [(np.float32, "DistL2", 24, True), (np.float32, "DistCosine", 100, True), (np.float32, "DistJeffreys", 24, True)]
          + [(np.uint8, m, d, False) for m in distref.INT_METRICS for d in U8_DIMS]
          + [(np.uint16, m, d, False) for m in distref.INT_METRICS for d in U16_DIMS]
          + [(np.uint32, m, 24, False) for m in distref.INT_METRICS]
          + [(np.int32, m, 24, False) for m in ("DistL1", "DistL2", "DistHamming")])
-INSERT_CASES = [(m, d, efc) for m in F32_OPS for d in F32_DIMS for efc in (48, 300)]
-LOG_METRICS = ("DistJeffreys", "DistJensenShannon")   # device logf against the oracle's std::log: not bit-exact
+INSERT_CASES = ([(m, d, efc) for m in F32_OPS for d in F32_DIMS for efc in (48, 300)]
+                + [(m, 100, efc) for m in PROB_OPS for efc in (48, 300)])
 
 
 def case_id(c):
@@ -38,6 +41,8 @@ def case_id(c):
 def data(dtype, metric, n, d, seed, ties=False):
     rng = np.random.default_rng(seed)
     dt = np.dtype(dtype)
+    if dt == np.float32 and metric in PROB_OPS:
+        return probabilities(n, d, seed, ties)
     if dt == np.float32:
         kind = "unit" if metric == "DistDot" else "uniform"
         dg = importlib.import_module("hnswlib-rs_b200").datagen
@@ -50,6 +55,19 @@ def data(dtype, metric, n, d, seed, ties=False):
         hi = {np.dtype(np.uint8): 256, np.dtype(np.uint16): 5000, np.dtype(np.uint32): 100000}.get(dt, 2000)
     lo = -hi if dt == np.int32 and metric != "DistHamming" else 0
     return rng.integers(lo, hi, (n, d)).astype(dt)
+
+
+def probabilities(n, d, seed, ties=False):
+    """n probability rows normalised in f32; every other row has about a third of its entries exactly 0, which Jeffreys'
+    1e-30 clamp and Jensen-Shannon's zero terms meet.  With ties, every row is stored 4 times."""
+    rng = np.random.default_rng(seed)
+    m = (n + 3) // 4 if ties else n
+    X = rng.random((m, d), dtype=np.float32)
+    odd = X[1::2]
+    odd[rng.random(odd.shape) < 1 / 3] = 0
+    X[X.sum(1) == 0, 0] = 1
+    X /= X.sum(1, keepdims=True)
+    return np.repeat(X, 4, axis=0)[:n].copy() if ties else X
 
 
 def cuobjdump():

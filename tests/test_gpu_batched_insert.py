@@ -27,8 +27,8 @@ import pytest
 
 from answers import same
 from batched import engine_batches, promoting_levels
-from graphs import (CASES, INSERT_CASES, LOG_METRICS, NTH, State, assert_same_graph, case_id, cuobjdump, data,
-                    insert_both, make_engine, make_oracle)
+from graphs import (CASES, INSERT_CASES, NTH, State, assert_same_graph, case_id, cuobjdump, data, insert_both,
+                    make_engine, make_oracle)
 from util import oracle_layers
 
 pytestmark = pytest.mark.gpu
@@ -53,17 +53,12 @@ def same_with_counters(h, o, Q, k, ef, what):
         assert cg[key] == co[key], (what, key, cg, co)
 
 
-def prob_data(n, d, seed):
-    X = np.random.default_rng(seed).random((n, d), dtype=np.float32) + np.float32(1e-3)
-    return X / X.sum(1, keepdims=True)
-
-
 def build_and_search(pkg, po, dtype, metric, d, efc, X, levels, sched=None, n=N):
     o = make_oracle(po, dtype, metric, d, M, efc, n)
     h = make_engine(pkg, dtype, metric, M, efc, n, sched)
     insert_both(pkg, h, o, X, levels, State(), sched, ledger=LEDGER)
     assert_same_graph(h, o, n)
-    Q = X[::10][:100].copy() if metric == "DistHellinger" else data(dtype, metric, 100, d, d + 100)
+    Q = data(dtype, metric, 100, d, d + 100)
     Q[:10] = X[:10]
     same_with_counters(h, o, Q, 10, 64, "lean")
     same_with_counters(h, o, Q, 10, 129, "generic")
@@ -72,8 +67,7 @@ def build_and_search(pkg, po, dtype, metric, d, efc, X, levels, sched=None, n=N)
 
 # ---------------------------------------------------------------- the insert instantiation matrix, batched
 MATRIX = ([(c[0], c[1], c[2], c[3], 200 if np.dtype(c[0]) == np.float32 else 48) for c in CASES]
-          + [(np.float32, m, d, False, efc) for m, d, efc in INSERT_CASES]
-          + [(np.float32, "DistHellinger", 24, False, 200)])
+          + [(np.float32, m, d, False, efc) for m, d, efc in INSERT_CASES])
 
 
 def matrix_id(c):
@@ -82,7 +76,7 @@ def matrix_id(c):
 
 @pytest.mark.parametrize("dtype,metric,d,ties,efc", MATRIX, ids=[matrix_id(c) for c in MATRIX])
 def test_batched_matrix(pkg, po, dtype, metric, d, ties, efc):
-    X = prob_data(N, d, d) if metric == "DistHellinger" else data(dtype, metric, N, d, d + 7, ties)
+    X = data(dtype, metric, N, d, d + 7, ties)
     build_and_search(pkg, po, dtype, metric, d, efc, X, promoting_levels(po, N, d))
     DONE.append(matrix_id((dtype, metric, d, ties, efc)))
 
@@ -293,26 +287,18 @@ def test_c2_full_size_equals_batched_oracle(pkg, po):
 
 
 # ---------------------------------------------------------------- the mini-ledger
-# instantiations exempt from bit equality in test_gpu_matrix (device logf against std::log), by their op's mangled name
-EXEMPT = {"10OpJeffreysE": "DistJeffreys", "4OpJSE": "DistJensenShannon"}
-
-
 def test_zz_every_insert_kernel_ran_batched(pkg):
     expected = len(MATRIX) + len(STALE_CASES) + 4 + 2 + 2 + 1 + 1 + 1 + 1 + 2 + 1 + 1
     if len(DONE) != expected:
         pytest.fail(f"the ledger needs every case of this module to pass: {len(DONE)} of {expected} did")
-    assert set(EXEMPT.values()) == set(LOG_METRICS)
     exe = cuobjdump()
     if exe is None:
         pytest.fail("cuobjdump (CUDA toolkit) not found: the compiled kernel list cannot be read")
     out = subprocess.run([exe, "-symbols", pkg.lib_path()], capture_output=True, text=True, check=True).stdout
     compiled = {s for s in re.findall(r"STO_ENTRY\s+(\S+)", out) if "insert_search_kernel" in s}
-    exempt = {s for s in compiled if any(k in s for k in EXEMPT)}
-    assert len(exempt) == len(EXEMPT), sorted(exempt)
     ran = {s for s in LEDGER if "insert_search_kernel" in s}
     assert ran <= compiled, sorted(ran - compiled)
-    missed = sorted(compiled - ran - exempt)
+    missed = sorted(compiled - ran)
     print(f"\ninsert ledger: {len(ran)} of {len(compiled)} insert_search_kernel entry points ran batched and bit-exact; "
-          f"exempt ({', '.join(sorted(EXEMPT.values()))}, not bit-exact in test_gpu_matrix): {len(exempt)}; "
           f"module wall time {time.time() - T0:.0f} s")
     assert not missed, f"{len(missed)} insert kernels never ran batched:\n" + "\n".join(missed)

@@ -141,32 +141,6 @@ def test_radius_equals_oracle(pkg, po, dtype, metric, d, ties):
             assert np.all(z[4] == 0) and np.array_equal(z[5], got[5]), f"{name}: knbn = 0 (binding)"
 
 
-# ---------------------------------------------------------------- 2. probability metrics
-@pytest.mark.parametrize("metric", ["DistHellinger", "DistJeffreys", "DistJensenShannon"])
-def test_probability_metrics(pkg, po, metric):
-    """test_gpu_exact's tolerance: 1e-5 relative on distances, >= 99 % identical ids; a total may differ only by
-    oracle distances within that tolerance of r"""
-    rng = np.random.default_rng(5)
-    X = rng.random((N, 32), dtype=np.float32) + np.float32(1e-3)
-    X /= X.sum(1, keepdims=True)
-    Q = rng.random((NQ, 32), dtype=np.float32) + np.float32(1e-3)
-    Q /= Q.sum(1, keepdims=True)
-    h = handle(pkg, X, metric)
-    D = all_dists(po, X, Q, metric, np.arange(N))
-    r = D[:, 49].copy()
-    got = h.search_exact_radius(Q, r, 64)
-    want = cut(expected(po, h, X, Q, 64, metric, np.arange(N)), r)
-    n = np.minimum(got[4], want[4])
-    ok = np.concatenate([got[2][i, :n[i]] == want[2][i, :n[i]] for i in range(NQ)])
-    assert ok.mean() >= 0.99
-    for i in range(NQ):
-        assert np.allclose(got[1][i, :n[i]], want[1][i, :n[i]], rtol=1e-5, atol=1e-7)
-        assert np.all(got[1][i, :got[4][i]] <= r[i])
-        lo = (D[i] <= r[i] * (1 - 1e-5) - 1e-7).sum()
-        hi = (D[i] <= r[i] * (1 + 1e-5) + 1e-7).sum()
-        assert lo <= got[5][i] <= hi, (i, got[5][i], lo, hi)
-
-
 # ---------------------------------------------------------------- 3. split launches
 def test_split_launches(pkg, po):
     """4 queries over 60 000 points split the scan over many CTAs, whose counts add up in `totals`; the same 4 queries
