@@ -95,6 +95,9 @@ struct ExactParams {
   // enter the queue
   const ExcludedRow* excluded;
   const uint32_t* excluded_ids;
+  // nullptr, or the Index's deleted points, one bit per internal id: tested, as the excluded list is, only for keys that
+  // would enter the queue, and so also kept out of the radius totals
+  const uint32_t* deleted;
 };
 
 // keys[0, c) (~0 = none) into the warp's sorted queue Q, 32 at a time: those Q accepts, inserted in lane order.  The keys
@@ -216,7 +219,8 @@ __global__ void __launch_bounds__(256, 2) exact_knn_kernel(ExactParams p) {
       const float dist = reduce8<Op>(a, p.g.dim);
       if (g == 0 && row_ok && q < nqt) {
         const uint64_t key = make_key(Op::post(dist), id);
-        if (key < thr[q] && !(p.excluded && in_excluded(p.excluded[q0 + q], p.excluded_ids, id)))
+        if (key < thr[q] && !(p.deleted && is_deleted(p.deleted, id)) &&
+            !(p.excluded && in_excluded(p.excluded[q0 + q], p.excluded_ids, id)))
           cand[q * B + atomicAdd(&ccount[q], 1)] = key;
       }
     }
@@ -307,7 +311,7 @@ static bool exact_shape(int d4, size_t k, size_t nq, ExactParams& p, size_t& sme
 }
 
 int Index::exact_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, size_t k,
-                        const std::vector<ExactGroup>& groups, bool sync, float* kernel_ms) {
+                        const std::vector<ExactGroup>& groups, const uint32_t* deleted, bool sync, float* kernel_ms) {
   cudaStream_t st = c.stream;
   // one group over every row: equal tiles over its points, taken from blockIdx (no tile table); else a tile table
   const bool tiled = !(groups.size() == 1 && groups[0].first == 0 && groups[0].count == nq);
@@ -325,6 +329,7 @@ int Index::exact_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, si
   p.totals = rows.totals;
   p.excluded = rows.excluded;
   p.excluded_ids = rows.excluded_ids;
+  p.deleted = deleted;
   p.out = rows.out;
   p.counts = rows.counts;
   k += rows.skip ? 1 : 0;  // the scan keeps k + 1 keys, each row is k wide (write_row)
@@ -443,8 +448,9 @@ int Index::bruteforce(const void* queries, size_t nq, int d, size_t k, uint32_t*
   if (nq == 0 || k == 0) return 0;
   if (d != dim) return fail("query length differs from the index dimension");
   std::vector<int32_t> counts(nq);
-  return search_batch(
-      {{queries}, nq, d, k, 0, Restriction(), true, {nullptr, nullptr, out_dist, out_ids, nullptr, counts.data()}});
+  HostBatch b{{queries}, nq, d, k, 0, Restriction(), true, {nullptr, nullptr, out_dist, out_ids, nullptr, counts.data()}};
+  b.stored = true;  // a store-level scan: deleted points are stored points
+  return search_batch(b);
 }
 
 }  // namespace hb

@@ -799,6 +799,47 @@ int hnsw_b200_get_attributes(const void* h, uint64_t first, uint64_t n, int64_t*
                        [](const Index* x, size_t p) { return hb::attr_unbias(x->attrs.host[p]); });
 }
 
+// Deleted points: the ranks split by placement, each partition's share marked on it, under the handle's locks taken
+// exclusively; every rank is checked before anything changes.  get_deleted reads as get_labels does.
+static int mark_deleted(void* h, const uint64_t* ranks, uint64_t n, bool on) {
+  Locked ix(h, EXCLUSIVE);
+  if (!ix) return -1;
+  if (n && !ranks) return set_err("ranks is NULL");
+  const uint64_t have = ix->nb_point();
+  for (uint64_t i = 0; i < n; ++i)
+    if (ranks[i] >= have)
+      return set_err("ranks[" + std::to_string(i) + "] = " + std::to_string(ranks[i]) + " is not below nb_point = " +
+                     std::to_string(have));
+  HB_NOT_VIEW(ix);
+  if (n == 0) return 0;
+  hb::DeviceRestore keep;
+  const std::vector<Index*>& hs = ix->holders();
+  const uint64_t P = hs.size();
+  std::vector<std::vector<uint64_t>> local(P);
+  for (uint64_t i = 0; i < n; ++i) {
+    const hb::Placed at = hb::place(ranks[i], P);
+    local[at.part].push_back(at.local);
+  }
+  for (uint64_t p = 0; p < P; ++p)
+    if (const int r = hs[p]->mark_deleted(local[p].data(), local[p].size(), on)) return pass(ix, ix->holder_fail((int)p, r));
+  return 0;
+}
+int hnsw_b200_delete_points(void* h, const uint64_t* ranks, uint64_t n) { return mark_deleted(h, ranks, n, true); }
+int hnsw_b200_restore_points(void* h, const uint64_t* ranks, uint64_t n) { return mark_deleted(h, ranks, n, false); }
+int hnsw_b200_get_deleted(const void* h, uint64_t first, uint64_t n, uint8_t* out) {
+  return get_per_point(h, first, n, out, "deleted points", [](const Index* x, size_t p) {
+    const std::vector<uint32_t>& w = x->deleted.host;
+    return (uint8_t)(p / 32 < w.size() ? (w[p / 32] >> (p % 32)) & 1u : 0u);
+  });
+}
+int64_t hnsw_b200_get_nb_deleted(const void* h) {
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
+  int64_t total = 0;
+  for (const Index* x : ix->holders()) total += (int64_t)x->deleted.count;
+  return total;
+}
+
 // Label sets of one label per query, for the calls that give no offsets: query i's set is {labels[i]}, or {LABEL_NONE}
 // (any label) when labels is NULL; the offsets 0, 1, ..., nq, and the nq LABEL_NONE values, are kept here
 struct OneLabelSets {

@@ -12,7 +12,9 @@
 // The FilterT predicate (filter.rs:7-24) is a device bitmap over internal ids, materialised by the host, or a point
 // label: the predicate label(p) == L, or label(p) in a set S of labels, over the label array of the graph store; and,
 // alone or with a label part, a range lo <= attr(p) <= hi over the attribute array of the graph store.  A row may also
-// name points it never admits (its excluded list, binary-searched), on top of its run's predicate or alone.
+// name points it never admits (its excluded list, binary-searched), on top of its run's predicate or alone, and no row
+// admits a deleted point (the Index's deleted-point bitmap).  Unrestricted rows of an Index with deleted points run here
+// too, as a run that admits every point and stops by the live rule (SearchParams::live_rows).
 #include "kernels.h"
 #include "search_core.cuh"
 
@@ -36,11 +38,30 @@ template <> struct SetLookupCall<OpJaccard<uint16_t>> { static constexpr bool va
 // other point of W entered it past that test, so W's later tests (keep_passing, the single-element clear, write_row's
 // post-filter) only compare the id with xep (member_pass).  A lookup inside filter_pass at those sites made the generic
 // u16 L1 and u32 Jaccard kernels spill (78 / 74 registers became 64 and 100 / 84 bytes spilled, inlined or called
-// alike).
+// alike).  A deleted point is looked up at the same two places, and its flag shares the excluded one.  With the bitmap
+// probe next to it, the generic u16 L1 kernel keeps its allocation (78 registers, no spill) only with the list lookup a
+// call (inlined: 64 registers and 100 bytes spilled).
+template <class Op> struct ExclLookupCall { static constexpr bool value = SetLookupCall<Op>::value; };
+template <> struct ExclLookupCall<OpCast<uint16_t, OpL1>> { static constexpr bool value = true; };
 template <class Op>
 __device__ __forceinline__ bool in_excluded(const RowFilter* f, uint32_t id) {
-  if constexpr (SetLookupCall<Op>::value) return in_sorted_call(f->excl, f->nexcl, id);
+  if constexpr (ExclLookupCall<Op>::value) return in_sorted_call(f->excl, f->nexcl, id);
   return in_sorted(f->excl, f->nexcl, id);
+}
+
+// A row's RowFilter in the warp's shared memory, with what the kernel adds per row: the Index's deleted points
+// (SearchParams::deleted), whether the row is in the live run (SearchParams::live_rows), and whether it removes any
+// point (excluded or deleted ones), the one word the chunk loop reads before and after the distances
+struct RowSlot : RowFilter {
+  const uint32_t* del;
+  uint32_t live;
+  uint32_t drops;
+};
+
+// the row never admits point id: it is deleted, or one of the row's excluded points
+template <class Op>
+__device__ __forceinline__ bool removed(const RowSlot* f, uint32_t id) {
+  return (f->del && is_deleted(f->del, id)) || (f->nexcl && in_excluded<Op>(f, id));
 }
 
 // the admission test of the run's predicate: the point's attribute against the query's range, then its label against
@@ -95,7 +116,7 @@ __device__ __forceinline__ int keep_passing(uint64_t* w, int n, const RowFilter*
 template <class Op, int CH, int U>
 __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const WarpSmem& s, const VisitedCfg& vc, Visited& vis,
                                                       SortedQueue& W, uint64_t* cbuf, uint32_t ccap,
-                                                      RowFilter* fslot, uint32_t ep, int ef, int layer,
+                                                      RowSlot* fslot, uint32_t ep, int ef, int layer,
                                                       Stats& st, bool& overflow) {
   const int lane = lane_id();
   const uint4* vec4 = reinterpret_cast<const uint4*>(g.vec);
@@ -110,8 +131,9 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
   }
   W.n = 1;
   uint32_t cn = 1;
-  // ep enters W before any test; if the row excludes it, every later test of W's members rejects it (member_pass)
-  if (lane == 0 && fslot->nexcl && in_excluded<Op>(fslot, ep)) fslot->xep = ep;
+  // ep enters W before any test; if the row excludes it or it is deleted, every later test of W's members rejects it
+  // (member_pass)
+  if (lane == 0 && removed<Op>(fslot, ep)) fslot->xep = ep;
   __syncwarp();
   for (;;) {
     // ---- C.pop(): nearest candidate (hnsw.rs:971)
@@ -145,12 +167,17 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
     const uint64_t fkey = W.w[W.n - 1] & ~1ull;
     // 981: the reference compares DISTANCES here (-(c.dist) > f.dist); with equal distances a larger id must not
     // trigger the retain pass (Hamming / Jaccard / integer L1 tie often)
-    if ((best >> 32) > (fkey >> 32) && W.n >= ef) W.n = keep_passing<Op>(W.w, W.n, fslot);  // 994-1000
+    const bool stop = (best >> 32) > (fkey >> 32);
+    const bool live_stop = stop && fslot->live;
+    if (stop && !live_stop && W.n >= ef) W.n = keep_passing<Op>(W.w, W.n, fslot);  // 994-1000
     const uint32_t c = key_id(best);
     int cap;
     const uint32_t* ids = list_ids(g, c, layer, cap);  // 1006
-    st.expansions += 1;
-    bool done = false;
+    // a live row returns W here, as without a filter (992-993): c is not expanded and C is emptied, so the next pop
+    // ends the search.  (An early break here cost 11 filtered kernels their register allocation; this form keeps it.)
+    if (live_stop) cn = 0;
+    st.expansions += !live_stop;
+    bool done = live_stop;
     for (int base = 0; base < cap && !done; base += 32) {
       const uint32_t nid = (base + lane < cap) ? ids[base + lane] : INVALID_ID;
       const unsigned valid = __ballot_sync(FULL, nid != INVALID_ID);
@@ -161,17 +188,18 @@ __device__ __forceinline__ void search_layer_filtered(const GraphView& g, const 
       if (cnt) {
         const int pos = __popc(m & ((1u << lane) - 1u));
         if (fresh) s.cand_id[pos] = nid;
-        // the chunk's excluded flags, in the unused upper half of the candidate-id region (nothing stays in a register
-        // across the distances)
+        // the chunk's excluded or deleted flags, in the unused upper half of the candidate-id region (nothing stays in a
+        // register across the distances)
         uint32_t* const excluded_flags = s.cand_id + 32;
-        if (fresh && fslot->nexcl) excluded_flags[pos] = in_excluded<Op>(fslot, nid);
+        if (fresh && fslot->drops) excluded_flags[pos] = removed<Op>(fslot, nid);
         __syncwarp();
         warp_dists<Op, CH, U>(vec4, g.d4, g.dim, s.q4, s.cand_id, cnt, s.cand_d);  // 1026
         __syncwarp();
         st.evals += cnt;
         const uint32_t my_id = lane < cnt ? s.cand_id[lane] : 0u;
         const uint64_t key = lane < cnt ? make_key(Op::post(s.cand_d[lane]), my_id) : ~0ull;
-        const bool my_pass = lane < cnt && !(fslot->nexcl && excluded_flags[lane]) && filter_pass<Op>(fslot, my_id);
+        const bool my_pass =
+            lane < cnt && !(fslot->drops && excluded_flags[lane]) && filter_pass<Op>(fslot, my_id);
         const unsigned passmask = __ballot_sync(FULL, my_pass);
         for (int j = 0; j < cnt; ++j) {  // strictly in list order: the accept rule sees the W of that moment
           if (W.n == 0) {                // 1019-1024
@@ -217,8 +245,8 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
                    reinterpret_cast<uint32_t*>(base + L.cand_id), reinterpret_cast<float*>(base + L.cand_d)};
   // the query's filter, read at each use so that the search loop holds no register for it: in the upper half of the
   // candidate-distance region, whose first 32 of 64 reserved entries are all this kernel scores into
-  static_assert(sizeof(RowFilter) <= 32 * 4, "a RowFilter fits the upper half of the candidate-distance region");
-  RowFilter* fslot = reinterpret_cast<RowFilter*>(base + L.cand_d + 32 * 4);
+  static_assert(sizeof(RowSlot) <= 32 * 4, "a RowSlot fits the upper half of the candidate-distance region");
+  RowSlot* fslot = reinterpret_cast<RowSlot*>(base + L.cand_d + 32 * 4);
   const uint32_t slot = blockIdx.x * (blockDim.x >> 5) + warp;  // the host launches fewer warps per CTA when shared memory is short
   Visited vis;
   vis.init(p.vis, slot);
@@ -231,13 +259,16 @@ __global__ void __launch_bounds__(SEARCH_THREADS) search_filter_kernel(SearchPar
     if (qi >= p.nq) break;
     stage_row_bytes(s.q4, query_row(g, p.q_ids, p.queries, p.q_stride_bytes, qi), p.q_bytes, g.d4 * 16);
     if (lane == 0) {
-      *fslot = p.filter_sel ? p.filter_table[p.filter_sel[qi]] : p.filter;
+      *static_cast<RowFilter*>(fslot) = p.filter_sel ? p.filter_table[p.filter_sel[qi]] : p.filter;
       fslot->xep = INVALID_ID;
+      fslot->del = p.deleted;
+      fslot->live = qi < p.live_rows;
       if (p.excluded) {  // the row's own part: its excluded points
         const ExcludedRow x = p.excluded[qi];
         fslot->excl = p.excluded_ids + x.off;
         fslot->nexcl = x.n;
       }
+      fslot->drops = fslot->nexcl || p.deleted;
     }
     __syncwarp();
     int count = 0;

@@ -190,7 +190,7 @@ int Index::plan(size_t nq, std::vector<Leg>& legs) {
 }
 
 int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>& sorted, Leg* legs, size_t n,
-                   std::vector<std::vector<uint32_t>>& bits, const LabelSets* sets) {
+                   std::vector<std::vector<uint32_t>>& bits, const LabelSets* sets, bool stored) {
   const std::vector<Index*>& hs = holders();
   const int P = (int)hs.size();
   if (rs.kind == Restriction::FILTER_T) {
@@ -229,30 +229,47 @@ int Index::resolve(const Restriction& rs, bool exact, const std::vector<int64_t>
     u.nslices = slices.size() - u.slice;
     return r;
   };
+  // a graph leg with deleted points: its unrestricted rows [0, plain) become one run over every point with the live
+  // stop rule, ahead of the leg's other runs
+  auto live_run = [](LegPlan& pl) {
+    if (pl.exact || !pl.deleted || !pl.plain) return;
+    LegPlan::Run u{0, pl.plain};
+    u.every = u.live = true;
+    pl.runs.push_back(u);
+    pl.plain = 0;
+  };
   int r = 0;
   for (Leg* l = legs; l < legs + n; ++l) {  // every leg, so that the caller reports the failure it chooses
     LegPlan& pl = l->plan;
     pl.exact = exact;
+    // labels, attributes and deleted points: the leg's own, or on a replica its copies of the handle's, made current first
+    const Index* src = parts ? l->rx : this;
+    if (!stored && l->rx->deleted_on_device(src, &pl.deleted)) {
+      r = l->rc = -1;
+      continue;
+    }
     if (!rs.per_row() && sorted.empty()) {  // every row unrestricted, or one run over every row
       LegPlan::Run u{0, l->count};
-      if (rs.kind == Restriction::NONE)
+      if (rs.kind == Restriction::NONE) {
         pl.plain = l->count;
-      else if (restrict_run(*l, rs.resident, u))
+        live_run(pl);
+      } else if (restrict_run(*l, rs.resident, u)) {
         r = l->rc = -1;
-      else
+      } else {
         pl.runs.push_back(u);
+      }
       continue;
     }
     const int64_t* key = sorted.data() + l->first;
     while (pl.plain < l->count && key[pl.plain] == -1) ++pl.plain;
-    // labels and attributes: the leg's own, or on a replica its copies of the handle's, made current first
-    const Index* src = parts ? l->rx : this;
     if (rs.kind == Restriction::ROW_LABEL_SETS && pl.plain < l->count &&
         (l->rx->on_device(&Index::labels, src, &pl.labels) || (rs.qrange && l->rx->on_device(&Index::attrs, src, &pl.attrs)))) {
       r = l->rc = -1;
       continue;
     }
-    for (size_t j = pl.plain, e; j < l->count; j = e) {  // one run per filter or label set
+    const size_t restricted = pl.plain;
+    live_run(pl);
+    for (size_t j = restricted, e; j < l->count; j = e) {  // one run per filter or label set
       for (e = j + 1; e < l->count && key[e] == key[j];) ++e;
       LegPlan::Run u{j, e - j};
       if (restrict_run(*l, key[j], u)) {
@@ -554,7 +571,7 @@ int Index::prepare_batch(const HostBatch& call, Ticket& t, bool replicas_first) 
     b.out.perm = t.perm.data();
   }
   if ((r = plan(b.nq, t.legs))) return r;
-  if (resolve(b.restriction, b.exact, sorted, t.legs.data(), t.legs.size(), t.bits, &t.sets))
+  if (resolve(b.restriction, b.exact, sorted, t.legs.data(), t.legs.size(), t.bits, &t.sets, b.stored))
     return legs_fail(t.legs.data(), t.legs.size(), replicas_first && !parts);
   return 0;
 }

@@ -168,7 +168,7 @@ int Index::ensure_points(size_t need) {
   size_t nc = std::max(need, graph_.cap * 2);
   if (graph_.cap == 0) nc = std::max(nc, std::max<size_t>(max_elements, 1024));
   int r;
-  if ((r = grow_store(false, nc, n))) return r;
+  if ((r = grow_store(false, nc, n)) || (r = grow_deleted(nc))) return r;
   graph_.cap = nc;
   return 0;
 }
@@ -706,6 +706,8 @@ int Index::search_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, s
   p.skip_ids = rows.skip;
   p.excluded = rows.excluded;
   p.excluded_ids = rows.excluded_ids;
+  p.deleted = f.deleted;
+  p.live_rows = f.live_rows;
   k += rows.skip ? 1 : 0;  // the search takes k + 1, each row is k wide (write_row)
   p.k = (int)k;
   p.ef = (int)std::max(ef_arg, k);  // hnsw.rs:1531
@@ -721,8 +723,10 @@ int Index::search_on_ctx(SearchCtx& c, const SearchCtx::Rows& rows, size_t nq, s
   p.filter = f.filter;
   p.stats = set.stats ? d_stats_.as<unsigned long long>() : nullptr;
   p.status = c.d_status.as<int>();
-  // rows with excluded points run filtered, also under a filter that admits every point (LegPlan::Run::every)
-  const bool filtered = f.sel != nullptr || f.filter.ptr != nullptr || f.filter.attr != nullptr || rows.excluded != nullptr;
+  // rows with excluded points, and every row of an Index with deleted points, run filtered, also under a filter that
+  // admits every point (LegPlan::Run::every)
+  const bool filtered = f.sel != nullptr || f.filter.ptr != nullptr || f.filter.attr != nullptr || rows.excluded != nullptr ||
+                        f.deleted != nullptr;
   QueryKernel kind = QueryKernel::Generic;
   if (filtered) kind = QueryKernel::Filtered;
   else if (set.tie_std) kind = QueryKernel::StdTie;  // unfiltered searches only
@@ -948,6 +952,7 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
   cudaStream_t st = c.stream;
   L.exact = plan.exact;
   L.plain = plan.plain;
+  L.filter.deleted = plan.deleted;
   if (plan.exact) {
     if (plan.plain) L.groups.push_back(ExactGroup{0, plan.plain, ExactScan()});
     size_t joined = 0;  // ids copied into the context
@@ -1003,6 +1008,7 @@ int Index::stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& L) {
       f.lo = u.lo;
       f.hi = u.hi;
     }
+    if (u.live) L.filter.live_rows = (uint32_t)u.count;  // the first run (resolve)
     if (several) sel.insert(sel.end(), u.count, (uint32_t)table.size());
     table.push_back(f);
   }
@@ -1028,7 +1034,7 @@ int Index::run_plan(SearchCtx& c, const SearchCtx::Launch& L, bool sync, float* 
     if (sync) HB_CUDA(cudaStreamSynchronize(st));
     return 0;
   }
-  if (L.exact) return exact_on_ctx(c, L.rows, L.nq, L.k, L.groups, sync, kernel_ms);
+  if (L.exact) return exact_on_ctx(c, L.rows, L.nq, L.k, L.groups, L.filter.deleted, sync, kernel_ms);
   int r;
   SearchCtx::Rows plain = L.rows;
   plain.excluded = nullptr;  // the unrestricted rows exclude no point (prepare_batch)

@@ -158,6 +158,16 @@ struct PointColumn {
   uint64_t version = 0;
 };
 
+// The deleted points of one Index (deleted.cu): a bit per internal id on the host and on the device, `count` bits set;
+// `version` counts the calls that changed it (a replica: the handle's version it copied).  The device bitmap covers the
+// graph store's capacity and grows with it, zero-filled (Index::ensure_points), so that a new point is live.
+struct DeletedSet {
+  std::vector<uint32_t> host{};
+  DeviceBuffer dev{};
+  size_t count = 0;
+  uint64_t version = 0;
+};
+
 struct DumpDescription {  // Description, /root/reference/src/hnswio.rs:846-870
   int format_version = 0;
   uint8_t dumpmode = 0, max_nb_connection = 0, nb_layer = 0;
@@ -187,11 +197,14 @@ struct ExactGroup {
 };
 
 // The restriction of one search launch, as SearchParams reads it: none (sel, filter.ptr and filter.attr null), `filter`
-// for every row, or row i under table[sel[i]]
+// for every row, or row i under table[sel[i]]; the Index's deleted points, which no row admits (nullptr: none); and the
+// rows [0, live_rows) of the live run (LegPlan::Run::live)
 struct LaunchFilter {
   RowFilter filter{nullptr, nullptr, LABEL_NONE, 0, nullptr, 0, 0};
   const RowFilter* table = nullptr;
   const uint32_t* sel = nullptr;
+  const uint32_t* deleted = nullptr;
+  uint32_t live_rows = 0;
 };
 
 // Resident filters (hnsw_b200_filter_new, filter_store.cu): a FilterT materialised once per handle, as one bitmap per
@@ -333,7 +346,8 @@ struct HostAnswers {
 
 // One host search batch: the rows `in`, k answers each into `out`.  `exact`: the exact scan of the points each row may
 // return (ef unused) instead of the graph search.  `excluded`: each row's points left out on top of its restriction
-// (made into in.excluded when the batch is planned).
+// (made into in.excluded when the batch is planned).  `stored`: a store-level scan (hnsw_b200_bruteforce), which returns
+// deleted points too.
 struct HostBatch {
   HostRows in;
   size_t nq = 0;
@@ -343,6 +357,7 @@ struct HostBatch {
   bool exact = false;
   AnswerArrays out;
   Exclusions excluded;
+  bool stored = false;
 };
 
 // A leg's restriction (Index::resolve): its rows [0, plain) are unrestricted, and `runs` cover the rest, each a range of
@@ -351,11 +366,14 @@ struct HostBatch {
 // latter within an attribute range on `attrs` unless its lo is 0.  In an exact batch its points are slices [slice,
 // slice + nslices): a filter's id list, or a label set's and range's slices of an exact-scan order.  A batch-wide filter
 // is a plan with no prefix and one run over every row.  Graph rows that exclude points and have no other restriction
-// are a run over every point (`every`), so that they run in the filtered kernel, which reads their lists.
+// are a run over every point (`every`), so that they run in the filtered kernel, which reads their lists.  On an Index
+// with deleted points (`deleted`, its bitmap on the leg's device) a graph leg has no unrestricted prefix: those rows are
+// a run over every point that stops by the live rule (`live`, SearchParams::live_rows).
 struct LegPlan {
   struct Run {
     size_t first, count;
     bool every = false;
+    bool live = false;
     const uint32_t* bits = nullptr;
     const uint32_t* host_bits = nullptr;
     const uint32_t* set = nullptr;  // the run's label set, nset values of a LabelSets
@@ -369,6 +387,7 @@ struct LegPlan {
   std::vector<ExactScan> slices;
   const uint32_t* labels = nullptr;
   const uint64_t* attrs = nullptr;  // the attribute array on the leg's device, when a run has a range
+  const uint32_t* deleted = nullptr;
 };
 
 // One Index's part of a batch: queries [first, first + count) searched on rx (the handle, a replica, or partition `part`)
@@ -469,9 +488,10 @@ class Index {
   // thread once per partition (a replica shares the handle's internal ids, and so its bits) into `bits`; a resident
   // filter is its copy on each leg's device; a label set needs the label array on the leg's device.  `exact`: each
   // run's slices (a filter's id list on the leg's device; a label set's scan_slices).  Nonzero when a leg could not have
-  // its plan; that leg's rc is set (legs_fail reports it).
+  // its plan; that leg's rc is set (legs_fail reports it).  Unless `stored`, a leg on an Index with deleted points
+  // carries their bitmap, and its unrestricted graph rows become a live run (LegPlan).
   int resolve(const Restriction& rs, bool exact, const std::vector<int64_t>& sorted, Leg* legs, size_t n,
-              std::vector<std::vector<uint32_t>>& bits, const LabelSets* sets = nullptr);
+              std::vector<std::vector<uint32_t>>& bits, const LabelSets* sets = nullptr, bool stored = false);
   // a per-row restriction: every filter of rs.filters[0, nq) is -1 or a live, current filter of this handle (else the
   // first bad position is refused), and `perm` orders the rows stably by filter, the unfiltered ones first; label sets,
   // each made ascending without repeats into `sets`, by set in lexicographic order, {LABEL_NONE} first (a decreasing
@@ -512,6 +532,16 @@ class Index {
   // exact-scan order (rebuilt when a column it is keyed on changed): per label of the set, its group, narrowed to the
   // range by binary search in a value-keyed order; slices that follow each other in the order are joined.
   int scan_slices(const uint32_t* set, size_t nset, uint64_t lo, uint64_t hi, std::vector<ExactScan>& slices);
+
+  // ---- deleted points (deleted.cu): points that no search returns, by internal id of this Index.  They stay in the
+  // graph and in the store, route searches and inserts, and are counted by nb_point.
+  DeletedSet deleted;
+  // the points ids[0, n) (the caller checked them below n) marked deleted (on) or live; the changed words are copied to
+  // the device and waited for, after the asynchronous device-resident launches that may read the bitmap are done
+  int mark_deleted(const uint64_t* ids, size_t count, bool on);
+  // the deleted-point bitmap on this Index's device as current as src's (src == this: its own; a replica: its copy of
+  // the handle's, refreshed when the handle's changed), or nullptr when src has no deleted point
+  int deleted_on_device(const Index* src, const uint32_t** d);
   // the batch b with device rows in and device answers out (b.in: queries, or qids and skip; b.out: nb and counts); the
   // restriction is none or a resident filter
   int search_device(const HostBatch& b, bool sync, float* kernel_ms);
@@ -601,7 +631,8 @@ class Index {
       }
     };
     // The launches of one leg on the context (run_plan): its rows, and the device view of the leg's plan (stage_plan).
-    // Graph: rows [0, plain) unrestricted, the others under `filter`.  Exact: the rows by the points they scan.
+    // Graph: rows [0, plain) unrestricted, the others under `filter`.  Exact: the rows by the points they scan, none of
+    // filter.deleted.
     struct Launch {
       Rows rows;
       size_t nq = 0, k = 0, ef = 0;
@@ -672,6 +703,7 @@ class Index {
   size_t row_size(int a) const;  // bytes of array a per point (per upper-layer list for ADJU, ADJU_D)
   int grow_store(bool per_list, size_t cap, size_t keep);
   int ensure_points(size_t need);
+  int grow_deleted(size_t cap);  // the deleted-point bitmap to `cap` points, the new bits zero (deleted.cu)
   int ensure_upper(size_t need_lists);
   // ---- point ledger: the host mirrors (h_level ... h_upoff) and the per-layer counts
   void resize_points(size_t count);
@@ -758,7 +790,7 @@ class Index {
   // the exact k nearest of rows [0, nq) of r, each group's rows among that group's points (aux.cu; the slices' scratch
   // sized before the launch); radius mode (r.radius): only those within each row's radius, their number into r.totals
   int exact_on_ctx(SearchCtx& c, const SearchCtx::Rows& r, size_t nq, size_t k, const std::vector<ExactGroup>& groups,
-                   bool sync, float* kernel_ms);
+                   const uint32_t* deleted, bool sync, float* kernel_ms);
   // the device view of a leg's plan in `run`, with what it needs uploaded into context c
   int stage_plan(SearchCtx& c, const LegPlan& plan, SearchCtx::Launch& run);
   // the launches of `run` on context c, after what they share (the checks, a radius launch's totals zeroed, an empty

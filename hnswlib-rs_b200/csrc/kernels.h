@@ -48,8 +48,8 @@ struct NeighbourOut {
 //   * none (attr == nullptr), or the attribute array (attr_bias values) and the range lo <= attr[p] <= hi, biased
 //     bounds with lo >= 1, so that a point without an attribute (0) is never in it;
 // and the row's own excluded points, excl[0, nexcl) ascending and distinct, which it never admits (nexcl == 0: none),
-// with xep the search's entry point when it is one of them (else INVALID_ID).  Those three are filled per row by the
-// filtered kernel (excl / nexcl from SearchParams::excluded) and are never part of a run's entry.
+// with xep the search's entry point when it is one of them or a deleted point (else INVALID_ID).  Those three are filled
+// per row by the filtered kernel (excl / nexcl from SearchParams::excluded) and are never part of a run's entry.
 struct RowFilter {
   const uint32_t* ptr;
   const uint32_t* set;
@@ -100,7 +100,17 @@ struct SearchParams {
   // filtered search: nullptr, or per row its excluded points in excluded_ids (RowFilter::excl)
   const ExcludedRow* excluded;
   const uint32_t* excluded_ids;
+  // filtered search: nullptr, or the searched Index's deleted points, one bit per internal id, which no row admits; and
+  // how many leading rows are the live run (LegPlan::Run::live), searched by the live stop rule: when the nearest
+  // candidate is farther than W's farthest member the search returns W, as an unfiltered search does, instead of
+  // dropping W's non-admitted members and expanding on.  (Fields after every other kernel's, and not on RowFilter, which
+  // SearchParams holds by value: the lean, std-tie and generic kernels keep their parameter offsets.)
+  const uint32_t* deleted;
+  uint32_t live_rows;
 };
+
+// whether bit `id` of the deleted-point bitmap `bits` is set
+__device__ __forceinline__ bool is_deleted(const uint32_t* bits, uint32_t id) { return (__ldg(bits + (id >> 5)) >> (id & 31)) & 1u; }
 
 // the label of a point that has none (hnsw_b200_set_labels): no label admits it
 constexpr uint32_t LABEL_NONE = 0xFFFFFFFFu;

@@ -122,6 +122,11 @@ def load_library():
     L.hnsw_b200_search_exact_radius_by_id.argtypes = [vp, vp, u64, vp, u64, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_flat_excluding.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_exact_excluding.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_delete_points.argtypes = [vp, vp, u64]
+    L.hnsw_b200_restore_points.argtypes = [vp, vp, u64]
+    L.hnsw_b200_get_deleted.argtypes = [vp, u64, u64, vp]
+    L.hnsw_b200_get_nb_deleted.restype = i64
+    L.hnsw_b200_get_nb_deleted.argtypes = [vp]
     L.hnsw_b200_get_stats.argtypes = [vp, vp, i32]
     L.hnsw_b200_set_stream.argtypes = [vp, vp]
     L.hnsw_b200_join.argtypes = [vp]
@@ -580,6 +585,34 @@ class Hnsw:
         out = np.empty(int(n), np.uint32)
         self._chk(self._L.hnsw_b200_get_labels(self._h, int(first), int(n), _p(out)))
         return out
+
+    def delete_points(self, ranks):
+        """hnsw_b200_delete_points: no search returns the points with these insertion ranks from now on (a partitioned
+        handle's global ranks).  They stay in the graph and the store; deleting a deleted point does nothing."""
+        r = np.ascontiguousarray(np.asarray(ranks, np.uint64).reshape(-1))
+        self._chk(self._L.hnsw_b200_delete_points(self._h, _p(r), r.size))
+
+    def restore_points(self, ranks):
+        """hnsw_b200_restore_points: the points with these insertion ranks are live again (restoring a live one does
+        nothing)"""
+        r = np.ascontiguousarray(np.asarray(ranks, np.uint64).reshape(-1))
+        self._chk(self._L.hnsw_b200_restore_points(self._h, _p(r), r.size))
+
+    def deleted(self, first=0, n=None):
+        """hnsw_b200_get_deleted: for the points first .. first + n - 1 (n None: to the last point), a bool array, True
+        for a deleted point"""
+        if n is None:
+            n = self.get_nb_point() - int(first)
+        out = np.empty(int(n), np.uint8)
+        self._chk(self._L.hnsw_b200_get_deleted(self._h, int(first), int(n), _p(out)))
+        return out.astype(bool)
+
+    def nb_deleted(self):
+        """hnsw_b200_get_nb_deleted: the number of deleted points"""
+        r = int(self._L.hnsw_b200_get_nb_deleted(self._h))
+        if r < 0:
+            raise HnswError(last_error())
+        return r
 
     def search_flat_labeled(self, queries, knbn, ef, labels, with_internal=True, with_pid=True):
         """hnsw_b200_search_flat_labeled: one batch, query i restricted to the points labelled labels[i] (LABEL_NONE:

@@ -264,7 +264,8 @@ int hnsw_b200_insert_flat(void* h, const void* vecs, uint64_t n, uint64_t dim, c
  *   out_internal = internal ids, out_pid = PointId (level, rank) pairs as int32[nq][knbn][2]
  * Filter (FilterT, /root/reference/src/filter.rs:7-24): filter_mode 0 none, 1 sorted origin-id
  * list (filter_ids / nfilter), 2 predicate callback evaluated ONCE per stored origin id on the
- * host and materialised to a device bitmap.  0 on success. */
+ * host and materialised to a device bitmap.  0 on success.
+ * Deleted points (hnsw_b200_delete_points) are never returned: see "Deleted points" below. */
 typedef int (*hnsw_b200_filter_fn)(uint64_t origin_id, void* ctx);
 int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
                           uint64_t ef_search, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,
@@ -315,7 +316,8 @@ int hnsw_b200_search_device(const void* h, const void* d_queries, uint64_t nq, u
  *     all); search_flat_filtered merges like an unfiltered search.  submit_filtered and search_device_filtered are
  *     refused there, as their unfiltered twins are.  filter_new on a partition view is refused.
  * Every other argument and output of the _filtered calls is that of its unfiltered twin; a submit_filtered ticket is
- * collected by hnsw_b200_search_flat_wait. */
+ * collected by hnsw_b200_search_flat_wait.
+ * Deleted points (hnsw_b200_delete_points) are never returned: see "Deleted points" below. */
 int64_t hnsw_b200_filter_new(const void* h, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,
                              hnsw_b200_filter_fn fn, void* ctx);
 int hnsw_b200_filter_free(const void* h, int64_t filter);
@@ -344,7 +346,8 @@ int hnsw_b200_search_device_filtered(const void* h, int64_t filter, const void* 
  *     then partition, then position) and reports internal ids as global insertion ranks; the device variant is refused,
  *     as search_device is.  A replicated handle shards the host variant like search_flat.  A partition view accepts -1
  *     and reports its local ids.
- *   Locks: the handle is taken shared, as for any search. */
+ *   Locks: the handle is taken shared, as for any search.
+ * Deleted points (hnsw_b200_delete_points) are never returned: see "Deleted points" below. */
 int hnsw_b200_search_exact(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
                            uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
 int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
@@ -375,7 +378,8 @@ int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_q
  *   Ignored: the tie mode and statistics, as for every exact call.  There is no device variant.
  *   Handles: a partitioned handle merges the partitions' rows by the partitioned rule (distance, then partition, then
  *     position), reports global ranks and sums the partitions' totals; a replicated handle shards the batch like
- *     search_exact; a partition view uses its local ids.  The handle is taken shared. */
+ *     search_exact; a partition view uses its local ids.  The handle is taken shared.
+ * Deleted points (hnsw_b200_delete_points) are never returned: see "Deleted points" below. */
 int hnsw_b200_search_exact_radius(const void* h, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
                                   const uint32_t* qset, const void* queries, uint64_t nq, uint64_t dim,
                                   const float* radius, uint64_t knbn, uint64_t* out_ids, float* out_dist,
@@ -402,7 +406,8 @@ int hnsw_b200_search_exact_radius_by_id(const void* h, const uint64_t* qids, uin
  *     each replica's device gets a filter's copies at their first use there.  A partition view owns no filters, so it
  *     accepts only -1 entries.
  *   Locks: the handle is taken shared; hnsw_b200_filter_free waits for the call.
- * Every other argument and output is that of hnsw_b200_search_flat_filtered / hnsw_b200_search_exact. */
+ * Every other argument and output is that of hnsw_b200_search_flat_filtered / hnsw_b200_search_exact.
+ * Deleted points (hnsw_b200_delete_points) are never returned: see "Deleted points" below. */
 int hnsw_b200_search_flat_per_query(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim,
                                     uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                     uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
@@ -432,7 +437,8 @@ int hnsw_b200_search_exact_per_query(const void* h, const int64_t* filters, cons
  *     shards the batch; each replica's device gets a copy of the labels at its first labelled search after they
  *     changed.  A partition view searches with its own partition's labels and reports local ids.  In the
  *     one-process-per-GPU mode (nccl_broadcast_index) labels are not broadcast: each rank sets its own.
- *   Filters: no label call reads or changes resident filters, and no filter call reads or changes labels. */
+ *   Filters: no label call reads or changes resident filters, and no filter call reads or changes labels.
+ * Deleted points (hnsw_b200_delete_points) are never returned: see "Deleted points" below. */
 #define HNSW_B200_LABEL_NONE 0xFFFFFFFFu
 int hnsw_b200_set_labels(void* h, uint64_t first, uint64_t n, const uint32_t* labels);
 int hnsw_b200_get_labels(const void* h, uint64_t first, uint64_t n, uint32_t* out);
@@ -455,7 +461,8 @@ int hnsw_b200_search_exact_labeled(const void* h, const uint32_t* qlabels, const
  *   Checks, before anything runs: qset_off must not decrease, and HNSW_B200_LABEL_NONE may not share a set with another
  *     label; the first bad row refuses the whole call, and the message names it.  qset_off or qset NULL with nq > 0 is
  *     refused; nq == 0 returns 0.
- *   Handles, locks and every other argument and output: as search_flat_labeled / search_exact_labeled. */
+ *   Handles, locks and every other argument and output: as search_flat_labeled / search_exact_labeled.
+ * Deleted points (hnsw_b200_delete_points) are never returned: see "Deleted points" below. */
 int hnsw_b200_search_flat_label_sets(const void* h, const uint64_t* qset_off, const uint32_t* qset, const void* queries,
                                      uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search, uint64_t* out_ids,
                                      float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
@@ -487,7 +494,8 @@ int hnsw_b200_search_exact_label_sets(const void* h, const uint64_t* qset_off, c
  *   Checks: those of search_*_label_sets, with their wording; qrange NULL with nq > 0 is refused, and so is exactly one
  *     of qset_off and qset NULL.  A NULL handle is refused and nq == 0 returns 0 before any other check.
  *   Handles: as search_*_label_sets; a replica's device gets a copy of the attributes at its first ranged search after
- *     they changed, and a partition view searches with its own partition's attributes and reports local ids. */
+ *     they changed, and a partition view searches with its own partition's attributes and reports local ids.
+ * Deleted points (hnsw_b200_delete_points) are never returned: see "Deleted points" below. */
 #define HNSW_B200_ATTR_NONE INT64_MIN /* the attribute of a point that has none */
 int hnsw_b200_set_attributes(void* h, uint64_t first, uint64_t n, const int64_t* values);
 int hnsw_b200_get_attributes(const void* h, uint64_t first, uint64_t n, int64_t* out);
@@ -524,7 +532,8 @@ int hnsw_b200_search_exact_ranges(const void* h, const int64_t* qrange, const ui
  *   search_device_by_id: d_qids on the device, answers as search_device / search_exact_device (exact != 0) leave them,
  *     no restriction or one resident filter, with their sync, join, stream_wait_last, check_status and overflow rules.
  *     To check the ids it reads them back once the work already on the handle's stream is done.  Refused on a
- *     partitioned handle. */
+ *     partitioned handle.
+ * Deleted points (hnsw_b200_delete_points) are never returned: see "Deleted points" below. */
 int hnsw_b200_get_vectors(const void* h, const uint64_t* ranks, uint64_t n, void* out /* [n][dim] elements */);
 int hnsw_b200_search_flat_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, uint64_t ef_search,
                                 int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
@@ -563,7 +572,8 @@ int hnsw_b200_search_device_by_id(const void* h, int exact, int64_t filter, cons
  *     partition, then position) and reports global ranks; a replicated handle shards the batch like search_flat; a
  *     partition view uses its local ids.  The handle is taken shared, and hnsw_b200_filter_free waits for the call.
  *   Not offered: by-stored-point (_by_id) variants, radius search, submit / wait and device-resident variants.
- * Every other argument and output is that of hnsw_b200_search_flat_ranges / hnsw_b200_search_exact_ranges. */
+ * Every other argument and output is that of hnsw_b200_search_flat_ranges / hnsw_b200_search_exact_ranges.
+ * Deleted points (hnsw_b200_delete_points) are never returned: see "Deleted points" below. */
 int hnsw_b200_search_flat_excluding(const void* h, const uint64_t* qx_off, const uint64_t* qx, int64_t filter,
                                     const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
                                     const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
@@ -573,6 +583,47 @@ int hnsw_b200_search_exact_excluding(const void* h, const uint64_t* qx_off, cons
                                      const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
                                      const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids,
                                      float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts);
+
+/* ---- Deleted points: points that no search returns (a replaced, withdrawn or expired item).  A deleted point stays in
+ * the graph and in the store: it still routes searches and inserts, later inserts may link it, and its rank, label,
+ * attribute and vector are kept, so that every rank-keyed column and resident filter stays valid.  Nothing is reclaimed.
+ *   Ranks: insertion ranks, as set_labels reads them: on a partitioned handle global ranks (g to partition g % P as
+ *     local id g / P), on a partition view its local ids.  Deleting a deleted point, or restoring a live one, does
+ *     nothing.  INTEGRATION.md shows how to map origin ids to ranks and how to replace an item.
+ *   Which points: call D the deleted points when a search's work is enqueued.
+ *   Restricted rows (a FilterT, a resident filter or a filter per query, labels, label sets or ranges, a non-empty
+ *     excluded list, also by stored point): row i is, bit for bit, the row of the same call under a resident filter
+ *     that admits exactly A_i \ D, A_i the row's admitted points (ids, distance bits, internal ids, PointIds, count
+ *     and, with statistics on, the traversal counters).
+ *   Unrestricted graph rows (search_flat, the reference entry points, submit / wait, search_device, _by_id): the
+ *     "live search" rule.  Row i is the row the filtered search returns under a filter admitting exactly the live
+ *     points, except that when the nearest candidate is farther than the farthest point held the search returns, as an
+ *     unfiltered search does, instead of dropping non-admitted points and expanding on.  A row whose entry point is
+ *     deleted may so return fewer than knbn.  A search that meets no deleted point returns the unfiltered row (tie
+ *     mode 0), except where the nearest candidate and the farthest point held are at equal distances: the unfiltered
+ *     rule stops there when the candidate's id is the larger, the live rule, which compares distances alone as the
+ *     filtered one does, expands on.  Such ties are common with Hamming, Jaccard and integer L1.  Live rows run the
+ *     filtered kernel and ignore the tie mode.
+ *   Exact and radius rows: the search_exact row under a resident filter admitting A_i \ D; radius totals do not count
+ *     deleted points.
+ *   With D empty (also after every deleted point was restored) every call runs the kernel and returns the rows it does
+ *     without deletions.  Store-level calls (bruteforce, dist_batch, export_*, flatten, flat_neighbours), get_nb_point
+ *     and file_dump still see every stored point; a reloaded dump has no deleted point (get_deleted saves the set).
+ *   Handles: a partitioned handle splits the ranks by placement; a partition view searches with its partition's set and
+ *     refuses delete and restore; a replica gets the set at its first sharded search after it changed;
+ *     hnsw_b200_nccl_broadcast_index does not send it.
+ *   Locks: delete and restore take the handle exclusively, as set_labels does, and wait for submitted tickets (collect
+ *     this thread's own first) and for asynchronous device-resident launches.  Work enqueued after the call returns sees
+ *     the new set, work enqueued before it the old one.
+ *   Checks: a NULL handle, ranks == NULL with n > 0, the first rank >= nb_point (named by position and value), and
+ *     delete or restore on a partition view are refused and change nothing; n == 0 returns 0.  get_deleted refuses a
+ *     range past nb_point or a NULL out.
+ * get_deleted writes out[i] = 1 for a deleted point first + i, else 0; get_nb_deleted returns the number of deleted
+ * points (-1 on a NULL handle). */
+int hnsw_b200_delete_points(void* h, const uint64_t* ranks, uint64_t n);
+int hnsw_b200_restore_points(void* h, const uint64_t* ranks, uint64_t n);
+int hnsw_b200_get_deleted(const void* h, uint64_t first, uint64_t n, uint8_t* out); /* 1 deleted, 0 live */
+int64_t hnsw_b200_get_nb_deleted(const void* h);
 
 /* Run this handle's kernels and copies on a caller-owned CUDA stream (cudaStream_t passed as void*; NULL
  * restores the handle's own stream), e.g. so that torch.cuda.Event on torch's current stream brackets them. */
