@@ -1020,6 +1020,54 @@ int hnsw_b200_search_exact_excluding(const void* h, const uint64_t* qx_off, cons
                         qset_off, qset);
 }
 
+// Planned search: count_admitted reads its restriction as the by-id calls do; the planned calls run each row on the graph
+// or by the exact scan per leg (Index::split_legs), under one_restriction's restriction and, with qx_off and qx, each
+// row's excluded points; out_exact (may be NULL) is written once the batch succeeded
+int hnsw_b200_count_admitted(const void* h, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                             const uint32_t* qset, uint64_t nq, uint64_t* out_count) {
+  OneLabelSets one;
+  Restriction rs;
+  if (int s = first_checks(h, "count_admitted", nq, false, nullptr, nullptr, nullptr)) return s < 0 ? -1 : 0;
+  if (one_restriction("count_admitted", nq, filter, qrange, qset_off, qset, one, rs)) return -1;
+  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset_off) return set_err("qset_off is NULL");
+  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset) return set_err("qset is NULL");
+  if (!out_count) return set_err("count_admitted: out_count is NULL");
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
+  return pass(ix, ix->count_admitted(rs, nq, out_count));
+}
+
+static int planned_call(const void* h, const char* name, bool by_id, HostBatch b, const uint64_t* qx_off, const uint64_t* qx,
+                        int64_t filter, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                        int32_t* out_exact) {
+  OneLabelSets one;
+  if (int s = first_checks(h, name, b.nq, by_id, b.in.qids, nullptr, nullptr)) return s < 0 ? -1 : 0;
+  if (qx && !qx_off) return set_err(std::string(name) + ": qx_off is NULL");
+  if (qx_off && !qx) return set_err(std::string(name) + ": qx is NULL");
+  if (one_restriction(name, b.nq, filter, qrange, qset_off, qset, one, b.restriction)) return -1;
+  b.excluded = {qx_off, qx};
+  b.planned = true;
+  b.out.exact = out_exact;
+  return (int)search_call(h, HOST, name, b, 1, nullptr);
+}
+int hnsw_b200_search_planned(const void* h, const uint64_t* qx_off, const uint64_t* qx, int64_t filter,
+                             const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset, const void* queries,
+                             uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search, uint64_t* out_ids,
+                             float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts,
+                             int32_t* out_exact) {
+  return planned_call(h, "search_planned", false, {{queries}, nq, (int)dim, knbn, ef_search, Restriction(), false,
+                      columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, qx_off, qx, filter, qrange, qset_off,
+                      qset, out_exact);
+}
+int hnsw_b200_search_planned_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, uint64_t ef_search,
+                                   int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                                   const uint32_t* qset, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                                   int32_t* out_pid, int32_t* out_counts, int32_t* out_exact) {
+  return planned_call(h, "search_planned_by_id", true, {{nullptr, nullptr, qids, exclude_self ? qids : nullptr}, nq, 0, knbn,
+                      ef_search, Restriction(), false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)},
+                      nullptr, nullptr, filter, qrange, qset_off, qset, out_exact);
+}
+
 // Radius search: the exact scan of host queries or of stored points (by_id), under one_restriction's restriction, each
 // row cut at its radius and its total of points within it into out_total (may be NULL).  knbn == 0 counts only: the
 // scan runs at k = 1 into scratch rows, the caller's row arrays may be NULL, and every count is 0.

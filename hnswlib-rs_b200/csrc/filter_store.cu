@@ -33,17 +33,33 @@ bool FilterStore::has(int64_t id) {
   return f_.count(id) != 0;
 }
 
-int FilterStore::use(int64_t id, int p, int nparts, const Index* rx, const uint32_t** d_bits, ExactScan* list) {
-  std::lock_guard<std::mutex> lk(mu_);
+FilterStore::Filter* FilterStore::current(int64_t id, int p, int nparts, const Index* rx) {
   auto it = f_.find(id);
-  if (it == f_.end()) return rx->fail(unknown_filter(id));
+  if (it == f_.end()) return rx->fail(unknown_filter(id)), nullptr;
   Filter& f = it->second;
   // the kernel reads one bit per stored point: a bitmap made over fewer points than the index now holds is refused
   if ((int)f.counts.size() != nparts)
-    return rx->fail("filter " + std::to_string(id) + " was made before the handle was partitioned: make a new filter");
+    return rx->fail("filter " + std::to_string(id) + " was made before the handle was partitioned: make a new filter"), nullptr;
   if (f.counts[p] != rx->n)
     return rx->fail("filter " + std::to_string(id) + " is stale: it covers " + std::to_string(f.counts[p]) + " points and the " +
-                    (nparts > 1 ? "partition" : "index") + " now holds " + std::to_string(rx->n) + ": make a new filter");
+                    (nparts > 1 ? "partition" : "index") + " now holds " + std::to_string(rx->n) + ": make a new filter"),
+           nullptr;
+  return &f;
+}
+
+int FilterStore::admitted(int64_t id, int p, int nparts, const Index* rx, size_t* count) {
+  std::lock_guard<std::mutex> lk(mu_);
+  const Filter* f = current(id, p, nparts, rx);
+  if (!f) return -1;
+  *count = f->admitted[p];
+  return 0;
+}
+
+int FilterStore::use(int64_t id, int p, int nparts, const Index* rx, const uint32_t** d_bits, ExactScan* list) {
+  std::lock_guard<std::mutex> lk(mu_);
+  Filter* fp = current(id, p, nparts, rx);
+  if (!fp) return -1;
+  Filter& f = *fp;
   const std::pair<int, int> key(p, rx->device);
   if (list) {
     auto l = f.ids.find(key);
@@ -85,6 +101,9 @@ int64_t Index::new_filter(int mode, const uint64_t* sorted_ids, size_t nids, int
   for (int p = 0; p < P; ++p) {  // on the calling thread: a callback runs once per stored point in all
     if (part[p]->make_filter_bits(mode, sorted_ids, nids, fn, ctx, f.bits[p])) return fail(part[p]->err());
     f.counts.push_back(part[p]->n);
+    size_t admitted = 0;
+    for (uint32_t w : f.bits[p]) admitted += __builtin_popcount(w);
+    f.admitted.push_back(admitted);
   }
   const int64_t id = filters.add(std::move(f));
   // the copy on the device of every partition now, so that no search pays for it

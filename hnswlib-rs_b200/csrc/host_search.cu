@@ -15,6 +15,7 @@
 #include <numeric>
 #include <set>
 
+#include "../../include/hnsw_b200.h"
 #include "index.h"
 #include "partition.h"
 
@@ -411,6 +412,86 @@ int Index::exclusion_lists(const Exclusions& x, size_t nq, Ticket& t) {
   return 0;
 }
 
+int Index::admitted(const Restriction& rs, int64_t key, const LabelSets& sets, int p, size_t* count) {
+  Index* rx = holders()[p];
+  if (rs.kind == Restriction::RESIDENT) return filters.admitted(rs.resident, p, (int)holders().size(), rx, count);
+  if (rs.kind != Restriction::ROW_LABEL_SETS || key < 0) {
+    *count = rx->n;
+    return 0;
+  }
+  std::vector<ExactScan> slices;
+  const size_t at = sets.off[key];
+  if (int r = rx->scan_slices(sets.values.data() + at, sets.off[key + 1] - at, sets.range[2 * key], sets.range[2 * key + 1],
+                              slices))
+    return r;
+  *count = 0;
+  for (const ExactScan& x : slices) *count += x.n;
+  return 0;
+}
+
+// The rows sorted as a search sorts them, so that each distinct key is counted once per holder
+int Index::count_admitted(const Restriction& rs, size_t nq, uint64_t* out) {
+  std::vector<size_t> perm;
+  std::vector<int64_t> sorted;
+  LabelSets sets;
+  int r;
+  if (rs.per_row() && (r = sort_rows(rs, nq, perm, sorted, sets))) return r;
+  std::vector<uint64_t> c(nq, 0);
+  for (int p = 0; p < (int)holders().size(); ++p) {
+    size_t n = 0;
+    for (size_t j = 0; j < nq; ++j) {
+      const int64_t key = sorted.empty() ? -1 : sorted[j];
+      if ((j == 0 || (!sorted.empty() && key != sorted[j - 1])) && (r = admitted(rs, key, sets, p, &n)))
+        return holder_fail(p, r);
+      c[perm.empty() ? j : perm[j]] += n;
+    }
+  }
+  std::copy(c.begin(), c.end(), out);
+  return 0;
+}
+
+// Row j of leg l takes the exact scan when the scan can hold its k' keys (k, plus 1 with exclude_self) at this dimension
+// and c^2 <= GAMMA n e D, in 128-bit integers: c the points its restriction admits on the leg's holder, n the points
+// stored there, e = max(ef, k') the ef the graph search runs at, D = 2 M the layer-0 list capacity.  A graph search over a
+// fraction s = c / n of the points reads about e D / s rows, the exact scan c rows: the two meet at c^2 = GAMMA n e D.
+// The counts are the holder's, so that a replica's leg decides as the handle does.
+int Index::split_legs(Ticket& t, const std::vector<int64_t>& sorted) {
+  const HostBatch& b = t.b;
+  const size_t kq = b.k + (b.in.skip ? 1 : 0);
+  t.exact.assign(b.nq, 0);
+  int r = 0;
+  for (Leg& l : t.legs) {
+    Index* cx = holders()[l.part];
+    // exact_shape's least shape; a k' of more keys than the budget has bytes never fits (and stays within int)
+    const bool fits = kq <= SMEM_BUDGET && exact_layout(cx->row_bytes / 16, (int)kq, 1, 1, 2).bytes <= SMEM_BUDGET;
+    const unsigned __int128 bound =
+        (unsigned __int128)HNSW_B200_PLANNED_GAMMA * cx->n * std::max(b.ef, kq) * (2 * (unsigned __int128)cx->M);
+    LegSplit& s = l.split;
+    s.on = true;
+    size_t c = 0;
+    for (size_t j = 0; j < l.count; ++j) {
+      const int64_t key = sorted.empty() ? -1 : sorted[l.first + j];
+      if ((j == 0 || (!sorted.empty() && key != sorted[l.first + j - 1])) &&
+          (l.rc = admitted(b.restriction, key, t.sets, l.part, &c)))
+        break;
+      const bool exact = fits && (unsigned __int128)c * c <= bound;
+      s.rows[exact].push_back(j);
+      t.exact[l.first + j] += exact;
+    }
+    for (int e = 0; e < 2 && !l.rc; ++e) {  // the exact part reads a graph batch's EVERY_POINT rows as unrestricted
+      if (s.rows[e].empty()) continue;
+      std::vector<int64_t> keys;
+      if (!sorted.empty())
+        for (size_t j : s.rows[e]) keys.push_back(e && sorted[l.first + j] == EVERY_POINT ? -1 : sorted[l.first + j]);
+      Leg part{l.rx, l.part, 0, s.rows[e].size()};
+      if (resolve(b.restriction, e == 1, keys, &part, 1, t.bits, &t.sets)) l.rc = part.rc;
+      s.plan[e] = std::move(part.plan);
+    }
+    if (l.rc) r = -1;
+  }
+  return r;
+}
+
 // The handle's error for the first failed leg of legs[0, n) (0 if none failed): in leg order, or the replicas' before the
 // root's (replicas_first, the synchronous sharded search's order).  A partition's and a replica's message name it.
 int Index::legs_fail(const Leg* legs, size_t n, bool replicas_first) {
@@ -497,12 +578,55 @@ static HostRows leg_rows(const HostRows& in, const Leg& l, size_t q_bytes, uint6
 
 void Index::begin_leg(const HostBatch& b, Leg& l) {
   if (l.ctx < 0) l.ctx = l.rx->acquire_ctx();
+  LegSplit& s = l.split;
+  if (s.on) {
+    s.running = s.rows[0].empty() && !s.rows[1].empty();
+    s.slots.resize(l.count * b.k);
+    s.counts.resize(l.count);
+  }
+  start_leg(b, l);
+}
+
+// A planned part runs on its rows gathered from the leg's (sorted_rows), so that its answers are its rows' in order
+void Index::start_leg(const HostBatch& b, Leg& l) {
   std::vector<uint64_t> local;
   std::vector<ExcludedRow> xrows;
   std::vector<uint32_t> xids;
-  const HostRows in = leg_rows(b.in, l, (size_t)b.d * es, parts ? parts->count() : 0, local, xrows, xids);
-  l.rc = l.rx->search_host_begin(l.ctx, in, l.count, b.d, b.k, b.ef, l.plan);
+  std::vector<unsigned char> part;
+  const size_t q_bytes = (size_t)b.d * es;
+  const HostRows in = leg_rows(b.in, l, q_bytes, parts ? parts->count() : 0, local, xrows, xids);
+  const LegSplit& s = l.split;
+  if (s.on) {
+    const std::vector<size_t>& rows = s.rows[s.running];
+    l.rc = l.rx->search_host_begin(l.ctx, sorted_rows(in, rows, q_bytes, part), rows.size(), b.d, b.k, b.ef,
+                                   s.plan[s.running]);
+  } else {
+    l.rc = l.rx->search_host_begin(l.ctx, in, l.count, b.d, b.k, b.ef, l.plan);
+  }
   l.begun = l.rc == 0;
+}
+
+// A planned leg: each part's answers scattered to its rows, then the exact part begun and collected after the graph
+// part, on the same context (a second lease while holding one could deadlock two callers).  Only the pending part is
+// re-run when its visited tables overflow (search_host_finish), so an exact row runs and is written once.
+HostAnswers Index::collect_leg(const HostBatch& b, Leg& l) {
+  HostAnswers a = l.rx->search_host_finish(l.ctx);
+  LegSplit& s = l.split;
+  if (!s.on) return a;
+  for (;;) {
+    if (a.rc) return a;
+    const std::vector<size_t>& rows = s.rows[s.running];
+    for (size_t i = 0; i < rows.size(); ++i) {
+      s.counts[rows[i]] = a.counts[i];
+      memcpy(s.slots.data() + rows[i] * b.k, a.slots + i * b.k, b.k * sizeof(NeighbourOut));
+    }
+    if (s.running == 1 || s.rows[1].empty()) break;
+    s.running = 1;
+    start_leg(b, l);
+    if (l.rc) return HostAnswers{nullptr, nullptr, nullptr, l.rc};
+    a = l.rx->search_host_finish(l.ctx);
+  }
+  return HostAnswers{s.slots.data(), s.counts.data(), nullptr, 0};
 }
 
 void Index::release_leg(Leg& l) {
@@ -518,7 +642,7 @@ void Index::release_leg(Leg& l) {
 // collects a leg, writes its slice of b.out and releases its context
 int Index::end_leg(Leg& l, const HostBatch& b) {
   if (l.begun) {
-    const HostAnswers a = l.rx->search_host_finish(l.ctx);
+    const HostAnswers a = collect_leg(b, l);
     l.rc = a.rc;
     if (!l.rc) put_slice(b.out, l.rx, l.first, l.count, b.k, a);
   }
@@ -571,16 +695,25 @@ int Index::prepare_batch(const HostBatch& call, Ticket& t, bool replicas_first) 
     b.out.perm = t.perm.data();
   }
   if ((r = plan(b.nq, t.legs))) return r;
-  if (resolve(b.restriction, b.exact, sorted, t.legs.data(), t.legs.size(), t.bits, &t.sets, b.stored))
+  if (b.planned ? split_legs(t, sorted)
+                : resolve(b.restriction, b.exact, sorted, t.legs.data(), t.legs.size(), t.bits, &t.sets, b.stored))
     return legs_fail(t.legs.data(), t.legs.size(), replicas_first && !parts);
   return 0;
 }
 
+// A planned batch writes each row's exact count (out.exact) once every leg succeeded
 int Index::search_batch(const HostBatch& call) {
   if (call.nq == 0) return 0;
   Ticket t;
   int r;
-  if ((r = prepare_batch(call, t, true))) return r;
+  if ((r = prepare_batch(call, t, true)) || (r = run_batch(t))) return r;
+  const AnswerArrays& out = t.b.out;
+  if (out.exact)
+    for (size_t j = 0; j < t.exact.size(); ++j) out.exact[out.perm ? out.perm[j] : j] = t.exact[j];
+  return 0;
+}
+
+int Index::run_batch(Ticket& t) {
   const HostBatch& b = t.b;
   std::vector<Leg>& legs = t.legs;
   const int n = (int)legs.size();
@@ -608,7 +741,7 @@ int Index::search_batch(const HostBatch& call) {
   std::vector<HostAnswers> a(n);
   for (int p = 0; p < n; ++p) {
     if (legs[p].begun) {
-      a[p] = legs[p].rx->search_host_finish(legs[p].ctx);
+      a[p] = collect_leg(b, legs[p]);
       legs[p].rc = a[p].rc;
     }
     if (legs[p].rc && bad < 0) bad = p;

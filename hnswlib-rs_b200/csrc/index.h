@@ -217,6 +217,7 @@ class FilterStore {
   struct Filter {
     std::vector<std::vector<uint32_t>> bits;  // [partition] bit per internal id (make_filter_bits)
     std::vector<size_t> counts;               // [partition] points stored when the filter was made
+    std::vector<size_t> admitted;             // [partition] points it admits (bits set in bits[partition])
     std::map<std::pair<int, int>, DeviceBuffer> dev;  // (partition, device) -> device copy of bits[partition]
     // (partition, device) -> the admitted internal ids of bits[partition], sorted, on the device, and their count; made
     // at the first exact search with the filter there
@@ -228,11 +229,14 @@ class FilterStore {
   // exists and that rx, partition p of `nparts`, still holds the points the filter was made over; if not, rx's error.
   // With `list`, the sorted id list of the admitted points instead (made and copied there on first use).
   int use(int64_t id, int p, int nparts, const Index* rx, const uint32_t** d_bits, ExactScan* list = nullptr);
+  // the number of points partition p's bitmap admits, after use's checks
+  int admitted(int64_t id, int p, int nparts, const Index* rx, size_t* count);
   void erase(int64_t id);  // frees its device copies; the caller waited for every search that may read them
 
  private:
   std::mutex mu_;
   std::map<int64_t, Filter> f_;
+  Filter* current(int64_t id, int p, int nparts, const Index* rx);  // use's checks (the caller holds mu_); nullptr: rx's error
 };
 
 class Partitions;  // partition.cu: the points of one handle split over several Index objects
@@ -279,6 +283,7 @@ struct AnswerArrays {
   int32_t* counts = nullptr;
   const size_t* perm = nullptr;  // row j of the batch is written to row perm[j] (nullptr: to row j)
   uint64_t* total = nullptr;
+  int32_t* exact = nullptr;  // a planned batch: per row, the legs that scanned it exactly (optional)
 };
 
 // What the rows of a batch may return: every point (NONE); the points a FilterT admits (FILTER_T: `mode` 1 sorted
@@ -358,6 +363,7 @@ struct HostBatch {
   AnswerArrays out;
   Exclusions excluded;
   bool stored = false;
+  bool planned = false;  // each row on the graph or by the exact scan, per leg, by the planned rule (exact unset)
 };
 
 // A leg's restriction (Index::resolve): its rows [0, plain) are unrestricted, and `runs` cover the rest, each a range of
@@ -390,8 +396,21 @@ struct LegPlan {
   const uint32_t* deleted = nullptr;
 };
 
+// A planned leg's rows split by the planned rule (Index::split_legs): rows[0] the leg rows that take the graph search,
+// rows[1] those that take the exact scan, each ascending and under its own plan.  The parts run one after the other on
+// the leg's one context, the graph part first (`running`: the part begun there), and their answers are gathered into
+// `slots` and `counts` in leg-row order, so that the leg's answers read as an unsplit leg's.
+struct LegSplit {
+  bool on = false;
+  std::vector<size_t> rows[2];
+  LegPlan plan[2];
+  int running = 0;
+  std::vector<NeighbourOut> slots;
+  std::vector<int32_t> counts;
+};
+
 // One Index's part of a batch: queries [first, first + count) searched on rx (the handle, a replica, or partition `part`)
-// on its leased context ctx, under its plan
+// on its leased context ctx, under its plan (a planned batch: its split's plans)
 struct Leg {
   Index* rx = nullptr;
   int part = 0;
@@ -400,6 +419,7 @@ struct Leg {
   bool begun = false;  // enqueued
   int rc = 0;
   LegPlan plan;
+  LegSplit split;
 };
 
 // A handle's settings (its setters, hnsw.rs:810-905).  One value, on the handle; its partitions and replicas read it
@@ -473,8 +493,10 @@ class Index {
     LabelSets sets;
     std::vector<ExcludedRow> xrows;  // per caller row, into xids (exclusion_lists)
     std::vector<uint32_t> xids;
+    std::vector<int32_t> exact;  // a planned batch: per batch row, the legs that scan it exactly
   };
   int search_batch(const HostBatch& b);
+  int run_batch(Ticket& t);  // the planned legs of t begun, collected and written
   int64_t submit_batch(const HostBatch& b);  // a ticket id, or < 0
   int finish_batch(Ticket& t);
   // submitted-but-not-waited host searches: anything that changes the graph waits for them (drain_pending)
@@ -504,6 +526,12 @@ class Index {
   int exclusion_lists(const Exclusions& x, size_t nq, Ticket& t);
   // the key sort_rows' keys leave free, which resolve makes a run over every point (LegPlan::Run::every)
   static constexpr int64_t EVERY_POINT = -2;
+  // out[i]: the points row i of rs admits (none, a resident filter, or label sets with optional ranges), summed over the
+  // holders, deleted points included; sort_rows' and the filters' checks refuse as a search would
+  int count_admitted(const Restriction& rs, size_t nq, uint64_t* out);
+  // the points that the row key `key` of rs (sort_rows' keys; -1 and EVERY_POINT: every point) admits on holder p:
+  // its n, a resident filter's count, or the lengths of a label set's scan_slices
+  int admitted(const Restriction& rs, int64_t key, const LabelSets& sets, int p, size_t* count);
 
   // ---- point labels and attributes (labels.cu): a u32 label per point, LABEL_NONE = none, and an int64 attribute per
   // point, stored as attr_bias(value), 0 = none (ATTR_NONE)
@@ -738,7 +766,12 @@ class Index {
   // ---- host search batches (host_search.cu)
   int plan(size_t nq, std::vector<Leg>& legs);
   int prepare_batch(const HostBatch& call, Ticket& t, bool replicas_first);
+  // a planned batch's legs split by the planned rule (t.exact counts the exact rows), each part resolved on its own
+  int split_legs(Ticket& t, const std::vector<int64_t>& sorted);
   void begin_leg(const HostBatch& b, Leg& l);
+  void start_leg(const HostBatch& b, Leg& l);  // enqueues the leg, or its running part
+  // a begun leg's answers: a planned leg's parts collected one after the other into its split
+  HostAnswers collect_leg(const HostBatch& b, Leg& l);
   void release_leg(Leg& l);
   int end_leg(Leg& l, const HostBatch& b);
   int legs_fail(const Leg* legs, size_t n, bool replicas_first);

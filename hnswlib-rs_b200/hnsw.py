@@ -122,6 +122,9 @@ def load_library():
     L.hnsw_b200_search_exact_radius_by_id.argtypes = [vp, vp, u64, vp, u64, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_flat_excluding.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp]
     L.hnsw_b200_search_exact_excluding.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp, u64, u64, u64, vp, vp, vp, vp, vp]
+    L.hnsw_b200_count_admitted.argtypes = [vp, i64, vp, vp, vp, u64, vp]
+    L.hnsw_b200_search_planned.argtypes = [vp, vp, vp, i64, vp, vp, vp, vp, u64, u64, u64, u64, vp, vp, vp, vp, vp, vp]
+    L.hnsw_b200_search_planned_by_id.argtypes = [vp, vp, u64, u64, u64, i32, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.hnsw_b200_delete_points.argtypes = [vp, vp, u64]
     L.hnsw_b200_restore_points.argtypes = [vp, vp, u64]
     L.hnsw_b200_get_deleted.argtypes = [vp, u64, u64, vp]
@@ -707,6 +710,54 @@ class Hnsw:
         """hnsw_b200_search_exact_excluding: search_flat_excluding with the exact search in place of the graph one"""
         return self._excluding(self._L.hnsw_b200_search_exact_excluding, queries, knbn, (), excluded, filter, sets, ranges,
                                with_internal, with_pid)
+
+    # ---- planned search (include/hnsw_b200.h "Planned search")
+    def _restriction(self, nq, filter, sets, ranges):
+        """the filter id and the (qrange, qset_off, qset) arrays (None: NULL) of a call that reads its restriction as
+        search_by_id does"""
+        rg = None if ranges is None else _ranges(ranges, nq)
+        off, vals = (None, None) if sets is None else _label_sets(sets, nq)
+        return _filter_id(filter), (rg, off, vals)
+
+    def count_admitted(self, filter=None, sets=None, ranges=None, n=None):
+        """hnsw_b200_count_admitted: for each of n rows (default: as many as sets or ranges has), the number of points
+        its restriction admits, deleted points included, as a uint64 array.  The restriction is search_by_id's."""
+        if n is None:
+            n = len(sets[0]) - 1 if isinstance(sets, tuple) else len(sets) if sets is not None else \
+                len(ranges) if ranges is not None else 1
+        out = np.zeros(int(n), np.uint64)
+        fid, rows = self._restriction(int(n), filter, sets, ranges)
+        self._chk(self._L.hnsw_b200_count_admitted(self._h, fid, *map(_p, rows), int(n), _p(out)))
+        return out
+
+    def search_planned(self, queries, knbn, ef, excluded=None, filter=None, sets=None, ranges=None, with_internal=True,
+                       with_pid=True):
+        """hnsw_b200_search_planned: each row on the graph (the row of search_flat_excluding) or by the exact scan (the
+        row of search_exact_excluding), whichever the planned rule picks for its admitted set.  excluded: as
+        search_flat_excluding takes it, or None.  Returns search_flat's (origin, dist, internal | None, pid | None,
+        counts) and exact i32[nq], the number of indexes (partitions) that scanned each row exactly."""
+        q = np.ascontiguousarray(queries, self.dtype)
+        nq = q.shape[0]
+        off, ids = (None, None) if excluded is None else _excluded(excluded, nq)
+        ans = self._answers(nq, knbn, with_internal, with_pid)
+        exact = np.empty(nq, np.int32)
+        fid, rows = self._restriction(nq, filter, sets, ranges)
+        self._chk(self._L.hnsw_b200_search_planned(self._h, _p(off), _p(ids), fid, *map(_p, rows), _p(q), *q.shape,
+                                                   int(knbn), int(ef), *map(_p, ans), _p(exact)))
+        return ans + (exact,)
+
+    def search_planned_by_id(self, qids, knbn, ef, filter=None, sets=None, ranges=None, exclude_self=False,
+                             with_internal=True, with_pid=True):
+        """hnsw_b200_search_planned_by_id: search_planned with query i the stored point qids[i], each row that of
+        search_by_id or search_exact_by_id.  Returns search_planned's tuple."""
+        q = np.ascontiguousarray(qids, np.uint64).reshape(-1)
+        nq = q.size
+        ans = self._answers(nq, knbn, with_internal, with_pid)
+        exact = np.empty(nq, np.int32)
+        fid, rows = self._restriction(nq, filter, sets, ranges)
+        self._chk(self._L.hnsw_b200_search_planned_by_id(self._h, _p(q), nq, int(knbn), int(ef), int(bool(exclude_self)),
+                                                         fid, *map(_p, rows), *map(_p, ans), _p(exact)))
+        return ans + (exact,)
 
     # ---- search by stored point (include/hnsw_b200.h "Search by stored point")
     def get_vectors(self, ranks):

@@ -625,6 +625,44 @@ int hnsw_b200_restore_points(void* h, const uint64_t* ranks, uint64_t n);
 int hnsw_b200_get_deleted(const void* h, uint64_t first, uint64_t n, uint8_t* out); /* 1 deleted, 0 live */
 int64_t hnsw_b200_get_nb_deleted(const void* h);
 
+/* ---- Planned search: each row on the graph or by the exact scan, whichever its admitted set makes cheaper, so that a
+ * batch that mixes small and large restrictions (tenants of very different sizes, filtered and unfiltered rows) needs
+ * no split by the caller.
+ *   count_admitted: out_count[i] = the number of points row i's restriction admits, deleted points included (they are
+ *     still scanned and still route the graph search, so they cost like live ones); excluded lists are not an argument.
+ *     The restriction is read as hnsw_b200_search_exact_by_id reads it.  A partitioned handle returns the sum over its
+ *     partitions, a partition view its own count.
+ *   The rule: row i on index p (the handle, or each partition of a partitioned handle) takes the exact scan when
+ *     k' = knbn (+ 1 with exclude_self) fits the exact scan at this dimension and c^2 <= GAMMA * n * e * D, in exact
+ *     integer arithmetic: c the row's count_admitted on p, n the points p holds, e = max(ef_search, k'), D = 2 *
+ *     max_nb_connection; otherwise the graph search.  A graph search over a fraction s = c / n of the points reads about
+ *     e D / s rows, the exact scan c rows.  GAMMA is HNSW_B200_PLANNED_GAMMA, measured on an H100 (DESIGN.md §4.2d).
+ *   Rows: a graph row is, bit for bit, the row of hnsw_b200_search_flat_excluding with the same restriction, list, knbn
+ *     and ef (_by_id: hnsw_b200_search_flat_by_id), an exact row the row of hnsw_b200_search_exact_excluding
+ *     (hnsw_b200_search_exact_by_id): ids, distance bits, internal ids, PointIds, counts; with statistics on, the
+ *     counters add what the graph rows' calls add, and the exact rows nothing.  out_exact[i] (may be NULL): the number
+ *     of indexes that scanned row i exactly, 0 or 1, or 0..P on a partitioned handle.
+ *   Lists: qx_off and qx as search_flat_excluding takes them, or both NULL for no lists.
+ *   Handles: a partitioned handle decides per partition and merges each row by the partitioned rule (distance, then
+ *     partition, then position), reporting global ranks; a replicated handle shards the batch like search_flat, and
+ *     decides as the handle does; a partition view uses its own points and local ids.  The handle is taken shared.
+ *   Checks, before anything runs, with the wording of the calls the rows are defined by: a NULL handle, nq == 0 (returns
+ *     0), qids NULL, exactly one of qx_off and qx NULL, a filter with sets or ranges, stale, foreign or unknown filters,
+ *     bad offsets, ranks >= nb_point.  A refused call leaves every output untouched.
+ *   Not offered: a resident filter per query, radius search, submit / wait and device-resident variants. */
+#define HNSW_B200_PLANNED_GAMMA 23
+int hnsw_b200_count_admitted(const void* h, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                             const uint32_t* qset, uint64_t nq, uint64_t* out_count);
+int hnsw_b200_search_planned(const void* h, const uint64_t* qx_off, const uint64_t* qx, int64_t filter,
+                             const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
+                             const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
+                             uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
+                             int32_t* out_counts, int32_t* out_exact);
+int hnsw_b200_search_planned_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, uint64_t ef_search,
+                                   int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
+                                   const uint32_t* qset, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
+                                   int32_t* out_pid, int32_t* out_counts, int32_t* out_exact);
+
 /* Run this handle's kernels and copies on a caller-owned CUDA stream (cudaStream_t passed as void*; NULL
  * restores the handle's own stream), e.g. so that torch.cuda.Event on torch's current stream brackets them. */
 int hnsw_b200_join(void* h);
