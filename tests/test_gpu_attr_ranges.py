@@ -13,42 +13,10 @@ import pytest
 from answers import per_group, same, same_as_single_filter_calls
 from exactref import expected, origin_ids
 from graphs import data
-from restrict import GRAPH_CASES, NONE, N, build, free, point_labels, unrestricted
+from restrict import (FULL, GRAPH_CASES, I64_MAX, I64_MIN, NONE, ROWS, N, admitted, build, free, point_attrs,
+                      point_labels, unrestricted)
 
 pytestmark = pytest.mark.gpu
-
-I64_MIN, I64_MAX = -(1 << 63), (1 << 63) - 1
-FULL = (I64_MIN, I64_MAX)
-
-
-def point_attrs(n, seed):
-    """values in [-1000, 1000) (~20 % of the points without one), one point at INT64_MIN + 1, one at INT64_MAX and one
-    at 4242, the only value outside [-1000, 1000)"""
-    rng = np.random.default_rng(seed)
-    a = rng.integers(-1000, 1000, n, dtype=np.int64)
-    a[rng.random(n) < 0.2] = I64_MIN
-    i = rng.choice(n, 3, replace=False)
-    a[i] = [I64_MIN + 1, I64_MAX, 4242]
-    return a
-
-
-# (label set, range): a range alone, with a one-label and a several-label set, with an empty set; full ranges with a
-# set and with [LABEL_NONE]; lo > hi; ranges admitting no point, one point (4242) and every point with an attribute;
-# bounds at INT64_MIN + 1 and INT64_MAX
-ROWS = [([NONE], (-100, 300)), ([0], (0, 500)), ([1, 2, 8], (-500, 499)), ([0, 1], FULL), ([NONE], FULL),
-        ([NONE], (10, 5)), ([NONE], (2000, 4000)), ([NONE], (4242, 4242)), ([NONE], (I64_MIN + 1, I64_MAX)),
-        ([NONE], (I64_MAX, I64_MAX)), ([NONE], (I64_MIN, I64_MIN + 1)), ([7, 8], (-1000, 999)), ([], (0, 100)),
-        ([2], (I64_MIN, 0)), ([NONE], (I64_MIN, I64_MIN))]
-
-
-def admitted(lab, attr, s, r):
-    m = np.ones(len(attr), bool)
-    if not unrestricted(s):
-        m &= np.isin(lab, np.array(s, np.uint32))
-    if tuple(r) != FULL:
-        m &= (attr != I64_MIN) & (attr >= r[0]) & (attr <= r[1])
-    return m
-
 
 def filters_for(h, lab, attr, og, rows=ROWS):
     """one resident filter per (set, range) row (None for the unrestricted one)"""

@@ -11,6 +11,7 @@ import torch  # imported first, so that torch's own NCCL is the one the library 
 from answers import device_answers, same, same_host_device
 from graphs import data
 from liveref import LiveRef
+from restrict import deleted_set
 from util import oracle_layers
 
 pytestmark = pytest.mark.gpu
@@ -30,24 +31,6 @@ def build(pkg, po, dtype, metric, d, seed=3):
     h.import_graph(X, og, lv, o.entry, oracle_layers(o))
     Q = data(dtype, metric, NQ, d, seed + 100)
     return X, Q, o, h
-
-
-def deleted_set(po, kind, X, Q, metric, entry, seed=11):
-    rng = np.random.default_rng(seed)
-    n = len(X)
-    if kind == "one":
-        return np.array([int(rng.integers(n))])
-    if kind == "entry":
-        return np.array([entry])
-    if kind == "top5":
-        return np.unique(po.bruteforce(X, Q, 5, metric, po.ORDER_GPU)[0])
-    if kind == "tenth":
-        return np.sort(rng.choice(n, n // 10, replace=False))
-    if kind == "half":
-        return np.sort(rng.choice(n, n // 2, replace=False))
-    if kind == "all_but_one":
-        return np.delete(np.arange(n), int(rng.integers(n)))
-    return np.arange(n)
 
 
 def live_of(n, dead):

@@ -15,6 +15,7 @@ import torch  # imported first, so that torch's own NCCL is the one the library 
 
 from answers import same, stats_sum
 from graphs import data
+from restrict import lists_for
 from util import oracle_layers
 
 pytestmark = pytest.mark.gpu
@@ -36,20 +37,6 @@ def build(pkg, po, dtype, metric, d, seed):
     h = pkg.Hnsw(M, N, 16, EFC, metric, dtype=dtype)
     h.import_graph(X, og, lv, o.entry, oracle_layers(o))
     return X, h
-
-
-def lists_for(po, X, Q, metric, entry, n, seed):
-    """row i's list, by kind i % 7: empty, one id, the query's brute-force top 20, the entry point, half of the points,
-    every point, and a random third of the points unsorted with repeats"""
-    rng = np.random.default_rng(seed)
-    top, _ = po.bruteforce(X, Q, 20, metric, po.ORDER_GPU)
-    out = []
-    for i in range(len(Q)):
-        kind = i % 7
-        out.append([np.zeros(0, np.int64), np.array([int(rng.integers(n))]), top[i].astype(np.int64),
-                    np.array([entry]), np.sort(rng.choice(n, n // 2, replace=False)), np.arange(n),
-                    np.concatenate([x := rng.choice(n, n // 3, replace=False), x[: n // 10]])][kind])
-    return out
 
 
 class Reference:

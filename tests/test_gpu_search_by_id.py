@@ -10,8 +10,9 @@ import pytest
 import torch  # device buffers; imported first, so that torch's own NCCL is the one the library binds at run time
 
 from answers import same
-from exactref import INVALID, expected, origin_ids
+from exactref import expected, origin_ids
 from graphs import data
+from restrict import minus_self
 from util import oracle_layers
 
 pytestmark = pytest.mark.gpu
@@ -36,22 +37,6 @@ def some_ids(n, seed, count=80):
     rng = np.random.default_rng(seed)
     q = rng.choice(n, count, replace=False)
     return np.concatenate([q, q[:5], [0, n - 1]]).astype(np.uint64)
-
-
-def minus_self(rows, qids, k):
-    """the (k + 1)-wide rows `rows` under the exclude_self rule, k wide"""
-    o, d, it, pid, c = rows
-    nq = len(qids)
-    ro = np.full((nq, k), np.iinfo(np.uint64).max, np.uint64)
-    rd = np.full((nq, k), np.inf, np.float32)
-    ri = np.full((nq, k), INVALID, np.uint32)
-    rp = np.full((nq, k, 2), -1, np.int32)
-    rc = np.zeros(nq, np.int32)
-    for i in range(nq):
-        keep = [j for j in range(c[i]) if it[i, j] != qids[i]][:k]
-        n = len(keep)
-        ro[i, :n], rd[i, :n], ri[i, :n], rp[i, :n], rc[i] = o[i, keep], d[i, keep], it[i, keep], pid[i, keep], n
-    return ro, rd, ri, rp, rc
 
 
 F32_CASES = [(np.float32, m, d) for m in ("DistL1", "DistL2", "DistDot", "DistCosine") for d in (24, 48, 100, 150)]
