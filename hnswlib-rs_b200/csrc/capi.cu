@@ -393,6 +393,39 @@ int hnsw_b200_file_dump(const void* h, const char* dir, const char* basename, in
   return 0;
 }
 
+int hnsw_b200_save(const void* h, const char* dir, const char* basename, int overwrite, char* used_basename,
+                   size_t used_cap) {
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
+  if (!dir || !basename) return set_err("NULL path");
+  std::string used;
+  if (pass(ix, ix->save(dir, basename, overwrite != 0, &used))) return -1;
+  if (used_basename && used_cap) {
+    strncpy(used_basename, used.c_str(), used_cap - 1);
+    used_basename[used_cap - 1] = 0;
+  }
+  return 0;
+}
+
+void* hnsw_b200_restore(const char* dir, const char* basename, int ndev, const int* devices) {
+  if (!dir || !basename) {
+    set_err("restore: NULL path");
+    return nullptr;
+  }
+  try {  // nothing may unwind through the C boundary (an allocation sized by the files may fail)
+    std::string e;
+    Index* ix = Index::restore(dir, basename, ndev, devices, g_device, e);
+    if (!ix) {
+      set_err(e);
+      return nullptr;
+    }
+    return new AnyApi{ix};
+  } catch (const std::exception& ex) {
+    set_err(std::string("restore: ") + ex.what());
+    return nullptr;
+  }
+}
+
 // load_hnsw_description, libext.rs:1170-1232.  `name` = path of the .hnsw.graph file.  Release with
 // hnsw_b200_free_description (upstream leaks it).
 const DescriptionFFI* load_hnsw_description(size_t flen, const uint8_t* name) {

@@ -230,10 +230,10 @@ int read_description(const std::string& graph_path, DumpDescription& out, std::s
 }
 
 // ------------------------------------------------------------------------------------------------ load
-int Index::load_dump(const std::string& dir, const std::string& basename) {
-  if (n != 0) return fail("load needs an empty index");
+// the pair <basename>.hnsw.graph / .hnsw.data into `out`, checked against this Index's element type, metric and M
+int Index::parse_dump(const std::string& dir, const std::string& basename, ParsedDump& out) const {
   const std::string gpath = dir + "/" + basename + ".hnsw.graph", dpath = dir + "/" + basename + ".hnsw.data";
-  DumpDescription de;
+  DumpDescription& de = out.de;
   std::string e;
   if (read_description(gpath, de, e)) return fail(e);
   if (de.format_version == 2) return fail("dump format v2 (bincode-encoded vectors) is not supported; re-dump with hnsw_rs >= 0.2");
@@ -274,9 +274,12 @@ int Index::load_dump(const std::string& dir, const std::string& basename) {
     int32_t rank;
     float dist;
   };
-  std::vector<uint64_t> origin;
-  std::vector<uint8_t> levels;
-  std::vector<unsigned char> vecs;
+  std::vector<uint64_t>& origin = out.origin;
+  std::vector<uint8_t>& levels = out.levels;
+  std::vector<unsigned char>& vecs = out.vecs;
+  origin.clear();
+  levels.clear();
+  vecs.clear();
   origin.reserve(N);
   levels.reserve(N);
   vecs.reserve(N * D * ES);
@@ -333,43 +336,57 @@ int Index::load_dump(const std::string& dir, const std::string& basename) {
     const size_t id = layer_start[lv] + (size_t)rk;
     return id < layer_start[lv + 1] ? (int64_t)id : -1;
   };
-  const int64_t entry_id = id_of(e_lv, e_rk);
-  if (entry_id < 0) return fail("entry point of the dump not found");
+  out.entry = id_of(e_lv, e_rk);
+  if (out.entry < 0) return fail("entry point of the dump not found");
   // ---- CSR per layer, neighbours resolved through their PointId (hnswio.rs:700-735)
-  std::vector<std::vector<uint64_t>> off(MAX_LAYERS);
-  std::vector<std::vector<uint32_t>> ids(MAX_LAYERS);
-  std::vector<std::vector<float>> ds(MAX_LAYERS);
+  out.off.assign(MAX_LAYERS, {});
+  out.ids.assign(MAX_LAYERS, {});
+  out.dists.assign(MAX_LAYERS, {});
   int nl = 0;
   for (int l = 0; l < MAX_LAYERS; ++l) {
-    off[l].assign(N + 1, 0);
+    out.off[l].assign(N + 1, 0);
     lists[l].resize(N);
     for (size_t p = 0; p < N; ++p) {
-      off[l][p] = ids[l].size();
+      out.off[l][p] = out.ids[l].size();
       for (const Nb& nb : lists[l][p]) {
         const int64_t q = id_of(nb.level, nb.rank);
         if (q < 0) return fail("neighbour PointId of the dump not found");
-        ids[l].push_back((uint32_t)q);
-        ds[l].push_back(nb.dist);
+        out.ids[l].push_back((uint32_t)q);
+        out.dists[l].push_back(nb.dist);
       }
     }
-    off[l][N] = ids[l].size();
-    if (!ids[l].empty()) nl = l + 1;
+    out.off[l][N] = out.ids[l].size();
+    if (!out.ids[l].empty()) nl = l + 1;
   }
-  nl = std::max(nl, 1);
-  std::vector<const uint64_t*> po(nl);
-  std::vector<const uint32_t*> pi(nl);
-  std::vector<const float*> pd(nl);
-  for (int l = 0; l < nl; ++l) {
-    po[l] = off[l].data();
-    pi[l] = ids[l].data();
-    pd[l] = ds[l].data();
+  out.nlayers = std::max(nl, 1);
+  out.n = N;
+  out.d = (int)D;
+  return 0;
+}
+
+int Index::import_dump(const ParsedDump& p) {
+  std::vector<const uint64_t*> po(p.nlayers);
+  std::vector<const uint32_t*> pi(p.nlayers);
+  std::vector<const float*> pd(p.nlayers);
+  for (int l = 0; l < p.nlayers; ++l) {
+    po[l] = p.off[l].data();
+    pi[l] = p.ids[l].data();
+    pd[l] = p.dists[l].data();
   }
-  ef_c = (int)de.ef;
+  return import_graph(p.vecs.data(), p.n, p.d, p.origin.data(), p.levels.data(), p.entry, p.nlayers, po.data(), pi.data(),
+                      pd.data());
+}
+
+int Index::load_dump(const std::string& dir, const std::string& basename) {
+  if (n != 0) return fail("load needs an empty index");
+  ParsedDump p;
+  int r;
+  if ((r = parse_dump(dir, basename, p))) return r;
+  ef_c = (int)p.de.ef;
   // the reference re-applies the stored scale as a FACTOR of 1/ln(M) on reload (hnswio.rs:773-777 with
   // hnsw.rs:339-352): levels drawn for points inserted after a reload follow that law, mirrored here
-  settings().level_scale = (1.0 / std::log((double)M)) * de.level_scale;
-  int r = import_graph(vecs.data(), N, (int)D, origin.data(), levels.data(), entry_id, nl, po.data(), pi.data(), pd.data());
-  if (r) return r;
+  settings().level_scale = (1.0 / std::log((double)M)) * p.de.level_scale;
+  if ((r = import_dump(p))) return r;
   if (ef_c > 2 * M) settings().extend_candidates = true;  // hnswio.rs:510,599: reloaded indexes extend candidates
   return 0;
 }

@@ -177,6 +177,21 @@ struct DumpDescription {  // Description, /root/reference/src/hnswio.rs:846-870
   long header_bytes = 0;
 };
 int read_description(const std::string& graph_path, DumpDescription& out, std::string& err);
+// A reference-format pair read into memory (Index::parse_dump): its points in file order (layer by layer, by PointId
+// rank within a layer), their vectors, and each layer's lists as CSR over those file positions
+struct ParsedDump {
+  DumpDescription de;
+  size_t n = 0;
+  int d = 0;
+  std::vector<uint64_t> origin;
+  std::vector<uint8_t> levels;
+  std::vector<unsigned char> vecs;  // [n][d] elements
+  int64_t entry = -1;
+  int nlayers = 1;  // layers [0, nlayers) hold lists
+  std::vector<std::vector<uint64_t>> off;  // [layer][n + 1]
+  std::vector<std::vector<uint32_t>> ids;
+  std::vector<std::vector<float>> dists;
+};
 int metric_from_name(const std::string& name);       // "DistL2" -> METRIC_L2; -1 if unknown
 int metric_from_type_name(const std::string& full);  // the same on the last `::` segment of a type path
 int dtype_from_type_name(const std::string& s);
@@ -593,7 +608,15 @@ class Index {
   int flatten(std::vector<uint64_t>& offsets, std::vector<uint64_t>& nb_origin, std::vector<float>& nb_dist) const;
   // dump / reload in the reference's two-file format (hnswio.cu)
   int file_dump(const std::string& dir, const std::string& basename, bool overwrite, std::string* used_basename);
-  int load_dump(const std::string& dir, const std::string& basename);
+  int load_dump(const std::string& dir, const std::string& basename);  // parse_dump + import_dump, as the reference reloads
+  int parse_dump(const std::string& dir, const std::string& basename, ParsedDump& out) const;
+  int import_dump(const ParsedDump& p);  // import_graph of p's points, internal ids in p's order
+  // saved indexes (saved.cu): the handle's pair(s) and a manifest of what the pairs do not hold (ranks, columns, deleted
+  // points, settings, level RNG), so that restore gives back the same index.  save refuses before it writes anything;
+  // restore returns a new handle, or nullptr with `err` set, leaving nothing behind.
+  int save(const std::string& dir, const std::string& basename, bool overwrite, std::string* used_basename);
+  static Index* restore(const std::string& dir, const std::string& basename, int ndev, const int* devices, int device,
+                        std::string& err);
   // the work counters summed over the holders (a query counts once per partition) and the replicas
   int get_stats(uint64_t* out4, bool reset);
 

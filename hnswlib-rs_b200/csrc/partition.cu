@@ -26,6 +26,11 @@ int Partitions::fail(int p, const std::string& why) const {
   return parent_->fail("partition " + std::to_string(p) + " (device " + std::to_string(ix_[p]->device) + "): " + why);
 }
 
+int Partitions::run(const std::function<int(int)>& job) {
+  const int bad = workers_.run(count(), job);
+  return bad < 0 ? 0 : fail(bad, ix_[bad]->err());
+}
+
 int Partitions::create(Index* parent, int nparts, const int* devices) {
   DeviceRestore keep;
   if (parent->owner) return parent->fail("partition: a partition view cannot be partitioned");

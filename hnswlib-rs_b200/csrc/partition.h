@@ -45,6 +45,10 @@ class Partitions {
              const int32_t* levels, int d);
   // the handle's error "partition p (device D): why"
   int fail(int p, const std::string& why) const;
+  // job(p) for every partition at once, one per worker; the first failure as fail(p, that partition's error)
+  int run(const std::function<int(int)>& job);
+  // why a failed insert left the partitions unusable for inserts ("" while they are not)
+  const std::string& broken() const { return broken_; }
 
  private:
   explicit Partitions(Index* parent) : parent_(parent) {}

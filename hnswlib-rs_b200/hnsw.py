@@ -8,6 +8,7 @@ an index without a usable CUDA device raises.
 """
 import ctypes as C
 import os
+import struct
 
 import numpy as np
 
@@ -61,6 +62,9 @@ def load_library():
     L.hnsw_b200_free_hnswio.argtypes = [vp]
     L.hnsw_b200_file_dump.argtypes = [vp, C.c_char_p, C.c_char_p, i32, C.c_char_p, sz]
     L.hnsw_b200_load_dump.restype = vp
+    L.hnsw_b200_save.argtypes = [vp, C.c_char_p, C.c_char_p, i32, C.c_char_p, sz]
+    L.hnsw_b200_restore.restype = vp
+    L.hnsw_b200_restore.argtypes = [C.c_char_p, C.c_char_p, i32, vp]
     L.hnsw_b200_load_dump.argtypes = [vp, i32, sz, C.c_char_p]
     L.load_hnsw_description.restype = vp
     L.load_hnsw_description.argtypes = [sz, C.c_char_p]
@@ -218,6 +222,9 @@ class Neighbour:
 
 _DT = {np.dtype(np.float32): (0, "f32"), np.dtype(np.uint8): (1, "u8"), np.dtype(np.uint16): (2, "u16"),
        np.dtype(np.uint32): (3, "u32"), np.dtype(np.int32): (4, "i32")}
+# the C ABI's metric ids (hnsw_b200.h), in order
+_METRICS = ("DistL1", "DistL2", "DistDot", "DistCosine", "DistHamming", "DistJaccard", "DistHellinger", "DistJeffreys",
+            "DistJensenShannon")
 
 
 def _filter_args(filter):
@@ -954,6 +961,35 @@ class Hnsw:
         self._suf = _DT[self.dtype][1]
         self.max_nb_connection = None
         self.ef_construction = None
+        return self
+
+    def save(self, path, basename, overwrite=True):
+        """hnsw_b200_save: the index with its ranks, labels, attributes, deleted points, settings and level RNG, as
+        <basename>.hnsw.graph / .hnsw.data (one pair <basename>-p<i> per partition of a partitioned handle) and the
+        manifest <basename>.hnsw.b200, under `path`.  Returns the basename used (a unique one when overwrite is False
+        and a file of the set exists)."""
+        used = C.create_string_buffer(4096)
+        self._chk(self._L.hnsw_b200_save(self._h, str(path).encode(), basename.encode(), int(bool(overwrite)), used, 4096))
+        return used.value.decode()
+
+    @classmethod
+    def restore(cls, path, basename, devices=None):
+        """hnsw_b200_restore: the index `save` wrote, its element type and metric read from the files.  devices: None
+        (the current device), or one device per saved partition (a device may repeat)."""
+        L = load_library()
+        d = None if devices is None else np.ascontiguousarray(devices, np.int32)
+        h = L.hnsw_b200_restore(str(path).encode(), basename.encode(), 0 if d is None else len(d), None if d is None else _p(d))
+        if not h:
+            raise HnswError("restore failed: " + last_error())
+        # the manifest begins u32 magic, version, dtype, metric, M, max_layer, u64 dim, ef_construction (saved.cu)
+        with open(os.path.join(str(path), basename + ".hnsw.b200"), "rb") as f:
+            _, _, code, metric, M, _, _, efc = struct.unpack("=6I2Q", f.read(40))
+        self = cls.__new__(cls)
+        self._L, self._h = L, h
+        self.dtype = next(t for t, (c, _) in _DT.items() if c == code)
+        self._suf = _DT[self.dtype][1]
+        self.dist_name = _METRICS[metric]
+        self.max_nb_connection, self.ef_construction = M, efc
         return self
 
     # ---- statistics / graph transfer (extensions)

@@ -56,6 +56,10 @@ extern "C" {
     fn hnsw_b200_replica_count(h: *const HnswApif32) -> c_int;
     // partitioned index (include/hnsw_b200.h "Partitioned index"): the points split over several devices
     fn hnsw_b200_partition(h: *mut HnswApif32, nparts: c_int, devices: *const c_int) -> c_int;
+    // saved indexes (include/hnsw_b200.h "Saved indexes"): dir and basename are NUL-terminated
+    fn hnsw_b200_save(h: *const HnswApif32, dir: *const u8, basename: *const u8, overwrite: c_int, used_basename: *mut u8,
+                      used_cap: usize) -> c_int;
+    fn hnsw_b200_restore(dir: *const u8, basename: *const u8, ndev: c_int, devices: *const c_int) -> *mut c_void;
     fn hnsw_b200_partition_count(h: *const HnswApif32) -> c_int;
     // resident filters (include/hnsw_b200.h "Resident filters"): a FilterT materialised once, passed by id
     fn hnsw_b200_filter_new(h: *const HnswApif32, filter_mode: c_int, filter_ids: *const u64, nfilter: u64,
@@ -222,6 +226,26 @@ impl<D: DistName> Hnsw<D> {
         if r == 0 { Ok(()) } else { Err(r) }
     }
     pub fn partition_count(&self) -> usize { unsafe { hnsw_b200_partition_count(self.h) as usize } }
+    /// Extension: save the index with its insertion ranks, labels, attributes, deleted points, settings and level RNG
+    /// (<basename>.hnsw.graph / .hnsw.data, one pair <basename>-p<i> per partition, and the manifest
+    /// <basename>.hnsw.b200 under `dir`).  Returns the basename used: a unique one when `overwrite` is false and a file
+    /// of the set exists.
+    pub fn save(&self, dir: &str, basename: &str, overwrite: bool) -> Result<String, i32> {
+        let (d, b) = (format!("{}\0", dir), format!("{}\0", basename));
+        let mut used = vec![0u8; 4096];
+        let r = unsafe { hnsw_b200_save(self.h, d.as_ptr(), b.as_ptr(), overwrite as c_int, used.as_mut_ptr(), used.len()) };
+        if r != 0 { return Err(r); }
+        let len = used.iter().position(|&c| c == 0).unwrap_or(used.len());
+        Ok(String::from_utf8_lossy(&used[..len]).into_owned())
+    }
+    /// Extension: the index `save` wrote, the same ranks, columns and settings; `devices`: empty for the current device,
+    /// or one device per saved partition.  None when the files are refused.  This shim serves f32 only: the saved index
+    /// must hold f32 vectors under the distance D.
+    pub fn restore(dir: &str, basename: &str, devices: &[i32]) -> Option<Self> {
+        let (d, b) = (format!("{}\0", dir), format!("{}\0", basename));
+        let h = unsafe { hnsw_b200_restore(d.as_ptr(), b.as_ptr(), devices.len() as c_int, devices.as_ptr()) };
+        if h.is_null() { None } else { Some(Hnsw { h: h as *mut HnswApif32, _d: PhantomData }) }
+    }
 
     /// hnsw.rs:1069-1071
     pub fn insert(&self, datav_with_id: (&[f32], usize)) {

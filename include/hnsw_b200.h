@@ -420,8 +420,8 @@ int hnsw_b200_search_exact_per_query(const void* h, const int64_t* filters, cons
  * labels, and no insert makes it stale, where a resident filter per tenant costs n/8 bytes per tenant and goes stale at
  * the next insert.
  *   Labels: every point starts with HNSW_B200_LABEL_NONE (new inserts, imports, reloaded dumps and replication blobs);
- *     no label admits such a point.  Labels are not written into the dump files: hnsw_b200_get_labels reads them back
- *     so that the caller can store them.
+ *     no label admits such a point.  Labels are not written into the dump files; hnsw_b200_save keeps them with the
+ *     index (see "Saved indexes").
  *   set_labels sets the labels of the points with insertion ranks [first, first + n) (a partitioned handle: global
  *     ranks, point g is local point g / P of partition g % P).  first + n > nb_point is refused and nothing changes;
  *     HNSW_B200_LABEL_NONE clears a label.  It takes the handle exclusively, as an insert does; a partition view refuses
@@ -477,7 +477,7 @@ int hnsw_b200_search_exact_label_sets(const void* h, const uint64_t* qset_off, c
  * of ids on the device and 8 + 8 bytes per point of sorted values on the host (by value, and by label and value, each
  * over the points with an attribute, the second only over those that also have a label).
  *   Attributes: every point starts with HNSW_B200_ATTR_NONE (new inserts, imports, reloaded dumps and replication
- *     blobs).  They are not written into the dump files (get_attributes reads them back) and nccl_broadcast_index does
+ *     blobs).  They are not written into the dump files (hnsw_b200_save keeps them) and nccl_broadcast_index does
  *     not broadcast them.  set_attributes / get_attributes address insertion ranks [first, first + n) exactly as
  *     set_labels / get_labels do, with the same range check, locks and partition placement; HNSW_B200_ATTR_NONE clears
  *     an attribute.  No attribute call reads or changes labels or resident filters, and no label or filter call reads or
@@ -608,7 +608,7 @@ int hnsw_b200_search_exact_excluding(const void* h, const uint64_t* qx_off, cons
  *     deleted points.
  *   With D empty (also after every deleted point was restored) every call runs the kernel and returns the rows it does
  *     without deletions.  Store-level calls (bruteforce, dist_batch, export_*, flatten, flat_neighbours), get_nb_point
- *     and file_dump still see every stored point; a reloaded dump has no deleted point (get_deleted saves the set).
+ *     and file_dump still see every stored point; a reloaded dump has no deleted point (hnsw_b200_save keeps the set).
  *   Handles: a partitioned handle splits the ranks by placement; a partition view searches with its partition's set and
  *     refuses delete and restore; a replica gets the set at its first sharded search after it changed;
  *     hnsw_b200_nccl_broadcast_index does not send it.
@@ -680,6 +680,36 @@ int hnsw_b200_file_dump(const void* h, const char* dir, const char* basename, in
                         size_t used_cap);
 void* hnsw_b200_load_dump(HnswIo* io, int dtype, size_t namelen, const uint8_t* cdistname);
 void hnsw_b200_free_description(const DescriptionFFI* d);
+
+/* ---- Saved indexes: save a handle and restore the same index, with its insertion ranks, origin ids, labels,
+ * attributes, deleted points, settings and level RNG, so that every rank a caller holds stays valid.  A plain
+ * file_dump / load keeps the graph only, and renumbers the points by level (rank r after a load is the r-th point of the
+ * file, which lists level 0 first): columns stored by rank must then be remapped through the origin ids.
+ *   Files, under dir: <basename>.hnsw.graph / .hnsw.data, byte for byte what file_dump writes for the handle; on a
+ *     partitioned handle one such pair per partition holding points, <basename>-p<i>.hnsw.graph / .hnsw.data, what
+ *     partition_view(i)'s file_dump writes; and the manifest <basename>.hnsw.b200, written last (DESIGN.md "Saved
+ *     indexes": the element type, metric, dimension, M, max_layer, ef_construction, max_elements, every setting but
+ *     statistics, the level RNG state, each partition's count and the insertion rank of each of its points in file order,
+ *     the size and a 64-bit checksum of every pair file, and the label, attribute and deleted columns when some point has
+ *     one).  Every pair loads with hnsw_b200_load_dump as a dump does.
+ *   save: overwrite = 0 keeps every existing file of the set and picks one unique "<basename>-<n>" for all of them, as
+ *     file_dump does; the basename used is written to used_basename (used_cap bytes, may be NULL).  An earlier manifest
+ *     of the same name is removed first, and a failed save removes the files it wrote.  The handle is taken shared; a
+ *     replicated handle saves its own index.  Refused before anything is written: a partition view, an empty handle, a
+ *     partitioned handle whose earlier insert failed, an index unusable after a CUDA failure.
+ *   restore: a new handle of the saved element type and metric, with the saved ranks, columns and settings; it serves
+ *     the reference entry points of its type and every extension, like hnsw_b200_load_dump's.  Searches on it return
+ *     what the saved handle returned, bit for bit (ids, distances, internal ids, PointIds, counters), and inserts continue
+ *     as the saved handle's would have.  An unpartitioned save takes ndev = 0 (the current device) or 1 (devices[0]); a
+ *     partitioned one ndev = P devices, which may repeat and need not be the saving run's, and reads the partitions in
+ *     parallel.  Refused, returning NULL with hnsw_b200_last_error naming the file, and leaving nothing allocated: a
+ *     missing or malformed manifest (magic, version, checksum, a rank list that is not a permutation), a pair file whose
+ *     size or checksum differs from the manifest's, a wrong ndev.
+ *   Not saved: resident filters (make them again: the same FilterT gives the same bitmap), replicas (replicate again),
+ *     NCCL state, and the exact-scan orders (rebuilt at first use). */
+int hnsw_b200_save(const void* h, const char* dir, const char* basename, int overwrite, char* used_basename,
+                   size_t used_cap);
+void* hnsw_b200_restore(const char* dir, const char* basename, int ndev, const int* devices);
 
 /* Traversal statistics of all searches since the last reset (device counters):
  * out[0] distance evaluations, out[1] expansions, out[2] adjacency ids read, out[3] queries.
