@@ -44,6 +44,14 @@ static int pass(Index* ix, int r) {
   if (r) g_err = ix->err();
   return r;
 }
+// Refuses the first of v[0, n) that is not below have = nb_point, naming it `what`[i]
+static int not_below(const std::string& what, const uint64_t* v, uint64_t n, uint64_t have) {
+  for (uint64_t i = 0; i < n; ++i)
+    if (v[i] >= have)
+      return set_err(what + "[" + std::to_string(i) + "] = " + std::to_string(v[i]) + " is not below nb_point = " +
+                     std::to_string(have));
+  return 0;
+}
 
 // The locks of one call on handle h, held for the guard's scope: the handle's `mu`, then on a partitioned handle every
 // partition's in partition order, all shared (searches, read-only queries) or all exclusive (anything that may change
@@ -639,58 +647,157 @@ int hnsw_b200_insert_flat(void* h, const void* vecs, uint64_t n, uint64_t dim, c
   return pass(ix, ix->insert(vecs, n, dim, nullptr, ids, levels, (int)dim));
 }
 
-// ---- searches.  Every search entry point below is one call of search_call, which holds the handle shared (Locked),
-// checks the arguments and runs the batch b:
+// ---- searches.  Every search entry point below is one Request, which search() checks and runs on the handle held
+// shared (Locked):
 //   * HOST: host rows in, host answers out, through the host batch driver; a partitioned handle searches every partition;
 //   * SUBMIT: the same, split in two (hnsw_b200_search_flat_wait collects it), so that one host thread keeps several
 //     batches in flight.  With replicas (hnsw_b200_replicate) every device gets its contiguous share enqueued at submit
 //     time.  Refused on a partitioned handle;
 //   * DEVICE: device rows in, device answers out (b.out.nb, b.out.counts), `sync` and `kernel_ms` as
 //     hnsw_b200_search_device takes them (the other two ignore them).  Refused on a partitioned handle.
-// `name` is the entry point a refusal on a partitioned handle names.  By stored point (b.in.qids, non-NULL) the queries
-// are the stored vectors of qids[0, nq), each below nb_point, in the handle's dimension; radii (b.in.radius, an exact
-// HOST call) are checked by the caller.
+// By stored point (b.in.qids) the queries are the stored vectors of qids[0, nq), each below nb_point, in the handle's
+// dimension.
+namespace {
 enum Via { HOST, SUBMIT, DEVICE };
-static int64_t search_call(const void* h, Via via, const char* name, HostBatch b, int sync, float* kernel_ms) {
-  Locked ix(h, SHARED);
-  if (!ix) return -1;
-  if (via != HOST) HB_NOT_PARTITIONED(ix, name);
-  if (via == DEVICE) return pass(ix, ix->search_device(b, sync != 0, kernel_ms));
-  if (via == HOST && b.nq == 0) return 0;
-  if (const uint64_t* qids = b.in.qids) {
-    const uint64_t have = ix->nb_point();
-    for (uint64_t i = 0; i < b.nq; ++i)
-      if (qids[i] >= have)
-        return set_err(std::string(name) + ": qids[" + std::to_string(i) + "] = " + std::to_string(qids[i]) +
-                       " is not below nb_point = " + std::to_string(have));
-    b.d = ix->dim;
+
+static Restriction label_sets(const uint64_t* off, const uint32_t* set, const int64_t* range) {
+  return {.kind = Restriction::ROW_LABEL_SETS, .qset_off = off, .qset = set, .qrange = range};
+}
+
+// Label sets of one label per query, for the calls that give no offsets: query i's set is {labels[i]}, or {LABEL_NONE}
+// (any label) when labels is NULL; the offsets 0, 1, ..., nq, and the nq LABEL_NONE values, are kept here
+struct OneLabelSets {
+  std::vector<uint64_t> off;
+  std::vector<uint32_t> none;
+  Restriction rows(uint64_t nq, const uint32_t* labels, const int64_t* qrange) {
+    off.resize(nq + 1);
+    std::iota(off.begin(), off.end(), (uint64_t)0);
+    if (!labels) none.assign(nq, hb::LABEL_NONE);
+    return label_sets(off.data(), labels ? labels : none.data(), qrange);
   }
-  const Restriction& rs = b.restriction;
+};
+
+// How a call reads its restriction.  FIXED: b.restriction as the entry point made it.  LABELS: a label per query,
+// query i's set {qlabels[i]}.  ROWS: a resident filter (`filter`; -1: none) or label sets (qset_off, qset) and ranges
+// (qrange) per query, but not both; a range without sets is a range within {LABEL_NONE}.
+enum Takes { FIXED, LABELS, ROWS };
+// The arguments a call refuses as NULL when nq > 0: b.in.qids, qlabels, qrange, b.excluded (else only one of its two
+// arrays NULL is refused), b.in.radius
+enum Need { QIDS = 1, QLABELS = 2, QRANGE = 4, QX = 8, RADIUS = 16 };
+
+// One search call as its entry point received it: the entry point's name (as refusals name it), how it runs, its batch
+// (with the excluded lists and the radii as passed), and its restriction's arguments as passed.  `early`: nq == 0
+// returns 0 before the handle is locked; otherwise a HOST call returns 0 under the lock, and SUBMIT and DEVICE go on.
+struct Request {
+  const char* name;
+  Via via = HOST;
+  HostBatch b;
+  Takes takes = FIXED;
+  int need = 0;
+  bool early = false;
+  int64_t filter = -1;
+  const uint32_t* qlabels = nullptr;
+  const int64_t* qrange = nullptr;
+  const uint64_t* qset_off = nullptr;
+  const uint32_t* qset = nullptr;
+  int sync = 1;
+  float* kernel_ms = nullptr;
+  OneLabelSets one{};          // the offsets of LABELS, and of ranges without sets
+  std::vector<float> radii{};  // b.in.radius as run: -0 read as 0, whose key is the smallest
+};
+
+// The checks of q that need no lock, in the header's order, and the restriction they leave in q.b.restriction: a NULL
+// handle, nq == 0 (early: 1, nothing to run), the NULL arguments, the radii (NaN or negative: refused), and a resident
+// filter together with sets or ranges.  -1: refused, 0: go on.
+static int prepare(const void* h, Request& q) {
+  HostBatch& b = q.b;
+  auto refuse = [&](const std::string& what) { return set_err(std::string(q.name) + ": " + what); };
+  if (!h) return set_err("NULL handle");
+  if (b.nq == 0 && q.early) return 1;
+  if (b.nq) {
+    if ((q.need & QIDS) && !b.in.qids) return refuse("qids is NULL");
+    if ((q.need & QLABELS) && !q.qlabels) return set_err("qlabels is NULL");
+    if ((q.need & QRANGE) && !q.qrange) return set_err("qrange is NULL");
+    if (((q.need & QX) || b.excluded.ids) && !b.excluded.off) return refuse("qx_off is NULL");
+    if (((q.need & QX) || b.excluded.off) && !b.excluded.ids) return refuse("qx is NULL");
+    if (q.need & RADIUS) {
+      if (!b.in.radius) return refuse("radius is NULL");
+      q.radii.resize(b.nq);
+      for (uint64_t i = 0; i < b.nq; ++i) {
+        const float r = b.in.radius[i];
+        if (std::isnan(r) || r < 0)
+          return refuse("radius[" + std::to_string(i) + "] = " + std::to_string(r) + " is " + (std::isnan(r) ? "NaN" : "negative"));
+        q.radii[i] = r == 0 ? 0.0f : r;
+      }
+      b.in.radius = q.radii.data();
+    }
+  }
+  if (q.takes == LABELS) b.restriction = q.one.rows(b.nq, q.qlabels, nullptr);
+  if (q.takes == ROWS) {
+    if (q.filter != -1 && (q.qrange || q.qset_off || q.qset))
+      return refuse("a resident filter cannot be combined with label sets or ranges");
+    if (q.qset_off || q.qset) b.restriction = label_sets(q.qset_off, q.qset, q.qrange);
+    else if (q.qrange) b.restriction = q.one.rows(b.nq, nullptr, q.qrange);
+    else if (q.filter != -1) b.restriction = {.kind = Restriction::RESIDENT, .resident = q.filter};
+  }
+  return 0;
+}
+
+// A per-row restriction without its arrays is refused
+static int missing_rows(const Restriction& rs) {
   if (rs.kind == Restriction::ROW_FILTERS && !rs.filters) return set_err("filters is NULL");
   if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset_off) return set_err("qset_off is NULL");
   if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset) return set_err("qset is NULL");
+  return 0;
+}
+
+// q checked and run: prepare's checks, then under the lock a partitioned handle (SUBMIT, DEVICE), nq == 0 (HOST: 0),
+// qids below nb_point, the restriction's and the answers' arrays.  A radius call with knbn == 0 counts only: the scan
+// runs at k = 1 into scratch rows, the caller's row arrays may be NULL, and every count is 0.  SUBMIT returns the ticket.
+static int64_t search(const void* h, Request q) {
+  if (const int s = prepare(h, q)) return s < 0 ? -1 : 0;
+  HostBatch& b = q.b;
+  Locked ix(h, SHARED);
+  if (!ix) return -1;
+  if (q.via != HOST) HB_NOT_PARTITIONED(ix, q.name);
+  if (q.via == DEVICE) return pass(ix, ix->search_device(b, q.sync != 0, q.kernel_ms));
+  if (q.via == HOST && b.nq == 0) return 0;
+  if (b.in.qids) {
+    if (not_below(std::string(q.name) + ": qids", b.in.qids, b.nq, ix->nb_point())) return -1;
+    b.d = ix->dim;
+  }
+  if (missing_rows(b.restriction)) return -1;
+  const bool count_only = b.in.radius && b.k == 0;
+  std::vector<uint64_t> scratch_ids(count_only ? b.nq : 0);
+  std::vector<float> scratch_dist(count_only ? b.nq : 0);
+  if (count_only) {
+    b.k = 1;
+    b.out.ids = scratch_ids.data();
+    b.out.dist = scratch_dist.data();
+    b.out.internal = nullptr;
+    b.out.pid = nullptr;
+  }
   if (!(b.in.queries || b.in.qids) || !b.out.ids || !b.out.dist || !b.out.counts || b.k == 0 || b.nq == 0)
     return set_err("bad argument");
-  if (via == HOST) return pass(ix, ix->search_batch(b));
-  const int64_t t = ix->submit_batch(b);
-  if (t < 0) g_err = ix->err();
-  return t;
+  if (q.via == SUBMIT) {
+    const int64_t t = ix->submit_batch(b);
+    if (t < 0) g_err = ix->err();
+    return t;
+  }
+  const int rc = pass(ix, ix->search_batch(b));
+  if (rc == 0 && count_only) std::fill(b.out.counts, b.out.counts + b.nq, 0);
+  return rc;
 }
 static AnswerArrays columns(uint64_t* ids, float* dist, uint32_t* internal, int32_t* pid, int32_t* counts) {
-  return AnswerArrays{nullptr, ids, dist, internal, pid, counts};
+  return {.ids = ids, .dist = dist, .internal = internal, .pid = pid, .counts = counts};
 }
 static AnswerArrays on_device(void* d_out, int32_t* d_counts) {
-  return AnswerArrays{(NeighbourOut*)d_out, nullptr, nullptr, nullptr, nullptr, d_counts};
+  return {.nb = (NeighbourOut*)d_out, .counts = d_counts};
 }
-static Restriction filter_t(int mode, const uint64_t* ids, uint64_t nids, hnsw_b200_filter_fn fn, void* ctx) {
-  return mode ? Restriction{Restriction::FILTER_T, mode, ids, nids, fn, ctx} : Restriction();
+static hb::HostRows by_id(const uint64_t* qids, int exclude_self) {
+  return {.qids = qids, .skip = exclude_self ? qids : nullptr};
 }
-static Restriction resident(int64_t f) { return {Restriction::RESIDENT, 0, nullptr, 0, nullptr, nullptr, f}; }
-static Restriction resident_or_all(int64_t f) { return f == -1 ? Restriction() : resident(f); }  // -1: every point
-static Restriction row_filters(const int64_t* f) { return {Restriction::ROW_FILTERS, 0, nullptr, 0, nullptr, nullptr, -1, f}; }
-static Restriction row_label_sets(const uint64_t* off, const uint32_t* set, const int64_t* range = nullptr) {
-  return {Restriction::ROW_LABEL_SETS, 0, nullptr, 0, nullptr, nullptr, -1, nullptr, off, set, range};
-}
+}  // namespace
 
 // hnsw_b200_search_flat and _search_flat_filtered: the filter is the FilterT arguments (filter_mode 1, 2) or one of the
 // handle's resident filters.  The kernels and the answers are the same.
@@ -698,28 +805,31 @@ int hnsw_b200_search_flat(const void* h, const void* queries, uint64_t nq, uint6
                           uint64_t ef_search, int filter_mode, const uint64_t* filter_ids, uint64_t nfilter,
                           hnsw_b200_filter_fn fn, void* ctx, uint64_t* out_ids, float* out_dist,
                           uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_flat",
-                          {{queries}, nq, (int)dim, knbn, ef_search, filter_t(filter_mode, filter_ids, nfilter, fn, ctx),
-                           false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
+  const Restriction filter = filter_mode ? Restriction{.kind = Restriction::FILTER_T, .mode = filter_mode, .ids = filter_ids,
+                                                       .nids = nfilter, .fn = fn, .ctx = ctx} : Restriction();
+  return (int)search(h, {.name = "search_flat", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn, .ef = ef_search,
+                         .restriction = filter, .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)}});
 }
 int hnsw_b200_search_flat_filtered(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim,
                                    uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                    uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_flat_filtered", {{queries}, nq, (int)dim, knbn, ef_search, resident(filter),
-                          false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
+  return (int)search(h, {.name = "search_flat_filtered", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .ef = ef_search, .restriction = {.kind = Restriction::RESIDENT, .resident = filter},
+                         .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)}});
 }
 
 int64_t hnsw_b200_search_flat_submit(const void* h, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
                                      uint64_t ef_search, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                      int32_t* out_pid, int32_t* out_counts) {
-  return search_call(h, SUBMIT, "search_flat_submit", {{queries}, nq, (int)dim, knbn, ef_search, Restriction(), false,
-                     columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
+  return search(h, {.name = "search_flat_submit", .via = SUBMIT, .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                    .ef = ef_search, .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)}});
 }
 int64_t hnsw_b200_search_flat_submit_filtered(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim,
                                               uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                               uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return search_call(h, SUBMIT, "search_flat_submit_filtered", {{queries}, nq, (int)dim, knbn, ef_search,
-                     resident(filter), false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
+  return search(h, {.name = "search_flat_submit_filtered", .via = SUBMIT, .b = {.in = {queries}, .nq = nq, .d = (int)dim,
+                    .k = knbn, .ef = ef_search, .restriction = {.kind = Restriction::RESIDENT, .resident = filter},
+                    .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)}});
 }
 
 int hnsw_b200_search_flat_wait(const void* h, int64_t ticket) {
@@ -735,21 +845,23 @@ int hnsw_b200_search_flat_wait(const void* h, int64_t ticket) {
 
 int hnsw_b200_search_device(const void* h, const void* d_queries, uint64_t nq, uint64_t knbn,
                             uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
-  return (int)search_call(h, DEVICE, "search_device", {{d_queries}, nq, 0, knbn, ef_search, Restriction(), false,
-                          on_device(d_out, d_counts)}, sync, kernel_ms);
+  return (int)search(h, {.name = "search_device", .via = DEVICE, .b = {.in = {d_queries}, .nq = nq, .k = knbn,
+                         .ef = ef_search, .out = on_device(d_out, d_counts)}, .sync = sync, .kernel_ms = kernel_ms});
 }
 int hnsw_b200_search_device_filtered(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                      uint64_t ef_search, void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
-  return (int)search_call(h, DEVICE, "search_device_filtered", {{d_queries}, nq, 0, knbn, ef_search, resident(filter),
-                          false, on_device(d_out, d_counts)}, sync, kernel_ms);
+  return (int)search(h, {.name = "search_device_filtered", .via = DEVICE, .b = {.in = {d_queries}, .nq = nq, .k = knbn,
+                         .ef = ef_search, .restriction = {.kind = Restriction::RESIDENT, .resident = filter},
+                         .out = on_device(d_out, d_counts)}, .sync = sync, .kernel_ms = kernel_ms});
 }
 
 // Exact search: the exact scan of the points a resident filter admits (filter >= 0) or of every point (-1), through the
 // same batch driver and device-resident path as the graph searches
 int hnsw_b200_search_exact(const void* h, int64_t filter, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn,
                            uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_exact", {{queries}, nq, (int)dim, knbn, 0, resident_or_all(filter), true,
-                          columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
+  return (int)search(h, {.name = "search_exact", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn, .exact = true,
+                         .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, .takes = ROWS,
+                         .filter = filter});
 }
 
 // A filter per query: filters[i] is a resident filter of the handle or -1; the graph search (ef_search) or the exact
@@ -757,15 +869,16 @@ int hnsw_b200_search_exact(const void* h, int64_t filter, const void* queries, u
 int hnsw_b200_search_flat_per_query(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim,
                                     uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                     uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_flat_per_query", {{queries}, nq, (int)dim, knbn, ef_search,
-                          row_filters(filters), false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1,
-                          nullptr);
+  return (int)search(h, {.name = "search_flat_per_query", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .ef = ef_search, .restriction = {.kind = Restriction::ROW_FILTERS, .filters = filters},
+                         .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)}});
 }
 int hnsw_b200_search_exact_per_query(const void* h, const int64_t* filters, const void* queries, uint64_t nq, uint64_t dim,
                                      uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                      int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_exact_per_query", {{queries}, nq, (int)dim, knbn, 0, row_filters(filters),
-                          true, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, 1, nullptr);
+  return (int)search(h, {.name = "search_exact_per_query", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .restriction = {.kind = Restriction::ROW_FILTERS, .filters = filters}, .exact = true,
+                         .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)}});
 }
 
 // Point labels (and attributes), addressed by insertion rank; on a partitioned handle each partition holds its share of
@@ -838,11 +951,7 @@ static int mark_deleted(void* h, const uint64_t* ranks, uint64_t n, bool on) {
   Locked ix(h, EXCLUSIVE);
   if (!ix) return -1;
   if (n && !ranks) return set_err("ranks is NULL");
-  const uint64_t have = ix->nb_point();
-  for (uint64_t i = 0; i < n; ++i)
-    if (ranks[i] >= have)
-      return set_err("ranks[" + std::to_string(i) + "] = " + std::to_string(ranks[i]) + " is not below nb_point = " +
-                     std::to_string(have));
+  if (not_below("ranks", ranks, n, ix->nb_point())) return -1;
   HB_NOT_VIEW(ix);
   if (n == 0) return 0;
   hb::DeviceRestore keep;
@@ -873,52 +982,21 @@ int64_t hnsw_b200_get_nb_deleted(const void* h) {
   return total;
 }
 
-// Label sets of one label per query, for the calls that give no offsets: query i's set is {labels[i]}, or {LABEL_NONE}
-// (any label) when labels is NULL; the offsets 0, 1, ..., nq, and the nq LABEL_NONE values, are kept here
-struct OneLabelSets {
-  std::vector<uint64_t> off;
-  std::vector<uint32_t> none;
-  Restriction rows(uint64_t nq, const uint32_t* labels, const int64_t* qrange) {
-    off.resize(nq + 1);
-    std::iota(off.begin(), off.end(), (uint64_t)0);
-    if (!labels) none.assign(nq, hb::LABEL_NONE);
-    return row_label_sets(off.data(), labels ? labels : none.data(), qrange);
-  }
-};
-
-// The restriction of a call that takes sets and ranges (-1 and no sets or ranges: none), refused when a resident filter
-// comes with sets or ranges; a range without sets is a range within {LABEL_NONE} per query (made in `one`), and sets
-// without ranges are the label-sets call's
-static int one_restriction(const char* name, uint64_t nq, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
-                           const uint32_t* qset, OneLabelSets& one, Restriction& rs) {
-  const bool rows = qrange || qset_off || qset;
-  if (filter != -1 && rows)
-    return set_err(std::string(name) + ": a resident filter cannot be combined with label sets or ranges");
-  rs = !rows ? resident_or_all(filter)
-             : qset_off || qset ? row_label_sets(qset_off, qset, qrange) : one.rows(nq, nullptr, qrange);
-  return 0;
-}
-
 // A label per query: labels[i] is the label query i is restricted to, or LABEL_NONE for none; the graph search
 // (ef_search) or the exact scan.  Query i's label set is {qlabels[i]}.
-static int labeled_call(const void* h, const char* name, const uint32_t* qlabels, bool exact, const void* queries,
-                        uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef, const AnswerArrays& out) {
-  if (h && nq && !qlabels) return set_err("qlabels is NULL");  // search_call answers a NULL handle and nq == 0 first
-  OneLabelSets one;
-  return (int)search_call(h, HOST, name, {{queries}, nq, (int)dim, knbn, ef, one.rows(nq, qlabels, nullptr), exact, out}, 1,
-                          nullptr);
-}
 int hnsw_b200_search_flat_labeled(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim,
                                   uint64_t knbn, uint64_t ef_search, uint64_t* out_ids, float* out_dist,
                                   uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return labeled_call(h, "search_flat_labeled", qlabels, false, queries, nq, dim, knbn, ef_search,
-                      columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return (int)search(h, {.name = "search_flat_labeled", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .ef = ef_search, .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)},
+                         .takes = LABELS, .need = QLABELS, .qlabels = qlabels});
 }
 int hnsw_b200_search_exact_labeled(const void* h, const uint32_t* qlabels, const void* queries, uint64_t nq, uint64_t dim,
                                    uint64_t knbn, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                    int32_t* out_pid, int32_t* out_counts) {
-  return labeled_call(h, "search_exact_labeled", qlabels, true, queries, nq, dim, knbn, 0,
-                      columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return (int)search(h, {.name = "search_exact_labeled", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .exact = true, .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)},
+                         .takes = LABELS, .need = QLABELS, .qlabels = qlabels});
 }
 
 // A label set per query: query i is restricted to the points whose label is one of qset[qset_off[i], qset_off[i + 1])
@@ -926,224 +1004,153 @@ int hnsw_b200_search_exact_labeled(const void* h, const uint32_t* qlabels, const
 int hnsw_b200_search_flat_label_sets(const void* h, const uint64_t* qset_off, const uint32_t* qset, const void* queries,
                                      uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search, uint64_t* out_ids,
                                      float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_flat_label_sets", {{queries}, nq, (int)dim, knbn, ef_search,
-                          row_label_sets(qset_off, qset), false, columns(out_ids, out_dist, out_internal, out_pid,
-                          out_counts)}, 1, nullptr);
+  return (int)search(h, {.name = "search_flat_label_sets", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .ef = ef_search, .restriction = label_sets(qset_off, qset, nullptr),
+                         .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)}});
 }
 int hnsw_b200_search_exact_label_sets(const void* h, const uint64_t* qset_off, const uint32_t* qset, const void* queries,
                                       uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids, float* out_dist,
                                       uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return (int)search_call(h, HOST, "search_exact_label_sets", {{queries}, nq, (int)dim, knbn, 0,
-                          row_label_sets(qset_off, qset), true, columns(out_ids, out_dist, out_internal, out_pid,
-                          out_counts)}, 1, nullptr);
+  return (int)search(h, {.name = "search_exact_label_sets", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .restriction = label_sets(qset_off, qset, nullptr), .exact = true,
+                         .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)}});
 }
 
 // Attribute ranges.  Query i is restricted to the points whose attribute is in [qrange[2i], qrange[2i + 1]]
 // ([INT64_MIN, INT64_MAX]: every point, also those without one) and whose label is one of qset[qset_off[i],
 // qset_off[i + 1]) ({LABEL_NONE}: any; qset_off and qset both NULL: {LABEL_NONE} for every query); the graph search
 // (ef_search) or the exact scan.
-static int ranged_call(const void* h, const char* name, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
-                       bool exact, const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef,
-                       const AnswerArrays& out) {
-  if (h && nq && !qrange) return set_err("qrange is NULL");  // search_call answers a NULL handle and nq == 0 first
-  OneLabelSets one;
-  Restriction rs;
-  one_restriction(name, nq, -1, qrange, qset_off, qset, one, rs);  // no resident filter: never refused
-  return (int)search_call(h, HOST, name, {{queries}, nq, (int)dim, knbn, ef, rs, exact, out}, 1, nullptr);
-}
 int hnsw_b200_search_flat_ranges(const void* h, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
                                  const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
                                  uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
                                  int32_t* out_counts) {
-  return ranged_call(h, "search_flat_ranges", qrange, qset_off, qset, false, queries, nq, dim, knbn, ef_search,
-                     columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return (int)search(h, {.name = "search_flat_ranges", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .ef = ef_search, .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)},
+                         .takes = ROWS, .need = QRANGE, .qrange = qrange, .qset_off = qset_off, .qset = qset});
 }
 int hnsw_b200_search_exact_ranges(const void* h, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
                                   const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids,
                                   float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return ranged_call(h, "search_exact_ranges", qrange, qset_off, qset, true, queries, nq, dim, knbn, 0,
-                     columns(out_ids, out_dist, out_internal, out_pid, out_counts));
+  return (int)search(h, {.name = "search_exact_ranges", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .exact = true, .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)},
+                         .takes = ROWS, .need = QRANGE, .qrange = qrange, .qset_off = qset_off, .qset = qset});
 }
 
 int hnsw_b200_search_exact_device(const void* h, int64_t filter, const void* d_queries, uint64_t nq, uint64_t knbn,
                                   void* d_out, int32_t* d_counts, int sync, float* kernel_ms) {
-  return (int)search_call(h, DEVICE, "search_exact_device", {{d_queries}, nq, 0, knbn, 0, resident_or_all(filter), true,
-                          on_device(d_out, d_counts)}, sync, kernel_ms);
+  return (int)search(h, {.name = "search_exact_device", .via = DEVICE, .b = {.in = {d_queries}, .nq = nq, .k = knbn,
+                         .exact = true, .out = on_device(d_out, d_counts)}, .takes = ROWS, .filter = filter,
+                         .sync = sync, .kernel_ms = kernel_ms});
 }
 
-// The checks a by-id or radius call starts with, in the header's order, before its restriction's: the NULL handle, then
-// nq == 0 (1: nothing to run), qids (by stored point), and a radius call's radii (r: as run, -0 read as 0, whose key is
-// the smallest; NULL: not a radius call).  -1: refused, 0: go on.
-static int first_checks(const void* h, const char* name, uint64_t nq, bool by_id, const uint64_t* qids,
-                        const float* radius, std::vector<float>* r) {
-  if (!h) return set_err("NULL handle");
-  if (nq == 0) return 1;
-  if (by_id && !qids) return set_err(std::string(name) + ": qids is NULL");
-  if (!r) return 0;
-  if (!radius) return set_err(std::string(name) + ": radius is NULL");
-  r->resize(nq);
-  for (uint64_t i = 0; i < nq; ++i) {
-    if (std::isnan(radius[i]) || radius[i] < 0)
-      return set_err(std::string(name) + ": radius[" + std::to_string(i) + "] = " + std::to_string(radius[i]) + " is " +
-                     (std::isnan(radius[i]) ? "NaN" : "negative"));
-    (*r)[i] = radius[i] == 0 ? 0.0f : radius[i];
-  }
-  return 0;
-}
-
-// Search by stored point (b.in.qids, and b.in.skip for exclude_self), under one_restriction's restriction
-static int by_id_call(const void* h, Via via, const char* name, HostBatch b, int64_t filter, const int64_t* qrange,
-                      const uint64_t* qset_off, const uint32_t* qset, int sync, float* kernel_ms) {
-  OneLabelSets one;
-  if (int s = first_checks(h, name, b.nq, true, b.in.qids, nullptr, nullptr)) return s < 0 ? -1 : 0;
-  if (one_restriction(name, b.nq, filter, qrange, qset_off, qset, one, b.restriction)) return -1;
-  return (int)search_call(h, via, name, b, sync, kernel_ms);
-}
+// Search by stored point (b.in.qids, and b.in.skip for exclude_self), under a ROWS restriction
 int hnsw_b200_search_flat_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, uint64_t ef_search,
                                 int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
                                 const uint32_t* qset, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                 int32_t* out_pid, int32_t* out_counts) {
-  return by_id_call(h, HOST, "search_flat_by_id", {{nullptr, nullptr, qids, exclude_self ? qids : nullptr}, nq, 0, knbn,
-                    ef_search, Restriction(), false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)},
-                    filter, qrange, qset_off, qset, 1, nullptr);
+  return (int)search(h, {.name = "search_flat_by_id", .b = {.in = by_id(qids, exclude_self), .nq = nq, .k = knbn,
+                         .ef = ef_search, .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)},
+                         .takes = ROWS, .need = QIDS, .early = true, .filter = filter, .qrange = qrange,
+                         .qset_off = qset_off, .qset = qset});
 }
 int hnsw_b200_search_exact_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, int exclude_self,
                                  int64_t filter, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
                                  uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
                                  int32_t* out_counts) {
-  return by_id_call(h, HOST, "search_exact_by_id", {{nullptr, nullptr, qids, exclude_self ? qids : nullptr}, nq, 0, knbn,
-                    0, Restriction(), true, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, filter,
-                    qrange, qset_off, qset, 1, nullptr);
+  return (int)search(h, {.name = "search_exact_by_id", .b = {.in = by_id(qids, exclude_self), .nq = nq, .k = knbn,
+                         .exact = true, .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts)},
+                         .takes = ROWS, .need = QIDS, .early = true, .filter = filter, .qrange = qrange,
+                         .qset_off = qset_off, .qset = qset});
 }
 int hnsw_b200_search_device_by_id(const void* h, int exact, int64_t filter, const uint64_t* d_qids, uint64_t nq,
                                   uint64_t knbn, uint64_t ef_search, int exclude_self, void* d_out, int32_t* d_counts,
                                   int sync, float* kernel_ms) {
-  return by_id_call(h, DEVICE, "search_device_by_id", {{nullptr, nullptr, d_qids, exclude_self ? d_qids : nullptr}, nq, 0,
-                    knbn, exact ? 0 : ef_search, Restriction(), exact != 0, on_device(d_out, d_counts)}, filter, nullptr,
-                    nullptr, nullptr, sync, kernel_ms);
+  return (int)search(h, {.name = "search_device_by_id", .via = DEVICE, .b = {.in = by_id(d_qids, exclude_self), .nq = nq,
+                         .k = knbn, .ef = exact ? 0 : ef_search, .exact = exact != 0, .out = on_device(d_out, d_counts)},
+                         .takes = ROWS, .need = QIDS, .early = true, .filter = filter, .sync = sync,
+                         .kernel_ms = kernel_ms});
 }
 
-// Excluded points per query: host queries under one_restriction's restriction, row i without the points of qx[qx_off[i],
+// Excluded points per query: host queries under a ROWS restriction, row i without the points of qx[qx_off[i],
 // qx_off[i + 1]) (insertion ranks; their check against nb_point runs under the handle's lock, Index::exclusion_lists)
-static int excluding_call(const void* h, const char* name, HostBatch b, const uint64_t* qx_off, const uint64_t* qx,
-                          int64_t filter, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset) {
-  OneLabelSets one;
-  if (int s = first_checks(h, name, b.nq, false, nullptr, nullptr, nullptr)) return s < 0 ? -1 : 0;
-  if (!qx_off) return set_err(std::string(name) + ": qx_off is NULL");
-  if (!qx) return set_err(std::string(name) + ": qx is NULL");
-  if (one_restriction(name, b.nq, filter, qrange, qset_off, qset, one, b.restriction)) return -1;
-  b.excluded = {qx_off, qx};
-  return (int)search_call(h, HOST, name, b, 1, nullptr);
-}
 int hnsw_b200_search_flat_excluding(const void* h, const uint64_t* qx_off, const uint64_t* qx, int64_t filter,
                                     const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
                                     const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search,
                                     uint64_t* out_ids, float* out_dist, uint32_t* out_internal, int32_t* out_pid,
                                     int32_t* out_counts) {
-  return excluding_call(h, "search_flat_excluding", {{queries}, nq, (int)dim, knbn, ef_search, Restriction(), false,
-                        columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, qx_off, qx, filter, qrange,
-                        qset_off, qset);
+  return (int)search(h, {.name = "search_flat_excluding", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .ef = ef_search, .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts),
+                         .excluded = {qx_off, qx}}, .takes = ROWS, .need = QX, .early = true, .filter = filter,
+                         .qrange = qrange, .qset_off = qset_off, .qset = qset});
 }
 int hnsw_b200_search_exact_excluding(const void* h, const uint64_t* qx_off, const uint64_t* qx, int64_t filter,
                                      const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
                                      const void* queries, uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t* out_ids,
                                      float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts) {
-  return excluding_call(h, "search_exact_excluding", {{queries}, nq, (int)dim, knbn, 0, Restriction(), true,
-                        columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, qx_off, qx, filter, qrange,
-                        qset_off, qset);
+  return (int)search(h, {.name = "search_exact_excluding", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .exact = true, .out = columns(out_ids, out_dist, out_internal, out_pid, out_counts),
+                         .excluded = {qx_off, qx}}, .takes = ROWS, .need = QX, .early = true, .filter = filter,
+                         .qrange = qrange, .qset_off = qset_off, .qset = qset});
 }
 
 // Planned search: count_admitted reads its restriction as the by-id calls do; the planned calls run each row on the graph
-// or by the exact scan per leg (Index::split_legs), under one_restriction's restriction and, with qx_off and qx, each
-// row's excluded points; out_exact (may be NULL) is written once the batch succeeded
+// or by the exact scan per leg (Index::split_legs), under a ROWS restriction and, with qx_off and qx, each row's
+// excluded points; out_exact (may be NULL) is written once the batch succeeded
 int hnsw_b200_count_admitted(const void* h, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
                              const uint32_t* qset, uint64_t nq, uint64_t* out_count) {
-  OneLabelSets one;
-  Restriction rs;
-  if (int s = first_checks(h, "count_admitted", nq, false, nullptr, nullptr, nullptr)) return s < 0 ? -1 : 0;
-  if (one_restriction("count_admitted", nq, filter, qrange, qset_off, qset, one, rs)) return -1;
-  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset_off) return set_err("qset_off is NULL");
-  if (rs.kind == Restriction::ROW_LABEL_SETS && !rs.qset) return set_err("qset is NULL");
+  Request q{.name = "count_admitted", .b = {.nq = nq}, .takes = ROWS, .early = true, .filter = filter, .qrange = qrange,
+            .qset_off = qset_off, .qset = qset};
+  if (const int s = prepare(h, q)) return s < 0 ? -1 : 0;
+  if (missing_rows(q.b.restriction)) return -1;
   if (!out_count) return set_err("count_admitted: out_count is NULL");
   Locked ix(h, SHARED);
   if (!ix) return -1;
-  return pass(ix, ix->count_admitted(rs, nq, out_count));
-}
-
-static int planned_call(const void* h, const char* name, bool by_id, HostBatch b, const uint64_t* qx_off, const uint64_t* qx,
-                        int64_t filter, const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset,
-                        int32_t* out_exact) {
-  OneLabelSets one;
-  if (int s = first_checks(h, name, b.nq, by_id, b.in.qids, nullptr, nullptr)) return s < 0 ? -1 : 0;
-  if (qx && !qx_off) return set_err(std::string(name) + ": qx_off is NULL");
-  if (qx_off && !qx) return set_err(std::string(name) + ": qx is NULL");
-  if (one_restriction(name, b.nq, filter, qrange, qset_off, qset, one, b.restriction)) return -1;
-  b.excluded = {qx_off, qx};
-  b.planned = true;
-  b.out.exact = out_exact;
-  return (int)search_call(h, HOST, name, b, 1, nullptr);
+  return pass(ix, ix->count_admitted(q.b.restriction, nq, out_count));
 }
 int hnsw_b200_search_planned(const void* h, const uint64_t* qx_off, const uint64_t* qx, int64_t filter,
                              const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset, const void* queries,
                              uint64_t nq, uint64_t dim, uint64_t knbn, uint64_t ef_search, uint64_t* out_ids,
                              float* out_dist, uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts,
                              int32_t* out_exact) {
-  return planned_call(h, "search_planned", false, {{queries}, nq, (int)dim, knbn, ef_search, Restriction(), false,
-                      columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, qx_off, qx, filter, qrange, qset_off,
-                      qset, out_exact);
+  return (int)search(h, {.name = "search_planned", .b = {.in = {queries}, .nq = nq, .d = (int)dim, .k = knbn,
+                         .ef = ef_search, .out = {.ids = out_ids, .dist = out_dist, .internal = out_internal,
+                         .pid = out_pid, .counts = out_counts, .exact = out_exact}, .excluded = {qx_off, qx},
+                         .planned = true}, .takes = ROWS, .early = true, .filter = filter, .qrange = qrange,
+                         .qset_off = qset_off, .qset = qset});
 }
 int hnsw_b200_search_planned_by_id(const void* h, const uint64_t* qids, uint64_t nq, uint64_t knbn, uint64_t ef_search,
                                    int exclude_self, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
                                    const uint32_t* qset, uint64_t* out_ids, float* out_dist, uint32_t* out_internal,
                                    int32_t* out_pid, int32_t* out_counts, int32_t* out_exact) {
-  return planned_call(h, "search_planned_by_id", true, {{nullptr, nullptr, qids, exclude_self ? qids : nullptr}, nq, 0, knbn,
-                      ef_search, Restriction(), false, columns(out_ids, out_dist, out_internal, out_pid, out_counts)},
-                      nullptr, nullptr, filter, qrange, qset_off, qset, out_exact);
+  return (int)search(h, {.name = "search_planned_by_id", .b = {.in = by_id(qids, exclude_self), .nq = nq, .k = knbn,
+                         .ef = ef_search, .out = {.ids = out_ids, .dist = out_dist, .internal = out_internal,
+                         .pid = out_pid, .counts = out_counts, .exact = out_exact}, .planned = true}, .takes = ROWS,
+                         .need = QIDS, .early = true, .filter = filter, .qrange = qrange, .qset_off = qset_off,
+                         .qset = qset});
 }
 
-// Radius search: the exact scan of host queries or of stored points (by_id), under one_restriction's restriction, each
-// row cut at its radius and its total of points within it into out_total (may be NULL).  knbn == 0 counts only: the
-// scan runs at k = 1 into scratch rows, the caller's row arrays may be NULL, and every count is 0.
-static int radius_call(const void* h, const char* name, bool by_id, HostBatch b, const float* radius, int64_t filter,
-                       const int64_t* qrange, const uint64_t* qset_off, const uint32_t* qset, uint64_t* out_total) {
-  std::vector<float> r;
-  OneLabelSets one;
-  if (int s = first_checks(h, name, b.nq, by_id, b.in.qids, radius, &r)) return s < 0 ? -1 : 0;
-  if (one_restriction(name, b.nq, filter, qrange, qset_off, qset, one, b.restriction)) return -1;
-  b.in.radius = r.data();
-  const size_t knbn = b.k;
-  std::vector<uint64_t> scratch_ids;
-  std::vector<float> scratch_dist;
-  if (knbn == 0) {
-    scratch_ids.resize(b.nq);
-    scratch_dist.resize(b.nq);
-    b.k = 1;
-    b.out.ids = scratch_ids.data();
-    b.out.dist = scratch_dist.data();
-    b.out.internal = nullptr;
-    b.out.pid = nullptr;
-  }
-  b.out.total = out_total;
-  const int rc = (int)search_call(h, HOST, name, b, 1, nullptr);
-  if (rc == 0 && knbn == 0) std::fill(b.out.counts, b.out.counts + b.nq, 0);
-  return rc;
-}
+// Radius search: the exact scan of host queries or of stored points, under a ROWS restriction, each row cut at its
+// radius and its total of points within it into out_total (may be NULL); knbn == 0 counts only (search)
 int hnsw_b200_search_exact_radius(const void* h, int64_t filter, const int64_t* qrange, const uint64_t* qset_off,
                                   const uint32_t* qset, const void* queries, uint64_t nq, uint64_t dim,
                                   const float* radius, uint64_t knbn, uint64_t* out_ids, float* out_dist,
                                   uint32_t* out_internal, int32_t* out_pid, int32_t* out_counts, uint64_t* out_total) {
-  return radius_call(h, "search_exact_radius", false, {{queries}, nq, (int)dim, knbn, 0, Restriction(), true,
-                     columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, radius, filter, qrange, qset_off,
-                     qset, out_total);
+  return (int)search(h, {.name = "search_exact_radius", .b = {.in = {.queries = queries, .radius = radius}, .nq = nq,
+                         .d = (int)dim, .k = knbn, .exact = true, .out = {.ids = out_ids, .dist = out_dist,
+                         .internal = out_internal, .pid = out_pid, .counts = out_counts, .total = out_total}},
+                         .takes = ROWS, .need = RADIUS, .early = true, .filter = filter, .qrange = qrange,
+                         .qset_off = qset_off, .qset = qset});
 }
 int hnsw_b200_search_exact_radius_by_id(const void* h, const uint64_t* qids, uint64_t nq, const float* radius,
                                         uint64_t knbn, int exclude_self, int64_t filter, const int64_t* qrange,
                                         const uint64_t* qset_off, const uint32_t* qset, uint64_t* out_ids,
                                         float* out_dist, uint32_t* out_internal, int32_t* out_pid,
                                         int32_t* out_counts, uint64_t* out_total) {
-  return radius_call(h, "search_exact_radius_by_id", true, {{nullptr, nullptr, qids, exclude_self ? qids : nullptr}, nq, 0,
-                     knbn, 0, Restriction(), true, columns(out_ids, out_dist, out_internal, out_pid, out_counts)}, radius,
-                     filter, qrange, qset_off, qset, out_total);
+  return (int)search(h, {.name = "search_exact_radius_by_id", .b = {.in = {.qids = qids, .skip = exclude_self ? qids :
+                         nullptr, .radius = radius}, .nq = nq, .k = knbn, .exact = true, .out = {.ids = out_ids,
+                         .dist = out_dist, .internal = out_internal, .pid = out_pid, .counts = out_counts,
+                         .total = out_total}}, .takes = ROWS, .need = QIDS | RADIUS, .early = true, .filter = filter,
+                         .qrange = qrange, .qset_off = qset_off, .qset = qset});
 }
 
 int hnsw_b200_get_vectors(const void* h, const uint64_t* ranks, uint64_t n, void* out) {
@@ -1152,11 +1159,7 @@ int hnsw_b200_get_vectors(const void* h, const uint64_t* ranks, uint64_t n, void
   if (n == 0) return 0;
   if (!ranks) return set_err("get_vectors: ranks is NULL");
   if (!out) return set_err("get_vectors: out is NULL");
-  const uint64_t have = ix->nb_point();
-  for (uint64_t i = 0; i < n; ++i)
-    if (ranks[i] >= have)
-      return set_err("get_vectors: ranks[" + std::to_string(i) + "] = " + std::to_string(ranks[i]) +
-                     " is not below nb_point = " + std::to_string(have));
+  if (not_below("get_vectors: ranks", ranks, n, ix->nb_point())) return -1;
   hb::DeviceRestore keep;
   return pass(ix, ix->get_vectors(ranks, n, out));
 }

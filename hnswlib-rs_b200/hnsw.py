@@ -196,7 +196,8 @@ def last_kernel_shape():
 
 
 def _p(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
+    """an array as a C pointer; None (NULL) and scalars as they are"""
+    return a.ctypes.data_as(C.c_void_p) if isinstance(a, np.ndarray) else a
 
 
 class HnswError(RuntimeError):
@@ -257,12 +258,14 @@ class ResidentFilter:
         self.free()
 
 
-def _filter_id(filter):
-    """the filter argument of the exact searches: a ResidentFilter's id, or -1 (every point) for None"""
+def _filter_id(filter, method=None):
+    """a filter argument that may only be a ResidentFilter: its id, or -1 (every point) for None.  Anything else is
+    refused, naming the method (None: the exact searches and the calls that take sets and ranges)."""
     if filter is None:
         return -1
     if not isinstance(filter, ResidentFilter):
-        raise TypeError("the exact searches take a ResidentFilter (Hnsw.make_filter) or None as their filter")
+        raise TypeError(f"{method} takes a ResidentFilter (Hnsw.make_filter) as its filter" if method else
+                        "the exact searches take a ResidentFilter (Hnsw.make_filter) or None as their filter")
     return filter.id
 
 
@@ -287,44 +290,37 @@ def _labels(labels, n, what):
     return np.ascontiguousarray(a, np.uint32)
 
 
-def _label_sets(sets, nq):
-    """the sets argument of the label-set searches, as (offsets u64[nq + 1], values u32[>= 1]): a sequence of nq
-    iterables of labels, or a tuple (offsets, values) as the C calls take it (query i: values[offsets[i]:offsets[i + 1]])"""
-    if isinstance(sets, tuple):
-        off, vals = sets
+def _csr(lists, nq, what):
+    """(offsets, values) of a list per query: a sequence of nq iterables, or a tuple (offsets, values) as the C calls
+    take it (query i: values[offsets[i]:offsets[i + 1]]), whose offsets must be nq + 1"""
+    if isinstance(lists, tuple):
+        off, vals = lists
         off, vals = np.asarray(off).reshape(-1), np.asarray(vals).reshape(-1)
         if off.shape != (nq + 1,):
-            raise ValueError(f"sets: {off.size} offsets for {nq} queries, expected {nq + 1}")
-        if off.size and (off.dtype.kind not in "iu" or off.min() < 0 or off.max() > vals.size):
-            raise ValueError(f"sets: offsets must be integers in [0, {vals.size}], the number of values")
-        off = np.ascontiguousarray(off, np.uint64)
-    else:
-        if len(sets) != nq:
-            raise ValueError(f"sets has {len(sets)} entries for {nq} queries")
-        parts = [np.asarray(x if isinstance(x, np.ndarray) else list(x), np.int64).reshape(-1) for x in sets]
-        off = np.zeros(nq + 1, np.uint64)
-        off[1:] = np.cumsum([x.size for x in parts])
-        vals = np.concatenate(parts) if parts else np.zeros(0, np.int64)
+            raise ValueError(f"{what}: {off.size} offsets for {nq} queries, expected {nq + 1}")
+        return off, vals
+    if len(lists) != nq:
+        raise ValueError(f"{what} has {len(lists)} entries for {nq} queries")
+    parts = [np.asarray(x if isinstance(x, np.ndarray) else list(x), np.int64).reshape(-1) for x in lists]
+    off = np.zeros(nq + 1, np.uint64)
+    off[1:] = np.cumsum([x.size for x in parts])
+    return off, np.concatenate(parts) if parts else np.zeros(0, np.int64)
+
+
+def _label_sets(sets, nq):
+    """the sets argument of the label-set searches (_csr's lists of labels), as (offsets u64[nq + 1], values
+    u32[>= 1])"""
+    off, vals = _csr(sets, nq, "sets")
+    if off.size and (off.dtype.kind not in "iu" or off.min() < 0 or off.max() > vals.size):
+        raise ValueError(f"sets: offsets must be integers in [0, {vals.size}], the number of values")
     vals = _labels(vals, vals.size, "sets")
-    return off, vals if vals.size else np.zeros(1, np.uint32)   # never a NULL pointer
+    return np.ascontiguousarray(off, np.uint64), vals if vals.size else np.zeros(1, np.uint32)   # never a NULL pointer
 
 
 def _excluded(excluded, nq):
-    """the excluded argument of the excluding searches, as (offsets u64[nq + 1], ranks u64[>= 1]): a sequence of nq
-    iterables of insertion ranks, or a tuple (offsets, ranks) as the C calls take it (query i: ranks[offsets[i]:
-    offsets[i + 1]])"""
-    if isinstance(excluded, tuple):
-        off, ids = excluded
-        off, ids = np.asarray(off).reshape(-1), np.asarray(ids).reshape(-1)
-        if off.shape != (nq + 1,):
-            raise ValueError(f"excluded: {off.size} offsets for {nq} queries, expected {nq + 1}")
-    else:
-        if len(excluded) != nq:
-            raise ValueError(f"excluded has {len(excluded)} entries for {nq} queries")
-        parts = [np.asarray(x if isinstance(x, np.ndarray) else list(x), np.int64).reshape(-1) for x in excluded]
-        off = np.zeros(nq + 1, np.uint64)
-        off[1:] = np.cumsum([x.size for x in parts])
-        ids = np.concatenate(parts) if parts else np.zeros(0, np.int64)
+    """the excluded argument of the excluding searches (_csr's lists of insertion ranks), as (offsets u64[nq + 1],
+    ranks u64[>= 1])"""
+    off, ids = _csr(excluded, nq, "excluded")
     for what, a in (("offsets", off), ("ranks", ids)):
         if a.size and (a.dtype.kind not in "iu" or a.min() < 0):
             raise ValueError(f"excluded: {what} must be non-negative integers")
@@ -366,6 +362,14 @@ def _ranges(ranges, nq):
         raise ValueError(f"ranges has shape {a.shape}, expected ({nq}, 2)")
     a = _int64s(a, "ranges: bounds are").reshape(-1)
     return a if a.size else np.zeros(2, np.int64)   # never a NULL pointer
+
+
+def _restriction(nq, filter, sets, ranges, ranged=False):
+    """the (filter, qrange, qset_off, qset) arguments of a call that takes a resident filter or sets and ranges (None:
+    NULL, filter -1); ranged: the ranges are required"""
+    rg = _ranges(ranges, nq) if ranged or ranges is not None else None
+    off, vals = (None, None) if sets is None else _label_sets(sets, nq)
+    return _filter_id(filter), rg, off, vals
 
 
 class Hnsw:
@@ -532,56 +536,54 @@ class Hnsw:
                 np.empty((nq, knbn), np.uint32) if with_internal else None,
                 np.empty((nq, knbn, 2), np.int32) if with_pid else None, np.empty(nq, np.int32))
 
-    def _host_search(self, fn, lead, q, knbn, mid, with_internal, with_pid):
-        """fn(handle, *lead, q, nq, d, knbn, *mid, *answer arrays) into fresh answer arrays, which it returns"""
-        ans = self._answers(q.shape[0], knbn, with_internal, with_pid)
-        self._chk(fn(self._h, *lead, _p(q), *q.shape, int(knbn), *mid, *map(_p, ans)))
-        return ans
+    def _host_search(self, fn, args, nq, knbn, with_internal, with_pid, *extra):
+        """fn(handle, *args, *answer arrays, *extra outputs) into fresh answer arrays (_answers) and an array of nq of
+        each dtype in extra, which it returns; arrays in args are passed as pointers"""
+        out = self._answers(nq, knbn, with_internal, with_pid) + tuple(np.empty(nq, t) for t in extra)
+        self._chk(fn(self._h, *map(_p, args), *map(_p, out)))
+        return out
 
-    def _filter_call(self, filter, name, resident_only=None):
-        """the C call of a filter= argument: (function, arguments ahead of the queries, FilterT arguments after ef).
-        hnsw_b200_<name> for None, hnsw_b200_<name>_filtered with the id of a ResidentFilter.  hnsw_b200_search_flat takes
-        a FilterT (a sorted id sequence or a callable) after ef, mode 0 for None; a method that takes only a
-        ResidentFilter (resident_only: its name) refuses anything else."""
-        if isinstance(filter, ResidentFilter):
-            return getattr(self._L, f"hnsw_b200_{name}_filtered"), (filter.id,), ()
-        if resident_only:
-            if filter is not None:
-                raise TypeError(f"{resident_only} takes a ResidentFilter (Hnsw.make_filter) as its filter")
-            return getattr(self._L, "hnsw_b200_" + name), (), ()
-        mode, fids, nf, cb = (0, None, 0, FILTER_FN(0)) if filter is None else _filter_args(filter)
-        return getattr(self._L, "hnsw_b200_" + name), (), (mode, _p(fids), nf, cb, None)
+    def _resident(self, name, filter, method):
+        """the C call of a filter= argument that may only be a ResidentFilter (_filter_id): hnsw_b200_<name> and no
+        argument for None, hnsw_b200_<name>_filtered and the filter's id (its argument ahead of the queries)"""
+        fid = _filter_id(filter, method)
+        return (getattr(self._L, f"hnsw_b200_{name}_filtered"), (fid,)) if filter is not None else \
+            (getattr(self._L, f"hnsw_b200_{name}"), ())
 
     def search_flat(self, queries, knbn, ef, filter=None, with_internal=True, with_pid=True):
         """Extension: flat batch.  Returns (origin u64[nq,k], dist f32[nq,k], internal u32[nq,k] | None,
         pid i32[nq,k,2] | None, counts).  filter: as search_filter takes it."""
         q = np.ascontiguousarray(queries, self.dtype)
-        fn, lead, tail = self._filter_call(filter, "search_flat")
-        return self._host_search(fn, lead, q, knbn, (int(ef),) + tail, with_internal, with_pid)
+        if isinstance(filter, ResidentFilter):   # hnsw_b200_search_flat_filtered
+            fn, lead, tail = self._L.hnsw_b200_search_flat_filtered, (filter.id,), ()
+        else:   # a FilterT after ef, mode 0 for None
+            fn, lead = self._L.hnsw_b200_search_flat, ()
+            tail = (0, None, 0, FILTER_FN(0), None) if filter is None else (*_filter_args(filter), None)
+        return self._host_search(fn, (*lead, q, *q.shape, int(knbn), int(ef), *tail), len(q), knbn, with_internal,
+                                 with_pid)
 
     def search_exact(self, queries, knbn, filter=None, with_internal=True, with_pid=True):
         """hnsw_b200_search_exact: the exact knbn nearest among the points a ResidentFilter admits (None: every point).
         Returns search_flat's (origin, dist, internal | None, pid | None, counts)."""
         q = np.ascontiguousarray(queries, self.dtype)
-        return self._host_search(self._L.hnsw_b200_search_exact, (_filter_id(filter),), q, knbn, (), with_internal,
-                                 with_pid)
+        return self._host_search(self._L.hnsw_b200_search_exact, (_filter_id(filter), q, *q.shape, int(knbn)), len(q),
+                                 knbn, with_internal, with_pid)
 
     def search_flat_per_query(self, queries, knbn, ef, filters, with_internal=True, with_pid=True):
         """hnsw_b200_search_flat_per_query: one batch, query i filtered by filters[i] (a ResidentFilter of this handle,
         or None for no filter).  Row i equals search_flat(queries[i:i+1], knbn, ef, filter=filters[i]).  Returns
         search_flat's (origin, dist, internal | None, pid | None, counts)."""
         q = np.ascontiguousarray(queries, self.dtype)
-        fids = _filter_ids(filters, q.shape[0])
-        return self._host_search(self._L.hnsw_b200_search_flat_per_query, (_p(fids),), q, knbn, (int(ef),), with_internal,
-                                 with_pid)
+        return self._host_search(self._L.hnsw_b200_search_flat_per_query,
+                                 (_filter_ids(filters, len(q)), q, *q.shape, int(knbn), int(ef)), len(q), knbn,
+                                 with_internal, with_pid)
 
     def search_exact_per_query(self, queries, knbn, filters, with_internal=True, with_pid=True):
         """hnsw_b200_search_exact_per_query: search_exact with query i over the points filters[i] admits (a
         ResidentFilter of this handle, or None for every point), in one batch.  Returns search_exact's tuple."""
         q = np.ascontiguousarray(queries, self.dtype)
-        fids = _filter_ids(filters, q.shape[0])
-        return self._host_search(self._L.hnsw_b200_search_exact_per_query, (_p(fids),), q, knbn, (), with_internal,
-                                 with_pid)
+        return self._host_search(self._L.hnsw_b200_search_exact_per_query, (_filter_ids(filters, len(q)), q, *q.shape,
+                                 int(knbn)), len(q), knbn, with_internal, with_pid)
 
     def set_labels(self, first, labels):
         """hnsw_b200_set_labels: the labels of the points with insertion ranks first .. first + len(labels) - 1
@@ -629,16 +631,15 @@ class Hnsw:
         every point).  Row i equals search_flat with a resident filter admitting exactly those points.  Returns
         search_flat's (origin, dist, internal | None, pid | None, counts)."""
         q = np.ascontiguousarray(queries, self.dtype)
-        lab = _labels(labels, q.shape[0], "labels")
-        return self._host_search(self._L.hnsw_b200_search_flat_labeled, (_p(lab),), q, knbn, (int(ef),), with_internal,
-                                 with_pid)
+        return self._host_search(self._L.hnsw_b200_search_flat_labeled, (_labels(labels, len(q), "labels"), q, *q.shape,
+                                 int(knbn), int(ef)), len(q), knbn, with_internal, with_pid)
 
     def search_exact_labeled(self, queries, knbn, labels, with_internal=True, with_pid=True):
         """hnsw_b200_search_exact_labeled: the exact knbn nearest of query i among the points labelled labels[i]
         (LABEL_NONE: every point), in one batch.  Returns search_exact's tuple."""
         q = np.ascontiguousarray(queries, self.dtype)
-        lab = _labels(labels, q.shape[0], "labels")
-        return self._host_search(self._L.hnsw_b200_search_exact_labeled, (_p(lab),), q, knbn, (), with_internal, with_pid)
+        return self._host_search(self._L.hnsw_b200_search_exact_labeled, (_labels(labels, len(q), "labels"), q,
+                                 *q.shape, int(knbn)), len(q), knbn, with_internal, with_pid)
 
     def search_flat_label_sets(self, queries, knbn, ef, sets, with_internal=True, with_pid=True):
         """hnsw_b200_search_flat_label_sets: one batch, query i restricted to the points whose label is in sets[i] (any
@@ -646,17 +647,15 @@ class Hnsw:
         a tuple (offsets, values).  Row i equals search_flat with a resident filter admitting exactly those points.
         Returns search_flat's (origin, dist, internal | None, pid | None, counts)."""
         q = np.ascontiguousarray(queries, self.dtype)
-        off, vals = _label_sets(sets, q.shape[0])
-        return self._host_search(self._L.hnsw_b200_search_flat_label_sets, (_p(off), _p(vals)), q, knbn, (int(ef),),
-                                 with_internal, with_pid)
+        return self._host_search(self._L.hnsw_b200_search_flat_label_sets, (*_label_sets(sets, len(q)), q, *q.shape,
+                                 int(knbn), int(ef)), len(q), knbn, with_internal, with_pid)
 
     def search_exact_label_sets(self, queries, knbn, sets, with_internal=True, with_pid=True):
         """hnsw_b200_search_exact_label_sets: the exact knbn nearest of query i among the points whose label is in
         sets[i] (as search_flat_label_sets takes it), in one batch.  Returns search_exact's tuple."""
         q = np.ascontiguousarray(queries, self.dtype)
-        off, vals = _label_sets(sets, q.shape[0])
-        return self._host_search(self._L.hnsw_b200_search_exact_label_sets, (_p(off), _p(vals)), q, knbn, (),
-                                 with_internal, with_pid)
+        return self._host_search(self._L.hnsw_b200_search_exact_label_sets, (*_label_sets(sets, len(q)), q, *q.shape,
+                                 int(knbn)), len(q), knbn, with_internal, with_pid)
 
     def set_attributes(self, first, values):
         """hnsw_b200_set_attributes: the int64 attributes of the points with insertion ranks first .. first +
@@ -670,37 +669,26 @@ class Hnsw:
         self._chk(self._L.hnsw_b200_get_attributes(self._h, int(first), int(n), _p(out)))
         return out
 
-    def _ranged(self, fn, queries, knbn, mid, ranges, sets, with_internal, with_pid):
-        q = np.ascontiguousarray(queries, self.dtype)
-        rg = _ranges(ranges, q.shape[0])
-        off, vals = (None, None) if sets is None else _label_sets(sets, q.shape[0])
-        return self._host_search(fn, (_p(rg), _p(off), _p(vals)), q, knbn, mid, with_internal, with_pid)
-
     def search_flat_ranges(self, queries, knbn, ef, ranges, sets=None, with_internal=True, with_pid=True):
         """hnsw_b200_search_flat_ranges: one batch, query i restricted to the points whose attribute lies in
         ranges[i] = (lo, hi), inclusive (RANGE_ALL: every point, also those without one; lo > hi: none), and, with sets
         (as search_flat_label_sets takes it), whose label is in sets[i].  Row i equals search_flat with a resident
         filter admitting exactly those points.  Returns search_flat's (origin, dist, internal | None, pid | None,
         counts)."""
-        return self._ranged(self._L.hnsw_b200_search_flat_ranges, queries, knbn, (int(ef),), ranges, sets, with_internal,
-                            with_pid)
+        q = np.ascontiguousarray(queries, self.dtype)
+        rows = _restriction(len(q), None, sets, ranges, ranged=True)[1:]
+        return self._host_search(self._L.hnsw_b200_search_flat_ranges, (*rows, q, *q.shape, int(knbn), int(ef)), len(q),
+                                 knbn, with_internal, with_pid)
 
     def search_exact_ranges(self, queries, knbn, ranges, sets=None, with_internal=True, with_pid=True):
         """hnsw_b200_search_exact_ranges: the exact knbn nearest of query i among the points search_flat_ranges
         admits for it, in one batch.  Returns search_exact's tuple."""
-        return self._ranged(self._L.hnsw_b200_search_exact_ranges, queries, knbn, (), ranges, sets, with_internal,
-                            with_pid)
-
-    # ---- excluded points per query (include/hnsw_b200.h "Excluded points per query")
-    def _excluding(self, fn, queries, knbn, mid, excluded, filter, sets, ranges, with_internal, with_pid):
         q = np.ascontiguousarray(queries, self.dtype)
-        nq = q.shape[0]
-        off, ids = _excluded(excluded, nq)
-        rg = None if ranges is None else _ranges(ranges, nq)
-        sets_off, vals = (None, None) if sets is None else _label_sets(sets, nq)
-        return self._host_search(fn, (_p(off), _p(ids), _filter_id(filter), _p(rg), _p(sets_off), _p(vals)), q, knbn, mid,
+        rows = _restriction(len(q), None, sets, ranges, ranged=True)[1:]
+        return self._host_search(self._L.hnsw_b200_search_exact_ranges, (*rows, q, *q.shape, int(knbn)), len(q), knbn,
                                  with_internal, with_pid)
 
+    # ---- excluded points per query (include/hnsw_b200.h "Excluded points per query")
     def search_flat_excluding(self, queries, knbn, ef, excluded, filter=None, sets=None, ranges=None, with_internal=True,
                               with_pid=True):
         """hnsw_b200_search_flat_excluding: query i without the points excluded[i] (insertion ranks, any order,
@@ -709,23 +697,18 @@ class Hnsw:
         tuple (offsets, ranks).  Row i equals search_flat with a resident filter admitting exactly the points its
         restriction admits minus excluded[i].  Returns search_flat's (origin, dist, internal | None, pid | None,
         counts)."""
-        return self._excluding(self._L.hnsw_b200_search_flat_excluding, queries, knbn, (int(ef),), excluded, filter, sets,
-                               ranges, with_internal, with_pid)
+        q = np.ascontiguousarray(queries, self.dtype)
+        args = (*_excluded(excluded, len(q)), *_restriction(len(q), filter, sets, ranges), q, *q.shape, int(knbn), int(ef))
+        return self._host_search(self._L.hnsw_b200_search_flat_excluding, args, len(q), knbn, with_internal, with_pid)
 
     def search_exact_excluding(self, queries, knbn, excluded, filter=None, sets=None, ranges=None, with_internal=True,
                                with_pid=True):
         """hnsw_b200_search_exact_excluding: search_flat_excluding with the exact search in place of the graph one"""
-        return self._excluding(self._L.hnsw_b200_search_exact_excluding, queries, knbn, (), excluded, filter, sets, ranges,
-                               with_internal, with_pid)
+        q = np.ascontiguousarray(queries, self.dtype)
+        args = (*_excluded(excluded, len(q)), *_restriction(len(q), filter, sets, ranges), q, *q.shape, int(knbn))
+        return self._host_search(self._L.hnsw_b200_search_exact_excluding, args, len(q), knbn, with_internal, with_pid)
 
     # ---- planned search (include/hnsw_b200.h "Planned search")
-    def _restriction(self, nq, filter, sets, ranges):
-        """the filter id and the (qrange, qset_off, qset) arrays (None: NULL) of a call that reads its restriction as
-        search_by_id does"""
-        rg = None if ranges is None else _ranges(ranges, nq)
-        off, vals = (None, None) if sets is None else _label_sets(sets, nq)
-        return _filter_id(filter), (rg, off, vals)
-
     def count_admitted(self, filter=None, sets=None, ranges=None, n=None):
         """hnsw_b200_count_admitted: for each of n rows (default: as many as sets or ranges has), the number of points
         its restriction admits, deleted points included, as a uint64 array.  The restriction is search_by_id's."""
@@ -733,8 +716,8 @@ class Hnsw:
             n = len(sets[0]) - 1 if isinstance(sets, tuple) else len(sets) if sets is not None else \
                 len(ranges) if ranges is not None else 1
         out = np.zeros(int(n), np.uint64)
-        fid, rows = self._restriction(int(n), filter, sets, ranges)
-        self._chk(self._L.hnsw_b200_count_admitted(self._h, fid, *map(_p, rows), int(n), _p(out)))
+        rows = _restriction(int(n), filter, sets, ranges)
+        self._chk(self._L.hnsw_b200_count_admitted(self._h, *map(_p, rows), int(n), _p(out)))
         return out
 
     def search_planned(self, queries, knbn, ef, excluded=None, filter=None, sets=None, ranges=None, with_internal=True,
@@ -744,27 +727,18 @@ class Hnsw:
         search_flat_excluding takes it, or None.  Returns search_flat's (origin, dist, internal | None, pid | None,
         counts) and exact i32[nq], the number of indexes (partitions) that scanned each row exactly."""
         q = np.ascontiguousarray(queries, self.dtype)
-        nq = q.shape[0]
-        off, ids = (None, None) if excluded is None else _excluded(excluded, nq)
-        ans = self._answers(nq, knbn, with_internal, with_pid)
-        exact = np.empty(nq, np.int32)
-        fid, rows = self._restriction(nq, filter, sets, ranges)
-        self._chk(self._L.hnsw_b200_search_planned(self._h, _p(off), _p(ids), fid, *map(_p, rows), _p(q), *q.shape,
-                                                   int(knbn), int(ef), *map(_p, ans), _p(exact)))
-        return ans + (exact,)
+        lists = (None, None) if excluded is None else _excluded(excluded, len(q))
+        args = (*lists, *_restriction(len(q), filter, sets, ranges), q, *q.shape, int(knbn), int(ef))
+        return self._host_search(self._L.hnsw_b200_search_planned, args, len(q), knbn, with_internal, with_pid, np.int32)
 
     def search_planned_by_id(self, qids, knbn, ef, filter=None, sets=None, ranges=None, exclude_self=False,
                              with_internal=True, with_pid=True):
         """hnsw_b200_search_planned_by_id: search_planned with query i the stored point qids[i], each row that of
         search_by_id or search_exact_by_id.  Returns search_planned's tuple."""
         q = np.ascontiguousarray(qids, np.uint64).reshape(-1)
-        nq = q.size
-        ans = self._answers(nq, knbn, with_internal, with_pid)
-        exact = np.empty(nq, np.int32)
-        fid, rows = self._restriction(nq, filter, sets, ranges)
-        self._chk(self._L.hnsw_b200_search_planned_by_id(self._h, _p(q), nq, int(knbn), int(ef), int(bool(exclude_self)),
-                                                         fid, *map(_p, rows), *map(_p, ans), _p(exact)))
-        return ans + (exact,)
+        args = (q, q.size, int(knbn), int(ef), int(bool(exclude_self)), *_restriction(q.size, filter, sets, ranges))
+        return self._host_search(self._L.hnsw_b200_search_planned_by_id, args, q.size, knbn, with_internal, with_pid,
+                                 np.int32)
 
     # ---- search by stored point (include/hnsw_b200.h "Search by stored point")
     def get_vectors(self, ranks):
@@ -785,30 +759,22 @@ class Hnsw:
         hit = np.flatnonzero((lv == level) & (rk == rank))
         return self.get_vectors(hit[:1])[0] if hit.size else None
 
-    def _by_id(self, fn, qids, knbn, mid, exclude_self, filter, sets, ranges, with_internal, with_pid):
-        q = np.ascontiguousarray(qids, np.uint64).reshape(-1)
-        nq = q.size
-        rg = None if ranges is None else _ranges(ranges, nq)
-        off, vals = (None, None) if sets is None else _label_sets(sets, nq)
-        ans = self._answers(nq, knbn, with_internal, with_pid)
-        self._chk(fn(self._h, _p(q), nq, int(knbn), *mid, int(bool(exclude_self)), _filter_id(filter), _p(rg), _p(off),
-                     _p(vals), *map(_p, ans)))
-        return ans
-
     def search_by_id(self, qids, knbn, ef, filter=None, sets=None, ranges=None, exclude_self=False, with_internal=True,
                      with_pid=True):
         """hnsw_b200_search_flat_by_id: query i is the stored point qids[i] (an insertion rank).  Row i equals
         search_flat (filter: a ResidentFilter), search_flat_label_sets (sets) or search_flat_ranges (ranges, optionally
         with sets) on get_vectors(qids[i]).  exclude_self: the row of knbn + 1 without the point itself (or without its
         last entry when it does not hold the point), cut to knbn.  Returns search_flat's tuple."""
-        return self._by_id(self._L.hnsw_b200_search_flat_by_id, qids, knbn, (int(ef),), exclude_self, filter, sets, ranges,
-                           with_internal, with_pid)
+        q = np.ascontiguousarray(qids, np.uint64).reshape(-1)
+        args = (q, q.size, int(knbn), int(ef), int(bool(exclude_self)), *_restriction(q.size, filter, sets, ranges))
+        return self._host_search(self._L.hnsw_b200_search_flat_by_id, args, q.size, knbn, with_internal, with_pid)
 
     def search_exact_by_id(self, qids, knbn, filter=None, sets=None, ranges=None, exclude_self=False, with_internal=True,
                            with_pid=True):
         """hnsw_b200_search_exact_by_id: search_by_id with the exact searches in place of the graph ones"""
-        return self._by_id(self._L.hnsw_b200_search_exact_by_id, qids, knbn, (), exclude_self, filter, sets, ranges,
-                           with_internal, with_pid)
+        q = np.ascontiguousarray(qids, np.uint64).reshape(-1)
+        args = (q, q.size, int(knbn), int(bool(exclude_self)), *_restriction(q.size, filter, sets, ranges))
+        return self._host_search(self._L.hnsw_b200_search_exact_by_id, args, q.size, knbn, with_internal, with_pid)
 
     def search_device_by_id(self, d_qids_ptr, nq, knbn, ef, d_out_ptr, d_counts_ptr, exclude_self=False, exact=False,
                             sync=True, filter=None):
@@ -838,17 +804,6 @@ class Hnsw:
         return ids, ds
 
     # ---- radius search (include/hnsw_b200.h "Radius search")
-    def _radius(self, fn, lead, nq, radius, knbn, filter, sets, ranges, with_internal, with_pid):
-        r = np.ascontiguousarray(np.broadcast_to(np.asarray(radius, np.float32), (nq,)))
-        rg = None if ranges is None else _ranges(ranges, nq)
-        off, vals = (None, None) if sets is None else _label_sets(sets, nq)
-        knbn = int(knbn)
-        ans = self._answers(nq, knbn, with_internal, with_pid)
-        totals = np.empty(nq, np.uint64)
-        restriction = (_filter_id(filter), _p(rg), _p(off), _p(vals))
-        self._chk(fn(self._h, *lead(restriction, _p(r)), *map(_p, ans), _p(totals)))
-        return ans + (totals,)
-
     def search_exact_radius(self, queries, radius, knbn, filter=None, sets=None, ranges=None, with_internal=True,
                             with_pid=True):
         """hnsw_b200_search_exact_radius: the points within radius of each query (a scalar or one value per query),
@@ -857,21 +812,21 @@ class Hnsw:
         only.  Returns search_exact's (origin, dist, internal | None, pid | None, counts) and totals u64[nq], the number
         of admitted points within each radius."""
         q = np.ascontiguousarray(queries, self.dtype)
-        nq, d = q.shape
-        return self._radius(self._L.hnsw_b200_search_exact_radius,
-                            lambda rs, r: rs + (_p(q), nq, d, r, int(knbn)),
-                            nq, radius, knbn, filter, sets, ranges, with_internal, with_pid)
+        r = np.ascontiguousarray(np.broadcast_to(np.asarray(radius, np.float32), (len(q),)))
+        args = (*_restriction(len(q), filter, sets, ranges), q, *q.shape, r, int(knbn))
+        return self._host_search(self._L.hnsw_b200_search_exact_radius, args, len(q), int(knbn), with_internal, with_pid,
+                                 np.uint64)
 
     def search_exact_radius_by_id(self, qids, radius, knbn, exclude_self=False, filter=None, sets=None, ranges=None,
                                   with_internal=True, with_pid=True):
         """hnsw_b200_search_exact_radius_by_id: search_exact_radius with query i the stored point qids[i] (an insertion
         rank).  exclude_self: search_exact_by_id's exclude_self row cut at the radius, and a total without the point
         itself.  Returns search_exact_radius's tuple."""
-        ids = np.ascontiguousarray(qids, np.uint64).reshape(-1)
-        nq = ids.size
-        return self._radius(self._L.hnsw_b200_search_exact_radius_by_id,
-                            lambda rs, r: (_p(ids), nq, r, int(knbn), int(bool(exclude_self))) + rs,
-                            nq, radius, knbn, filter, sets, ranges, with_internal, with_pid)
+        q = np.ascontiguousarray(qids, np.uint64).reshape(-1)
+        r = np.ascontiguousarray(np.broadcast_to(np.asarray(radius, np.float32), (q.size,)))
+        args = (q, q.size, r, int(knbn), int(bool(exclude_self)), *_restriction(q.size, filter, sets, ranges))
+        return self._host_search(self._L.hnsw_b200_search_exact_radius_by_id, args, q.size, int(knbn), with_internal,
+                                 with_pid, np.uint64)
 
     def radius_graph(self, radius, knbn=64, batch=65536):
         """every stored point's complete list of the other points within radius, by insertion rank, as CSR
@@ -920,7 +875,7 @@ class Hnsw:
         """hnsw_b200_search_flat_submit: enqueue a batch, return a ticket for wait_flat (up to 4 outstanding).
         filter: None or a ResidentFilter (hnsw_b200_search_flat_submit_filtered)."""
         q = np.ascontiguousarray(queries, self.dtype)
-        fn, lead, _ = self._filter_call(filter, "search_flat_submit", "submit_flat")
+        fn, lead = self._resident("search_flat_submit", filter, "submit_flat")
         ans = self._answers(q.shape[0], knbn, with_internal, with_pid)
         t = fn(self._h, *lead, _p(q), *q.shape, int(knbn), int(ef), *map(_p, ans))
         if t < 0:
@@ -1043,7 +998,7 @@ class Hnsw:
         Returns the kernel's CUDA-event time in ms when sync is true.  filter: None or a ResidentFilter
         (hnsw_b200_search_device_filtered)."""
         ms = C.c_float(0.0)
-        fn, lead, _ = self._filter_call(filter, "search_device", "search_device")
+        fn, lead = self._resident("search_device", filter, "search_device")
         self._chk(fn(self._h, *lead, C.c_void_p(d_queries_ptr), nq, int(knbn), int(ef), C.c_void_p(d_out_ptr),
                      C.c_void_p(d_counts_ptr), int(bool(sync)), C.byref(ms) if sync else None))
         return float(ms.value)
